@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- agent-steps/sec of the env-step + PPO-rollout hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -18,7 +18,10 @@ defaults (config.yaml:12-42) with its batch:minibatch ratio of 4.
            reference's evaluate loop).
 `--impl reference` / `cpu_baseline`: the oracle's CPU restatement of the same path (oracle/: C vectoriser + env with
            OpenMP over all host cores, Python sort_training_data, C GAE, numpy flatten, torch-CPU policy and PPO
-           update) on a bounded sample of the workload.  /root/reference itself cannot travel to the GPU box.
+           update) on a bounded sample of the workload.
+`--dump-outputs DIR`: after the timed steps, what the last timed step computed (rollout rows, advantages, the updated
+           policy parameters, the losses) as DIR/<name>.npy; with the same arguments the inputs are the same every run, so
+           two builds can be compared output for output.
 """
 import argparse
 import json
@@ -57,6 +60,8 @@ def parse_args():
     ap.add_argument('--epochs', type=int, default=4)
     ap.add_argument('--kernels-only', action='store_true', help='skip the PPO loop; report the per-kernel rooflines')
     ap.add_argument('--ref-horizon', type=int, default=8, help='bounded sample: env steps per reference-arm step')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the last timed step computed as DIR/<name>.npy (float32 / float64, < 64 MB in all)')
     return ap.parse_args()
 
 
@@ -74,7 +79,7 @@ def ppo_config(num_envs, horizon, device, seed=1, cuda_graph=True, minibatches=4
 # ------------------------------------------------------------------------------------------------ clocks
 class ClockSampler:
     """nvidia-smi clocks / throttle reasons sampled every 50 ms from the start of the timed region; when that region is shorter
-    than ~0.6 s (K steps of 3.6 ms) the same steps keep running, untimed, until at least that long has been sampled under load
+    than ~0.6 s the same steps keep running, untimed, until at least that long has been sampled under load
     (`window` in the JSON says so)."""
     Q = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
@@ -116,7 +121,19 @@ class ClockSampler:
                 'reasons': sorted(reasons), 'samples': len(sm)}
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+def gpu_info(index=0):
+    """Name and power limit of the card the numbers were measured on (part of every absolute number)."""
+    info = {'name': torch.cuda.get_device_name(index), 'power_limit_w': None, 'sm_count': torch.cuda.get_device_properties(index).multi_processor_count}
+    try:
+        out = subprocess.run(['nvidia-smi', f'--id={index}', '--query-gpu=power.limit', '--format=csv,noheader,nounits'],
+                             capture_output=True, text=True, timeout=20).stdout.strip()
+        info['power_limit_w'] = float(out.splitlines()[0])
+    except Exception:
+        pass
+    return info
+
+
+# ------------------------------------------------------------------------------------------------ device arm
 def make_b200(args, rank, world, host_buffers, cuda_graph):
     import pufferlib_b200.vector as pvec
     from pufferlib_b200 import clean_pufferl, models, distributed as pdist
@@ -213,7 +230,7 @@ def kernel_rooflines(data, args, peak_gbs, peak_src):
         finally:
             lib.pb_snake_set_variant(4)
 
-    # GAE (+returns): 20 B per agent-step.  8 rotating input/output sets (8 x 42 MB > the 126 MB L2) so every launch
+    # GAE (+returns): 20 B per agent-step.  8 rotating input/output sets (8 x 42 MB > the 50 MB L2) so every launch
     # streams from HBM like it does after a 1 GiB rollout has passed through the cache.
     exp.num_envs, exp.horizon = n, h
     exp.compute_gae(0.99, 0.95)                     # allocates the workspace, sets kernel attributes
@@ -294,7 +311,7 @@ def kernel_rooflines(data, args, peak_gbs, peak_src):
                 vec.fused_rollout(exp, pol)
         roll(0)
         t_roll = time_launches(roll, 4)
-        out['rollout'] = dict(kernel='k_breakout_rollout (tcgen05 policy + env, persistent)', seconds=t_roll,
+        out['rollout'] = dict(kernel='k_breakout_rollout (wgmma policy + env, persistent)', seconds=t_roll,
                               bytes_per_launch=n * h * (o + 4 + 4 + 4 + 4 + 8), launches_per_step=1)
         exp.ptr = 0
         for k_ in ('env_step', 'policy_step'):
@@ -338,7 +355,7 @@ def kernel_rooflines(data, args, peak_gbs, peak_src):
         out['ppo_loss'] = dict(kernel='k_ppo_loss', seconds=t_loss, bytes_per_launch=mb * (8 * n_act + 32 + 4),
                                launches_per_step=args.minibatches * args.epochs)
         del hid, douts, dpre, outs, gouts
-        # the fused tcgen05 minibatch update (forward + loss + backward in one kernel): algorithmic bytes = the observation
+        # the fused wgmma minibatch update (forward + loss + backward in one kernel): algorithmic bytes = the observation
         # rows (read once) + 24 B of per-row scalars; launched on zero-copy slab views of the rollout like train() does
         mu = getattr(data, 'manual_update', None)
         if mu is not None and getattr(mu, 'used_fused', False) and o == 512:
@@ -368,8 +385,8 @@ def kernel_rooflines(data, args, peak_gbs, peak_src):
                 with torch.no_grad():
                     upd(0)
                     t_upd = time_launches(upd, 8)
-                out['mlp_update'] = dict(kernel=('k_mlp_update_xt (tcgen05 forward / x^T / dW + mma.sync epilogue)' if dw_mode == 'kernel' else
-                                                 'k_mlp_update_fused (tcgen05, dPre to HBM, dW: cuBLAS)') + ' + k_update_reduce', seconds=t_upd,
+                out['mlp_update'] = dict(kernel=('k_mlp_update (wgmma forward / dW + mma.sync epilogue)' if dw_mode == 'kernel' else
+                                                 'k_mlp_update (wgmma, dPre to HBM, dW: cuBLAS)') + ' + k_update_reduce', seconds=t_upd,
                                          bytes_per_launch=mb * (512 + 28 + (512 if dpre_b is not None else 0)),
                                          launches_per_step=nm * args.epochs,
                                          tf32_tflops=round(2 * 2 * mb * 128 * 128 / t_upd / 1e12, 1))
@@ -379,14 +396,7 @@ def kernel_rooflines(data, args, peak_gbs, peak_src):
         v['share_s'] = v['seconds'] * v['launches_per_step']
     dom = max(out, key=lambda k: out[k]['share_s'])
     d = out[dom]
-    # DRAM traffic per launch from the committed `ncu --set full` capture of this workload (profiles/), else null
-    traffic = None
-    try:
-        tr = json.load(open(os.path.join(REPO, 'profiles', 'ncu_traffic_r02.json')))['bytes_per_launch']
-        if args.env == 'breakout' and n == 16384 and h == 128:
-            traffic = tr.get({'env_step': 'breakout', 'obs_gather': 'gather'}.get(dom, dom))
-    except Exception:
-        pass
+    traffic = None       # no profiler capture of this workload is stored with the project
     roof = {'bound': 'hbm', 'kernel': d['kernel'], 'achieved': round(d['achieved'], 1), 'peak': peak_gbs,
             'peak_source': peak_src, 'unit': 'GB/s', 'frac': round(d['frac'], 4), 'traffic': traffic,
             'algorithmic_bytes_per_launch': d['bytes_per_launch'], 'avg_launch_us': round(d['seconds'] * 1e6, 2)}
@@ -397,12 +407,45 @@ def kernel_rooflines(data, args, peak_gbs, peak_src):
     return roof, others
 
 
+DUMP_ROWS = 262144          # per-row rollout outputs: a fixed, seeded sample of rows (1 MB per array)
+DUMP_OBS_ROWS = 4096        # observation rows of the sample (whole rows)
+
+
+def dump_outputs(data, out_dir):
+    """What the last evaluate() + train() computed, as a caller of that path receives it: the rollout rows (actions, log
+    probabilities, values, rewards, dones, observations), the advantages, the updated policy parameters and the losses.
+    Per-row arrays larger than DUMP_ROWS are sampled at fixed seeded rows (the same rows every run)."""
+    os.makedirs(out_dir, exist_ok=True)
+    exp = data.experience
+    torch.cuda.synchronize()
+    n_rows = exp.actions.numel()
+    rows = np.arange(n_rows) if n_rows <= DUMP_ROWS else np.sort(np.random.default_rng(0).choice(n_rows, DUMP_ROWS, replace=False))
+    idx = torch.as_tensor(rows, device=exp.actions.device)
+    arrays = {'rows': rows.astype(np.float64)}
+    adv = exp.advantages_tm if getattr(exp, 'advantages_tm', None) is not None else exp.advantages
+    for name, t in (('actions', exp.actions), ('logprobs', exp.logprobs), ('values', exp.values), ('rewards', exp.rewards),
+                    ('dones', exp.dones), ('advantages', adv)):
+        arrays[name] = t.reshape(-1)[idx].double().cpu().numpy() if name == 'actions' else t.reshape(-1)[idx].float().cpu().numpy()
+    obs_rows = rows[np.linspace(0, len(rows) - 1, min(DUMP_OBS_ROWS, len(rows))).astype(np.int64)]
+    arrays['obs_rows'] = obs_rows.astype(np.float64)
+    arrays['obs'] = exp.obs.reshape(n_rows, -1)[torch.as_tensor(obs_rows, device=exp.obs.device)].float().cpu().numpy()
+    for name, prm in data.policy.named_parameters():
+        arrays['param.' + name] = prm.detach().float().cpu().numpy()
+    arrays['losses'] = np.asarray([float(getattr(data.losses, k)) for k in sorted(vars(data.losses))], dtype=np.float64)
+    total = 0
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+        total += a.nbytes
+    assert total <= 64 << 20, f'dump is {total} bytes'
+    return sorted(arrays)
+
+
 def load_peak():
     p = os.path.join(REPO, 'MEASURED_PEAKS.json')
     try:
         return float(json.load(open(p))['hbm_gbs']), 'MEASURED_PEAKS.json (measured copy bandwidth)'
     except Exception:
-        return 6650.0, 'fallback 6.65 TB/s (B200_PROFILING.md)'
+        return 3350.0, 'fallback 3.35 TB/s (H100 SXM5 HBM3 specification)'
 
 
 def run_b200(args):
@@ -429,6 +472,7 @@ def run_b200(args):
     launches0, replays0, treplays0 = _native.lib().pb_launch_count(), data.graph_replays, data.train_graph_replays
     seg0 = getattr(data.train_segments, 'replayed_launches', 0)
     ms = timed_steps(data, cp, args.steps, world)
+    dumped = dump_outputs(data, args.dump_outputs) if args.dump_outputs and rank == 0 else None
     launches = ((_native.lib().pb_launch_count() - launches0) + (data.graph_replays - replays0) * data.graph_launches
                 + (data.train_graph_replays - treplays0) * data.train_graph_launches
                 + (getattr(data.train_segments, 'replayed_launches', 0) - seg0))
@@ -476,7 +520,7 @@ def run_b200(args):
     if world == 1 and not args.no_extra_configs:
         import copy
         for key, kw in (('c3_snake', dict(env='snake', num_envs=65536, horizon=256)),
-                        ('c4_pong', dict(env='pong', num_envs=8192, horizon=128))):
+                        ('c4_pong', dict(env='pong', num_envs=4096, horizon=128))):
             try:
                 a2 = copy.copy(args)
                 for k_, v_ in kw.items():
@@ -509,8 +553,10 @@ def run_b200(args):
                        'cuda_graph_train': 'whole' if data.train_graph_state == 2 else ('segments' if data.train_segments else False), 'zero_copy_minibatches': getattr(data.experience, '_slabs', None) is not None, 'note': data.msg},
             'e2e': e2e, 'gpu_launches': int(launches), 'roofline': roof, 'roofline_kernels': roof_all,
             'roofline_other_configs': extra,
-            'cpu_baseline': cpu, 'clocks': clk, 'profile_s': prof, 'env_stats': stats,
+            'cpu_baseline': cpu, 'clocks': clk, 'gpu': gpu_info(local), 'profile_s': prof, 'env_stats': stats,
         }
+        if dumped is not None:
+            line['dumped_outputs'] = {'dir': args.dump_outputs, 'arrays': dumped}
         print(json.dumps(line))
     cp.close(data)
     if world > 1:

@@ -1,7 +1,7 @@
-/* pufferlib_b200.h -- C ABI of libpuffer_b200.so: the B200 (sm_100a) env-step + PPO-rollout hot path.
+/* pufferlib_b200.h -- C ABI of libpuffer_b200.so: the H100 (sm_90a) env-step + PPO-rollout hot path.
  *
  * This is the drop-in boundary for PufferLib's vectorised env step / rollout / GAE / minibatch path.
- * Every entry point below names the reference interface it replaces (paths under /root/reference).
+ * Every entry point below names the reference interface it replaces (paths under the reference checkout).
  * The reference has no C ABI of its own on this path: its native seams are the `PufferEnv` buffer-injection
  * protocol (pufferlib/environment.py:1-21 + vector.py:97-110) and two Cython functions
  * (c_gae.pyx:11 `compute_gae`, pufferlib/extensions.pyx:19,32 `emulate`/`nativize`); the rest is Python
@@ -237,7 +237,7 @@ int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const float* w_en
  * The H-iteration body of clean_pufferl.evaluate (clean_pufferl.py:84-124: recv -> policy -> store -> send) for a
  * breakout handle and models.Default (128 features, 128 hidden, n_act <= 4) in ONE launch: a CTA owns 128 envs for all
  * `horizon` steps, env state in registers, observation tile in shared memory feeding both the TMA store to the rollout
- * tensor and the tcgen05 encoder GEMM (W_enc resident in shared memory), heads + sampling + value / logprob / action row
+ * tensor and the wgmma encoder GEMM (W_enc resident in shared memory), heads + sampling + value / logprob / action row
  * stores by the env's own thread.  Rollout tensors are time-major [horizon * N] (row t*N + e); row 0 takes reward / done
  * from the carry buffers (the vecenv's own buffers, pb_env_out with dones_f32), the step that closes the rollout writes
  * the carry buffers (obs / rewards / terminals / dones_f32) -- the bound-rollout convention of vector.B200.  Sampling:
@@ -266,8 +266,8 @@ int pb_mlp_tail_backward(const float* dout, int64_t dout_stride, const float* w_
 /* -- fused minibatch update (forward + PPO loss + backward) -------------------------------------------------------------
  * One minibatch of clean_pufferl.train (clean_pufferl.py:186-244) for models.Default (pufferlib/models.py:12-62) with
  * 128 fp32 input features, 128 hidden units and <= 7 actions, up to and including the gradients, in ONE persistent
- * tcgen05 kernel (+ a small deterministic partial-sum kernel): encoder GEMM and dW_enc = dPre^T x on the 5th-gen tensor
- * cores (kind::tf32, fp32 accumulation in TMEM), heads / pb_ppo_loss row math / ReLU backward in the epilogue warps.
+ * wgmma kernel (+ a small deterministic partial-sum kernel): encoder GEMM and dW_enc = dPre^T x on the Hopper tensor
+ * cores (TF32, fp32 accumulation in registers), heads / pb_ppo_loss row math / ReLU backward on the accumulator registers.
  * The observations are read from HBM once; hidden and dPre never leave the SM.
  *   x            n_slabs slabs of slab_rows rows x 128 features, row stride ldx floats; slab s starts slab_stride_rows rows
  *                after slab s-1 (the zero-copy minibatch view of the time-major rollout; n_slabs = 1: a plain matrix)
@@ -278,19 +278,17 @@ int pb_mlp_tail_backward(const float* dout, int64_t dout_stride, const float* w_
  *   returns      nullable: advantages (raw) + old_values is used (clean_pufferl.py:476-481)
  *   grad_flat    [128*128 + 8*128 + 128 + 8]: dW_enc | dW_heads | db_enc | db_heads  (what pb_clip_adam consumes)
  *   stats8       the six loss sums of pb_ppo_loss (zeroed here)
- *   dpre_out     null: dW_enc = dPre^T x is accumulated inside the kernel (MN-major UMMAs; x is loaded a second time in the
- *                SWIZZLE_128B_BASE32B layout the tensor core requires for transposed 32-bit operands).  Non-null: dPre
+ *   dpre_out     null: dW_enc = dPre^T x is accumulated inside the kernel (wgmma with x^T fragments in registers and
+ *                dPre^T in shared memory).  Non-null: dPre
  *                [M][128] (slab-major rows) is written there instead and the dW_enc part of grad_flat is left to the caller
  *   dbg_*        nullable dumps of relu(h) [M][128], dPre [M][128], dOut [M][8] for validation. */
 size_t pb_mlp_update_workspace_bytes(void);
-/* 1 = two x layouts per tile (K-major + MN-major TMA loads), 2 = one x layout, x^T formed on the tensor core */
+/* epilogue products: 1 = fp32 head / dPre products, 2 = TF32 mma.sync products (default) */
 int pb_mlp_update_set_variant(int32_t variant);
 /* the reduce step of pb_mlp_update_fused also leaves the sum of squares of the gradient it wrote as pb_mlp_update_sumsq_parts()
  * doubles at byte pb_mlp_update_sumsq_offset() of the workspace (dW-in-kernel mode): input of pb_clip_adam_parts */
 size_t pb_mlp_update_sumsq_offset(void);
 int32_t pb_mlp_update_sumsq_parts(void);
-/* profiling hook (variant 2): SM-clock stamps of tiles 8..11, [grid][18 warps][4][8] int64; NULL switches it off */
-int pb_mlp_update_debug_clock(long long* buf);
 int pb_mlp_update_fused(const float* x, int64_t ldx, int64_t slab_rows, int64_t slab_stride_rows, int32_t n_slabs,
                         const float* w_enc, const float* b_enc, const float* w_heads, const float* b_heads,
                         const int64_t* actions, const float* old_logprobs, const float* advantages, const float* returns,

@@ -1,8 +1,10 @@
-"""Compile the reference's OWN ``c_gae.pyx`` from where it lies under /root/reference.  TEST INFRASTRUCTURE.
+"""Compile the reference's OWN ``c_gae.pyx`` from a PufferLib source checkout.  TEST INFRASTRUCTURE.
 
-Recipe (no reference build system involved): ``cython`` translates /root/reference/c_gae.pyx to C in a temp
-dir, ``gcc`` compiles that one file into ``oracle/_ref/c_gae*.so`` (git-ignored, travels to the GPU box with
-the snapshot).  Nothing is copied into the repo history.  ``load()`` imports the built module if present.
+The checkout is the directory named by the environment variable PUFFERLIB_REFERENCE (nothing is built without it).
+Recipe (no reference build system involved): ``cython`` translates its c_gae.pyx to C in a temp dir, ``gcc``
+compiles that one file into ``oracle/_ref/c_gae*.so`` (git-ignored).  Nothing is copied into the repo history.
+``load()`` imports the built module if present; tests/golden/generate.py stores its outputs as golden data, so the
+tests compare against the reference without it.
 """
 import glob
 import importlib.util
@@ -13,17 +15,23 @@ import sysconfig
 import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = '/root/reference'
 OUT = os.path.join(HERE, '_ref')
+
+
+def reference_dir():
+    """The PufferLib source checkout named by PUFFERLIB_REFERENCE, or None."""
+    ref = os.environ.get('PUFFERLIB_REFERENCE')
+    return ref if ref and os.path.exists(os.path.join(ref, 'c_gae.pyx')) else None
 
 
 def build(force=False):
     existing = glob.glob(os.path.join(OUT, 'c_gae*.so'))
     if existing and not force:
         return existing[0]
-    src = os.path.join(REF, 'c_gae.pyx')
-    if not os.path.exists(src):
+    ref = reference_dir()
+    if ref is None:
         return None
+    src = os.path.join(ref, 'c_gae.pyx')
     import numpy as np
     os.makedirs(OUT, exist_ok=True)
     ext = sysconfig.get_config_var('EXT_SUFFIX')

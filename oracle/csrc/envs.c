@@ -1,7 +1,7 @@
 /* Scalar plain-C restatement of oracle/SPEC.md (breakout, snake, pong) + the reference vectoriser's send loop.
  * TEST INFRASTRUCTURE (see oracle/__init__.py): the checker for the CUDA env kernels and the CPU baseline.
  *
- * Vectoriser semantics follow /root/reference/pufferlib/vector.py:137-156 (per env: `if env.done: reset() else
+ * Vectoriser semantics follow reference pufferlib/vector.py:137-156 (per env: `if env.done: reset() else
  * step()`), emulation.py:187-192,219-224 (buffer rows) and postprocess.py:22-54 (EpisodeStats).  The dynamics
  * are OUR spec (parity unpinned against the reference, SPEC.md header).  One env at a time, straightforward
  * array code -- deliberately not shaped like the CUDA kernels.  `#pragma omp parallel for` over envs is the

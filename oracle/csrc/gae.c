@@ -1,6 +1,6 @@
 /* Plain-C restatement of the reference's GAE recurrence.  TEST INFRASTRUCTURE (see oracle/__init__.py).
  *
- * Follows /root/reference/c_gae.pyx:11-32: one backward chain over the flat, (env_id, step)-sorted batch,
+ * Follows reference c_gae.pyx:11-32: one backward chain over the flat, (env_id, step)-sorted batch,
  * all arithmetic in C `float`, association exactly as written there:
  *     nextnonterminal = 1.0 - dones[t+1]
  *     delta       = rewards[t+1] + gamma * values[t+1] * nextnonterminal - values[t]

@@ -1,6 +1,6 @@
 """``clean_pufferl.Experience`` + the train-side prep, restated in numpy.  TEST INFRASTRUCTURE.
 
-Follows /root/reference/clean_pufferl.py:
+Follows reference clean_pufferl.py:
   :382-434  __init__  (flat [batch_size] arrays in arrival (ptr) order, validation errors)
   :436-450  store     (masked rows appended at ptr; sort key (env_id, step) per row)
   :452-464  sort_training_data  (lexicographic argsort -> idxs; b_idxs_obs = idxs.reshape(rows, n_mb, bptt).transpose(1,0,2))

@@ -1,6 +1,6 @@
 """``c_gae.compute_gae`` restated.  TEST INFRASTRUCTURE (see oracle/__init__.py).
 
-``compute_gae_np``  sequential numpy-fp32 loop following /root/reference/c_gae.pyx:24-30 (small cases).
+``compute_gae_np``  sequential numpy-fp32 loop following reference c_gae.pyx:24-30 (small cases).
 ``compute_gae``     ctypes call into ``oracle/csrc/gae.c`` (same recurrence in C, any size).
 ``compute_gae_f64`` the recurrence in float64 (C): ground truth used to put both the reference's and the
                     CUDA scan's rounding error on one scale in the tolerance tests.

@@ -1,7 +1,7 @@
 """MT19937 exactly as CPython's ``random`` module drives it.  TEST INFRASTRUCTURE (see oracle/__init__.py).
 
 The reference's ``Squared.reset`` draws its target with ``random.sample(possible_targets, 1)`` from the
-process-global ``random`` after ``random.seed(seed)`` (/root/reference/pufferlib/environments/ocean/ocean.py:448-461).
+process-global ``random`` after ``random.seed(seed)`` (reference pufferlib/environments/ocean/ocean.py:448-461).
 For an int seed CPython's ``random.seed`` is ``init_by_array(key)`` with ``key`` = the little-endian 32-bit
 words of ``abs(seed)`` (one word for seed < 2**32), and ``random.sample(pop, 1)`` with ``len(pop) == 24`` is one
 ``_randbelow_with_getrandbits(24)``: ``r = getrandbits(5)`` (= ``genrand_uint32() >> 27``) repeated until

@@ -1,6 +1,6 @@
 """``vector.Serial`` over N ``Squared`` envs, restated as one array program.  TEST INFRASTRUCTURE.
 
-Follows (all under /root/reference/pufferlib/):
+Follows (all under reference pufferlib/):
   environments/ocean/ocean.py:424        MOVES table
   environments/ocean/ocean.py:444-446    _all_possible_targets (x-major perimeter order)
   environments/ocean/ocean.py:448-463    Squared.reset  (grid=0, agent -1 at centre, one target +1)

@@ -1,4 +1,4 @@
-"""pufferlib_b200 -- B200-native (sm_100a) env-step + PPO-rollout hot path behind PufferLib's own interfaces.
+"""pufferlib_b200 -- H100-native (sm_90a) env-step + PPO-rollout hot path behind PufferLib's own interfaces.
 
     import pufferlib_b200.vector, pufferlib_b200.clean_pufferl
     vecenv = pufferlib_b200.vector.make(pufferlib_b200.environments.ocean.env_creator('squared'),

@@ -87,7 +87,6 @@ SIGNATURES = {
     'pb_rollout_debug_buffers': (C.c_int, [C.c_void_p, C.c_void_p]),
     'pb_mlp_update_workspace_bytes': (C.c_size_t, []),
     'pb_mlp_update_set_variant': (C.c_int, [C.c_int32]),
-    'pb_mlp_update_debug_clock': (C.c_int, [C.c_void_p]),
     'pb_mlp_update_fused': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32] + [C.c_void_p] * 10 +
                             [C.c_int64, C.c_int32, C.c_float, C.c_int32, C.c_float, C.c_float, C.c_float] + [C.c_void_p] * 3 +
                             [C.c_size_t] + [C.c_void_p] * 5),
@@ -133,7 +132,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(SO_PATH):
             raise RuntimeError(
-                f'{SO_PATH} is missing: build it with `python -m pufferlib_b200.build` (nvcc, sm_100a). '
+                f'{SO_PATH} is missing: build it with `python -m pufferlib_b200.build` (nvcc, sm_90a). '
                 'pufferlib_b200 has no CPU fallback.')
         handle = C.CDLL(SO_PATH)
         for name, (res, args) in SIGNATURES.items():

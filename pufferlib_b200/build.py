@@ -1,9 +1,9 @@
-"""Build libpuffer_b200.so in-tree with nvcc for sm_100a (and nothing else).
+"""Build libpuffer_b200.so in-tree with nvcc for sm_90a (H100; nothing else).
 
     python -m pufferlib_b200.build [--force] [--verbose]
 
 The shared library has a plain C ABI (include/pufferlib_b200.h) and links only cudart: no torch, no pybind.
-It is written next to this file so the gpurun snapshot carries it to the B200 box.
+It is written next to this file, so the package imports from the source tree.
 """
 import glob
 import os
@@ -14,9 +14,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, 'csrc')
 SO = os.path.join(HERE, 'libpuffer_b200.so')
-NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
+NVCC = os.environ.get('NVCC') or os.path.join(os.environ.get('CUDA_HOME', '/usr/local/cuda'), 'bin', 'nvcc')
 
-ARCH_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '-I', os.path.join(REPO, 'include'), '-I', CSRC]
 
 
@@ -58,23 +58,5 @@ def build(force=False, verbose=False):
     return SO
 
 
-EXP_SO = os.path.join(HERE, 'libpuffer_b200_exp.so')
-
-
-def build_experimental(force=False, verbose=False):
-    """csrc/experimental/*.cu -> libpuffer_b200_exp.so: the tcgen05 descriptor probe (umma_probe.cu) behind the layout facts
-    DESIGN.md section 7 lists.  Nothing in the product path loads it; tests/experimental/ holds the scripts that drive it."""
-    srcs = sorted(glob.glob(os.path.join(CSRC, 'experimental', '*.cu')))
-    deps = srcs + glob.glob(os.path.join(CSRC, '*.cuh'))
-    if not force and os.path.exists(EXP_SO) and all(os.path.getmtime(EXP_SO) >= os.path.getmtime(d) for d in deps):
-        return EXP_SO
-    cmd = [NVCC] + ARCH_FLAGS + COMMON + (['-Xptxas', '-v'] if verbose else []) + ['-shared', '-o', EXP_SO] + srcs + \
-        ['-lcudart']
-    subprocess.check_call(cmd)
-    return EXP_SO
-
-
 if __name__ == '__main__':
     print(build(force='--force' in sys.argv, verbose='--verbose' in sys.argv))
-    if '--experimental' in sys.argv:
-        print(build_experimental(force='--force' in sys.argv, verbose='--verbose' in sys.argv))

@@ -1,6 +1,6 @@
 """``clean_pufferl`` create / evaluate / train / close with the reference signatures, device-resident.
 
-Mirrors /root/reference/clean_pufferl.py: ``create`` (:30-73), ``evaluate`` (:75-154), ``train`` (:156-292),
+Mirrors reference clean_pufferl.py: ``create`` (:30-73), ``evaluate`` (:75-154), ``train`` (:156-292),
 ``close`` (:294-304), ``Experience`` (:380-482), ``make_losses`` (:369-378), ``seed_everything``.  What changes:
 
 * ``Experience`` tensors all live in HBM in arrival order (row t*N + e) -- the same memory layout the reference
@@ -186,10 +186,10 @@ def slab_row_index(num_envs, horizon, num_minibatches, bptt_horizon):
     return rows.transpose(1, 0, 2).reshape(num_minibatches, g_ * r_)
 
 
-# the fused tcgen05 minibatch-update kernel (csrc/mlp_update.cu) is the default where it applies; config.fused_update
+# the fused wgmma minibatch-update kernel (csrc/mlp_update.cu) is the default where it applies; config.fused_update
 # overrides
 FUSED_UPDATE_DEFAULT = True
-FUSED_UPDATE_DW_DEFAULT = 'kernel'      # dW_enc inside the fused kernel (6.45 ms/step at C2) vs 'cublas' (dPre to HBM + split-K GEMM, 7.7 ms)
+FUSED_UPDATE_DW_DEFAULT = 'kernel'      # dW_enc inside the fused kernel vs 'cublas' (dPre to HBM + split-K GEMM)
 # the persistent rollout kernel (pb_rollout_breakout_mlp) likewise; config.fused_rollout overrides
 FUSED_ROLLOUT_DEFAULT = True
 
@@ -199,7 +199,7 @@ class _DefaultMLPUpdate:
     instead of through autograd: with 17k parameters and 524k-row minibatches the update is a fixed chain of seven
     large kernels, and everything autograd, clip_grad_norm_ and the optimizer add around it (gradient scaling by the
     upstream 1.0, AccumulateGrad copies, ~12 norm/clip/Adam launches, 6 launches to re-pack the heads, 8 to fold the
-    statistics) is ~120 us of 3-us launches per minibatch.  Chain per minibatch:
+    statistics) is a dozen short launches per minibatch.  Chain per minibatch:
         encoder GEMM (+bias+ReLU epilogue, one per slab) -> 8-column head GEMM -> pb_ppo_loss (loss statistics +
         analytic dLoss/dOut) -> pb_mlp_tail_backward (dPre, dW_heads, db_heads, db_enc) -> split-K dW_enc GEMM + sum
         [-> gradient all-reduce over ONE flat buffer when world_size > 1] -> pb_clip_adam -> pb_pack_heads.
@@ -334,7 +334,7 @@ class _DefaultMLPUpdate:
         x = x.flatten(2)
         assert row_slab_stride is None or self._fused_ok(x, config)
         if self._fused_ok(x, config):
-            # ONE tcgen05 kernel: x read once, hidden / dPre stay on the SM, gradients land in self.gflat
+            # ONE wgmma kernel: x read once, hidden / dPre stay on the SM, gradients land in self.gflat
             g_, r_, _ = x.shape
             lib = _native.lib()
             if self.stats is None or self.stats.shape[0] != n_stats:
@@ -343,7 +343,7 @@ class _DefaultMLPUpdate:
                 self.fused_ws = torch.empty(lib.pb_mlp_update_workspace_bytes(), dtype=torch.uint8, device=self.gflat.device)
             self.mb_rows = g_ * r_
             m_ = self.model
-            # where dW_enc = dPre^T x is formed: inside the kernel (MN-major UMMAs, dPre never leaves the SM), or by a
+            # where dW_enc = dPre^T x is formed: inside the kernel (wgmma, dPre never leaves the SM), or by a
             # library GEMM on dPre written to HBM (config.fused_update_dw = 'cublas')
             in_kernel = str(getattr(config, 'fused_update_dw', FUSED_UPDATE_DW_DEFAULT)) == 'kernel'
             if not in_kernel and (self.fused_dpre is None or self.fused_dpre.shape[0] != g_ * r_):
@@ -818,7 +818,7 @@ def _rollout_loop(data, infos):
     policy, vecenv = data.policy, data.vecenv
     on_device = not getattr(vecenv, 'host_buffers', False)
     io = data.io
-    # the whole horizon as ONE persistent kernel (env state in registers, tcgen05 policy, csrc/env_breakout.cu) where it applies
+    # the whole horizon as ONE persistent kernel (env state in registers, wgmma policy, csrc/env_breakout.cu) where it applies
     if bool(getattr(config, 'fused_rollout', FUSED_ROLLOUT_DEFAULT)) and hasattr(vecenv, 'fused_rollout_ok') and \
             data.fused_rows and vecenv.fused_rollout_ok(experience, policy):
         with profile.env:
@@ -837,7 +837,7 @@ def _rollout_loop(data, infos):
 
         with profile.eval_misc:
             # sum(mask) of clean_pufferl.py:90; count_nonzero instead of the Python-level sum over a numpy array, which
-            # costs 1 ms per env step at N = 16384
+            # costs a host round trip per env step
             data.global_step += len(env_id) if (on_device or device_feed) else int(np.count_nonzero(mask))
             if on_device or device_feed:
                 o_device = o      # the device copy of the observations already exists: no H2D (clean_pufferl.py:92-95)

@@ -14,6 +14,7 @@
 
 #include "env_common.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -50,7 +51,7 @@ __device__ __forceinline__ void bk_physics(int& px, int& lives, int& in_play, in
                                            int& reward, bool& terminal, float& score) {
     // actions are clamped to [0, 3] by the spec (a < 0 -> NOOP, a > 3 -> LEFT).  Written as three comparisons on the raw
     // value: ptxas 12.9 turned `a = clamp(a, 0, 3); if (a == 3) ..` into a VIMNMX.RELU with predicate outputs whose
-    // predicate came out true for a == 2 on sm_100a (the paddle moved left instead of right; caught by the oracle tests)
+    // predicate came out true for a == 2 when targeting sm_100a (the paddle moved left instead of right; caught by the oracle tests)
     const bool fire = a == 1, go_right = a == 2, go_left = a >= 3;
     if (go_right) px = min(px + 4, 136);
     if (go_left) px = max(px - 4, 0);
@@ -182,15 +183,16 @@ __global__ void __launch_bounds__(128) k_breakout(BreakoutState st, int n, const
 // =====================================================================================================================
 // Persistent rollout: H vectorised env steps WITH the policy in the loop in ONE launch (config C2 / C5: breakout +
 // models.Default 128 -> 128 -> {n_act, 1}).  Replaces the H x (k_breakout + k_policy_mlp_sample) launches of
-// clean_pufferl.evaluate (/root/reference/clean_pufferl.py:84-124: recv -> policy -> store -> send): the policy weights
-// are frozen during a rollout and the envs are independent, so a CTA owns 128 envs for all H steps --
+// clean_pufferl.evaluate (recv -> policy -> store -> send): the policy weights are frozen during a rollout and the envs are
+// independent, so a CTA owns 128 envs for all H steps --
 //   * env state lives in REGISTERS across steps (thread = env); HBM sees it once at the start and once at the end;
 //   * the observation row is built once, into a SWIZZLE_128B K-major tile in shared memory, from where (a) four TMA tensor
-//     stores write it to the rollout tensor (fully coalesced 64 KB per tile) and (b) the 5th-gen tensor core consumes it:
-//     hidden = obs . W_enc^T as 16 tcgen05.mma.kind::tf32 (M = 128 envs, N = 128, K = 8) into TMEM, W_enc resident in
-//     shared memory for the whole rollout (one TMA load per CTA instead of one 64 KB re-stage per CTA per env step);
-//   * thread = env = TMEM lane reads its hidden row back (tcgen05.ld), applies bias + ReLU, the two heads (W_heads as
-//     constant-bank FFMA operands), samples the action by inverse CDF on the counter-based uniform of
+//     stores (issued by warp 4) write it to the rollout tensor (fully coalesced 64 KB per tile) and (b) the Hopper tensor
+//     core consumes it: the four env warps are one warpgroup and compute hidden = obs . W_enc^T as two wgmma chains
+//     (M = 64 envs, N = 128, K = 8 per instruction, accumulators in registers), W_enc resident in shared memory for the
+//     whole rollout (one TMA load per CTA instead of one 64 KB re-stage per CTA per env step);
+//   * bias + ReLU on the accumulator, staged K-major in the observation tile that is not in flight; the two heads on
+//     mma.sync fragments; then thread = env samples the action by inverse CDF on the counter-based uniform of
 //     pb_policy_mlp_sample (same key: seed, step counter, env row), stores value / logprob / action rows, and steps its
 //     env with that action -- no global round trip between policy and env.
 // Observation values are k/256, k/8, k/4 or 0/1: exact in TF32, so only W_enc is rounded (truncated) by the tensor core.
@@ -198,13 +200,12 @@ __global__ void __launch_bounds__(128) k_breakout(BreakoutState st, int n, const
 // copied from the vecenv's own buffers), step t's outputs go to row t+1, the step that closes the rollout writes the
 // vecenv's own buffers again.
 // =====================================================================================================================
-constexpr int RO_ENVS = 128;                 // envs per CTA = UMMA M = TMEM lanes
-constexpr int RO_THREADS = 160;              // warps 0..3: env / epilogue threads, warp 4: MMA + TMA issue
+constexpr int RO_ENVS = 128;                 // envs per CTA = two wgmma M blocks of 64
+constexpr int RO_THREADS = 160;              // warps 0..3: env / policy threads (one warpgroup), warp 4: TMA issue
 constexpr int RO_KBLK_BYTES = RO_ENVS * 32 * 4;          // 16 KiB: [128 rows][32 floats]
 constexpr int RO_TILE_BYTES = 4 * RO_KBLK_BYTES;         // 64 KiB
 constexpr int RO_SMEM_W = 0, RO_SMEM_X = RO_TILE_BYTES, RO_SMEM_BAR = 3 * RO_TILE_BYTES;
 constexpr int RO_SMEM_TOTAL = RO_SMEM_BAR + 128;
-constexpr int RO_TMEM_COLS = 128;
 constexpr int RO_HEADS = 5;                  // live rows of the 8-row head matrix: breakout has 4 actions + the value
 
 __constant__ float c_ro_wh[8 * 128];
@@ -244,27 +245,6 @@ __device__ __forceinline__ void ro_tma_store_2d(const CUtensorMap* map, int c0, 
                      reinterpret_cast<uint64_t>(map)),
                  "r"(c0), "r"(c1), "r"(smem_u32(src))
                  : "memory");
-}
-__device__ __forceinline__ uint64_t ro_desc_kmajor(uint32_t saddr) {   // SWIZZLE_128B K-major (see csrc/mlp_update.cu)
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-constexpr uint32_t RO_IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-
-__device__ __forceinline__ void ro_tmem_ld32(uint32_t taddr, float (&r)[32]) {
-    uint32_t u[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]), "=r"(u[8]),
-          "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]), "=r"(u[16]),
-          "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]), "=r"(u[24]),
-          "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) r[i] = __uint_as_float(u[i]);
 }
 
 // the observation row of one env (same values as k_breakout's cooperative row write) into row r of a SW128 K-major tile
@@ -306,8 +286,7 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RO_SMEM_BAR);
     uint64_t* w_full = bars;          // W_enc landed
     uint64_t* tile_full = bars + 1;   // [2] observation tile written by the 128 env threads
-    uint64_t* h_full = bars + 3;      // hidden accumulator complete
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+    uint64_t* tile_free = bars + 3;   // the tensor store of the previous step has finished reading its tile
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int e0 = blockIdx.x * RO_ENVS;
     const int H = p.horizon;
@@ -316,54 +295,24 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
         mbar_init(w_full, 1);
         mbar_init(&tile_full[0], RO_ENVS);
         mbar_init(&tile_full[1], RO_ENVS);
-        mbar_init(h_full, 1);
+        mbar_init(tile_free, 1);
         mbar_fence_init();
     }
-    if (warp == 4) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"((uint32_t)RO_TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 4) {
-        // ================= MMA + TMA issue (one thread) =================
+        // ================= TMA issue (one thread) =================
         if (lane == 0) {
             mbar_expect_tx(w_full, RO_TILE_BYTES);
             for (int kb = 0; kb < 4; ++kb) ro_tma_load_2d(smem + RO_SMEM_W + kb * RO_KBLK_BYTES, &map_w, kb * 32, 0, w_full);
-            mbar_wait(w_full, 0);
-            const uint32_t w_addr = smem_u32(smem + RO_SMEM_W);
             for (int t = 0; t <= H; ++t) {
                 const int s = t & 1;
                 uint8_t* tile = smem + RO_SMEM_X + s * RO_TILE_BYTES;
                 mbar_wait(&tile_full[s], (uint32_t)((t >> 1) & 1));     // all 128 rows of obs(t) are in the tile
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                // the tensor store of obs(t-1) has finished READING the other tile before the commit below lets the env
-                // threads (who wait for h_full(t)) overwrite it with obs(t+1); it had a whole step: no stall in practice
+                // the tensor store of obs(t-1) has finished READING the other tile: the env threads may stage relu(h) of
+                // step t there and then overwrite it with obs(t+1); it had a whole step: no stall in practice
                 tma_wait_read<0>();
-                if (t < H) {
-                    const uint32_t x_addr = smem_u32(tile);
-#pragma unroll
-                    for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            asm volatile(
-                                "{\n\t"
-                                ".reg .pred p;\n\t"
-                                "setp.ne.b32 p, %4, 0;\n\t"
-                                "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-                                "}\n" ::"r"(tmem_base),
-                                "l"(ro_desc_kmajor(x_addr + kb * RO_KBLK_BYTES + k * 32)),
-                                "l"(ro_desc_kmajor(w_addr + kb * RO_KBLK_BYTES + k * 32)), "r"(RO_IDESC), "r"((kb | k) ? 1u : 0u)
-                                : "memory");
-                    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                                     smem_u32(h_full))
-                                 : "memory");
-                }
+                asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(tile_free)) : "memory");
                 // the same tile goes to HBM: rollout row t, or the vecenv's own observation buffer for the closing step
                 const CUtensorMap* map = t < H ? &map_obs : &map_carry;
                 const int row0 = t < H ? t * p.n + e0 : e0;
@@ -373,7 +322,7 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
             tma_wait_all<0>();
         }
     } else {
-        // ================= env threads: thread = env = TMEM lane =================
+        // ================= env threads: thread = env; warps 0..3 = the warpgroup of the policy products =================
         const int r = threadIdx.x;                    // 0..127
         const int e = e0 + r;                         // n is a multiple of 128 (checked by the launcher)
         const uint64_t seed_e = p.st.seed + (uint64_t)e;
@@ -395,41 +344,59 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
         fence_proxy_async_smem();
         asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tile_full[0])) : "memory");
 
-        // head products on mma.sync fragments (like k_mlp_update_xt and k_policy_mlp_sample): out[32 rows][8] = relu(h) . W_heads^T
+        // head products on mma.sync fragments (like k_mlp_update and k_policy_mlp_sample): out[32 rows][8] = relu(h) . W_heads^T
         // with the warp's relu(h) staged K-major ([hidden unit][row], 16-byte pieces XORed with unit & 7) in the observation
         // tile that is NOT in flight, W_heads fragments resident in registers (k = t + 4j <-> hidden unit 8kb + 2t + j), and the
-        // m index permuted (m = g + 8h of block mb <-> row 4g + 2mb + h) so that an A fragment is one LDS.128.  A thread-per-row
-        // FFMA formulation (640 FFMA + constant loads per step at one warp per scheduler) was 25 % of the step.
+        // m index permuted (m = g + 8h of block mb <-> row 4g + 2mb + h) so that an A fragment is one LDS.128.
         const int g = lane >> 2, tq = lane & 3;
         uint32_t hb[16][2];
+        float benc[16][2];                            // b_enc of the accumulator columns 8j + 2tq + {0, 1}
 #pragma unroll
         for (int kb = 0; kb < 16; ++kb) {
             hb[kb][0] = ro_to_tf32(c_ro_wh[g * 128 + 8 * kb + 2 * tq]);
             hb[kb][1] = ro_to_tf32(c_ro_wh[g * 128 + 8 * kb + 2 * tq + 1]);
+            benc[kb][0] = c_ro_benc[8 * kb + 2 * tq];
+            benc[kb][1] = c_ro_benc[8 * kb + 2 * tq + 1];
         }
         const float bh_row[8] = {c_ro_bh[0], c_ro_bh[1], c_ro_bh[2], c_ro_bh[3], c_ro_bh[4], c_ro_bh[5], c_ro_bh[6], c_ro_bh[7]};
+        const uint32_t w_addr = smem_u32(smem + RO_SMEM_W);
+        mbar_wait(w_full, 0);
 
         for (int t = 0; t < H; ++t) {
-            // ---- policy on obs(t): hidden row from TMEM -> heads -> sample
-            mbar_wait(h_full, (uint32_t)(t & 1));
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            // (the MMA thread waited for the tensor store of obs(t-1) before it committed h_full(t): the other tile is free)
-            uint8_t* blk = smem + RO_SMEM_X + ((t + 1) & 1) * RO_TILE_BYTES + warp * RO_KBLK_BYTES;   // [128 hidden units][32 rows]
-            uint8_t* st_row = blk + ((lane & 3) << 2);
-            const uint32_t taddr = tmem_base + ((uint32_t)(32 * warp) << 16);
+            // ---- policy on obs(t): hidden = obs . W_enc^T on the tensor core -> bias + ReLU -> heads -> sample
+            asm volatile("bar.sync 1, 128;" ::: "memory");      // every row of obs(t) is in the tile (each writer fenced)
+            const uint32_t x_addr = smem_u32(smem + RO_SMEM_X + (t & 1) * RO_TILE_BYTES);
+            uint8_t* other = smem + RO_SMEM_X + ((t + 1) & 1) * RO_TILE_BYTES;
+            mbar_wait(tile_free, (uint32_t)(t & 1));           // the other tile is no longer read by a tensor store
+#pragma unroll 1
+            for (int half = 0; half < 2; ++half) {             // envs 64 half .. 64 half + 63 of the CTA
+                float acc[64];
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                float v[32];
-                ro_tmem_ld32(taddr + 32 * c, v);
+                for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+                wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 32; ++k) {
-                    const float rh = fmaxf(v[k] + c_ro_benc[32 * c + k], 0.f);
-                    if (DBG && p.dbg_hidden && t == 0) p.dbg_hidden[(int64_t)e * 128 + 32 * c + k] = rh;
-                    *reinterpret_cast<float*>(st_row + (32 * c + k) * 128 + ((((lane >> 2) ^ (k & 7))) << 4)) = rh;
-                }
+                for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        wgmma_m64n128k8_ss(acc, wgmma_desc_sw128(x_addr + kb * RO_KBLK_BYTES + half * 8192 + k * 32),
+                                           wgmma_desc_sw128(w_addr + kb * RO_KBLK_BYTES + k * 32), (kb | k) ? 1 : 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc);
+                // relu(h + b_enc) of rows 64 half + 16 warp + g (+8), hidden units 8j + 2tq (+1) -> block of the row's warp
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        const int row = 64 * half + 16 * warp + g + 8 * (q >> 1), k = 8 * j + 2 * tq + (q & 1);
+                        const float rh = fmaxf(acc[4 * j + q] + benc[j][q & 1], 0.f);
+                        if (DBG && p.dbg_hidden && t == 0) p.dbg_hidden[(int64_t)(e0 + row) * 128 + k] = rh;
+                        *reinterpret_cast<float*>(other + (row >> 5) * RO_KBLK_BYTES + k * 128 +
+                                                  ((((row & 31) >> 2) ^ (k & 7)) << 4) + (row & 3) * 4) = rh;
+                    }
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
+            asm volatile("bar.sync 1, 128;" ::: "memory");      // every relu(h) row is staged
+            uint8_t* blk = other + warp * RO_KBLK_BYTES;        // [128 hidden units][32 rows]: rows 32 warp .. 32 warp + 31
             float out[8];
             {
                 float hp[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
@@ -558,11 +525,6 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
         p.acc.ep_return[e] = ep_ret;
         p.acc.ep_length[e] = ep_len;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 4)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)RO_TMEM_COLS)
-                     : "memory");
 }
 
 __global__ void k_counter_add(uint64_t* c, uint64_t v) { *c += v; }

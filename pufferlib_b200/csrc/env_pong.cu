@@ -1,4 +1,4 @@
-// env_pong.cu -- N Pong instances with (4,84,84) uint8 frame-stack observations (oracle/SPEC.md §Pong), sm_100a.
+// env_pong.cu -- N Pong instances with (4,84,84) uint8 frame-stack observations (oracle/SPEC.md §Pong), sm_90a.
 //
 // Dynamics are the builder's spec (the reference's pong is ALE behind third-party wrappers: SURVEY.md §0); the
 // observation layout (4,84,84) uint8 NCHW, oldest frame first, is the reference's (atari/environment.py:37-39,

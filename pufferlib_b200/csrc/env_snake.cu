@@ -1,4 +1,4 @@
-// env_snake.cu -- N Snake instances (oracle/SPEC.md §Snake) behind the reference vectoriser semantics (sm_100a).
+// env_snake.cu -- N Snake instances (oracle/SPEC.md §Snake) behind the reference vectoriser semantics (sm_90a).
 //
 // Dynamics are the builder's spec (no snake exists in the reference: SURVEY.md §0); vectoriser / EpisodeStats
 // conventions are the reference's (vector.py:147-151, emulation.py:187-192, postprocess.py:22-54).  Bit-exact

@@ -1,6 +1,6 @@
-// env_squared.cu -- N instances of ocean.Squared behind vector.Serial semantics, on the device (sm_100a).
+// env_squared.cu -- N instances of ocean.Squared behind vector.Serial semantics, on the device (sm_90a).
 //
-// Bit-exact restatement of (paths under /root/reference/pufferlib/):
+// Bit-exact restatement of (paths under reference pufferlib/):
 //   environments/ocean/ocean.py:406-513   Squared (grid (2d+1)^2 fp32 in {-1,0,1}; 8 moves; reward 1 - Linf/d;
 //                                         done when tick >= d; one perimeter target; teleport to centre on the rim)
 //   environments/ocean/environment.py:28-31  distance_to_target=3, num_targets=1

@@ -1,7 +1,7 @@
-// gae.cu -- GAE as a single-pass affine suffix scan with decoupled look-back (sm_100a).
+// gae.cu -- GAE as a single-pass affine suffix scan with decoupled look-back (sm_90a).
 //
-// Replaces /root/reference/clean_pufferl.py:163-169 (sort_training_data + 3 numpy gathers) and
-// /root/reference/c_gae.pyx:11-32 (compute_gae).  Recurrence over the sorted batch f = e*H + t, B = N*H:
+// Replaces reference clean_pufferl.py:163-169 (sort_training_data + 3 numpy gathers) and
+// reference c_gae.pyx:11-32 (compute_gae).  Recurrence over the sorted batch f = e*H + t, B = N*H:
 //     A[B-1] = 0;   A[f] = a_f + b_f * A[f+1]
 //     nnt = 1 - d[f+1];  a_f = r[f+1] + (gamma*v[f+1])*nnt - v[f];  b_f = (gamma*lambda)*nnt
 // Affine maps compose associatively, (a,b)o(a',b') = (a + b a', b b'), so the chain is a suffix scan.
@@ -801,7 +801,10 @@ __global__ void __launch_bounds__(THREADS) k_gae_tile(GaeParams p) {
     }
 }
 
-int g_gae_variant = 0;   // 0: by horizon (measured: 2 at H <= 128, 3 above); 2 / 3: k_gae_tile double- / single-buffered; 1: k_gae_fast
+// 0: by horizon -- 2 at H <= 128, 3 above (H100 80GB HBM3 at 700 W, bench.py: C2 H = 128 23.7 us double- vs 25.0 us
+// single-buffered; C3 H = 256 162 us single- vs 177 us double-buffered); 2 / 3: k_gae_tile double- / single-buffered;
+// 1: k_gae_fast
+int g_gae_variant = 0;
 
 struct GaePlan {
     int fastKC;   // > 0: k_gae_fast<fastKC, nbuf>
@@ -921,7 +924,7 @@ extern "C" int pb_gae_tm(const float* rewards, const float* values, const float*
         k_gae_tile<KC, NBUF, THREADS><<<grid, THREADS, smem2, s>>>(p);                                                \
     }
         const bool v2_ok = !(returns_sorted && advantages_time_major);   // v2 stages two outputs: adv + (ret | adv_tm)
-        const int variant = g_gae_variant ? g_gae_variant : (g.fastKC == 1 ? 2 : 3);   // C2 (H = 128): 17.8 us either way; C3 (H = 256): 95 vs 119 us
+        const int variant = g_gae_variant ? g_gae_variant : (g.fastKC == 1 ? 2 : 3);   // double-buffered tiles for H = 128, single-buffered above
         if (variant == 2 && v2_ok) {
             if (g.fastKC == 1) PB_GAE_TILE(1, 2, 256) else if (g.fastKC == 2) PB_GAE_TILE(1, 2, 512) else PB_GAE_TILE(2, 1, 512)
         } else if (variant == 3 && v2_ok) {   // single-buffered tiles (more CTAs per SM), coalesced outputs

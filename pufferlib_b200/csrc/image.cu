@@ -1,14 +1,14 @@
-// image.cu -- image-observation row movers staged through shared memory by the TMA engine (sm_100a).
+// image.cu -- image-observation row movers staged through shared memory by the TMA engine (sm_90a).
 //
 //   pb_image_pack            frame-stack pack: obs_out[e] = [prev_obs[e][1..S-1], new_frame[e]]  (or S copies of the
 //                            new frame where reset_mask[e]).  Replaces the LazyFrames -> ndarray materialisation
-//                            inside `self.obs[:] = ob` (/root/reference/pufferlib/emulation.py:161-162) for the
+//                            inside `self.obs[:] = ob` (reference pufferlib/emulation.py:161-162) for the
 //                            (4,84,84) uint8 stack built by atari/environment.py:37-39.
-//   pb_minibatch_gather_tma  `b_obs = obs[b_idxs_obs]` (/root/reference/clean_pufferl.py:477) for rows >= 4 KiB.
+//   pb_minibatch_gather_tma  `b_obs = obs[b_idxs_obs]` (reference clean_pufferl.py:477) for rows >= 4 KiB.
 //
 // One warp per CTA; ONE elected thread drives a ring of STAGES shared-memory buffers: cp.async.bulk global->shared
 // (mbarrier complete_tx) then cp.async.bulk shared->global (bulk_group); no register staging, no LSU traffic.
-// 148 SMs x 2 resident CTAs x STAGES x <=28 KiB in flight covers the HBM latency-bandwidth product many times over.
+// 132 SMs x 2 resident CTAs x STAGES x <=28 KiB in flight covers the HBM latency-bandwidth product many times over.
 #include "pb_common.cuh"
 #include "tma.cuh"
 

@@ -1,6 +1,6 @@
-// mlp_tail.cu -- backward of the policy's "tail" (ReLU -> action/value heads) in one pass over the hidden layer (sm_100a).
+// mlp_tail.cu -- backward of the policy's "tail" (ReLU -> action/value heads) in one pass over the hidden layer (sm_90a).
 //
-// The configured policy is models.Default (/root/reference/pufferlib/models.py:12-62): Linear(obs->H)+ReLU, then two
+// The configured policy is models.Default (reference pufferlib/models.py:12-62): Linear(obs->H)+ReLU, then two
 // heads H->n_act and H->1.  In train (clean_pufferl.py:193-244) the backward of everything after the encoder GEMM is
 // memory-bound work on [M, H] tensors that ATen runs as five launches, each re-reading 268 MB at M = 524288:
 //   dHidden = dOut @ W_heads           (skinny GEMM, 8 columns)         dW_heads = dOut^T @ hidden   (skinny GEMM)

@@ -1,61 +1,61 @@
-// mlp_update.cu -- the whole minibatch forward + PPO loss + backward of models.Default in ONE persistent
-// tcgen05 kernel: the observations are read from HBM once, `hidden` / `dPre` never leave the SM.
+// mlp_update.cu -- the whole minibatch forward + PPO loss + backward of models.Default in ONE persistent Hopper kernel
+// (wgmma + TMA + mbarrier): the observations are read from HBM once, `hidden` / `dPre` never leave the SM.
 //
-// Replaces, per minibatch of clean_pufferl.train (/root/reference/clean_pufferl.py:186-244; policy =
-// /root/reference/pufferlib/models.py:12-62 with 128 input features, 128 hidden units, <= 7 actions), the chain
-//     hidden = relu(x W_enc^T + b_enc)            (cuBLAS GEMM, writes 268 MB at M = 524288)
-//     out    = hidden W_heads^T + b_heads         (cuBLAS GEMM, reads hidden)
+// Replaces, per minibatch of clean_pufferl.train (policy = models.Default with 128 input features, 128 hidden units,
+// <= 7 actions), the chain
+//     hidden = relu(x W_enc^T + b_enc)            (library GEMM, writes 268 MB at M = 524288)
+//     out    = hidden W_heads^T + b_heads         (library GEMM, reads hidden)
 //     pb_ppo_loss(out) -> dOut, statistics        (csrc/ppo_loss.cu)
 //     pb_mlp_tail_backward(dOut, hidden) -> dPre, dW_heads, db_enc, db_heads      (csrc/mlp_tail.cu, reads hidden, writes dPre)
-//     dW_enc = dPre^T x                           (split-K cuBLAS GEMM, reads dPre and x)
-// which streams `hidden` / `dPre` through HBM five times (1.9 GB, ~350 us per minibatch).  Here the algorithmic traffic is
-// x once (268 MB) + 28 B of per-row scalars (ncu: 287 MB of DRAM traffic per launch).
+//     dW_enc = dPre^T x                           (split-K library GEMM, reads dPre and x)
+// which streams `hidden` / `dPre` through HBM five times.  Here the algorithmic traffic is x once + 28 B of per-row scalars.
 //
-// Two kernels, the second one is the product path (pb_mlp_update_set_variant, default 2; DESIGN.md 3b):
-//   k_mlp_update_fused (variant 1, and the dPre-to-HBM mode of both variants): every x tile is loaded twice, K-major for
-//       the forward product and MN-major (SWIZZLE_128B_BASE32B, the only MN-major layout the tensor core takes for 32-bit
-//       operands) for dW_enc^T = x^T dPre; thread-per-row epilogue with the head products as constant-bank FFMAs.  293 us.
-//   k_mlp_update_xt (variant 2): ONE x layout; x^T is formed on the tensor core by a "sliding identity" MMA into tensor
-//       memory and enters the dW product as a TS operand; the 64 KB that frees hold a whole tile of dPre; 16 epilogue warps
-//       do all per-element products on mma.sync fragments.  168-190 us.
-// Both: warp 0 TMA producer, warp 1 single-thread tcgen05.mma issue + TMEM allocation, the rest epilogue; the dW_enc^T
-// accumulator lives in TMEM across all tiles of a CTA; per-CTA partials go to a workspace and k_update_reduce sums them
-// deterministically into the flat gradient buffer [dW_enc (hid x feat) | dW_heads (8 x hid) | db_enc | db_heads] of
-// clean_pufferl._DefaultMLPUpdate, leaving per-block sums of squares for pb_clip_adam_parts.
+// One kernel, k_mlp_update, two warpgroups (256 threads), one CTA per SM looping over 64-row tiles of the minibatch:
+//   * thread 0 keeps NSTAGE x tiles in flight (TMA, K-major SWIZZLE_128B), W_enc is resident in shared memory;
+//   * hidden^T [128 hidden units][64 rows] = W_enc . x^T on the tensor core (wgmma SS, warpgroup wg: hidden units
+//     64wg..64wg+63), so every thread holds two hidden units x 32 rows in registers;
+//   * relu(hidden)^T goes to shared memory once (K-major [hidden unit][row]); the head products, the loss row math (four
+//     lanes per row), g^T = W_heads^T dOut^T, dPre^T = g^T masked by the ReLU, db_enc and dW_heads^T = relu(h)^T dOut all
+//     work on the registers of that accumulator layout;
+//   * dW_enc^T [feature][hidden unit] += x^T . dPre on the tensor core (wgmma RS: x^T fragments read from the x tile, dPre^T
+//     from shared memory as the K-major B operand); the accumulator stays in registers across all tiles of the CTA.
+// Per-CTA partials go to a workspace and k_update_reduce sums them deterministically into the flat gradient buffer
+// [dW_enc (hid x feat) | dW_heads (8 x hid) | db_enc | db_heads] of clean_pufferl._DefaultMLPUpdate, leaving per-block
+// sums of squares for pb_clip_adam_parts.
 //
-// Descriptor encodings were validated on hardware with csrc/experimental/umma_probe.cu (tests/experimental/
-// check_umma_probe.py, check_umma_transpose.py).  Every mbarrier wait is bounded (tma.cuh: __trap instead of a hang).
+// Epilogue precision (pb_mlp_update_set_variant): variant 2 (default) takes the head, g^T and dW_heads products on mma.sync
+// with TF32 operands and fp32 accumulation -- the precision class of torch.set_float32_matmul_precision('high'), which
+// clean_pufferl sets; variant 1 forms the head and g^T products with fp32 FFMAs.  The dPre-to-HBM mode (dW_enc by the
+// caller) runs the variant-1 epilogue.  Every mbarrier wait is bounded (tma.cuh: __trap instead of a hang).
 #include <cuda.h>
 #include <stdlib.h>
 
 #include "pb_common.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int TILE_M = 128, HID = 128, FEAT = 128, NO = 8;
+constexpr int TILE_M = 64, HID = 128, FEAT = 128, NO = 8;
 constexpr int KBLK = 32;                               // floats per 128-byte swizzle row
-constexpr int KBLK_BYTES = TILE_M * KBLK * 4;          // 16 KiB: one [128 rows][32 floats] box
-constexpr int TILE_BYTES = 4 * KBLK_BYTES;             // 64 KiB
-constexpr int NCHUNK = 4, CHUNK_COLS = 32;
-constexpr int CHUNK_BYTES = TILE_M * CHUNK_COLS * 4;   // 16 KiB: [128 rows][32 hid] MN-major (N contiguous)
-constexpr int SMEM_W = 0;                              // W_enc, K-major SWIZZLE_128B, resident
-constexpr int SMEM_XK = TILE_BYTES;                    // x tile for the forward product: K-major SWIZZLE_128B
-constexpr int SMEM_XM = 2 * TILE_BYTES;                // x tile for the dW product: MN-major SWIZZLE_128B_BASE32B
-constexpr int SMEM_CH = 3 * TILE_BYTES;                // two dPre chunk buffers (one per column half)
-constexpr int SMEM_BAR = SMEM_CH + 2 * CHUNK_BYTES;
-constexpr int SMEM_TOTAL = SMEM_BAR + 256;
-constexpr int THREADS = 320;                           // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-constexpr int TMEM_COLS = 512;
-constexpr int TMEM_DW = 256;                           // first column of the dW^T accumulator
-constexpr int TMEM_XCHG = 384;                         // 16 columns: the partial head sums the two warps of a row exchange
+constexpr int W_KBLK_BYTES = HID * KBLK * 4;           // 16 KiB: [128 hidden units][32 features]
+constexpr int X_KBLK_BYTES = TILE_M * KBLK * 4;        // 8 KiB: [64 rows][32 features]
+constexpr int X_TILE_BYTES = 4 * X_KBLK_BYTES;         // 32 KiB
+constexpr int G_KBLK_BYTES = HID * 32 * 4;             // 16 KiB: [128 hidden units][32 rows]
+constexpr int NSTAGE = 3;                              // x tiles in flight per SM
+constexpr int THREADS = 256;                           // two warpgroups
+constexpr int SM_W = 0;                                // W_enc, K-major SWIZZLE_128B, resident
+constexpr int SM_X = 4 * W_KBLK_BYTES;                 // NSTAGE x tiles, K-major SWIZZLE_128B
+constexpr int SM_G = SM_X + NSTAGE * X_TILE_BYTES;     // relu(h)^T, then dPre^T: two [128 hidden][32 rows] K-major blocks
+constexpr int SM_WH = SM_G + 2 * G_KBLK_BYTES;         // W_heads [8][128]
+constexpr int SM_BE = SM_WH + NO * HID * 4;            // b_enc [128]
+constexpr int SM_OUT = SM_BE + HID * 4;                // head outputs [2 hidden halves][64 rows][8]
+constexpr int SM_DO = SM_OUT + 2 * TILE_M * NO * 4;    // dOut [64 rows][8]
+constexpr int SM_RED = SM_DO + TILE_M * NO * 4;        // db_heads partials [8 warps][8]
+constexpr int SM_BAR = SM_RED + 8 * NO * 4;
+constexpr int SMEM_TOTAL = SM_BAR + 64;
 constexpr int TAIL = NO * HID + HID + NO;              // dW_heads | db_enc | db_heads
-static_assert(SMEM_TOTAL <= 232448, "shared memory budget");
-
-// W_heads [8][128], b_enc [128], b_heads [8]: uniform per warp at every use -> constant-bank operands of the FFMAs
-__constant__ float c_wh[NO * HID];
-__constant__ float c_benc[HID];
-__constant__ float c_bh[NO];
+static_assert(SMEM_TOTAL <= 227 * 1024, "shared memory budget (227 KiB per block on sm_90)");
 
 struct FusedParams {
     const int64_t* actions;
@@ -79,10 +79,9 @@ struct FusedParams {
     float* dbg_hidden;         // nullable [m][128]
     float* dbg_dpre;           // nullable [m][128]
     float* dbg_dout;           // nullable [m][8]
-    const float* w_heads;      // [8][128], b_enc [128], b_heads [8] in global memory (variant 2 reads them directly)
+    const float* w_heads;      // [8][128], b_enc [128], b_heads [8]
     const float* b_enc;
     const float* b_heads;
-    long long* dbg_clk;        // profiling only: [grid][18 warps][4 tiles][8 events] SM clock stamps of tiles 8..11 (variant 2)
 };
 
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
@@ -92,564 +91,37 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
         "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
         : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// SWIZZLE_128B descriptors (PTX ISA tcgen05 shared-memory descriptor; cute/arch/mma_sm100_desc.hpp): start>>4 | LBO>>4 <<16
-// | SBO>>4 <<32 | version 1 <<46 | layout 2 <<61.  K-major: LBO unused (1), SBO = 1024 B between 8-row groups.
-// MN-major: LBO = distance between 32-element MN groups, SBO = 1024 B between 8-k groups.
-__device__ __forceinline__ uint64_t desc_kmajor(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// MN-major 32-bit operands: layout type 1 (SWIZZLE_128B_BASE32B), atoms of 4 k x 128 B, SBO = 512 B between 4-k groups,
-// LBO = distance between 32-element MN groups
-__device__ __forceinline__ uint64_t desc_mn32(uint32_t saddr, uint32_t lbo_bytes) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | (32ull << 32) | (1ull << 46) | (1ull << 61);
-}
-// instruction descriptor: D fmt F32 (1<<4) | A TF32 (2<<7) | B TF32 (2<<10) | A major bit 15 | B major bit 16 | N>>3 <<17 | M>>4 <<24
-constexpr uint32_t IDESC_FWD = (1u << 4) | (2u << 7) | (2u << 10) | ((HID >> 3) << 17) | ((TILE_M >> 4) << 24);
-constexpr uint32_t IDESC_DW = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((CHUNK_COLS >> 3) << 17) |
-                              ((FEAT >> 4) << 24);
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
-    asm volatile(   // A operand from tensor memory: lanes = rows (M), columns = K
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(b_desc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-                 "r"(__float_as_uint(r[0])), "r"(__float_as_uint(r[1])), "r"(__float_as_uint(r[2])), "r"(__float_as_uint(r[3])),
-                 "r"(__float_as_uint(r[4])), "r"(__float_as_uint(r[5])), "r"(__float_as_uint(r[6])), "r"(__float_as_uint(r[7]))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&r)[8]) {
-    uint32_t u[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7])
-                 : "r"(taddr)
-                 : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) r[i] = __uint_as_float(u[i]);
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&r)[32]) {
-    uint32_t u[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]), "=r"(u[8]),
-          "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]), "=r"(u[16]),
-          "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]), "=r"(u[24]),
-          "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) r[i] = __uint_as_float(u[i]);
-}
 
 __device__ __forceinline__ uint32_t to_tf32(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
     return r;
 }
-__device__ __forceinline__ void mma_tf32(float& c0, float& c1, float& z0, float& z1, const uint32_t (&a)[2], uint32_t b0,
-                                         uint32_t b1) {
-    // m16n8k8: rows 8..15 of A are zero (a1 = a3 = 0), their accumulators (z0, z1) are shared dummies
+
+// mma.sync m16n8k8 TF32: a0 (g, t)  a1 (g + 8, t)  a2 (g, t + 4)  a3 (g + 8, t + 4);  b0 (k = t, n = g)  b1 (k = t + 4, n = g);
+// c0 c1 (g, 2t + {0,1})  c2 c3 (g + 8, 2t + {0,1})      [g = lane >> 2, t = lane & 3]
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c0), "+f"(c1), "+f"(z0), "+f"(z1)
-                 : "r"(a[0]), "r"(0u), "r"(a[1]), "r"(0u), "r"(b0), "r"(b1));
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// The row math of k_ppo_loss<PACKED> (csrc/ppo_loss.cu; clean_pufferl.py:202-238 + frameworks/cleanrl.py:25-47):
-// z[0..n_act) logits, z[n_act] value -> dOut[8] (already scaled by 1/M) and the six per-row statistics.
+// byte offset of element (hidden unit n, tile row l) in the relu(h)^T / dPre^T buffer: two K-major SWIZZLE_128B blocks of
+// [128 hidden units][32 rows] (rows 0..31, 32..63) -- the layout of a wgmma B operand with N = hidden units, K = rows
+__device__ __forceinline__ uint32_t g_off(int n, int l) {
+    return (uint32_t)((l >> 5) * G_KBLK_BYTES + n * 128 + ((((l & 31) >> 2) ^ (n & 7)) << 4) + (l & 3) * 4);
+}
+// byte offset of element (tile row r, feature f) in an x tile (four K-major SWIZZLE_128B blocks of [64 rows][32 features])
+__device__ __forceinline__ uint32_t x_off(int r, int f) {
+    return (uint32_t)((f >> 5) * X_KBLK_BYTES + r * 128 + ((((f & 31) >> 2) ^ (r & 7)) << 4) + (f & 3) * 4);
+}
+
 struct RowStats { float pg, v, ent, okl, kl, clipped; };
-__device__ __forceinline__ RowStats ppo_row(const float (&zin)[8], const FusedParams& p, int act, float old_lp, float adv,
-                                            float ret, float old_v, float (&gro)[8]) {
-    float z[8];
-    float mx = -INFINITY;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        z[k] = zin[k];
-        if (k < p.n_act) mx = fmaxf(mx, z[k]);
-    }
-    float v_new = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k)
-        if (k == p.n_act) v_new = z[k];
-    float sum = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k)
-        if (k < p.n_act) sum += expf(z[k] - mx);
-    const float lse = mx + logf(sum);
-    const int a = act < 0 ? 0 : (act >= p.n_act ? p.n_act - 1 : act);
-    float ent = 0.f, nl_a = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k)
-        if (k < p.n_act) {
-            const float nl = z[k] - lse, pk = expf(nl);
-            ent -= pk * nl;
-            if (k == a) nl_a = nl;
-            z[k] = nl;
-        }
-    const float logratio = nl_a - old_lp;
-    const float ratio = expf(logratio);
-    const float pg1 = -adv * ratio;
-    const float rc = fminf(fmaxf(ratio, 1.f - p.clip), 1.f + p.clip);
-    const float pg2 = -adv * rc;
-    const float pg = fmaxf(pg1, pg2);
-    const float in_range = (ratio >= 1.f - p.clip && ratio <= 1.f + p.clip) ? 1.f : 0.f;
-    float g_ratio;
-    if (pg1 > pg2) g_ratio = -adv;
-    else if (pg1 < pg2) g_ratio = -adv * in_range;
-    else g_ratio = 0.5f * (-adv) + 0.5f * (-adv * in_range);
-    const float inv_m = 1.0f / (float)p.m;
-    const float g_nlp = g_ratio * ratio * inv_m;
-    const float dv = v_new - ret;
-    float vl, g_v;
-    if (p.clip_vloss) {
-        const float d = v_new - old_v;
-        const float dc = fminf(fmaxf(d, -p.vclip), p.vclip);
-        const float vc = old_v + dc;
-        const float vu = dv * dv, vcl = (vc - ret) * (vc - ret);
-        vl = fmaxf(vu, vcl);
-        const float v_in = (d >= -p.vclip && d <= p.vclip) ? 1.f : 0.f;
-        const float gu = 2.f * dv, gc = 2.f * (vc - ret) * v_in;
-        g_v = vu > vcl ? gu : (vu < vcl ? gc : 0.5f * (gu + gc));
-    } else {
-        vl = dv * dv;
-        g_v = 2.f * dv;
-    }
-    const float gv_out = 0.5f * p.vf_coef * g_v * inv_m;
-    const float g_ent = p.ent_coef * inv_m;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        gro[k] = 0.f;
-        if (k < p.n_act) {
-            const float pk = expf(z[k]);
-            gro[k] = g_nlp * ((k == a ? 1.f : 0.f) - pk) + g_ent * pk * (z[k] + ent);
-        }
-        if (k == p.n_act) gro[k] = gv_out;
-    }
-    RowStats s;
-    s.pg = pg; s.v = vl; s.ent = ent; s.okl = -logratio; s.kl = (ratio - 1.f) - logratio;
-    s.clipped = fabsf(ratio - 1.f) > p.clip ? 1.f : 0.f;
-    return s;
-}
 
-// NH = live rows of the 8-row head matrix (n_act logits + the value): rows >= NH are zero padding, their products are skipped
-// byte offset of element (row r, column j) of a [128 rows][32 floats] chunk in the SWIZZLE_128B_BASE32B layout (32-byte
-// pieces of a 128-byte row, piece index ^= row & 3): the layout the tensor core requires for MN-major 32-bit operands
-// (UMMA layout type 1; TMA writes it with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B).  Conflict-free for the fragment loads of
-// the dW_heads mma.sync and for the column sums; 2-way for the row-owner 128-bit stores.
-__device__ __forceinline__ uint32_t chunk32_off(int r, int j) {
-    return (uint32_t)(r * 128 + ((((j >> 3) ^ (r & 3))) << 5) + ((j & 7) << 2));
-}
-
-// DW_KERNEL = true : dW_enc^T accumulated in TMEM by MN-major UMMAs (x tile loaded a second time in the BASE32B layout)
-// DW_KERNEL = false: dPre goes to HBM (p.dpre_out) and the caller forms dW_enc = dPre^T x with a library GEMM
-template <int NH, bool DW_KERNEL>
-__global__ void __launch_bounds__(THREADS, 1)
-k_mlp_update_fused(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_x32,
-                   const __grid_constant__ CUtensorMap map_w, const FusedParams p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SMEM_BAR);
-    uint64_t* w_full = bars;              // W_enc resident
-    uint64_t* xk_full = bars + 1;         // forward operand tile (K-major SW128) landed
-    uint64_t* xk_empty = bars + 2;        // ... consumed by the forward MMAs
-    uint64_t* xm_full = bars + 3;         // dW operand tile (MN-major BASE32B) landed
-    uint64_t* xm_empty = bars + 4;        // ... consumed by the dW MMAs of the tile
-    uint64_t* h_full = bars + 5;          // [2] forward accumulator complete
-    uint64_t* h_empty = bars + 7;         // [2] drained by the 8 epilogue warps
-    uint64_t* dp_full = bars + 9;         // [2] dPre chunk of column half hh written (4 warps)
-    uint64_t* dp_empty = bars + 11;       // [2] ... consumed by its dW MMAs
-    uint64_t* dw_done = bars + 13;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (threadIdx.x == 0) {
-        mbar_init(w_full, 1);
-        mbar_init(xk_full, 1);
-        mbar_init(xk_empty, 1);
-        mbar_init(xm_full, 1);
-        mbar_init(xm_empty, 1);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&h_full[i], 1);
-            mbar_init(&h_empty[i], 8);
-            mbar_init(&dp_full[i], 4);
-            mbar_init(&dp_empty[i], 1);
-        }
-        mbar_init(dw_done, 1);
-        mbar_fence_init();
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"((uint32_t)TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const int n_my = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // tiles of this CTA (>= 1)
-
-    // per-thread results of the epilogue warps, reduced after the role loops.  Epilogue warp (q, hh): TMEM lane quadrant q
-    // (tile rows 32q..32q+31), column half hh = hidden units 64hh..64hh+63 = chunks 2hh, 2hh+1.
-    float acc_wh[2][4][2];               // dW_heads[a = lane>>2][j = 32(2hh+cc) + 8nb + 2(lane&3) + {0,1}]  (this warp's rows)
-    float acc_benc[2];                   // db_enc[32(2hh+cc) + lane]
-    float acc_bh[NO];                    // db_heads (this thread's rows; hh == 0 only)
-    double st[6] = {0, 0, 0, 0, 0, 0};
-#pragma unroll
-    for (int cc = 0; cc < 2; ++cc) {
-        acc_benc[cc] = 0.f;
-#pragma unroll
-        for (int nb = 0; nb < 4; ++nb) acc_wh[cc][nb][0] = acc_wh[cc][nb][1] = 0.f;
-    }
-#pragma unroll
-    for (int k = 0; k < NO; ++k) acc_bh[k] = 0.f;
-
-    if (warp == 0) {
-        // ================= TMA producer =================
-        if (lane == 0) {
-            mbar_expect_tx(w_full, TILE_BYTES);
-            for (int kb = 0; kb < 4; ++kb) tma_load_2d(smem + SMEM_W + kb * KBLK_BYTES, &map_w, kb * KBLK, 0, w_full);
-            for (int it = 0; it < n_my; ++it) {
-                const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-                const int64_t row0 = (int64_t)(tile / p.tiles_per_slab) * p.slab_stride_rows +
-                                     (int64_t)(tile % p.tiles_per_slab) * TILE_M;
-                mbar_wait(xk_empty, (uint32_t)((it & 1) ^ 1));          // forward MMAs of tile it-1 have read the buffer
-                mbar_expect_tx(xk_full, TILE_BYTES);
-                for (int kb = 0; kb < 4; ++kb) tma_load_2d(smem + SMEM_XK + kb * KBLK_BYTES, &map_x, kb * KBLK, (int)row0, xk_full);
-                if (DW_KERNEL) {   // the same rows again (L2 hits) in the MN-major layout of the dW product
-                    mbar_wait(xm_empty, (uint32_t)((it & 1) ^ 1));      // dW MMAs of tile it-1 done
-                    mbar_expect_tx(xm_full, TILE_BYTES);
-                    for (int kb = 0; kb < 4; ++kb)
-                        tma_load_2d(smem + SMEM_XM + kb * KBLK_BYTES, &map_x32, kb * KBLK, (int)row0, xm_full);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ================= MMA issuer (one thread) =================
-        if (lane == 0) {
-            const uint32_t w_addr = smem_u32(smem + SMEM_W);
-            const uint32_t xk_addr = smem_u32(smem + SMEM_XK), xm_addr = smem_u32(smem + SMEM_XM);
-            auto forward = [&](int it) {
-                const int s = it & 1, ph = (it >> 1) & 1;
-                mbar_wait(&h_empty[s], ph ^ 1);                  // epilogue drained accumulator stage s (tile it - 2)
-                mbar_wait(xk_full, (uint32_t)(it & 1));          // x tile landed
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(s * HID);
-#pragma unroll
-                for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        umma_tf32(d_tmem, desc_kmajor(xk_addr + kb * KBLK_BYTES + k * 32),
-                                  desc_kmajor(w_addr + kb * KBLK_BYTES + k * 32), IDESC_FWD, (kb | k) ? 1u : 0u);
-                umma_commit(&h_full[s]);
-                umma_commit(xk_empty);                           // the K-major tile may be overwritten: next tile's load starts
-            };
-            mbar_wait(w_full, 0);
-            forward(0);
-            for (int it = 0; it < n_my; ++it) {
-                if (it + 1 < n_my) forward(it + 1);              // overlaps the epilogue of tile `it`
-                if (DW_KERNEL) {
-                    mbar_wait(xm_full, (uint32_t)(it & 1));
-                    // chunks arrive alternately from the two column halves: 0 (hh 0), 2 (hh 1), 1 (hh 0), 3 (hh 1)
-#pragma unroll 1
-                    for (int i = 0; i < NCHUNK; ++i) {
-                        const int hh = i & 1, cc = i >> 1, c = 2 * hh + cc;
-                        const int u = it * 2 + cc;               // use count of chunk buffer hh
-                        mbar_wait(&dp_full[hh], (uint32_t)(u & 1));
-                        tc_fence_after();
-                        const uint32_t ch_addr = smem_u32(smem + SMEM_CH + hh * CHUNK_BYTES);
-                        const uint32_t d_tmem = tmem_base + (uint32_t)(TMEM_DW + c * CHUNK_COLS);
-#pragma unroll
-                        for (int k = 0; k < TILE_M / 8; ++k)      // K = 8 rows per MMA = two 512-byte atoms
-                            umma_tf32(d_tmem, desc_mn32(xm_addr + k * 1024, KBLK_BYTES), desc_mn32(ch_addr + k * 1024, KBLK_BYTES),
-                                      IDESC_DW, (it | k) ? 1u : 0u);
-                        umma_commit(&dp_empty[hh]);
-                    }
-                    umma_commit(xm_empty);
-                }
-            }
-            umma_commit(dw_done);
-        }
-    } else {
-        // ================= epilogue warps: thread = tile row (TMEM lane 32q + lane), column half hh =================
-        const int q = warp & 3, hh = (warp - 2) >> 2;
-        const int g = lane >> 2, t = lane & 3;
-        const int rloc = 32 * q + lane;                        // row inside the tile
-        uint8_t* buf = smem + SMEM_CH + hh * CHUNK_BYTES;      // this half's chunk buffer; this warp owns rows 32q..32q+31
-        const uint32_t xchg = tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)TMEM_XCHG;
-        float z0 = 0.f, z1 = 0.f;                              // dummy accumulators of the zero A rows
-        for (int it = 0; it < n_my; ++it) {
-            const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-            const int s = it & 1, ph = (it >> 1) & 1;
-            const int slab = tile / p.tiles_per_slab;
-            const int64_t lrow = (int64_t)(tile % p.tiles_per_slab) * TILE_M + rloc;
-            const bool valid = lrow < p.slab_rows;
-            const int64_t i = (int64_t)slab * p.slab_rows + lrow;            // slab-major position (dPre / debug rows)
-            const int64_t ri = (int64_t)slab * p.row_slab_stride + lrow;     // position in the per-row arrays
-            int act = 0;
-            float old_lp = 0.f, adv = 0.f, ret = 0.f, old_v = 0.f;
-            if (valid) {
-                act = (int)p.actions[ri];
-                old_lp = p.old_logprobs[ri];
-                adv = p.adv[ri];
-                old_v = (p.clip_vloss || !p.returns) ? p.old_values[ri] : 0.f;
-                ret = p.returns ? p.returns[ri] : adv + old_v;
-                if (p.adv_norm) adv = (adv - p.adv_norm[0]) * p.adv_norm[1];
-            }
-            mbar_wait(&h_full[s], ph);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(s * HID);
-
-            // ---- pass 1: this half's share of the head products, exchanged with the partner warp through tensor memory
-            float out[NO];
-#pragma unroll
-            for (int a = 0; a < NO; ++a) out[a] = 0.f;
-#pragma unroll
-            for (int cc = 0; cc < 2; ++cc) {
-                float v[32];
-                if (hh == 0) {      // (compile-time column offsets: every c_wh / c_benc operand is a constant-bank immediate)
-                    tmem_ld32(taddr + 32 * cc, v);
-#pragma unroll
-                    for (int k = 0; k < 32; ++k) {
-                        const float rh = fmaxf(v[k] + c_benc[32 * cc + k], 0.f);
-#pragma unroll
-                        for (int a = 0; a < NH; ++a) out[a] = fmaf(rh, c_wh[a * HID + 32 * cc + k], out[a]);
-                    }
-                } else {
-                    tmem_ld32(taddr + 64 + 32 * cc, v);
-#pragma unroll
-                    for (int k = 0; k < 32; ++k) {
-                        const float rh = fmaxf(v[k] + c_benc[64 + 32 * cc + k], 0.f);
-#pragma unroll
-                        for (int a = 0; a < NH; ++a) out[a] = fmaf(rh, c_wh[a * HID + 64 + 32 * cc + k], out[a]);
-                    }
-                }
-            }
-            {
-            tmem_st8(xchg + 8 * hh, out);
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            tc_fence_before();
-            asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");     // the two warps of quadrant q
-            tc_fence_after();
-            }
-            {
-                float other[NO];
-                tmem_ld8(xchg + 8 * (hh ^ 1), other);
-#pragma unroll
-                for (int a = 0; a < NO; ++a) out[a] = (hh == 0 ? out[a] + other[a] : other[a] + out[a]) + c_bh[a];   // same order in both
-            }
-            // the partner must have read my partial before the next tile overwrites it: second rendezvous at the end of the tile
-
-            // ---- loss row math -> dOut (both warps of the pair compute it; the statistics are taken by hh == 0)
-            float dO[NO];
-#pragma unroll
-            for (int a = 0; a < NO; ++a) dO[a] = 0.f;
-            if (valid) {
-                const RowStats rs = ppo_row(out, p, act, old_lp, adv, ret, old_v, dO);
-                if (hh == 0) {
-                    st[0] += rs.pg; st[1] += rs.v; st[2] += rs.ent; st[3] += rs.okl; st[4] += rs.kl; st[5] += rs.clipped;
-                    if (p.dbg_dout) {
-                        *reinterpret_cast<float4*>(p.dbg_dout + i * 8) = make_float4(dO[0], dO[1], dO[2], dO[3]);
-                        *reinterpret_cast<float4*>(p.dbg_dout + i * 8 + 4) = make_float4(dO[4], dO[5], dO[6], dO[7]);
-                    }
-                }
-            }
-            if (hh == 0) {
-#pragma unroll
-                for (int a = 0; a < NO; ++a) acc_bh[a] += dO[a];
-            }
-
-            // ---- A fragments of the dW_heads mma (A[m = head a][k = row]) staged through this warp's rows of its half's
-            //      chunk buffer (32 B per row; private to the warp until a dPre chunk is published)
-            uint32_t afr[4][2];
-            {
-                if (DW_KERNEL) mbar_wait(&dp_empty[hh], (uint32_t)(((it * 2) & 1) ^ 1));
-                *reinterpret_cast<float4*>(buf + rloc * 128) = make_float4(dO[0], dO[1], dO[2], dO[3]);
-                *reinterpret_cast<float4*>(buf + rloc * 128 + 16) = make_float4(dO[4], dO[5], dO[6], dO[7]);
-                __syncwarp();
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {
-                    afr[ks][0] = to_tf32(*reinterpret_cast<const float*>(buf + (32 * q + 8 * ks + t) * 128 + g * 4));
-                    afr[ks][1] = to_tf32(*reinterpret_cast<const float*>(buf + (32 * q + 8 * ks + t + 4) * 128 + g * 4));
-                }
-                __syncwarp();
-            }
-
-            // ---- pass 2: this half's two 32-column chunks: dPre, dW_heads, db_enc
-#pragma unroll
-            for (int cc = 0; cc < 2; ++cc) {
-                float v[32], dp[32];
-                const int col0 = 64 * hh + 32 * cc;           // first hidden unit of the chunk (hh is warp-uniform)
-                tmem_ld32(taddr + col0, v);
-                if (hh == 0) {
-#pragma unroll
-                    for (int k = 0; k < 32; ++k) {
-                        const float pre = v[k] + c_benc[32 * cc + k];
-                        float gk = 0.f;
-#pragma unroll
-                        for (int a = 0; a < NH; ++a) gk = fmaf(dO[a], c_wh[a * HID + 32 * cc + k], gk);
-                        dp[k] = pre > 0.f ? gk : 0.f;
-                        v[k] = fmaxf(pre, 0.f);
-                    }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 32; ++k) {
-                        const float pre = v[k] + c_benc[64 + 32 * cc + k];
-                        float gk = 0.f;
-#pragma unroll
-                        for (int a = 0; a < NH; ++a) gk = fmaf(dO[a], c_wh[a * HID + 64 + 32 * cc + k], gk);
-                        dp[k] = pre > 0.f ? gk : 0.f;
-                        v[k] = fmaxf(pre, 0.f);
-                    }
-                }
-                if (valid && p.dbg_hidden) {
-#pragma unroll
-                    for (int k = 0; k < 32; k += 4) {
-                        *reinterpret_cast<float4*>(p.dbg_hidden + i * HID + col0 + k) = make_float4(v[k], v[k + 1], v[k + 2], v[k + 3]);
-                        *reinterpret_cast<float4*>(p.dbg_dpre + i * HID + col0 + k) = make_float4(dp[k], dp[k + 1], dp[k + 2], dp[k + 3]);
-                    }
-                }
-                if (!DW_KERNEL && valid) {    // dPre row segment to HBM (128 contiguous bytes per thread)
-#pragma unroll
-                    for (int k = 0; k < 32; k += 4)
-                        __stcs(reinterpret_cast<float4*>(p.dpre_out + i * HID + col0 + k), make_float4(dp[k], dp[k + 1], dp[k + 2], dp[k + 3]));
-                }
-                if (DW_KERNEL) mbar_wait(&dp_empty[hh], (uint32_t)(((it * 2 + cc) & 1) ^ 1));   // last use of the buffer consumed
-                // relu(h) chunk of this warp's 32 rows (TF32-rounded) -> B fragments of the dW_heads mma
-                {
-#pragma unroll
-                for (int j8 = 0; j8 < 4; ++j8) {
-                    uint8_t* dst = buf + rloc * 128 + ((j8 ^ (rloc & 3)) << 5);
-                    *reinterpret_cast<uint4*>(dst) = make_uint4(to_tf32(v[8 * j8]), to_tf32(v[8 * j8 + 1]), to_tf32(v[8 * j8 + 2]), to_tf32(v[8 * j8 + 3]));
-                    *reinterpret_cast<uint4*>(dst + 16) = make_uint4(to_tf32(v[8 * j8 + 4]), to_tf32(v[8 * j8 + 5]), to_tf32(v[8 * j8 + 6]), to_tf32(v[8 * j8 + 7]));
-                }
-                __syncwarp();
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {
-                    const int r0 = 32 * q + 8 * ks + t;
-#pragma unroll
-                    for (int nb = 0; nb < 4; ++nb) {
-                        const uint32_t b0 = *reinterpret_cast<const uint32_t*>(buf + chunk32_off(r0, 8 * nb + g));
-                        const uint32_t b1 = *reinterpret_cast<const uint32_t*>(buf + chunk32_off(r0 + 4, 8 * nb + g));
-                        mma_tf32(acc_wh[cc][nb][0], acc_wh[cc][nb][1], z0, z1, afr[ks], b0, b1);
-                    }
-                }
-                __syncwarp();
-                }
-                // dPre chunk -> the same rows, BASE32B layout (the MN-major B operand of the dW UMMA)
-#pragma unroll
-                for (int j8 = 0; j8 < 4; ++j8) {
-                    uint8_t* dst = buf + rloc * 128 + ((j8 ^ (rloc & 3)) << 5);
-                    *reinterpret_cast<float4*>(dst) = make_float4(dp[8 * j8], dp[8 * j8 + 1], dp[8 * j8 + 2], dp[8 * j8 + 3]);
-                    *reinterpret_cast<float4*>(dst + 16) = make_float4(dp[8 * j8 + 4], dp[8 * j8 + 5], dp[8 * j8 + 6], dp[8 * j8 + 7]);
-                }
-                if (DW_KERNEL) fence_proxy_async_smem();
-                __syncwarp();
-                if (DW_KERNEL && lane == 0) mbar_arrive(&dp_full[hh]);
-                // db_enc: column sums over this warp's rows (the UMMA only reads the buffer)
-                float cs = 0.f;
-#pragma unroll 8
-                for (int r = 0; r < 32; ++r) cs += *reinterpret_cast<const float*>(buf + chunk32_off(32 * q + r, lane));
-                acc_benc[cc] += cs;
-                __syncwarp();                                    // (mode without UMMA: the next chunk overwrites the rows)
-            }
-            tc_fence_before();
-            asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");     // both warps are done with the exchange columns
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&h_empty[s]);
-        }
-        // ---- the dW^T accumulator of this CTA: TMEM lane = feature, column = hidden unit; this warp dumps its column half
-        if (DW_KERNEL) {
-            mbar_wait(dw_done, 0);
-            tc_fence_after();
-            float* pd = p.part_dw + ((int64_t)blockIdx.x * FEAT + rloc) * HID;
-#pragma unroll 1
-            for (int cc = 0; cc < 2; ++cc) {
-                float v[32];
-                const int col0 = 64 * hh + 32 * cc;
-                tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(TMEM_DW + col0), v);
-#pragma unroll
-                for (int k = 0; k < 32; k += 4)
-                    *reinterpret_cast<float4*>(pd + col0 + k) = make_float4(v[k], v[k + 1], v[k + 2], v[k + 3]);
-            }
-        }
-        if (hh == 0) {   // loss statistics: warp reduce, one fp64 atomic per warp and statistic
-#pragma unroll
-            for (int k = 0; k < 6; ++k) {
-                double x = st[k];
-#pragma unroll
-                for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
-                if (lane == 0) atomicAdd(p.stats + k, x);
-            }
-        }
-    }
-
-    // ================= CTA reduction of the small gradients (8 epilogue warps -> one partial row) =================
-    tc_fence_before();
-    __syncthreads();                       // every role is done: all MMAs retired, all TMA loads consumed
-    float* red = reinterpret_cast<float*>(smem + SMEM_XK);         // [4 quadrants][TAIL] scratch in the (now idle) x tile
-    if (warp >= 2) {
-        const int q = warp & 3, hh = (warp - 2) >> 2, g = lane >> 2, t = lane & 3;
-        float* mine = red + q * TAIL;      // the two warps of a quadrant fill disjoint columns of the same row
-#pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-            const int col0 = 64 * hh + 32 * cc;
-#pragma unroll
-            for (int nb = 0; nb < 4; ++nb) {
-                mine[g * HID + col0 + 8 * nb + 2 * t] = acc_wh[cc][nb][0];
-                mine[g * HID + col0 + 8 * nb + 2 * t + 1] = acc_wh[cc][nb][1];
-            }
-            mine[NO * HID + col0 + lane] = acc_benc[cc];
-        }
-        if (hh == 0) {
-#pragma unroll
-            for (int k = 0; k < NO; ++k) {
-                float x = acc_bh[k];
-#pragma unroll
-                for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
-                if (lane == 0) mine[NO * HID + HID + k] = x;
-            }
-        }
-    }
-    __syncthreads();
-    float* pt = p.part_tail + (int64_t)blockIdx.x * TAIL;
-    for (int j = threadIdx.x; j < TAIL; j += THREADS) pt[j] = red[j] + red[TAIL + j] + red[2 * TAIL + j] + red[3 * TAIL + j];
-    if (warp == 1)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS)
-                     : "memory");
-}
-
-// ppo_row with FOUR lanes per row: lane `sub` (0..3) of the row owns outputs sub and sub + 4 (logits below n_act, the value at
-// index n_act); row-wide maxima / sums go through width-4 shuffles.  Same arithmetic as ppo_row, which remains the
-// statement of the math; every lane of the warp must call it (shuffles).  Returns dOut of the two owned outputs.
+// The row math of k_ppo_loss<PACKED> (csrc/ppo_loss.cu; clean_pufferl.py:202-238 + frameworks/cleanrl.py:25-47) with FOUR
+// lanes per row: lane `sub` (0..3) of the row owns outputs sub and sub + 4 (logits below n_act, the value at index n_act);
+// row-wide maxima / sums go through width-4 shuffles.  Every lane of the warp must call it (shuffles).  Returns dOut of the
+// two owned outputs (already scaled by 1/M) and the six per-row statistics.
 __device__ __forceinline__ RowStats ppo_row_sub(float z_lo, float z_hi, int sub, int lane, const FusedParams& p, int act,
                                                 float old_lp, float adv, float ret, float old_v, float& g_lo, float& g_hi) {
     const unsigned full = 0xffffffffu;
@@ -711,472 +183,355 @@ __device__ __forceinline__ RowStats ppo_row_sub(float z_lo, float z_hi, int sub,
     return s;
 }
 
-// ---------------------------------------------------------------------------------------------------------------------
-// Variant 2: ONE x layout.  The tensor core only takes MN-major 32-bit operands in the BASE32B layout, so variant 1 loads
-// every x tile twice (K-major for the forward product, MN-major for dW) and has no shared memory left to overlap anything.
-// Here the dW product takes x^T from TENSOR memory instead:
-//     x^T[feat][row]    = I . x^T           SS MMA: A = an 8 KB "sliding identity" (no-swizzle K-major, see x2_write_identity),
-//                                           B = the K-major x tile the forward product just read
-//     dW^T[feat][hid]  += x^T . dPre        TS MMA: A = that accumulator (lanes = feat, columns = rows), B = dPre written by the
-//                                           epilogue as K-major SWIZZLE_128B blocks [128 hid][32 rows] (one per row quadrant)
-// (validated on hardware by tests/experimental/check_umma_transpose.py).  The 64 KB the second x tile used to take hold a
-// whole tile of dPre, so the epilogue never waits for the tensor core inside a tile, and there are 16 epilogue warps
-// (4 per scheduler: row quadrant q x column quarter c) instead of 8.
-// TMEM: [0,256) two forward accumulators, [256,384) x^T, [384,512) dW^T (lives across all tiles of the CTA).
-constexpr int X2_THREADS = 576;                          // warp 0 TMA, warp 1 MMA, warps 2..17 epilogue
-constexpr int X2_W = 0, X2_XK = TILE_BYTES, X2_G = 2 * TILE_BYTES;     // W_enc | x tile | 4 dPre blocks of 16 KiB
-constexpr int X2_XCH = 3 * TILE_BYTES;                   // [4 q][4 c][32 rows][10]: partial head sums (8 used; 10 = bank spread)
-constexpr int X2_XCH_ROW = 10, X2_XCH_Q = 4 * 32 * X2_XCH_ROW;
-constexpr int X2_ID = X2_XCH + 4 * X2_XCH_Q * 4;         // sliding identity: 2 strips of 32 core matrices
-constexpr int X2_DO = X2_ID + 8192;                      // [4 q][32 rows][9]: dOut of the tile (8 used)
-constexpr int X2_DO_ROW = 9, X2_DO_Q = 320;
-constexpr int X2_BE = X2_DO + 4 * X2_DO_Q * 4;           // b_enc [128]
-constexpr int X2_BAR = X2_BE + 512;
-constexpr int X2_TOTAL = X2_BAR + 256;
-constexpr int X2_TMEM_XT = 256, X2_TMEM_DW = 384;
-constexpr int X2_ID_GROUP = 128, X2_ID_STRIP = 32 * X2_ID_GROUP;
-static_assert(X2_TOTAL <= 232448, "shared memory budget");
-
-// no-swizzle K-major descriptor: 8-row x 16-byte core matrices, LBO = distance between the two core matrices of a K = 8
-// slice, SBO = distance between 8-row groups
-__device__ __forceinline__ uint64_t desc_nosw(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-           (1ull << 46);
-}
-
-// Layout of a dPre block (K-major SWIZZLE_128B, [128 hidden units][32 rows of the quadrant]): element (hidden unit n, row l)
-// sits at byte  n * 128 + (((l >> 2) ^ (n & 7)) << 4) + ((l & 3) << 2)  -- hidden unit n = MN row of 128 B, the quadrant's rows
-// along K in 16-byte pieces XORed with n & 7.  The epilogue's addresses (st_row, ha_base, wb_base) are instances of it.
-
-// mma.sync m16n8k8 TF32 with all four A registers: a0 (g, t)  a1 (g + 8, t)  a2 (g, t + 4)  a3 (g + 8, t + 4);
-// b0 (k = t, n = g)  b1 (k = t + 4, n = g);  c0 c1 (g, 2t + {0,1})  c2 c3 (g + 8, 2t + {0,1})      [g = lane >> 2, t = lane & 3]
-__device__ __forceinline__ void mma_tf32_full(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-template <int REGS, bool CLK>
-__global__ void __maxnreg__(REGS)
-k_mlp_update_xt(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const FusedParams p) {
+// TF32_EPI  : head / g^T / dW_heads products on mma.sync with TF32 operands (variant 2); else fp32 FFMAs for the head and
+//             g^T products and TF32 (round-to-nearest operands) for dW_heads (variant 1)
+// DW_KERNEL : dW_enc^T accumulated on the tensor core; else dPre goes to HBM (p.dpre_out) and the caller forms dW_enc
+template <bool TF32_EPI, bool DW_KERNEL>
+__global__ void __launch_bounds__(THREADS, 1)
+k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const FusedParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + X2_BAR);
-    uint64_t* w_full = bars;
-    uint64_t* xk_full = bars + 1;         // x tile landed
-    uint64_t* xk_empty = bars + 2;        // ... read by the forward AND the transposing MMAs
-    uint64_t* h_full = bars + 3;          // [2] forward accumulator complete
-    uint64_t* h_empty = bars + 5;         // [2] read by the 16 epilogue warps
-    uint64_t* dp_full = bars + 7;         // [4] dPre block of row quadrant q written (4 warps)
-    uint64_t* dp_empty = bars + 11;       // [4] ... consumed by its dW MMAs
-    uint64_t* dw_done = bars + 15;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + SM_BAR);
+    uint64_t* x_full = w_full + 1;                                 // [NSTAGE]
+    float* wh = reinterpret_cast<float*>(smem + SM_WH);
+    const float* be = reinterpret_cast<const float*>(smem + SM_BE);
+    float* outp = reinterpret_cast<float*>(smem + SM_OUT);
+    float* dos = reinterpret_cast<float*>(smem + SM_DO);
+    float* red = reinterpret_cast<float*>(smem + SM_RED);
+    uint8_t* gbuf = smem + SM_G;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+    const int wg = warp >> 2, wq = warp & 3;
+    const int n_my = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // tiles of this CTA (>= 1)
 
-    if (threadIdx.x == 0) {
+    auto issue = [&](int it) {           // thread 0: x tile `it` of this CTA into stage it % NSTAGE
+        const int tile = (int)blockIdx.x + it * (int)gridDim.x;
+        const int64_t row0 = (int64_t)(tile / p.tiles_per_slab) * p.slab_stride_rows + (int64_t)(tile % p.tiles_per_slab) * TILE_M;
+        const int s = it % NSTAGE;
+        mbar_expect_tx(&x_full[s], X_TILE_BYTES);
+        for (int kb = 0; kb < 4; ++kb)
+            tma_load_2d(smem + SM_X + s * X_TILE_BYTES + kb * X_KBLK_BYTES, &map_x, kb * KBLK, (int)row0, &x_full[s]);
+    };
+    if (tid == 0) {
         mbar_init(w_full, 1);
-        mbar_init(xk_full, 1);
-        mbar_init(xk_empty, 1);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&h_full[i], 1);
-            mbar_init(&h_empty[i], 16);
-        }
-        for (int i = 0; i < 4; ++i) {
-            mbar_init(&dp_full[i], 4);
-            mbar_init(&dp_empty[i], 1);
-        }
-        mbar_init(dw_done, 1);
+        for (int s = 0; s < NSTAGE; ++s) mbar_init(&x_full[s], 1);
         mbar_fence_init();
     }
-    // sliding identity: strip s (features 4s..4s+3 of a K = 8 slice) is 32 core matrices of 8 rows x 16 B, all zero except
-    // number 15, whose row r holds a 1 at column r - 4s.  MMA k reads from (15 - k) core matrices in: row group k of A sees
-    // the identity block, every other row group zeros.
-    for (int i = threadIdx.x; i < 8192 / 16; i += X2_THREADS) reinterpret_cast<uint4*>(smem + X2_ID)[i] = make_uint4(0, 0, 0, 0);
-    if (threadIdx.x < HID) reinterpret_cast<float*>(smem + X2_BE)[threadIdx.x] = p.b_enc[threadIdx.x];
+    for (int i = tid; i < NO * HID; i += THREADS) wh[i] = p.w_heads[i];
+    if (tid < HID) reinterpret_cast<float*>(smem + SM_BE)[tid] = p.b_enc[tid];
     __syncthreads();
-    if (threadIdx.x < 8) {
-        const int r = threadIdx.x;
-        *reinterpret_cast<float*>(smem + X2_ID + (r >> 2) * X2_ID_STRIP + 15 * X2_ID_GROUP + r * 16 + (r & 3) * 4) = 1.0f;
+    if (tid == 0) {
+        mbar_expect_tx(w_full, 4 * W_KBLK_BYTES);
+        for (int kb = 0; kb < 4; ++kb) tma_load_2d(smem + SM_W + kb * W_KBLK_BYTES, &map_w, kb * KBLK, 0, w_full);
+        for (int it = 0; it < NSTAGE && it < n_my; ++it) issue(it);
     }
-    fence_proxy_async_smem();
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"((uint32_t)TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const int n_my = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    auto stamp = [&](int it, int ev) {
-        if (CLK && p.dbg_clk && lane == 0 && it >= 8 && it < 12) p.dbg_clk[(((int64_t)blockIdx.x * 18 + warp) * 4 + (it - 8)) * 8 + ev] = clock64();
-    };
 
-    // epilogue warp (q, c): TMEM lane quadrant q (tile rows 32q..32q+31), hidden units 32c..32c+31
-    float acc_wh[2][4];                  // dW_heads[head 2t + (i & 1)][32c + 16mb + 8(i >> 1) + g] (this warp's rows)
-    float st[6] = {0, 0, 0, 0, 0, 0};    // per-thread statistics of <= 28 tiles: fp32 here, fp64 across threads
-    float acc_be[4] = {0.f, 0.f, 0.f, 0.f};   // db_enc[32c + 8nb + (lane >> 2)], this lane's 8 rows of every tile
-    float acc_bh2[2] = {0.f, 0.f};       // db_heads[lane & 3], [(lane & 3) + 4] over this lane's rows
+    // this thread's two hidden units in the hidden^T accumulator (rows of the wgmma D fragment)
+    const int hr0 = 64 * wg + 16 * wq + g, hr1 = hr0 + 8;
+    // the loss: four lanes per tile row (ppo_row_sub)
+    const int lr = tid >> 2, sub = tid & 3;
+    const float bh_lo = p.b_heads[sub], bh_hi = p.b_heads[sub + 4];
+    // W_heads operands, resident in registers
+    uint32_t hb[8][2], ga[4];            // TF32_EPI: heads B fragments (hidden half warp >> 2), g^T A fragment
+    float whr[2][NO];                    // fp32 epilogue: W_heads[a][hr0], W_heads[a][hr1]
+    if (TF32_EPI) {
+        const int hh = warp >> 2;
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb) acc_wh[mb][0] = acc_wh[mb][1] = acc_wh[mb][2] = acc_wh[mb][3] = 0.f;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            mbar_expect_tx(w_full, TILE_BYTES);
-            for (int kb = 0; kb < 4; ++kb) tma_load_2d(smem + X2_W + kb * KBLK_BYTES, &map_w, kb * KBLK, 0, w_full);
-            for (int it = 0; it < n_my; ++it) {
-                const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-                const int64_t row0 = (int64_t)(tile / p.tiles_per_slab) * p.slab_stride_rows +
-                                     (int64_t)(tile % p.tiles_per_slab) * TILE_M;
-                stamp(it, 0);
-                mbar_wait(xk_empty, (uint32_t)((it & 1) ^ 1));
-                stamp(it, 1);
-                mbar_expect_tx(xk_full, TILE_BYTES);
-                for (int kb = 0; kb < 4; ++kb) tma_load_2d(smem + X2_XK + kb * KBLK_BYTES, &map_x, kb * KBLK, (int)row0, xk_full);
-            }
+        for (int ks = 0; ks < 8; ++ks) {
+            hb[ks][0] = to_tf32(wh[g * HID + 64 * hh + 8 * ks + t]);
+            hb[ks][1] = to_tf32(wh[g * HID + 64 * hh + 8 * ks + t + 4]);
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t w_addr = smem_u32(smem + X2_W), xk_addr = smem_u32(smem + X2_XK);
-            const uint32_t g_addr = smem_u32(smem + X2_G), id_addr = smem_u32(smem + X2_ID);
-            auto forward = [&](int it) {
-                const int s = it & 1, ph = (it >> 1) & 1;
-                stamp(it, 0);
-                mbar_wait(&h_empty[s], ph ^ 1);
-                stamp(it, 1);
-                mbar_wait(xk_full, (uint32_t)(it & 1));
-                stamp(it, 2);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(s * HID);
-#pragma unroll
-                for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        umma_tf32(d_tmem, desc_kmajor(xk_addr + kb * KBLK_BYTES + k * 32),
-                                  desc_kmajor(w_addr + kb * KBLK_BYTES + k * 32), IDESC_FWD, (kb | k) ? 1u : 0u);
-                umma_commit(&h_full[s]);
-            };
-            auto transpose = [&]() {     // x^T of the tile in the x buffer (the dW MMAs of the previous tile were issued before)
-#pragma unroll
-                for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        umma_tf32(tmem_base + X2_TMEM_XT,
-                                  desc_nosw(id_addr + (15 - (4 * kb + k)) * X2_ID_GROUP, X2_ID_STRIP, X2_ID_GROUP),
-                                  desc_kmajor(xk_addr + kb * KBLK_BYTES + k * 32), IDESC_FWD, (kb | k) ? 1u : 0u);
-                umma_commit(xk_empty);   // the x tile may be overwritten: the next load starts
-            };
-            mbar_wait(w_full, 0);
-            forward(0);
-            transpose();
-            for (int it = 0; it < n_my; ++it) {
-                if (it + 1 < n_my) forward(it + 1);
-#pragma unroll 1
-                for (int q = 0; q < 4; ++q) {
-                    mbar_wait(&dp_full[q], (uint32_t)(it & 1));
-                    stamp(it, 3 + q);
-                    tc_fence_after();
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)      // K = 8 tile rows per MMA
-                        umma_tf32_ts(tmem_base + X2_TMEM_DW, tmem_base + (uint32_t)(X2_TMEM_XT + 32 * q + 8 * k),
-                                     desc_kmajor(g_addr + q * KBLK_BYTES + k * 32), IDESC_FWD, (it | q | k) ? 1u : 0u);
-                    umma_commit(&dp_empty[q]);
-                }
-                if (it + 1 < n_my) transpose();
-                stamp(it, 7);
-            }
-            umma_commit(dw_done);
-        }
+        ga[0] = to_tf32(wh[t * HID + hr0]);
+        ga[1] = to_tf32(wh[t * HID + hr1]);
+        ga[2] = to_tf32(wh[(t + 4) * HID + hr0]);
+        ga[3] = to_tf32(wh[(t + 4) * HID + hr1]);
     } else {
-        // ================= epilogue: all per-element products on the warp-level tensor core path (mma.sync, TF32 operands
-        // = the raw fp32 bits, low mantissa bits ignored like the UMMA products; fp32 accumulation -- the precision class of
-        // torch.set_float32_matmul_precision('high'), clean_pufferl.py:22).  Thread = row only for the TMEM read and the ReLU;
-        // everything else works on mma fragments of the warp's [32 rows][32 hidden units] block staged in its part of the
-        // dPre block.  The m / n / k indices of the three products are PERMUTED so that every fragment a lane needs is a run
-        // of 4 or 8 consecutive rows of one hidden unit (one or two 16-byte pieces of the K-major block: LDS.128 / STS.128),
-        // and so that the relu(h) fragments of the dW_heads product sit exactly where the g^T accumulators need their mask.
-        const int q = warp & 3, c = (warp - 2) >> 2;
-        const int g = lane >> 2, t = lane & 3;
-        uint8_t* mine = smem + X2_G + q * KBLK_BYTES + 32 * c * 128;   // hidden units 32c..32c+31 x the quadrant's 32 rows
-        float* xch = reinterpret_cast<float*>(smem + X2_XCH) + q * X2_XCH_Q;              // [4 c][32 rows][10]
-        float* dos = reinterpret_cast<float*>(smem + X2_DO) + q * X2_DO_Q;                // [32 rows][9]
-        const float4* be4 = reinterpret_cast<const float4*>(smem + X2_BE) + 8 * c;
-        // W_heads fragments of this column quarter (TF32), resident in registers:
-        //   heads   out[row][a] = sum_j rh[row][j] W[a][j]:  B[k][n = a], k = t + 4h <-> hidden unit 8kb + 2t + h
-        //   g^T     g[j][row]   = sum_a W[a][j] dO[row][a]:  A[m][k = a], m = g + 8h <-> hidden unit 16mb + 8h + g
-        uint32_t hb[4][2], ga[2][4];
 #pragma unroll
-        for (int kb = 0; kb < 4; ++kb) {
-            hb[kb][0] = to_tf32(p.w_heads[g * HID + 32 * c + 8 * kb + 2 * t]);
-            hb[kb][1] = to_tf32(p.w_heads[g * HID + 32 * c + 8 * kb + 2 * t + 1]);
+        for (int a = 0; a < NO; ++a) {
+            whr[0][a] = wh[a * HID + hr0];
+            whr[1][a] = wh[a * HID + hr1];
         }
-#pragma unroll
-        for (int mb = 0; mb < 2; ++mb) {
-            ga[mb][0] = to_tf32(p.w_heads[t * HID + 32 * c + 16 * mb + g]);
-            ga[mb][1] = to_tf32(p.w_heads[t * HID + 32 * c + 16 * mb + g + 8]);
-            ga[mb][2] = to_tf32(p.w_heads[(t + 4) * HID + 32 * c + 16 * mb + g]);
-            ga[mb][3] = to_tf32(p.w_heads[(t + 4) * HID + 32 * c + 16 * mb + g + 8]);
-        }
-        // addresses inside the warp's part of the dPre block (see g_off), hoisted out of the tile loop
-        uint8_t* const st_row = mine + ((lane & 3) << 2);       // thread = row: element (hidden unit k, row lane) at k * 128 + piece ((lane >> 2) ^ (k & 7))
-        uint8_t* ha_base[2];                                    // heads A: hidden unit 8kb + 2t + h, rows 4g..4g+3 (one piece)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) ha_base[h] = mine + (2 * t + h) * 128 + ((g ^ (2 * t + h)) << 4);
-        uint8_t* wb_base[2];                                    // dW_heads B / g^T C: hidden unit 8nb + g, rows 8t..8t+3 | 8t+4..8t+7
-#pragma unroll
-        for (int e = 0; e < 2; ++e) wb_base[e] = mine + g * 128 + ((((2 * t + e) ^ g)) << 4);
-
-        // the loss: warp c evaluates rows 8c..8c+7 of the quadrant, four lanes per row (ppo_row_sub)
-        const int lr = 8 * c + (lane >> 2), sub = lane & 3;
-        const float bh_lo = p.b_heads[sub], bh_hi = p.b_heads[sub + 4];
-        // per-row scalars of the loss rows, loaded ONE TILE AHEAD with volatile loads issued right after the second barrier
-        // (plain loads get sunk to their first use by the compiler, which puts their HBM latency back on the critical path)
-        struct RowIn { int act; float old_lp, adv, ret, old_v; bool valid; };
-        const float adv_mean = p.adv_norm ? p.adv_norm[0] : 0.f, adv_rstd = p.adv_norm ? p.adv_norm[1] : 1.f;
-        const bool need_old_v = p.clip_vloss || !p.returns;
-        auto ldg_f32 = [](const float* ptr) { float v; asm volatile("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(ptr)); return v; };
-        auto ldg_s64 = [](const int64_t* ptr) { long long v; asm volatile("ld.global.s64 %0, [%1];" : "=l"(v) : "l"(ptr)); return v; };
-        auto load_row = [&](int it) {
-            RowIn r;
-            r.act = 0; r.old_lp = 0.f; r.adv = 0.f; r.ret = 0.f; r.old_v = 0.f; r.valid = false;
-            if (it >= n_my) return r;
-            const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-            const int slab = tile / p.tiles_per_slab, tis = tile - slab * p.tiles_per_slab;
-            const int64_t lrow = (int64_t)tis * TILE_M + 32 * q + lr;
-            r.valid = lrow < p.slab_rows;
-            const int64_t ri = (int64_t)slab * p.row_slab_stride + lrow;     // position in the per-row arrays
-            if (r.valid) {
-                r.act = (int)ldg_s64(p.actions + ri);
-                r.old_lp = ldg_f32(p.old_logprobs + ri);
-                r.adv = ldg_f32(p.adv + ri);
-                if (need_old_v) r.old_v = ldg_f32(p.old_values + ri);
-                if (p.returns) r.ret = ldg_f32(p.returns + ri);
-            }
-            return r;
-        };
-        RowIn row = load_row(0);
-        for (int it = 0; it < n_my; ++it) {
-            const int s = it & 1, ph = (it >> 1) & 1;
-            // debug dumps only: slab-major position of tile row 0 of this quadrant, rows of the slab left in the tile
-            int64_t dbg_row0 = 0, rows_left = 32;
-            if (p.dbg_hidden || p.dbg_dout || p.dbg_dpre) {
-                const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-                dbg_row0 = (int64_t)(tile / p.tiles_per_slab) * p.slab_rows + (int64_t)(tile % p.tiles_per_slab) * TILE_M + 32 * q;
-                rows_left = p.slab_rows - ((int64_t)(tile % p.tiles_per_slab) * TILE_M + 32 * q);
-            }
-
-            // ---- 1. h -> relu(h + b_enc) into the warp's part of the dPre block (K-major: [hidden unit][row])
-            stamp(it, 0);
-            mbar_wait(&h_full[s], ph);
-            stamp(it, 1);
-            tc_fence_after();
-            {
-                float v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(s * HID + 32 * c), v);
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&h_empty[s]);                      // the accumulator stage is free already
-                mbar_wait(&dp_empty[q], (uint32_t)((it & 1) ^ 1));            // the dW MMAs of the previous tile have read the block
-                stamp(it, 2);
-#pragma unroll
-                for (int k4 = 0; k4 < 8; ++k4) {
-                    const float4 b = be4[k4];
-                    v[4 * k4] = fmaxf(v[4 * k4] + b.x, 0.f);
-                    v[4 * k4 + 1] = fmaxf(v[4 * k4 + 1] + b.y, 0.f);
-                    v[4 * k4 + 2] = fmaxf(v[4 * k4 + 2] + b.z, 0.f);
-                    v[4 * k4 + 3] = fmaxf(v[4 * k4 + 3] + b.w, 0.f);
-                }
-#pragma unroll
-                for (int k = 0; k < 32; ++k) *reinterpret_cast<float*>(st_row + ((((lane >> 2) ^ (k & 7))) << 4) + k * 128) = v[k];
-                if (p.dbg_hidden && lane < rows_left) {
-#pragma unroll
-                    for (int k = 0; k < 32; k += 4)
-                        *reinterpret_cast<float4*>(p.dbg_hidden + (dbg_row0 + lane) * HID + 32 * c + k) = make_float4(v[k], v[k + 1], v[k + 2], v[k + 3]);
-                }
-            }
-            __syncwarp();
-
-            // ---- 2. this quarter's share of the head products.  m = g + 8h of block mb <-> row 4g + 2mb + h
-            {
-                float hp[2][4];
-#pragma unroll
-                for (int mb = 0; mb < 2; ++mb) hp[mb][0] = hp[mb][1] = hp[mb][2] = hp[mb][3] = 0.f;
-#pragma unroll
-                for (int kb = 0; kb < 4; ++kb) {
-                    const float4 lo = *reinterpret_cast<const float4*>(ha_base[0] + kb * 1024);   // hidden unit 8kb + 2t
-                    const float4 hi = *reinterpret_cast<const float4*>(ha_base[1] + kb * 1024);   // hidden unit 8kb + 2t + 1
-                    const uint32_t a0[4] = {__float_as_uint(lo.x), __float_as_uint(lo.y), __float_as_uint(hi.x), __float_as_uint(hi.y)};
-                    const uint32_t a1[4] = {__float_as_uint(lo.z), __float_as_uint(lo.w), __float_as_uint(hi.z), __float_as_uint(hi.w)};
-                    mma_tf32_full(hp[0], a0, hb[kb][0], hb[kb][1]);
-                    mma_tf32_full(hp[1], a1, hb[kb][0], hb[kb][1]);
-                }
-#pragma unroll
-                for (int mb = 0; mb < 2; ++mb) {
-                    *reinterpret_cast<float2*>(xch + (c * 32 + 4 * g + 2 * mb) * X2_XCH_ROW + 2 * t) = make_float2(hp[mb][0], hp[mb][1]);
-                    *reinterpret_cast<float2*>(xch + (c * 32 + 4 * g + 2 * mb + 1) * X2_XCH_ROW + 2 * t) = make_float2(hp[mb][2], hp[mb][3]);
-                }
-            }
-            stamp(it, 3);
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory");
-            stamp(it, 4);
-
-            // ---- 3. the loss row math on the summed head outputs -> dOut tile of the quadrant
-            {
-                float z_lo = bh_lo, z_hi = bh_hi;
-#pragma unroll
-                for (int cq = 0; cq < 4; ++cq) {                                    // fixed order
-                    z_lo += xch[(cq * 32 + lr) * X2_XCH_ROW + sub];
-                    z_hi += xch[(cq * 32 + lr) * X2_XCH_ROW + sub + 4];
-                }
-                const float ret = p.returns ? row.ret : row.adv + row.old_v;       // returns = raw advantages + old values (:476-481)
-                const float adv = (row.adv - adv_mean) * adv_rstd;
-                float g_lo, g_hi;
-                const RowStats rs = ppo_row_sub(z_lo, z_hi, sub, lane, p, row.act, row.old_lp, adv, ret, row.old_v, g_lo, g_hi);
-                if (!row.valid) g_lo = g_hi = 0.f;
-                if (row.valid && sub == 0) {
-                    st[0] += rs.pg; st[1] += rs.v; st[2] += rs.ent; st[3] += rs.okl; st[4] += rs.kl; st[5] += rs.clipped;
-                }
-                acc_bh2[0] += g_lo;
-                acc_bh2[1] += g_hi;
-                dos[lr * X2_DO_ROW + sub] = g_lo;
-                dos[lr * X2_DO_ROW + sub + 4] = g_hi;
-                if (p.dbg_dout && row.valid) {
-                    p.dbg_dout[(dbg_row0 + lr) * 8 + sub] = g_lo;
-                    p.dbg_dout[(dbg_row0 + lr) * 8 + sub + 4] = g_hi;
-                }
-            }
-            stamp(it, 5);
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory");
-            stamp(it, 6);
-
-            // ---- 4. per 16 hidden units (block mb):
-            //         g^T[hidden unit][row] = W^T . dO^T        n = 2t' + j of block nb' <-> row 8t' + 2nb' + j
-            //         dW_heads^T += rh^T . dO                   k = t + 4j of block ks  <-> row 8t + 2ks + j,  m = g + 8h <-> unit 16mb + 8h + g
-            //      the rh fragments of the second product sit exactly where the first one's accumulators need their mask, and
-            //      dPre goes back to the same places: no lane touches another lane's elements in this step
-            {
-                uint32_t gb[4][2], bfr[4][2];
-#pragma unroll
-                for (int nb = 0; nb < 4; ++nb) {                 // dO as B[k = head][n = row] (g^T) and as B[k = row][n = head] (dW_heads^T)
-                    const int rn = 8 * (g >> 1) + 2 * nb + (g & 1);
-                    gb[nb][0] = __float_as_uint(dos[rn * X2_DO_ROW + t]);
-                    gb[nb][1] = __float_as_uint(dos[rn * X2_DO_ROW + t + 4]);
-                    bfr[nb][0] = __float_as_uint(dos[(8 * t + 2 * nb) * X2_DO_ROW + g]);
-                    bfr[nb][1] = __float_as_uint(dos[(8 * t + 2 * nb + 1) * X2_DO_ROW + g]);
-                }
-#pragma unroll
-                for (int mb = 0; mb < 2; ++mb) {
-                    float gt[4][4];                              // [nb'][2h + j]: hidden unit 16mb + 8h + g, row 8t + 2nb' + j
-#pragma unroll
-                    for (int nb = 0; nb < 4; ++nb) {
-                        gt[nb][0] = gt[nb][1] = gt[nb][2] = gt[nb][3] = 0.f;
-                        mma_tf32_full(gt[nb], ga[mb], gb[nb][0], gb[nb][1]);
-                    }
-                    float4 lo[2], hi[2];
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        lo[h] = *reinterpret_cast<const float4*>(wb_base[0] + (2 * mb + h) * 1024);   // rows 8t .. 8t+3
-                        hi[h] = *reinterpret_cast<const float4*>(wb_base[1] + (2 * mb + h) * 1024);   // rows 8t+4 .. 8t+7
-                    }
-                    // A[m = g + 8h][k = t + 4j] = rh[row 8t + 2ks + j][hidden unit 16mb + 8h + g]
-                    const uint32_t a0[4] = {__float_as_uint(lo[0].x), __float_as_uint(lo[1].x), __float_as_uint(lo[0].y), __float_as_uint(lo[1].y)};
-                    const uint32_t a1[4] = {__float_as_uint(lo[0].z), __float_as_uint(lo[1].z), __float_as_uint(lo[0].w), __float_as_uint(lo[1].w)};
-                    const uint32_t a2[4] = {__float_as_uint(hi[0].x), __float_as_uint(hi[1].x), __float_as_uint(hi[0].y), __float_as_uint(hi[1].y)};
-                    const uint32_t a3[4] = {__float_as_uint(hi[0].z), __float_as_uint(hi[1].z), __float_as_uint(hi[0].w), __float_as_uint(hi[1].w)};
-                    mma_tf32_full(acc_wh[mb], a0, bfr[0][0], bfr[0][1]);
-                    mma_tf32_full(acc_wh[mb], a1, bfr[1][0], bfr[1][1]);
-                    mma_tf32_full(acc_wh[mb], a2, bfr[2][0], bfr[2][1]);
-                    mma_tf32_full(acc_wh[mb], a3, bfr[3][0], bfr[3][1]);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const float4 d0 = make_float4(lo[h].x > 0.f ? gt[0][2 * h] : 0.f, lo[h].y > 0.f ? gt[0][2 * h + 1] : 0.f,
-                                                      lo[h].z > 0.f ? gt[1][2 * h] : 0.f, lo[h].w > 0.f ? gt[1][2 * h + 1] : 0.f);
-                        const float4 d1 = make_float4(hi[h].x > 0.f ? gt[2][2 * h] : 0.f, hi[h].y > 0.f ? gt[2][2 * h + 1] : 0.f,
-                                                      hi[h].z > 0.f ? gt[3][2 * h] : 0.f, hi[h].w > 0.f ? gt[3][2 * h + 1] : 0.f);
-                        *reinterpret_cast<float4*>(wb_base[0] + (2 * mb + h) * 1024) = d0;
-                        *reinterpret_cast<float4*>(wb_base[1] + (2 * mb + h) * 1024) = d1;
-                        acc_be[2 * mb + h] += ((d0.x + d0.y) + (d0.z + d0.w)) + ((d1.x + d1.y) + (d1.z + d1.w));
-                        if (p.dbg_dpre) {
-                            const float dv[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
-#pragma unroll
-                            for (int r8 = 0; r8 < 8; ++r8)
-                                if (8 * t + r8 < rows_left) p.dbg_dpre[(dbg_row0 + 8 * t + r8) * HID + 32 * c + 16 * mb + 8 * h + g] = dv[r8];
-                        }
-                    }
-                }
-            }
-            row = load_row(it + 1);          // (volatile loads: issued here, where few registers are live)
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&dp_full[q]);
-            stamp(it, 7);
-        }
-        // ---- the dW^T accumulator: TMEM lane = feature, column = hidden unit
-        mbar_wait(dw_done, 0);
-        tc_fence_after();
-        {
-            float v[32];
-            float* pd = p.part_dw + ((int64_t)blockIdx.x * FEAT + 32 * q + lane) * HID + 32 * c;
-            tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(X2_TMEM_DW + 32 * c), v);
-#pragma unroll
-            for (int k = 0; k < 32; k += 4) *reinterpret_cast<float4*>(pd + k) = make_float4(v[k], v[k + 1], v[k + 2], v[k + 3]);
-        }
-#pragma unroll
-        for (int k = 0; k < 6; ++k) {          // statistics: the sub == 0 lanes hold this warp's rows
-            double x = (double)st[k];
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
-            if (lane == 0) atomicAdd(p.stats + k, x);
-        }
-        // db_enc: the four lanes of a hidden unit (t = 0..3) hold its 4 x 8 rows; db_heads: the eight lanes with the same sub
-#pragma unroll
-        for (int nb = 0; nb < 4; ++nb) {
-            acc_be[nb] += __shfl_xor_sync(0xffffffffu, acc_be[nb], 1);
-            acc_be[nb] += __shfl_xor_sync(0xffffffffu, acc_be[nb], 2);
-        }
-#pragma unroll
-        for (int j = 0; j < 2; ++j)
-#pragma unroll
-            for (int off = 4; off < 32; off <<= 1) acc_bh2[j] += __shfl_xor_sync(0xffffffffu, acc_bh2[j], off);
     }
 
-    // ================= CTA reduction of the small gradients =================
-    tc_fence_before();
-    __syncthreads();                           // every role is done: all MMAs retired, the x tile is scratch now
-    if (warp >= 2) {
-        const int q = warp & 3, c = (warp - 2) >> 2, g = lane >> 2, t = lane & 3;
-        float* red = reinterpret_cast<float*>(smem + X2_XK);
-        float* mine_r = red + q * TAIL;
+    float dwacc[64];                     // dW_enc^T [feature 64wg + 16wq + g (+8)][hidden unit 8j + 2t (+1)]
 #pragma unroll
-        for (int nb = 0; nb < 4; ++nb) {
-            mine_r[(2 * t) * HID + 32 * c + 8 * nb + g] = acc_wh[nb >> 1][2 * (nb & 1)];
-            mine_r[(2 * t + 1) * HID + 32 * c + 8 * nb + g] = acc_wh[nb >> 1][2 * (nb & 1) + 1];
-            if (t == 0) mine_r[NO * HID + 32 * c + 8 * nb + g] = acc_be[nb];
+    for (int i = 0; i < 64; ++i) dwacc[i] = 0.f;
+    float dwh[4] = {0.f, 0.f, 0.f, 0.f};  // dW_heads^T [hr0 | hr1][head 2t | 2t + 1]
+    float be_acc[2] = {0.f, 0.f};        // db_enc[hr0], db_enc[hr1] over this thread's rows
+    float bh_acc[2] = {0.f, 0.f};        // db_heads[sub], [sub + 4] over this thread's loss rows
+    double st[6] = {0, 0, 0, 0, 0, 0};
+    const float adv_mean = p.adv_norm ? p.adv_norm[0] : 0.f, adv_rstd = p.adv_norm ? p.adv_norm[1] : 1.f;
+    const bool need_old_v = p.clip_vloss || !p.returns;
+    const uint32_t w_addr = smem_u32(smem + SM_W), g_addr = smem_u32(gbuf);
+
+    for (int it = 0; it < n_my; ++it) {
+        const int s = it % NSTAGE;
+        const int tile = (int)blockIdx.x + it * (int)gridDim.x;
+        const int slab = tile / p.tiles_per_slab, tis = tile - slab * p.tiles_per_slab;
+        const int64_t lrow0 = (int64_t)tis * TILE_M;                          // slab-local row of tile row 0
+        const int rows_left = (int)(p.slab_rows - lrow0 < TILE_M ? p.slab_rows - lrow0 : TILE_M);
+        const int64_t i0 = (int64_t)slab * p.slab_rows + lrow0;               // slab-major position (dPre / debug rows)
+        // per-row inputs of the loss row (issued before the waits: their latency hides behind the forward product)
+        const bool valid = lr < rows_left;
+        int act = 0;
+        float old_lp = 0.f, adv = 0.f, ret = 0.f, old_v = 0.f;
+        if (valid) {
+            const int64_t ri = (int64_t)slab * p.row_slab_stride + lrow0 + lr;
+            act = (int)p.actions[ri];
+            old_lp = p.old_logprobs[ri];
+            adv = p.adv[ri];
+            if (need_old_v) old_v = p.old_values[ri];
+            if (p.returns) ret = p.returns[ri];
         }
-        if (lane < 4) {                        // db_heads partial of this warp's rows: [16 warps][8] behind the four TAIL rows
-            red[4 * TAIL + (warp - 2) * NO + lane] = acc_bh2[0];
-            red[4 * TAIL + (warp - 2) * NO + lane + 4] = acc_bh2[1];
+        if (it == 0) mbar_wait(w_full, 0);
+        mbar_wait(&x_full[s], (uint32_t)((it / NSTAGE) & 1));
+        const uint8_t* xs = smem + SM_X + s * X_TILE_BYTES;
+        const uint32_t x_addr = smem_u32(xs);
+
+        // ---- 1. hidden^T = W_enc[64wg .. 64wg + 63] . x^T  (M = hidden units, N = 64 rows, K = 128 features)
+        float h[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) h[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                wgmma_m64n64k8_ss(h, wgmma_desc_sw128(w_addr + kb * W_KBLK_BYTES + wg * 8192 + k * 32),
+                                  wgmma_desc_sw128(x_addr + kb * X_KBLK_BYTES + k * 32), (kb | k) ? 1 : 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(h);
+
+        // ---- 2. relu(h + b_enc)^T -> shared memory (the operand of the head products)
+        {
+            const float b0 = be[hr0], b1 = be[hr1];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                h[4 * j] = fmaxf(h[4 * j] + b0, 0.f);
+                h[4 * j + 1] = fmaxf(h[4 * j + 1] + b0, 0.f);
+                h[4 * j + 2] = fmaxf(h[4 * j + 2] + b1, 0.f);
+                h[4 * j + 3] = fmaxf(h[4 * j + 3] + b1, 0.f);
+                const int l = 8 * j + 2 * t;
+                *reinterpret_cast<float2*>(gbuf + g_off(hr0, l)) = make_float2(h[4 * j], h[4 * j + 1]);
+                *reinterpret_cast<float2*>(gbuf + g_off(hr1, l)) = make_float2(h[4 * j + 2], h[4 * j + 3]);
+                if (p.dbg_hidden) {
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int le = l + (e & 1), he = (e & 2) ? hr1 : hr0;
+                        if (le < rows_left) p.dbg_hidden[(i0 + le) * HID + he] = h[4 * j + e];
+                    }
+                }
+            }
         }
+        __syncthreads();
+
+        // ---- 3. head products: out[row][a] = relu(h)[row] . W_heads[a]
+        if (TF32_EPI) {      // warp: rows 16(warp & 3) .. +15, hidden half warp >> 2; partial sums of the two halves to outp
+            const int l0 = 16 * (warp & 3) + g, hh = warp >> 2;
+            float c[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks) {
+                const int n0 = 64 * hh + 8 * ks + t;
+                const uint32_t a[4] = {*reinterpret_cast<const uint32_t*>(gbuf + g_off(n0, l0)),
+                                       *reinterpret_cast<const uint32_t*>(gbuf + g_off(n0, l0 + 8)),
+                                       *reinterpret_cast<const uint32_t*>(gbuf + g_off(n0 + 4, l0)),
+                                       *reinterpret_cast<const uint32_t*>(gbuf + g_off(n0 + 4, l0 + 8))};
+                mma_tf32(c, a, hb[ks][0], hb[ks][1]);
+            }
+            *reinterpret_cast<float2*>(outp + (hh * TILE_M + l0) * NO + 2 * t) = make_float2(c[0], c[1]);
+            *reinterpret_cast<float2*>(outp + (hh * TILE_M + l0 + 8) * NO + 2 * t) = make_float2(c[2], c[3]);
+        } else {             // thread = (row, pair of heads), fp32 FFMAs over all 128 hidden units
+            const int l = tid & (TILE_M - 1), a0 = 2 * (tid >> 6);
+            float o0 = 0.f, o1 = 0.f;
+            if (a0 <= p.n_act) {
+#pragma unroll 8
+                for (int n = 0; n < HID; ++n) {
+                    const float rh = *reinterpret_cast<const float*>(gbuf + g_off(n, l));
+                    o0 = fmaf(rh, wh[a0 * HID + n], o0);
+                    o1 = fmaf(rh, wh[(a0 + 1) * HID + n], o1);
+                }
+            }
+            *reinterpret_cast<float2*>(outp + l * NO + a0) = make_float2(o0, o1);
+        }
+        __syncthreads();
+
+        // ---- 4. the loss row math -> dOut of the tile
+        {
+            float z_lo = bh_lo + outp[lr * NO + sub], z_hi = bh_hi + outp[lr * NO + sub + 4];
+            if (TF32_EPI) {
+                z_lo += outp[(TILE_M + lr) * NO + sub];
+                z_hi += outp[(TILE_M + lr) * NO + sub + 4];
+            }
+            const float r_ = p.returns ? ret : adv + old_v;       // returns = raw advantages + old values (:476-481)
+            const float a_ = (adv - adv_mean) * adv_rstd;
+            float g_lo, g_hi;
+            const RowStats rs = ppo_row_sub(z_lo, z_hi, sub, lane, p, act, old_lp, a_, r_, old_v, g_lo, g_hi);
+            if (!valid) g_lo = g_hi = 0.f;
+            if (valid && sub == 0) {
+                st[0] += rs.pg; st[1] += rs.v; st[2] += rs.ent; st[3] += rs.okl; st[4] += rs.kl; st[5] += rs.clipped;
+            }
+            bh_acc[0] += g_lo;
+            bh_acc[1] += g_hi;
+            dos[lr * NO + sub] = g_lo;
+            dos[lr * NO + sub + 4] = g_hi;
+            if (p.dbg_dout && valid) {
+                p.dbg_dout[(i0 + lr) * 8 + sub] = g_lo;
+                p.dbg_dout[(i0 + lr) * 8 + sub + 4] = g_hi;
+            }
+        }
+        __syncthreads();
+
+        // ---- 5. g^T = W_heads^T dOut^T (same fragment layout as hidden^T), dPre^T = g^T where relu(h) > 0, db_enc, and
+        //         dW_heads^T += relu(h)^T dOut with the hidden^T registers as the A fragments (k = t <-> row 8j + 2t,
+        //         k = t + 4 <-> row 8j + 2t + 1)
+        float dp[32];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            if (TF32_EPI) {
+                float c[4] = {0.f, 0.f, 0.f, 0.f};
+                mma_tf32(c, ga, __float_as_uint(dos[(8 * j + g) * NO + t]), __float_as_uint(dos[(8 * j + g) * NO + t + 4]));
+                dp[4 * j] = c[0]; dp[4 * j + 1] = c[1]; dp[4 * j + 2] = c[2]; dp[4 * j + 3] = c[3];
+            } else {
+                const int l = 8 * j + 2 * t;
+                const float4 d0a = *reinterpret_cast<const float4*>(dos + l * NO), d0b = *reinterpret_cast<const float4*>(dos + l * NO + 4);
+                const float4 d1a = *reinterpret_cast<const float4*>(dos + (l + 1) * NO), d1b = *reinterpret_cast<const float4*>(dos + (l + 1) * NO + 4);
+                const float d0[8] = {d0a.x, d0a.y, d0a.z, d0a.w, d0b.x, d0b.y, d0b.z, d0b.w};
+                const float d1[8] = {d1a.x, d1a.y, d1a.z, d1a.w, d1b.x, d1b.y, d1b.z, d1b.w};
+                float s00 = 0.f, s01 = 0.f, s10 = 0.f, s11 = 0.f;
+#pragma unroll
+                for (int a = 0; a < NO; ++a) {
+                    s00 = fmaf(d0[a], whr[0][a], s00);
+                    s01 = fmaf(d1[a], whr[0][a], s01);
+                    s10 = fmaf(d0[a], whr[1][a], s10);
+                    s11 = fmaf(d1[a], whr[1][a], s11);
+                }
+                dp[4 * j] = s00; dp[4 * j + 1] = s01; dp[4 * j + 2] = s10; dp[4 * j + 3] = s11;
+            }
+#pragma unroll
+            for (int e = 0; e < 4; ++e) dp[4 * j + e] = h[4 * j + e] > 0.f ? dp[4 * j + e] : 0.f;
+            be_acc[0] += dp[4 * j] + dp[4 * j + 1];
+            be_acc[1] += dp[4 * j + 2] + dp[4 * j + 3];
+            const float b0 = dos[(8 * j + 2 * t) * NO + g], b1 = dos[(8 * j + 2 * t + 1) * NO + g];
+            if (TF32_EPI) {
+                const uint32_t a[4] = {__float_as_uint(h[4 * j]), __float_as_uint(h[4 * j + 2]), __float_as_uint(h[4 * j + 1]),
+                                       __float_as_uint(h[4 * j + 3])};
+                mma_tf32(dwh, a, __float_as_uint(b0), __float_as_uint(b1));
+            } else {
+                const uint32_t a[4] = {to_tf32(h[4 * j]), to_tf32(h[4 * j + 2]), to_tf32(h[4 * j + 1]), to_tf32(h[4 * j + 3])};
+                mma_tf32(dwh, a, to_tf32(b0), to_tf32(b1));
+            }
+            const int l = 8 * j + 2 * t;
+            if (p.dbg_dpre) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int le = l + (e & 1), he = (e & 2) ? hr1 : hr0;
+                    if (le < rows_left) p.dbg_dpre[(i0 + le) * HID + he] = dp[4 * j + e];
+                }
+            }
+            // dPre^T over relu(h)^T (every read of relu(h)^T, step 3, is behind the last barrier): TF32 rounded to nearest as
+            // the operand of the dW product, or exact for the row writes of the dPre-to-HBM mode
+            if (DW_KERNEL) {
+                *reinterpret_cast<uint2*>(gbuf + g_off(hr0, l)) = make_uint2(to_tf32(dp[4 * j]), to_tf32(dp[4 * j + 1]));
+                *reinterpret_cast<uint2*>(gbuf + g_off(hr1, l)) = make_uint2(to_tf32(dp[4 * j + 2]), to_tf32(dp[4 * j + 3]));
+            } else {
+                *reinterpret_cast<float2*>(gbuf + g_off(hr0, l)) = make_float2(dp[4 * j], dp[4 * j + 1]);
+                *reinterpret_cast<float2*>(gbuf + g_off(hr1, l)) = make_float2(dp[4 * j + 2], dp[4 * j + 3]);
+            }
+        }
+
+        // ---- 6. dW_enc^T [64wg .. 64wg + 63][128] += x^T . dPre  (M = features, N = hidden units, K = 64 rows).  Both
+        //         operands are rounded to nearest TF32 (truncation would bias a sum over the whole minibatch)
+        if (DW_KERNEL) {
+            fence_proxy_async_smem();            // dPre^T written by the generic proxy, read by the tensor core
+            __syncthreads();
+            const int f0 = 64 * wg + 16 * wq + g;
+            uint32_t xa[8][4];                   // all A fragments of the tile: registers stay owned until the wait
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks) {
+                const int r0 = 8 * ks + t;
+                xa[ks][0] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0)));
+                xa[ks][1] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0 + 8)));
+                xa[ks][2] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0)));
+                xa[ks][3] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0 + 8)));
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks)
+                wgmma_m64n128k8_rs(dwacc, xa[ks], wgmma_desc_sw128(g_addr + (ks >> 2) * G_KBLK_BYTES + (ks & 3) * 32), 1);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(dwacc);
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
+        } else {
+            // ---- 6'. dPre rows to HBM: warp w writes rows 8w .. 8w + 7, one whole 512-byte row per store instruction
+            __syncthreads();
+#pragma unroll
+            for (int k = 0; k < TILE_M / 8; ++k) {
+                const int l = 8 * warp + k;
+                if (l < rows_left) {
+                    const int n = 4 * lane;
+                    const float4 v = make_float4(*reinterpret_cast<const float*>(gbuf + g_off(n, l)),
+                                                 *reinterpret_cast<const float*>(gbuf + g_off(n + 1, l)),
+                                                 *reinterpret_cast<const float*>(gbuf + g_off(n + 2, l)),
+                                                 *reinterpret_cast<const float*>(gbuf + g_off(n + 3, l)));
+                    __stcs(reinterpret_cast<float4*>(p.dpre_out + (i0 + l) * HID + n), v);
+                }
+            }
+        }
+        __syncthreads();                         // every read of x stage s and of the shared tile buffers is done
+        if (tid == 0 && it + NSTAGE < n_my) {
+            fence_proxy_async_smem();
+            issue(it + NSTAGE);
+        }
+    }
+
+    // ================= per-CTA partials =================
+    if (DW_KERNEL) {
+        float* pd = p.part_dw + (int64_t)blockIdx.x * FEAT * HID;
+        const int f0 = 64 * wg + 16 * wq + g;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            *reinterpret_cast<float2*>(pd + f0 * HID + 8 * j + 2 * t) = make_float2(dwacc[4 * j], dwacc[4 * j + 1]);
+            *reinterpret_cast<float2*>(pd + (f0 + 8) * HID + 8 * j + 2 * t) = make_float2(dwacc[4 * j + 2], dwacc[4 * j + 3]);
+        }
+    }
+    float* pt = p.part_tail + (int64_t)blockIdx.x * TAIL;
+    pt[(2 * t) * HID + hr0] = dwh[0];
+    pt[(2 * t + 1) * HID + hr0] = dwh[1];
+    pt[(2 * t) * HID + hr1] = dwh[2];
+    pt[(2 * t + 1) * HID + hr1] = dwh[3];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {        // db_enc: the four lanes of a hidden unit hold disjoint rows
+        be_acc[k] += __shfl_xor_sync(0xffffffffu, be_acc[k], 1);
+        be_acc[k] += __shfl_xor_sync(0xffffffffu, be_acc[k], 2);
+    }
+    if (t == 0) {
+        pt[NO * HID + hr0] = be_acc[0];
+        pt[NO * HID + hr1] = be_acc[1];
+    }
+#pragma unroll
+    for (int k = 0; k < 2; ++k)          // db_heads: the eight lanes with the same sub
+#pragma unroll
+        for (int off = 4; off < 32; off <<= 1) bh_acc[k] += __shfl_xor_sync(0xffffffffu, bh_acc[k], off);
+    if (lane < 4) {
+        red[warp * NO + lane] = bh_acc[0];
+        red[warp * NO + lane + 4] = bh_acc[1];
+    }
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {        // loss statistics: the sub == 0 lanes hold this warp's rows
+        double x = st[k];
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
+        if (lane == 0) atomicAdd(p.stats + k, x);
     }
     __syncthreads();
-    {
-        const float* red = reinterpret_cast<const float*>(smem + X2_XK);   // [4 quadrants][TAIL] | [16 warps][8] db_heads partials
-        float* pt = p.part_tail + (int64_t)blockIdx.x * TAIL;
-        for (int j = threadIdx.x; j < TAIL; j += X2_THREADS) {
-            float v;
-            if (j < NO * HID + HID) {
-                v = red[j] + red[TAIL + j] + red[2 * TAIL + j] + red[3 * TAIL + j];
-            } else {
-                v = 0.f;
-                for (int w = 0; w < 16; ++w) v += red[4 * TAIL + w * NO + (j - NO * HID - HID)];
-            }
-            pt[j] = v;
-        }
+    if (tid < NO) {
+        float v = 0.f;
+        for (int w = 0; w < THREADS / 32; ++w) v += red[w * NO + tid];
+        pt[NO * HID + HID + tid] = v;
     }
-    if (warp == 1)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS)
-                     : "memory");
 }
 
 // Deterministic sum of the per-CTA partials into the flat gradient buffer:
@@ -1223,14 +578,14 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-int make_map2(EncodeTiledFn fn, CUtensorMap* map, const float* base, int64_t rows, int64_t row_stride_floats,
-              CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
+// 2-D map of a [rows][128] fp32 matrix (row stride in floats), boxes of [box_rows][32 floats] with the 128-byte swizzle
+int make_map2(EncodeTiledFn fn, CUtensorMap* map, const float* base, int64_t rows, int64_t row_stride_floats, int box_rows) {
     const cuuint64_t dims[2] = {(cuuint64_t)FEAT, (cuuint64_t)rows};
     const cuuint64_t strides[1] = {(cuuint64_t)row_stride_floats * 4};
-    const cuuint32_t box[2] = {(cuuint32_t)KBLK, (cuuint32_t)TILE_M};
+    const cuuint32_t box[2] = {(cuuint32_t)KBLK, (cuuint32_t)box_rows};
     const cuuint32_t estr[2] = {1, 1};
     const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     PB_REQUIRE(r == CUDA_SUCCESS, PB_ERR_CUDA, "cuTensorMapEncodeTiled failed: %d", (int)r);
     return PB_OK;
@@ -1238,19 +593,13 @@ int make_map2(EncodeTiledFn fn, CUtensorMap* map, const float* base, int64_t row
 
 int num_sms() { return pb_num_sms(); }
 
-long long* g_dbg_clk = nullptr;
-int g_update_variant = 2;     // 1 = two x layouts (k_mlp_update_fused), 2 = one x layout + transposing MMA (k_mlp_update_xt)
+int g_update_variant = 2;     // 1 = fp32 head / g^T products, 2 = TF32 mma.sync epilogue
 
 }  // namespace
 
 extern "C" int pb_mlp_update_set_variant(int32_t variant) {
     PB_REQUIRE(variant == 1 || variant == 2, PB_ERR_INVALID, "pb_mlp_update_set_variant: 1 or 2");
     g_update_variant = variant;
-    return PB_OK;
-}
-
-extern "C" int pb_mlp_update_debug_clock(long long* buf) {     // profiling hook: see FusedParams::dbg_clk; nullptr = off
-    g_dbg_clk = buf;
     return PB_OK;
 }
 
@@ -1293,10 +642,9 @@ extern "C" int pb_mlp_update_fused(const float* x, int64_t ldx, int64_t slab_row
     const int64_t n_tiles = tiles_per_slab * n_slabs;
     const int64_t map_rows = (int64_t)(n_slabs - 1) * slab_stride_rows + slab_rows;
     PB_REQUIRE(n_tiles <= 0x7FFFFFFF && map_rows <= 0x7FFFFFFF, PB_ERR_UNSUPPORTED, "pb_mlp_update_fused: too many rows");
-    alignas(64) CUtensorMap map_x, map_x32, map_w;
-    int rc = make_map2((EncodeTiledFn)fn, &map_x, x, map_rows, ldx);
-    if (rc == PB_OK) rc = make_map2((EncodeTiledFn)fn, &map_x32, x, map_rows, ldx, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
-    if (rc == PB_OK) rc = make_map2((EncodeTiledFn)fn, &map_w, w_enc, HID, FEAT);
+    alignas(64) CUtensorMap map_x, map_w;
+    int rc = make_map2((EncodeTiledFn)fn, &map_x, x, map_rows, ldx, TILE_M);
+    if (rc == PB_OK) rc = make_map2((EncodeTiledFn)fn, &map_w, w_enc, HID, FEAT, HID);
     if (rc != PB_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     const int grid = n_tiles < num_sms() ? (int)n_tiles : num_sms();
@@ -1307,37 +655,19 @@ extern "C" int pb_mlp_update_fused(const float* x, int64_t ldx, int64_t slab_row
     p.tiles_per_slab = (int)tiles_per_slab; p.n_tiles = (int)n_tiles; p.n_act = n_act;
     p.clip = clip_coef; p.vclip = vf_clip_coef; p.vf_coef = vf_coef; p.ent_coef = ent_coef; p.clip_vloss = clip_vloss;
     p.part_dw = (float*)workspace; p.part_tail = (float*)workspace + (size_t)num_sms() * FEAT * HID;
-    p.dbg_clk = g_dbg_clk;
     p.w_heads = w_heads; p.b_enc = b_enc; p.b_heads = b_heads;
     p.stats = stats8; p.dpre_out = dpre_out; p.dbg_hidden = dbg_hidden; p.dbg_dpre = dbg_dpre; p.dbg_dout = dbg_dout;
     PB_CUDA(cudaMemsetAsync(stats8, 0, 8 * sizeof(double), s));
-    if (dpre_out || g_update_variant != 2) {      // variant 1 takes the small operands from the constant bank
-        PB_CUDA(cudaMemcpyToSymbolAsync(c_wh, w_heads, sizeof(float) * NO * HID, 0, cudaMemcpyDeviceToDevice, s));
-        PB_CUDA(cudaMemcpyToSymbolAsync(c_benc, b_enc, sizeof(float) * HID, 0, cudaMemcpyDeviceToDevice, s));
-        PB_CUDA(cudaMemcpyToSymbolAsync(c_bh, b_heads, sizeof(float) * NO, 0, cudaMemcpyDeviceToDevice, s));
-    }
-    // dispatch on the live head rows (n_act + 1: 5 for the 4-action configs, 8 = generic) and on where dW_enc is formed
     static bool attr_set = false;
     if (!attr_set) {
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update_fused<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update_fused<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update_fused<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update_fused<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update_xt<96, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, X2_TOTAL));
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update_xt<96, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, X2_TOTAL));
+        PB_CUDA(cudaFuncSetAttribute(k_mlp_update<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
+        PB_CUDA(cudaFuncSetAttribute(k_mlp_update<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
+        PB_CUDA(cudaFuncSetAttribute(k_mlp_update<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
         attr_set = true;
     }
-    if (dpre_out) {
-        if (n_act + 1 <= 5) k_mlp_update_fused<5, false><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_x32, map_w, p);
-        else k_mlp_update_fused<8, false><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_x32, map_w, p);
-    } else if (g_update_variant == 2) {
-        // 18 warps = 5 on two of the four schedulers: 16384 registers / (5 x 32) caps the kernel at 96 per thread
-        if (p.dbg_clk) k_mlp_update_xt<96, true><<<grid, X2_THREADS, X2_TOTAL, s>>>(map_x, map_w, p);
-        else k_mlp_update_xt<96, false><<<grid, X2_THREADS, X2_TOTAL, s>>>(map_x, map_w, p);
-    } else {
-        if (n_act + 1 <= 5) k_mlp_update_fused<5, true><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_x32, map_w, p);
-        else k_mlp_update_fused<8, true><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_x32, map_w, p);
-    }
+    if (dpre_out) k_mlp_update<false, false><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_w, p);
+    else if (g_update_variant == 2) k_mlp_update<true, true><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_w, p);
+    else k_mlp_update<false, true><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_w, p);
     PB_LAUNCH_CHECK();
     k_update_reduce<<<REDUCE_BLOCKS, 256, 0, s>>>(dpre_out ? nullptr : p.part_dw, p.part_tail, grid, grad_flat,
                                                   reinterpret_cast<double*>((char*)workspace + pb_mlp_update_sumsq_offset()));

@@ -1,8 +1,8 @@
-// optim.cu -- the optimizer step of clean_pufferl.train for small policies, ONE launch (sm_100a).
+// optim.cu -- the optimizer step of clean_pufferl.train for small policies, ONE launch (sm_90a).
 //
-// Replaces /root/reference/clean_pufferl.py:240-244
+// Replaces reference clean_pufferl.py:240-244
 //     torch.nn.utils.clip_grad_norm_(policy.parameters(), max_grad_norm);  optimizer.step()      (Adam, eps 1e-5)
-// which for the 17k-parameter models.Default is ~12 launches of 3-17 us each per minibatch (multi-tensor L2 norms,
+// which for the 17k-parameter models.Default is ~12 short launches per minibatch (multi-tensor L2 norms,
 // cleanup, reciprocal / clamp / multiply, fused Adam): latency, not work.  Here a single 1024-thread CTA makes two
 // passes over the gradients (<= 1 M elements): global L2 norm -> clip coefficient, then the Adam update with the
 // bias corrections of torch.optim.Adam(capturable=True): step counters, moments and parameters are the optimizer's

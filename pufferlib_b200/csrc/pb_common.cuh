@@ -1,4 +1,4 @@
-// pb_common.cuh -- shared helpers for libpuffer_b200.so (sm_100a only; no other arch is supported).
+// pb_common.cuh -- shared helpers for libpuffer_b200.so (sm_90a only; no other arch is supported).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,7 +37,7 @@ static inline int64_t pb_ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b
 __device__ __forceinline__ int64_t pb_ceil_div_dev(int64_t a, int64_t b) { return (a + b - 1) / b; }
 #endif
 
-// SM count of the current device (B200: 148 = 2 dies x 74), queried once per device; grids are sized in multiples of it
+// SM count of the current device (H100 SXM: 132), queried once per device; grids are sized in multiples of it
 int pb_num_sms();
 #define PB_NUM_SMS (pb_num_sms())
 

@@ -1,8 +1,8 @@
-// peer.cu -- gradient all-reduce over NVLink peer memory, fused into the optimizer step (sm_100a, one node).
+// peer.cu -- gradient all-reduce over NVLink peer memory, fused into the optimizer step (sm_90a, one node).
 //
 // The reference has no distributed path (SURVEY §8e); ours shards envs over the GPUs of one box and sums ONE flat
 // fp32 gradient buffer per optimizer step (17 157 floats = 68.6 KB for models.Default).  At that size an NCCL call is
-// pure launch / host latency (measured round 1: 16 calls per step outside the CUDA graph cost 1.4 ms of a 10 ms step),
+// pure launch / host latency (16 calls per step outside the CUDA graph),
 // so the exchange is done by the optimizer kernel itself: every rank owns a cudaMalloc'ed buffer mapped into all peers
 // (cudaIpc*), copies its gradients into it, raises a flag in every peer's buffer, waits for the peers' flags, and sums
 // all ranks' buffers in rank order with direct NVLink loads -- identical bits on every rank, no host involvement, so

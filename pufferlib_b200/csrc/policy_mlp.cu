@@ -1,6 +1,6 @@
 // policy_mlp.cu -- the rollout-time forward of models.Default fused with the sampling epilogue, ONE launch per env step.
 //
-// Replaces, inside the evaluate loop (/root/reference/clean_pufferl.py:107-117), the chain
+// Replaces, inside the evaluate loop (reference clean_pufferl.py:107-117), the chain
 //   encoder Linear + ReLU -> action head + value head (pufferlib/models.py:12-62) -> sample_logits
 //   (pufferlib/frameworks/cleanrl.py:25-47) -> Experience.store of value / logprob / action (clean_pufferl.py:443-446)
 // which the library path runs as 2 GEMM launches + sampler + counter update.  At rollout time M = num_envs rows (16384),
@@ -13,8 +13,8 @@
 //     fragment itself (the k order of the second product is permuted to match the C-fragment layout);
 //   * a quad shuffle gathers each row's 8 outputs, one lane per row does logsumexp / inverse-CDF sampling / logprob /
 //     entropy and writes action, logprob, value straight into the rollout rows.
-// Tensor-core path note: this is a 128x128x128 tile per CTA, far below the size where tcgen05/TMEM pays; the large
-// training GEMMs stay on cuBLAS (tcgen05 inside the library).
+// Tensor-core path note: this is a 128x128x128 tile per CTA, far below the size where a wgmma pipeline pays; the large
+// training GEMMs of the generic path stay on cuBLAS.
 #include "pb_common.cuh"
 #include "tma.cuh"
 

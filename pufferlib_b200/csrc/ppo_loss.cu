@@ -1,7 +1,7 @@
-// ppo_loss.cu -- the PPO minibatch loss of clean_pufferl.train, forward AND backward, in one pass (sm_100a).
+// ppo_loss.cu -- the PPO minibatch loss of clean_pufferl.train, forward AND backward, in one pass (sm_90a).
 //
-// Replaces /root/reference/clean_pufferl.py:202-238 plus the action-given branch of sample_logits
-// (/root/reference/pufferlib/frameworks/cleanrl.py:25-47) for one Discrete head:
+// Replaces reference clean_pufferl.py:202-238 plus the action-given branch of sample_logits
+// (reference pufferlib/frameworks/cleanrl.py:25-47) for one Discrete head:
 //     normalized = logits - logsumexp(logits);  newlogprob = normalized[action];  entropy = -sum(p * normalized)
 //     logratio = newlogprob - old_logprob;  ratio = exp(logratio)
 //     old_approx_kl = mean(-logratio);  approx_kl = mean((ratio - 1) - logratio);  clipfrac = mean(|ratio - 1| > clip)

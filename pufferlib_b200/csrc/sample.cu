@@ -1,6 +1,6 @@
-// sample.cu -- fused categorical sampling epilogue for one Discrete head (sm_100a).
+// sample.cu -- fused categorical sampling epilogue for one Discrete head (sm_90a).
 //
-// Replaces, for the sampling case, /root/reference/pufferlib/frameworks/cleanrl.py:25-47 (sample_logits):
+// Replaces, for the sampling case, reference pufferlib/frameworks/cleanrl.py:25-47 (sample_logits):
 //   normalized = logits - logsumexp(logits);  action ~ multinomial(softmax(normalized));
 //   logprob = normalized[action];  entropy = -sum(softmax * normalized)          (cleanrl.py:12-23)
 // and, optionally, the policy-output part of Experience.store (clean_pufferl.py:443-446) by writing action /

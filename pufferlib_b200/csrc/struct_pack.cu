@@ -1,8 +1,8 @@
-// struct_pack.cu -- batch pack / unpack of structured (Dict / Tuple) observations into C-aligned records (sm_100a).
+// struct_pack.cu -- batch pack / unpack of structured (Dict / Tuple) observations into C-aligned records (sm_90a).
 //
-// Replaces, for N samples at once on the device, /root/reference/pufferlib/extensions.pyx:19-30 (`emulate`: the
+// Replaces, for N samples at once on the device, reference pufferlib/extensions.pyx:19-30 (`emulate`: the
 // recursive per-leaf `np_struct[key][()] = sample` into an `np.dtype(..., align=True)` record,
-// /root/reference/pufferlib/emulation.py:68-80) and :32-49 (`nativize`, the inverse).  The layout (leaf byte offsets
+// reference pufferlib/emulation.py:68-80) and :32-49 (`nativize`, the inverse).  The layout (leaf byte offsets
 // and sizes incl. alignment padding) is computed on the host by pufferlib_b200/emulation.py with numpy's own rules.
 // One warp per record: lanes stride over the record's bytes, find the covering leaf (<= 32 leaves, warp-uniform
 // table in registers/constant bank) and move one byte each -- 32 consecutive bytes per warp request, so global

@@ -1,4 +1,4 @@
-// tma.cuh -- 1-D bulk async copies (TMA engine, SASS UBLKCP) + mbarrier helpers, inline PTX for sm_100a.
+// tma.cuh -- 1-D bulk async copies (TMA engine, SASS UBLKCP) + mbarrier helpers, inline PTX for sm_90a.
 // Used to stage whole image-observation rows through shared memory: global -> shared (mbarrier complete_tx),
 // shared -> global (bulk_group).  Addresses and sizes must be multiples of 16 bytes.
 #pragma once

@@ -1,12 +1,12 @@
-// train_prep.cu -- rollout-buffer write, minibatch construction and advantage normalisation (sm_100a).
+// train_prep.cu -- rollout-buffer write, minibatch construction and advantage normalisation (sm_90a).
 //
-// Replaces, from /root/reference/clean_pufferl.py:
+// Replaces, from reference clean_pufferl.py:
 //   :443-446  Experience.store (value / logprob / action rows)        -> pb_rollout_store
 //   :442      obs[ptr:end] = obs[indices] (all-True mask)            -> pb_copy_rows
 //   :466-482  Experience.flatten_batch (scalar tensors)              -> pb_flatten_batch
 //   :477      b_obs = obs[b_idxs_obs]                                 -> pb_minibatch_gather (LSU path; TMA path in image.cu)
 //   :211-213  per-minibatch advantage normalisation                   -> pb_adv_norm
-// All of these are HBM-bound byte movers: coalesced, vectorised, grid sized in multiples of the 148 SMs.
+// All of these are HBM-bound byte movers: coalesced, vectorised, grid sized in multiples of the SM count.
 #include "pb_common.cuh"
 
 namespace {

@@ -1,14 +1,14 @@
 """Structured observation layout + device-side pack / unpack (SURVEY §8 row a-4).
 
 Mirrors, with the same names and results:
-  /root/reference/pufferlib/emulation.py:68-80    dtype_from_space   (np.dtype(..., align=True) C-struct layout)
-  /root/reference/pufferlib/emulation.py:82-94    flatten_space
-  /root/reference/pufferlib/emulation.py:96-112   emulate_observation_space (flat Box of the common leaf dtype / uint8)
-  /root/reference/pufferlib/pytorch.py:48-100     nativize_dtype -> (torch dtype, shape, offset, delta) tree
-  /root/reference/pufferlib/pytorch.py:103-145    nativize_tensor (zero-copy typed views of the flat batch)
-  /root/reference/pufferlib/extensions.pyx:19-30  emulate  -> ``emulate_batch``: N samples at once on the device
+  reference pufferlib/emulation.py:68-80    dtype_from_space   (np.dtype(..., align=True) C-struct layout)
+  reference pufferlib/emulation.py:82-94    flatten_space
+  reference pufferlib/emulation.py:96-112   emulate_observation_space (flat Box of the common leaf dtype / uint8)
+  reference pufferlib/pytorch.py:48-100     nativize_dtype -> (torch dtype, shape, offset, delta) tree
+  reference pufferlib/pytorch.py:103-145    nativize_tensor (zero-copy typed views of the flat batch)
+  reference pufferlib/extensions.pyx:19-30  emulate  -> ``emulate_batch``: N samples at once on the device
                                                   (pb_struct_pack gathers the leaf tensors into C-aligned records)
-  /root/reference/pufferlib/extensions.pyx:32-49  nativize -> ``nativize_batch`` (pb_struct_unpack)
+  reference pufferlib/extensions.pyx:32-49  nativize -> ``nativize_batch`` (pb_struct_unpack)
 The layout functions are pure host logic (numpy); the batch pack / unpack are CUDA kernels behind the C ABI.
 """
 import ctypes as C

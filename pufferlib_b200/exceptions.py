@@ -1,4 +1,4 @@
-"""Same exception names and meaning as /root/reference/pufferlib/exceptions.py."""
+"""Same exception names and meaning as reference pufferlib/exceptions.py."""
 
 
 class APIUsageError(RuntimeError):

@@ -1,6 +1,6 @@
 """``pufferlib.frameworks.cleanrl`` equivalent: logits -> action / logprob / entropy, and the Policy wrapper.
 
-Reference: /root/reference/pufferlib/frameworks/cleanrl.py:25-47 (sample_logits), :50-66 (Policy).
+Reference: reference pufferlib/frameworks/cleanrl.py:25-47 (sample_logits), :50-66 (Policy).
 ``sample_logits`` is the plain torch formulation (used in train, where actions are given);
 ``Policy(fused_sample=True)`` routes the sampling case through the fused CUDA epilogue pb_sample_logits.
 """

@@ -1,9 +1,9 @@
 """Policies for the configs in BASELINE.json: PyTorch modules, dense GEMMs on cuBLAS/cuDNN (tensor cores).
 
 Same architecture and call convention as the reference (adjacent to the hot path, not rewritten):
-  Default        /root/reference/pufferlib/models.py:12-62   Linear(prod(obs)->hidden)+ReLU; heads hidden->n_act, ->1
-  Convolutional  /root/reference/pufferlib/models.py:113-157 NatureCNN for (4,84,84) uint8 (atari/torch.py:8-18)
-  layer_init     /root/reference/pufferlib/pytorch.py:193-199
+  Default        reference pufferlib/models.py:12-62   Linear(prod(obs)->hidden)+ReLU; heads hidden->n_act, ->1
+  Convolutional  reference pufferlib/models.py:113-157 NatureCNN for (4,84,84) uint8 (atari/torch.py:8-18)
+  layer_init     reference pufferlib/pytorch.py:193-199
 """
 import numpy as np
 import torch
@@ -75,7 +75,7 @@ class _DefaultMLPFunction(torch.autograd.Function):
         db_enc = grads[8 * hid:9 * hid]
         db_cat = grads[9 * hid:]
         # dW_enc = dPre^T @ x is one 128x128 output tile with K = M: as a batched GEMM over 64 K-slices (+ a 64-way sum)
-        # the library GEMM runs at the HBM roofline (91 us vs 193 us at M = 524288; profiles/tools/gemm_variants.py)
+        # gives the library GEMM enough parallel work at this shape
         split = 64
         if x.dim() == 3:            # slab form: the K-slices tile each slab, partial products into one buffer
             g_, r_, f_ = x.shape

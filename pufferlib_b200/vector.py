@@ -1,6 +1,6 @@
 """``pufferlib.vector`` surface for device-resident envs: make / reset / step / send / recv.
 
-Mirrors /root/reference/pufferlib/vector.py: ``make`` (:577-637) with the same validation and error
+Mirrors reference pufferlib/vector.py: ``make`` (:577-637) with the same validation and error
 messages, module-level ``reset``/``step`` (:44-53), the RESET/SEND/RECV flag protocol and prechecks (:17-42),
 ``joint_space`` (:55-68), ``make_seeds`` (:639-650) and the ``Serial`` object surface (:70-166).  The backend
 class ``B200`` replaces Serial/Multiprocessing: instead of N Python env objects stepped in a loop it owns one
@@ -356,7 +356,7 @@ class B200:
     def actions_to_host(self, actions):
         """Device actions -> the pinned host action array (async, on the caller's stream); valid after host_sync()."""
         # a kernel store into the pinned (UVA-mapped) host array, not a DMA copy: the copy engine is busy with the 8 MB
-        # observation blocks of this and earlier steps, and a 128 KB cudaMemcpyAsync would queue behind them (150 us per step)
+        # observation blocks of this and earlier steps, and a 128 KB cudaMemcpyAsync would queue behind them
         a = actions.reshape(-1)
         if a.dtype != torch.int64 or not a.is_contiguous():
             a = a.to(torch.int64).contiguous()

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(REPO, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100; run with -m gpu)')
 
 
 def load_golden(name):

@@ -1,11 +1,11 @@
-"""Hardware check of the fused tcgen05 minibatch-update kernel (csrc/mlp_update.cu).
+"""Hardware check of the fused wgmma minibatch-update kernel (csrc/mlp_update.cu).
 
 Stage-wise: every stage's reference is computed from the kernel's OWN previous-stage dump (hidden -> dOut -> dPre ->
 gradients), so a mismatch names the stage that is wrong; then an end-to-end comparison against the validated chain
 (cuBLAS GEMMs + pb_ppo_loss + pb_mlp_tail_backward + dW GEMM), then timing at the bench minibatch.  Not collected by
-pytest; run on a B200 box under a timeout:
+pytest (tests/test_gpu_update_kernel.py drives `case`); run by hand on an H100 under a timeout:
 
-    gpurun --timeout 300 -- 'timeout 200 python tests/experimental/check_mlp_update_fused.py'
+    timeout 200 python tests/experimental/check_mlp_update_fused.py [--variant 1|2]
 """
 import ctypes as C
 import os
@@ -96,9 +96,9 @@ def case(slab_rows, n_slabs, slab_stride, n_act, seed):
                                      ret, oval, n_act, debug=True)
     torch.cuda.synchronize()
     ok = True
-    # stage 1: forward UMMA (TF32 = truncated operands, fp32 accumulate) + bias + ReLU
+    # stage 1: forward wgmma (TF32 = truncated operands, fp32 accumulate) + bias + ReLU
     h_ref = torch.relu(trunc_tf32(x).double() @ trunc_tf32(w_enc).double().t() + b_enc.double())
-    ok &= check('hidden (forward UMMA)', dh, h_ref, 2e-5)
+    ok &= check('hidden (forward wgmma)', dh, h_ref, 2e-5)
     # stage 2: heads + loss from the kernel's own hidden
     if TF32_EPILOGUE:        # the kernel's heads product takes TF32-truncated operands (mma.sync), fp32 accumulation
         out = (trunc_tf32(dh).double() @ rna_tf32(w_cat).double().t() + b_cat.double()).float()
@@ -117,7 +117,7 @@ def case(slab_rows, n_slabs, slab_stride, n_act, seed):
     dw_enc = gflat[:128 * 128].view(128, 128)
     tail = gflat[128 * 128:]
     dw_heads, db_enc, db_heads = tail[:1024].view(8, 128), tail[1024:1152], tail[1152:]
-    ok &= check('dW_enc (MN-major UMMA)', dw_enc, trunc_tf32(dp).double().t() @ trunc_tf32(x).double(), 2e-5)
+    ok &= check('dW_enc (wgmma)', dw_enc, rna_tf32(dp).double().t() @ rna_tf32(x).double(), 2e-5)   # operands rounded to nearest
     ok &= check('dW_heads (mma.sync)', dw_heads, (trunc_tf32(do).double().t() @ trunc_tf32(dh).double()) if TF32_EPILOGUE else
                 (rna_tf32(do).double().t() @ rna_tf32(dh).double()), 2e-5)
     ok &= check('db_enc', db_enc, dp.double().sum(0), 2e-5)

@@ -4,7 +4,7 @@
 
 Sizes are tiny on purpose (the tools slow kernels down 10-100x); every kernel family of the hot path is launched at least
 once: env steps, GAE (single-pass tile kernel and the general one), train-prep, PPO loss, policy step, tail backward,
-clip+Adam, the fused tcgen05 update and the persistent rollout."""
+clip+Adam, the fused wgmma update and the persistent rollout."""
 import os
 import sys
 

@@ -1,13 +1,16 @@
-"""Generate golden vectors by running the UNMODIFIED reference (/root/reference) in this container.
+"""Generate golden vectors by running the UNMODIFIED reference (a PufferLib source checkout named by PUFFERLIB_REFERENCE).
 
-    python tests/golden/generate.py        # writes tests/golden/*.npz
+    PUFFERLIB_REFERENCE=<checkout> python tests/golden/generate.py        # writes tests/golden/*.npz
 
-The reference cannot travel to the GPU box, so its outputs are committed here as small fixtures:
+The tests must not need the reference, so its outputs are committed here as small fixtures:
 
   squared_*.npz     pufferlib.vector.make(ocean.env_creator('squared'), backend=Serial) driven by a fixed
                     action tape (np.random.default_rng(0)); every recv() row (obs/reward/terminal/trunc/mask)
                     and every info dict.                        [vector.py:70-166, ocean.py:406-513]
   gae.npz           c_gae.compute_gae (the reference's Cython, built by pyximport) on seeded inputs.
+  c_gae_samples.npz the same function (compiled by oracle/build_ref.py) on the inputs of test_gpu_gae.py and
+                    test_oracle_golden.py that compare against it: whole outputs up to 8192 elements, else a fixed
+                    seeded sample of 8192 positions (index + value).
   experience_*.npz  clean_pufferl.Experience store -> sort_training_data -> compute_gae -> flatten_batch and
                     the per-minibatch advantage normalisation of clean_pufferl.train (torch CPU fp32).
 
@@ -19,7 +22,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
-sys.path[:0] = [os.path.join(REPO, 'oracle', 'shim'), '/root/reference']
+sys.path[:0] = [os.path.join(REPO, 'oracle', 'shim'), os.environ['PUFFERLIB_REFERENCE']]
 
 import warnings
 warnings.filterwarnings('ignore')
@@ -233,7 +236,46 @@ def gen_lstm():
           'params', sum(v.size for k, v in out.items() if k.startswith('init/')))
 
 
+C_GAE_SAMPLE = 8192
+# (h, n, seed, p_done, gamma, lam): test_gpu_gae.test_gae_vs_reference_compiled_c_gae (time-major [h, n] inputs)
+C_GAE_DEVICE_CASES = [(128, 64, 7 * 128 + 64, 0.02, 0.99, 0.95), (256, 1024, 7 * 256 + 1024, 0.01, 0.99, 0.95),
+                      (4096, 1, 7 * 4096 + 1, 0.05, 0.9, 0.8), (16, 333, 7 * 16 + 333, 0.2, 1.0, 1.0),
+                      (128, 16384, 7 * 128 + 16384, 0.01, 0.99, 0.95)]
+# (n, p_done, gamma, lam): test_oracle_golden.test_gae_oracle_vs_reference_compiled_c_gae (flat inputs, seed = n)
+C_GAE_FLAT_CASES = [(2, 0.0, 0.99, 0.95), (1000, 0.02, 0.99, 0.95), (50000, 0.1, 0.9, 0.5), (4096, 1.0, 0.99, 0.95),
+                    (4096, 0.0, 1.0, 1.0)]
+
+
+def c_gae_sample(out, key, ref, seed):
+    ref = np.asarray(ref, dtype=np.float32)
+    if ref.size <= C_GAE_SAMPLE:
+        idx = np.arange(ref.size, dtype=np.int32)
+    else:
+        idx = np.sort(np.random.default_rng(seed).choice(ref.size, C_GAE_SAMPLE, replace=False)).astype(np.int32)
+    out[key + '_idx'], out[key + '_adv'] = idx, ref[idx]
+
+
+def gen_c_gae_samples():
+    sys.path.insert(0, REPO)
+    from oracle import build_ref
+    build_ref.build()
+    cg = build_ref.load()
+    out = {}
+    for k, (h, n, seed, p_done, gamma, lam) in enumerate(C_GAE_DEVICE_CASES):
+        rng = np.random.default_rng(seed)                       # test_gpu_gae.make_inputs
+        r = rng.standard_normal((h, n)).astype(np.float32)
+        v = rng.standard_normal((h, n)).astype(np.float32)
+        d = (rng.random((h, n)) < p_done).astype(np.float32)
+        rs, vs, ds = (np.ascontiguousarray(x.T).reshape(-1) for x in (r, v, d))
+        c_gae_sample(out, f'device{k}', cg.compute_gae(ds, vs, rs, gamma, lam), seed)
+    for k, (n, p_done, gamma, lam) in enumerate(C_GAE_FLAT_CASES):
+        d, v, r = gae_inputs(n, n, p_done)
+        c_gae_sample(out, f'flat{k}', cg.compute_gae(d, v, r, gamma, lam), n)
+    np.savez_compressed(os.path.join(HERE, 'c_gae_samples.npz'), **out)
+
+
 if __name__ == '__main__':
+    gen_c_gae_samples()
     gen_squared()
     gen_squared_multiprocessing()
     cg = gen_gae()

@@ -1,7 +1,7 @@
 """2-rank hardware check of the NVLink peer-memory all-reduce and the one-graph multi-GPU update (torchrun):
 
-    gpurun --gpus 2 --timeout 600 -- 'timeout 300 python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 \
-        --master-addr 127.0.0.1 --master-port 29511 tests/multi_gpu/check_peer_update.py'
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 \
+        tests/multi_gpu/check_peer_update.py
 
 1. PeerComm.all_reduce_ against torch.distributed.all_reduce (NCCL) on random buffers, 200 back-to-back calls, eager and
    inside a CUDA graph (bit-identical results on both ranks).

@@ -1,5 +1,5 @@
 """Host-side structured-observation layout vs the reference's own known-answer vectors
-(/root/reference/tests/test_pytorch.py:14-134, copied here as expected VALUES -- they are test data, not code) and vs
+(reference tests/test_pytorch.py:14-134, copied here as expected VALUES -- they are test data, not code) and vs
 numpy's aligned-struct rules (pufferlib/emulation.py:68-80)."""
 import numpy as np
 import pytest

@@ -150,7 +150,7 @@ def test_manual_update_matches_autograd_update():
 
 @pytest.mark.parametrize('dw', ['cublas', 'kernel'])
 def test_fused_update_kernel_matches_kernel_chain(dw):
-    """train() through pb_mlp_update_fused (ONE tcgen05 kernel per minibatch: csrc/mlp_update.cu) vs the kernel chain it
+    """train() through pb_mlp_update_fused (ONE wgmma kernel per minibatch: csrc/mlp_update.cu) vs the kernel chain it
     replaces (cuBLAS GEMMs + pb_ppo_loss + pb_mlp_tail_backward + split-K dW): same rollout, same minibatches.  Both
     compute the dense products in TF32 (operands truncated by the tensor core), so gradients agree to TF32 noise; the
     statistics come from the same row math."""

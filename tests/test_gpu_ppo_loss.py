@@ -1,5 +1,5 @@
 """pb_ppo_loss (one-pass PPO loss forward + analytic backward) vs the torch fp32 formulation of
-/root/reference/clean_pufferl.py:202-238 differentiated by autograd.  Tolerance: 1e-5 relative on the loss and the
+reference clean_pufferl.py:202-238 differentiated by autograd.  Tolerance: 1e-5 relative on the loss and the
 statistics, 1e-5 * max|grad| absolute on the gradients (fp32 expf / logf vs ATen's; no reordering beyond the sums)."""
 import pytest
 import torch

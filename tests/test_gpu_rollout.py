@@ -2,7 +2,7 @@
 in one launch.  Env rows must replay bit-exactly through the oracle with the actions the kernel sampled (same dynamics,
 same bound-rollout row convention, carry-over between rollouts); policy outputs are checked against fp64 torch math on the
 stored observations (the encoder product is TF32 on the tensor core), and the sampled actions against the inverse CDF of
-the counter-based uniform.  Reference loop: /root/reference/clean_pufferl.py:84-124."""
+the counter-based uniform.  Reference loop: reference clean_pufferl.py:84-124."""
 import numpy as np
 import pytest
 import torch

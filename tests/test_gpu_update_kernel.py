@@ -1,8 +1,8 @@
 """pb_mlp_update_fused through the C ABI, stage by stage (tests/experimental/check_mlp_update_fused.py has the details):
-forward UMMA vs TF32-truncated fp64 math, dOut / statistics vs pb_ppo_loss on the kernel's own head outputs, dPre, and every
+forward wgmma vs TF32-truncated fp64 math, dOut / statistics vs pb_ppo_loss on the kernel's own head outputs, dPre, and every
 gradient section vs fp64 products of the kernel's own dumps; then the same launch without dumps, and the dPre-to-HBM mode.
 Shapes: one tile, a ragged tile count, more tiles than SMs, several slabs with gaps (the zero-copy minibatch layout), 1 / 4 / 7
-actions.  Reference of the math: /root/reference/clean_pufferl.py:186-244 with the policy of pufferlib/models.py:12-62."""
+actions.  Reference of the math: reference clean_pufferl.py:186-244 with the policy of pufferlib/models.py:12-62."""
 import os
 import sys
 

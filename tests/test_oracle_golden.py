@@ -122,19 +122,20 @@ def test_experience_validation_errors():
         oexp.Experience(100, 3, 50, (7, 7), np.float32)
 
 
-@pytest.mark.parametrize('n,p_done,gamma,lam', [(2, 0.0, 0.99, 0.95), (1000, 0.02, 0.99, 0.95), (50000, 0.1, 0.9, 0.5),
-                                                (4096, 1.0, 0.99, 0.95), (4096, 0.0, 1.0, 1.0)])
-def test_gae_oracle_vs_reference_compiled_c_gae(n, p_done, gamma, lam):
-    """The oracle's C restatement against the reference's own c_gae.pyx compiled from /root/reference (oracle/_ref):
-    bit for bit, at sizes the golden file does not hold."""
-    from oracle import build_ref
-    ref_mod = build_ref.load()
-    if ref_mod is None:
-        pytest.skip('oracle/_ref not built (no /root/reference at build time)')
+C_GAE_FLAT_CASES = [(2, 0.0, 0.99, 0.95), (1000, 0.02, 0.99, 0.95), (50000, 0.1, 0.9, 0.5), (4096, 1.0, 0.99, 0.95),
+                    (4096, 0.0, 1.0, 1.0)]       # the order of tests/golden/generate.py: case k is stored as flat{k}
+
+
+@pytest.mark.parametrize('n,p_done,gamma,lam', C_GAE_FLAT_CASES)
+def test_gae_oracle_vs_reference_compiled_c_gae(golden, n, p_done, gamma, lam):
+    """The oracle's C restatement against the reference's own c_gae.pyx (its outputs stored in
+    tests/golden/c_gae_samples.npz by tests/golden/generate.py): bit for bit, at sizes the golden gae file does not hold."""
+    g = golden('c_gae_samples')
+    k = C_GAE_FLAT_CASES.index((n, p_done, gamma, lam))
     d, v, r = gae_inputs(n, seed=n, p_done=p_done)
-    ref = np.asarray(ref_mod.compute_gae(d, v, r, gamma, lam))
     got = ogae.compute_gae(d, v, r, gamma, lam)
-    assert np.array_equal(ref.view(np.uint32), got.view(np.uint32))
+    idx, ref = g[f'flat{k}_idx'], g[f'flat{k}_adv']
+    assert np.array_equal(ref.view(np.uint32), got[idx].view(np.uint32))
 
 
 @pytest.mark.parametrize('case', ['squared_mp_n8_w2', 'squared_mp_n12_w4'])

@@ -233,6 +233,34 @@ int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const float* w_en
                          int32_t n_act, uint64_t seed, uint64_t* counter_dev, uint32_t* ticket_dev, int64_t* actions,
                          float* logprobs, float* values, float* entropies, void* stream);
 
+/* -- fused rollout-time recurrent policy step ------------------------------------------------------------------------
+ * For LSTMWrapper(models.Default) with one LSTM layer of input and hidden size 128 (pufferlib/models.py:64-111, the
+ * recurrent wrapper of cleanrl.py:69-93) at rollout time (clean_pufferl.py:100-117): encoder Linear + ReLU, the LSTM cell,
+ * both heads, sample_logits (frameworks/cleanrl.py:25-47), the value / logprob / action row stores and the in-place
+ * lstm_h / lstm_c update in ONE launch per env step (mma.sync TF32 tensor-core tiles, fp32 accumulate; the gates never
+ * leave the SM).  Per row r < m:
+ *   e = relu(x W_enc^T + b_enc);  z = e W_ih^T + h W_hh^T + b_ih + b_hh  (gate order i, f, g, o);
+ *   c' = sigmoid(f) c + sigmoid(i) tanh(g);  h' = sigmoid(o) tanh(c');  out = h' W_cat^T + b_cat.
+ * obs: [m] rows of in_features (<= 128) fp32, obs_stride floats apart (no alignment needed).  h, c: [m][128] fp32,
+ * h_stride / c_stride floats apart (even, 8-byte aligned), read and then overwritten in place; the state is not reset on
+ * done (as clean_pufferl.py:100-105).  Packed operands (models.LSTMWrapper.fused_operands builds them):
+ *   w_enc   [128][136]        W_enc rounded to TF32 (cvt.rna), columns past in_features zero;
+ *   b_enc   [128];
+ *   w_gates [16][32][264]     chunk ch, row 8j + u = gate j (i, f, g, o) of hidden unit 8ch + u, i.e. row 128j + 8ch + u of
+ *                             [W_ih | W_hh] (weight_ih_l0 | weight_hh_l0), columns 0..127 from W_ih, 128..255 from W_hh,
+ *                             256..263 zero; rounded to TF32 (cvt.rna); 16-byte aligned;
+ *   b_gates [16][32]          b_ih + b_hh in the same chunk order;
+ *   w_heads [n_out][128], b_heads [n_out]: n_act logit rows | value row | zero rows, n_out = n_act + 1 rounded up to 8.
+ * Sampling: the counter-based inverse CDF of pb_policy_mlp_sample on (seed, *counter_dev, row); with a non-null ticket_dev
+ * the last CTA advances *counter_dev by 1.  Rows >= m are never read or written.  PB_ERR_UNSUPPORTED for in_features > 128,
+ * input_size or hidden_size != 128, n_act > 15. */
+int pb_policy_lstm_sample(const float* obs, int64_t obs_stride, int32_t in_features, const float* w_enc,
+                          const float* b_enc, const float* w_gates, const float* b_gates, const float* w_heads,
+                          const float* b_heads, float* h, int64_t h_stride, float* c, int64_t c_stride, int64_t m,
+                          int32_t input_size, int32_t hidden_size, int32_t n_act, uint64_t seed, uint64_t* counter_dev,
+                          uint32_t* ticket_dev, int64_t* actions, float* logprobs, float* values, float* entropies,
+                          void* stream);
+
 /* -- persistent rollout (env steps with the policy in the loop) -------------------------------------------------------
  * The H-iteration body of clean_pufferl.evaluate (clean_pufferl.py:84-124: recv -> policy -> store -> send) for a
  * breakout handle and models.Default (128 features, 128 hidden, n_act <= 4) in ONE launch: a CTA owns 128 envs for all

@@ -79,6 +79,9 @@ SIGNATURES = {
                     C.c_int64, C.c_void_p, C.c_void_p]),
     'pb_policy_mlp_sample': (C.c_int, [C.c_void_p, C.c_int64] + [C.c_void_p] * 4 + [C.c_int64, C.c_int32, C.c_int32,
                              C.c_int32, C.c_uint64] + [C.c_void_p] * 6 + [C.c_void_p]),
+    'pb_policy_lstm_sample': (C.c_int, [C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 6 + [C.c_void_p, C.c_int64,
+                              C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_uint64]
+                              + [C.c_void_p] * 6 + [C.c_void_p]),
     'pb_mlp_tail_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int32]),
     'pb_mlp_tail_backward': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
                              C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -789,7 +789,7 @@ def create(config, vecenv, policy, optimizer=None, wandb=None):
         optimizer = torch.optim.Adam(policy.parameters(), lr=lr, eps=1e-5, fused=True, capturable=graphed)
 
     model = getattr(policy, 'policy', None)
-    if hasattr(model, 'invalidate_cache'):      # cached head matrix of models.Default: stale after every optimizer step
+    if hasattr(model, 'invalidate_cache'):      # cached head matrix / packed operands: stale after every optimizer step
         optimizer.register_step_post_hook(lambda *a, **k: model.invalidate_cache())
 
     grad_bucket = None
@@ -852,13 +852,20 @@ def _rollout_loop(data, infos):
                 # clean_pufferl.py:100-105: h = lstm_h[:, env_id] -> policy -> lstm_h[:, env_id] = h.  env_id is a
                 # contiguous range here (every env, or one pool group): slices instead of index gathers
                 lo, hi = int(env_id[0]), int(env_id[0]) + len(env_id)
+                fused = data.fused_rows and experience.num_envs is not None
                 if lo == 0 and hi == experience.lstm_h.shape[1]:
                     h_in, c_in = experience.lstm_h, experience.lstm_c
+                elif fused:     # the fused step updates the slices in place
+                    h_in, c_in = experience.lstm_h[:, lo:hi], experience.lstm_c[:, lo:hi]
                 else:
                     h_in, c_in = experience.lstm_h[:, lo:hi].contiguous(), experience.lstm_c[:, lo:hi].contiguous()
-                actions, logprob, _, value, (h, c) = policy(o_device, (h_in, c_in))
-                experience.lstm_h[:, lo:hi].copy_(h)
-                experience.lstm_c[:, lo:hi].copy_(c)
+                if fused:
+                    actions, logprob, _, value, (h, c) = policy(o_device, (h_in, c_in), out=experience.rows())
+                else:
+                    actions, logprob, _, value, (h, c) = policy(o_device, (h_in, c_in))
+                if h.data_ptr() != h_in.data_ptr() or c.data_ptr() != c_in.data_ptr():   # not updated in place
+                    experience.lstm_h[:, lo:hi].copy_(h)
+                    experience.lstm_c[:, lo:hi].copy_(c)
             elif data.fused_rows and experience.num_envs is not None:
                 actions, logprob, _, value = policy(o_device, out=experience.rows())
             else:

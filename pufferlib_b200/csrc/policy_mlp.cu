@@ -16,6 +16,7 @@
 // Tensor-core path note: this is a 128x128x128 tile per CTA, far below the size where a wgmma pipeline pays; the large
 // training GEMMs of the generic path stay on cuBLAS.
 #include "pb_common.cuh"
+#include "policy_sample.cuh"
 #include "tma.cuh"
 
 namespace {
@@ -24,16 +25,6 @@ constexpr int PM_K = 128;           // obs features
 constexpr int PM_H = 128;           // hidden units
 constexpr int PM_PITCH = PM_K + 8;  // shared row pitch in floats (544 B): conflict-free 64-bit fragment loads
 
-__device__ __forceinline__ uint32_t to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return r;
-}
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 struct PolicyParams {
     const float* obs; int64_t obs_stride;      // [M][128] fp32
     const float* w_enc; const float* b_enc;    // [128][128], [128]
@@ -137,34 +128,9 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
             float z[8];
 #pragma unroll
             for (int k = 0; k < 8; ++k) z[k] = t ? rowv[1][k] : rowv[0][k];
-            float mx = -INFINITY;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) if (k < p.n_act) mx = fmaxf(mx, z[k]);
-            float sum = 0.f;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) if (k < p.n_act) sum += expf(z[k] - mx);
-            const float lse = mx + logf(sum);
-            const uint32_t rnd = pb_mix32(p.seed * 0x9E3779B97F4A7C15ull + offset * 0xD1B54A32D192ED03ull +
-                                          (uint64_t)r * 0x2545F4914F6CDD1Dull);
-            const float u = (float)(rnd >> 8) * (1.0f / 16777216.0f);
-            float cdf = 0.f, ent = 0.f, lp = 0.f, value = 0.f;
-            int a = -1;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                if (k < p.n_act) {
-                    const float nl = z[k] - lse, pk = expf(nl);
-                    ent -= pk * nl;
-                    cdf += pk;
-                    if (a < 0 && u < cdf) { a = k; lp = nl; }
-                }
-                if (k == p.n_act) value = z[k];
-            }
-            if (a < 0) {   // rounding left cdf a hair below u: last action with non-negligible probability
-#pragma unroll
-                for (int k = 7; k >= 0; --k)
-                    if (a < 0 && k < p.n_act && z[k] - lse > -80.f) { a = k; lp = z[k] - lse; }
-                if (a < 0) { a = p.n_act - 1; lp = z[a] - lse; }
-            }
+            int a;
+            float lp, ent, value;
+            pb_sample_row<8>(z, p.n_act, pb_policy_uniform(p.seed, offset, r), a, lp, ent, value);
             p.actions[r] = a;
             p.logprobs[r] = lp;
             p.values[r] = value;

@@ -125,11 +125,19 @@ class Policy(torch.nn.Module):
 
 class RecurrentPolicy(torch.nn.Module):
     """Wrap a recurrent model (reference: pufferlib/frameworks/cleanrl.py:69-93):
-    forward(x, state=None, action=None) -> (action, logprob, entropy, value, state)."""
+    forward(x, state=None, action=None, out=None) -> (action, logprob, entropy, value, state).
 
-    def __init__(self, policy):
+    ``fused_sample=True``: when sampling under no_grad with a model pb_policy_lstm_sample supports
+    (models.LSTMWrapper.fused_supported), the whole step -- encoder, LSTM cell, heads, sampling, row stores -- is ONE
+    kernel and ``state`` is updated in place and returned.  Anything else takes the unfused path."""
+
+    def __init__(self, policy, fused_sample=False, seed=0):
         super().__init__()
         self.policy = policy
+        self.fused_sample = fused_sample
+        self._seed = int(seed)
+        self._counter = None     # device-side draw counter: CUDA-graph replays keep drawing fresh numbers
+        self._ticket = None      # exit ticket of pb_policy_lstm_sample (its last CTA advances the counter)
 
     @property
     def lstm(self):
@@ -139,10 +147,54 @@ class RecurrentPolicy(torch.nn.Module):
             return self.policy.lstm
         raise ValueError('Policy must have a subnetwork named lstm or recurrent')
 
-    def get_action_and_value(self, x, state=None, action=None):
+    def get_action_and_value(self, x, state=None, action=None, out=None):
+        """``out`` (optional, fused sampling only): (values_row, logprobs_row, actions_row) rollout row views the kernel
+        writes into directly."""
+        if action is None and self.fused_sample and not torch.is_grad_enabled():
+            fused = self._policy_step_fused(x, state, out)
+            if fused is not None:
+                return fused
+            if state is not None:      # rollout slices lstm_h[:, lo:hi] of a multi-layer state are strided views
+                state = tuple(s.contiguous() for s in state)
         logits, value, state = self.policy(x, state)
         action, logprob, ent = sample_logits(logits, action)
         return action, logprob, ent, value, state
 
-    def forward(self, x, state=None, action=None):
-        return self.get_action_and_value(x, state, action)
+    def _policy_step_fused(self, x, state, out=None):
+        """LSTMWrapper(models.Default) step as ONE kernel (pb_policy_lstm_sample); None if it does not apply."""
+        model = self.policy
+        if not (hasattr(model, 'fused_operands') and model.fused_supported(x)):
+            return None
+        n, dev = x.shape[0], x.device
+        x2 = x.reshape(n, -1)
+        if x2.stride(1) != 1:
+            return None
+        if state is None:
+            state = (torch.zeros(1, n, 128, device=dev), torch.zeros(1, n, 128, device=dev))
+        h, c = state
+        for s in (h, c):     # [1, n, 128] fp32 rows (a slice lstm_h[:, lo:hi] of the rollout state is fine)
+            if not (s.dim() == 3 and tuple(s.shape) == (1, n, 128) and s.dtype == torch.float32 and s.device == dev
+                    and s.stride(2) == 1 and s.stride(1) % 2 == 0 and s.data_ptr() % 8 == 0):
+                return None
+        if out is None:
+            value = torch.empty(n, dtype=torch.float32, device=dev)
+            logprob = torch.empty(n, dtype=torch.float32, device=dev)
+            actions = torch.empty(n, dtype=torch.int64, device=dev)
+        else:
+            value, logprob, actions = (t[:n] for t in out)
+        ent = torch.empty(n, dtype=torch.float32, device=dev)
+        if self._counter is None:
+            self._counter = torch.zeros(1, dtype=torch.int64, device=dev)
+        if self._ticket is None:
+            self._ticket = torch.zeros(1, dtype=torch.int32, device=dev)
+        w_enc, b_enc, w_gates, b_gates, w_cat, b_cat = model.fused_operands()
+        n_act = model.policy.decoder.weight.shape[0]
+        _native.check(_native.lib().pb_policy_lstm_sample(
+            _native.ptr(x2), x2.stride(0), x2.shape[1], _native.ptr(w_enc), _native.ptr(b_enc), _native.ptr(w_gates),
+            _native.ptr(b_gates), _native.ptr(w_cat), _native.ptr(b_cat), _native.ptr(h), h.stride(1), _native.ptr(c),
+            c.stride(1), n, 128, 128, n_act, C.c_uint64(self._seed), _native.ptr(self._counter), _native.ptr(self._ticket),
+            _native.ptr(actions), _native.ptr(logprob), _native.ptr(value), _native.ptr(ent), _native.stream_ptr()))
+        return actions, logprob, ent, value, (h, c)
+
+    def forward(self, x, state=None, action=None, out=None):
+        return self.get_action_and_value(x, state, action, out)

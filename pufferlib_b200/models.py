@@ -95,6 +95,12 @@ class _DefaultMLPFunction(torch.autograd.Function):
                 db_cat[n_act:n_act + 1], None)
 
 
+def _round_tf32(w):
+    """fp32 -> nearest TF32 value (ties away from zero: cvt.rna), kept as fp32 bits."""
+    bits = w.detach().contiguous().view(torch.int32)
+    return ((bits + 0x1000) & ~0x1FFF).view(torch.float32)
+
+
 def layer_init(layer, std=np.sqrt(2), bias_const=0.0):
     torch.nn.init.orthogonal_(layer.weight, std)
     torch.nn.init.constant_(layer.bias, bias_const)
@@ -116,17 +122,19 @@ class Default(nn.Module):
         self._head_cache.clear()
 
     def head_matrix(self):
-        """(w_cat [8, H], b_cat [8]): n_act logit rows | value row | zero padding; cached under no_grad."""
+        """(w_cat [R, H], b_cat [R]): n_act logit rows | value row | zero padding up to R = the next multiple of 8 rows
+        (8 for n_act <= 7); cached under no_grad."""
         cache = self._head_cache
         key = (self.decoder.weight.data_ptr(), torch.cuda.is_current_stream_capturing())
         if not torch.is_grad_enabled() and cache.get('key') == key:
             return cache['w'], cache['b']
         n_act, hid = self.decoder.weight.shape
+        rows = -(-(n_act + 1) // 8) * 8
         with torch.no_grad():
-            w_cat = self.decoder.weight.new_zeros(8, hid)
+            w_cat = self.decoder.weight.new_zeros(rows, hid)
             w_cat[:n_act] = self.decoder.weight
             w_cat[n_act] = self.value_head.weight[0]
-            b_cat = self.decoder.weight.new_zeros(8)
+            b_cat = self.decoder.weight.new_zeros(rows)
             b_cat[:n_act] = self.decoder.bias
             b_cat[n_act] = self.value_head.bias[0]
         if not torch.is_grad_enabled():
@@ -215,6 +223,54 @@ class LSTMWrapper(nn.Module):
                 nn.init.constant_(param, 0)
             elif 'weight' in name:
                 nn.init.orthogonal_(param, 1.0)
+        self._fused_cache = {}
+
+    def invalidate_cache(self):
+        """Call after the parameters changed (clean_pufferl does: optimizer post-step hook, start of evaluate, end of
+        train).  Clears the packed operands of fused_operands() and the inner policy's cache."""
+        self._fused_cache.clear()
+        if hasattr(self.policy, 'invalidate_cache'):
+            self.policy.invalidate_cache()
+
+    def fused_supported(self, x):
+        """Can pb_policy_lstm_sample run this model on observations x?  One LSTM layer with bias, input and hidden size
+        128, a models.Default inner policy with a 128-unit encoder and <= 15 actions, fp32 CUDA observations of <= 128
+        features."""
+        rnn, inner = self.recurrent, self.policy
+        if not (isinstance(inner, Default) and rnn.num_layers == 1 and rnn.bias and rnn.input_size == 128
+                and rnn.hidden_size == 128 and getattr(rnn, 'proj_size', 0) == 0):
+            return False
+        n_act, hid = inner.decoder.weight.shape
+        feats = int(np.prod(self.obs_shape))
+        return (tuple(inner.encoder.weight.shape) == (128, feats) and hid == 128 and n_act <= 15 and feats <= 128
+                and x.is_cuda and x.dtype == torch.float32 and rnn.weight_ih_l0.dtype == torch.float32)
+
+    def fused_operands(self):
+        """The packed operands of pb_policy_lstm_sample (layouts in include/pufferlib_b200.h):
+        (w_enc [128, 136] TF32, b_enc [128], w_gates [16 * 32, 264] TF32 in chunk order, b_gates [16 * 32] = b_ih + b_hh
+        in chunk order, w_cat [8 or 16, 128], b_cat).  Cached under no_grad, keyed like Default.head_matrix."""
+        cache = self._fused_cache
+        rnn, inner = self.recurrent, self.policy
+        key = (inner.encoder.weight.data_ptr(), rnn.weight_ih_l0.data_ptr(), rnn.weight_hh_l0.data_ptr(),
+               inner.decoder.weight.data_ptr(), torch.cuda.is_current_stream_capturing())
+        if not torch.is_grad_enabled() and cache.get('key') == key:
+            return cache['ops']
+        with torch.no_grad():
+            w = inner.encoder.weight
+            w_enc = w.new_zeros(128, 136)
+            w_enc[:, :w.shape[1]] = _round_tf32(w)
+            # chunk ch, row 8j + u <- gate j of unit 8ch + u = row 128j + 8ch + u of [W_ih | W_hh]
+            dev = w.device
+            order = (torch.arange(4, device=dev)[None, :, None] * 128 + torch.arange(16, device=dev)[:, None, None] * 8
+                     + torch.arange(8, device=dev)[None, None, :]).reshape(-1)
+            w_gates = w.new_zeros(16 * 32, 264)
+            w_gates[:, :256] = _round_tf32(torch.cat([rnn.weight_ih_l0, rnn.weight_hh_l0], dim=1)[order])
+            b_gates = (rnn.bias_ih_l0 + rnn.bias_hh_l0)[order].contiguous()
+            w_cat, b_cat = inner.head_matrix()
+            ops = (w_enc, inner.encoder.bias.detach(), w_gates, b_gates, w_cat, b_cat)
+        if not torch.is_grad_enabled():
+            cache['key'], cache['ops'] = key, ops
+        return ops
 
     def forward(self, x, state):
         nd = len(self.obs_shape)

@@ -803,7 +803,7 @@ def create(config, vecenv, policy, optimizer=None, wandb=None):
         experience=experience, profile=profile, losses=losses, wandb=wandb, global_step=0, epoch=0, stats={},
         msg=msg, last_log_time=0, utilization=None, grad_bucket=grad_bucket,
         io=pufferlib_b200.namespace(h2d=0, d2h=0), graph_state=0, rollout_graph=None, graph_steps=0,
-        graph_launches=0, graph_replays=0, train_graph_state=0, train_graph=None, train_result=None, train_graph_launches=0, train_graph_replays=0, train_segments=None, train_acc=None, own_optimizer=own_optimizer, manual_update=None,
+        graph_launches=0, graph_replays=0, train_graph_state=0, train_graph=None, train_result=None, train_graph_launches=0, train_graph_replays=0, train_segments=None, train_acc=None, own_optimizer=own_optimizer, manual_update=None, train_minibatch_path=None,
         fused_rows=bool(getattr(policy, 'fused_sample', False)) and hasattr(vecenv, 'bind_rollout'),
         # one-kernel PPO loss (pb_ppo_loss): needs a wrapper exposing .policy(obs) -> (logits, value), one Discrete head
         fused_loss=bool(getattr(config, 'fused_loss', True)) and hasattr(policy, 'policy')
@@ -1045,6 +1045,8 @@ def _train_device_part(data, seg=None):
                 experience.flatten_batch()
             if config.norm_adv:
                 experience.normalize_advantages(slabs=slabs)
+    # which minibatch form the update reads: rollout tensors in place, slab copies of the per-row tensors, or gathered copies
+    data.train_minibatch_path = 'direct' if direct else ('slabs' if slabs else 'gathered')
 
     n_mb = experience.num_minibatches
     if seg is not None:                        # persistent accumulator: the segment graphs update it in place

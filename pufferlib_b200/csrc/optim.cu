@@ -203,11 +203,13 @@ __global__ void __launch_bounds__(CAP_THREADS) k_clip_adam_parts(AdamArgs a, con
     __syncthreads();
     if (s_last && pack.w_cat) {          // the last CTA sees every CTA's parameter updates: rebuild the 8-row head matrix (pb_pack_heads)
         __threadfence();
+        // the head parameters were just written by other CTAs of this launch: read them from L2 (this CTA's L1 may hold a
+        // line it loaded while updating its own share, e.g. w_val[96..127] split between two CTAs at n_act = 4)
         for (int j = tid; j < 8 * pack.hid; j += CAP_THREADS) {
             const int r = j / pack.hid, c = j % pack.hid;
-            pack.w_cat[j] = r < pack.n_act ? pack.w_dec[(int64_t)r * pack.hid + c] : (r == pack.n_act ? pack.w_val[c] : 0.f);
+            pack.w_cat[j] = r < pack.n_act ? __ldcg(pack.w_dec + (int64_t)r * pack.hid + c) : (r == pack.n_act ? __ldcg(pack.w_val + c) : 0.f);
         }
-        if (tid < 8) pack.b_cat[tid] = tid < pack.n_act ? pack.b_dec[tid] : (tid == pack.n_act ? pack.b_val[0] : 0.f);
+        if (tid < 8) pack.b_cat[tid] = tid < pack.n_act ? __ldcg(pack.b_dec + tid) : (tid == pack.n_act ? __ldcg(pack.b_val) : 0.f);
     }
 }
 

@@ -369,3 +369,120 @@ def test_lstm_parity_vs_reference(golden):
         clean_pufferl.close(data)
     finally:
         torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = tf32
+
+
+@pytest.mark.parametrize('n,bptt,nm,kw', [
+    (36, 8, 2, dict(update_epochs=2, anneal_lr=True, total_timesteps=4 * 36 * 128, max_grad_norm=1e-3)),
+    (64, 16, 4, dict(update_epochs=2, norm_adv=False, max_grad_norm=1e9))], ids=['R288_clipped', 'R1024_raw_adv'])
+def test_direct_slab_update_replays_through_gathered_minibatches(n, bptt, nm, kw):
+    """train() on the benchmark's path -- the fused update reading the arrival-order rollout tensors in place
+    (Experience.direct_minibatch: row_slab_stride = nm * R, returns and advantage normalisation formed in the kernel), then
+    pb_clip_adam_parts with the head rebuild in its last CTA -- replayed step by step from a snapshot of the rollout, the
+    parameters and the Adam state: minibatch membership and advantages from the oracles in float64, the normalisation of
+    clean_pufferl.py:211-213, pb_mlp_update_fused on contiguous gathered rows with explicit returns, pb_clip_adam (the
+    single-CTA norm pass) and pb_pack_heads.  The same kernel runs on both sides, so only the order of fp32 sums and the
+    fp32 vs fp64 advantages differ.  A: R = 288 (ragged tiles, 8 slabs), two epochs, annealed lr, every step clipped;
+    B: R = 1024, raw advantages, no clipping.  With breakout's 4 actions, one 128-byte line of the value-head weight is
+    updated by two CTAs of pb_clip_adam_parts (asserted below): a head matrix rebuilt from a stale copy of that line would
+    change the next minibatch."""
+    import ctypes as C
+    import util_update as uu
+    from pufferlib_b200 import models
+    from pufferlib_b200.frameworks import cleanrl
+    h = 128
+    vec = pvec.make(ocean.env_creator('breakout'), num_envs=n, backend=pvec.B200)
+    torch.manual_seed(0)
+    pol = cleanrl.Policy(models.Default(vec.driver_env), fused_sample=True, seed=7).cuda()
+    cfg = make_config(n, h, env='breakout', bptt_horizon=bptt, minibatch_size=n * h // nm, **kw)
+    data = clean_pufferl.create(cfg, vec, pol)
+    clean_pufferl.evaluate(data)
+    clean_pufferl.train(data)                    # the Adam state exists and the learning rate is annealed once
+    assert data.train_minibatch_path == 'direct'
+    clean_pufferl.evaluate(data)
+    exp, model, opt = data.experience, pol.policy, data.optimizer
+    params = [model.encoder.weight, model.encoder.bias, model.decoder.weight, model.decoder.bias, model.value_head.weight,
+              model.value_head.bias]
+    assert uu.split_lines(params[2:], first=128 * 128 + 128) > 0
+    mine = [p.detach().clone() for p in params]
+    st = [{k: opt.state[p][k].clone() for k in ('exp_avg', 'exp_avg_sq', 'step')} for p in params]
+    group = opt.param_groups[0]
+    lr, (b1, b2), eps = float(group['lr']), group['betas'], group['eps']
+    roll = {k: cpu(getattr(exp, k)).copy() for k in ('obs', 'actions', 'logprobs', 'values', 'rewards', 'dones')}
+    clean_pufferl.train(data)
+    assert data.train_minibatch_path == 'direct' and data.manual_update.used_fused
+
+    # the replay
+    dev = torch.device('cuda')
+    lib, s = _native.lib(), _native.stream_ptr()
+    n_act = model.decoder.weight.shape[0]
+    ora = oexp.Experience(n * h, bptt, n * h // nm, (128,), np.float32)
+    for k, v in roll.items():
+        getattr(ora, k)[:] = v
+    ora.sort_keys = [(e, t) for t in range(h) for e in range(n)]
+    idx = ora.sort_training_data()
+    ora.flatten_batch(ogae.compute_gae_f64(ora.dones[idx], ora.values[idx], ora.rewards[idx], cfg.gamma, cfg.gae_lambda))
+    w_cat, b_cat = torch.zeros(8, 128, device=dev), torch.zeros(8, device=dev)
+
+    def pack_heads(ps, wc, bc):
+        _native.check(lib.pb_pack_heads(_native.ptr(ps[2]), _native.ptr(ps[3]), _native.ptr(ps[4]), _native.ptr(ps[5]), n_act,
+                                        128, _native.ptr(wc), _native.ptr(bc), None, None, 0, s))
+    pack_heads(mine, w_cat, b_cat)
+    ws = uu.workspace(dev)
+    loss_cfg = (cfg.clip_coef, int(cfg.clip_vloss), cfg.vf_clip_coef, cfg.vf_coef, cfg.ent_coef)
+    stats, norms = torch.zeros(6, dtype=torch.float64, device=dev), []
+    norm_out = torch.zeros(1, device=dev)
+    m = n * h // nm
+    t = lambda a, dtype=torch.float32: torch.as_tensor(np.ascontiguousarray(a).reshape(-1), device=dev).to(dtype)
+    for epoch in range(cfg.update_epochs):
+        for mb in range(nm):
+            a64 = ora.b_advantages[mb].astype(np.float64)
+            if cfg.norm_adv:
+                a64 = (a64 - a64.mean()) / (a64.std(ddof=1) + 1e-8)
+            x = torch.as_tensor(ora.b_obs[mb].reshape(m, 128), device=dev)
+            gflat, st8 = uu.fused(x, 128, m, m, 1, mine[0], mine[1], w_cat, b_cat, t(ora.b_actions[mb], torch.int64),
+                                  t(ora.b_logprobs[mb]), t(a64), t(ora.b_returns[mb]), t(ora.b_values[mb]), n_act, False,
+                                  cfg=loss_cfg, ws=ws)[:2]
+            stats += st8[:6]
+            grads = uu.grad_views(gflat, n_act)
+            arr = (_native.AdamTensor * 6)()
+            for k in range(6):
+                arr[k] = _native.AdamTensor(mine[k].data_ptr(), st[k]['exp_avg'].data_ptr(), st[k]['exp_avg_sq'].data_ptr(),
+                                            st[k]['step'].data_ptr(), grads[k].data_ptr(), mine[k].numel())
+            _native.check(lib.pb_clip_adam(arr, 6, C.c_float(cfg.max_grad_norm), C.c_float(1.0), C.c_float(lr), None,
+                                           C.c_float(b1), C.c_float(b2), C.c_float(eps), _native.ptr(norm_out), s))
+            pack_heads(mine, w_cat, b_cat)
+            norms.append(float(norm_out))
+    torch.cuda.synchronize()
+    n_steps = cfg.update_epochs * nm
+    if cfg.max_grad_norm < 1:
+        assert min(norms) > cfg.max_grad_norm, norms          # every step clipped
+    else:
+        assert max(norms) < cfg.max_grad_norm, norms
+    errs = {}
+    for k, p in enumerate(params):
+        errs[f'param{k}'] = float((p.detach() - mine[k]).abs().max())
+        for name in ('exp_avg', 'exp_avg_sq'):
+            errs[f'{name}{k}'] = uu.rel(opt.state[p][name], st[k][name])
+        assert float(opt.state[p]['step']) == float(st[k]['step']) == float(n_steps * 2)
+    print('replay errors', {k: f'{v:.2e}' for k, v in errs.items()}, 'norms', norms)
+    for k in range(6):
+        # one Adam step moves a parameter by at most ~lr; the two sides agree to 1e-3 of that per step
+        assert errs[f'param{k}'] <= 1e-3 * lr * n_steps, errs
+        assert errs[f'exp_avg{k}'] <= 1e-4 and errs[f'exp_avg_sq{k}'] <= 1e-4, errs
+    # the head matrix train() leaves is the packed form of its own parameters, bit for bit, and the replay's up to the above
+    mu = data.manual_update
+    w_ref, b_ref = torch.full_like(w_cat, 9.0), torch.full_like(b_cat, 9.0)
+    pack_heads([p.detach() for p in params], w_ref, b_ref)
+    torch.cuda.synchronize()
+    assert torch.equal(mu.w_cat, w_ref) and torch.equal(mu.b_cat, b_ref)
+    assert float((mu.w_cat - w_cat).abs().max()) <= 1e-3 * lr * n_steps
+    # the reported losses: per-minibatch means / n_mb summed over the epochs (clean_pufferl.py:249-254)
+    tot = (stats / (m * nm)).cpu().numpy()
+    tot[1] *= 0.5
+    got = np.array([data.losses.policy_loss, data.losses.value_loss, data.losses.entropy, data.losses.old_approx_kl,
+                    data.losses.approx_kl, data.losses.clipfrac])
+    # the policy loss is a mean of O(1) terms that nearly cancel (normalised advantages have mean 0): fp32 vs fp64 advantages
+    # move it by ~1e-7 of a term
+    assert abs(got[0] - tot[0]) <= 1e-6, (got, tot)
+    assert np.allclose(got[1:], tot[1:], rtol=1e-4, atol=0), (got, tot)
+    clean_pufferl.close(data)

@@ -92,6 +92,84 @@ def test_clip_adam_parts_matches_single_cta_kernel(world, n_parts):
             assert float((pa[k] - pb[k]).abs().max()) <= 1e-7
 
 
+@pytest.mark.parametrize('lr_on_device,grad_scale', [(True, 1.0), (False, 0.5)])
+@pytest.mark.parametrize('n_act', range(1, 8))
+def test_clip_adam_parts_on_fused_update_gradients(n_act, lr_on_device, grad_scale):
+    """The optimizer step of the fused train() path as _DefaultMLPUpdate runs it: pb_mlp_update_fused leaves the gradient in
+    the flat buffer and its sums of squares in the workspace, pb_clip_adam_parts takes the norm from those partials, clips,
+    steps Adam on the six gradient views and rebuilds the head matrix in its last CTA; the next minibatch's forward reads
+    that head matrix.  Five steps (clipping on steps 1 and 3 only) vs clip_grad_norm_ + torch.optim.Adam(eps=1e-5, fused,
+    capturable); the head matrix bitwise equal to pb_pack_heads of the updated parameters after every step.
+
+    Each parameter is its own allocation, as the nn.Linear weights and biases of a models.Default are.  The kernel hands
+    element j of the concatenated parameters to CTA (j // 256) % 32, so a 128-byte line of w_val can then be updated by two
+    CTAs (n_act = 2, 4, 6); the last CTA must not rebuild the head matrix from a stale copy of such a line in its L1."""
+    import util_update as uu
+    dev = torch.device('cuda')
+    torch.manual_seed(20 + n_act)
+    lib = _native.lib()
+    # the decoder weight and bias are the first n_act rows of 8-row buffers: reads of the head rebuild stay in bounds even
+    # when it indexes one row too far
+    w_dec, b_dec = torch.zeros(8, 128, device=dev), torch.zeros(8, device=dev)
+    ours = [torch.randn(128, 128, device=dev) * 0.1, torch.randn(128, device=dev) * 0.1, w_dec[:n_act], b_dec[:n_act],
+            torch.randn(1, 128, device=dev) * 0.1, torch.randn(1, device=dev) * 0.1]
+    ours[2].copy_(torch.randn(n_act, 128, device=dev) * 0.1)
+    ours[3].copy_(torch.randn(n_act, device=dev) * 0.1)
+    if n_act in (2, 4, 6):
+        assert uu.split_lines(ours[2:], first=128 * 128 + 128) > 0
+    ref = [p.detach().clone().requires_grad_(True) for p in ours]
+    lr = 2.5e-4
+    lr_t = torch.tensor(lr, device=dev)
+    opt = torch.optim.Adam(ref, lr=lr_t.clone() if lr_on_device else lr, eps=1e-5, fused=True, capturable=True)
+    state = [dict(step=torch.zeros((), device=dev), m=torch.zeros_like(p), v=torch.zeros_like(p)) for p in ours]
+    w_cat, b_cat = torch.zeros(8, 128, device=dev), torch.zeros(8, device=dev)
+    s = _native.stream_ptr()
+
+    def pack_heads(wc, bc):
+        _native.check(lib.pb_pack_heads(_native.ptr(ours[2]), _native.ptr(ours[3]), _native.ptr(ours[4]), _native.ptr(ours[5]),
+                                        n_act, 128, _native.ptr(wc), _native.ptr(bc), None, None, 0, s))
+    pack_heads(w_cat, b_cat)
+    head_pack = _native.HeadPack(ours[2].data_ptr(), ours[3].data_ptr(), ours[4].data_ptr(), ours[5].data_ptr(),
+                                 w_cat.data_ptr(), b_cat.data_ptr(), n_act, 128)
+    ws = uu.workspace(dev)
+    parts = C.c_void_p(ws.data_ptr() + lib.pb_mlp_update_sumsq_offset())
+    norm_out = torch.zeros(1, device=dev)
+    m = 1000
+    for it in range(5):
+        x = torch.randn(m, 128, device=dev)
+        act = torch.randint(0, n_act, (m,), device=dev)
+        olp = -torch.rand(m, device=dev) - 0.5
+        adv, ret, oval = torch.randn(m, device=dev), torch.randn(m, device=dev), torch.randn(m, device=dev)
+        gflat = uu.fused(x, 128, m, m, 1, ours[0], ours[1], w_cat, b_cat, act, olp, adv, ret, oval, n_act, False, ws=ws)[0]
+        grads = uu.grad_views(gflat, n_act)
+        norm = grad_scale * float(torch.sqrt(sum((g.double() ** 2).sum() for g in grads)))
+        max_norm = norm * (0.5 if it in (1, 3) else 2.0)
+        for p, g in zip(ref, grads):
+            p.grad = (g * grad_scale).clone()       # grad_scale (1 / world) scales the summed gradient before the clip
+        ref_norm = float(torch.nn.utils.clip_grad_norm_(ref, max_norm))
+        opt.step()
+        arr = (_native.AdamTensor * 6)()
+        for k in range(6):
+            arr[k] = _native.AdamTensor(ours[k].data_ptr(), state[k]['m'].data_ptr(), state[k]['v'].data_ptr(),
+                                        state[k]['step'].data_ptr(), grads[k].data_ptr(), ours[k].numel())
+        _native.check(lib.pb_clip_adam_parts(
+            arr, 6, C.c_float(max_norm), C.c_float(grad_scale), C.c_float(0.0 if lr_on_device else lr),
+            _native.ptr(lr_t) if lr_on_device else None, C.c_float(0.9), C.c_float(0.999), C.c_float(1e-5), _native.ptr(norm_out),
+            parts, lib.pb_mlp_update_sumsq_parts(), None, C.byref(head_pack), s))
+        w_ref, b_ref = torch.full_like(w_cat, 9.0), torch.full_like(b_cat, 9.0)
+        pack_heads(w_ref, b_ref)
+        torch.cuda.synchronize()
+        assert abs(float(norm_out) - ref_norm) <= 1e-6 * ref_norm, (it, float(norm_out), ref_norm)
+        for k in range(6):
+            st = opt.state[ref[k]]
+            assert float(state[k]['step']) == float(st['step']) == it + 1
+            # exp_avg carries the clip coefficient linearly (Adam's step nearly cancels it)
+            for mine, theirs in ((state[k]['m'], st['exp_avg']), (state[k]['v'], st['exp_avg_sq'])):
+                assert torch.allclose(mine, theirs, rtol=1e-5, atol=1e-6 * float(theirs.abs().max())), (it, k)
+            assert float((ours[k] - ref[k].detach()).abs().max()) <= 1e-3 * lr * (it + 1), (it, k)
+        assert torch.equal(w_cat, w_ref) and torch.equal(b_cat, b_ref), it
+
+
 @pytest.mark.parametrize('n_act,features', [(4, 128), (7, 49), (1, 300)])
 def test_pack_heads_matches_torch_construction(n_act, features):
     dev = torch.device('cuda')

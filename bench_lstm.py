@@ -1,15 +1,19 @@
 #!/usr/bin/env python
 """bench_lstm.py -- the recurrent policy on the device path: RecurrentPolicy(LSTMWrapper(Default), fused_sample=True).
 
-    python bench_lstm.py [--env breakout|squared] [--num-envs N] [--horizon H] [--steps K] [--warmup W]
+    python bench_lstm.py [--env breakout|squared] [--num-envs N] [--horizon H] [--steps K] [--warmup W] [--fused-update]
 
 Prints one JSON line with
-  * agent-steps/s of the PPO loop (CUDA-graphed rollout, recurrent update on cuDNN autograd), the same step definition
-    as bench.py;
+  * agent-steps/s of the PPO loop (CUDA-graphed rollout; recurrent update on cuDNN autograd, or with --fused-update on
+    the BPTT kernels pb_lstm_bptt_forward / _backward + pb_ppo_loss), the same step definition as bench.py;
   * `policy_step`: the rollout-time policy step, fused (pb_policy_lstm_sample: one kernel) vs unfused
     (fused_sample=False), measured in the same process on the rollout's own observation rows;
   * `roofline_kernels.policy_lstm_step`: algorithmic HBM bytes 4F + 2048 + 16 per row over the fused step time, against
-    the H100 SXM data-sheet 3.35 TB/s; the packed weights each CTA streams from L2 are reported separately.
+    the H100 SXM data-sheet 3.35 TB/s; the packed weights each CTA streams from L2 are reported separately;
+  * `update`: forward + loss + backward of one training minibatch ([B segments, T = 16 steps] of the rollout), fused
+    (forward_packed_seq + fused_ppo_loss_packed) vs cuDNN (the LSTMWrapper forward + the autograd loss, as train() runs
+    it), in the same process on the same minibatch, from CUDA events; with the algorithmic bytes and TF32 FLOPs per row
+    of the fused path and the share of each data-sheet bound.
 Shared pieces (PPO config, timed steps, card name and power limit) come from bench.py.  Writes nothing to the tree.
 """
 import argparse
@@ -32,6 +36,8 @@ def parse_args():
     ap.add_argument('--epochs', type=int, default=4)
     ap.add_argument('--no-graph', action='store_true')
     ap.add_argument('--reps', type=int, default=256, help='policy steps per timed CUDA graph')
+    ap.add_argument('--fused-update', action='store_true', help='train() on the fused BPTT kernels')
+    ap.add_argument('--update-reps', type=int, default=10, help='timed minibatch updates per path')
     return ap.parse_args()
 
 
@@ -103,6 +109,69 @@ def policy_step_times(data, reps=256):
     return res
 
 
+def update_cost_per_row(feats, n_out, steps):
+    """Algorithmic HBM bytes and TF32 tensor-core FLOPs per minibatch row of the fused update (forward kernel, loss
+    kernel, backward kernel, weight-gradient GEMMs and column sums), from the shapes.  n_out = R head columns."""
+    H, G = 128, 512
+    state = 4 * 4 * H / steps                                   # h0, c0 read and h_T, c_T written, once per segment
+    nbytes = {
+        'forward': 4 * feats + 4 * 1024 + 4 * n_out + state,     # x; saved row written; out written
+        'loss': 4 * n_out + 28 + 4 * n_out,                     # out + 7 per-row scalars read; dOut written
+        'backward': 4 * n_out + 4 * (H + 4 * H + H) + 4 * G + 4 * H,   # dOut, e, activations, c read; dz, dPre written
+        'weight_grads': 2 * 4 * G + 4 * 2 * H + 2 * 4 * H + 4 * feats + 2 * 4 * n_out + 4 * H,
+        # dz (GEMM + column sum), [e | h_prev], dPre (GEMM + sum), x, dOut (GEMM + sum), h
+    }
+    flops = {
+        'forward': 2 * (feats * H + 2 * H * G + H * n_out),      # encoder, gates, heads
+        'backward': 2 * (G * 2 * H),                              # dz [W_ih | W_hh]
+        'weight_grads': 2 * (G * 2 * H + H * feats + n_out * H),  # dW_ih | dW_hh, dW_enc, dW_cat
+    }
+    return nbytes, flops
+
+
+def update_times(data, reps=10):
+    """Device time of forward + loss + backward of one training minibatch (minibatch 0 of the last train(), initial
+    state None), fused (forward_packed_seq + fused_ppo_loss_packed + backward) and cuDNN (the RecurrentPolicy forward
+    over the segments + the autograd loss of train() + backward), alternating, each bracketed by CUDA events; median of
+    `reps` after 2 warm-ups.  The optimizer step is not included."""
+    from pufferlib_b200 import clean_pufferl as cp
+    policy, exp, cfg = data.policy, data.experience, data.config
+    obs, atn, lp = exp.b_obs[0], exp.b_actions[0], exp.b_logprobs[0]
+    val, ret, adv = exp.b_values[0], exp.b_returns[0], exp.b_advantages[0]
+    model = policy.policy
+
+    def fused():
+        out, n_act, _ = model.forward_packed_seq(obs, None)
+        loss, _ = cp.fused_ppo_loss_packed(out, n_act, atn, lp, adv, ret, val, cfg)
+        loss.backward()
+
+    def cudnn():
+        _, newlogprob, entropy, newvalue, _ = policy(obs, state=None, action=atn)
+        ratio = (newlogprob - lp.reshape(-1)).exp()
+        a = adv.reshape(-1)
+        pg = torch.max(-a * ratio, -a * torch.clamp(ratio, 1 - cfg.clip_coef, 1 + cfg.clip_coef)).mean()
+        v = newvalue.view(-1)
+        r = ret.reshape(-1)
+        vc = val.reshape(-1) + torch.clamp(v - val.reshape(-1), -cfg.vf_clip_coef, cfg.vf_clip_coef)
+        v_loss = 0.5 * torch.max((v - r) ** 2, (vc - r) ** 2).mean()
+        (pg - cfg.ent_coef * entropy.mean() + v_loss * cfg.vf_coef).backward()
+
+    runs = {'fused': fused, 'cudnn': cudnn}
+    times = {k: [] for k in runs}
+    for i in range(reps + 2):
+        for k, run in runs.items():
+            policy.zero_grad(set_to_none=True)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            run()
+            e1.record()
+            torch.cuda.synchronize()
+            if i >= 2:
+                times[k].append(e0.elapsed_time(e1) * 1e-3)
+    policy.zero_grad(set_to_none=True)
+    return {k: float(np.median(v)) for k, v in times.items()}, tuple(obs.shape[:2])
+
+
 def main(args):
     import pufferlib_b200.vector as pvec
     from pufferlib_b200 import clean_pufferl as cp, models
@@ -114,7 +183,7 @@ def main(args):
     torch.manual_seed(1)
     net = models.LSTMWrapper(vec.driver_env, models.Default(vec.driver_env, hidden_size=128), input_size=128,
                              hidden_size=128)
-    policy = cleanrl.RecurrentPolicy(net, fused_sample=True, seed=1).cuda()
+    policy = cleanrl.RecurrentPolicy(net, fused_sample=True, seed=1, fused_update=args.fused_update).cuda()
     cfg = ppo_config(n, h, 'cuda', seed=1, cuda_graph=not args.no_graph, minibatches=args.minibatches,
                      epochs=args.epochs, env=args.env)
     data = cp.create(cfg, vec, policy)
@@ -123,7 +192,11 @@ def main(args):
         cp.train(data)
     ms = timed_steps(data, cp, args.steps, 1)
     prof = {k: round(v, 4) for k, v in dict(data.profile).items() if k.endswith('_time')}
+    recurrent_path = data.train_recurrent_path
     times = policy_step_times(data, args.reps)
+    upd, (seg, bptt) = update_times(data, args.update_reps)
+    n_act = vec.single_action_space.n
+    n_out = -(-(n_act + 1) // 8) * 8
     # algorithmic HBM bytes of one fused step: x (4F), h and c read and written (4 x 512), value + logprob + action (16)
     feats = int(np.prod(vec.single_observation_space.shape))
     step_bytes = n * (4 * feats + 2048 + 16)
@@ -139,7 +212,8 @@ def main(args):
         'config': {'workload': f'{args.env} num_envs={n} horizon={h} RecurrentPolicy(LSTMWrapper(Default)) hidden=128 '
                                'fused_sample=True', 'global_batch': n * h, 'minibatch_size': n * h // args.minibatches,
                    'update_epochs': args.epochs, 'bptt_horizon': 16, 'cuda_graph_rollout': not args.no_graph,
-                   'update': 'cuDNN LSTM autograd'},
+                   'update': 'fused BPTT kernels' if args.fused_update else 'cuDNN LSTM autograd',
+                   'train_recurrent_path': recurrent_path},
         'policy_step': {
             'fused_us': round(t_f * 1e6, 2), 'unfused_us': round(t_u * 1e6, 2), 'speedup': round(t_u / t_f, 2),
             'fused_eager_us': round(times['fused']['eager_seconds'] * 1e6, 2),
@@ -152,10 +226,30 @@ def main(args):
             'avg_launch_us': round(t_f * 1e6, 2), 'achieved': round(step_bytes / t_f / 1e9, 1),
             'frac': round(bound_s / t_f, 4), 'launches_per_step': h,
             'l2_weight_bytes_per_cta': weight_bytes, 'l2_weight_bytes_per_launch': weight_bytes * ctas}},
+        'update': update_section(upd, seg, bptt, feats, n_out),
         'gpu': gpu_info(0), 'profile_s': prof, 'env_stats': {k: float(v) for k, v in data.stats.items()},
     }
     print(json.dumps(line))
     cp.close(data)
+
+
+def update_section(upd, seg, bptt, feats, n_out):
+    rows = seg * bptt
+    nbytes, flops = update_cost_per_row(feats, n_out, bptt)
+    b_row, f_row = sum(nbytes.values()), sum(flops.values())
+    peak_gbs, peak_tflops = 3350.0, 495.0
+    t_bytes, t_flops = rows * b_row / (peak_gbs * 1e9), rows * f_row / (peak_tflops * 1e12)
+    t_f, t_c = upd['fused'], upd['cudnn']
+    return {
+        'minibatch': {'segments': seg, 'bptt': bptt, 'rows': rows},
+        'fused_ms': round(t_f * 1e3, 3), 'cudnn_ms': round(t_c * 1e3, 3), 'speedup': round(t_c / t_f, 2),
+        'method': 'forward + loss + backward per minibatch (no optimizer step), CUDA events, median',
+        'bytes_per_row': nbytes, 'tf32_flops_per_row': flops,
+        'hbm_bound_ms': round(t_bytes * 1e3, 3), 'tf32_bound_ms': round(t_flops * 1e3, 3),
+        'share_of_hbm_bound': round(t_bytes / t_f, 4), 'share_of_tf32_bound': round(t_flops / t_f, 4),
+        'bound_by': 'hbm' if t_bytes >= t_flops else 'tf32',
+        'peak_source': 'H100 SXM5 data sheet: 3.35 TB/s HBM3, 495 TFLOP/s dense TF32 (700 W); not measured',
+    }
 
 
 if __name__ == '__main__':

@@ -261,6 +261,36 @@ int pb_policy_lstm_sample(const float* obs, int64_t obs_stride, int32_t in_featu
                           uint32_t* ticket_dev, int64_t* actions, float* logprobs, float* values, float* entropies,
                           void* stream);
 
+/* -- recurrent minibatch forward / backward over bptt segments ----------------------------------------------------------
+ * The training-time LSTMWrapper(models.Default) of clean_pufferl.py:186-238 on [B segments, T steps] (the [rows, bptt,
+ * *obs] minibatch of clean_pufferl.py:188-191), same model envelope and packed operands as pb_policy_lstm_sample.
+ * Rows are in (b, t) order: row b*T + t.
+ * pb_lstm_bptt_forward: obs row b*T + t at obs + (b*T + t) * obs_stride (in_features <= 128 fp32, no alignment needed);
+ *   h0, c0 [B][128] or null (zeros).  Per step the formula of pb_policy_lstm_sample (same rounding: T = 1 computes what
+ *   the rollout step computes).  Writes
+ *   out   [B*T][R] fp32, R = 8 for n_act <= 7, else 16: n_act logits | value | the head bias of the zero rows;
+ *   h_out, c_out [B][128]: the state after step T - 1;
+ *   saved [B*T][1024] fp32 (4096 B per row): [e | h_prev | sigmoid(i) | sigmoid(f) | tanh(g) | sigmoid(o) | c | h],
+ *         128 floats each (gates unit-major), e = relu(x W_enc^T + b_enc), h_prev = the state the step started from.
+ * pb_lstm_bptt_backward: dout [B*T][R] (the loss gradient w.r.t. out, R as above), saved and c0 of the forward,
+ *   w_gates_t [16][256][40] (models.LSTMWrapper.gate_weights_transposed: chunk ch, row n, column 8j + u = row 128j +
+ *   8ch + u, column n of [W_ih | W_hh], rounded to TF32; columns 32..39 zero; 16-byte aligned), w_heads as in the
+ *   forward.  The final state gets no gradient.  Writes
+ *   dz   [B*T][512]: dLoss/d(gate pre-activations), nn.LSTM order i | f | g | o, unit-major;
+ *   dpre [B*T][128]: dLoss/d(encoder pre-activation).
+ *   The weight gradients follow by GEMMs: dW_ih | dW_hh = dz^T [e | h_prev], db_ih = db_hh = column sums of dz,
+ *   dW_enc = dpre^T x, db_enc = column sums of dpre, dW_cat = dout^T h, db_cat = column sums of dout.
+ * Segments >= B are never read or written.  PB_ERR_UNSUPPORTED (before any launch) for in_features > 128, input_size or
+ * hidden_size != 128, n_act > 15.  Pointers 8-byte aligned unless stated otherwise. */
+int pb_lstm_bptt_forward(const float* obs, int64_t obs_stride, int32_t in_features, int64_t batch, int32_t steps,
+                         const float* h0, const float* c0, const float* w_enc, const float* b_enc, const float* w_gates,
+                         const float* b_gates, const float* w_heads, const float* b_heads, int32_t input_size,
+                         int32_t hidden_size, int32_t n_act, float* out, float* h_out, float* c_out, float* saved,
+                         void* stream);
+int pb_lstm_bptt_backward(const float* dout, const float* saved, const float* c0, const float* w_gates_t,
+                          const float* w_heads, int64_t batch, int32_t steps, int32_t input_size, int32_t hidden_size,
+                          int32_t n_act, float* dz, float* dpre, void* stream);
+
 /* -- persistent rollout (env steps with the policy in the loop) -------------------------------------------------------
  * The H-iteration body of clean_pufferl.evaluate (clean_pufferl.py:84-124: recv -> policy -> store -> send) for a
  * breakout handle and models.Default (128 features, 128 hidden, n_act <= 4) in ONE launch: a CTA owns 128 envs for all

@@ -82,6 +82,10 @@ SIGNATURES = {
     'pb_policy_lstm_sample': (C.c_int, [C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 6 + [C.c_void_p, C.c_int64,
                               C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_uint64]
                               + [C.c_void_p] * 6 + [C.c_void_p]),
+    'pb_lstm_bptt_forward': (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32] + [C.c_void_p] * 8
+                             + [C.c_int32] * 3 + [C.c_void_p] * 4 + [C.c_void_p]),
+    'pb_lstm_bptt_backward': (C.c_int, [C.c_void_p] * 5 + [C.c_int64] + [C.c_int32] * 4 + [C.c_void_p] * 2
+                              + [C.c_void_p]),
     'pb_mlp_tail_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int32]),
     'pb_mlp_tail_backward': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
                              C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -803,7 +803,7 @@ def create(config, vecenv, policy, optimizer=None, wandb=None):
         experience=experience, profile=profile, losses=losses, wandb=wandb, global_step=0, epoch=0, stats={},
         msg=msg, last_log_time=0, utilization=None, grad_bucket=grad_bucket,
         io=pufferlib_b200.namespace(h2d=0, d2h=0), graph_state=0, rollout_graph=None, graph_steps=0,
-        graph_launches=0, graph_replays=0, train_graph_state=0, train_graph=None, train_result=None, train_graph_launches=0, train_graph_replays=0, train_segments=None, train_acc=None, own_optimizer=own_optimizer, manual_update=None, train_minibatch_path=None,
+        graph_launches=0, graph_replays=0, train_graph_state=0, train_graph=None, train_result=None, train_graph_launches=0, train_graph_replays=0, train_segments=None, train_acc=None, own_optimizer=own_optimizer, manual_update=None, train_minibatch_path=None, train_recurrent_path=None,
         fused_rows=bool(getattr(policy, 'fused_sample', False)) and hasattr(vecenv, 'bind_rollout'),
         # one-kernel PPO loss (pb_ppo_loss): needs a wrapper exposing .policy(obs) -> (logits, value), one Discrete head
         fused_loss=bool(getattr(config, 'fused_loss', True)) and hasattr(policy, 'policy')
@@ -1058,6 +1058,10 @@ def _train_device_part(data, seg=None):
         acc = torch.zeros(6, device=device)    # policy, value, entropy, old_kl, kl, clipfrac
     obs_shape = data.vecenv.single_observation_space.shape
     fused = data.fused_loss and experience.lstm_h is None
+    # recurrent models: the fused BPTT update when the policy asks for it (RecurrentPolicy(fused_update=True)); the
+    # model decides per minibatch whether it applies (data.train_recurrent_path records which path ran)
+    rec_fused = experience.lstm_h is not None and bool(getattr(data.policy, 'fused_update', False)) and \
+        bool(getattr(config, 'fused_loss', True))
     carry = {'lstm_state': None, 'approx_kl': None}
     if manual is not None:
         manual.pack_heads()                      # the parameters may have changed since the last train() (checkpoints)
@@ -1099,13 +1103,19 @@ def _train_device_part(data, seg=None):
                 if packed is None:
                     logits, newvalue = model(obs.reshape(-1, *obs_shape))
             elif experience.lstm_h is not None:       # clean_pufferl.py:188-191: [rows, bptt, *obs] segments
-                _, newlogprob, entropy, newvalue, st_ = data.policy(obs, state=carry['lstm_state'], action=atn)
+                if rec_fused and hasattr(getattr(data.policy, 'policy', None), 'forward_packed_seq'):
+                    packed = data.policy.policy.forward_packed_seq(obs, carry['lstm_state'])
+                if packed is not None:     # BPTT kernels; the loss hands back ONE [B*T, R] gradient
+                    st_ = packed[2]
+                else:
+                    _, newlogprob, entropy, newvalue, st_ = data.policy(obs, state=carry['lstm_state'], action=atn)
+                data.train_recurrent_path = 'cudnn' if packed is None else 'fused'
                 carry['lstm_state'] = (st_[0].detach(), st_[1].detach())
             else:
                 _, newlogprob, entropy, newvalue = data.policy(obs.reshape(-1, *obs_shape), action=atn)
 
         with profile.train_misc:
-            if fused:
+            if fused or packed is not None:
                 if packed is not None:
                     loss, st = fused_ppo_loss_packed(packed[0], packed[1], atn, log_probs, adv, ret, val, config)
                 else:

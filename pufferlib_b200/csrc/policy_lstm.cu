@@ -40,6 +40,7 @@
 // h_prev and h' in the kernel, W_enc and the gate weights on the host (models.LSTMWrapper.fused_operands), W_cat in the
 // kernel.  Accumulation, biases, the cell update and the sampler are fp32.
 #include "pb_common.cuh"
+#include "lstm_cell.cuh"
 #include "policy_sample.cuh"
 #include "tma.cuh"
 
@@ -47,14 +48,7 @@ namespace {
 
 constexpr int PL_ROWS = 128;                       // rows per CTA
 constexpr int PL_THREADS = 256;                    // 8 warps x 16 rows
-constexpr int PL_F = 128;                          // x tile columns (obs features, zero padded)
-constexpr int PL_H = 128;                          // LSTM input size = hidden size
-constexpr int PL_XP = PL_F + 8;                    // 136: x / W_enc / W_heads pitch (conflict-free 64-bit loads)
-constexpr int PL_GP = 2 * PL_H + 8;                // 264: gate-weight row pitch, K = [e (128) | h (128)] + pad
-constexpr int PL_CHUNKS = PL_H / 8;                // 16 chunks of 8 units = 32 gate columns
-constexpr int PL_CHUNK = 32 * PL_GP;               // floats per chunk (33792 B)
-constexpr uint32_t PL_CHUNK_BYTES = PL_CHUNK * 4u;
-constexpr uint32_t PL_WENC_BYTES = PL_H * PL_XP * 4u;
+// PL_F, PL_H, PL_XP, PL_GP, PL_CHUNKS, PL_CHUNK(_BYTES), PL_WENC_BYTES: lstm_cell.cuh
 
 // shared-memory carve-up, in floats
 constexpr int SM_X = 0;                            // [128][136] observation tile
@@ -79,8 +73,6 @@ struct LstmParams {
     uint64_t seed; uint64_t* counter; unsigned int* ticket;
     int64_t* actions; float* logprobs; float* values; float* entropies;
 };
-
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 
 template <int NC>
 __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams p) {
@@ -136,42 +128,19 @@ __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams
     for (int ks = 0; ks < 16; ++ks) {
         const float2 x0 = va ? *reinterpret_cast<const float2*>(h_a + 8 * ks + 2 * t) : make_float2(0.f, 0.f);
         const float2 x1 = vb ? *reinterpret_cast<const float2*>(h_b + 8 * ks + 2 * t) : make_float2(0.f, 0.f);
-        hA[ks][0] = to_tf32(x0.x); hA[ks][1] = to_tf32(x1.x); hA[ks][2] = to_tf32(x0.y); hA[ks][3] = to_tf32(x1.y);
+        lstm_a_frag(hA[ks], x0.x, x0.y, x1.x, x1.y);
     }
     __syncthreads();                               // x tile, small operands and the barrier inits are visible
 
     // ---- encoder: warp w owns rows 16w..16w+15 and all 128 hidden columns; K = F rounded up to 8 (the rest is zero)
     float acc[16][4];
-#pragma unroll
-    for (int nt = 0; nt < 16; ++nt) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }
-    {
-        const float* xa = sX + lr * PL_XP + 2 * t;
-        const float* wb = sWe + g * PL_XP + 2 * t;
-        const int ksteps = (F + 7) >> 3;
-        mbar_wait(&bars[0], 0);
-#pragma unroll 2
-        for (int ks = 0; ks < ksteps; ++ks) {
-            const float2 x0 = *reinterpret_cast<const float2*>(xa + 8 * ks);
-            const float2 x1 = *reinterpret_cast<const float2*>(xa + 8 * PL_XP + 8 * ks);
-            const uint32_t a[4] = {to_tf32(x0.x), to_tf32(x1.x), to_tf32(x0.y), to_tf32(x1.y)};
-#pragma unroll
-            for (int nt = 0; nt < 16; ++nt) {
-                const float2 w = *reinterpret_cast<const float2*>(wb + 8 * nt * PL_XP + 8 * ks);   // B[k][n] = W[n][k]
-                mma_tf32(acc[nt], a, __float_as_uint(w.x), __float_as_uint(w.y));
-            }
-        }
-    }
+    mbar_wait(&bars[0], 0);
+    lstm_encoder(acc, sX + lr * PL_XP + 2 * t, sWe + g * PL_XP + 2 * t, F);
     // relu(acc + b) as A fragments: C fragment of n-tile nt = columns 8nt + {2t, 2t+1} of rows {g, g+8} -> k slots {t, t+4}
+    lstm_encoder_relu(acc, sBe, t);
     uint32_t eA[16][4];
 #pragma unroll
-    for (int nt = 0; nt < 16; ++nt) {
-        const int c0 = 8 * nt + 2 * t;
-        const float b0 = sBe[c0], b1 = sBe[c0 + 1];
-        eA[nt][0] = to_tf32(fmaxf(acc[nt][0] + b0, 0.f));
-        eA[nt][1] = to_tf32(fmaxf(acc[nt][2] + b0, 0.f));
-        eA[nt][2] = to_tf32(fmaxf(acc[nt][1] + b1, 0.f));
-        eA[nt][3] = to_tf32(fmaxf(acc[nt][3] + b1, 0.f));
-    }
+    for (int nt = 0; nt < 16; ++nt) lstm_a_frag(eA[nt], acc[nt][0], acc[nt][1], acc[nt][2], acc[nt][3]);
 
     // ---- gates chunk by chunk, cell update in registers, head product accumulated over the chunks
     float out[NC / 8][4];
@@ -185,36 +154,17 @@ __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams
         const float2 ca = va ? *reinterpret_cast<const float2*>(c_a + u0) : make_float2(0.f, 0.f);
         const float2 cb = vb ? *reinterpret_cast<const float2*>(c_b + u0) : make_float2(0.f, 0.f);
         float gacc[4][4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { gacc[j][0] = gacc[j][1] = gacc[j][2] = gacc[j][3] = 0.f; }
         mbar_wait(&bars[1 + s], (uint32_t)(ch >> 1) & 1u);
-        const float* wc = wlane + s * PL_CHUNK;
-#pragma unroll
-        for (int ks = 0; ks < 32; ++ks) {
-            const uint32_t(&a)[4] = ks < 16 ? eA[ks] : hA[ks - 16];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float2 w = *reinterpret_cast<const float2*>(wc + 8 * j * PL_GP + 8 * ks);
-                mma_tf32(gacc[j], a, __float_as_uint(w.x), __float_as_uint(w.y));
-            }
-        }
+        lstm_gate_chunk(gacc, eA, hA, wlane + s * PL_CHUNK);
         __syncthreads();                           // every warp is done with stage s: refill it with chunk ch + 2
         if (tid == 0 && ch + 2 < PL_CHUNKS) {
             mbar_expect_tx(&bars[1 + s], PL_CHUNK_BYTES);
             tma_load_1d(sWg + s * PL_CHUNK, p.w_gates + (int64_t)(ch + 2) * PL_CHUNK, PL_CHUNK_BYTES, &bars[1 + s]);
         }
         // gacc[j][e]: gate j of (row g, u0), (row g, u0 + 1), (row g + 8, u0), (row g + 8, u0 + 1) for e = 0..3
-        const float* bg = sBg + 32 * ch + 2 * t;
         const float cp[4] = {ca.x, ca.y, cb.x, cb.y};
-        float cn[4], hn[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int q = e & 1;
-            const float zi = gacc[0][e] + bg[q], zf = gacc[1][e] + bg[8 + q];
-            const float zg = gacc[2][e] + bg[16 + q], zo = gacc[3][e] + bg[24 + q];
-            cn[e] = sigmoidf_(zf) * cp[e] + sigmoidf_(zi) * tanhf(zg);
-            hn[e] = sigmoidf_(zo) * tanhf(cn[e]);
-        }
+        float act[4][4], cn[4], hn[4];
+        lstm_cell(gacc, sBg + 32 * ch + 2 * t, cp, act, cn, hn);
         if (va) {
             *reinterpret_cast<float2*>(c_a + u0) = make_float2(cn[0], cn[1]);
             *reinterpret_cast<float2*>(h_a + u0) = make_float2(hn[0], hn[1]);
@@ -223,13 +173,8 @@ __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams
             *reinterpret_cast<float2*>(c_b + u0) = make_float2(cn[2], cn[3]);
             *reinterpret_cast<float2*>(h_b + u0) = make_float2(hn[2], hn[3]);
         }
-        // heads: this chunk is k-step ch of h' W_cat^T, slots t <-> unit u0 and t + 4 <-> unit u0 + 1
-        const uint32_t a[4] = {to_tf32(hn[0]), to_tf32(hn[2]), to_tf32(hn[1]), to_tf32(hn[3])};
-#pragma unroll
-        for (int q = 0; q < NC / 8; ++q) {
-            const float* wh = sWh + (8 * q + g) * PL_XP + u0;
-            mma_tf32(out[q], a, to_tf32(wh[0]), to_tf32(wh[1]));
-        }
+        // heads: this chunk is k-step ch of h' W_cat^T
+        lstm_head_chunk<NC>(out, hn, sWh, g, u0);
     }
 
     // ---- out[q]: (row g, cols 8q + 2t, +1), (row g + 8, same).  Gather the NC columns of a row across its quad.

@@ -129,12 +129,17 @@ class RecurrentPolicy(torch.nn.Module):
 
     ``fused_sample=True``: when sampling under no_grad with a model pb_policy_lstm_sample supports
     (models.LSTMWrapper.fused_supported), the whole step -- encoder, LSTM cell, heads, sampling, row stores -- is ONE
-    kernel and ``state`` is updated in place and returned.  Anything else takes the unfused path."""
+    kernel and ``state`` is updated in place and returned.  Anything else takes the unfused path.
 
-    def __init__(self, policy, fused_sample=False, seed=0):
+    ``fused_update=True``: train() runs the minibatch forward and backward of such a model on the fused BPTT kernels
+    (models.LSTMWrapper.forward_packed_seq: pb_lstm_bptt_forward / _backward) with the fused PPO loss instead of the
+    cuDNN LSTM and the autograd loss; other models keep the cuDNN path."""
+
+    def __init__(self, policy, fused_sample=False, seed=0, fused_update=False):
         super().__init__()
         self.policy = policy
         self.fused_sample = fused_sample
+        self.fused_update = fused_update
         self._seed = int(seed)
         self._counter = None     # device-side draw counter: CUDA-graph replays keep drawing fresh numbers
         self._ticket = None      # exit ticket of pb_policy_lstm_sample (its last CTA advances the counter)

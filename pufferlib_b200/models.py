@@ -95,6 +95,66 @@ class _DefaultMLPFunction(torch.autograd.Function):
                 db_cat[n_act:n_act + 1], None)
 
 
+def _gemm_tn(a, b, split=64):
+    """a^T @ b for a [M, Na], b [M, Nb] with unit column stride (row slices of wider rows are fine): a small output with
+    K = M, so for large M a batched GEMM over `split` K-slices plus a sum gives the library GEMM enough parallel work."""
+    m = a.shape[0]
+    if m % split == 0 and m // split >= 256:
+        return torch.bmm(a.view(split, m // split, -1).transpose(1, 2), b.view(split, m // split, -1)).sum(0)
+    return a.t() @ b
+
+
+class _LSTMBPTTFunction(torch.autograd.Function):
+    """LSTMWrapper(models.Default) over a minibatch of bptt segments as one autograd node (the fused recurrent update).
+
+    forward : pb_lstm_bptt_forward -- encoder, LSTM cell over the T steps and both heads; returns the packed head output
+              out [B*T, R] (n_act logits | value | zero pad, rows b*T + t) and the final state (h_T, c_T) [B, 128], and
+              keeps the saved-activation rows [B*T, 1024] for the backward.
+    backward: pb_lstm_bptt_backward -- dz (the gate pre-activations) and dPre (the encoder pre-activation) in reverse
+              time; the weight gradients are library GEMMs on those buffers (_gemm_tn).  The observations and the initial
+              state get no gradient; neither does the final state (train() hands it on detached)."""
+
+    @staticmethod
+    def forward(ctx, x, h0, c0, ops, w_enc, b_enc, w_ih, w_hh, b_ih, b_hh, w_dec, b_dec, w_val, b_val):
+        from pufferlib_b200 import _native
+        w_enc_p, b_enc_p, w_gates, b_gates, w_cat, b_cat, w_gates_t = ops
+        (bsz, steps, feats), n_act = x.shape, w_dec.shape[0]
+        m = bsz * steps
+        out = x.new_empty(m, w_cat.shape[0])
+        h_out, c_out = x.new_empty(bsz, 128), x.new_empty(bsz, 128)
+        saved = x.new_empty(m, 1024)
+        P = _native.ptr
+        _native.check(_native.lib().pb_lstm_bptt_forward(
+            P(x), x.stride(1), feats, bsz, steps, P(h0), P(c0), P(w_enc_p), P(b_enc_p), P(w_gates), P(b_gates), P(w_cat),
+            P(b_cat), 128, 128, n_act, P(out), P(h_out), P(c_out), P(saved), _native.stream_ptr()))
+        ctx.save_for_backward(x, c0, saved, w_gates_t, w_cat)
+        ctx.n_act = n_act
+        ctx.mark_non_differentiable(h_out, c_out)
+        return out, h_out, c_out
+
+    @staticmethod
+    def backward(ctx, dout, _dh, _dc):
+        from pufferlib_b200 import _native
+        x, c0, saved, w_gates_t, w_cat = ctx.saved_tensors
+        (bsz, steps, feats), n_act = x.shape, ctx.n_act
+        m = bsz * steps
+        dout = dout.contiguous()
+        dz = x.new_empty(m, 512)
+        dpre = x.new_empty(m, 128)
+        P = _native.ptr
+        _native.check(_native.lib().pb_lstm_bptt_backward(
+            P(dout), P(saved), P(c0), P(w_gates_t), P(w_cat), bsz, steps, 128, 128, n_act, P(dz), P(dpre),
+            _native.stream_ptr()))
+        dw_gates = _gemm_tn(dz, saved[:, :256])            # dz^T [e | h_prev] = [dW_ih | dW_hh]
+        db_gates = dz.sum(0)
+        dw_enc = _gemm_tn(dpre, x.reshape(m, feats))
+        dw_cat = _gemm_tn(dout, saved[:, 896:])             # dOut^T h
+        db_cat = dout.sum(0)
+        # b_ih and b_hh get the same gradient, as separate tensors (their .grad must not alias)
+        return (None, None, None, None, dw_enc, dpre.sum(0), dw_gates[:, :128], dw_gates[:, 128:], db_gates,
+                db_gates.clone(), dw_cat[:n_act], db_cat[:n_act], dw_cat[n_act:n_act + 1], db_cat[n_act:n_act + 1])
+
+
 def _round_tf32(w):
     """fp32 -> nearest TF32 value (ties away from zero: cvt.rna), kept as fp32 bits."""
     bits = w.detach().contiguous().view(torch.int32)
@@ -271,6 +331,56 @@ class LSTMWrapper(nn.Module):
         if not torch.is_grad_enabled():
             cache['key'], cache['ops'] = key, ops
         return ops
+
+    def gate_weights_transposed(self):
+        """The gate weights for the backward product of pb_lstm_bptt_backward: [16 * 256, 40] TF32 (cvt.rna); chunk ch,
+        row n, column 8j + u = row 128j + 8ch + u, column n of [W_ih | W_hh]; columns 32..39 zero.  Cached under
+        no_grad, keyed like fused_operands."""
+        cache = self._fused_cache
+        rnn = self.recurrent
+        key = (rnn.weight_ih_l0.data_ptr(), rnn.weight_hh_l0.data_ptr(), torch.cuda.is_current_stream_capturing())
+        if not torch.is_grad_enabled() and cache.get('tkey') == key:
+            return cache['wt']
+        with torch.no_grad():
+            w = _round_tf32(torch.cat([rnn.weight_ih_l0, rnn.weight_hh_l0], dim=1))      # [512, 256]
+            wt = w.new_zeros(16, 256, 40)
+            # w.view(4, 16, 8, 256)[j, ch, u, n] = row 128j + 8ch + u -> [ch, n, 8j + u]
+            wt[:, :, :32] = w.view(4, 16, 8, 256).permute(1, 3, 0, 2).reshape(16, 256, 32)
+            wt = wt.view(16 * 256, 40)
+        if not torch.is_grad_enabled():
+            cache['tkey'], cache['wt'] = key, wt
+        return wt
+
+    def forward_packed_seq(self, x, state=None):
+        """The training forward over bptt segments on the fused kernels (pb_lstm_bptt_forward / _backward):
+        x [B, T, *obs], state (h, c) of shape [1, B, 128] (detached) or None (zeros).  -> (out [B*T, R], n_act,
+        (h_T, c_T) [1, B, 128]) with logits = out[:, :n_act], value = out[:, n_act], rows b*T + t; or None when the fast
+        path does not apply (fused_supported fails, the inner Default's fast_path is off, or the layout is not one the
+        kernel reads).  The packed operands are rebuilt on every call that records gradients."""
+        nd = len(self.obs_shape)
+        if x.dim() != nd + 2 or tuple(x.shape[2:]) != self.obs_shape or x.shape[0] == 0:
+            return None
+        if not (self.fused_supported(x) and getattr(self.policy, 'fast_path', False)):
+            return None
+        bsz, steps = x.shape[:2]
+        x3 = x.reshape(bsz, steps, -1)
+        if x3.stride(2) != 1 or x3.stride(0) != steps * x3.stride(1):
+            return None                     # rows (b, t) must be equally spaced
+        h0 = c0 = None
+        if state is not None:
+            h0, c0 = state
+            for s in (h0, c0):
+                if (tuple(s.shape) != (1, bsz, 128) or s.dtype != torch.float32 or s.device != x.device
+                        or s.requires_grad):
+                    return None
+            h0, c0 = h0[0].contiguous(), c0[0].contiguous()
+        inner, rnn = self.policy, self.recurrent
+        ops = self.fused_operands() + (self.gate_weights_transposed(),)
+        out, h, c = _LSTMBPTTFunction.apply(
+            x3, h0, c0, ops, inner.encoder.weight, inner.encoder.bias, rnn.weight_ih_l0, rnn.weight_hh_l0,
+            rnn.bias_ih_l0, rnn.bias_hh_l0, inner.decoder.weight, inner.decoder.bias, inner.value_head.weight,
+            inner.value_head.bias)
+        return out, inner.decoder.weight.shape[0], (h.unsqueeze(0), c.unsqueeze(0))
 
     def forward(self, x, state):
         nd = len(self.obs_shape)

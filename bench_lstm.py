@@ -11,9 +11,14 @@ Prints one JSON line with
   * `roofline_kernels.policy_lstm_step`: algorithmic HBM bytes 4F + 2048 + 16 per row over the fused step time, against
     the H100 SXM data-sheet 3.35 TB/s; the packed weights each CTA streams from L2 are reported separately;
   * `update`: forward + loss + backward of one training minibatch ([B segments, T = 16 steps] of the rollout), fused
-    (forward_packed_seq + fused_ppo_loss_packed) vs cuDNN (the LSTMWrapper forward + the autograd loss, as train() runs
-    it), in the same process on the same minibatch, from CUDA events; with the algorithmic bytes and TF32 FLOPs per row
-    of the fused path and the share of each data-sheet bound.
+    (forward_packed_seq on the minibatch form train() used: the segment view of the rollout buffer, or the gathered
+    copy) + fused_ppo_loss_packed vs cuDNN (the LSTMWrapper forward on the gathered segments + the autograd loss, as
+    train() runs it), in the same process on the same minibatch, from CUDA events; with the algorithmic bytes and TF32
+    FLOPs per row of the fused path and the share of each data-sheet bound;
+  * `train` (with --fused-update and graphs): train() alone, captured in one CUDA graph vs eager, on two trainers built
+    the same way in one process and alternated, CUDA events around each call, median; the project's kernel launches per
+    train() (pb_launch_count), the peak memory each kind of call allocates beyond what was allocated before it, and the
+    observation bytes the segment view no longer gathers.
 Shared pieces (PPO config, timed steps, card name and power limit) come from bench.py.  Writes nothing to the tree.
 """
 import argparse
@@ -38,6 +43,7 @@ def parse_args():
     ap.add_argument('--reps', type=int, default=256, help='policy steps per timed CUDA graph')
     ap.add_argument('--fused-update', action='store_true', help='train() on the fused BPTT kernels')
     ap.add_argument('--update-reps', type=int, default=10, help='timed minibatch updates per path')
+    ap.add_argument('--train-reps', type=int, default=10, help='timed train() calls per trainer (captured, eager)')
     return ap.parse_args()
 
 
@@ -131,12 +137,19 @@ def update_cost_per_row(feats, n_out, steps):
 
 def update_times(data, reps=10):
     """Device time of forward + loss + backward of one training minibatch (minibatch 0 of the last train(), initial
-    state None), fused (forward_packed_seq + fused_ppo_loss_packed + backward) and cuDNN (the RecurrentPolicy forward
-    over the segments + the autograd loss of train() + backward), alternating, each bracketed by CUDA events; median of
-    `reps` after 2 warm-ups.  The optimizer step is not included."""
+    state None), fused (forward_packed_seq on the minibatch form the last train() read + fused_ppo_loss_packed +
+    backward) and cuDNN (the RecurrentPolicy forward over the gathered segments + the autograd loss of train() +
+    backward), alternating, each bracketed by CUDA events; median of `reps` after 2 warm-ups.  The optimizer step is not
+    included.  -> (times, (segments, bptt), minibatch form)."""
     from pufferlib_b200 import clean_pufferl as cp
     policy, exp, cfg = data.policy, data.experience, data.config
-    obs, atn, lp = exp.b_obs[0], exp.b_actions[0], exp.b_logprobs[0]
+    form = data.train_minibatch_path
+    if form == 'segments':       # [E, G, T, *obs] view of the rollout buffer; the cuDNN forward gets a gathered copy
+        seg = exp.segment_obs(0)
+        obs, obs_g = seg, seg.reshape(-1, *seg.shape[2:])
+    else:
+        obs = obs_g = exp.b_obs[0]
+    atn, lp = exp.b_actions[0], exp.b_logprobs[0]
     val, ret, adv = exp.b_values[0], exp.b_returns[0], exp.b_advantages[0]
     model = policy.policy
 
@@ -146,7 +159,7 @@ def update_times(data, reps=10):
         loss.backward()
 
     def cudnn():
-        _, newlogprob, entropy, newvalue, _ = policy(obs, state=None, action=atn)
+        _, newlogprob, entropy, newvalue, _ = policy(obs_g, state=None, action=atn)
         ratio = (newlogprob - lp.reshape(-1)).exp()
         a = adv.reshape(-1)
         pg = torch.max(-a * ratio, -a * torch.clamp(ratio, 1 - cfg.clip_coef, 1 + cfg.clip_coef)).mean()
@@ -169,15 +182,16 @@ def update_times(data, reps=10):
             if i >= 2:
                 times[k].append(e0.elapsed_time(e1) * 1e-3)
     policy.zero_grad(set_to_none=True)
-    return {k: float(np.median(v)) for k, v in times.items()}, tuple(obs.shape[:2])
+    return {k: float(np.median(v)) for k, v in times.items()}, tuple(obs_g.shape[:2]), form
 
 
-def main(args):
+def make_trainer(args, train_graph):
+    """Vecenv, RecurrentPolicy(LSTMWrapper(Default)) and trainer, the same for every call but for `train_graph`
+    (config.cuda_graph_train); the rollout is captured unless --no-graph."""
     import pufferlib_b200.vector as pvec
     from pufferlib_b200 import clean_pufferl as cp, models
     from pufferlib_b200.environments import ocean
     from pufferlib_b200.frameworks import cleanrl
-    torch.cuda.set_device(0)
     n, h = args.num_envs, args.horizon
     vec = pvec.make(ocean.env_creator(args.env), num_envs=n, backend=pvec.B200.options(exact_infos=False))
     torch.manual_seed(1)
@@ -186,15 +200,65 @@ def main(args):
     policy = cleanrl.RecurrentPolicy(net, fused_sample=True, seed=1, fused_update=args.fused_update).cuda()
     cfg = ppo_config(n, h, 'cuda', seed=1, cuda_graph=not args.no_graph, minibatches=args.minibatches,
                      epochs=args.epochs, env=args.env)
-    data = cp.create(cfg, vec, policy)
+    cfg.cuda_graph_train = train_graph
+    return cp.create(cfg, vec, policy)
+
+
+def train_peak(cp, data):
+    """One train(); -> (bytes allocated at its peak beyond what was allocated before it, pb_launch_count delta)."""
+    from pufferlib_b200 import _native
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    base, l0 = torch.cuda.memory_allocated(), _native.lib().pb_launch_count()
+    cp.train(data)
+    torch.cuda.synchronize()
+    return torch.cuda.max_memory_allocated() - base, _native.lib().pb_launch_count() - l0
+
+
+def train_times(args, graphed):
+    """train() alone, captured (`graphed`, already warmed up: eager call, then capture + first replay) vs eager (a
+    second trainer built the same way, config.cuda_graph_train=False), alternating; each call after its own rollout,
+    bracketed by CUDA events (train() ends in its one device-to-host read, so the events span the whole call, host
+    launch gaps included); median of --train-reps after 2 warm-ups per trainer."""
+    from pufferlib_b200 import clean_pufferl as cp
+    eager = make_trainer(args, train_graph=False)
+    runs = {'captured': graphed, 'eager': eager}
+    times = {k: [] for k in runs}
+    peaks, launches = {}, {}
+    for i in range(args.train_reps + 2):
+        for k, d in runs.items():
+            cp.evaluate(d)
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            cp.train(d)
+            e1.record()
+            torch.cuda.synchronize()
+            if i >= 2:
+                times[k].append(e0.elapsed_time(e1) * 1e-3)
+    for k, d in runs.items():            # one more call each, untimed: memory and launches
+        cp.evaluate(d)
+        peaks[k], launches[k] = train_peak(cp, d)
+    state, paths = eager.train_graph_state, (graphed.train_recurrent_path, eager.train_recurrent_path)
+    cp.close(eager)
+    return {k: float(np.median(v)) for k, v in times.items()}, peaks, launches, state, paths
+
+
+def main(args):
+    from pufferlib_b200 import clean_pufferl as cp
+    torch.cuda.set_device(0)
+    n, h = args.num_envs, args.horizon
+    data = make_trainer(args, train_graph=not args.no_graph)
+    vec, policy = data.vecenv, data.policy
+    warm_peaks = []           # per warm-up train(): the first is eager; with a captured update the second captures
     for _ in range(max(args.warmup, 2)):
         cp.evaluate(data)
-        cp.train(data)
+        warm_peaks.append(train_peak(cp, data)[0])
     ms = timed_steps(data, cp, args.steps, 1)
     prof = {k: round(v, 4) for k, v in dict(data.profile).items() if k.endswith('_time')}
-    recurrent_path = data.train_recurrent_path
+    recurrent_path, minibatch_path = data.train_recurrent_path, data.train_minibatch_path
     times = policy_step_times(data, args.reps)
-    upd, (seg, bptt) = update_times(data, args.update_reps)
+    upd, (seg, bptt), form = update_times(data, args.update_reps)
     n_act = vec.single_action_space.n
     n_out = -(-(n_act + 1) // 8) * 8
     # algorithmic HBM bytes of one fused step: x (4F), h and c read and written (4 x 512), value + logprob + action (16)
@@ -213,7 +277,8 @@ def main(args):
                                'fused_sample=True', 'global_batch': n * h, 'minibatch_size': n * h // args.minibatches,
                    'update_epochs': args.epochs, 'bptt_horizon': 16, 'cuda_graph_rollout': not args.no_graph,
                    'update': 'fused BPTT kernels' if args.fused_update else 'cuDNN LSTM autograd',
-                   'train_recurrent_path': recurrent_path},
+                   'train_recurrent_path': recurrent_path, 'train_minibatch_path': minibatch_path,
+                   'train_graph_state': data.train_graph_state},
         'policy_step': {
             'fused_us': round(t_f * 1e6, 2), 'unfused_us': round(t_u * 1e6, 2), 'speedup': round(t_u / t_f, 2),
             'fused_eager_us': round(times['fused']['eager_seconds'] * 1e6, 2),
@@ -226,11 +291,35 @@ def main(args):
             'avg_launch_us': round(t_f * 1e6, 2), 'achieved': round(step_bytes / t_f / 1e9, 1),
             'frac': round(bound_s / t_f, 4), 'launches_per_step': h,
             'l2_weight_bytes_per_cta': weight_bytes, 'l2_weight_bytes_per_launch': weight_bytes * ctas}},
-        'update': update_section(upd, seg, bptt, feats, n_out),
+        'update': dict(update_section(upd, seg, bptt, feats, n_out), fused_minibatch_form=form),
+        'train': train_section(args, data, warm_peaks, feats),
         'gpu': gpu_info(0), 'profile_s': prof, 'env_stats': {k: float(v) for k, v in data.stats.items()},
     }
     print(json.dumps(line))
     cp.close(data)
+
+
+def train_section(args, data, warm_peaks, feats):
+    n, h = args.num_envs, args.horizon
+    if data.train_graph_state != 2:
+        return {'skipped': f'the update of this run is not captured (train_graph_state {data.train_graph_state}, path '
+                           f'{data.train_recurrent_path}; captured updates need --fused-update and graphs)'}
+    t, peaks, launches, eager_state, paths = train_times(args, data)
+    gather_bytes = 2 * h * n * 4 * feats           # pb_minibatch_gather: every observation row read once, written once
+    return {
+        'captured_ms': round(t['captured'] * 1e3, 3), 'eager_ms': round(t['eager'] * 1e3, 3),
+        'eager_over_captured': round(t['eager'] / t['captured'], 3),
+        'method': 'train() alone, two trainers built the same way, alternated; CUDA events around each call, median of '
+                  f'{args.train_reps}',
+        'recurrent_path': {'captured': paths[0], 'eager': paths[1]}, 'eager_train_graph_state': eager_state,
+        'launches_per_train': {'captured': {'graph_launches': 1, 'project_kernels_in_graph': data.train_graph_launches,
+                                            'project_kernels_launched_from_python': launches['captured']},
+                               'eager': {'project_kernels_launched_from_python': launches['eager']},
+                               'note': 'pb_launch_count counts this project\'s kernels only, not torch / cuBLAS ones'},
+        'peak_bytes_beyond_allocated': {'eager_first_call': warm_peaks[0], 'capture_call': warm_peaks[1],
+                                        'replay': peaks['captured'], 'eager': peaks['eager']},
+        'obs_gather_bytes_saved_per_train': gather_bytes, 'b_obs_bytes_not_allocated': h * n * 4 * feats,
+    }
 
 
 def update_section(upd, seg, bptt, feats, n_out):

@@ -291,6 +291,33 @@ int pb_lstm_bptt_backward(const float* dout, const float* saved, const float* c0
                           const float* w_heads, int64_t batch, int32_t steps, int32_t input_size, int32_t hidden_size,
                           int32_t n_act, float* dz, float* dpre, void* stream);
 
+/* The same two kernels on strided observation rows, so that a minibatch can be read in place from the rollout buffer.
+ * Segment b of the batch is (e, g) = (b / groups, b % groups); batch % groups == 0.  Strides are in floats.
+ * pb_lstm_bptt_forward_rows: obs row (b, t) at obs + (b / groups) * stride_e + (b % groups) * stride_g + t * stride_t;
+ *   stride_e, stride_t (and stride_g when groups > 1) >= in_features.  h0, c0, out, h_out, c_out and saved keep the
+ *   dense (b, t) order of pb_lstm_bptt_forward, which is the case groups = 1, stride_e = T * obs_stride,
+ *   stride_t = obs_stride.
+ * pb_lstm_bptt_backward_rows: dpre row (b, t) at dpre + (b / groups) * dpre_stride_e + (b % groups) * dpre_stride_g +
+ *   t * dpre_stride_t; those strides even and >= 128 (dpre_stride_g only checked when groups > 1).  dz keeps row b*T + t.
+ *   pb_lstm_bptt_backward is the case groups = 1, dpre_stride_e = 128 T, dpre_stride_t = 128.
+ * The segment view of Experience.segment_obs: minibatch mb of the reference (segments r = e*G + g, G = S / n_mb time
+ * windows of T = bptt steps per env, S = horizon / bptt, n_mb | S) read from the arrival-order obs [horizon][N][F]:
+ *   obs + mb*T*N*F, groups = G, stride_e = F, stride_g = n_mb*T*N*F, stride_t = N*F.
+ * With dpre_stride_e = 128, dpre_stride_g = 128 T N, dpre_stride_t = 128 N, dPre row (b, t) lands at ((b % G) T + t) N
+ * + b / G: G slabs of T*N rows in the order of the observation slabs obs + (g*n_mb + mb)*T*N*F, so that
+ * dW_enc = sum_g dPre_g^T x_g.  Both compute bitwise what the dense entry points compute on the gathered copy (only the
+ * load and store addresses differ).  PB_ERR_INVALID (before any launch) for groups < 1, batch % groups != 0, strides
+ * below a row, null or misaligned pointers; PB_ERR_UNSUPPORTED as above; PB_OK without a launch for batch = 0. */
+int pb_lstm_bptt_forward_rows(const float* obs, int32_t in_features, int64_t batch, int32_t steps, int32_t groups,
+                              int64_t stride_e, int64_t stride_g, int64_t stride_t, const float* h0, const float* c0,
+                              const float* w_enc, const float* b_enc, const float* w_gates, const float* b_gates,
+                              const float* w_heads, const float* b_heads, int32_t input_size, int32_t hidden_size,
+                              int32_t n_act, float* out, float* h_out, float* c_out, float* saved, void* stream);
+int pb_lstm_bptt_backward_rows(const float* dout, const float* saved, const float* c0, const float* w_gates_t,
+                               const float* w_heads, int64_t batch, int32_t steps, int32_t input_size,
+                               int32_t hidden_size, int32_t n_act, int32_t groups, int64_t dpre_stride_e,
+                               int64_t dpre_stride_g, int64_t dpre_stride_t, float* dz, float* dpre, void* stream);
+
 /* -- persistent rollout (env steps with the policy in the loop) -------------------------------------------------------
  * The H-iteration body of clean_pufferl.evaluate (clean_pufferl.py:84-124: recv -> policy -> store -> send) for a
  * breakout handle and models.Default (128 features, 128 hidden, n_act <= 4) in ONE launch: a CTA owns 128 envs for all

@@ -86,6 +86,10 @@ SIGNATURES = {
                              + [C.c_int32] * 3 + [C.c_void_p] * 4 + [C.c_void_p]),
     'pb_lstm_bptt_backward': (C.c_int, [C.c_void_p] * 5 + [C.c_int64] + [C.c_int32] * 4 + [C.c_void_p] * 2
                               + [C.c_void_p]),
+    'pb_lstm_bptt_forward_rows': (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32] + [C.c_int64] * 3
+                                  + [C.c_void_p] * 8 + [C.c_int32] * 3 + [C.c_void_p] * 4 + [C.c_void_p]),
+    'pb_lstm_bptt_backward_rows': (C.c_int, [C.c_void_p] * 5 + [C.c_int64] + [C.c_int32] * 5 + [C.c_int64] * 3
+                                   + [C.c_void_p] * 2 + [C.c_void_p]),
     'pb_mlp_tail_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int32]),
     'pb_mlp_tail_backward': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
                              C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -672,8 +672,9 @@ class Experience:
             advantages=self.advantages_tm[lo:], row_slab_stride=self.num_minibatches * r_,
             adv_norm=self.adv_norm[mb] if norm_adv else None)
 
-    def flatten_batch(self, advantages=None):
-        """clean_pufferl.py:466-482 (advantages: sorted-order device tensor, default self.advantages)."""
+    def flatten_batch(self, advantages=None, gather_obs=True):
+        """clean_pufferl.py:466-482 (advantages: sorted-order device tensor, default self.advantages).  gather_obs=False
+        skips the observation gather (b_obs): the recurrent update then reads segment_obs() views instead."""
         adv = self.advantages if advantages is None else advantages
         n, h = self.num_envs, self.horizon
         lib, s = _native.lib(), _native.stream_ptr()
@@ -682,6 +683,8 @@ class Experience:
             _native.ptr(adv), _native.ptr(self.b_actions), _native.ptr(self.b_logprobs), _native.ptr(self.b_dones),
             _native.ptr(self.b_values), _native.ptr(self.b_advantages), _native.ptr(self.b_returns),
             _native.ptr(self.returns), n, h, self.num_minibatches, self.minibatch_rows, self.bptt_horizon, s))
+        if not gather_obs:
+            return
         _native.check(lib.pb_minibatch_gather(
             _native.ptr(self.obs), _native.ptr(self.b_obs), self.obs_row_bytes, n, h, self.num_minibatches,
             self.minibatch_rows, self.bptt_horizon, 0, self.num_minibatches, s))
@@ -721,6 +724,17 @@ class Experience:
         """Observations of minibatch mb as a zero-copy view [G, bptt*N, *obs] of the rollout buffer."""
         g_, r_ = self._slabs.shape
         return self.obs.view(g_, self.num_minibatches, r_, *self.obs_shape)[:, mb]
+
+    def segment_obs(self, mb):
+        """Observations of minibatch mb of clean_pufferl.py:466-482 for a recurrent policy, as a zero-copy view
+        [N, G, bptt, *obs] of the rollout buffer (needs slab_layout).  Row r of the reference's minibatch is bptt segment
+        s = r*nm + mb; with S = H/bptt a multiple of nm that is env e = r // G in time window k = (r % G)*nm + mb, whose
+        step j is arrival row (k*bptt + j)*N + e.  So view [e, g, j] = segment r = e*G + g, and the segments keep the
+        reference's row order (the state carried between minibatches means the same)."""
+        n, nm, bptt = self.num_envs, self.num_minibatches, self.bptt_horizon
+        g_, _ = slab_layout(n, self.horizon, nm, bptt)
+        nd = len(self.obs_shape)
+        return self.obs.view(g_, nm, bptt, n, *self.obs_shape)[:, mb].permute(2, 0, 1, *range(3, 3 + nd))
 
     def normalize_advantages(self, slabs=False):
         """clean_pufferl.py:211-213 for every minibatch at once -> self.b_advantages_normalized."""
@@ -911,6 +925,17 @@ def _rollout_loop(data, infos):
         vecenv.join()            # pool mode: side-stream env steps rejoin the caller's stream (and any graph capture)
 
 
+def _recurrent_update_fused(data):
+    """Does train() run the recurrent update on the fused BPTT kernels (LSTMWrapper.forward_packed_seq)?  Decided on the
+    host from what forward_packed_seq checks, so that it is known before any capture: RecurrentPolicy(fused_update=True),
+    config.fused_loss, a model the kernels cover (fused_supported on the rollout observations) and the inner Default's
+    fast_path."""
+    experience, model = data.experience, getattr(data.policy, 'policy', None)
+    return (experience.lstm_h is not None and bool(getattr(data.policy, 'fused_update', False))
+            and bool(getattr(data.config, 'fused_loss', True)) and hasattr(model, 'forward_packed_seq')
+            and model.fused_supported(experience.obs) and bool(getattr(model.policy, 'fast_path', False)))
+
+
 def _invalidate_policy_cache(data):
     model = getattr(data.policy, 'policy', None)
     if hasattr(model, 'invalidate_cache'):
@@ -1024,6 +1049,9 @@ def _train_device_part(data, seg=None):
     model = getattr(data.policy, 'policy', None)
     want_slabs = data.fused_loss and experience.lstm_h is None and hasattr(model, 'forward_packed_slabs') and \
         bool(getattr(config, 'zero_copy_minibatches', True))
+    # recurrent models: the fused BPTT update when the policy asks for it and the model is covered (RecurrentPolicy(
+    # fused_update=True); data.train_recurrent_path records which path ran)
+    rec_fused = _recurrent_update_fused(data)
     manual = None
     if _DefaultMLPUpdate.eligible(data):
         if getattr(data, 'manual_update', None) is None or data.manual_update.stale():
@@ -1031,6 +1059,9 @@ def _train_device_part(data, seg=None):
         manual = data.manual_update
     with profile.train_misc:
         experience.sort_training_data()
+        # the fused recurrent update reads its minibatch segments in place (Experience.segment_obs): no b_obs copy
+        segments = rec_fused and bool(getattr(config, 'zero_copy_minibatches', True)) and slab_layout(
+            experience.num_envs, experience.horizon, experience.num_minibatches, experience.bptt_horizon) is not None
         # the fused update kernel reads the ARRIVAL-order rollout tensors through slab strides: no minibatch copies at all
         # (GAE writes the advantages in arrival order as well; the advantage normalisation constants are applied on the fly)
         direct = want_slabs and manual is not None and experience.direct_slabs_ok(manual, config)
@@ -1042,11 +1073,12 @@ def _train_device_part(data, seg=None):
             experience.compute_gae(config.gamma, config.gae_lambda)
             slabs = want_slabs and experience.flatten_batch_slabs()
             if not slabs:
-                experience.flatten_batch()
+                experience.flatten_batch(gather_obs=not segments)
             if config.norm_adv:
                 experience.normalize_advantages(slabs=slabs)
-    # which minibatch form the update reads: rollout tensors in place, slab copies of the per-row tensors, or gathered copies
-    data.train_minibatch_path = 'direct' if direct else ('slabs' if slabs else 'gathered')
+    # which minibatch form the update reads: rollout tensors in place, slab copies of the per-row tensors, segment views of
+    # the observations (recurrent), or gathered copies
+    data.train_minibatch_path = 'direct' if direct else ('slabs' if slabs else ('segments' if segments else 'gathered'))
 
     n_mb = experience.num_minibatches
     if seg is not None:                        # persistent accumulator: the segment graphs update it in place
@@ -1058,10 +1090,6 @@ def _train_device_part(data, seg=None):
         acc = torch.zeros(6, device=device)    # policy, value, entropy, old_kl, kl, clipfrac
     obs_shape = data.vecenv.single_observation_space.shape
     fused = data.fused_loss and experience.lstm_h is None
-    # recurrent models: the fused BPTT update when the policy asks for it (RecurrentPolicy(fused_update=True)); the
-    # model decides per minibatch whether it applies (data.train_recurrent_path records which path ran)
-    rec_fused = experience.lstm_h is not None and bool(getattr(data.policy, 'fused_update', False)) and \
-        bool(getattr(config, 'fused_loss', True))
     carry = {'lstm_state': None, 'approx_kl': None}
     if manual is not None:
         manual.pack_heads()                      # the parameters may have changed since the last train() (checkpoints)
@@ -1080,7 +1108,7 @@ def _train_device_part(data, seg=None):
             atn, log_probs, val, ret = sl.actions[mb], sl.logprobs[mb], sl.values[mb], sl.returns[mb]
             adv = sl.advantages_normalized[mb] if config.norm_adv else sl.advantages[mb]
         else:
-            obs = experience.b_obs[mb]
+            obs = experience.segment_obs(mb) if segments else experience.b_obs[mb]
             atn = experience.b_actions[mb]
             log_probs = experience.b_logprobs[mb]
             val = experience.b_values[mb]
@@ -1103,7 +1131,7 @@ def _train_device_part(data, seg=None):
                 if packed is None:
                     logits, newvalue = model(obs.reshape(-1, *obs_shape))
             elif experience.lstm_h is not None:       # clean_pufferl.py:188-191: [rows, bptt, *obs] segments
-                if rec_fused and hasattr(getattr(data.policy, 'policy', None), 'forward_packed_seq'):
+                if rec_fused:
                     packed = data.policy.policy.forward_packed_seq(obs, carry['lstm_state'])
                 if packed is not None:     # BPTT kernels; the loss hands back ONE [B*T, R] gradient
                     st_ = packed[2]
@@ -1200,9 +1228,10 @@ def _train_device_part(data, seg=None):
 
 
 def train(data):
-    """One PPO update (reference: clean_pufferl.py:156-292).  With ``config.cuda_graph`` (no target_kl, no
-    LSTM) the device part is captured once -- after an eager first call that initialises the optimizer state -- and
-    replayed as ONE graph launch; the learning rate lives in a device tensor so annealing works under replay."""
+    """One PPO update (reference: clean_pufferl.py:156-292).  With ``config.cuda_graph`` (no target_kl; recurrent
+    policies only on one GPU with the fused BPTT update) the device part is captured once -- after an eager first call
+    that initialises the optimizer state -- and replayed as ONE graph launch; the learning rate lives in a device tensor
+    so annealing works under replay."""
     config, profile, experience = data.config, data.profile, data.experience
     data.losses = make_losses()
     losses = data.losses
@@ -1221,8 +1250,11 @@ def train(data):
     # memory) keeps the update out of ONE graph; with the peer all-reduce fused into pb_clip_adam_peer there is none
     mu = getattr(data, 'manual_update', None)
     nccl_in_loop = data.grad_bucket is not None and not (mu is not None and (mu.world == 1 or mu.peer is not None))
+    # a recurrent update is captured only on the fused BPTT kernels (decided on the host, before any capture) and without
+    # a gradient all-reduce; the cuDNN path stays eager
+    rec_graphable = experience.lstm_h is not None and data.grad_bucket is None and _recurrent_update_fused(data)
     graphable = want_graph and not nccl_in_loop and \
-        config.target_kl is None and experience.lstm_h is None and data.train_graph_state >= 0
+        config.target_kl is None and (experience.lstm_h is None or rec_graphable) and data.train_graph_state >= 0
     segmented = want_graph and nccl_in_loop and \
         config.target_kl is None and experience.lstm_h is None and data.train_graph_state >= 0
     if segmented and data.train_graph_state >= 1:
@@ -1239,11 +1271,21 @@ def train(data):
                 torch.cuda.synchronize()
                 launches0 = _native.lib().pb_launch_count()
                 graph = torch.cuda.CUDAGraph()
+                data.train_recurrent_path = None
                 with torch.cuda.graph(graph):
                     data.train_result = _train_device_part(data)
-                data.train_graph = graph
-                data.train_graph_launches = _native.lib().pb_launch_count() - launches0
-                data.train_graph_state = 2
+                if experience.lstm_h is not None and data.train_recurrent_path != 'fused':
+                    # the captured recurrent update did not run on the BPTT kernels: keep it eager (capture ran nothing)
+                    del graph
+                    data.train_result, data.train_graph_state = None, -1
+                    data.msg = (f'train graph dropped: the recurrent update took the {data.train_recurrent_path} path; '
+                                'running eager')
+                    torch.cuda.synchronize()
+                    result = _train_device_part(data)
+                else:
+                    data.train_graph = graph
+                    data.train_graph_launches = _native.lib().pb_launch_count() - launches0
+                    data.train_graph_state = 2
             except Exception as e:          # capture is an optimisation: fall back to eager for good
                 data.train_graph_state = -1
                 data.msg = f'train graph capture failed ({type(e).__name__}: {e}); running eager'

@@ -27,6 +27,15 @@
 // (row, unit) pairs are directly the A fragments of four k-steps (the k-slot trick) and the B fragments are conflict-free
 // 64-bit loads (pitch 40).  The weight gradients are library GEMMs on dz, dPre and the saved rows (models.py).
 //
+// Row addresses.  Segment b = (e, g) = (b / G, b % G) reads x(b, t) = obs + e s_e + g s_g + t s_t and writes dPre row
+// (b, t) at dpre + e d_e + g d_g + t d_t; every other buffer stays dense in row b*T + t.  pb_lstm_bptt_forward / _backward
+// are the gathered case (G = 1: a contiguous [B, T, F] copy, dPre row b*T + t); the _rows entry points also take the
+// segment view of Experience.segment_obs, which reads minibatch mb of the reference in place from the arrival-order
+// rollout buffer and writes dPre in the order of its G observation slabs (layouts in include/pufferlib_b200.h).  The
+// forward computes its CTA's 128 x-row bases once (pad columns of the x tile); the backward its two dPre row bases once
+// per thread.  Nothing else changes: the same values reach the same fragment slots, so both layouts give bitwise the
+// same out, state, saved rows, dz and (permuted) dPre.
+//
 // Saved-activation row (1024 floats = 4096 B per (b, t) row): [e (128) | h_prev (128) | sigmoid(i) | sigmoid(f) |
 // tanh(g) | sigmoid(o) (4 x 128, unit-major) | c_t (128) | h_t (128)]; [e | h_prev] is the operand of dW_ih | dW_hh,
 // h_t that of dW_cat.  At B*T = 524 288 rows (breakout's minibatch) that is 2.1 GB.
@@ -40,7 +49,7 @@
 // accumulation, biases and the cell fp32), so the forward at T = 1 computes what the rollout step computes.  In the
 // backward, dz (and the packed weights, on the host) are rounded to TF32 for the product; everything else is fp32.
 //
-// Resources (nvcc 12.9 -Xptxas -v, sm_90a): forward 218 176 B shared memory, 213 / 216 registers (8 / 16 head
+// Resources (nvcc 12.9 -Xptxas -v, sm_90a): forward 218 176 B shared memory, 211 / 216 registers (8 / 16 head
 // columns); backward 221 184 B shared memory, 232 registers; no spills.  Time (bench_lstm.py, H100 80GB HBM3,
 // 700 W power limit): forward + loss + backward of a 524 288-row minibatch 7.53 ms, vs 35.65 ms on cuDNN autograd.
 #include "lstm_cell.cuh"
@@ -84,7 +93,7 @@ static_assert(BWD_SMEM <= 227 * 1024, "shared memory over the sm_90 per-CTA limi
 static_assert(BW_CHUNK_BYTES % 16 == 0, "bulk copy alignment");
 
 struct FwdParams {
-    const float* obs; int64_t obs_stride; int in_features;
+    const float* obs; int64_t s_e, s_g, s_t; int groups; int in_features;   // x(b, t) = obs + (b/G) s_e + (b%G) s_g + t s_t
     int64_t batch; int steps;
     const float* h0; const float* c0;              // [B][128] or null (zeros)
     const float* w_enc; const float* b_enc;        // [128][136] TF32, [128]
@@ -98,6 +107,7 @@ struct BwdParams {
     const float* w_gates_t; const float* w_heads;  // [16][256][40] TF32, [NC][128]
     int64_t batch; int steps; int n_act;
     float* dz; float* dpre;
+    int groups; int64_t d_e, d_g, d_t;             // dPre row (b, t) at dpre + (b/G) d_e + (b%G) d_g + t d_t
 };
 
 // this thread's slot of a [chunk][warp][lane] float4 fragment array
@@ -108,6 +118,9 @@ __device__ __forceinline__ float2 ld2(const float* p, bool ok) {
     return ok ? *reinterpret_cast<const float2*>(p) : make_float2(0.f, 0.f);
 }
 __device__ __forceinline__ void st2(float* p, float a, float b) { *reinterpret_cast<float2*>(p) = make_float2(a, b); }
+// x-row base of local segment r (floats from obs), kept in the pad columns 128..129 of the x tile's row r: the tile load
+// writes and lstm_encoder reads columns < 128 only, so the 128 bases are computed once and cost no shared memory
+__device__ __forceinline__ int64_t* xrow(float* sX, int r) { return reinterpret_cast<int64_t*>(sX + r * PL_XP + PL_F); }
 
 template <int NC>
 __global__ void __launch_bounds__(BT_THREADS, 1) k_lstm_bptt_fwd(FwdParams p) {
@@ -146,6 +159,10 @@ __global__ void __launch_bounds__(BT_THREADS, 1) k_lstm_bptt_fwd(FwdParams p) {
     for (int i = tid; i < 4 * PL_H; i += BT_THREADS) sBg[i] = p.b_gates[i];
     for (int i = tid; i < NC * PL_H; i += BT_THREADS) sWh[(i >> 7) * PL_XP + (i & (PL_H - 1))] = p.w_heads[i];
     if (tid < NC) sBh[tid] = p.b_heads[tid];
+    if (tid < BT_ROWS) {                           // visible after the first barrier of phase 1
+        const int64_t b = b0 + tid;
+        *xrow(sX, tid) = (b / p.groups) * p.s_e + (b % p.groups) * p.s_g;
+    }
 
     const int lr = 16 * warp + g;                  // local segments lr (fragment rows g) and lr + 8 (g + 8)
     const bool va = lr < valid, vb = lr + 8 < valid;
@@ -157,7 +174,7 @@ __global__ void __launch_bounds__(BT_THREADS, 1) k_lstm_bptt_fwd(FwdParams p) {
         __syncthreads();                           // the previous step's tile is consumed
         for (int i = tid; i < BT_ROWS * PL_F; i += BT_THREADS) {
             const int r = i >> 7, k = i & (PL_F - 1);
-            sX[r * PL_XP + k] = (r < valid && k < F) ? p.obs[((b0 + r) * T + st) * p.obs_stride + k] : 0.f;
+            sX[r * PL_XP + k] = (r < valid && k < F) ? p.obs[*xrow(sX, r) + st * p.s_t + k] : 0.f;
         }
         __syncthreads();
         if (st == 0) mbar_wait(&bars[0], 0);
@@ -289,6 +306,9 @@ __global__ void __launch_bounds__(BT_THREADS, 1) k_lstm_bptt_bwd(BwdParams p) {
     const int lr = 16 * warp + g;
     const bool va = lr < valid, vb = lr + 8 < valid;
     const int64_t ra0 = (b0 + lr) * T, rb0 = ra0 + 8 * (int64_t)T;
+    const int64_t ba = b0 + lr, bb = ba + 8;       // dPre rows (b, 0) of the two segments
+    float* const dpa = p.dpre + (ba / p.groups) * p.d_e + (ba % p.groups) * p.d_g;
+    float* const dpb = p.dpre + (bb / p.groups) * p.d_e + (bb % p.groups) * p.d_g;
     const float* wlane = sWt + g * BW_P + 2 * t;
     // acc[0..15]: de (n-tile nt = encoder units 8nt..), acc[16 + ch]: dh_{t-1} of chunk ch, both in chunk element order
     float acc[32][4];
@@ -384,8 +404,8 @@ __global__ void __launch_bounds__(BT_THREADS, 1) k_lstm_bptt_bwd(BwdParams p) {
         for (int nt = 0; nt < 16; ++nt) {
             const int k = 8 * nt + 2 * t;
             const float2 ea = ld2(sa + SV_E + k, va), eb = ld2(sb + SV_E + k, vb);
-            if (va) st2(p.dpre + ra * PL_H + k, ea.x > 0.f ? acc[nt][0] : 0.f, ea.y > 0.f ? acc[nt][1] : 0.f);
-            if (vb) st2(p.dpre + rb * PL_H + k, eb.x > 0.f ? acc[nt][2] : 0.f, eb.y > 0.f ? acc[nt][3] : 0.f);
+            if (va) st2(dpa + st * p.d_t + k, ea.x > 0.f ? acc[nt][0] : 0.f, ea.y > 0.f ? acc[nt][1] : 0.f);
+            if (vb) st2(dpb + st * p.d_t + k, eb.x > 0.f ? acc[nt][2] : 0.f, eb.y > 0.f ? acc[nt][3] : 0.f);
         }
     }
 }
@@ -400,6 +420,61 @@ int launch(K kernel, const P& p, size_t smem, cudaStream_t stream) {
 
 bool aligned(const void* ptr, uintptr_t a) { return ((uintptr_t)ptr & (a - 1)) == 0; }
 
+// The checks and launch behind both forward entry points: x(b, t) = obs + (b / G) s_e + (b % G) s_g + t s_t (floats)
+int forward_rows(const char* fn, const float* obs, int32_t in_features, int64_t batch, int32_t steps, int32_t groups,
+                 int64_t s_e, int64_t s_g, int64_t s_t, const float* h0, const float* c0, const float* w_enc,
+                 const float* b_enc, const float* w_gates, const float* b_gates, const float* w_heads,
+                 const float* b_heads, int32_t input_size, int32_t hidden_size, int32_t n_act, float* out, float* h_out,
+                 float* c_out, float* saved, void* stream) {
+    PB_REQUIRE(batch >= 0 && steps >= 1, PB_ERR_INVALID, "%s: need batch >= 0 and steps >= 1", fn);
+    PB_REQUIRE(groups >= 1 && batch % groups == 0, PB_ERR_INVALID, "%s: need groups >= 1 dividing batch (got %d, %lld)",
+               fn, groups, (long long)batch);
+    PB_REQUIRE(in_features >= 1 && in_features <= PL_F, PB_ERR_UNSUPPORTED,
+               "%s: observation features must be in [1, %d] (got %d)", fn, PL_F, in_features);
+    PB_REQUIRE(input_size == PL_H && hidden_size == PL_H, PB_ERR_UNSUPPORTED,
+               "%s: built for LSTM input and hidden size %d (got %d, %d)", fn, PL_H, input_size, hidden_size);
+    PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "%s: n_act must be in [1, 15]", fn);
+    if (batch == 0) return PB_OK;
+    PB_REQUIRE(obs && w_enc && b_enc && w_gates && b_gates && w_heads && b_heads && out && h_out && c_out && saved,
+               PB_ERR_INVALID, "%s: null pointer", fn);
+    PB_REQUIRE(s_e >= in_features && s_t >= in_features && (groups == 1 || s_g >= in_features), PB_ERR_INVALID,
+               "%s: observation strides must be at least in_features", fn);
+    PB_REQUIRE(aligned(w_enc, 16) && aligned(w_gates, 16), PB_ERR_INVALID, "%s: w_enc / w_gates must be 16-byte aligned",
+               fn);
+    PB_REQUIRE(aligned(out, 8) && aligned(h_out, 8) && aligned(c_out, 8) && aligned(saved, 8) && aligned(h0, 8) &&
+                   aligned(c0, 8),
+               PB_ERR_INVALID, "%s: out / h / c / saved must be 8-byte aligned", fn);
+    FwdParams p{obs, s_e, s_g, s_t, groups, in_features, batch, steps, h0, c0, w_enc, b_enc, w_gates, b_gates, w_heads,
+                b_heads, out, h_out, c_out, saved};
+    cudaStream_t s = (cudaStream_t)stream;
+    return n_act + 1 <= 8 ? launch(k_lstm_bptt_fwd<8>, p, FWD_SMEM, s) : launch(k_lstm_bptt_fwd<16>, p, FWD_SMEM, s);
+}
+
+// The checks and launch behind both backward entry points: dPre row (b, t) at dpre + (b / G) d_e + (b % G) d_g + t d_t
+int backward_rows(const char* fn, const float* dout, const float* saved, const float* c0, const float* w_gates_t,
+                  const float* w_heads, int64_t batch, int32_t steps, int32_t input_size, int32_t hidden_size,
+                  int32_t n_act, int32_t groups, int64_t d_e, int64_t d_g, int64_t d_t, float* dz, float* dpre,
+                  void* stream) {
+    PB_REQUIRE(batch >= 0 && steps >= 1, PB_ERR_INVALID, "%s: need batch >= 0 and steps >= 1", fn);
+    PB_REQUIRE(groups >= 1 && batch % groups == 0, PB_ERR_INVALID, "%s: need groups >= 1 dividing batch (got %d, %lld)",
+               fn, groups, (long long)batch);
+    PB_REQUIRE(input_size == PL_H && hidden_size == PL_H, PB_ERR_UNSUPPORTED,
+               "%s: built for LSTM input and hidden size %d (got %d, %d)", fn, PL_H, input_size, hidden_size);
+    PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "%s: n_act must be in [1, 15]", fn);
+    if (batch == 0) return PB_OK;
+    PB_REQUIRE(dout && saved && w_gates_t && w_heads && dz && dpre, PB_ERR_INVALID, "%s: null pointer", fn);
+    PB_REQUIRE(d_e >= PL_H && d_t >= PL_H && (groups == 1 || d_g >= PL_H) && d_e % 2 == 0 && d_g % 2 == 0 &&
+                   d_t % 2 == 0,
+               PB_ERR_INVALID, "%s: dPre strides must be even and at least %d floats", fn, PL_H);
+    PB_REQUIRE(aligned(w_gates_t, 16), PB_ERR_INVALID, "%s: w_gates_t must be 16-byte aligned", fn);
+    PB_REQUIRE(aligned(dout, 8) && aligned(saved, 8) && aligned(c0, 8) && aligned(w_heads, 8) && aligned(dz, 8) &&
+                   aligned(dpre, 8),
+               PB_ERR_INVALID, "%s: dout / saved / c0 / w_heads / dz / dpre must be 8-byte aligned", fn);
+    BwdParams p{dout, saved, c0, w_gates_t, w_heads, batch, steps, n_act, dz, dpre, groups, d_e, d_g, d_t};
+    cudaStream_t s = (cudaStream_t)stream;
+    return n_act + 1 <= 8 ? launch(k_lstm_bptt_bwd<8>, p, BWD_SMEM, s) : launch(k_lstm_bptt_bwd<16>, p, BWD_SMEM, s);
+}
+
 }  // namespace
 
 extern "C" int pb_lstm_bptt_forward(const float* obs, int64_t obs_stride, int32_t in_features, int64_t batch,
@@ -408,42 +483,36 @@ extern "C" int pb_lstm_bptt_forward(const float* obs, int64_t obs_stride, int32_
                                     const float* w_heads, const float* b_heads, int32_t input_size,
                                     int32_t hidden_size, int32_t n_act, float* out, float* h_out, float* c_out,
                                     float* saved, void* stream) {
-    PB_REQUIRE(batch >= 0 && steps >= 1, PB_ERR_INVALID, "pb_lstm_bptt_forward: need batch >= 0 and steps >= 1");
-    PB_REQUIRE(in_features >= 1 && in_features <= PL_F, PB_ERR_UNSUPPORTED,
-               "pb_lstm_bptt_forward: observation features must be in [1, %d] (got %d)", PL_F, in_features);
-    PB_REQUIRE(input_size == PL_H && hidden_size == PL_H, PB_ERR_UNSUPPORTED,
-               "pb_lstm_bptt_forward: built for LSTM input and hidden size %d (got %d, %d)", PL_H, input_size, hidden_size);
-    PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "pb_lstm_bptt_forward: n_act must be in [1, 15]");
-    if (batch == 0) return PB_OK;
-    PB_REQUIRE(obs && w_enc && b_enc && w_gates && b_gates && w_heads && b_heads && out && h_out && c_out && saved,
-               PB_ERR_INVALID, "pb_lstm_bptt_forward: null pointer");
-    PB_REQUIRE(obs_stride >= in_features, PB_ERR_INVALID, "pb_lstm_bptt_forward: obs_stride < in_features");
-    PB_REQUIRE(aligned(w_enc, 16) && aligned(w_gates, 16), PB_ERR_INVALID,
-               "pb_lstm_bptt_forward: w_enc / w_gates must be 16-byte aligned");
-    PB_REQUIRE(aligned(out, 8) && aligned(h_out, 8) && aligned(c_out, 8) && aligned(saved, 8) && aligned(h0, 8) &&
-                   aligned(c0, 8),
-               PB_ERR_INVALID, "pb_lstm_bptt_forward: out / h / c / saved must be 8-byte aligned");
-    FwdParams p{obs, obs_stride, in_features, batch, steps, h0, c0, w_enc, b_enc, w_gates, b_gates, w_heads, b_heads,
-                out, h_out, c_out, saved};
-    cudaStream_t s = (cudaStream_t)stream;
-    return n_act + 1 <= 8 ? launch(k_lstm_bptt_fwd<8>, p, FWD_SMEM, s) : launch(k_lstm_bptt_fwd<16>, p, FWD_SMEM, s);
+    // the gathered layout: one group, row b*T + t at obs + (b*T + t) * obs_stride
+    return forward_rows("pb_lstm_bptt_forward", obs, in_features, batch, steps, 1, (int64_t)steps * obs_stride, 0,
+                        obs_stride, h0, c0, w_enc, b_enc, w_gates, b_gates, w_heads, b_heads, input_size, hidden_size,
+                        n_act, out, h_out, c_out, saved, stream);
+}
+
+extern "C" int pb_lstm_bptt_forward_rows(const float* obs, int32_t in_features, int64_t batch, int32_t steps,
+                                         int32_t groups, int64_t stride_e, int64_t stride_g, int64_t stride_t,
+                                         const float* h0, const float* c0, const float* w_enc, const float* b_enc,
+                                         const float* w_gates, const float* b_gates, const float* w_heads,
+                                         const float* b_heads, int32_t input_size, int32_t hidden_size, int32_t n_act,
+                                         float* out, float* h_out, float* c_out, float* saved, void* stream) {
+    return forward_rows("pb_lstm_bptt_forward_rows", obs, in_features, batch, steps, groups, stride_e, stride_g,
+                        stride_t, h0, c0, w_enc, b_enc, w_gates, b_gates, w_heads, b_heads, input_size, hidden_size,
+                        n_act, out, h_out, c_out, saved, stream);
 }
 
 extern "C" int pb_lstm_bptt_backward(const float* dout, const float* saved, const float* c0, const float* w_gates_t,
                                      const float* w_heads, int64_t batch, int32_t steps, int32_t input_size,
                                      int32_t hidden_size, int32_t n_act, float* dz, float* dpre, void* stream) {
-    PB_REQUIRE(batch >= 0 && steps >= 1, PB_ERR_INVALID, "pb_lstm_bptt_backward: need batch >= 0 and steps >= 1");
-    PB_REQUIRE(input_size == PL_H && hidden_size == PL_H, PB_ERR_UNSUPPORTED,
-               "pb_lstm_bptt_backward: built for LSTM input and hidden size %d (got %d, %d)", PL_H, input_size,
-               hidden_size);
-    PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "pb_lstm_bptt_backward: n_act must be in [1, 15]");
-    if (batch == 0) return PB_OK;
-    PB_REQUIRE(dout && saved && w_gates_t && w_heads && dz && dpre, PB_ERR_INVALID, "pb_lstm_bptt_backward: null pointer");
-    PB_REQUIRE(aligned(w_gates_t, 16), PB_ERR_INVALID, "pb_lstm_bptt_backward: w_gates_t must be 16-byte aligned");
-    PB_REQUIRE(aligned(dout, 8) && aligned(saved, 8) && aligned(c0, 8) && aligned(w_heads, 8) && aligned(dz, 8) &&
-                   aligned(dpre, 8),
-               PB_ERR_INVALID, "pb_lstm_bptt_backward: dout / saved / c0 / w_heads / dz / dpre must be 8-byte aligned");
-    BwdParams p{dout, saved, c0, w_gates_t, w_heads, batch, steps, n_act, dz, dpre};
-    cudaStream_t s = (cudaStream_t)stream;
-    return n_act + 1 <= 8 ? launch(k_lstm_bptt_bwd<8>, p, BWD_SMEM, s) : launch(k_lstm_bptt_bwd<16>, p, BWD_SMEM, s);
+    // dPre dense [B*T][128] in row order b*T + t
+    return backward_rows("pb_lstm_bptt_backward", dout, saved, c0, w_gates_t, w_heads, batch, steps, input_size,
+                         hidden_size, n_act, 1, (int64_t)steps * PL_H, 0, PL_H, dz, dpre, stream);
+}
+
+extern "C" int pb_lstm_bptt_backward_rows(const float* dout, const float* saved, const float* c0,
+                                          const float* w_gates_t, const float* w_heads, int64_t batch, int32_t steps,
+                                          int32_t input_size, int32_t hidden_size, int32_t n_act, int32_t groups,
+                                          int64_t dpre_stride_e, int64_t dpre_stride_g, int64_t dpre_stride_t,
+                                          float* dz, float* dpre, void* stream) {
+    return backward_rows("pb_lstm_bptt_backward_rows", dout, saved, c0, w_gates_t, w_heads, batch, steps, input_size,
+                         hidden_size, n_act, groups, dpre_stride_e, dpre_stride_g, dpre_stride_t, dz, dpre, stream);
 }

@@ -75,29 +75,28 @@ class _DefaultMLPFunction(torch.autograd.Function):
         db_enc = grads[8 * hid:9 * hid]
         db_cat = grads[9 * hid:]
         # dW_enc = dPre^T @ x is one 128x128 output tile with K = M: as a batched GEMM over 64 K-slices (+ a 64-way sum)
-        # gives the library GEMM enough parallel work at this shape
-        split = 64
-        if x.dim() == 3:            # slab form: the K-slices tile each slab, partial products into one buffer
-            g_, r_, f_ = x.shape
-            sp = max(1, split // g_)
-            while r_ % sp:
-                sp //= 2
-            part = x.new_empty(g_ * sp, hid, f_)
-            for g in range(g_):
-                torch.bmm(dpre[g * r_:(g + 1) * r_].view(sp, r_ // sp, hid).transpose(1, 2),
-                          x[g].view(sp, r_ // sp, f_), out=part[g * sp:(g + 1) * sp])
-            dw_enc = part.sum(0)
-        elif m % split == 0 and m // split >= 256:
-            dw_enc = torch.bmm(dpre.view(split, m // split, hid).transpose(1, 2), x.view(split, m // split, -1)).sum(0)
-        else:
-            dw_enc = dpre.t() @ x
+        # gives the library GEMM enough parallel work at this shape (slab form: K-slices per slab)
+        dw_enc = _gemm_tn(dpre, x)
         return (None, dw_enc, db_enc, dw_cat[:n_act], db_cat[:n_act], dw_cat[n_act:n_act + 1],
                 db_cat[n_act:n_act + 1], None)
 
 
 def _gemm_tn(a, b, split=64):
     """a^T @ b for a [M, Na], b [M, Nb] with unit column stride (row slices of wider rows are fine): a small output with
-    K = M, so for large M a batched GEMM over `split` K-slices plus a sum gives the library GEMM enough parallel work."""
+    K = M, so for large M a batched GEMM over `split` K-slices plus a sum gives the library GEMM enough parallel work.
+    b may also be G equally strided row slabs [G, R, Nb] (a strided view of the rollout buffer) with a = [G*R, Na] in
+    slab-major order: then the K-slices tile each slab (split / G per slab, halved until they divide R), every slab's
+    batched GEMM writes its partial products into one buffer and one sum reduces them; nothing is gathered."""
+    if b.dim() == 3:
+        g_, r_, nb = b.shape
+        sp = max(1, split // g_)
+        while r_ % sp:
+            sp //= 2
+        part = b.new_empty(g_ * sp, a.shape[1], nb)
+        for g in range(g_):
+            torch.bmm(a[g * r_:(g + 1) * r_].view(sp, r_ // sp, a.shape[1]).transpose(1, 2), b[g].view(sp, r_ // sp, nb),
+                      out=part[g * sp:(g + 1) * sp])
+        return part.sum(0)
     m = a.shape[0]
     if m % split == 0 and m // split >= 256:
         return torch.bmm(a.view(split, m // split, -1).transpose(1, 2), b.view(split, m // split, -1)).sum(0)
@@ -112,21 +111,32 @@ class _LSTMBPTTFunction(torch.autograd.Function):
               keeps the saved-activation rows [B*T, 1024] for the backward.
     backward: pb_lstm_bptt_backward -- dz (the gate pre-activations) and dPre (the encoder pre-activation) in reverse
               time; the weight gradients are library GEMMs on those buffers (_gemm_tn).  The observations and the initial
-              state get no gradient; neither does the final state (train() hands it on detached)."""
+              state get no gradient; neither does the final state (train() hands it on detached).
+    x is either the gathered minibatch [B, T, F] or the segment view [E, G, T, F] of Experience.segment_obs (segment
+    b = e*G + g, read in place from the rollout buffer; pb_lstm_bptt_forward_rows / _backward_rows).  The segment view
+    writes dPre in the order of its G observation slabs [G, T*E] so that dW_enc is the slab form of _gemm_tn; every
+    other buffer, and the state, keep row order b*T + t."""
 
     @staticmethod
     def forward(ctx, x, h0, c0, ops, w_enc, b_enc, w_ih, w_hh, b_ih, b_hh, w_dec, b_dec, w_val, b_val):
         from pufferlib_b200 import _native
         w_enc_p, b_enc_p, w_gates, b_gates, w_cat, b_cat, w_gates_t = ops
-        (bsz, steps, feats), n_act = x.shape, w_dec.shape[0]
+        n_act, seg = w_dec.shape[0], x.dim() == 4
+        bsz, steps, feats = (x.shape[0] * x.shape[1],) + tuple(x.shape[2:]) if seg else x.shape
         m = bsz * steps
         out = x.new_empty(m, w_cat.shape[0])
         h_out, c_out = x.new_empty(bsz, 128), x.new_empty(bsz, 128)
         saved = x.new_empty(m, 1024)
-        P = _native.ptr
-        _native.check(_native.lib().pb_lstm_bptt_forward(
-            P(x), x.stride(1), feats, bsz, steps, P(h0), P(c0), P(w_enc_p), P(b_enc_p), P(w_gates), P(b_gates), P(w_cat),
-            P(b_cat), 128, 128, n_act, P(out), P(h_out), P(c_out), P(saved), _native.stream_ptr()))
+        P, lib = _native.ptr, _native.lib()
+        if seg:
+            _native.check(lib.pb_lstm_bptt_forward_rows(
+                P(x), feats, bsz, steps, x.shape[1], x.stride(0), x.stride(1), x.stride(2), P(h0), P(c0), P(w_enc_p),
+                P(b_enc_p), P(w_gates), P(b_gates), P(w_cat), P(b_cat), 128, 128, n_act, P(out), P(h_out), P(c_out),
+                P(saved), _native.stream_ptr()))
+        else:
+            _native.check(lib.pb_lstm_bptt_forward(
+                P(x), x.stride(1), feats, bsz, steps, P(h0), P(c0), P(w_enc_p), P(b_enc_p), P(w_gates), P(b_gates),
+                P(w_cat), P(b_cat), 128, 128, n_act, P(out), P(h_out), P(c_out), P(saved), _native.stream_ptr()))
         ctx.save_for_backward(x, c0, saved, w_gates_t, w_cat)
         ctx.n_act = n_act
         ctx.mark_non_differentiable(h_out, c_out)
@@ -136,18 +146,27 @@ class _LSTMBPTTFunction(torch.autograd.Function):
     def backward(ctx, dout, _dh, _dc):
         from pufferlib_b200 import _native
         x, c0, saved, w_gates_t, w_cat = ctx.saved_tensors
-        (bsz, steps, feats), n_act = x.shape, ctx.n_act
+        n_act, seg = ctx.n_act, x.dim() == 4
+        bsz, steps, feats = (x.shape[0] * x.shape[1],) + tuple(x.shape[2:]) if seg else x.shape
         m = bsz * steps
         dout = dout.contiguous()
         dz = x.new_empty(m, 512)
         dpre = x.new_empty(m, 128)
-        P = _native.ptr
-        _native.check(_native.lib().pb_lstm_bptt_backward(
-            P(dout), P(saved), P(c0), P(w_gates_t), P(w_cat), bsz, steps, 128, 128, n_act, P(dz), P(dpre),
-            _native.stream_ptr()))
+        P, lib = _native.ptr, _native.lib()
+        if seg:       # dPre row (e, g, t) -> (g*T + t)*E + e: slab g holds the rows of observation slab g, (t, e) order
+            e_, g_ = x.shape[:2]
+            _native.check(lib.pb_lstm_bptt_backward_rows(
+                P(dout), P(saved), P(c0), P(w_gates_t), P(w_cat), bsz, steps, 128, 128, n_act, g_, 128, 128 * steps * e_,
+                128 * e_, P(dz), P(dpre), _native.stream_ptr()))
+            x_rows = x.permute(1, 2, 0, 3).view(g_, steps * e_, feats)     # [G, T*E, F] slabs, a view (forward_packed_seq)
+        else:
+            _native.check(lib.pb_lstm_bptt_backward(
+                P(dout), P(saved), P(c0), P(w_gates_t), P(w_cat), bsz, steps, 128, 128, n_act, P(dz), P(dpre),
+                _native.stream_ptr()))
+            x_rows = x.reshape(m, feats)
         dw_gates = _gemm_tn(dz, saved[:, :256])            # dz^T [e | h_prev] = [dW_ih | dW_hh]
         db_gates = dz.sum(0)
-        dw_enc = _gemm_tn(dpre, x.reshape(m, feats))
+        dw_enc = _gemm_tn(dpre, x_rows)
         dw_cat = _gemm_tn(dout, saved[:, 896:])             # dOut^T h
         db_cat = dout.sum(0)
         # b_ih and b_hh get the same gradient, as separate tensors (their .grad must not alias)
@@ -353,19 +372,33 @@ class LSTMWrapper(nn.Module):
 
     def forward_packed_seq(self, x, state=None):
         """The training forward over bptt segments on the fused kernels (pb_lstm_bptt_forward / _backward):
-        x [B, T, *obs], state (h, c) of shape [1, B, 128] (detached) or None (zeros).  -> (out [B*T, R], n_act,
-        (h_T, c_T) [1, B, 128]) with logits = out[:, :n_act], value = out[:, n_act], rows b*T + t; or None when the fast
-        path does not apply (fused_supported fails, the inner Default's fast_path is off, or the layout is not one the
-        kernel reads).  The packed operands are rebuilt on every call that records gradients."""
+        x [B, T, *obs], or the strided segment view [E, G, T, *obs] of Experience.segment_obs with segment b = e*G + g
+        (B = E*G; read in place, pb_lstm_bptt_forward_rows / _backward_rows); state (h, c) of shape [1, B, 128] (detached)
+        or None (zeros).  -> (out [B*T, R], n_act, (h_T, c_T) [1, B, 128]) with logits = out[:, :n_act],
+        value = out[:, n_act], rows b*T + t in both cases; or None when the fast path does not apply (fused_supported
+        fails, the inner Default's fast_path is off, or the layout is not one the kernel reads).  The packed operands are
+        rebuilt on every call that records gradients."""
         nd = len(self.obs_shape)
-        if x.dim() != nd + 2 or tuple(x.shape[2:]) != self.obs_shape or x.shape[0] == 0:
+        if x.dim() not in (nd + 2, nd + 3) or tuple(x.shape[x.dim() - nd:]) != self.obs_shape:
             return None
         if not (self.fused_supported(x) and getattr(self.policy, 'fast_path', False)):
             return None
-        bsz, steps = x.shape[:2]
-        x3 = x.reshape(bsz, steps, -1)
-        if x3.stride(2) != 1 or x3.stride(0) != steps * x3.stride(1):
-            return None                     # rows (b, t) must be equally spaced
+        lead = x.shape[:x.dim() - nd]
+        bsz, steps = int(np.prod(lead[:-1])), lead[-1]
+        if bsz == 0:
+            return None
+        if len(lead) == 3:
+            try:           # rows of equal stride in each of E, G, T; the [G, T*E] observation slabs of dW_enc are a view
+                x3 = x.view(*lead, -1)
+                x3.permute(1, 2, 0, 3).view(lead[1], steps * lead[0], -1)
+            except RuntimeError:
+                return None
+            if x3.stride(3) != 1:
+                return None
+        else:
+            x3 = x.reshape(bsz, steps, -1)
+            if x3.stride(2) != 1 or x3.stride(0) != steps * x3.stride(1):
+                return None                     # rows (b, t) must be equally spaced
         h0 = c0 = None
         if state is not None:
             h0, c0 = state

@@ -26,7 +26,7 @@ import numpy as np
 import torch
 
 import pufferlib_b200
-from pufferlib_b200 import _native
+from pufferlib_b200 import _native, models
 from pufferlib_b200.exceptions import APIUsageError
 
 torch.set_float32_matmul_precision('high')   # clean_pufferl.py:22
@@ -150,18 +150,19 @@ class _FusedPPOLoss(torch.autograd.Function):
                 None)
 
 
+def _loss_cfg(config):
+    return (float(config.clip_coef), bool(config.clip_vloss), float(config.vf_clip_coef), float(config.vf_coef),
+            float(config.ent_coef))
+
+
 def fused_ppo_loss(logits, value, actions, old_logprobs, adv, returns, old_values, config):
     """-> (loss, stats) with stats = [pg_loss, v_loss, entropy, old_approx_kl, approx_kl, clipfrac] (detached)."""
-    cfg = (float(config.clip_coef), bool(config.clip_vloss), float(config.vf_clip_coef), float(config.vf_coef),
-           float(config.ent_coef))
-    return _FusedPPOLoss.apply(logits, value, actions, old_logprobs, adv, returns, old_values, cfg, 0)
+    return _FusedPPOLoss.apply(logits, value, actions, old_logprobs, adv, returns, old_values, _loss_cfg(config), 0)
 
 
 def fused_ppo_loss_packed(out, n_act, actions, old_logprobs, adv, returns, old_values, config):
     """Same, on the packed head output [M, 8] of models.Default.forward_packed (one [M, 8] gradient back)."""
-    cfg = (float(config.clip_coef), bool(config.clip_vloss), float(config.vf_clip_coef), float(config.vf_coef),
-           float(config.ent_coef))
-    return _FusedPPOLoss.apply(out, None, actions, old_logprobs, adv, returns, old_values, cfg, int(n_act))
+    return _FusedPPOLoss.apply(out, None, actions, old_logprobs, adv, returns, old_values, _loss_cfg(config), int(n_act))
 
 
 def slab_layout(num_envs, horizon, num_minibatches, bptt_horizon):
@@ -203,6 +204,8 @@ class _DefaultMLPUpdate:
         encoder GEMM (+bias+ReLU epilogue, one per slab) -> 8-column head GEMM -> pb_ppo_loss (loss statistics +
         analytic dLoss/dOut) -> pb_mlp_tail_backward (dPre, dW_heads, db_heads, db_enc) -> split-K dW_enc GEMM + sum
         [-> gradient all-reduce over ONE flat buffer when world_size > 1] -> pb_clip_adam -> pb_pack_heads.
+    train() passes each minibatch as Experience.minibatch() to forward_backward; where _fused_ok holds (minibatch_form
+    asks it too) the chain is ONE kernel, pb_mlp_update_fused.
     Same math as the autograd path (tests/test_gpu_experience.py::test_manual_update_matches_autograd_update); the
     optimizer's own state tensors are updated in place, so state_dict() and optimizer.step() keep working."""
 
@@ -297,17 +300,23 @@ class _DefaultMLPUpdate:
         (optimizer.load_state_dict() replaces them): the caller rebuilds the update object."""
         return self._current_state_ptrs() != self._state_ptrs
 
-    def _buffers(self, m, n_stats):
+    def _buffers(self, m):
         if self.rows != m:
             z = dict(dtype=torch.float32, device=self.gflat.device)
             self.hidden, self.dpre = torch.empty(m, self.hid, **z), torch.empty(m, self.hid, **z)
             self.out, self.dout = torch.empty(m, 8, **z), torch.empty(m, 8, **z)
             self.ws = torch.empty(_native.lib().pb_mlp_tail_workspace_bytes(m, self.hid), dtype=torch.uint8,
                                   device=self.gflat.device)
-            self.part = None
             self.rows = m
-        if self.stats is None or self.stats.shape[0] != n_stats:
-            self.stats = torch.zeros(n_stats, 8, dtype=torch.float64, device=self.gflat.device)
+
+    def _dw_enc(self, dpre, x):
+        """dW_enc = dPre^T x into self.dw_enc (a view of gflat): the split-K slab GEMM of models._gemm_tn, its partial
+        products in the cached self.part."""
+        g_, r_, f_ = x.shape
+        shape = (g_ * models._slab_split(g_, r_), self.hid, f_)
+        if self.part is None or self.part.shape != shape:
+            self.part = torch.empty(shape, dtype=torch.float32, device=x.device)
+        models._gemm_tn(dpre, x, out=self.dw_enc, part=self.part)
 
     def pack_heads(self):
         m = self.model
@@ -324,21 +333,21 @@ class _DefaultMLPUpdate:
                 and (x.shape[0] == 1 or (x.stride(0) % x.stride(1) == 0 and x.stride(0) >= x.shape[1] * x.stride(1))))
 
     @torch.no_grad()
-    def forward_backward(self, k, n_stats, obs, slab_form, atn, log_probs, adv, ret, val, config, row_slab_stride=None,
-                         adv_norm=None):
-        """obs: slab view [G, R, *obs] (slab_form) or [M, *obs]; the rest [M] in slab-major order -- or, with
-        row_slab_stride (fused kernel only), arrival-order tensors whose slab s starts at element s * row_slab_stride;
-        adv_norm: device (mean, 1/(std+1e-8)) applied to `adv` inside the kernel; ret None: adv + val.  Statistics of this
-        minibatch go to row k of self.stats."""
-        x = obs if slab_form else obs.reshape(1, atn.numel(), -1)
-        x = x.flatten(2)
-        assert row_slab_stride is None or self._fused_ok(x, config)
-        if self._fused_ok(x, config):
+    def forward_backward(self, k, n_stats, mb, config):
+        """mb (Experience.minibatch): obs a slab view [G, R, *obs] (mb.slab_form) or [M, *obs]; actions, logprobs,
+        values, advantages [M] in slab-major order -- or, with row_slab_stride (fused kernel only), arrival-order tensors whose
+        slab s starts at element s * row_slab_stride; adv_norm: device (mean, 1/(std+1e-8)) applied to the advantages
+        inside the kernel; returns None: advantages + values.  Statistics of this minibatch go to row k of self.stats."""
+        x = (mb.obs if mb.slab_form else mb.obs.reshape(1, mb.actions.numel(), -1)).flatten(2)
+        if self.stats is None or self.stats.shape[0] != n_stats:
+            self.stats = torch.zeros(n_stats, 8, dtype=torch.float64, device=self.gflat.device)
+        atn, log_probs, adv, ret, val = mb.actions, mb.logprobs, mb.advantages, mb.returns, mb.values
+        fused = self._fused_ok(x, config)
+        assert mb.row_slab_stride is None or fused
+        if fused:
             # ONE wgmma kernel: x read once, hidden / dPre stay on the SM, gradients land in self.gflat
             g_, r_, _ = x.shape
             lib = _native.lib()
-            if self.stats is None or self.stats.shape[0] != n_stats:
-                self.stats = torch.zeros(n_stats, 8, dtype=torch.float64, device=self.gflat.device)
             if self.fused_ws is None:
                 self.fused_ws = torch.empty(lib.pb_mlp_update_workspace_bytes(), dtype=torch.uint8, device=self.gflat.device)
             self.mb_rows = g_ * r_
@@ -353,29 +362,21 @@ class _DefaultMLPUpdate:
                 _native.ptr(m_.encoder.weight), _native.ptr(m_.encoder.bias), _native.ptr(self.w_cat), _native.ptr(self.b_cat),
                 _native.ptr(atn.reshape(-1)), _native.ptr(log_probs.reshape(-1)), _native.ptr(adv.reshape(-1)),
                 _native.ptr(ret.reshape(-1)) if ret is not None else None, _native.ptr(val.reshape(-1)),
-                _native.ptr(adv_norm) if adv_norm is not None else None, r_ if row_slab_stride is None else int(row_slab_stride),
+                _native.ptr(mb.adv_norm) if mb.adv_norm is not None else None,
+                r_ if mb.row_slab_stride is None else int(mb.row_slab_stride),
                 self.n_act, C.c_float(config.clip_coef),
                 int(bool(config.clip_vloss)), C.c_float(config.vf_clip_coef), C.c_float(config.vf_coef),
                 C.c_float(config.ent_coef), _native.ptr(self.gflat), C.c_void_p(self.stats.data_ptr() + 64 * k),
                 _native.ptr(self.fused_ws), self.fused_ws.numel(), None if in_kernel else _native.ptr(self.fused_dpre),
                 None, None, None, _native.stream_ptr()))
-            if not in_kernel:       # split-K batched GEMM per slab + one sum, as in the kernel chain below
-                f_ = x.shape[2]
-                sp = max(1, 64 // g_)
-                while r_ % sp:
-                    sp //= 2
-                if self.part is None or self.part.shape != (g_ * sp, self.hid, f_):
-                    self.part = torch.empty(g_ * sp, self.hid, f_, dtype=torch.float32, device=x.device)
-                for g in range(g_):
-                    torch.bmm(self.fused_dpre[g * r_:(g + 1) * r_].view(sp, r_ // sp, self.hid).transpose(1, 2),
-                              x[g].view(sp, r_ // sp, f_), out=self.part[g * sp:(g + 1) * sp])
-                torch.sum(self.part, 0, out=self.dw_enc)
+            if not in_kernel:
+                self._dw_enc(self.fused_dpre, x)
             self.used_fused = True
             return
         x = x.float()
         g_, r_, f_ = x.shape
         m, hid = g_ * r_, self.hid
-        self._buffers(m, n_stats)
+        self._buffers(m)
         self.mb_rows = m
         model, lib, s = self.model, _native.lib(), _native.stream_ptr()
         w_enc, b_enc = model.encoder.weight, model.encoder.bias
@@ -393,15 +394,7 @@ class _DefaultMLPUpdate:
         _native.check(lib.pb_mlp_tail_backward(_native.ptr(self.dout), 8, _native.ptr(self.w_cat),
                                                _native.ptr(self.hidden), m, hid, _native.ptr(self.dpre),
                                                _native.ptr(self.tail), _native.ptr(self.ws), self.ws.numel(), s))
-        sp = max(1, 64 // g_)
-        while r_ % sp:
-            sp //= 2
-        if self.part is None or self.part.shape != (g_ * sp, hid, f_):
-            self.part = torch.empty(g_ * sp, hid, f_, dtype=torch.float32, device=x.device)
-        for g in range(g_):
-            torch.bmm(self.dpre[g * r_:(g + 1) * r_].view(sp, r_ // sp, hid).transpose(1, 2),
-                      x[g].view(sp, r_ // sp, f_), out=self.part[g * sp:(g + 1) * sp])
-        torch.sum(self.part, 0, out=self.dw_enc)
+        self._dw_enc(self.dpre, x)
 
     def all_reduce(self):
         if self.world > 1 and self.peer is None:
@@ -518,6 +511,7 @@ class Experience:
         self._gae_ws = None
         self.advantages_tm = None     # arrival-order advantages (pb_gae_tm) for the in-place (direct slab) update
         self.adv_norm = None          # [nm, 2]: (mean, 1 / (std + 1e-8)) per minibatch
+        self.form, self.norm_adv = None, False      # what prepare() laid out for minibatch()
 
     @property
     def b_obs(self):
@@ -636,16 +630,45 @@ class Experience:
                                  self._gae_ws.numel(), _native.stream_ptr()))
         return self.advantages
 
-    def direct_slabs_ok(self, manual, config):
-        """Can the update read the rollout tensors in place (zero-copy observations AND zero-copy per-row tensors)?  Needs
-        the slab layout, the GAE tile kernel's time-major output and the fused update kernel for these observations."""
-        n, h, nm, bptt = self.num_envs, self.horizon, self.num_minibatches, self.bptt_horizon
-        layout = slab_layout(n, h, nm, bptt)
-        if layout is None or not _native.lib().pb_gae_time_major_supported(n, h):
-            return False
-        g_, r_ = layout
-        x0 = self.obs.view(g_, nm, r_, *self.obs_shape)[:, 0].flatten(2)
-        return manual._fused_ok(x0, config)
+    def prepare(self, form, config):
+        """After sort_training_data: GAE, the layout of minibatch form `form` (minibatch_form) and the advantage
+        normalisation of clean_pufferl.py:211-213, for every minibatch at once; minibatch() then reads them."""
+        self.form, self.norm_adv = form, bool(config.norm_adv)
+        if form == 'direct':
+            self.compute_gae(config.gamma, config.gae_lambda, time_major=True)
+            self.prepare_direct_slabs(config.norm_adv)
+            return
+        self.compute_gae(config.gamma, config.gae_lambda)
+        if form == 'slabs':
+            self.flatten_batch_slabs()
+        else:
+            self.flatten_batch(gather_obs=form == 'gathered')
+        if config.norm_adv:
+            self.normalize_advantages(slabs=form == 'slabs')
+
+    def minibatch(self, mb):
+        """Minibatch mb of the form prepare() laid out, as one namespace for every form: obs, slab_form (obs is a slab
+        view [G, R, *obs]), actions, logprobs, values, advantages, returns (None: the kernel forms them), adv_norm and
+        row_slab_stride (direct form: the per-row tensors are the rollout tensors, slab s = rows (s*nm + mb)*R .. +R)."""
+        if self.form == 'direct':
+            r_ = self._slabs.shape[1]
+            lo = mb * r_
+            return pufferlib_b200.namespace(
+                obs=self.slab_obs(mb), slab_form=True, actions=self.actions[lo:], logprobs=self.logprobs[lo:],
+                values=self.values[lo:], advantages=self.advantages_tm[lo:], returns=None,
+                row_slab_stride=self.num_minibatches * r_, adv_norm=self.adv_norm[mb] if self.norm_adv else None)
+        if self.form == 'slabs':
+            sl = self._slabs
+            obs = self.slab_obs(mb)
+            rows = (sl.actions, sl.logprobs, sl.values, sl.advantages_normalized if self.norm_adv else sl.advantages,
+                    sl.returns)
+        else:
+            obs = self.segment_obs(mb) if self.form == 'segments' else self.b_obs[mb]
+            rows = (self.b_actions, self.b_logprobs, self.b_values,
+                    self.b_advantages_normalized if self.norm_adv else self.b_advantages, self.b_returns)
+        atn, log_probs, val, adv, ret = (t[mb] for t in rows)
+        return pufferlib_b200.namespace(obs=obs, slab_form=self.form == 'slabs', actions=atn, logprobs=log_probs,
+                                        values=val, advantages=adv, returns=ret, row_slab_stride=None, adv_norm=None)
 
     def prepare_direct_slabs(self, norm_adv):
         """After compute_gae(time_major=True): the returns of clean_pufferl.py:476 (for the explained variance) and the
@@ -662,15 +685,6 @@ class Experience:
             _native.check(_native.lib().pb_adv_stats_slabs(
                 _native.ptr(self.advantages_tm), r_, g_, nm, _native.ptr(self.adv_norm), _native.ptr(self._advnorm_ws),
                 self._advnorm_ws.numel(), _native.stream_ptr()))
-
-    def direct_minibatch(self, mb, norm_adv):
-        """Minibatch mb as views of the rollout tensors: slab s of the minibatch = rows (s*nm + mb)*R .. +R."""
-        g_, r_ = self._slabs.shape
-        lo = mb * r_
-        return pufferlib_b200.namespace(
-            obs=self.slab_obs(mb), actions=self.actions[lo:], logprobs=self.logprobs[lo:], old_values=self.values[lo:],
-            advantages=self.advantages_tm[lo:], row_slab_stride=self.num_minibatches * r_,
-            adv_norm=self.adv_norm[mb] if norm_adv else None)
 
     def flatten_batch(self, advantages=None, gather_obs=True):
         """clean_pufferl.py:466-482 (advantages: sorted-order device tensor, default self.advantages).  gather_obs=False
@@ -721,8 +735,8 @@ class Experience:
         return True
 
     def slab_obs(self, mb):
-        """Observations of minibatch mb as a zero-copy view [G, bptt*N, *obs] of the rollout buffer."""
-        g_, r_ = self._slabs.shape
+        """Observations of minibatch mb as a zero-copy view [G, bptt*N, *obs] of the rollout buffer (slab_layout)."""
+        g_, r_ = slab_layout(self.num_envs, self.horizon, self.num_minibatches, self.bptt_horizon)
         return self.obs.view(g_, self.num_minibatches, r_, *self.obs_shape)[:, mb]
 
     def segment_obs(self, mb):
@@ -936,6 +950,25 @@ def _recurrent_update_fused(data):
             and model.fused_supported(experience.obs) and bool(getattr(model.policy, 'fast_path', False)))
 
 
+def minibatch_form(data, manual):
+    """The minibatch form of this train(), from the shapes, the config and what the update engine accepts (manual: the
+    _DefaultMLPUpdate, or None): 'direct' (manual's fused kernel reads the arrival-order rollout tensors in place),
+    'slabs' (order-free fused loss: per-row tensors copied slab-major, obs a view), 'segments' (the fused recurrent
+    update on bptt segment views of obs) or 'gathered' (the reference layout: b_obs and the b_* tensors)."""
+    config, exp = data.config, data.experience
+    n, h, nm = exp.num_envs, exp.horizon, exp.num_minibatches
+    if not bool(getattr(config, 'zero_copy_minibatches', True)) or slab_layout(n, h, nm, exp.bptt_horizon) is None:
+        return 'gathered'
+    if exp.lstm_h is not None:
+        return 'segments' if _recurrent_update_fused(data) else 'gathered'
+    if not (data.fused_loss and hasattr(getattr(data.policy, 'policy', None), 'forward_packed_slabs')):
+        return 'gathered'
+    if manual is not None and _native.lib().pb_gae_time_major_supported(n, h) and \
+            manual._fused_ok(exp.slab_obs(0).flatten(2), config):
+        return 'direct'
+    return 'slabs'
+
+
 def _invalidate_policy_cache(data):
     model = getattr(data.policy, 'policy', None)
     if hasattr(model, 'invalidate_cache'):
@@ -1045,10 +1078,6 @@ def _train_device_part(data, seg=None):
     device = experience.device
     _invalidate_policy_cache(data)     # nothing cached by the rollout (eager or captured) may leak into an update graph
 
-    # zero-copy minibatches (Experience.flatten_batch_slabs): order-free loss only, i.e. the fused non-LSTM path
-    model = getattr(data.policy, 'policy', None)
-    want_slabs = data.fused_loss and experience.lstm_h is None and hasattr(model, 'forward_packed_slabs') and \
-        bool(getattr(config, 'zero_copy_minibatches', True))
     # recurrent models: the fused BPTT update when the policy asks for it and the model is covered (RecurrentPolicy(
     # fused_update=True); data.train_recurrent_path records which path ran)
     rec_fused = _recurrent_update_fused(data)
@@ -1059,26 +1088,8 @@ def _train_device_part(data, seg=None):
         manual = data.manual_update
     with profile.train_misc:
         experience.sort_training_data()
-        # the fused recurrent update reads its minibatch segments in place (Experience.segment_obs): no b_obs copy
-        segments = rec_fused and bool(getattr(config, 'zero_copy_minibatches', True)) and slab_layout(
-            experience.num_envs, experience.horizon, experience.num_minibatches, experience.bptt_horizon) is not None
-        # the fused update kernel reads the ARRIVAL-order rollout tensors through slab strides: no minibatch copies at all
-        # (GAE writes the advantages in arrival order as well; the advantage normalisation constants are applied on the fly)
-        direct = want_slabs and manual is not None and experience.direct_slabs_ok(manual, config)
-        if direct:
-            experience.compute_gae(config.gamma, config.gae_lambda, time_major=True)
-            experience.prepare_direct_slabs(config.norm_adv)
-            slabs = True
-        else:
-            experience.compute_gae(config.gamma, config.gae_lambda)
-            slabs = want_slabs and experience.flatten_batch_slabs()
-            if not slabs:
-                experience.flatten_batch(gather_obs=not segments)
-            if config.norm_adv:
-                experience.normalize_advantages(slabs=slabs)
-    # which minibatch form the update reads: rollout tensors in place, slab copies of the per-row tensors, segment views of
-    # the observations (recurrent), or gathered copies
-    data.train_minibatch_path = 'direct' if direct else ('slabs' if slabs else ('segments' if segments else 'gathered'))
+        data.train_minibatch_path = minibatch_form(data, manual)
+        experience.prepare(data.train_minibatch_path, config)
 
     n_mb = experience.num_minibatches
     if seg is not None:                        # persistent accumulator: the segment graphs update it in place
@@ -1096,35 +1107,18 @@ def _train_device_part(data, seg=None):
     n_stats = config.update_epochs * n_mb
 
     def forward_backward(mb, k=0):              # k = epoch * n_mb + mb: the manual path's statistics row
-        if direct:
-            with profile.train_forward:
-                d = experience.direct_minibatch(mb, config.norm_adv)
-                manual.forward_backward(k, n_stats, d.obs, True, d.actions, d.logprobs, d.advantages, None, d.old_values, config,
-                                        row_slab_stride=d.row_slab_stride, adv_norm=d.adv_norm)
-            return
-        if slabs:
-            sl = experience._slabs
-            obs = experience.slab_obs(mb)
-            atn, log_probs, val, ret = sl.actions[mb], sl.logprobs[mb], sl.values[mb], sl.returns[mb]
-            adv = sl.advantages_normalized[mb] if config.norm_adv else sl.advantages[mb]
-        else:
-            obs = experience.segment_obs(mb) if segments else experience.b_obs[mb]
-            atn = experience.b_actions[mb]
-            log_probs = experience.b_logprobs[mb]
-            val = experience.b_values[mb]
-            adv = experience.b_advantages_normalized[mb] if config.norm_adv else experience.b_advantages[mb]
-            ret = experience.b_returns[mb]
-
+        b = experience.minibatch(mb)
         if manual is not None:
             with profile.train_forward:
-                manual.forward_backward(k, n_stats, obs, bool(slabs), atn, log_probs, adv, ret, val, config)
+                manual.forward_backward(k, n_stats, b, config)
             return
+        obs, atn, log_probs, val, adv, ret = b.obs, b.actions, b.logprobs, b.values, b.advantages, b.returns
 
         with profile.train_forward:
             packed = None
             if fused:          # logits / value straight from the model; loss + its gradient in one kernel
                 model = data.policy.policy
-                if slabs:
+                if b.slab_form:
                     packed = model.forward_packed_slabs(obs)
                 elif hasattr(model, 'forward_packed'):
                     packed = model.forward_packed(obs.reshape(-1, *obs_shape))

@@ -21,7 +21,7 @@ class _DefaultMLPFunction(torch.autograd.Function):
     """
 
     @staticmethod
-    def forward(ctx, x, w_enc, b_enc, w_dec, b_dec, w_val, b_val, cache):
+    def forward(ctx, x, w_enc, b_enc, w_dec, b_dec, w_val, b_val, model):
         n_act, hid = w_dec.shape
         if x.dim() == 3:
             # slab form [G, R, F]: G equally spaced row slabs of the rollout buffer (a strided VIEW, see
@@ -36,23 +36,9 @@ class _DefaultMLPFunction(torch.autograd.Function):
                 hidden = torch._addmm_activation(b_enc, x, w_enc.t(), use_gelu=False)
             except (AttributeError, RuntimeError):
                 hidden = torch.relu(torch.addmm(b_enc, x, w_enc.t()))
-        # the 8-row head matrix: rebuilt on every forward that records gradients (the parameters change every optimizer
-        # step, and fused optimizers do NOT bump tensor._version, so it cannot be cached across steps); under no_grad
-        # (the rollout: 128 forwards with frozen parameters) it is built once and reused until invalidate_cache()
+        # the head matrix of Default.head_matrix, cached only when no parameter records gradients
         # (torch.is_grad_enabled() is always False inside Function.forward: decide from the inputs that need gradients)
-        use_cache = not any(ctx.needs_input_grad[1:7])
-        key = (w_dec.data_ptr(), torch.cuda.is_current_stream_capturing())
-        if use_cache and cache.get('key') == key:
-            w_cat, b_cat = cache['w'], cache['b']
-        else:
-            w_cat = x.new_zeros(8, hid)
-            w_cat[:n_act] = w_dec
-            w_cat[n_act] = w_val[0]
-            b_cat = x.new_zeros(8)
-            b_cat[:n_act] = b_dec
-            b_cat[n_act] = b_val[0]
-            if use_cache:
-                cache['key'], cache['w'], cache['b'] = key, w_cat, b_cat
+        w_cat, b_cat = model.head_matrix(cache=not any(ctx.needs_input_grad[1:7]))
         out = torch.addmm(b_cat, hidden, w_cat.t())
         ctx.save_for_backward(x, hidden, w_cat)
         ctx.n_act = n_act
@@ -81,22 +67,29 @@ class _DefaultMLPFunction(torch.autograd.Function):
                 db_cat[n_act:n_act + 1], None)
 
 
-def _gemm_tn(a, b, split=64):
+def _slab_split(g_, r_, split=64):
+    """K-slices per slab in the slab form of _gemm_tn: split / G, halved until they divide R."""
+    sp = max(1, split // g_)
+    while r_ % sp:
+        sp //= 2
+    return sp
+
+
+def _gemm_tn(a, b, split=64, out=None, part=None):
     """a^T @ b for a [M, Na], b [M, Nb] with unit column stride (row slices of wider rows are fine): a small output with
     K = M, so for large M a batched GEMM over `split` K-slices plus a sum gives the library GEMM enough parallel work.
     b may also be G equally strided row slabs [G, R, Nb] (a strided view of the rollout buffer) with a = [G*R, Na] in
-    slab-major order: then the K-slices tile each slab (split / G per slab, halved until they divide R), every slab's
-    batched GEMM writes its partial products into one buffer and one sum reduces them; nothing is gathered."""
+    slab-major order: then the K-slices tile each slab (_slab_split), every slab's batched GEMM writes its partial
+    products into one buffer (or `part`, [G * _slab_split(G, R, split), Na, Nb]) and one sum reduces them into `out`."""
     if b.dim() == 3:
         g_, r_, nb = b.shape
-        sp = max(1, split // g_)
-        while r_ % sp:
-            sp //= 2
-        part = b.new_empty(g_ * sp, a.shape[1], nb)
+        sp = _slab_split(g_, r_, split)
+        if part is None:
+            part = b.new_empty(g_ * sp, a.shape[1], nb)
         for g in range(g_):
             torch.bmm(a[g * r_:(g + 1) * r_].view(sp, r_ // sp, a.shape[1]).transpose(1, 2), b[g].view(sp, r_ // sp, nb),
                       out=part[g * sp:(g + 1) * sp])
-        return part.sum(0)
+        return torch.sum(part, 0, out=out)
     m = a.shape[0]
     if m % split == 0 and m // split >= 256:
         return torch.bmm(a.view(split, m // split, -1).transpose(1, 2), b.view(split, m // split, -1)).sum(0)
@@ -200,13 +193,15 @@ class Default(nn.Module):
         train)."""
         self._head_cache.clear()
 
-    def head_matrix(self):
+    def head_matrix(self, cache=None):
         """(w_cat [R, H], b_cat [R]): n_act logit rows | value row | zero padding up to R = the next multiple of 8 rows
-        (8 for n_act <= 7); cached under no_grad."""
-        cache = self._head_cache
+        (8 for n_act <= 7).  Cached until invalidate_cache() when `cache` is true (default: under no_grad); built anew
+        otherwise, since fused optimizers do not bump tensor._version and the cache cannot see an optimizer step."""
+        if cache is None:
+            cache = not torch.is_grad_enabled()
         key = (self.decoder.weight.data_ptr(), torch.cuda.is_current_stream_capturing())
-        if not torch.is_grad_enabled() and cache.get('key') == key:
-            return cache['w'], cache['b']
+        if cache and self._head_cache.get('key') == key:
+            return self._head_cache['w'], self._head_cache['b']
         n_act, hid = self.decoder.weight.shape
         rows = -(-(n_act + 1) // 8) * 8
         with torch.no_grad():
@@ -216,20 +211,18 @@ class Default(nn.Module):
             b_cat = self.decoder.weight.new_zeros(rows)
             b_cat[:n_act] = self.decoder.bias
             b_cat[n_act] = self.value_head.bias[0]
-        if not torch.is_grad_enabled():
-            cache['key'], cache['w'], cache['b'] = key, w_cat, b_cat
+        if cache:
+            self._head_cache.update(key=key, w=w_cat, b=b_cat)
         return w_cat, b_cat
 
     def encoder_weight_tf32(self):
-        """The encoder weight rounded to TF32 (round-to-nearest, ties away: cvt.rna) for pb_policy_mlp_sample, which
-        feeds the bits straight to the tensor cores; cached with the head matrix (same invalidation)."""
+        """The encoder weight rounded to TF32 (_round_tf32) for pb_policy_mlp_sample, which feeds the bits straight to
+        the tensor cores; cached with the head matrix (same invalidation)."""
         cache = self._head_cache
         key = (self.encoder.weight.data_ptr(), torch.cuda.is_current_stream_capturing())
         if not torch.is_grad_enabled() and cache.get('ekey') == key:
             return cache['wenc']
-        with torch.no_grad():
-            bits = self.encoder.weight.detach().contiguous().view(torch.int32)
-            w = ((bits + 0x1000) & ~0x1FFF).view(torch.float32)
+        w = _round_tf32(self.encoder.weight)
         if not torch.is_grad_enabled():
             cache['ekey'], cache['wenc'] = key, w
         return w
@@ -246,7 +239,7 @@ class Default(nn.Module):
             return None
         out = _DefaultMLPFunction.apply(x.float().contiguous(), self.encoder.weight, self.encoder.bias,
                                         self.decoder.weight, self.decoder.bias, self.value_head.weight,
-                                        self.value_head.bias, self._head_cache)
+                                        self.value_head.bias, self)
         return out, self.decoder.weight.shape[0]
 
     def forward_packed_slabs(self, slabs):
@@ -258,7 +251,7 @@ class Default(nn.Module):
             return None
         out = _DefaultMLPFunction.apply(slabs.float(), self.encoder.weight, self.encoder.bias,
                                         self.decoder.weight, self.decoder.bias, self.value_head.weight,
-                                        self.value_head.bias, self._head_cache)
+                                        self.value_head.bias, self)
         return out, self.decoder.weight.shape[0]
 
     def forward(self, observations):

@@ -376,7 +376,7 @@ def test_lstm_parity_vs_reference(golden):
     (64, 16, 4, dict(update_epochs=2, norm_adv=False, max_grad_norm=1e9))], ids=['R288_clipped', 'R1024_raw_adv'])
 def test_direct_slab_update_replays_through_gathered_minibatches(n, bptt, nm, kw):
     """train() on the benchmark's path -- the fused update reading the arrival-order rollout tensors in place
-    (Experience.direct_minibatch: row_slab_stride = nm * R, returns and advantage normalisation formed in the kernel), then
+    (Experience.minibatch 'direct': row_slab_stride = nm * R, returns and advantage normalisation formed in the kernel), then
     pb_clip_adam_parts with the head rebuild in its last CTA -- replayed step by step from a snapshot of the rollout, the
     parameters and the Adam state: minibatch membership and advantages from the oracles in float64, the normalisation of
     clean_pufferl.py:211-213, pb_mlp_update_fused on contiguous gathered rows with explicit returns, pb_clip_adam (the

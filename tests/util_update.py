@@ -9,7 +9,7 @@ hand-run tests/experimental/check_mlp_update_fused.py.  Not collected by pytest 
     as the tensor core does (see reference_update), so it is not an fp32-exact reference and cannot see a wrong TF32
     rounding of the forward operands: only the stage-1 check covers that;
   * the per-block sums of squares the reduce step leaves in the workspace for pb_clip_adam_parts, after every launch.
-It covers the arguments the zero-copy train() path passes (Experience.direct_minibatch): arrival-order per-row arrays with
+It covers the arguments the zero-copy train() path passes (Experience.minibatch 'direct'): arrival-order per-row arrays with
 row_slab_stride = nm * R and the pointer offset by mb * R (every element of the other minibatches is NaN, so a misindexed read
 poisons the gradient), returns formed in the kernel (returns=None), the advantage normalisation applied in the kernel
 (adv_norm), and clip_vloss / coefficients other than the benchmark's.
@@ -160,7 +160,7 @@ def case(slab_rows, n_slabs, slab_stride, n_act, seed, variant=2, nm=None, retur
          cfg=CFG, ws=None):
     """One minibatch of `n_slabs` slabs of `slab_rows` rows whose x rows start `slab_stride` rows apart.
 
-    nm (arrival-order rows, as Experience.direct_minibatch): the per-row arrays live in buffers of n_slabs * nm slabs, the
+    nm (arrival-order rows, as Experience.minibatch 'direct'): the per-row arrays live in buffers of n_slabs * nm slabs, the
     minibatch's slab s at slab s * nm + 1, and the kernel gets the pointer offset by one slab and row_slab_stride = nm * R;
     every other element is NaN.  Otherwise they are contiguous, slab-major.  returns=False: the kernel forms raw advantages +
     old values; old_values=False (needs returns and clip_vloss = 0): no old values at all; adv_norm: the kernel normalises

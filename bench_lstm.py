@@ -32,7 +32,7 @@ from bench import METRIC, UNIT, gpu_info, ppo_config, timed_steps
 
 def parse_args():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--env', default='breakout', choices=['breakout', 'squared'])
+    ap.add_argument('--env', default='breakout', choices=['breakout', 'squared', 'memory'])
     ap.add_argument('--num-envs', type=int, default=16384)
     ap.add_argument('--horizon', type=int, default=128)
     ap.add_argument('--steps', type=int, default=5)
@@ -295,8 +295,38 @@ def main(args):
         'train': train_section(args, data, warm_peaks, feats),
         'gpu': gpu_info(0), 'profile_s': prof, 'env_stats': {k: float(v) for k, v in data.stats.items()},
     }
+    if args.env == 'memory':
+        line['memory_env_step'] = memory_env_step_times(n)
     print(json.dumps(line))
     cp.close(data)
+
+
+def memory_env_step_times(n, cycles=20):
+    """The memory env step alone (no policy), CUDA events around each send: a step-send vs a reset-send.  At the
+    default mem_length=2, mem_delay=2 every episode is 5 steps and all envs reset together, so every 6th send is a
+    reset-send; it also regenerates N * 6 outputs of the shared MT19937 stream in one CTA (k_mem_prepare)."""
+    import pufferlib_b200.vector as pvec
+    from pufferlib_b200.environments import ocean
+    vec = pvec.make(ocean.env_creator('memory'), num_envs=n, backend=pvec.B200)
+    actions = torch.zeros(n, dtype=torch.int64, device='cuda')
+    vec.async_reset(1)
+    vec.recv()
+    times = {'step': [], 'reset': []}
+    for k in range(6 * cycles):
+        reset = k % 6 == 5
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        vec.send(actions)
+        b.record()
+        vec.recv()
+        b.synchronize()
+        times['reset' if reset else 'step'].append(a.elapsed_time(b) * 1e3)
+    vec.close()
+    med = {k: float(np.median(v)) for k, v in times.items()}
+    return {'step_send_us': round(med['step'], 2), 'reset_send_us': round(med['reset'], 2),
+            'mt_outputs_per_reset_send': n * 6, 'mt_twists_per_reset_send': round(n * 6 / 624, 1),
+            'method': f'median of {len(times["step"])} step-sends and {len(times["reset"])} reset-sends, CUDA events '
+                      'around send() (env kernels + host launch), after warm-up by the PPO loop in the same process'}
 
 
 def train_section(args, data, warm_peaks, feats):

@@ -43,7 +43,11 @@ enum {
     PB_ERR_UNSUPPORTED = -4
 };
 
-enum { PB_ENV_SQUARED = 0, PB_ENV_BREAKOUT = 1, PB_ENV_SNAKE = 2, PB_ENV_PONG = 3 };
+enum {
+    PB_ENV_SQUARED = 0, PB_ENV_BREAKOUT = 1, PB_ENV_SNAKE = 2, PB_ENV_PONG = 3,
+    /* the reference's ocean test envs (environments/ocean/ocean.py; creators environment.py:33-46, 67-70) */
+    PB_ENV_MEMORY = 4, PB_ENV_PASSWORD = 5, PB_ENV_STOCHASTIC = 6, PB_ENV_BANDIT = 7
+};
 enum { PB_DTYPE_F32 = 0, PB_DTYPE_U8 = 1 };
 
 typedef struct pb_env pb_env; /* opaque: N env instances resident on one GPU */
@@ -58,7 +62,12 @@ typedef struct {
                                  SQUARED : [0]=distance_to_target (default 3; ocean/environment.py:28)
                                  BREAKOUT: [0]=max_ticks (default 4096)
                                  SNAKE   : [0]=max_ticks (default 1024)
-                                 PONG    : [0]=max_score (default 5) [1]=max_ticks (default 4096) */
+                                 PONG    : [0]=max_score (default 5) [1]=max_ticks (default 4096)
+                                 MEMORY  : [0]=mem_length in [1, 64] (default 2) [1]=mem_delay + 1, mem_delay in
+                                           [0, 1024] (0 = default 2)                    ocean.py:64-123
+                                 PASSWORD: [0]=password_length in [1, 128] (default 5)  ocean.py:228-281
+                                 STOCHASTIC: no iparam; p is dparam[0]; episodes are 100 steps  ocean.py:529-582
+                                 BANDIT  : [0]=num_actions in [1, 32768] (default 10)   ocean.py:8-62 */
 } pb_env_config;
 
 typedef struct {
@@ -97,6 +106,13 @@ uint64_t pb_launch_count(void);
  * Serial.send's per-env `if env.done: reset() else: step()` loop (vector.py:137-156), the GymnasiumPufferEnv
  * buffer writes (emulation.py:169-228) and EpisodeStats (postprocess.py:8-54), for the device-native env kinds. */
 int pb_env_create(const pb_env_config* cfg, pb_env** out);
+/* pb_env_create with kind-specific fp64 parameters (python floats of the reference creators), read from host memory;
+ * n_dparam = 0 takes the defaults:  STOCHASTIC: [0]=p (0.7);  BANDIT: [0]=reward_scale (1) [1]=reward_noise (1, only
+ * whether it is nonzero matters, ocean.py:55-57).  Other kinds ignore dparam.  pb_env_create(cfg) is
+ * pb_env_create_ex(cfg, NULL, 0).  Out-of-envelope parameters are refused with PB_ERR_INVALID.
+ * MEMORY and STOCHASTIC pass seed + i to np.random.seed (ocean.py:87-90, 551-554), which refuses seeds outside
+ * [0, 2**32): pb_env_reset refuses them too (PB_ERR_INVALID) when seed + env_index_offset + N - 1 >= 2**32. */
+int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_host, int32_t n_dparam, pb_env** out);
 int pb_env_destroy(pb_env* env);
 int pb_env_get_info(const pb_env* env, pb_env_info* out);
 
@@ -122,6 +138,9 @@ int pb_snake_set_variant(int32_t lanes_per_env);
 int pb_env_episode_rows(pb_env* env, const double** episode_return, const int32_t** episode_length,
                         const float** score);
 int pb_env_stats_read(pb_env* env, double* out4_host, int clear, void* stream);
+/* The score of pb_env_episode_rows in fp64, for the kinds whose score is a python float that fp32 does not hold
+ * (STOCHASTIC: 1 - (p - frac)**2); *score = NULL for the kinds without one (their fp32 score is exact). */
+int pb_env_episode_score_f64(pb_env* env, const double** score);
 
 /* -- rollout ---------------------------------------------------------------------------------------------------
  * Replaces the policy-output part of Experience.store (clean_pufferl.py:443-446): one fused copy of value /

@@ -64,11 +64,12 @@ void pb_env_free_common(pb_env* env) {
     if (env->h_stats_pinned) cudaFreeHost(env->h_stats_pinned);
 }
 
-extern "C" int pb_env_create(const pb_env_config* cfg, pb_env** out) {
+extern "C" int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_host, int32_t n_dparam, pb_env** out) {
     PB_REQUIRE(cfg && out, PB_ERR_INVALID, "pb_env_create: null pointer");
+    PB_REQUIRE(n_dparam >= 0 && (n_dparam == 0 || dparam_host), PB_ERR_INVALID, "pb_env_create_ex: bad dparam");
     *out = nullptr;
     PB_REQUIRE(cfg->num_envs >= 1, PB_ERR_INVALID, "num_envs must be at least 1");  // vector.py:578-579
-    PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_PONG, PB_ERR_INVALID, "unknown env kind %d",
+    PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_BANDIT, PB_ERR_INVALID, "unknown env kind %d",
                cfg->kind);
     int ndev = 0;
     PB_CUDA(cudaGetDeviceCount(&ndev));
@@ -85,6 +86,7 @@ extern "C" int pb_env_create(const pb_env_config* cfg, pb_env** out) {
             case PB_ENV_BREAKOUT: rc = pb_breakout_create(env); break;
             case PB_ENV_SNAKE: rc = pb_snake_create(env); break;
             case PB_ENV_PONG: rc = pb_pong_create(env); break;
+            default: rc = pb_ocean_create(env, dparam_host, n_dparam); break;
         }
     }
     if (rc != PB_OK) {
@@ -96,6 +98,10 @@ extern "C" int pb_env_create(const pb_env_config* cfg, pb_env** out) {
     env->info.num_envs = cfg->num_envs;
     *out = env;
     return PB_OK;
+}
+
+extern "C" int pb_env_create(const pb_env_config* cfg, pb_env** out) {
+    return pb_env_create_ex(cfg, nullptr, 0, out);
 }
 
 extern "C" int pb_env_destroy(pb_env* env) {
@@ -162,6 +168,12 @@ extern "C" int pb_env_episode_rows(pb_env* env, const double** episode_return, c
     if (episode_return) *episode_return = env->d_row_return;
     if (episode_length) *episode_length = env->d_row_length;
     if (score) *score = env->d_row_score;
+    return PB_OK;
+}
+
+extern "C" int pb_env_episode_score_f64(pb_env* env, const double** score) {
+    PB_REQUIRE(env && score, PB_ERR_INVALID, "pb_env_episode_score_f64: null pointer");
+    *score = env->d_row_score64;
     return PB_OK;
 }
 

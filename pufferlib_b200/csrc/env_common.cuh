@@ -26,6 +26,7 @@ struct pb_env {
     double* d_row_return;    // values of the episode that ended on the most recent step (valid where terminal)
     int32_t* d_row_length;
     float* d_row_score;
+    double* d_row_score64;   // optional [N]: the score in fp64, for kinds whose score is a python float (NULL otherwise)
     double* d_stats;         // [PB_STAT_SLOTS][4] episodes, sum return, sum length, sum score (slot = warp hash:
                              // same-address atomics serialise in L2, spreading them keeps the step kernel flat)
     double* h_stats_pinned;  // [PB_STAT_SLOTS][4] pinned staging for pb_env_stats_read
@@ -47,6 +48,7 @@ int pb_squared_create(pb_env* env);
 int pb_breakout_create(pb_env* env);
 int pb_snake_create(pb_env* env);
 int pb_pong_create(pb_env* env);
+int pb_ocean_create(pb_env* env, const double* dparam, int n_dparam);   // memory, password, stochastic, bandit
 
 struct EpisodeAcc {
     double* ep_return;
@@ -55,6 +57,7 @@ struct EpisodeAcc {
     int32_t* row_length;
     float* row_score;
     double* stats;
+    double* row_score64;     // may be NULL
 };
 
 #ifdef __CUDACC__
@@ -63,7 +66,7 @@ struct EpisodeAcc {
 // postprocess.py:18-20 clears the accumulators).
 
 __device__ __forceinline__ void episode_update(const EpisodeAcc& acc, int64_t e, bool active, bool reset_row,
-                                               double reward, bool finished, float score) {
+                                               double reward, bool finished, double score) {
     double ret = 0.0;
     int len = 0;
     if (active) {
@@ -78,7 +81,8 @@ __device__ __forceinline__ void episode_update(const EpisodeAcc& acc, int64_t e,
             if (finished) {
                 acc.row_return[e] = ret;
                 acc.row_length[e] = len;
-                acc.row_score[e] = score;
+                acc.row_score[e] = (float)score;
+                if (acc.row_score64) acc.row_score64[e] = score;
             }
         }
     }
@@ -86,7 +90,7 @@ __device__ __forceinline__ void episode_update(const EpisodeAcc& acc, int64_t e,
     const bool fin = active && !reset_row && finished;
     const unsigned m = __ballot_sync(0xffffffffu, fin);
     if (m) {
-        double r = fin ? ret : 0.0, l = fin ? (double)len : 0.0, s = fin ? (double)score : 0.0;
+        double r = fin ? ret : 0.0, l = fin ? (double)len : 0.0, s = fin ? score : 0.0;
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) {
             r += __shfl_xor_sync(0xffffffffu, r, off);
@@ -104,9 +108,15 @@ __device__ __forceinline__ void episode_update(const EpisodeAcc& acc, int64_t e,
     }
 }
 
+// the kinds whose score is an fp32 value
+__device__ __forceinline__ void episode_update(const EpisodeAcc& acc, int64_t e, bool active, bool reset_row,
+                                               double reward, bool finished, float score) {
+    episode_update(acc, e, active, reset_row, reward, finished, (double)score);
+}
+
 #endif
 
 static inline EpisodeAcc pb_episode_acc(const pb_env* env) {
     return EpisodeAcc{env->d_ep_return, env->d_ep_length, env->d_row_return, env->d_row_length, env->d_row_score,
-                      env->d_stats};
+                      env->d_stats, env->d_row_score64};
 }

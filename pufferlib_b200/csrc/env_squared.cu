@@ -19,10 +19,9 @@
 // cooperatively (lanes stride across the (2d+1)^2 floats of one row: coalesced 128 B stores); reward / flag /
 // done rows are [N]-contiguous stores.  Per-env state is 8 bytes in HBM.
 #include "env_common.cuh"
+#include "mt19937.cuh"
 
 namespace {
-
-constexpr int MT_N = 624, MT_M = 397;
 
 struct SquaredState {
     int d, g, n_targets, bits;  // distance_to_target, grid size, 8d perimeter cells, bit_length(8d)
@@ -42,53 +41,17 @@ __host__ __device__ inline void target_from_index(int j, int g, int& x, int& y) 
     else { const int m = j - g; x = 1 + (m >> 1); y = (m & 1) ? g - 1 : 0; }
 }
 
-__device__ __forceinline__ uint32_t mt_temper(uint32_t y) {
-    y ^= y >> 11;
-    y ^= (y << 7) & 0x9D2C5680u;
-    y ^= (y << 15) & 0xEFC60000u;
-    y ^= y >> 18;
-    return y;
-}
-__device__ __forceinline__ uint32_t mt_mix(uint32_t u, uint32_t v) {
-    const uint32_t y = (u & 0x80000000u) | (v & 0x7FFFFFFFu);
-    return (y >> 1) ^ ((y & 1u) ? 0x9908B0DFu : 0u);
-}
-
 // async_reset: env i <- random.seed(seed + i); target = possible_targets[randbelow(8d)]
 __global__ void __launch_bounds__(64) k_sq_seed(SquaredState st, int n, uint64_t seed_base, uint8_t* done) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     uint32_t mt[MT_N];
-    // random.seed(int): init_by_array(32-bit little-endian words of |seed|)
-    const uint64_t s = seed_base + (uint64_t)i;
-    uint32_t key[2] = {(uint32_t)s, (uint32_t)(s >> 32)};
-    const int klen = key[1] ? 2 : 1;
-    mt[0] = 19650218u;
-    for (int k = 1; k < MT_N; ++k) mt[k] = 1812433253u * (mt[k - 1] ^ (mt[k - 1] >> 30)) + (uint32_t)k;
-    int a = 1, b = 0;
-    for (int k = (MT_N > klen ? MT_N : klen); k; --k) {
-        mt[a] = (mt[a] ^ ((mt[a - 1] ^ (mt[a - 1] >> 30)) * 1664525u)) + key[b] + (uint32_t)b;
-        ++a; ++b;
-        if (a >= MT_N) { mt[0] = mt[MT_N - 1]; a = 1; }
-        if (b >= klen) b = 0;
-    }
-    for (int k = MT_N - 1; k; --k) {
-        mt[a] = (mt[a] ^ ((mt[a - 1] ^ (mt[a - 1] >> 30)) * 1566083941u)) - (uint32_t)a;
-        ++a;
-        if (a >= MT_N) { mt[0] = mt[MT_N - 1]; a = 1; }
-    }
-    mt[0] = 0x80000000u;
+    mt_seed_by_array(mt, seed_base + (uint64_t)i);   // random.seed(int)
     int idx = MT_N;
     int draw;
-    for (;;) {
-        if (idx >= MT_N) {
-            for (int k = 0; k < MT_N; ++k)
-                mt[k] = mt[(k + MT_M) % MT_N] ^ mt_mix(mt[k], mt[(k + 1) % MT_N]);
-            idx = 0;
-        }
-        draw = (int)(mt_temper(mt[idx++]) >> (32 - st.bits));
-        if (draw < st.n_targets) break;
-    }
+    do {
+        draw = (int)(mt_next(mt, idx) >> (32 - st.bits));
+    } while (draw >= st.n_targets);
     int tx, ty;
     target_from_index(draw, st.g, tx, ty);
     st.d_target[i] = (uint16_t)(tx | (ty << 8));
@@ -103,73 +66,21 @@ __global__ void __launch_bounds__(64) k_sq_seed(SquaredState st, int n, uint64_t
 // One block: rank the envs that reset on this send and produce their draws from the global stream.
 constexpr int PREP_THREADS = 256;
 
-__device__ int block_exclusive_scan(int v, int* total, int* s_warp) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int x = v;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, x, off);
-        if (lane >= off) x += y;
-    }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    int base = 0, tot = 0;
-    for (int w = 0; w < PREP_THREADS / 32; ++w) {
-        if (w < warp) base += s_warp[w];
-        tot += s_warp[w];
-    }
-    __syncthreads();
-    *total = tot;
-    return base + x - v;
-}
-
 __global__ void __launch_bounds__(PREP_THREADS) k_sq_prepare(SquaredState st, int n, const uint8_t* done) {
     __shared__ uint32_t mt[MT_N];
     __shared__ int s_warp[PREP_THREADS / 32];
     __shared__ int s_idx, s_newidx;
     const int tid = threadIdx.x;
-    // ranks in env order
-    int R = 0;
-    for (int base = 0; base < n; base += PREP_THREADS) {
-        const int e = base + tid;
-        const int flag = (e < n && done[e]) ? 1 : 0;
-        int tot;
-        const int off = block_exclusive_scan(flag, &tot, s_warp);
-        if (e < n) st.d_rank[e] = flag ? R + off : -1;
-        R += tot;
-    }
+    const int R = rank_resets<PREP_THREADS>(done, n, st.d_rank, s_warp);   // ranks in env order
     if (R == 0) return;
     for (int k = tid; k < MT_N; k += PREP_THREADS) mt[k] = st.d_mt[k];
     if (tid == 0) s_idx = (int)st.d_mt[MT_N];
     __syncthreads();
     int accepted = 0;
     while (accepted < R) {
-        if (s_idx >= MT_N) {  // parallel twist: 3 independent spans + the wrap-around element
-            uint32_t v[3];
-            int cnt = 0;
-            for (int k = tid; k < MT_N - MT_M; k += PREP_THREADS) v[cnt++] = mt[k + MT_M] ^ mt_mix(mt[k], mt[k + 1]);
-            __syncthreads();
-            cnt = 0;
-            for (int k = tid; k < MT_N - MT_M; k += PREP_THREADS) mt[k] = v[cnt++];
-            __syncthreads();
-            cnt = 0;
-            for (int k = MT_N - MT_M + tid; k < 2 * (MT_N - MT_M); k += PREP_THREADS)
-                v[cnt++] = mt[k - (MT_N - MT_M)] ^ mt_mix(mt[k], mt[k + 1]);
-            __syncthreads();
-            cnt = 0;
-            for (int k = MT_N - MT_M + tid; k < 2 * (MT_N - MT_M); k += PREP_THREADS) mt[k] = v[cnt++];
-            __syncthreads();
-            cnt = 0;
-            for (int k = 2 * (MT_N - MT_M) + tid; k < MT_N - 1; k += PREP_THREADS)
-                v[cnt++] = mt[k - (MT_N - MT_M)] ^ mt_mix(mt[k], mt[k + 1]);
-            __syncthreads();
-            cnt = 0;
-            for (int k = 2 * (MT_N - MT_M) + tid; k < MT_N - 1; k += PREP_THREADS) mt[k] = v[cnt++];
-            __syncthreads();
-            if (tid == 0) {
-                mt[MT_N - 1] = mt[MT_M - 1] ^ mt_mix(mt[MT_N - 1], mt[0]);
-                s_idx = 0;
-            }
+        if (s_idx >= MT_N) {
+            mt_twist_block<PREP_THREADS>(mt);
+            if (tid == 0) s_idx = 0;
             __syncthreads();
         }
         const int start = s_idx;
@@ -179,7 +90,7 @@ __global__ void __launch_bounds__(PREP_THREADS) k_sq_prepare(SquaredState st, in
         if (valid) draw = (int)(mt_temper(mt[pos]) >> (32 - st.bits));
         const int acc = (valid && draw < st.n_targets) ? 1 : 0;
         int tot;
-        const int off = block_exclusive_scan(acc, &tot, s_warp);
+        const int off = block_exclusive_scan<PREP_THREADS>(acc, &tot, s_warp);
         if (acc && accepted + off < R) {
             st.d_draws[accepted + off] = draw;
             if (accepted + off == R - 1) s_newidx = pos + 1;  // stream position just after the last used output

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from pufferlib_b200 import _native, spaces
-from pufferlib_b200.environments import resolve
+from pufferlib_b200.environments import GLOBAL_STREAM_KINDS, resolve_config
 from pufferlib_b200.exceptions import APIUsageError
 from pufferlib_b200.namespace import Namespace, namespace
 
@@ -140,9 +140,9 @@ class B200:
         for k in kwargs:
             if k not in ('num_workers', 'batch_size', 'zero_copy', 'backend'):
                 raise APIUsageError(f'Invalid argument: {k}')
-        kind, iparam = resolve(env_creators[0], env_args[0], env_kwargs[0])
+        kind, iparam, dparam = resolve_config(env_creators[0], env_args[0], env_kwargs[0])
         for c, a, k in zip(env_creators, env_args, env_kwargs):
-            if resolve(c, a, k) != (kind, iparam):
+            if resolve_config(c, a, k) != (kind, iparam, dparam):
                 raise APIUsageError('B200 backend: all env creators / args must be identical')
         if not torch.cuda.is_available():
             raise RuntimeError('pufferlib_b200 needs a CUDA device (no CPU fallback)')
@@ -153,12 +153,13 @@ class B200:
         self.exact_infos = self.host_buffers if exact_infos is None else bool(exact_infos)
         lib = _native.lib()
         # num_workers (the reference's Multiprocessing argument): every worker PROCESS there runs a Serial over its envs
-        # with its own process-global `random` stream (vector.py:168-190, seeds sliced per worker at :424-428).  Only envs
-        # that draw from that global stream depend on it (ocean.Squared); for them the envs are split into one pb_env
-        # shard per worker, each with its own MT19937 stream, writing into the same contiguous buffers.  The other
-        # kinds key their counter-based RNG by global env index, so the worker split cannot change their results.
+        # with its own process-global `random` / `np.random` stream (vector.py:168-190, seeds sliced per worker at
+        # :424-428).  Only envs that draw from such a global stream depend on it (GLOBAL_STREAM_KINDS); for them the envs
+        # are split into one pb_env shard per worker, each with its own MT19937 stream, writing into the same contiguous
+        # buffers.  The other kinds key their RNG by global env index or draw nothing, so the worker split cannot change
+        # their results.
         workers = kwargs.get('num_workers') or 1
-        if kind != 'squared' or workers <= 1:
+        if kind not in GLOBAL_STREAM_KINDS or workers <= 1:
             workers = 1
         if num_envs % workers != 0:
             raise APIUsageError('num_envs must be divisible by num_workers')
@@ -169,7 +170,8 @@ class B200:
                                     reserved=0, env_index_offset=int(env_index_offset) + w * per,
                                     iparam=(C.c_int32 * 8)(*iparam))
             handle = C.c_void_p()
-            _native.check(lib.pb_env_create(C.byref(cfg), C.byref(handle)))
+            dp = (C.c_double * max(len(dparam), 1))(*dparam)
+            _native.check(lib.pb_env_create_ex(C.byref(cfg), dp, len(dparam), C.byref(handle)))
             self._shards.append((handle, w * per, per))
         self._handle = self._shards[0][0]
         info = _native.EnvInfo()
@@ -459,19 +461,32 @@ class B200:
             return []
         lib = _native.lib()
         n = self.num_agents
-        # the three per-env arrays through ONE staging tensor and ONE device->host copy (one sync instead of three)
-        stage = torch.empty(16 * n, dtype=torch.uint8, device=self.buf.terminals.device)
+        # the per-env arrays through ONE staging tensor and ONE device->host copy (one sync instead of three); kinds with
+        # an fp64 score (a python float in the reference) add it behind the fp32 rows
+        stage = torch.empty(24 * n, dtype=torch.uint8, device=self.buf.terminals.device)
         base, s_ = stage.data_ptr(), _native.stream_ptr()
+        f64 = []
         for handle, lo, cnt in self._shards:
-            p_ret, p_len, p_score = C.c_void_p(), C.c_void_p(), C.c_void_p()
+            p_ret, p_len, p_score, p_s64 = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
             _native.check(lib.pb_env_episode_rows(handle, C.byref(p_ret), C.byref(p_len), C.byref(p_score)))
-            for src, off, nbytes in ((p_ret.value, 8 * lo, 8 * cnt), (p_len.value, 8 * n + 4 * lo, 4 * cnt),
-                                     (p_score.value, 12 * n + 4 * lo, 4 * cnt)):
+            _native.check(lib.pb_env_episode_score_f64(handle, C.byref(p_s64)))
+            parts = [(p_ret.value, 8 * lo, 8 * cnt), (p_len.value, 8 * n + 4 * lo, 4 * cnt),
+                     (p_score.value, 12 * n + 4 * lo, 4 * cnt)]
+            if p_s64.value:
+                parts.append((p_s64.value, 16 * n + 8 * lo, 8 * cnt))
+                f64.append((lo, cnt))
+            for src, off, nbytes in parts:
                 _native.check(lib.pb_copy_rows(C.c_void_p(src), nbytes, C.c_void_p(base + off), nbytes, nbytes, 1, s_))
-        host = stage.cpu().numpy()
+        host = stage[:24 * n if f64 else 16 * n].cpu().numpy()
         ret, length, score = host[:8 * n].view(np.float64), host[8 * n:12 * n].view(np.int32), \
-            host[12 * n:].view(np.float32)
+            host[12 * n:16 * n].view(np.float32)
         self.d2h_bytes += n * 16
+        if f64:
+            score = score.astype(np.float64)
+            score64 = host[16 * n:].view(np.float64)
+            for lo, cnt in f64:
+                score[lo:lo + cnt] = score64[lo:lo + cnt]
+            self.d2h_bytes += n * 8
         return [{'episode_return': float(ret[i]), 'episode_length': int(length[i]), 'score': float(score[i])}
                 for i in idx]
 

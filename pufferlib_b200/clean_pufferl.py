@@ -99,8 +99,9 @@ class _FusedPPOLoss(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logits, value, actions, old_logprobs, adv, returns, old_values, cfg, packed_n_act):
-        """packed_n_act > 0: `logits` is the packed head output [M, 8] (logits | value | zero pad) and `value` is
-        ignored; the gradient comes back as ONE [M, 8] tensor (no slice/cat nodes in the autograd graph)."""
+        """packed_n_act > 0: `logits` is the packed head output [M, R] (logits | value | zero pad; R = 8 for
+        n_act <= 7, 16 for n_act <= 15) and `value` is ignored; the gradient comes back as ONE [M, R] tensor (no
+        slice/cat nodes in the autograd graph)."""
         clip_coef, clip_vloss, vf_clip_coef, vf_coef, ent_coef = cfg
         dev = logits.device
         if packed_n_act:
@@ -109,8 +110,8 @@ class _FusedPPOLoss(torch.autograd.Function):
             assert out.stride(1) == 1 and out.dtype == torch.float32
             l_ptr, l_stride = out.data_ptr(), out.stride(0)
             v_ptr, v_stride = out.data_ptr() + 4 * n_act, out.stride(0)
-            # [M, 8] rows: the kernel writes whole rows (zero padding included); other widths need the memset
-            grad = torch.empty_like(out) if out.shape[1] == 8 and n_act <= 7 else torch.zeros_like(out)
+            # [M, 8] and [M, 16] rows: the kernel writes whole rows (zero padding included); other widths need the memset
+            grad = torch.empty_like(out) if out.shape[1] in (8, 16) and n_act < out.shape[1] else torch.zeros_like(out)
             gl_ptr, gl_stride, gv_ptr, gv_stride = grad.data_ptr(), grad.stride(0), grad.data_ptr() + 4 * n_act, grad.stride(0)
             ctx.packed = True
             ctx.save_for_backward(grad)
@@ -161,7 +162,8 @@ def fused_ppo_loss(logits, value, actions, old_logprobs, adv, returns, old_value
 
 
 def fused_ppo_loss_packed(out, n_act, actions, old_logprobs, adv, returns, old_values, config):
-    """Same, on the packed head output [M, 8] of models.Default.forward_packed (one [M, 8] gradient back)."""
+    """Same, on the packed head output [M, R] of models.Default.forward_packed or models.LSTMWrapper.forward_packed_seq
+    (R = 8 for n_act <= 7, 16 for n_act <= 15): one [M, R] gradient back."""
     return _FusedPPOLoss.apply(out, None, actions, old_logprobs, adv, returns, old_values, _loss_cfg(config), int(n_act))
 
 
@@ -201,11 +203,12 @@ class _DefaultMLPUpdate:
     large kernels, and everything autograd, clip_grad_norm_ and the optimizer add around it (gradient scaling by the
     upstream 1.0, AccumulateGrad copies, ~12 norm/clip/Adam launches, 6 launches to re-pack the heads, 8 to fold the
     statistics) is a dozen short launches per minibatch.  Chain per minibatch:
-        encoder GEMM (+bias+ReLU epilogue, one per slab) -> 8-column head GEMM -> pb_ppo_loss (loss statistics +
-        analytic dLoss/dOut) -> pb_mlp_tail_backward (dPre, dW_heads, db_heads, db_enc) -> split-K dW_enc GEMM + sum
-        [-> gradient all-reduce over ONE flat buffer when world_size > 1] -> pb_clip_adam -> pb_pack_heads.
+        encoder GEMM (+bias+ReLU epilogue, one per slab) -> R-column head GEMM -> pb_ppo_loss (loss statistics +
+        analytic dLoss/dOut) -> pb_mlp_tail_backward_ex (dPre, dW_heads, db_heads, db_enc) -> split-K dW_enc GEMM + sum
+        [-> gradient all-reduce over ONE flat buffer when world_size > 1] -> pb_clip_adam -> pb_pack_heads,
+    with R = 8 head rows for n_act <= 7 and 16 for 8 <= n_act <= 15 (models.Default.head_matrix).
     train() passes each minibatch as Experience.minibatch() to forward_backward; where _fused_ok holds (minibatch_form
-    asks it too) the chain is ONE kernel, pb_mlp_update_fused.
+    asks it too; <= 7 actions) the chain is ONE kernel, pb_mlp_update_fused.
     Same math as the autograd path (tests/test_gpu_experience.py::test_manual_update_matches_autograd_update); the
     optimizer's own state tensors are updated in place, so state_dict() and optimizer.step() keep working."""
 
@@ -224,7 +227,7 @@ class _DefaultMLPUpdate:
             if world > 1:
                 return False      # opt-out: ranks > 1 on the autograd + GradBucket (NCCL) path
         n_act, hid = model.decoder.weight.shape
-        if hid != 128 or n_act > 7 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
+        if hid != 128 or n_act > 15 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
             return False
         g = opt.param_groups[0]
         if len(opt.param_groups) != 1 or g.get('amsgrad') or g.get('weight_decay') or g.get('maximize'):
@@ -240,15 +243,16 @@ class _DefaultMLPUpdate:
         dev = model.encoder.weight.device
         self.n_act, self.hid = model.decoder.weight.shape
         self.features = model.encoder.weight.shape[1]
-        hid, f_, n_act = self.hid, self.features, self.n_act
+        self.head_rows = 8 if self.n_act + 1 <= 8 else 16
+        hid, f_, n_act, rows = self.hid, self.features, self.n_act, self.head_rows
         z = dict(dtype=torch.float32, device=dev)
-        # ONE flat gradient buffer: dW_enc | dW_heads (8 x hid) | db_enc | db_heads (8)  (also the all-reduce bucket)
-        self.gflat = torch.zeros(hid * f_ + 8 * hid + hid + 8, **z)
+        # ONE flat gradient buffer: dW_enc | dW_heads (R x hid) | db_enc | db_heads (R)  (also the all-reduce bucket)
+        self.gflat = torch.zeros(hid * f_ + rows * hid + hid + rows, **z)
         self.dw_enc = self.gflat[:hid * f_].view(hid, f_)
         self.tail = self.gflat[hid * f_:]
-        dw_cat = self.tail[:8 * hid].view(8, hid)
-        db_enc, db_cat = self.tail[8 * hid:9 * hid], self.tail[9 * hid:]
-        self.w_cat, self.b_cat = torch.zeros(8, hid, **z), torch.zeros(8, **z)
+        dw_cat = self.tail[:rows * hid].view(rows, hid)
+        db_enc, db_cat = self.tail[rows * hid:(rows + 1) * hid], self.tail[(rows + 1) * hid:]
+        self.w_cat, self.b_cat = torch.zeros(rows, hid, **z), torch.zeros(rows, **z)
         params = [model.encoder.weight, model.encoder.bias, model.decoder.weight, model.decoder.bias,
                   model.value_head.weight, model.value_head.bias]
         grads = [self.dw_enc, db_enc, dw_cat[:n_act], db_cat[:n_act], dw_cat[n_act:n_act + 1], db_cat[n_act:n_act + 1]]
@@ -304,9 +308,9 @@ class _DefaultMLPUpdate:
         if self.rows != m:
             z = dict(dtype=torch.float32, device=self.gflat.device)
             self.hidden, self.dpre = torch.empty(m, self.hid, **z), torch.empty(m, self.hid, **z)
-            self.out, self.dout = torch.empty(m, 8, **z), torch.empty(m, 8, **z)
-            self.ws = torch.empty(_native.lib().pb_mlp_tail_workspace_bytes(m, self.hid), dtype=torch.uint8,
-                                  device=self.gflat.device)
+            self.out, self.dout = torch.empty(m, self.head_rows, **z), torch.empty(m, self.head_rows, **z)
+            self.ws = torch.empty(_native.lib().pb_mlp_tail_workspace_bytes_ex(m, self.hid, self.head_rows),
+                                  dtype=torch.uint8, device=self.gflat.device)
             self.rows = m
 
     def _dw_enc(self, dpre, x):
@@ -327,9 +331,10 @@ class _DefaultMLPUpdate:
 
     def _fused_ok(self, x, config):
         """pb_mlp_update_fused (csrc/mlp_update.cu): fp32 observations with exactly 128 features in equally spaced row
-        slabs -- the C2 / C5 workload.  Everything else takes the kernel chain below."""
+        slabs and <= 7 actions (the 8-row head matrix) -- the C2 / C5 workload.  Everything else takes the kernel chain
+        below."""
         return (bool(getattr(config, 'fused_update', FUSED_UPDATE_DEFAULT)) and x.dtype == torch.float32 and x.shape[2] == 128
-                and self.hid == 128 and x.stride(2) == 1 and x.stride(1) % 4 == 0 and x.data_ptr() % 16 == 0
+                and self.hid == 128 and self.head_rows == 8 and x.stride(2) == 1 and x.stride(1) % 4 == 0 and x.data_ptr() % 16 == 0
                 and (x.shape[0] == 1 or (x.stride(0) % x.stride(1) == 0 and x.stride(0) >= x.shape[1] * x.stride(1))))
 
     @torch.no_grad()
@@ -384,16 +389,16 @@ class _DefaultMLPUpdate:
             torch._addmm_activation(b_enc, x[g], w_enc.t(), use_gelu=False, out=self.hidden[g * r_:(g + 1) * r_])
         torch.addmm(self.b_cat, self.hidden, self.w_cat.t(), out=self.out)
         cp = C.c_void_p
-        o_ptr, d_ptr, n_act = self.out.data_ptr(), self.dout.data_ptr(), self.n_act
+        o_ptr, d_ptr, n_act, rows = self.out.data_ptr(), self.dout.data_ptr(), self.n_act, self.head_rows
         _native.check(lib.pb_ppo_loss(
-            cp(o_ptr), 8, cp(o_ptr + 4 * n_act), 8, _native.ptr(atn.reshape(-1)), _native.ptr(log_probs.reshape(-1)),
+            cp(o_ptr), rows, cp(o_ptr + 4 * n_act), rows, _native.ptr(atn.reshape(-1)), _native.ptr(log_probs.reshape(-1)),
             _native.ptr(adv.reshape(-1)), _native.ptr(ret.reshape(-1)), _native.ptr(val.reshape(-1)), m, n_act,
             C.c_float(config.clip_coef), int(bool(config.clip_vloss)), C.c_float(config.vf_clip_coef),
-            C.c_float(config.vf_coef), C.c_float(config.ent_coef), cp(d_ptr), 8, cp(d_ptr + 4 * n_act), 8,
+            C.c_float(config.vf_coef), C.c_float(config.ent_coef), cp(d_ptr), rows, cp(d_ptr + 4 * n_act), rows,
             cp(self.stats.data_ptr() + 64 * k), s))
-        _native.check(lib.pb_mlp_tail_backward(_native.ptr(self.dout), 8, _native.ptr(self.w_cat),
-                                               _native.ptr(self.hidden), m, hid, _native.ptr(self.dpre),
-                                               _native.ptr(self.tail), _native.ptr(self.ws), self.ws.numel(), s))
+        _native.check(lib.pb_mlp_tail_backward_ex(_native.ptr(self.dout), rows, _native.ptr(self.w_cat),
+                                                  _native.ptr(self.hidden), m, hid, _native.ptr(self.dpre),
+                                                  _native.ptr(self.tail), _native.ptr(self.ws), self.ws.numel(), rows, s))
         self._dw_enc(self.dpre, x)
 
     def all_reduce(self):

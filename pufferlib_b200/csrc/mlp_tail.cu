@@ -5,24 +5,39 @@
 // memory-bound work on [M, H] tensors that ATen runs as five launches, each re-reading 268 MB at M = 524288:
 //   dHidden = dOut @ W_heads           (skinny GEMM, 8 columns)         dW_heads = dOut^T @ hidden   (skinny GEMM)
 //   db_heads = sum_rows dOut           dPre = dHidden * (hidden > 0)    db_enc = sum_rows dPre
-// This kernel does all five reading `hidden` ONCE and writing dPre once (2 * 4H + 32 B per row).  The dense H x H
+// This kernel does all five reading `hidden` ONCE and writing dPre once (2 * 4H + 4 NO B per row).  The dense H x H
 // encoder GEMMs (forward, and dW_enc = dPre^T @ obs) stay on cuBLAS tensor cores.
+// NO = the padded head rows: 8 for n_act <= 7, 16 for 8 <= n_act <= 15 (models.Default.head_matrix); both kernels are
+// templates on it.
 // A warp owns rows; lane l owns columns 4l..4l+3 (one float4 per row per lane, 512 B coalesced for H = 128); the
 // head weights live in registers (NO x 4 per lane); per-lane accumulators (dW: NO x 4, db_enc: 4) are reduced over
 // the block's warps in shared memory and written as ONE partial row per block; a second tiny kernel sums the
 // partials in a fixed order (deterministic, no atomics).
+// Registers at NO = 16: the weights and the dW accumulators alone are 128 per thread, so the TMA kernel runs one
+// 256-thread CTA per SM (its 4-stage ring still keeps 72 KB per SM in flight).  Moving W_heads to shared memory would
+// add 16 LDS.128 per row and warp to the 5 the row needs, about the whole shared-memory bandwidth budget of a row at
+// HBM speed, so the weights stay in registers.
 #include "pb_common.cuh"
 #include "tma.cuh"
 
 namespace {
 
-constexpr int NO = 8;          // padded number of head outputs (n_act + 1 <= 8)
 constexpr int MT_THREADS = 256;
 constexpr int MT_WARPS = MT_THREADS / 32;
 constexpr int ROWS_PER_BLOCK = 512;
 
+// the row's NO head gradients from NO / 4 float4s (every lane of the warp reads the same bytes: a broadcast)
+template <int NO>
+__device__ __forceinline__ void tail_load_dout(const float* src, float (&d)[NO]) {
+#pragma unroll
+    for (int j = 0; j < NO / 4; ++j) {
+        const float4 v = *reinterpret_cast<const float4*>(src + 4 * j);
+        d[4 * j] = v.x; d[4 * j + 1] = v.y; d[4 * j + 2] = v.z; d[4 * j + 3] = v.w;
+    }
+}
+
 // partial layout per block: [NO*H] dW_heads | [H] db_enc | [NO] db_heads
-template <int H>
+template <int H, int NO>
 __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd(const float* __restrict__ dout, int64_t dout_stride,
                                                             const float* __restrict__ w_heads,   // [NO][H]
                                                             const float* __restrict__ hidden,    // [M][H] post-ReLU
@@ -31,7 +46,11 @@ __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd(const float* __rest
     static_assert(H % 128 == 0, "H must be a multiple of 128 (one or more float4 per lane)");
     constexpr int Q = H / 128;                  // float4s per lane per row
     constexpr int PSTRIDE = NO * H + H + NO;
-    __shared__ float s_red[MT_WARPS][PSTRIDE > 2048 ? 1 : PSTRIDE];   // H = 128: 8 x 1160 floats = 37 KB
+    // the block reduction goes through [WARPS][8 H + H + NO] floats (H = 128: 37 KB at NO = 8, 37.4 KB at NO = 16) in
+    // NO / 8 passes of 8 dW_heads rows; the first pass also carries db_enc and db_heads.  NO = 8 is one pass over the
+    // whole partial row.
+    constexpr int RSTRIDE = 8 * H + H + NO;
+    __shared__ float s_red[MT_WARPS][RSTRIDE];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 
     float4 w[NO][Q];
@@ -55,10 +74,9 @@ __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd(const float* __rest
     const int64_t row_end = min(row0 + ROWS_PER_BLOCK, m);
 #pragma unroll 2
     for (int64_t r = row0 + warp; r < row_end; r += MT_WARPS) {
-        // the row's 8 head gradients: every lane reads the same 32 bytes (broadcast)
-        const float4 d0 = *reinterpret_cast<const float4*>(dout + r * dout_stride);
-        const float4 d1 = *reinterpret_cast<const float4*>(dout + r * dout_stride + 4);
-        const float d[NO] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+        // the row's NO head gradients: every lane reads the same 4 NO bytes (broadcast)
+        float d[NO];
+        tail_load_dout<NO>(dout + r * dout_stride, d);
 #pragma unroll
         for (int k = 0; k < NO; ++k) acc_o[k] += d[k];
 #pragma unroll
@@ -81,33 +99,63 @@ __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd(const float* __rest
     }
     // ---- block reduction: every warp deposits its partial, then the block sums the 8 deposits column-wise
     float* mine = s_red[warp];
-#pragma unroll
-    for (int k = 0; k < NO; ++k)
-#pragma unroll
-        for (int q = 0; q < Q; ++q) *reinterpret_cast<float4*>(mine + k * H + 128 * q + 4 * lane) = acc_w[k][q];
-#pragma unroll
-    for (int q = 0; q < Q; ++q) *reinterpret_cast<float4*>(mine + NO * H + 128 * q + 4 * lane) = acc_b[q];
-    if (lane == 0)
-#pragma unroll
-        for (int k = 0; k < NO; ++k) mine[NO * H + H + k] = acc_o[k];
-    __syncthreads();
     float* out = partials + (int64_t)blockIdx.x * PSTRIDE;
-    for (int j = threadIdx.x; j < PSTRIDE; j += MT_THREADS) {
-        float s = 0.f;
+    if constexpr (NO == 8) {   // the partial row fits: one pass, s_red row = partial row
 #pragma unroll
-        for (int wq = 0; wq < MT_WARPS; ++wq) s += s_red[wq][j];
-        out[j] = s;
+        for (int k = 0; k < NO; ++k)
+#pragma unroll
+            for (int q = 0; q < Q; ++q) *reinterpret_cast<float4*>(mine + k * H + 128 * q + 4 * lane) = acc_w[k][q];
+#pragma unroll
+        for (int q = 0; q < Q; ++q) *reinterpret_cast<float4*>(mine + NO * H + 128 * q + 4 * lane) = acc_b[q];
+        if (lane == 0)
+#pragma unroll
+            for (int k = 0; k < NO; ++k) mine[NO * H + H + k] = acc_o[k];
+        __syncthreads();
+        for (int j = threadIdx.x; j < PSTRIDE; j += MT_THREADS) {
+            float s = 0.f;
+#pragma unroll
+            for (int wq = 0; wq < MT_WARPS; ++wq) s += s_red[wq][j];
+            out[j] = s;
+        }
+    } else {
+        // pass p: dW_heads rows 8p..8p+7 at s_red[.][0, 8H); pass 0 also db_enc at [8H, 9H) and db_heads at [9H, 9H + NO)
+#pragma unroll
+        for (int pass = 0; pass < NO / 8; ++pass) {
+            if (pass > 0) __syncthreads();   // the previous pass has been summed
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+#pragma unroll
+                for (int q = 0; q < Q; ++q)
+                    *reinterpret_cast<float4*>(mine + k * H + 128 * q + 4 * lane) = acc_w[8 * pass + k][q];
+            if (pass == 0) {
+#pragma unroll
+                for (int q = 0; q < Q; ++q) *reinterpret_cast<float4*>(mine + 8 * H + 128 * q + 4 * lane) = acc_b[q];
+                if (lane == 0)
+#pragma unroll
+                    for (int k = 0; k < NO; ++k) mine[9 * H + k] = acc_o[k];
+            }
+            __syncthreads();
+            const int n = pass == 0 ? RSTRIDE : 8 * H;
+            for (int j = threadIdx.x; j < n; j += MT_THREADS) {
+                float s = 0.f;
+#pragma unroll
+                for (int wq = 0; wq < MT_WARPS; ++wq) s += s_red[wq][j];
+                // s_red column j -> partial column: dW rows of this pass, then (pass 0) db_enc | db_heads after all NO rows
+                out[j < 8 * H ? 8 * pass * H + j : (NO - 8) * H + j] = s;
+            }
+        }
     }
 }
 
-// TMA-staged variant (dout contiguous [M][8]): the hidden rows and their head gradients are pulled into a 4-stage
-// shared-memory ring by cp.async.bulk (one elected thread, mbarrier complete_tx), 32 rows = 16 KiB + 1 KiB per stage,
-// so ~64 KiB per CTA is in flight independently of the register budget; the warps consume from shared memory
-// (conflict-free LDS.128) and stream dPre straight back to HBM.
+// TMA-staged variant (dout contiguous [M][NO]): the hidden rows and their head gradients are pulled into a 4-stage
+// shared-memory ring by cp.async.bulk (one elected thread, mbarrier complete_tx), 32 rows = 16 KiB + NO / 8 KiB per
+// stage, so ~64 KiB per CTA is in flight independently of the register budget; the warps consume from shared memory
+// (conflict-free LDS.128) and stream dPre straight back to HBM.  Dynamic shared memory: the ring plus the [WARPS][PSTRIDE]
+// reduction buffer, 105 KB at NO = 8 (2 CTAs per SM), 140.5 KB at NO = 16.
 constexpr int TT_STAGES = 4;
 constexpr int TT_CHUNK = 32;   // rows per stage
 
-template <int H>
+template <int H, int NO>
 __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd_tma(const float* __restrict__ dout,      // [M][NO]
                                                                 const float* __restrict__ w_heads,   // [NO][H]
                                                                 const float* __restrict__ hidden,    // [M][H] post-ReLU
@@ -160,9 +208,8 @@ __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd_tma(const float* __
         for (int i = 0; i < TT_CHUNK / MT_WARPS; ++i) {
             const int rl = warp + i * MT_WARPS;
             if (rl < rows) {
-                const float4 d0 = *reinterpret_cast<const float4*>(cd + rl * NO);
-                const float4 d1 = *reinterpret_cast<const float4*>(cd + rl * NO + 4);
-                const float d[NO] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+                float d[NO];
+                tail_load_dout<NO>(cd + rl * NO, d);
                 const float4 h = *reinterpret_cast<const float4*>(ch + rl * H + 4 * lane);
                 float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
@@ -214,39 +261,63 @@ __global__ void __launch_bounds__(256) k_reduce_partials(const float* __restrict
     if (lane == 0) out[j] = s;
 }
 
+template <int NO>
+int launch_tail(const float* dout, int64_t dout_stride, const float* w_heads, const float* hidden, int64_t m, float* dpre,
+                float* workspace, int blocks, cudaStream_t s) {
+    const int pstride = NO * 128 + 128 + NO;
+    if (dout_stride == NO) {   // contiguous head gradients: TMA-staged pipeline
+        const size_t smem = (size_t)TT_STAGES * (TT_CHUNK * 128 * 4 + TT_CHUNK * NO * 4) + (size_t)MT_WARPS * pstride * 4;
+        PB_CUDA(cudaFuncSetAttribute(k_mlp_tail_bwd_tma<128, NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_mlp_tail_bwd_tma<128, NO><<<blocks, MT_THREADS, smem, s>>>(dout, w_heads, hidden, dpre, workspace, m);
+    } else {
+        k_mlp_tail_bwd<128, NO><<<blocks, MT_THREADS, 0, s>>>(dout, dout_stride, w_heads, hidden, dpre, workspace, m);
+    }
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
+
 }  // namespace
 
-extern "C" size_t pb_mlp_tail_workspace_bytes(int64_t m, int32_t hidden) {
-    if (m <= 0 || hidden <= 0) return 16;
+extern "C" size_t pb_mlp_tail_workspace_bytes_ex(int64_t m, int32_t hidden, int32_t head_rows) {
+    if (m <= 0 || hidden <= 0 || (head_rows != 8 && head_rows != 16)) return 16;
     const int64_t blocks = pb_ceil_div(m, ROWS_PER_BLOCK);
-    return (size_t)blocks * (size_t)(NO * hidden + hidden + NO) * sizeof(float);
+    return (size_t)blocks * (size_t)(head_rows * hidden + hidden + head_rows) * sizeof(float);
+}
+
+extern "C" size_t pb_mlp_tail_workspace_bytes(int64_t m, int32_t hidden) {
+    return pb_mlp_tail_workspace_bytes_ex(m, hidden, 8);
+}
+
+extern "C" int pb_mlp_tail_backward_ex(const float* dout, int64_t dout_stride, const float* w_heads, const float* hidden,
+                                       int64_t m, int32_t hidden_size, float* dpre, float* grads_out, void* workspace,
+                                       size_t workspace_bytes, int32_t head_rows, void* stream) {
+    PB_REQUIRE(m >= 1, PB_ERR_INVALID, "pb_mlp_tail_backward: m must be positive");
+    PB_REQUIRE(hidden_size == 128, PB_ERR_UNSUPPORTED, "pb_mlp_tail_backward: hidden size %d (only 128 is built)",
+               hidden_size);
+    PB_REQUIRE(head_rows == 8 || head_rows == 16, PB_ERR_UNSUPPORTED,
+               "pb_mlp_tail_backward: head_rows %d (8 and 16 are built)", head_rows);
+    PB_REQUIRE(dout && w_heads && hidden && dpre && grads_out && workspace, PB_ERR_INVALID,
+               "pb_mlp_tail_backward: null pointer");
+    PB_REQUIRE(dout_stride >= head_rows && dout_stride % 4 == 0 && ((uintptr_t)dout & 15) == 0 &&
+                   ((uintptr_t)hidden & 15) == 0 && ((uintptr_t)dpre & 15) == 0 && ((uintptr_t)w_heads & 15) == 0,
+               PB_ERR_INVALID, "pb_mlp_tail_backward: dout needs %d padded columns; pointers must be 16-byte aligned",
+               head_rows);
+    PB_REQUIRE(workspace_bytes >= pb_mlp_tail_workspace_bytes_ex(m, hidden_size, head_rows), PB_ERR_INVALID,
+               "pb_mlp_tail_backward: workspace too small");
+    const int blocks = (int)pb_ceil_div(m, ROWS_PER_BLOCK);
+    const int pstride = head_rows * hidden_size + hidden_size + head_rows;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int rc = head_rows == 8 ? launch_tail<8>(dout, dout_stride, w_heads, hidden, m, dpre, (float*)workspace, blocks, s)
+                                  : launch_tail<16>(dout, dout_stride, w_heads, hidden, m, dpre, (float*)workspace, blocks, s);
+    if (rc != PB_OK) return rc;
+    k_reduce_partials<<<(pstride * 32 + 255) / 256, 256, 0, s>>>((const float*)workspace, blocks, pstride, grads_out);
+    PB_LAUNCH_CHECK();
+    return PB_OK;
 }
 
 extern "C" int pb_mlp_tail_backward(const float* dout, int64_t dout_stride, const float* w_heads, const float* hidden,
                                     int64_t m, int32_t hidden_size, float* dpre, float* grads_out, void* workspace,
                                     size_t workspace_bytes, void* stream) {
-    PB_REQUIRE(m >= 1, PB_ERR_INVALID, "pb_mlp_tail_backward: m must be positive");
-    PB_REQUIRE(hidden_size == 128, PB_ERR_UNSUPPORTED, "pb_mlp_tail_backward: hidden size %d (only 128 is built)",
-               hidden_size);
-    PB_REQUIRE(dout && w_heads && hidden && dpre && grads_out && workspace, PB_ERR_INVALID,
-               "pb_mlp_tail_backward: null pointer");
-    PB_REQUIRE(dout_stride >= NO && dout_stride % 4 == 0 && ((uintptr_t)dout & 15) == 0 && ((uintptr_t)hidden & 15) == 0 &&
-                   ((uintptr_t)dpre & 15) == 0 && ((uintptr_t)w_heads & 15) == 0,
-               PB_ERR_INVALID, "pb_mlp_tail_backward: dout needs 8 padded columns; pointers must be 16-byte aligned");
-    PB_REQUIRE(workspace_bytes >= pb_mlp_tail_workspace_bytes(m, hidden_size), PB_ERR_INVALID,
-               "pb_mlp_tail_backward: workspace too small");
-    const int blocks = (int)pb_ceil_div(m, ROWS_PER_BLOCK);
-    const int pstride = NO * hidden_size + hidden_size + NO;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (dout_stride == NO) {   // contiguous head gradients: TMA-staged pipeline
-        const size_t smem = (size_t)TT_STAGES * (TT_CHUNK * 128 * 4 + TT_CHUNK * NO * 4) + (size_t)MT_WARPS * pstride * 4;
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_tail_bwd_tma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_mlp_tail_bwd_tma<128><<<blocks, MT_THREADS, smem, s>>>(dout, w_heads, hidden, dpre, (float*)workspace, m);
-    } else {
-        k_mlp_tail_bwd<128><<<blocks, MT_THREADS, 0, s>>>(dout, dout_stride, w_heads, hidden, dpre, (float*)workspace, m);
-    }
-    PB_LAUNCH_CHECK();
-    k_reduce_partials<<<(pstride * 32 + 255) / 256, 256, 0, s>>>((const float*)workspace, blocks, pstride, grads_out);
-    PB_LAUNCH_CHECK();
-    return PB_OK;
+    return pb_mlp_tail_backward_ex(dout, dout_stride, w_heads, hidden, m, hidden_size, dpre, grads_out, workspace,
+                                   workspace_bytes, 8, stream);
 }

@@ -9,9 +9,10 @@
 //     (cp.async.bulk, one per row, two mbarriers);
 //   * hidden = relu(X W^T + b) on the tensor cores (mma.sync m16n8k8 TF32, fp32 accumulate; a warp owns 16 rows x 128
 //     columns, accumulators stay in registers -- `hidden` is never written to memory);
-//   * the two heads (n_act logits + value, padded to 8 columns) are a second mma whose A operand is the accumulator
-//     fragment itself (the k order of the second product is permuted to match the C-fragment layout);
-//   * a quad shuffle gathers each row's 8 outputs, one lane per row does logsumexp / inverse-CDF sampling / logprob /
+//   * the two heads (n_act logits + value, padded to NC = 8 columns for n_act <= 7, 16 for n_act <= 15) are a second
+//     mma whose A operand is the accumulator fragment itself (the k order of the second product is permuted to match the
+//     C-fragment layout); NC = 16 is two n8 blocks on the same A fragments;
+//   * a quad shuffle gathers each row's NC outputs, one lane per row does logsumexp / inverse-CDF sampling / logprob /
 //     entropy and writes action, logprob, value straight into the rollout rows.
 // Tensor-core path note: this is a 128x128x128 tile per CTA, far below the size where a wgmma pipeline pays; the large
 // training GEMMs of the generic path stay on cuBLAS.
@@ -28,23 +29,25 @@ constexpr int PM_PITCH = PM_K + 8;  // shared row pitch in floats (544 B): confl
 struct PolicyParams {
     const float* obs; int64_t obs_stride;      // [M][128] fp32
     const float* w_enc; const float* b_enc;    // [128][128], [128]
-    const float* w_heads; const float* b_heads;  // [8][128], [8]  (n_act logits | value | zero pad)
+    const float* w_heads; const float* b_heads;  // [NC][128], [NC]  (n_act logits | value | zero pad)
     int64_t m; int n_act;
     uint64_t seed; uint64_t* counter; unsigned int* ticket;
     int64_t* actions; float* logprobs; float* values; float* entropies;   // [M] each (entropies may be null)
 };
 
-// 64 rows per CTA, one warp per 16 rows: 128 threads, 104 KB shared -> 2 CTAs per SM, 256 CTAs at 16384 rows
+// 64 rows per CTA, one warp per 16 rows: 128 threads, 104 KB shared (+ 4 KB more head rows at NC = 16) -> 2 CTAs per
+// SM, 256 CTAs at 16384 rows
 constexpr int PM_ROWS = 64;
 constexpr int PM_THREADS = 2 * PM_ROWS;
 
+template <int NC>
 __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p) {
     extern __shared__ __align__(128) float smem[];
     float* sX = smem;                              // [64][136]
     float* sW = smem + PM_ROWS * PM_PITCH;         // [128][136]  (row = hidden unit, col = input feature)
-    __shared__ float sWh[8][PM_H];
+    __shared__ float sWh[NC][PM_H];
     __shared__ float sBe[PM_H];
-    __shared__ float sBh[8];
+    __shared__ float sBh[NC];
     __shared__ __align__(8) uint64_t bars[2];      // [0]: obs tile + W rows 0..63, [1]: W rows 64..127
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
@@ -65,9 +68,9 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
 #pragma unroll 8
         for (int q = 0; q < PM_K / 4; ++q) *reinterpret_cast<float4*>(sX + tid * PM_PITCH + 4 * q) = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    for (int i = tid; i < 8 * PM_H; i += PM_THREADS) sWh[i >> 7][i & 127] = p.w_heads[i];
+    for (int i = tid; i < NC * PM_H; i += PM_THREADS) sWh[i >> 7][i & 127] = p.w_heads[i];
     if (tid < PM_H) sBe[tid] = p.b_enc[tid];
-    if (tid < 8) sBh[tid] = p.b_heads[tid];
+    if (tid < NC) sBh[tid] = p.b_heads[tid];
     __syncthreads();
     if (tid < valid) tma_load_1d(sX + tid * PM_PITCH, p.obs + (row0 + tid) * p.obs_stride, PM_K * 4u, &bars[0]);
     tma_load_1d(sW + tid * PM_PITCH, p.w_enc + (int64_t)tid * PM_K, PM_K * 4u, &bars[tid >> 6]);
@@ -98,8 +101,11 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
         }
     }
     // ---- bias + ReLU on the accumulators; heads = hidden @ Wh^T as a second mma with A = the C fragments:
-    //      C fragment of n-tile nt holds columns 8nt + {2t, 2t+1} of rows {g, g+8}; use them as k slots {t, t+4}
-    float out[4] = {0.f, 0.f, 0.f, 0.f};
+    //      C fragment of n-tile nt holds columns 8nt + {2t, 2t+1} of rows {g, g+8}; use them as k slots {t, t+4};
+    //      head block q8 (columns 8q8..8q8+7) takes B from head rows 8q8 + g
+    float out[NC / 8][4];
+#pragma unroll
+    for (int q8 = 0; q8 < NC / 8; ++q8) { out[q8][0] = out[q8][1] = out[q8][2] = out[q8][3] = 0.f; }
 #pragma unroll
     for (int nt = 0; nt < 16; ++nt) {
         const int c0 = 8 * nt + 2 * t;
@@ -109,28 +115,33 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
         a[1] = to_tf32(fmaxf(acc[nt][2] + b0, 0.f));      // (g+8, col c0)   -> k slot t
         a[2] = to_tf32(fmaxf(acc[nt][1] + b1, 0.f));      // (g,   col c0+1) -> k slot t+4
         a[3] = to_tf32(fmaxf(acc[nt][3] + b1, 0.f));      // (g+8, col c0+1) -> k slot t+4
-        mma_tf32(out, a, to_tf32(sWh[g][c0]), to_tf32(sWh[g][c0 + 1]));   // B[k slot][n = g]
-    }
-    // out: (row g, cols 2t, 2t+1), (row g+8, cols 2t, 2t+1).  Gather the 8 columns of a row across its quad.
-    float rowv[2][8];
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        const int src = (lane & ~3) | q;
-        const float v0 = __shfl_sync(0xffffffffu, out[0], src), v1 = __shfl_sync(0xffffffffu, out[1], src);
-        const float v2 = __shfl_sync(0xffffffffu, out[2], src), v3 = __shfl_sync(0xffffffffu, out[3], src);
-        rowv[0][2 * q] = v0 + sBh[2 * q]; rowv[0][2 * q + 1] = v1 + sBh[2 * q + 1];
-        rowv[1][2 * q] = v2 + sBh[2 * q]; rowv[1][2 * q + 1] = v3 + sBh[2 * q + 1];
+        for (int q8 = 0; q8 < NC / 8; ++q8)   // B[k slot][n = g]
+            mma_tf32(out[q8], a, to_tf32(sWh[8 * q8 + g][c0]), to_tf32(sWh[8 * q8 + g][c0 + 1]));
+    }
+    // out[q8]: (row g, cols 8q8 + 2t, +1), (row g+8, same).  Gather the NC columns of a row across its quad.
+    float rowv[2][NC];
+#pragma unroll
+    for (int q8 = 0; q8 < NC / 8; ++q8) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int src = (lane & ~3) | q, k = 8 * q8 + 2 * q;
+            const float v0 = __shfl_sync(0xffffffffu, out[q8][0], src), v1 = __shfl_sync(0xffffffffu, out[q8][1], src);
+            const float v2 = __shfl_sync(0xffffffffu, out[q8][2], src), v3 = __shfl_sync(0xffffffffu, out[q8][3], src);
+            rowv[0][k] = v0 + sBh[k]; rowv[0][k + 1] = v1 + sBh[k + 1];
+            rowv[1][k] = v2 + sBh[k]; rowv[1][k + 1] = v3 + sBh[k + 1];
+        }
     }
     // lane t == 0 finishes row g, lane t == 1 finishes row g + 8
     if (t < 2) {
         const int64_t r = row0 + 16 * warp + g + 8 * t;
         if (r < p.m) {
-            float z[8];
+            float z[NC];
 #pragma unroll
-            for (int k = 0; k < 8; ++k) z[k] = t ? rowv[1][k] : rowv[0][k];
+            for (int k = 0; k < NC; ++k) z[k] = t ? rowv[1][k] : rowv[0][k];
             int a;
             float lp, ent, value;
-            pb_sample_row<8>(z, p.n_act, pb_policy_uniform(p.seed, offset, r), a, lp, ent, value);
+            pb_sample_row<NC>(z, p.n_act, pb_policy_uniform(p.seed, offset, r), a, lp, ent, value);
             p.actions[r] = a;
             p.logprobs[r] = lp;
             p.values[r] = value;
@@ -152,6 +163,15 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
     }
 }
 
+template <int NC>
+int launch(const PolicyParams& p, cudaStream_t stream) {
+    const size_t smem = (size_t)(PM_ROWS + PM_H) * PM_PITCH * sizeof(float);
+    PB_CUDA(cudaFuncSetAttribute(k_policy_mlp_sample<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_policy_mlp_sample<NC><<<(unsigned)pb_ceil_div(p.m, PM_ROWS), PM_THREADS, smem, stream>>>(p);
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
+
 }  // namespace
 
 extern "C" int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const float* w_enc, const float* b_enc,
@@ -163,7 +183,7 @@ extern "C" int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const 
     PB_REQUIRE(in_features == PM_K && hidden_size == PM_H, PB_ERR_UNSUPPORTED,
                "pb_policy_mlp_sample: built for 128 input features and 128 hidden units (got %d, %d)", in_features,
                hidden_size);
-    PB_REQUIRE(n_act >= 1 && n_act <= 7, PB_ERR_UNSUPPORTED, "pb_policy_mlp_sample: n_act must be in [1, 7]");
+    PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "pb_policy_mlp_sample: n_act must be in [1, 15]");
     PB_REQUIRE(obs && w_enc && b_enc && w_heads && b_heads && actions && logprobs && values, PB_ERR_INVALID,
                "pb_policy_mlp_sample: null pointer");
     PB_REQUIRE(obs_stride >= PM_K && obs_stride % 4 == 0 && ((uintptr_t)obs & 15) == 0 && ((uintptr_t)w_enc & 15) == 0,
@@ -171,9 +191,6 @@ extern "C" int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const 
     PB_REQUIRE(!ticket_dev || counter_dev, PB_ERR_INVALID, "pb_policy_mlp_sample: ticket_dev needs counter_dev");
     PolicyParams p{obs, obs_stride, w_enc, b_enc, w_heads, b_heads, m, n_act, seed, counter_dev, ticket_dev,
                    actions, logprobs, values, entropies};
-    const size_t smem = (size_t)(PM_ROWS + PM_H) * PM_PITCH * sizeof(float);
-    PB_CUDA(cudaFuncSetAttribute(k_policy_mlp_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_policy_mlp_sample<<<(unsigned)pb_ceil_div(m, PM_ROWS), PM_THREADS, smem, (cudaStream_t)stream>>>(p);
-    PB_LAUNCH_CHECK();
-    return PB_OK;
+    // w_heads / b_heads: the head matrix of models.Default.head_matrix, 8 rows for n_act <= 7, else 16
+    return n_act + 1 <= 8 ? launch<8>(p, (cudaStream_t)stream) : launch<16>(p, (cudaStream_t)stream);
 }

@@ -13,7 +13,7 @@
 // value once, accumulates the 7 means (warp shuffle -> block -> one atomic per block and statistic, fp64) and writes
 // the ANALYTIC gradients dloss/dlogits and dloss/dvalue (already scaled by 1/M), which the host feeds to autograd
 // for the network backward.  Tie rules follow ATen (maximum: ties split the gradient; clamp: inclusive bounds).
-// HBM traffic per row: 4*A + 28 B read, 4*A + 4 B written.
+// HBM traffic per row: 4*A + 28 B read, 4*A + 4 B written (packed rows: 4*W + 24 B read, 4*W written).
 #include "pb_common.cuh"
 
 namespace {
@@ -38,21 +38,26 @@ struct PpoParams {
     int clip_vloss;
 };
 
-// PACKED: logits / value / grads all live in [m][8] rows (n_act logits | value | zero pad): 128-bit row accesses
-template <bool PACKED>
+// PW = 0: separate logits / value / gradient buffers, any strides.  PW = 8 or 16: logits / value / grads all live in
+// [m][PW] rows (n_act logits | value | zero pad): PW / 4 128-bit accesses per row, every row written whole
+template <int PW>
 __global__ void __launch_bounds__(PL_THREADS) k_ppo_loss(PpoParams p) {
+    constexpr bool PACKED = PW > 0;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     double s_pg = 0, s_v = 0, s_ent = 0, s_okl = 0, s_kl = 0, s_clip = 0;
     if (i < p.m) {
         float z[PL_MAX_ACT];
         float mx = -INFINITY;
         float v_packed = 0.f;
-        if (PACKED) {   // one 32-byte row: two 128-bit loads
-            const float4 a0 = *reinterpret_cast<const float4*>(p.logits + i * 8);
-            const float4 a1 = *reinterpret_cast<const float4*>(p.logits + i * 8 + 4);
-            const float row[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+        if (PACKED) {   // one PW * 4-byte row: PW / 4 128-bit loads
+            float row[PW ? PW : 4];
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
+            for (int q = 0; q < PW / 4; ++q) {
+                const float4 a = *reinterpret_cast<const float4*>(p.logits + i * PW + 4 * q);
+                row[4 * q] = a.x; row[4 * q + 1] = a.y; row[4 * q + 2] = a.z; row[4 * q + 3] = a.w;
+            }
+#pragma unroll
+            for (int k = 0; k < PW; ++k) {
                 z[k] = row[k];
                 if (k == p.n_act) v_packed = row[k];
             }
@@ -117,21 +122,25 @@ __global__ void __launch_bounds__(PL_THREADS) k_ppo_loss(PpoParams p) {
         if (!PACKED) p.grad_value[i * p.gvstride] = gv_out;
         // d loss / d logits_j = g_nlp * (delta_ja - p_j) + ent_coef/M * p_j * (nl_j + H)
         const float g_ent = p.ent_coef * inv_m;
-        float gro[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        float gro[PW ? PW : 4];
+#pragma unroll
+        for (int k = 0; k < PW; ++k) gro[k] = 0.f;
 #pragma unroll
         for (int k = 0; k < PL_MAX_ACT; ++k)
             if (k < p.n_act) {
                 const float pk = expf(z[k]);
                 const float gk = g_nlp * ((k == a ? 1.f : 0.f) - pk) + g_ent * pk * (z[k] + ent);
-                if (PACKED) { if (k < 8) gro[k] = gk; }
+                if (PACKED) { if (k < PW) gro[k] = gk; }
                 else p.grad_logits[i * p.glstride + k] = gk;
             }
-        if (PACKED) {   // the whole 8-column gradient row (zero padding included) in two 128-bit stores
+        if (PACKED) {   // the whole PW-column gradient row (zero padding included) in PW / 4 128-bit stores
 #pragma unroll
-            for (int k = 0; k < 8; ++k)
+            for (int k = 0; k < PW; ++k)
                 if (k == p.n_act) gro[k] = gv_out;
-            *reinterpret_cast<float4*>(p.grad_logits + i * 8) = make_float4(gro[0], gro[1], gro[2], gro[3]);
-            *reinterpret_cast<float4*>(p.grad_logits + i * 8 + 4) = make_float4(gro[4], gro[5], gro[6], gro[7]);
+#pragma unroll
+            for (int q = 0; q < PW / 4; ++q)
+                *reinterpret_cast<float4*>(p.grad_logits + i * PW + 4 * q) =
+                    make_float4(gro[4 * q], gro[4 * q + 1], gro[4 * q + 2], gro[4 * q + 3]);
         }
         s_pg = pg; s_v = vl; s_ent = ent; s_okl = -logratio; s_kl = (ratio - 1.f) - logratio;
         s_clip = fabsf(ratio - 1.f) > p.clip ? 1.0 : 0.0;
@@ -174,12 +183,17 @@ extern "C" int pb_ppo_loss(const float* logits, int64_t logits_stride, const flo
     PpoParams p{logits, logits_stride, value, value_stride, actions, old_logprobs, advantages, returns, old_values,
                 grad_logits, grad_logits_stride, grad_value, grad_value_stride, stats8, m, n_act, clip_coef, vf_clip_coef,
                 vf_coef, ent_coef, clip_vloss};
-    // packed rows: logits, value, and both gradients share [m][8] buffers (value = column n_act of the logits rows)
-    const bool packed = logits_stride == 8 && grad_logits_stride == 8 && n_act <= 7 && value == logits + n_act &&
-                        value_stride == 8 && grad_value == grad_logits + n_act && grad_value_stride == 8 &&
-                        ((uintptr_t)logits & 15) == 0 && ((uintptr_t)grad_logits & 15) == 0;
-    if (packed) k_ppo_loss<true><<<(unsigned)pb_ceil_div(m, PL_THREADS), PL_THREADS, 0, s>>>(p);
-    else k_ppo_loss<false><<<(unsigned)pb_ceil_div(m, PL_THREADS), PL_THREADS, 0, s>>>(p);
+    // packed rows: logits, value, and both gradients share [m][W] buffers, W = 8 (n_act <= 7) or 16 (n_act <= 15), with
+    // the value at column n_act of the logits rows
+    auto packed = [&](int w) {
+        return logits_stride == w && grad_logits_stride == w && n_act <= w - 1 && value == logits + n_act &&
+               value_stride == w && grad_value == grad_logits + n_act && grad_value_stride == w &&
+               ((uintptr_t)logits & 15) == 0 && ((uintptr_t)grad_logits & 15) == 0;
+    };
+    const unsigned grid = (unsigned)pb_ceil_div(m, PL_THREADS);
+    if (packed(8)) k_ppo_loss<8><<<grid, PL_THREADS, 0, s>>>(p);
+    else if (packed(16)) k_ppo_loss<16><<<grid, PL_THREADS, 0, s>>>(p);
+    else k_ppo_loss<0><<<grid, PL_THREADS, 0, s>>>(p);
     PB_LAUNCH_CHECK();
     return PB_OK;
 }

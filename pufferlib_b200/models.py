@@ -15,9 +15,11 @@ class _DefaultMLPFunction(torch.autograd.Function):
     """models.Default as one autograd node on the device fast path.
 
     forward : hidden = relu(x @ W_enc^T + b_enc)  -- bias + ReLU fused into the cuBLASLt GEMM epilogue;
-              out    = hidden @ W_cat^T + b_cat    -- both heads in ONE 8-column GEMM (n_act logits, value, zero pad).
-    backward: pb_mlp_tail_backward reads `hidden` once and produces dPre (heads dX + ReLU backward), dW_heads, db_heads
-              and db_enc; the dense dW_enc = dPre^T @ x stays on cuBLAS tensor cores.  x (the observations) has no grad.
+              out    = hidden @ W_cat^T + b_cat    -- both heads in ONE R-column GEMM (n_act logits, value, zero pad;
+                                                      R = 8 for n_act <= 7, 16 for n_act <= 15: Default.head_matrix).
+    backward: pb_mlp_tail_backward_ex reads `hidden` once and produces dPre (heads dX + ReLU backward), dW_heads,
+              db_heads and db_enc; the dense dW_enc = dPre^T @ x stays on cuBLAS tensor cores.  x (the observations) has
+              no grad.
     """
 
     @staticmethod
@@ -48,18 +50,18 @@ class _DefaultMLPFunction(torch.autograd.Function):
     def backward(ctx, dout):
         from pufferlib_b200 import _native
         x, hidden, w_cat = ctx.saved_tensors
-        n_act, (m, hid) = ctx.n_act, hidden.shape
+        n_act, (m, hid), rows = ctx.n_act, hidden.shape, w_cat.shape[0]
         dout = dout.contiguous()
         dpre = torch.empty_like(hidden)
-        grads = torch.empty(8 * hid + hid + 8, dtype=torch.float32, device=x.device)
+        grads = torch.empty(rows * hid + hid + rows, dtype=torch.float32, device=x.device)
         lib = _native.lib()
-        ws = torch.empty(lib.pb_mlp_tail_workspace_bytes(m, hid), dtype=torch.uint8, device=x.device)
-        _native.check(lib.pb_mlp_tail_backward(_native.ptr(dout), dout.stride(0), _native.ptr(w_cat), _native.ptr(hidden),
-                                               m, hid, _native.ptr(dpre), _native.ptr(grads), _native.ptr(ws),
-                                               ws.numel(), _native.stream_ptr()))
-        dw_cat = grads[:8 * hid].view(8, hid)
-        db_enc = grads[8 * hid:9 * hid]
-        db_cat = grads[9 * hid:]
+        ws = torch.empty(lib.pb_mlp_tail_workspace_bytes_ex(m, hid, rows), dtype=torch.uint8, device=x.device)
+        _native.check(lib.pb_mlp_tail_backward_ex(_native.ptr(dout), dout.stride(0), _native.ptr(w_cat),
+                                                  _native.ptr(hidden), m, hid, _native.ptr(dpre), _native.ptr(grads),
+                                                  _native.ptr(ws), ws.numel(), rows, _native.stream_ptr()))
+        dw_cat = grads[:rows * hid].view(rows, hid)
+        db_enc = grads[rows * hid:(rows + 1) * hid]
+        db_cat = grads[(rows + 1) * hid:]
         # dW_enc = dPre^T @ x is one 128x128 output tile with K = M: as a batched GEMM over 64 K-slices (+ a 64-way sum)
         # gives the library GEMM enough parallel work at this shape (slab form: K-slices per slab)
         dw_enc = _gemm_tn(dpre, x)
@@ -185,7 +187,7 @@ class Default(nn.Module):
         self.encoder = nn.Linear(int(np.prod(env.single_observation_space.shape)), hidden_size)
         self.decoder = layer_init(nn.Linear(hidden_size, env.single_action_space.n), std=0.01)
         self.value_head = nn.Linear(hidden_size, 1)
-        self.fast_path = True     # fused forward epilogues + pb_mlp_tail_backward (CUDA, hidden 128, <= 7 actions)
+        self.fast_path = True     # fused forward epilogues + pb_mlp_tail_backward (CUDA, hidden 128, <= 15 actions)
         self._head_cache = {}
 
     def invalidate_cache(self):
@@ -195,7 +197,7 @@ class Default(nn.Module):
 
     def head_matrix(self, cache=None):
         """(w_cat [R, H], b_cat [R]): n_act logit rows | value row | zero padding up to R = the next multiple of 8 rows
-        (8 for n_act <= 7).  Cached until invalidate_cache() when `cache` is true (default: under no_grad); built anew
+        (8 for n_act <= 7, 16 for n_act <= 15).  Cached until invalidate_cache() when `cache` is true (default: under no_grad); built anew
         otherwise, since fused optimizers do not bump tensor._version and the cache cannot see an optimizer step."""
         if cache is None:
             cache = not torch.is_grad_enabled()
@@ -229,11 +231,12 @@ class Default(nn.Module):
 
     def _fast_ok(self, x):
         n_act, hid = self.decoder.weight.shape
-        return self.fast_path and x.is_cuda and hid == 128 and n_act + 1 <= 8 and not x.requires_grad
+        return self.fast_path and x.is_cuda and hid == 128 and n_act + 1 <= 16 and not x.requires_grad
 
     def forward_packed(self, observations):
-        """-> (out [M, 8], n_act) with logits = out[:, :n_act], value = out[:, n_act] (zero padding after), or None
-        when the fast path does not apply.  Lets the fused PPO loss hand back ONE [M, 8] gradient."""
+        """-> (out [M, R], n_act) with logits = out[:, :n_act], value = out[:, n_act] (zero padding after; R = 8 for
+        n_act <= 7, 16 for n_act <= 15), or None when the fast path does not apply.  Lets the fused PPO loss hand back
+        ONE [M, R] gradient."""
         x = observations.view(observations.shape[0], -1)
         if not self._fast_ok(x):
             return None

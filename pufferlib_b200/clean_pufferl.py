@@ -207,8 +207,8 @@ class _DefaultMLPUpdate:
         analytic dLoss/dOut) -> pb_mlp_tail_backward_ex (dPre, dW_heads, db_heads, db_enc) -> split-K dW_enc GEMM + sum
         [-> gradient all-reduce over ONE flat buffer when world_size > 1] -> pb_clip_adam -> pb_pack_heads,
     with R = 8 head rows for n_act <= 7 and 16 for 8 <= n_act <= 15 (models.Default.head_matrix).
-    train() passes each minibatch as Experience.minibatch() to forward_backward; where _fused_ok holds (minibatch_form
-    asks it too; <= 7 actions) the chain is ONE kernel, pb_mlp_update_fused.
+    train() passes each minibatch as Experience.minibatch() to forward_backward; where _fused_ok holds (update_plan asks
+    it once per train() and sets used_fused; <= 7 actions) the chain is ONE kernel, pb_mlp_update_fused.
     Same math as the autograd path (tests/test_gpu_experience.py::test_manual_update_matches_autograd_update); the
     optimizer's own state tensors are updated in place, so state_dict() and optimizer.step() keep working."""
 
@@ -221,11 +221,6 @@ class _DefaultMLPUpdate:
             return False
         if config.target_kl is not None or not getattr(data, 'own_optimizer', False):
             return False
-        if not bool(getattr(config, 'manual_update_multi_gpu', True)):
-            world = torch.distributed.get_world_size() if (torch.distributed.is_available() and
-                                                            torch.distributed.is_initialized()) else 1
-            if world > 1:
-                return False      # opt-out: ranks > 1 on the autograd + GradBucket (NCCL) path
         n_act, hid = model.decoder.weight.shape
         if hid != 128 or n_act > 15 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
             return False
@@ -268,6 +263,7 @@ class _DefaultMLPUpdate:
                                                  st['step'].data_ptr(), g.data_ptr(), p.numel())
         self._keep = (params, grads)
         self._state_ptrs = self._current_state_ptrs()
+        # used_fused: this train() runs pb_mlp_update_fused rather than the kernel chain (set by update_plan)
         self.fused_ws, self.used_fused, self.fused_dpre, self.part = None, False, None, None
         self.rows = 0
         self.stats = None
@@ -347,9 +343,8 @@ class _DefaultMLPUpdate:
         if self.stats is None or self.stats.shape[0] != n_stats:
             self.stats = torch.zeros(n_stats, 8, dtype=torch.float64, device=self.gflat.device)
         atn, log_probs, adv, ret, val = mb.actions, mb.logprobs, mb.advantages, mb.returns, mb.values
-        fused = self._fused_ok(x, config)
-        assert mb.row_slab_stride is None or fused
-        if fused:
+        assert mb.row_slab_stride is None or self.used_fused
+        if self.used_fused:
             # ONE wgmma kernel: x read once, hidden / dPre stay on the SM, gradients land in self.gflat
             g_, r_, _ = x.shape
             lib = _native.lib()
@@ -376,7 +371,6 @@ class _DefaultMLPUpdate:
                 None, None, None, _native.stream_ptr()))
             if not in_kernel:
                 self._dw_enc(self.fused_dpre, x)
-            self.used_fused = True
             return
         x = x.float()
         g_, r_, f_ = x.shape
@@ -415,7 +409,7 @@ class _DefaultMLPUpdate:
         hyper = (C.c_float(float(config.max_grad_norm)), C.c_float(1.0 / self.world),
                  C.c_float(0.0 if lr_dev is not None else float(lr)), lr_dev, C.c_float(b1), C.c_float(b2), C.c_float(g['eps']), None)
         in_kernel = str(getattr(config, 'fused_update_dw', FUSED_UPDATE_DW_DEFAULT)) == 'kernel'
-        if self.used_fused and in_kernel and (self.world == 1 or self.peer is not None) and bool(getattr(config, 'adam_parts', True)):
+        if self.used_fused and in_kernel and (self.world == 1 or self.peer is not None):
             # the fused update's reduce step left the gradient's sum of squares as partial sums: multi-CTA clip + Adam without a
             # norm pass; several ranks: sliced peer all-reduce first, which leaves its own partial sums of squares
             m = self.model
@@ -838,9 +832,10 @@ def create(config, vecenv, policy, optimizer=None, wandb=None):
         io=pufferlib_b200.namespace(h2d=0, d2h=0), graph_state=0, rollout_graph=None, graph_steps=0,
         graph_launches=0, graph_replays=0, train_graph_state=0, train_graph=None, train_result=None, train_graph_launches=0, train_graph_replays=0, train_segments=None, train_acc=None, own_optimizer=own_optimizer, manual_update=None, train_minibatch_path=None, train_recurrent_path=None,
         fused_rows=bool(getattr(policy, 'fused_sample', False)) and hasattr(vecenv, 'bind_rollout'),
-        # one-kernel PPO loss (pb_ppo_loss): needs a wrapper exposing .policy(obs) -> (logits, value), one Discrete head
+        # one-kernel PPO loss (pb_ppo_loss) where the update engine has one (update_plan): needs a wrapper exposing the
+        # model as .policy, one Discrete head
         fused_loss=bool(getattr(config, 'fused_loss', True)) and hasattr(policy, 'policy')
-        and not hasattr(policy, 'lstm') and len(tuple(vecenv.single_action_space.shape)) == 0,
+        and len(tuple(vecenv.single_action_space.shape)) == 0,
     )
 
 
@@ -944,34 +939,76 @@ def _rollout_loop(data, infos):
         vecenv.join()            # pool mode: side-stream env steps rejoin the caller's stream (and any graph capture)
 
 
-def _recurrent_update_fused(data):
-    """Does train() run the recurrent update on the fused BPTT kernels (LSTMWrapper.forward_packed_seq)?  Decided on the
-    host from what forward_packed_seq checks, so that it is known before any capture: RecurrentPolicy(fused_update=True),
-    config.fused_loss, a model the kernels cover (fused_supported on the rollout observations) and the inner Default's
-    fast_path."""
-    experience, model = data.experience, getattr(data.policy, 'policy', None)
-    return (experience.lstm_h is not None and bool(getattr(data.policy, 'fused_update', False))
-            and bool(getattr(data.config, 'fused_loss', True)) and hasattr(model, 'forward_packed_seq')
-            and model.fused_supported(experience.obs) and bool(getattr(model.policy, 'fast_path', False)))
-
-
-def minibatch_form(data, manual):
-    """The minibatch form of this train(), from the shapes, the config and what the update engine accepts (manual: the
-    _DefaultMLPUpdate, or None): 'direct' (manual's fused kernel reads the arrival-order rollout tensors in place),
-    'slabs' (order-free fused loss: per-row tensors copied slab-major, obs a view), 'segments' (the fused recurrent
-    update on bptt segment views of obs) or 'gathered' (the reference layout: b_obs and the b_* tensors)."""
-    config, exp = data.config, data.experience
+def update_plan(data):
+    """How this train() runs, decided on the host after sort_training_data and before anything is launched or captured.
+    Returns namespace(engine, form, capture, manual).  engine, what runs one minibatch's forward, loss and backward:
+        'mlp_fused'  _DefaultMLPUpdate on pb_mlp_update_fused (one kernel per minibatch)
+        'mlp_chain'  _DefaultMLPUpdate's hand-written kernel chain
+        'packed'     autograd through Default.forward_packed(_slabs) + fused_ppo_loss_packed
+        'model'      autograd through model(obs) + fused_ppo_loss (Convolutional; Default with fast_path=False)
+        'bptt'       LSTMWrapper.forward_packed_seq (the fused BPTT kernels) + fused_ppo_loss_packed
+        'cudnn'      the policy's recurrent forward (cuDNN LSTM) + the reference loss
+        'reference'  the policy's forward + the reference loss (fused_loss=False)
+    form, the layout Experience.prepare builds: 'direct' (the fused kernel reads the arrival-order rollout tensors in
+    place), 'slabs' (order-free loss: per-row tensors copied slab-major, obs a view), 'segments' (the BPTT kernels on bptt
+    segment views of obs) or 'gathered' (the reference layout: b_obs and the b_* tensors).  capture: 'whole' (ONE graph),
+    'segments' (per-segment graphs around an NCCL all-reduce, _SegmentGraphs) or None (eager).  manual: this call's
+    _DefaultMLPUpdate (built here, and rebuilt when optimizer.load_state_dict() replaced the Adam state it holds), or None.
+    Sets data.manual_update, train_minibatch_path, train_recurrent_path and manual.used_fused."""
+    config, exp, model = data.config, data.experience, getattr(data.policy, 'policy', None)
+    if data.manual_update is not None and data.manual_update.stale():
+        # the hand-written update and any captured graph hold the old addresses: rebuild both (eager call now, capture
+        # again on the next one)
+        if data.manual_update.peer is not None:
+            data.manual_update.peer.close()          # collective: every rank loaded the same checkpoint
+        data.manual_update = None
+        if data.train_graph_state > 0:
+            data.train_graph, data.train_segments, data.train_graph_state = None, None, 0
+    manual = None
+    if _DefaultMLPUpdate.eligible(data):
+        if data.manual_update is None:
+            data.manual_update = _DefaultMLPUpdate(data)
+        manual = data.manual_update
     n, h, nm = exp.num_envs, exp.horizon, exp.num_minibatches
-    if not bool(getattr(config, 'zero_copy_minibatches', True)) or slab_layout(n, h, nm, exp.bptt_horizon) is None:
-        return 'gathered'
+    zero_copy = bool(getattr(config, 'zero_copy_minibatches', True)) and \
+        slab_layout(n, h, nm, exp.bptt_horizon) is not None
     if exp.lstm_h is not None:
-        return 'segments' if _recurrent_update_fused(data) else 'gathered'
-    if not (data.fused_loss and hasattr(getattr(data.policy, 'policy', None), 'forward_packed_slabs')):
-        return 'gathered'
-    if manual is not None and _native.lib().pb_gae_time_major_supported(n, h) and \
-            manual._fused_ok(exp.slab_obs(0).flatten(2), config):
-        return 'direct'
-    return 'slabs'
+        bptt = (data.fused_loss and bool(getattr(data.policy, 'fused_update', False))
+                and hasattr(model, 'forward_packed_seq') and model.fused_supported(exp.obs)
+                and bool(getattr(model.policy, 'fast_path', False)))
+        engine, form = ('bptt', 'segments' if zero_copy else 'gathered') if bptt else ('cudnn', 'gathered')
+    elif manual is not None:
+        # every minibatch of a form is this view shifted by whole minibatches of rows, and the observations _fused_ok
+        # accepts have 512-byte rows (128 fp32 features): minibatch 0 answers for all of them
+        x = exp.slab_obs(0).flatten(2) if zero_copy else exp.b_obs[0].reshape(1, exp.minibatch_size, -1)
+        engine = 'mlp_fused' if manual._fused_ok(x, config) else 'mlp_chain'
+        form = 'gathered' if not zero_copy else \
+            'direct' if engine == 'mlp_fused' and _native.lib().pb_gae_time_major_supported(n, h) else 'slabs'
+    elif data.fused_loss:
+        default = hasattr(model, 'forward_packed_slabs')
+        engine = 'packed' if default and model._fast_ok(exp.obs) else 'model'
+        form = 'slabs' if zero_copy and default else 'gathered'
+    else:
+        engine, form = 'reference', 'gathered'
+
+    capture = None
+    if bool(getattr(config, 'cuda_graph_train', getattr(config, 'cuda_graph', False))) and config.target_kl is None \
+            and data.train_graph_state >= 0:
+        # an NCCL call inside the update loop (autograd path on several ranks, or the hand-written update without peer
+        # memory) keeps the update out of ONE graph -- capturing it hung on this stack (torch 2.11 / NCCL 2.28) -- so it
+        # is captured in segments around an ordinary all-reduce call; with the peer all-reduce fused into
+        # pb_clip_adam_peer there is none
+        nccl_call = data.grad_bucket is not None and (manual is None or manual.peer is None)
+        if exp.lstm_h is None:
+            capture = 'segments' if nccl_call else 'whole'
+        elif engine == 'bptt' and data.grad_bucket is None:
+            capture = 'whole'           # the cuDNN path and recurrent updates on several ranks stay eager
+
+    data.train_minibatch_path = form
+    data.train_recurrent_path = {'bptt': 'fused', 'cudnn': 'cudnn'}.get(engine)
+    if manual is not None:
+        manual.used_fused = engine == 'mlp_fused'
+    return pufferlib_b200.namespace(engine=engine, form=form, capture=capture, manual=manual)
 
 
 def _invalidate_policy_cache(data):
@@ -1074,27 +1111,47 @@ class _SegmentGraphs:
         self.replayed_launches = getattr(self, 'replayed_launches', 0) + self.launches[key]
 
 
-def _train_device_part(data, seg=None):
+def _ppo_loss(newlogprob, entropy, newvalue, log_probs, adv, ret, val, config):
+    """clean_pufferl.py:202-238 in torch ops -> (loss, stats) like fused_ppo_loss."""
+    logratio = newlogprob - log_probs.reshape(-1)
+    ratio = logratio.exp()
+    with torch.no_grad():
+        old_approx_kl = (-logratio).mean()
+        approx_kl = ((ratio - 1) - logratio).mean()
+        clipfrac = ((ratio - 1.0).abs() > config.clip_coef).float().mean()
+
+    adv = adv.reshape(-1)
+    pg_loss1 = -adv * ratio
+    pg_loss2 = -adv * torch.clamp(ratio, 1 - config.clip_coef, 1 + config.clip_coef)
+    pg_loss = torch.max(pg_loss1, pg_loss2).mean()
+
+    newvalue = newvalue.view(-1)
+    if config.clip_vloss:
+        v_loss_unclipped = (newvalue - ret) ** 2
+        v_clipped = val + torch.clamp(newvalue - val, -config.vf_clip_coef, config.vf_clip_coef)
+        v_loss_clipped = (v_clipped - ret) ** 2
+        v_loss = 0.5 * torch.max(v_loss_unclipped, v_loss_clipped).mean()
+    else:
+        v_loss = 0.5 * ((newvalue - ret) ** 2).mean()
+
+    entropy_loss = entropy.mean()
+    loss = pg_loss - config.ent_coef * entropy_loss + v_loss * config.vf_coef
+    with torch.no_grad():
+        stats = torch.stack([pg_loss, v_loss, entropy_loss, old_approx_kl, approx_kl, clipfrac])
+    return loss, stats
+
+
+def _train_device_part(data, plan, seg=None):
     """Everything of train() that runs on the device without touching the host: GAE, minibatch construction, the
-    update_epochs x num_minibatches optimizer steps, the loss statistics.  No synchronisation inside, so the whole
-    thing can be captured in ONE CUDA graph (single GPU, see train) or, with ``seg``, as per-segment graphs around
-    the gradient all-reduce (multi-GPU)."""
+    update_epochs x num_minibatches optimizer steps, the loss statistics, the way `plan` (update_plan) says.  No
+    synchronisation inside, so the whole thing can be captured in ONE CUDA graph (single GPU, see train) or, with
+    ``seg``, as per-segment graphs around the gradient all-reduce (multi-GPU)."""
     config, profile, experience = data.config, data.profile, data.experience
     device = experience.device
     _invalidate_policy_cache(data)     # nothing cached by the rollout (eager or captured) may leak into an update graph
-
-    # recurrent models: the fused BPTT update when the policy asks for it and the model is covered (RecurrentPolicy(
-    # fused_update=True); data.train_recurrent_path records which path ran)
-    rec_fused = _recurrent_update_fused(data)
-    manual = None
-    if _DefaultMLPUpdate.eligible(data):
-        if getattr(data, 'manual_update', None) is None or data.manual_update.stale():
-            data.manual_update = _DefaultMLPUpdate(data)
-        manual = data.manual_update
+    manual, engine, model = plan.manual, plan.engine, getattr(data.policy, 'policy', None)
     with profile.train_misc:
-        experience.sort_training_data()
-        data.train_minibatch_path = minibatch_form(data, manual)
-        experience.prepare(data.train_minibatch_path, config)
+        experience.prepare(plan.form, config)
 
     n_mb = experience.num_minibatches
     if seg is not None:                        # persistent accumulator: the segment graphs update it in place
@@ -1105,7 +1162,6 @@ def _train_device_part(data, seg=None):
     else:
         acc = torch.zeros(6, device=device)    # policy, value, entropy, old_kl, kl, clipfrac
     obs_shape = data.vecenv.single_observation_space.shape
-    fused = data.fused_loss and experience.lstm_h is None
     carry = {'lstm_state': None, 'approx_kl': None}
     if manual is not None:
         manual.pack_heads()                      # the parameters may have changed since the last train() (checkpoints)
@@ -1120,58 +1176,33 @@ def _train_device_part(data, seg=None):
         obs, atn, log_probs, val, adv, ret = b.obs, b.actions, b.logprobs, b.values, b.advantages, b.returns
 
         with profile.train_forward:
-            packed = None
-            if fused:          # logits / value straight from the model; loss + its gradient in one kernel
-                model = data.policy.policy
-                if b.slab_form:
+            if engine in ('packed', 'bptt'):     # the model's own kernels; the loss hands back ONE [M, R] gradient
+                if engine == 'bptt':             # clean_pufferl.py:188-191: [rows, bptt, *obs] segments
+                    packed = model.forward_packed_seq(obs, carry['lstm_state'])
+                elif b.slab_form:
                     packed = model.forward_packed_slabs(obs)
-                elif hasattr(model, 'forward_packed'):
+                else:
                     packed = model.forward_packed(obs.reshape(-1, *obs_shape))
                 if packed is None:
-                    logits, newvalue = model(obs.reshape(-1, *obs_shape))
-            elif experience.lstm_h is not None:       # clean_pufferl.py:188-191: [rows, bptt, *obs] segments
-                if rec_fused:
-                    packed = data.policy.policy.forward_packed_seq(obs, carry['lstm_state'])
-                if packed is not None:     # BPTT kernels; the loss hands back ONE [B*T, R] gradient
-                    st_ = packed[2]
-                else:
-                    _, newlogprob, entropy, newvalue, st_ = data.policy(obs, state=carry['lstm_state'], action=atn)
-                data.train_recurrent_path = 'cudnn' if packed is None else 'fused'
+                    raise RuntimeError(f'the {engine} engine refused minibatch {mb} of form {plan.form}: update_plan '
+                                       'and the model disagree on what its kernels cover')
+                if engine == 'bptt':
+                    carry['lstm_state'] = (packed[2][0].detach(), packed[2][1].detach())
+            elif engine == 'model':
+                logits, newvalue = model(obs.reshape(-1, *obs_shape))
+            elif engine == 'cudnn':
+                _, newlogprob, entropy, newvalue, st_ = data.policy(obs, state=carry['lstm_state'], action=atn)
                 carry['lstm_state'] = (st_[0].detach(), st_[1].detach())
             else:
                 _, newlogprob, entropy, newvalue = data.policy(obs.reshape(-1, *obs_shape), action=atn)
 
         with profile.train_misc:
-            if fused or packed is not None:
-                if packed is not None:
-                    loss, st = fused_ppo_loss_packed(packed[0], packed[1], atn, log_probs, adv, ret, val, config)
-                else:
-                    loss, st = fused_ppo_loss(logits, newvalue, atn, log_probs, adv, ret, val, config)
-                pg_loss, v_loss, entropy_loss, old_approx_kl, approx_kl, clipfrac = st.unbind(0)
+            if engine in ('packed', 'bptt'):
+                loss, st = fused_ppo_loss_packed(packed[0], packed[1], atn, log_probs, adv, ret, val, config)
+            elif engine == 'model':
+                loss, st = fused_ppo_loss(logits, newvalue, atn, log_probs, adv, ret, val, config)
             else:
-                logratio = newlogprob - log_probs.reshape(-1)
-                ratio = logratio.exp()
-                with torch.no_grad():
-                    old_approx_kl = (-logratio).mean()
-                    approx_kl = ((ratio - 1) - logratio).mean()
-                    clipfrac = ((ratio - 1.0).abs() > config.clip_coef).float().mean()
-
-                adv = adv.reshape(-1)
-                pg_loss1 = -adv * ratio
-                pg_loss2 = -adv * torch.clamp(ratio, 1 - config.clip_coef, 1 + config.clip_coef)
-                pg_loss = torch.max(pg_loss1, pg_loss2).mean()
-
-                newvalue = newvalue.view(-1)
-                if config.clip_vloss:
-                    v_loss_unclipped = (newvalue - ret) ** 2
-                    v_clipped = val + torch.clamp(newvalue - val, -config.vf_clip_coef, config.vf_clip_coef)
-                    v_loss_clipped = (v_clipped - ret) ** 2
-                    v_loss = 0.5 * torch.max(v_loss_unclipped, v_loss_clipped).mean()
-                else:
-                    v_loss = 0.5 * ((newvalue - ret) ** 2).mean()
-
-                entropy_loss = entropy.mean()
-                loss = pg_loss - config.ent_coef * entropy_loss + v_loss * config.vf_coef
+                loss, st = _ppo_loss(newlogprob, entropy, newvalue, log_probs, adv, ret, val, config)
 
         with profile.learn:
             if data.grad_bucket is not None:
@@ -1181,9 +1212,8 @@ def _train_device_part(data, seg=None):
             loss.backward()
 
         with profile.train_misc, torch.no_grad():
-            acc.add_(torch.stack([pg_loss.detach(), v_loss.detach(), entropy_loss.detach(), old_approx_kl,
-                                  approx_kl, clipfrac]) / n_mb)
-        carry['approx_kl'] = approx_kl
+            acc.add_(st / n_mb)
+        carry['approx_kl'] = st[4]
 
     def optimizer_step():
         with profile.learn:
@@ -1234,35 +1264,16 @@ def train(data):
     config, profile, experience = data.config, data.profile, data.experience
     data.losses = make_losses()
     losses = data.losses
-    if getattr(data, 'manual_update', None) is not None and data.manual_update.stale():
-        # optimizer.load_state_dict() (try_load_checkpoint) replaced the Adam state tensors: the hand-written update
-        # and any captured graph hold the old addresses -- rebuild both (eager call now, re-capture on the next one)
-        if getattr(data.manual_update, 'peer', None) is not None:
-            data.manual_update.peer.close()          # collective: every rank loaded the same checkpoint
-        data.manual_update = None
-        if data.train_graph_state > 0:
-            data.train_graph, data.train_segments, data.train_graph_state = None, None, 0
-    # multi-GPU: capturing the NCCL all-reduce inside one big graph hung on this stack (torch 2.11 / NCCL 2.28); ranks > 1
-    # use per-segment graphs around an ordinary all-reduce call instead (see `segmented`)
-    want_graph = bool(getattr(config, 'cuda_graph_train', getattr(config, 'cuda_graph', False)))
-    # an NCCL call inside the update loop (autograd path on several ranks, or the hand-written update without peer
-    # memory) keeps the update out of ONE graph; with the peer all-reduce fused into pb_clip_adam_peer there is none
-    mu = getattr(data, 'manual_update', None)
-    nccl_in_loop = data.grad_bucket is not None and not (mu is not None and (mu.world == 1 or mu.peer is not None))
-    # a recurrent update is captured only on the fused BPTT kernels (decided on the host, before any capture) and without
-    # a gradient all-reduce; the cuDNN path stays eager
-    rec_graphable = experience.lstm_h is not None and data.grad_bucket is None and _recurrent_update_fused(data)
-    graphable = want_graph and not nccl_in_loop and \
-        config.target_kl is None and (experience.lstm_h is None or rec_graphable) and data.train_graph_state >= 0
-    segmented = want_graph and nccl_in_loop and \
-        config.target_kl is None and experience.lstm_h is None and data.train_graph_state >= 0
-    if segmented and data.train_graph_state >= 1:
+    with profile.train_misc:
+        experience.sort_training_data()        # host-side bookkeeping only (clean_pufferl.py:452-464)
+        plan = update_plan(data)
+    if plan.capture == 'segments' and data.train_graph_state >= 1:
         if data.train_segments is None:
             data.train_segments = _SegmentGraphs()
-        result = _train_device_part(data, seg=data.train_segments)
-    elif not graphable or data.train_graph_state == 0:
-        result = _train_device_part(data)
-        if graphable or segmented:
+        result = _train_device_part(data, plan, seg=data.train_segments)
+    elif plan.capture is None or data.train_graph_state == 0:
+        result = _train_device_part(data, plan)
+        if plan.capture is not None:
             data.train_graph_state = 1
     else:
         if data.train_graph_state == 1:
@@ -1270,32 +1281,20 @@ def train(data):
                 torch.cuda.synchronize()
                 launches0 = _native.lib().pb_launch_count()
                 graph = torch.cuda.CUDAGraph()
-                data.train_recurrent_path = None
                 with torch.cuda.graph(graph):
-                    data.train_result = _train_device_part(data)
-                if experience.lstm_h is not None and data.train_recurrent_path != 'fused':
-                    # the captured recurrent update did not run on the BPTT kernels: keep it eager (capture ran nothing)
-                    del graph
-                    data.train_result, data.train_graph_state = None, -1
-                    data.msg = (f'train graph dropped: the recurrent update took the {data.train_recurrent_path} path; '
-                                'running eager')
-                    torch.cuda.synchronize()
-                    result = _train_device_part(data)
-                else:
-                    data.train_graph = graph
-                    data.train_graph_launches = _native.lib().pb_launch_count() - launches0
-                    data.train_graph_state = 2
+                    data.train_result = _train_device_part(data, plan)
+                data.train_graph = graph
+                data.train_graph_launches = _native.lib().pb_launch_count() - launches0
+                data.train_graph_state = 2
             except Exception as e:          # capture is an optimisation: fall back to eager for good
                 data.train_graph_state = -1
                 data.msg = f'train graph capture failed ({type(e).__name__}: {e}); running eager'
                 torch.cuda.synchronize()
-                result = _train_device_part(data)
+                result = _train_device_part(data, plan)
         if data.train_graph_state == 2:
             with profile.learn:
                 data.train_graph.replay()
             data.train_graph_replays += 1
-            experience.ptr = 0            # what sort_training_data leaves behind (clean_pufferl.py:461-463)
-            experience.step = 0
             result = data.train_result
 
     _invalidate_policy_cache(data)          # graph replays update the parameters without running python hooks

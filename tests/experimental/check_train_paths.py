@@ -51,6 +51,10 @@ CASES = {
     'lstm_gathered': ('breakout', 256, 64, 'lstm', {}, dict(minibatch_size=256 * 64 // 2, zero_copy_minibatches=False)),
     'lstm_cudnn_hidden64': ('squared', 64, 16, 'lstm', dict(fused_update=False, hidden=64),
                             dict(bptt_horizon=8, minibatch_size=64 * 16 // 2)),
+    'fast_path_off_slabs': ('breakout', 64, 128, 'mlp', dict(fast_path=False), {}),    # model(obs) + fused_ppo_loss
+    'squared_heads16_graph': ('squared', 64, 64, 'mlp', {}, dict(cuda_graph=True)),      # Discrete(8): 16-row chain
+    'lstm_cudnn_graph': ('squared', 64, 16, 'lstm', dict(fused_update=False, hidden=64),
+                         dict(bptt_horizon=8, minibatch_size=64 * 16 // 2, cuda_graph=True)),
 }
 
 
@@ -69,6 +73,8 @@ def build(env, n, h, kind, pol_kw, cfg_kw):
         pol = cleanrl.RecurrentPolicy(net, fused_sample=True, seed=3, fused_update=pol_kw.get('fused_update', True))
     else:
         net = models.Convolutional(vec.driver_env) if kind == 'conv' else models.Default(vec.driver_env)
+        if 'fast_path' in pol_kw:
+            net.fast_path = pol_kw['fast_path']
         pol = cleanrl.Policy(net, fused_sample=pol_kw.get('fused_sample', kind == 'mlp'), seed=7)
     return clean_pufferl.create(config(env, n, h, **cfg_kw), vec, pol.cuda())
 

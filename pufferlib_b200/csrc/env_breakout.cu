@@ -13,6 +13,7 @@
 #include <cuda.h>
 
 #include "env_common.cuh"
+#include "policy_sample.cuh"
 #include "tma.cuh"
 #include "wgmma.cuh"
 
@@ -427,34 +428,12 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
             if (DBG && p.dbg_out && t == 0)
 #pragma unroll
                 for (int a = 0; a < 8; ++a) p.dbg_out[(int64_t)e * 8 + a] = out[a];
-            // sample_logits (frameworks/cleanrl.py:25-47) by inverse CDF -- the arithmetic of k_policy_mlp_sample, with the
-            // action count fixed at compile time (breakout: 4 logits, value in column 4)
-            constexpr int NA = RO_HEADS - 1;
-            float mx = out[0];
-#pragma unroll
-            for (int k = 1; k < NA; ++k) mx = fmaxf(mx, out[k]);
-            float sum = 0.f;
-#pragma unroll
-            for (int k = 0; k < NA; ++k) sum += expf(out[k] - mx);
-            const float lse = mx + logf(sum);
-            const uint32_t rnd = pb_mix32(p.seed * 0x9E3779B97F4A7C15ull + (offset0 + (uint64_t)t) * 0xD1B54A32D192ED03ull +
-                                          (uint64_t)e * 0x2545F4914F6CDD1Dull);
-            const float u = (float)(rnd >> 8) * (1.0f / 16777216.0f);
-            const float value = out[NA];
-            float cdf = 0.f, lp = 0.f;
-            int act = -1;
-#pragma unroll
-            for (int k = 0; k < NA; ++k) {
-                const float nl = out[k] - lse, pk = expf(nl);
-                cdf += pk;
-                if (act < 0 && u < cdf) { act = k; lp = nl; }
-            }
-            if (act < 0) {   // rounding left cdf a hair below u: last action with non-negligible probability
-#pragma unroll
-                for (int k = NA - 1; k >= 0; --k)
-                    if (act < 0 && out[k] - lse > -80.f) { act = k; lp = out[k] - lse; }
-                if (act < 0) { act = NA - 1; lp = out[NA - 1] - lse; }
-            }
+            // sample_logits (frameworks/cleanrl.py:25-47): the epilogue of k_policy_mlp_sample (pb_sample_row), with the
+            // action count fixed at compile time (breakout: 4 logits, value in column 4); the entropy is not stored
+            int act;
+            float lp, ent_unused, value;
+            pb_sample_row<8>(out, RO_HEADS - 1, pb_policy_uniform(p.seed, offset0 + (uint64_t)t, e), act, lp,
+                                    ent_unused, value);
             const int64_t row = (int64_t)t * p.n + e;
             p.values[row] = value;
             p.logprobs[row] = lp;

@@ -1,10 +1,19 @@
-// policy_sample.cuh -- pieces shared by the fused rollout-time policy kernels (policy_mlp.cu, policy_lstm.cu):
+// policy_sample.cuh -- pieces shared by every kernel that samples actions (policy_mlp.cu, policy_lstm.cu, sample.cu and
+// the persistent rollout kernel of env_breakout.cu):
 //   * to_tf32 / mma_tf32: round-to-nearest TF32 conversion (cvt.rna) and the mma.sync m16n8k8 TF32 tile product;
 //   * pb_policy_uniform: the counter-based uniform of a row, u = mix(seed, step counter, row) in [0, 1), 24 bits;
-//   * pb_sample_row<NC>: one row's sampling epilogue over NC padded head outputs z[0..NC) = n_act logits | value | pad:
-//     logsumexp, the inverse CDF (first k with u < cdf_k), the fallback when rounding leaves cdf_{n_act-1} below u,
-//     logprob of the sampled action and the entropy (reference frameworks/cleanrl.py:25-47).
-// The bits of pb_sample_row<8> are those of the epilogue pb_policy_mlp_sample had before it moved here.
+//   * pb_sample_row<NC>: one row's sampling epilogue over NC padded head outputs z[0..NC) = n_act logits | value | pad
+//     (reference frameworks/cleanrl.py:25-47): lse = max z + log sum exp(z - max z), the probabilities
+//     p_k = exp(z_k - lse) (softmax(normalized) of the reference), their running sums c_k and their total T = c_{n-1}.
+//     The draw is the first k with u' < c_k.  For logits of ordinary size T is 1 up to the rounding of the p_k (a few
+//     ulps) and u' = u.  When the logits share a large offset C, lse is rounded on the grid of ulp(C) and T misses 1 by
+//     up to ulp(C)/2; that whole shortfall (or excess) would land on one action, so past |T - 1| > 2^-20 the draw
+//     renormalises, u' = u*T, as torch.multinomial does with its weights.  The bias left below that bound is under 2^-20
+//     of probability per row.  u <= 1 - 2^-24 gives fl(u*T) < T = the last running sum bit for bit, so the renormalised
+//     draw always finds a k; otherwise (u >= T < 1, at most 2^-20 of the rows) it takes the last action with p_k > 0.
+//     A zero-probability action is never drawn.  logprob = z_a - lse (the reference's normalized[a]);
+//     entropy = -sum (p_k/T) * max(z_k - lse, -FLT_MAX) (cleanrl.entropy of softmax(normalized), -inf logits kept
+//     finite as there).
 #pragma once
 #include "pb_common.cuh"
 
@@ -35,27 +44,31 @@ __device__ __forceinline__ void pb_sample_row(const float (&z)[NC], int n_act, f
 #pragma unroll
     for (int k = 0; k < NC; ++k) if (k < n_act) sum += expf(z[k] - mx);
     const float lse = mx + logf(sum);
+    float pk[NC];
+    float tot = 0.f;
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+        pk[k] = k < n_act ? expf(z[k] - lse) : 0.f;
+        tot += pk[k];                                  // the pad terms add exact zeros
+    }
+    const float uu = fabsf(tot - 1.f) > 0x1p-20f ? u * tot : u, inv = 1.f / tot;
     float cdf = 0.f, ent = 0.f, lp = 0.f, v = 0.f;
-    int a = -1;
+    int a = -1, last = 0;
 #pragma unroll
     for (int k = 0; k < NC; ++k) {
         if (k < n_act) {
-            const float nl = z[k] - lse, pk = expf(nl);
-            ent -= pk * nl;
-            cdf += pk;
-            if (a < 0 && u < cdf) { a = k; lp = nl; }
+            const float nl = z[k] - lse;
+            ent -= pk[k] * inv * fmaxf(nl, -3.4028234663852886e38f);
+            cdf += pk[k];
+            if (a < 0 && uu < cdf) { a = k; lp = nl; }
+            if (pk[k] > 0.f) last = k;
         }
         if (k == n_act) v = z[k];
     }
-    if (a < 0) {   // rounding left cdf a hair below u: last action with non-negligible probability
+    if (a < 0) {   // u >= T < 1 within the rounding of T: the last action with a non-zero probability
+        a = last;
 #pragma unroll
-        for (int k = NC - 1; k >= 0; --k)
-            if (a < 0 && k < n_act && z[k] - lse > -80.f) { a = k; lp = z[k] - lse; }
-        if (a < 0) {
-            a = n_act - 1;
-#pragma unroll
-            for (int k = 0; k < NC; ++k) if (k == a) lp = z[k] - lse;    // static indices: z stays in registers
-        }
+        for (int k = 0; k < NC; ++k) if (k == a) lp = z[k] - lse;    // static indices: z stays in registers
     }
     action = a;
     logprob = lp;

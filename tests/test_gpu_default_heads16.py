@@ -70,46 +70,74 @@ def _tail_inputs(m, n_act, rows, seed):
     return hidden, dout, w
 
 
-def _tail(dout, w, hidden, rows, legacy=False):
+def _tail(dout, w, hidden, rows, legacy=False, ws=None):
     m = hidden.shape[0]
     lib = _native.lib()
-    dpre = torch.full_like(hidden, 5.0)
-    grads = torch.full((rows * 128 + 128 + rows,), 5.0, device=DEV)
+    dpre = torch.full_like(hidden, float('nan'))
+    grads = torch.full((rows * 128 + 128 + rows,), float('nan'), device=DEV)
     if legacy:
         ws = torch.empty(lib.pb_mlp_tail_workspace_bytes(m, 128), dtype=torch.uint8, device=DEV)
         _native.check(lib.pb_mlp_tail_backward(_native.ptr(dout), dout.stride(0), _native.ptr(w), _native.ptr(hidden), m,
                                                128, _native.ptr(dpre), _native.ptr(grads), _native.ptr(ws), ws.numel(),
                                                _native.stream_ptr()))
     else:
-        ws = torch.empty(lib.pb_mlp_tail_workspace_bytes_ex(m, 128, rows), dtype=torch.uint8, device=DEV)
+        if ws is None:
+            ws = torch.empty(lib.pb_mlp_tail_workspace_bytes_ex(m, 128, rows), dtype=torch.uint8, device=DEV)
         _native.check(lib.pb_mlp_tail_backward_ex(_native.ptr(dout), dout.stride(0), _native.ptr(w), _native.ptr(hidden),
                                                   m, 128, _native.ptr(dpre), _native.ptr(grads), _native.ptr(ws),
                                                   ws.numel(), rows, _native.stream_ptr()))
     return dpre, grads
 
 
-@pytest.mark.parametrize('m', [1, 37, 4096, 524288 + 17])
-@pytest.mark.parametrize('n_act', [8, 15])
-@pytest.mark.parametrize('strided', [False, True])
-def test_mlp_tail_backward_16_rows(m, n_act, strided):
-    """pb_mlp_tail_backward_ex(head_rows=16) vs fp64 torch on the same inputs: dPre, dW_heads, db_heads, db_enc within 1e-5
-    of each output's maximum (all fp32 FMA).  strided: dout rows 20 floats apart take the generic kernel, contiguous
-    [M, 16] rows the TMA-staged one.  The padding rows of dW_heads and db_heads are exactly 0."""
-    hidden, dout, w = _tail_inputs(m, n_act, 16, m + n_act)
-    if strided:
-        wide = torch.zeros(m, 20, device=DEV)
-        wide[:, :16] = dout
-        dout = wide[:, :16]
-    dpre, grads = _tail(dout, w, hidden, 16)
+def _check_tail(dpre, grads, hidden, dout, w, rows, n_act):
     h64, d64, w64 = hidden.double(), dout.double(), w.double()
     ref_dpre = (d64 @ w64) * (h64 > 0)
-    refs = {'dpre': (dpre, ref_dpre), 'dW_heads': (grads[:16 * 128].view(16, 128), d64.t() @ h64),
-            'db_enc': (grads[16 * 128:17 * 128], ref_dpre.sum(0)), 'db_heads': (grads[17 * 128:], d64.sum(0))}
+    refs = {'dpre': (dpre, ref_dpre), 'dW_heads': (grads[:rows * 128].view(rows, 128), d64.t() @ h64),
+            'db_enc': (grads[rows * 128:(rows + 1) * 128], ref_dpre.sum(0)), 'db_heads': (grads[(rows + 1) * 128:], d64.sum(0))}
     for name, (got, ref) in refs.items():
-        err = float((got.double() - ref).abs().max())
+        err = float((got.double() - ref).abs().max())      # NaN (a row or an entry never written) fails too
         assert err <= 1e-5 * float(ref.abs().max()) + 1e-30, (name, err, float(ref.abs().max()))
-    assert float(grads[:16 * 128].view(16, 128)[n_act + 1:].abs().sum()) == 0.0
-    assert float(grads[17 * 128:][n_act + 1:].abs().sum()) == 0.0
+    assert float(grads[:rows * 128].view(rows, 128)[n_act + 1:].abs().sum()) == 0.0
+    assert float(grads[(rows + 1) * 128:][n_act + 1:].abs().sum()) == 0.0
+
+
+TAIL_HEADS = [(8, 1), (8, 4), (8, 7), (16, 8), (16, 15)]
+
+
+@pytest.mark.parametrize('m', [1, 31, 32, 33, 37, 511, 512, 513, 4096, 524288 + 17])
+@pytest.mark.parametrize('head_rows,n_act', TAIL_HEADS)
+@pytest.mark.parametrize('strided', [False, True])
+def test_mlp_tail_backward_matches_fp64(m, head_rows, n_act, strided):
+    """pb_mlp_tail_backward_ex on 8-row (n_act <= 7) and 16-row heads vs fp64 torch on the same inputs: dPre, dW_heads,
+    db_heads, db_enc within 1e-5 of each output's maximum (all fp32 FMA).  strided: dout rows head_rows + 4 floats apart
+    take the generic kernel, contiguous [M, head_rows] rows the TMA-staged one.  M runs over the edges of its 32-row TMA
+    chunks and 512-row CTAs; dPre and the gradients start as NaN, so a row the kernel skips fails.  The padding rows of
+    dW_heads and db_heads are exactly 0."""
+    hidden, dout, w = _tail_inputs(m, n_act, head_rows, m + n_act)
+    if strided:
+        wide = torch.zeros(m, head_rows + 4, device=DEV)
+        wide[:, :head_rows] = dout
+        dout = wide[:, :head_rows]
+    dpre, grads = _tail(dout, w, hidden, head_rows)
+    _check_tail(dpre, grads, hidden, dout, w, head_rows, n_act)
+
+
+@pytest.mark.parametrize('head_rows,n_act', [(8, 5), (16, 11)])
+@pytest.mark.parametrize('strided', [False, True])
+def test_mlp_tail_backward_small_launch_on_a_large_workspace(head_rows, n_act, strided):
+    """A launch of 513 rows on the workspace a 524 305-row launch just filled with its per-CTA partials: the reduction
+    reads only the small launch's own partials."""
+    lib = _native.lib()
+    big, small = 524288 + 17, 513
+    ws = torch.empty(lib.pb_mlp_tail_workspace_bytes_ex(big, 128, head_rows), dtype=torch.uint8, device=DEV)
+    for m in (big, small):
+        hidden, dout, w = _tail_inputs(m, n_act, head_rows, m)
+        if strided:
+            wide = torch.zeros(m, head_rows + 4, device=DEV)
+            wide[:, :head_rows] = dout
+            dout = wide[:, :head_rows]
+        dpre, grads = _tail(dout, w, hidden, head_rows, ws=ws)
+    _check_tail(dpre, grads, hidden, dout, w, head_rows, n_act)
 
 
 @pytest.mark.parametrize('m', [37, 524288 + 17])

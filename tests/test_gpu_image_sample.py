@@ -61,25 +61,6 @@ def test_sample_logits_logprob_entropy_match_torch(n, n_act):
     assert torch.equal(ar, actions) and torch.equal(lr, logprob) and torch.equal(vr, value)
 
 
-def test_sample_logits_distribution():
-    """Empirical action frequencies follow softmax(logits) (chi-square style bound), and draws change with offset."""
-    dev = torch.device('cuda')
-    n, n_act = 400000, 5
-    row = torch.tensor([0.1, 1.5, -0.7, 0.0, 2.2], device=dev)
-    logits = row.repeat(n, 1).contiguous()
-    p = torch.softmax(row, 0).cpu().numpy()
-    acts = []
-    for off in (0, 1):
-        a = torch.empty(n, dtype=torch.int64, device=dev)
-        _native.check(_native.lib().pb_sample_logits(_native.ptr(logits), n_act, n, n_act, C.c_uint64(1), C.c_uint64(off), None,
-                                                     _native.ptr(a), None, None, None, 1, None, None, None,
-                                                     _native.stream_ptr()))
-        acts.append(a)
-        freq = np.bincount(a.cpu().numpy(), minlength=n_act) / n
-        assert np.abs(freq - p).max() < 5 * np.sqrt(p.max() / n) + 1e-3
-    assert not torch.equal(acts[0], acts[1])
-
-
 def test_fused_policy_writes_rollout_rows_and_strided_heads():
     """cleanrl.Policy(fused_sample=True): both heads come out of one GEMM (strided logits / value) and the epilogue
     writes value / logprob / action straight into the given rollout rows."""

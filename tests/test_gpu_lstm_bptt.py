@@ -15,7 +15,8 @@ import pufferlib_b200.vector as pvec
 from pufferlib_b200 import _native, clean_pufferl, models
 from pufferlib_b200.environments import ocean
 from pufferlib_b200.frameworks import cleanrl
-from test_gpu_policy_lstm import fake_env, make_config, rna, sharpen
+from test_gpu_policy_lstm import fake_env, make_config, sharpen
+from util_gpu import rna
 
 gpu = pytest.mark.gpu
 TOL_STEP = 2e-4         # T = 1 outputs vs fp64 (the rollout step's bound)

@@ -16,6 +16,7 @@ import pufferlib_b200.vector as pvec
 from pufferlib_b200 import _native, clean_pufferl, models, spaces
 from pufferlib_b200.environments import ocean
 from pufferlib_b200.frameworks import cleanrl
+from util_gpu import off_boundary_mismatches, rna
 
 gpu = pytest.mark.gpu
 TOL = 2e-4              # per-step kernel outputs vs the fp64 restatement
@@ -24,30 +25,6 @@ TOL_ROLLOUT = 5e-4      # the same after up to 128 recurrent steps (the fp64 sta
 
 def cpu(x):
     return x.detach().cpu().numpy()
-
-
-def mix32(x):
-    """pb_mix32 (csrc/pb_common.cuh) on a uint64 array."""
-    with np.errstate(over='ignore'):
-        x = x + np.uint64(0x9E3779B97F4A7C15)
-        x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
-        x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
-        x = x ^ (x >> np.uint64(31))
-    return (x >> np.uint64(32)).astype(np.uint32)
-
-
-def uniforms(seed, offset, n):
-    """pb_policy_uniform (csrc/policy_sample.cuh) for rows 0..n-1."""
-    with np.errstate(over='ignore'):
-        key = (np.uint64(seed) * np.uint64(0x9E3779B97F4A7C15) + np.uint64(offset) * np.uint64(0xD1B54A32D192ED03)
-               + np.arange(n, dtype=np.uint64) * np.uint64(0x2545F4914F6CDD1D))
-    return (mix32(key) >> np.uint32(8)).astype(np.float32) * np.float32(1.0 / 16777216.0)
-
-
-def rna(t):
-    """Nearest TF32 value (ties away from zero, cvt.rna) of the fp32 value of t, as fp64."""
-    bits = t.detach().float().contiguous().view(torch.int32)
-    return ((bits + 0x1000) & ~0x1FFF).view(torch.float32).double()
 
 
 def reference_step(net, x, h, c):
@@ -62,16 +39,6 @@ def reference_step(net, x, h, c):
     h2 = torch.sigmoid(o) * torch.tanh(c2)
     w_cat, b_cat = inner.head_matrix()
     return h2, c2, rna(h2) @ rna(w_cat).t() + b_cat.double()
-
-
-def off_boundary_mismatches(actions, logits, seed, offset):
-    """Rows whose action is not the first k with u < cdf_k, among rows with u more than 1e-4 from every cdf_k."""
-    n, n_act = logits.shape
-    cdf = (logits - logits.logsumexp(-1, keepdim=True)).exp().cumsum(-1).cpu().numpy()
-    u = uniforms(seed, offset, n).astype(np.float64)
-    want = (u[:, None] >= cdf).sum(-1).clip(max=n_act - 1)
-    near = (np.abs(u[:, None] - cdf) < 1e-4).any(-1)
-    return int(((want != actions) & ~near).sum())
 
 
 def fake_env(obs_shape, n_act, dtype=np.float32):

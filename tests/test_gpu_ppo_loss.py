@@ -30,7 +30,8 @@ def reference_loss(logits, value, actions, old_lp, adv, ret, old_v, cfg):
     return loss, torch.stack([pg, vl, ent, old_kl, kl, clipfrac]).detach()
 
 
-@pytest.mark.parametrize('m,n_act', [(1, 4), (1000, 4), (4097, 6), (524288, 4), (333, 18)])
+@pytest.mark.parametrize('m,n_act', [(1, 4), (1000, 4), (4097, 6), (524288, 4), (333, 18), (4097, 1), (4097, 32),
+                                     (1, 32)])
 @pytest.mark.parametrize('clip_vloss', [True, False])
 def test_ppo_loss_matches_torch_autograd(m, n_act, clip_vloss):
     dev = torch.device('cuda')

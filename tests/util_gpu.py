@@ -7,6 +7,52 @@ import torch
 from pufferlib_b200 import _native
 
 
+def mix32(x):
+    """pb_mix32 (csrc/pb_common.cuh) on a uint64 array."""
+    with np.errstate(over='ignore'):
+        x = x + np.uint64(0x9E3779B97F4A7C15)
+        x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        x = x ^ (x >> np.uint64(31))
+    return (x >> np.uint64(32)).astype(np.uint32)
+
+
+def uniforms(seed, offset, n):
+    """pb_policy_uniform (csrc/policy_sample.cuh) for rows 0..n-1: the uniforms every sampler draws with."""
+    with np.errstate(over='ignore'):
+        key = (np.uint64(seed) * np.uint64(0x9E3779B97F4A7C15) + np.uint64(offset) * np.uint64(0xD1B54A32D192ED03)
+               + np.arange(n, dtype=np.uint64) * np.uint64(0x2545F4914F6CDD1D))
+    return (mix32(key) >> np.uint32(8)).astype(np.float32) * np.float32(1.0 / 16777216.0)
+
+
+def rna(t):
+    """Nearest TF32 value (ties away from zero, cvt.rna) of the fp32 value of t, as fp64."""
+    bits = t.detach().float().contiguous().view(torch.int32)
+    return ((bits + 0x1000) & ~0x1FFF).view(torch.float32).double()
+
+
+def restated_draw(probs, u, window):
+    """The inverse-CDF draw of pb_sample_row restated on fp64 probabilities [n, A] (numpy) and the uniforms u [n]:
+    -> (actions: the first k with u < cdf_k, near: rows whose u lies within `window` of an inner boundary cdf_k,
+    k < A - 1, where the kernel's fp32 weights may decide either way)."""
+    cdf = np.cumsum(probs, -1)
+    u = np.asarray(u, np.float64)[:, None]
+    want = (u >= cdf).sum(-1).clip(max=probs.shape[1] - 1)
+    near = (np.abs(u - cdf[:, :-1]) < window).any(-1)
+    return want, near
+
+
+def softmax64(logits):
+    """fp64 softmax of logits (a torch tensor, any float type) -> numpy [n, A]."""
+    return torch.softmax(logits.double(), -1).cpu().numpy()
+
+
+def off_boundary_mismatches(actions, logits, seed, offset, window=1e-4):
+    """Rows whose action is not the first k with u < cdf_k, among rows with u more than `window` from every cdf_k."""
+    want, near = restated_draw(softmax64(logits), uniforms(seed, offset, logits.shape[0]), window)
+    return int(((want != np.asarray(actions)) & ~near).sum())
+
+
 def gae_device(rewards_tm, values_tm, dones_tm, gamma, lam, want_returns=True):
     """rewards/values/dones: numpy [H, N] (arrival order).  Returns (advantages_sorted, returns_sorted) numpy."""
     h, n = rewards_tm.shape

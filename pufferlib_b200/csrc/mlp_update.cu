@@ -19,6 +19,12 @@
 //     work on the registers of that accumulator layout;
 //   * dW_enc^T [feature][hidden unit] += x^T . dPre on the tensor core (wgmma RS: x^T fragments read from the x tile, dPre^T
 //     from shared memory as the K-major B operand); the accumulator stays in registers across all tiles of the CTA.
+// The tensor core works one tile ahead of the epilogue: at the end of tile it, the forward product of tile it + 1 is issued
+// first and the dW_enc product of tile it after it; tile it + 1 waits only for its forward (wgmma_wait<1>), so the dW_enc
+// product runs under the epilogue of tile it + 1 and is retired just before the next one is issued.  That takes two
+// relu(h)^T / dPre^T buffers (tile it uses buffer it & 1) and keeps the x^T fragments of the product in flight in
+// registers; the x ring has two stages so that shared memory still fits.  Neither accumulator is written by anything but
+// wgmma between issue and wait (the first product into each has scale-d 0), so ptxas keeps the products asynchronous.
 // Per-CTA partials go to a workspace and k_update_reduce sums them deterministically into the flat gradient buffer
 // [dW_enc (hid x feat) | dW_heads (8 x hid) | db_enc | db_heads] of clean_pufferl._DefaultMLPUpdate, leaving per-block
 // sums of squares for pb_clip_adam_parts.
@@ -27,6 +33,11 @@
 // with TF32 operands and fp32 accumulation -- the precision class of torch.set_float32_matmul_precision('high'), which
 // clean_pufferl sets; variant 1 forms the head and g^T products with fp32 FFMAs.  The dPre-to-HBM mode (dW_enc by the
 // caller) runs the variant-1 epilogue.  Every mbarrier wait is bounded (tma.cuh: __trap instead of a hang).
+//
+// Built with -DPB_UPDATE_PHASES (bench_update.py builds such a library of its own), lane 0 of each warpgroup records
+// clock64() at the phase boundaries of the first PH_TILES tiles of its CTA into a buffer set by
+// pb_mlp_update_set_phase_buffer; pb_mlp_update_phase_names names the phases.  Without the macro none of that code
+// exists (the SASS of the library is the same with and without it).
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -42,12 +53,13 @@ constexpr int W_KBLK_BYTES = HID * KBLK * 4;           // 16 KiB: [128 hidden un
 constexpr int X_KBLK_BYTES = TILE_M * KBLK * 4;        // 8 KiB: [64 rows][32 features]
 constexpr int X_TILE_BYTES = 4 * X_KBLK_BYTES;         // 32 KiB
 constexpr int G_KBLK_BYTES = HID * 32 * 4;             // 16 KiB: [128 hidden units][32 rows]
-constexpr int NSTAGE = 3;                              // x tiles in flight per SM
+constexpr int NSTAGE = 2;                              // x tiles in flight per SM
 constexpr int THREADS = 256;                           // two warpgroups
 constexpr int SM_W = 0;                                // W_enc, K-major SWIZZLE_128B, resident
 constexpr int SM_X = 4 * W_KBLK_BYTES;                 // NSTAGE x tiles, K-major SWIZZLE_128B
-constexpr int SM_G = SM_X + NSTAGE * X_TILE_BYTES;     // relu(h)^T, then dPre^T: two [128 hidden][32 rows] K-major blocks
-constexpr int SM_WH = SM_G + 2 * G_KBLK_BYTES;         // W_heads [8][128]
+constexpr int G_BUF_BYTES = 2 * G_KBLK_BYTES;         // relu(h)^T, then dPre^T: two [128 hidden][32 rows] K-major blocks
+constexpr int SM_G = SM_X + NSTAGE * X_TILE_BYTES;     // two such buffers: tile it uses buffer it & 1
+constexpr int SM_WH = SM_G + 2 * G_BUF_BYTES;          // W_heads [8][128]
 constexpr int SM_BE = SM_WH + NO * HID * 4;            // b_enc [128]
 constexpr int SM_OUT = SM_BE + HID * 4;                // head outputs [2 hidden halves][64 rows][8]
 constexpr int SM_DO = SM_OUT + 2 * TILE_M * NO * 4;    // dOut [64 rows][8]
@@ -82,7 +94,20 @@ struct FusedParams {
     const float* w_heads;      // [8][128], b_enc [128], b_heads [8]
     const float* b_enc;
     const float* b_heads;
+#ifdef PB_UPDATE_PHASES
+    unsigned long long* phases;
+#endif
 };
+#ifdef PB_UPDATE_PHASES
+constexpr int PH_TILES = 32, PH_N = 8;                 // [grid][warpgroups][PH_TILES][PH_N] clock64 stamps
+#define PB_PHASE(k, idx)                                                                                               \
+    do {                                                                                                               \
+        if (p.phases && (tid & 127) == 0 && (k) < PH_TILES)                                                            \
+            p.phases[(((int64_t)blockIdx.x * (THREADS / 128) + (tid >> 7)) * PH_TILES + (k)) * PH_N + (idx)] = clock64(); \
+    } while (0)
+#else
+#define PB_PHASE(k, idx) do {} while (0)
+#endif
 
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
     asm volatile(
@@ -197,7 +222,6 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
     float* outp = reinterpret_cast<float*>(smem + SM_OUT);
     float* dos = reinterpret_cast<float*>(smem + SM_DO);
     float* red = reinterpret_cast<float*>(smem + SM_RED);
-    uint8_t* gbuf = smem + SM_G;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
     const int wg = warp >> 2, wq = warp & 3;
     const int n_my = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // tiles of this CTA (>= 1)
@@ -251,19 +275,45 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
         }
     }
 
-    float dwacc[64];                     // dW_enc^T [feature 64wg + 16wq + g (+8)][hidden unit 8j + 2t (+1)]
-#pragma unroll
-    for (int i = 0; i < 64; ++i) dwacc[i] = 0.f;
+    float dwacc[64];                     // dW_enc^T [feature 64wg + 16wq + g (+8)][hidden unit 8j + 2t (+1)]; the first
+                                         // wgmma into it has scale-d 0 (no zeroing between asynchronous products)
     float dwh[4] = {0.f, 0.f, 0.f, 0.f};  // dW_heads^T [hr0 | hr1][head 2t | 2t + 1]
     float be_acc[2] = {0.f, 0.f};        // db_enc[hr0], db_enc[hr1] over this thread's rows
     float bh_acc[2] = {0.f, 0.f};        // db_heads[sub], [sub + 4] over this thread's loss rows
     double st[6] = {0, 0, 0, 0, 0, 0};
     const float adv_mean = p.adv_norm ? p.adv_norm[0] : 0.f, adv_rstd = p.adv_norm ? p.adv_norm[1] : 1.f;
     const bool need_old_v = p.clip_vloss || !p.returns;
-    const uint32_t w_addr = smem_u32(smem + SM_W), g_addr = smem_u32(gbuf);
+    const uint32_t w_addr = smem_u32(smem + SM_W);
+
+    // ---- 1. hidden^T = W_enc[64wg .. 64wg + 63] . x^T  (M = hidden units, N = 64 rows, K = 128 features), issued one
+    //         tile ahead: the forward of tile it + 1 goes to the tensor core before the dW_enc product of tile it, and
+    //         that product completes under the epilogue of tile it + 1 (retired by the wgmma_wait<0> of step 6)
+    float h[32];
+    auto forward = [&](int it) {
+        const int s = it % NSTAGE;
+        mbar_wait(&x_full[s], (uint32_t)((it / NSTAGE) & 1));
+        const uint32_t x_addr = smem_u32(smem + SM_X + s * X_TILE_BYTES);
+        wgmma_fence();                   // the first wgmma has scale-d 0: h needs no zeroing
+#pragma unroll
+        for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                wgmma_m64n64k8_ss(h, wgmma_desc_sw128(w_addr + kb * W_KBLK_BYTES + wg * 8192 + k * 32),
+                                  wgmma_desc_sw128(x_addr + kb * X_KBLK_BYTES + k * 32), (kb | k) ? 1 : 0);
+        wgmma_commit();
+    };
+    uint32_t xa[8][4];                   // x^T A fragments of the dW_enc product in flight (owned until its wait)
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) xa[ks][i] = 0u;
+    mbar_wait(w_full, 0);
+    forward(0);
 
     for (int it = 0; it < n_my; ++it) {
         const int s = it % NSTAGE;
+        uint8_t* gbuf = smem + SM_G + (it & 1) * G_BUF_BYTES;
+        const uint32_t g_addr = smem_u32(gbuf);
         const int tile = (int)blockIdx.x + it * (int)gridDim.x;
         const int slab = tile / p.tiles_per_slab, tis = tile - slab * p.tiles_per_slab;
         const int64_t lrow0 = (int64_t)tis * TILE_M;                          // slab-local row of tile row 0
@@ -281,48 +331,40 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
             if (need_old_v) old_v = p.old_values[ri];
             if (p.returns) ret = p.returns[ri];
         }
-        if (it == 0) mbar_wait(w_full, 0);
-        mbar_wait(&x_full[s], (uint32_t)((it / NSTAGE) & 1));
+        PB_PHASE(it, 0);
         const uint8_t* xs = smem + SM_X + s * X_TILE_BYTES;
-        const uint32_t x_addr = smem_u32(xs);
-
-        // ---- 1. hidden^T = W_enc[64wg .. 64wg + 63] . x^T  (M = hidden units, N = 64 rows, K = 128 features)
-        float h[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) h[i] = 0.f;
-        wgmma_fence();
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                wgmma_m64n64k8_ss(h, wgmma_desc_sw128(w_addr + kb * W_KBLK_BYTES + wg * 8192 + k * 32),
-                                  wgmma_desc_sw128(x_addr + kb * X_KBLK_BYTES + k * 32), (kb | k) ? 1 : 0);
-        wgmma_commit();
-        wgmma_wait<0>();
+        // the forward of this tile is done; the dW_enc product of the previous tile (committed after it) may still run
+        if (DW_KERNEL && it > 0) wgmma_wait<1>();
+        else wgmma_wait<0>();
         wgmma_fence_acc(h);
+        float hv[32];                            // the epilogue works on a copy: h stays the forward's accumulator only
+#pragma unroll
+        for (int i = 0; i < 32; ++i) hv[i] = h[i];
+        PB_PHASE(it, 1);
 
         // ---- 2. relu(h + b_enc)^T -> shared memory (the operand of the head products)
         {
             const float b0 = be[hr0], b1 = be[hr1];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                h[4 * j] = fmaxf(h[4 * j] + b0, 0.f);
-                h[4 * j + 1] = fmaxf(h[4 * j + 1] + b0, 0.f);
-                h[4 * j + 2] = fmaxf(h[4 * j + 2] + b1, 0.f);
-                h[4 * j + 3] = fmaxf(h[4 * j + 3] + b1, 0.f);
+                hv[4 * j] = fmaxf(hv[4 * j] + b0, 0.f);
+                hv[4 * j + 1] = fmaxf(hv[4 * j + 1] + b0, 0.f);
+                hv[4 * j + 2] = fmaxf(hv[4 * j + 2] + b1, 0.f);
+                hv[4 * j + 3] = fmaxf(hv[4 * j + 3] + b1, 0.f);
                 const int l = 8 * j + 2 * t;
-                *reinterpret_cast<float2*>(gbuf + g_off(hr0, l)) = make_float2(h[4 * j], h[4 * j + 1]);
-                *reinterpret_cast<float2*>(gbuf + g_off(hr1, l)) = make_float2(h[4 * j + 2], h[4 * j + 3]);
+                *reinterpret_cast<float2*>(gbuf + g_off(hr0, l)) = make_float2(hv[4 * j], hv[4 * j + 1]);
+                *reinterpret_cast<float2*>(gbuf + g_off(hr1, l)) = make_float2(hv[4 * j + 2], hv[4 * j + 3]);
                 if (p.dbg_hidden) {
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
                         const int le = l + (e & 1), he = (e & 2) ? hr1 : hr0;
-                        if (le < rows_left) p.dbg_hidden[(i0 + le) * HID + he] = h[4 * j + e];
+                        if (le < rows_left) p.dbg_hidden[(i0 + le) * HID + he] = hv[4 * j + e];
                     }
                 }
             }
         }
         __syncthreads();
+        PB_PHASE(it, 2);
 
         // ---- 3. head products: out[row][a] = relu(h)[row] . W_heads[a]
         if (TF32_EPI) {      // warp: rows 16(warp & 3) .. +15, hidden half warp >> 2; partial sums of the two halves to outp
@@ -353,6 +395,7 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
             *reinterpret_cast<float2*>(outp + l * NO + a0) = make_float2(o0, o1);
         }
         __syncthreads();
+        PB_PHASE(it, 3);
 
         // ---- 4. the loss row math -> dOut of the tile
         {
@@ -379,6 +422,7 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
             }
         }
         __syncthreads();
+        PB_PHASE(it, 4);
 
         // ---- 5. g^T = W_heads^T dOut^T (same fragment layout as hidden^T), dPre^T = g^T where relu(h) > 0, db_enc, and
         //         dW_heads^T += relu(h)^T dOut with the hidden^T registers as the A fragments (k = t <-> row 8j + 2t,
@@ -407,16 +451,16 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
                 dp[4 * j] = s00; dp[4 * j + 1] = s01; dp[4 * j + 2] = s10; dp[4 * j + 3] = s11;
             }
 #pragma unroll
-            for (int e = 0; e < 4; ++e) dp[4 * j + e] = h[4 * j + e] > 0.f ? dp[4 * j + e] : 0.f;
+            for (int e = 0; e < 4; ++e) dp[4 * j + e] = hv[4 * j + e] > 0.f ? dp[4 * j + e] : 0.f;
             be_acc[0] += dp[4 * j] + dp[4 * j + 1];
             be_acc[1] += dp[4 * j + 2] + dp[4 * j + 3];
             const float b0 = dos[(8 * j + 2 * t) * NO + g], b1 = dos[(8 * j + 2 * t + 1) * NO + g];
             if (TF32_EPI) {
-                const uint32_t a[4] = {__float_as_uint(h[4 * j]), __float_as_uint(h[4 * j + 2]), __float_as_uint(h[4 * j + 1]),
-                                       __float_as_uint(h[4 * j + 3])};
+                const uint32_t a[4] = {__float_as_uint(hv[4 * j]), __float_as_uint(hv[4 * j + 2]), __float_as_uint(hv[4 * j + 1]),
+                                       __float_as_uint(hv[4 * j + 3])};
                 mma_tf32(dwh, a, __float_as_uint(b0), __float_as_uint(b1));
             } else {
-                const uint32_t a[4] = {to_tf32(h[4 * j]), to_tf32(h[4 * j + 2]), to_tf32(h[4 * j + 1]), to_tf32(h[4 * j + 3])};
+                const uint32_t a[4] = {to_tf32(hv[4 * j]), to_tf32(hv[4 * j + 2]), to_tf32(hv[4 * j + 1]), to_tf32(hv[4 * j + 3])};
                 mma_tf32(dwh, a, to_tf32(b0), to_tf32(b1));
             }
             const int l = 8 * j + 2 * t;
@@ -440,11 +484,17 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
 
         // ---- 6. dW_enc^T [64wg .. 64wg + 63][128] += x^T . dPre  (M = features, N = hidden units, K = 64 rows).  Both
         //         operands are rounded to nearest TF32 (truncation would bias a sum over the whole minibatch)
+        PB_PHASE(it, 5);
         if (DW_KERNEL) {
             fence_proxy_async_smem();            // dPre^T written by the generic proxy, read by the tensor core
-            __syncthreads();
+            wgmma_wait<0>();                     // the previous tile's dW_enc product: its A registers and buffer are free
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
+            __syncthreads();                     // dPre^T of both warpgroups is in the buffer
+            if (it + 1 < n_my) forward(it + 1);
             const int f0 = 64 * wg + 16 * wq + g;
-            uint32_t xa[8][4];                   // all A fragments of the tile: registers stay owned until the wait
 #pragma unroll
             for (int ks = 0; ks < 8; ++ks) {
                 const int r0 = 8 * ks + t;
@@ -456,14 +506,10 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < 8; ++ks)
-                wgmma_m64n128k8_rs(dwacc, xa[ks], wgmma_desc_sw128(g_addr + (ks >> 2) * G_KBLK_BYTES + (ks & 3) * 32), 1);
+                wgmma_m64n128k8_rs(dwacc, xa[ks], wgmma_desc_sw128(g_addr + (ks >> 2) * G_KBLK_BYTES + (ks & 3) * 32),
+                                   (it | ks) ? 1 : 0);
             wgmma_commit();
-            wgmma_wait<0>();
-            wgmma_fence_acc(dwacc);
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)
-#pragma unroll
-                for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
+            PB_PHASE(it, 6);
         } else {
             // ---- 6'. dPre rows to HBM: warp w writes rows 8w .. 8w + 7, one whole 512-byte row per store instruction
             __syncthreads();
@@ -479,12 +525,21 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
                     __stcs(reinterpret_cast<float4*>(p.dpre_out + (i0 + l) * HID + n), v);
                 }
             }
+            if (it + 1 < n_my) forward(it + 1);
         }
-        __syncthreads();                         // every read of x stage s and of the shared tile buffers is done
+        __syncthreads();                         // every read of x stage s is done
         if (tid == 0 && it + NSTAGE < n_my) {
             fence_proxy_async_smem();
             issue(it + NSTAGE);
         }
+    }
+    if (DW_KERNEL) {                             // the last tile's dW_enc product
+        wgmma_wait<0>();
+        wgmma_fence_acc(dwacc);
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
     }
 
     // ================= per-CTA partials =================
@@ -595,7 +650,32 @@ int num_sms() { return pb_num_sms(); }
 
 int g_update_variant = 2;     // 1 = fp32 head / g^T products, 2 = TF32 mma.sync epilogue
 
+#ifdef PB_UPDATE_PHASES
+unsigned long long* g_phases = nullptr;
+#endif
 }  // namespace
+#ifdef PB_UPDATE_PHASES
+// clock64 stamps of the next launches: [grid][warpgroups][PH_TILES][PH_N] (nullptr: none)
+extern "C" int pb_mlp_update_set_phase_buffer(void* buf) {
+    g_phases = static_cast<unsigned long long*>(buf);
+    return PB_OK;
+}
+// -> warpgroups per CTA; tiles sampled per CTA, stamps per tile
+extern "C" int32_t pb_mlp_update_phase_layout(int32_t* tiles, int32_t* n) {
+    *tiles = PH_TILES;
+    *n = PH_N;
+    return THREADS / 128;
+}
+// what each warpgroup's stamps delimit (one comma-separated list per warpgroup, ';' between warpgroups): phase i runs from
+// stamp i to stamp i + 1, the last one to the next tile's stamp 0
+extern "C" const char* pb_mlp_update_phase_names(void) {
+#define PB_PHASE_NAMES "forward wgmma wait,bias + ReLU store + barrier,head products + barrier,loss rows + barrier," \
+                       "g^T / dPre^T / dW_heads,previous dW_enc wait + barrier + next forward + dW_enc issue," \
+                       "barrier + refill + next row loads"
+    return PB_PHASE_NAMES ";" PB_PHASE_NAMES;
+#undef PB_PHASE_NAMES
+}
+#endif
 
 extern "C" int pb_mlp_update_set_variant(int32_t variant) {
     PB_REQUIRE(variant == 1 || variant == 2, PB_ERR_INVALID, "pb_mlp_update_set_variant: 1 or 2");
@@ -657,6 +737,9 @@ extern "C" int pb_mlp_update_fused(const float* x, int64_t ldx, int64_t slab_row
     p.part_dw = (float*)workspace; p.part_tail = (float*)workspace + (size_t)num_sms() * FEAT * HID;
     p.w_heads = w_heads; p.b_enc = b_enc; p.b_heads = b_heads;
     p.stats = stats8; p.dpre_out = dpre_out; p.dbg_hidden = dbg_hidden; p.dbg_dpre = dbg_dpre; p.dbg_dout = dbg_dout;
+#ifdef PB_UPDATE_PHASES
+    p.phases = g_phases;
+#endif
     PB_CUDA(cudaMemsetAsync(stats8, 0, 8 * sizeof(double), s));
     static bool attr_set = false;
     if (!attr_set) {

@@ -18,10 +18,15 @@
  *     PB_ERR_CUDA.
  *   - One host thread per GPU drives a handle; the library creates no threads and is re-entrant per handle.
  *
+ * Agent rows: a kind has A agents per env (pb_env_agents_per_env; A = 2 for MULTIAGENT, 1 for every other kind).
+ * Agent a of env e is row e*A + a, the order of the reference's Serial._assign_buffers (vector.py:97-110).  Seeds,
+ * env_index_offset and num_envs count envs; observations, rewards, flags and actions count agent rows (N*A of them).
+ *
  * Rollout layout ("arrival order", identical to the reference's Experience tensors when every mask is True and
- * agent_ids == arange(N), clean_pufferl.py:390-397,436-450): row index = t*N + e for step t, env e.
- * "Sorted order" (what Experience.sort_training_data produces, clean_pufferl.py:452-464) is f = e*H + t; on the
- * device that permutation is arithmetic, no index tensor exists.
+ * agent_ids == arange(N*A), clean_pufferl.py:390-397,436-450): row index = t*(N*A) + e*A + a for step t, env e,
+ * agent a (t*N + e when A = 1).  "Sorted order" (what Experience.sort_training_data produces,
+ * clean_pufferl.py:452-464) is f = r*H + t for agent row r; on the device that permutation is arithmetic, no index
+ * tensor exists.  The GAE, minibatch and policy entry points below work on rows: their num_envs is N*A.
  */
 #ifndef PUFFERLIB_B200_H
 #define PUFFERLIB_B200_H
@@ -46,7 +51,9 @@ enum {
 enum {
     PB_ENV_SQUARED = 0, PB_ENV_BREAKOUT = 1, PB_ENV_SNAKE = 2, PB_ENV_PONG = 3,
     /* the reference's ocean test envs (environments/ocean/ocean.py; creators environment.py:33-46, 67-70) */
-    PB_ENV_MEMORY = 4, PB_ENV_PASSWORD = 5, PB_ENV_STOCHASTIC = 6, PB_ENV_BANDIT = 7
+    PB_ENV_MEMORY = 4, PB_ENV_PASSWORD = 5, PB_ENV_STOCHASTIC = 6, PB_ENV_BANDIT = 7,
+    /* two PettingZoo agents per env (ocean.py:149-208 behind PettingZooPufferEnv, emulation.py:236-420) */
+    PB_ENV_MULTIAGENT = 8
 };
 enum { PB_DTYPE_F32 = 0, PB_DTYPE_U8 = 1 };
 
@@ -54,7 +61,7 @@ typedef struct pb_env pb_env; /* opaque: N env instances resident on one GPU */
 
 typedef struct {
     int32_t kind;             /* PB_ENV_* */
-    int32_t num_envs;         /* N: env instances (== agents) on this GPU */
+    int32_t num_envs;         /* N: env instances on this GPU (N*A agent rows, see "Agent rows" above) */
     int32_t device;           /* CUDA device ordinal */
     int32_t reserved;
     int64_t env_index_offset; /* global index of local env 0 (multi-GPU shards seed by GLOBAL index) */
@@ -67,7 +74,9 @@ typedef struct {
                                            [0, 1024] (0 = default 2)                    ocean.py:64-123
                                  PASSWORD: [0]=password_length in [1, 128] (default 5)  ocean.py:228-281
                                  STOCHASTIC: no iparam; p is dparam[0]; episodes are 100 steps  ocean.py:529-582
-                                 BANDIT  : [0]=num_actions in [1, 32768] (default 10)   ocean.py:8-62 */
+                                 BANDIT  : [0]=num_actions in [1, 32768] (default 10)   ocean.py:8-62
+                                 MULTIAGENT: no parameters (any non-zero iparam or any dparam is refused)
+                                                                                        ocean.py:149-208 */
 } pb_env_config;
 
 typedef struct {
@@ -85,13 +94,14 @@ typedef struct {
  * the env kernel then stores straight into rollout row t (replaces buf.observations[row][:] = ob,
  * emulation.py:158-164, plus the obs/reward/done part of Experience.store, clean_pufferl.py:442-447). */
 typedef struct {
-    void* obs;            /* env e writes obs_bytes at (char*)obs + e*obs_stride */
-    int64_t obs_stride;   /* bytes between consecutive envs' rows (>= obs_bytes) */
-    float* rewards;       /* [N] fp32                          (buf.rewards,     emulation.py:219-221) */
-    uint8_t* terminals;   /* [N] bool as one byte               (buf.terminals)   */
-    uint8_t* truncations; /* [N] bool, always 0 for these envs  (buf.truncations); constants: written by reset, and by */
-    uint8_t* masks;       /* [N] bool, always 1 (buf.masks)       a step only into buffers other than the previous call's */
-    float* dones_f32;     /* optional [N]: terminal as 0.f/1.f  (Experience.dones, clean_pufferl.py:395,447); may be NULL */
+    void* obs;            /* agent row r = e*A + a writes obs_bytes at (char*)obs + r*obs_stride */
+    int64_t obs_stride;   /* bytes between consecutive rows (>= obs_bytes) */
+    /* every array below has N*A entries, one per agent row (N when A = 1) */
+    float* rewards;       /* fp32                          (buf.rewards,     emulation.py:219-221) */
+    uint8_t* terminals;   /* bool as one byte               (buf.terminals)   */
+    uint8_t* truncations; /* bool, always 0 for these envs  (buf.truncations); constants: written by reset, and by */
+    uint8_t* masks;       /* bool, always 1 (buf.masks)       a step only into buffers other than the previous call's */
+    float* dones_f32;     /* optional: terminal as 0.f/1.f  (Experience.dones, clean_pufferl.py:395,447); may be NULL */
 } pb_env_out;
 
 const char* pb_last_error(void);
@@ -115,13 +125,17 @@ int pb_env_create(const pb_env_config* cfg, pb_env** out);
 int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_host, int32_t n_dparam, pb_env** out);
 int pb_env_destroy(pb_env* env);
 int pb_env_get_info(const pb_env* env, pb_env_info* out);
+/* A, the agents per env (PettingZooPufferEnv.num_agents, emulation.py:262): 2 for MULTIAGENT, 1 otherwise.  The
+ * outputs of reset / step and the actions of a step have N*A rows in the "Agent rows" order above. */
+int pb_env_agents_per_env(const pb_env* env, int32_t* out);
 
 /* vector.py:112-135: (re)seed env i with seed + env_index_offset + i (make_seeds, vector.py:639-641), reset it and
  * write the reset rows (r=0, terminal=False, truncation=False, mask=True; emulation.py:187-192). */
 int pb_env_reset(pb_env* env, uint64_t seed, const pb_env_out* out, void* stream);
 
 /* vector.py:137-156: envs whose previous row was terminal reset (action ignored, reset row written), all others
- * step with actions[e] (int64, Discrete).  PB_ERR_STATE before the first reset.  `actions` is validated on the
+ * step with actions[e] (int64, Discrete; actions[e*A + a] for agent a).  A multi-agent env resets when all of its
+ * agents' previous rows were terminal (PettingZooPufferEnv.done, emulation.py:283-284, 415).  PB_ERR_STATE before the first reset.  `actions` is validated on the
  * device only by clamping into [0, num_actions) -- the host layer does the reference's first-send
  * action_space.contains check (vector.py:36-39). */
 int pb_env_step(pb_env* env, const int64_t* actions, const pb_env_out* out, void* stream);
@@ -141,6 +155,12 @@ int pb_env_stats_read(pb_env* env, double* out4_host, int clear, void* stream);
 /* The score of pb_env_episode_rows in fp64, for the kinds whose score is a python float that fp32 does not hold
  * (STOCHASTIC: 1 - (p - frac)**2); *score = NULL for the kinds without one (their fp32 score is exact). */
 int pb_env_episode_score_f64(pb_env* env, const double** score);
+/* Per-agent statistics of the multi-agent kinds (MultiagentEpisodeStats, postprocess.py:147-179, which computes
+ * episode_return / episode_length and then drops them: only the env's own per-agent info values are kept):
+ * out4_host = {env steps, sum of agent 1's score, sum of agent 2's score, 0} accumulated on the device since the last
+ * read with clear != 0.  Copies 32 bytes to host memory and synchronises `stream` once.  PB_ERR_INVALID for kinds
+ * with one agent per env (pb_env_stats_read serves those). */
+int pb_env_agent_stats_read(pb_env* env, double* out4_host, int clear, void* stream);
 
 /* -- rollout ---------------------------------------------------------------------------------------------------
  * Replaces the policy-output part of Experience.store (clean_pufferl.py:443-446): one fused copy of value /

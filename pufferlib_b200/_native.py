@@ -12,7 +12,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get('PUFFERLIB_B200_SO', os.path.join(HERE, 'libpuffer_b200.so'))   # override: debug builds
 
 PB_OK, PB_ERR_INVALID, PB_ERR_CUDA, PB_ERR_STATE, PB_ERR_UNSUPPORTED = 0, -1, -2, -3, -4
-ENV_KINDS = {'squared': 0, 'breakout': 1, 'snake': 2, 'pong': 3, 'memory': 4, 'password': 5, 'stochastic': 6, 'bandit': 7}
+ENV_KINDS = {'squared': 0, 'breakout': 1, 'snake': 2, 'pong': 3, 'memory': 4, 'password': 5, 'stochastic': 6, 'bandit': 7,
+             'multiagent': 8}
 DTYPE_F32, DTYPE_U8 = 0, 1
 
 
@@ -58,11 +59,13 @@ SIGNATURES = {
     'pb_env_episode_score_f64': (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     'pb_env_destroy': (C.c_int, [C.c_void_p]),
     'pb_env_get_info': (C.c_int, [C.c_void_p, C.POINTER(EnvInfo)]),
+    'pb_env_agents_per_env': (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     'pb_env_reset': (C.c_int, [C.c_void_p, C.c_uint64, C.POINTER(EnvOut), C.c_void_p]),
     'pb_env_step': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(EnvOut), C.c_void_p]),
     'pb_env_episode_rows': (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                       C.POINTER(C.c_void_p)]),
     'pb_env_stats_read': (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_int, C.c_void_p]),
+    'pb_env_agent_stats_read': (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_int, C.c_void_p]),
     'pb_rollout_store': (C.c_int, [C.c_void_p] * 6 + [C.c_int64, C.c_void_p]),
     'pb_copy_rows': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]),
     'pb_gae_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int64]),

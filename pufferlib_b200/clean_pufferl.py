@@ -774,6 +774,17 @@ class _LazyIdxs:
         return self.n * self.h
 
 
+def unroll_nested_dict(d):
+    """pufferlib.utils.unroll_nested_dict (utils.py:56-65): nested info dicts as flat 'outer/inner' keys, e.g. a
+    multi-agent env's {1: {'score': 1}} as '1/score'; a flat dict unchanged."""
+    for k, v in d.items():
+        if isinstance(v, dict):
+            for k2, v2 in unroll_nested_dict(v):
+                yield f'{k}/{k2}', v2
+        else:
+            yield k, v
+
+
 def _set_lr(optimizer, lr):
     """The learning rate is a device tensor when the optimizer is capturable (graph replays read it in place)."""
     cur = optimizer.param_groups[0]['lr']
@@ -916,7 +927,7 @@ def _rollout_loop(data, infos):
                     vecenv.host_sync(actions_only=True)
                     info = []
             for i in info:
-                for k, v in i.items():
+                for k, v in unroll_nested_dict(i):
                     infos[k].append(v)
 
         with profile.env:

@@ -69,7 +69,7 @@ extern "C" int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_h
     PB_REQUIRE(n_dparam >= 0 && (n_dparam == 0 || dparam_host), PB_ERR_INVALID, "pb_env_create_ex: bad dparam");
     *out = nullptr;
     PB_REQUIRE(cfg->num_envs >= 1, PB_ERR_INVALID, "num_envs must be at least 1");  // vector.py:578-579
-    PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_BANDIT, PB_ERR_INVALID, "unknown env kind %d",
+    PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_MULTIAGENT, PB_ERR_INVALID, "unknown env kind %d",
                cfg->kind);
     int ndev = 0;
     PB_CUDA(cudaGetDeviceCount(&ndev));
@@ -79,6 +79,7 @@ extern "C" int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_h
     pb_env* env = (pb_env*)calloc(1, sizeof(pb_env));
     PB_REQUIRE(env, PB_ERR_CUDA, "out of host memory");
     env->cfg = *cfg;
+    env->agents_per_env = 1;
     int rc = pb_env_alloc_common(env);
     if (rc == PB_OK) {
         switch (cfg->kind) {
@@ -116,6 +117,12 @@ extern "C" int pb_env_destroy(pb_env* env) {
 extern "C" int pb_env_get_info(const pb_env* env, pb_env_info* out) {
     PB_REQUIRE(env && out, PB_ERR_INVALID, "pb_env_get_info: null pointer");
     *out = env->info;
+    return PB_OK;
+}
+
+extern "C" int pb_env_agents_per_env(const pb_env* env, int32_t* out) {
+    PB_REQUIRE(env && out, PB_ERR_INVALID, "pb_env_agents_per_env: null pointer");
+    *out = env->agents_per_env;
     return PB_OK;
 }
 
@@ -188,6 +195,21 @@ extern "C" int pb_env_stats_read(pb_env* env, double* out4_host, int clear, void
     for (int k = 0; k < 4; ++k) out4_host[k] = 0.0;
     for (int slot = 0; slot < PB_STAT_SLOTS; ++slot)
         for (int k = 0; k < 4; ++k) out4_host[k] += env->h_stats_pinned[slot * 4 + k];
+    return PB_OK;
+}
+
+extern "C" int pb_env_agent_stats_read(pb_env* env, double* out4_host, int clear, void* stream) {
+    PB_REQUIRE(env && out4_host, PB_ERR_INVALID, "pb_env_agent_stats_read: null pointer");
+    PB_REQUIRE(env->d_agent_stats, PB_ERR_INVALID, "pb_env_agent_stats_read: env kind %d has one agent per env",
+               env->cfg.kind);
+    cudaStream_t s = (cudaStream_t)stream;
+    PB_CUDA(cudaSetDevice(env->cfg.device));
+    const size_t bytes = 4 * sizeof(unsigned long long);
+    unsigned long long* h = (unsigned long long*)env->h_stats_pinned;   // 32 of its bytes
+    PB_CUDA(cudaMemcpyAsync(h, env->d_agent_stats, bytes, cudaMemcpyDeviceToHost, s));
+    if (clear) PB_CUDA(cudaMemsetAsync(env->d_agent_stats, 0, bytes, s));
+    PB_CUDA(cudaStreamSynchronize(s));
+    for (int k = 0; k < 4; ++k) out4_host[k] = (double)h[k];   // integer counts: exact below 2**53
     return PB_OK;
 }
 

@@ -38,6 +38,8 @@ struct pb_env {
     const void* const_trunc;
     const void* const_masks;
     bool write_const;
+    int32_t agents_per_env;  // A: every pb_env_out array has N*A rows (1 for the single-agent kinds)
+    unsigned long long* d_agent_stats;   // [4] multi-agent kinds: env steps, per-agent score sums (NULL otherwise)
     void* kind;              // kind-specific state
 };
 
@@ -48,7 +50,8 @@ int pb_squared_create(pb_env* env);
 int pb_breakout_create(pb_env* env);
 int pb_snake_create(pb_env* env);
 int pb_pong_create(pb_env* env);
-int pb_ocean_create(pb_env* env, const double* dparam, int n_dparam);   // memory, password, stochastic, bandit
+int pb_ocean_create(pb_env* env, const double* dparam, int n_dparam);   // memory, password, stochastic, bandit,
+                                                                         // multiagent
 
 struct EpisodeAcc {
     double* ep_return;

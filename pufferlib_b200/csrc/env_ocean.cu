@@ -1,6 +1,7 @@
-// env_ocean.cu -- the reference's ocean test envs Memory, Password, Stochastic and Bandit, N instances each behind
-// vector.Serial semantics, on the device (sm_90a).  Each env probes one learning ability: recall (memory),
-// exploration (password), a stochastic optimum (stochastic), credit assignment under reward noise (bandit).
+// env_ocean.cu -- the reference's ocean test envs Memory, Password, Stochastic, Bandit and Multiagent, N instances
+// each behind vector.Serial semantics, on the device (sm_90a).  Each env probes one learning ability: recall (memory),
+// exploration (password), a stochastic optimum (stochastic), credit assignment under reward noise (bandit), one
+// policy serving two agents that need different actions (multiagent: two agent rows per env, see multiagent_step).
 //
 // Bit-exact restatement of (paths under reference pufferlib/):
 //   environments/ocean/ocean.py:64-123    Memory      (obs = digit on ticks < L else 0; reward for 0 on the
@@ -11,7 +12,10 @@
 //   environments/ocean/ocean.py:8-62      Bandit      (one-step episodes; (correct + randn*scale)*scale)
 //   environments/ocean/environment.py:33-46, 67-70   creator defaults: memory L=2 D=2, password 5, stochastic
 //                                                      p=0.7 horizon=100, bandit 10 arms scale 1 noise 1
+//   environments/ocean/ocean.py:149-208   Multiagent  (agent 1 rewarded for action 0, agent 2 for action 1; every
+//                                                      step terminal for both, so every second send resets)
 //   postprocess.py:8-54 EpisodeStats, emulation.py:169-228 buffer rows, vector.py:112-156 Serial
+//   postprocess.py:147-179 MultiagentEpisodeStats (per-agent infos only), emulation.py:236-420 PettingZooPufferEnv
 //
 // RNG parity (numpy's legacy process-global np.random, MT19937 seeded by init_genrand):
 //   memory     async_reset seeds env i with seed+i and draws 2L+D digits (randint(0, 2) = genrand & 1); every later
@@ -62,6 +66,7 @@ struct OceanState {
     double* d_gauss;             // [N] bandit: G[j]
     double* d_prox;              // [101*102/2] stochastic: 1 - (p - c/t)**2 at t*(t+1)/2 + c
     double* d_score64;           // [N] fp64 episode score
+    unsigned long long* d_agent_stats;   // [4] multiagent: env steps, agent 1 / agent 2 score sums, 0
 };
 
 // -- memory RNG -------------------------------------------------------------------------------------------------
@@ -163,12 +168,55 @@ struct OcOut {
     bool write_const;
 };
 
+// Multiagent behind PettingZooPufferEnv: env e owns agent rows 2e (agent 1) and 2e + 1 (agent 2).  Every step ends
+// with both agents terminal (ocean.py:163-166, returned unchanged by step), so all_done holds and the next send
+// resets: sends alternate between reset rows and step rows.  One lane per env; the caller's warp is whole.
+template <int MODE>
+__device__ __forceinline__ void multiagent_step(const OceanState& st, int e, bool active,
+                                                const int64_t* __restrict__ actions, uint8_t* done, const OcOut& out) {
+    const bool step = active && MODE == 1 && !done[e];   // done[e]: all agents' previous rows were terminal
+    bool r0 = false, r1 = false;
+    if (active) {
+        if (step) {            // ocean.py:186-208: agent 1 is rewarded for action 0, agent 2 for action 1
+            const int64_t a0 = actions[2 * (int64_t)e], a1 = actions[2 * (int64_t)e + 1];
+            r0 = a0 <= 0;      // clamped into [0, 2) like every kind's actions
+            r1 = a1 >= 1;
+        }
+        const int64_t row = 2 * (int64_t)e;
+        // the observation is the constant dict {1: [0], 2: [1]}; written on every send because a bound rollout gives
+        // every send fresh rows (emulation.py:340-345 reset rows, 395-406 step rows)
+        *(float*)(out.obs + row * out.obs_stride) = 0.f;
+        *(float*)(out.obs + (row + 1) * out.obs_stride) = 1.f;
+        out.rewards[row] = r0 ? 1.f : 0.f;
+        out.rewards[row + 1] = r1 ? 1.f : 0.f;
+        out.terminals[row] = out.terminals[row + 1] = step ? 1 : 0;
+        if (out.write_const) {
+            out.truncations[row] = out.truncations[row + 1] = 0;
+            out.masks[row] = out.masks[row + 1] = 1;
+        }
+        if (out.dones_f32) out.dones_f32[row] = out.dones_f32[row + 1] = step ? 1.f : 0.f;
+        done[e] = step ? 1 : 0;
+    }
+    // per-agent statistics (the score info of each agent equals its reward): one integer atomic per warp and quantity
+    const unsigned m = __ballot_sync(0xffffffffu, step);
+    const unsigned s0 = __ballot_sync(0xffffffffu, r0), s1 = __ballot_sync(0xffffffffu, r1);
+    if (m && (threadIdx.x & 31) == 0) {
+        atomicAdd(st.d_agent_stats + 0, (unsigned long long)__popc(m));
+        if (s0) atomicAdd(st.d_agent_stats + 1, (unsigned long long)__popc(s0));
+        if (s1) atomicAdd(st.d_agent_stats + 2, (unsigned long long)__popc(s1));
+    }
+}
+
 // mode 0: write reset rows for every env (after async_reset); mode 1: vectoriser send (reset-or-step)
 template <int KIND, int MODE>
 __global__ void __launch_bounds__(128) k_ocean_step(OceanState st, int n, const int64_t* __restrict__ actions,
                                                    uint8_t* done, OcOut out, EpisodeAcc acc) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     const bool active = e < n;
+    if constexpr (KIND == PB_ENV_MULTIAGENT) {
+        multiagent_step<MODE>(st, e, active, actions, done, out);   // no EpisodeStats (postprocess.py:147-179)
+        return;
+    }
     float reward = 0.f;
     double reward_d = 0.0, score = 0.0;
     bool terminal = false, reset_row = true;
@@ -297,6 +345,7 @@ int ocean_launch(pb_env* env, int mode, const int64_t* actions, const pb_env_out
         case PB_ENV_MEMORY: launch_kind<PB_ENV_MEMORY>(*st, mode, n, actions, env->d_done, o, acc, s); break;
         case PB_ENV_PASSWORD: launch_kind<PB_ENV_PASSWORD>(*st, mode, n, actions, env->d_done, o, acc, s); break;
         case PB_ENV_STOCHASTIC: launch_kind<PB_ENV_STOCHASTIC>(*st, mode, n, actions, env->d_done, o, acc, s); break;
+        case PB_ENV_MULTIAGENT: launch_kind<PB_ENV_MULTIAGENT>(*st, mode, n, actions, env->d_done, o, acc, s); break;
         default: launch_kind<PB_ENV_BANDIT>(*st, mode, n, actions, env->d_done, o, acc, s); break;
     }
     PB_LAUNCH_CHECK();
@@ -334,7 +383,9 @@ void ocean_destroy(pb_env* env) {
     if (!st) return;
     cudaFree(st->d_tick); cudaFree(st->d_bits); cudaFree(st->d_guess); cudaFree(st->d_mt); cudaFree(st->d_rank);
     cudaFree(st->d_digits); cudaFree(st->d_gauss); cudaFree(st->d_prox); cudaFree(st->d_score64);
+    cudaFree(st->d_agent_stats);
     env->d_row_score64 = nullptr;
+    env->d_agent_stats = nullptr;
     delete st;
     env->kind = nullptr;
 }
@@ -392,6 +443,15 @@ int pb_ocean_create(pb_env* env, const double* dparam, int n_dparam) {
         PB_CUDA(cudaMalloc(&st->d_prox, prox.size() * sizeof(double)));
         PB_CUDA(cudaMemcpy(st->d_prox, prox.data(), prox.size() * sizeof(double), cudaMemcpyHostToDevice));
         lo = 0.f;
+    } else if (kind == PB_ENV_MULTIAGENT) {   // make_multiagent() takes no arguments (environment.py:69-72)
+        for (int k = 0; k < 8; ++k)
+            PB_REQUIRE(ip[k] == 0, PB_ERR_INVALID, "multiagent: takes no parameters (iparam[%d] = %d)", k, ip[k]);
+        PB_REQUIRE(n_dparam == 0, PB_ERR_INVALID, "multiagent: takes no parameters (%d dparam given)", n_dparam);
+        env->agents_per_env = 2;
+        PB_CUDA(cudaMalloc(&st->d_agent_stats, 4 * sizeof(unsigned long long)));
+        PB_CUDA(cudaMemset(st->d_agent_stats, 0, 4 * sizeof(unsigned long long)));
+        env->d_agent_stats = st->d_agent_stats;
+        lo = 0.f;              // Box(0, 1, (1,)) for both agents (ocean.py:171-173)
     } else {
         st->n_act = ip[0] > 0 ? ip[0] : 10;
         st->scale = dp(0, 1.0);
@@ -409,13 +469,15 @@ int pb_ocean_create(pb_env* env, const double* dparam, int n_dparam) {
         cudaFree(d_sol);
         PB_CUDA(err);
     }
-    if (kind != PB_ENV_BANDIT) {
-        PB_CUDA(cudaMalloc(&st->d_tick, n * sizeof(uint32_t)));
-        PB_CUDA(cudaMemset(st->d_tick, 0, n * sizeof(uint32_t)));
+    if (kind != PB_ENV_MULTIAGENT) {   // multiagent keeps no state but the per-env done flag
+        if (kind != PB_ENV_BANDIT) {
+            PB_CUDA(cudaMalloc(&st->d_tick, n * sizeof(uint32_t)));
+            PB_CUDA(cudaMemset(st->d_tick, 0, n * sizeof(uint32_t)));
+        }
+        PB_CUDA(cudaMalloc(&st->d_score64, n * sizeof(double)));
+        PB_CUDA(cudaMemset(st->d_score64, 0, n * sizeof(double)));
+        env->d_row_score64 = st->d_score64;
     }
-    PB_CUDA(cudaMalloc(&st->d_score64, n * sizeof(double)));
-    PB_CUDA(cudaMemset(st->d_score64, 0, n * sizeof(double)));
-    env->d_row_score64 = st->d_score64;
     env->info.obs_dtype = PB_DTYPE_F32;
     env->info.obs_ndim = 1;
     env->info.obs_shape[0] = obs_len;

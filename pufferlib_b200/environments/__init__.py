@@ -5,6 +5,9 @@ The reference passes ``env_creator`` callables to ``vector.make`` and the backen
 device-resident multi-env (the PufferEnv seam, pufferlib/environment.py:1-21).  A creator is recognised by a
 ``b200_kind`` attribute (ours) or by name for the reference's own ``make_squared``, ``make_memory``, ...
 (pufferlib/environments/ocean/environment.py:28-72), so the reference's creator can be passed unchanged.
+
+A kind may have several agents per env (multiagent: two); the backend reads that number from the library
+(pb_env_agents_per_env) and sizes every row buffer by agents, as the reference's vectorisers do (vector.py:85-92).
 """
 import math
 import operator
@@ -13,7 +16,7 @@ from pufferlib_b200.exceptions import APIUsageError
 
 KNOWN_BY_NAME = {'make_squared': 'squared', 'make_breakout': 'breakout', 'make_snake': 'snake', 'make_pong': 'pong',
                  'make_memory': 'memory', 'make_password': 'password', 'make_stochastic': 'stochastic',
-                 'make_bandit': 'bandit'}
+                 'make_bandit': 'bandit', 'make_multiagent': 'multiagent'}
 
 # Kinds whose reference env draws from a process-global RNG stream (CPython's `random` for squared, numpy's
 # `np.random` for memory and bandit): their results depend on which envs share a process, so the B200 backend gives
@@ -92,6 +95,9 @@ def resolve_config(creator, args, kwargs):
     elif kind == 'pong':
         iparam[0] = int(kwargs.pop('max_score', 0))
         iparam[1] = int(kwargs.pop('max_ticks', 0))
+    elif kind == 'multiagent':
+        if args or kwargs:      # make_multiagent() takes no arguments (ocean/environment.py:69-72)
+            raise APIUsageError(f'multiagent: takes no arguments, got args {list(args or ())} kwargs {sorted(kwargs)}')
     elif kind in OCEAN_PARAMS:
         v = _ocean_values(kind, args, kwargs)
         if kind == 'memory':

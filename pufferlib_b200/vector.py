@@ -103,7 +103,7 @@ class _DriverEnv:
         self.observation_space = vec.single_observation_space
         self.action_space = vec.single_action_space
         self.emulated = vec.emulated
-        self.num_agents = 1
+        self.num_agents = vec.agents_per_env     # PettingZooPufferEnv.num_agents (emulation.py:262); 1 for Gymnasium envs
         self.render_mode = 'ansi'
         self._vec = vec
 
@@ -176,6 +176,13 @@ class B200:
         self._handle = self._shards[0][0]
         info = _native.EnvInfo()
         _native.check(lib.pb_env_get_info(self._handle, C.byref(info)))
+        # A agents per env (2 for multiagent): every row buffer, the actions and agent_ids count the N*A agents, agent a of
+        # env e at row e*A + a (Serial._assign_buffers, vector.py:97-110); seeds and shards still count envs
+        agents = C.c_int32()
+        _native.check(lib.pb_env_agents_per_env(self._handle, C.byref(agents)))
+        self.agents_per_env = int(agents.value)
+        self._envs = num_envs
+        rows = num_envs * self.agents_per_env
         self.obs_bytes = int(info.obs_bytes)
         self._obs_torch_dtype = _TORCH_DTYPES[info.obs_dtype]
         obs_shape = tuple(info.obs_shape[i] for i in range(info.obs_ndim))
@@ -184,24 +191,24 @@ class B200:
         self.single_action_space = spaces.Discrete(info.num_actions)
         self.emulated = namespace(observation_dtype=self.single_observation_space.dtype,
                                   emulated_observation_dtype=self.single_observation_space.dtype)
-        self.agents_per_batch = num_envs
-        self.num_agents = num_envs
-        self.action_space = joint_space(self.single_action_space, num_envs)
-        self.observation_space = joint_space(self.single_observation_space, num_envs)
-        self.agent_ids = np.arange(num_envs)
+        self.agents_per_batch = rows
+        self.num_agents = rows
+        self.action_space = joint_space(self.single_action_space, rows)
+        self.observation_space = joint_space(self.single_observation_space, rows)
+        self.agent_ids = np.arange(rows)
         self.initialized = False
         self.flag = RESET
         self.infos = []
         with torch.cuda.device(self.device):
             self.buf = namespace(
-                observations=torch.zeros((num_envs, *obs_shape), dtype=self._obs_torch_dtype, device=self.device),
-                rewards=torch.zeros(num_envs, dtype=torch.float32, device=self.device),
-                terminals=torch.zeros(num_envs, dtype=torch.bool, device=self.device),
-                truncations=torch.zeros(num_envs, dtype=torch.bool, device=self.device),
-                masks=torch.ones(num_envs, dtype=torch.bool, device=self.device),
-                dones_f32=torch.zeros(num_envs, dtype=torch.float32, device=self.device),
+                observations=torch.zeros((rows, *obs_shape), dtype=self._obs_torch_dtype, device=self.device),
+                rewards=torch.zeros(rows, dtype=torch.float32, device=self.device),
+                terminals=torch.zeros(rows, dtype=torch.bool, device=self.device),
+                truncations=torch.zeros(rows, dtype=torch.bool, device=self.device),
+                masks=torch.ones(rows, dtype=torch.bool, device=self.device),
+                dones_f32=torch.zeros(rows, dtype=torch.float32, device=self.device),
             )
-            self._actions_dev = torch.zeros(num_envs, dtype=torch.int64, device=self.device)
+            self._actions_dev = torch.zeros(rows, dtype=torch.int64, device=self.device)
         self.driver_env = _DriverEnv(self)
         # rollout binding (clean_pufferl.create): step outputs go straight into Experience rows
         self._rollout = None
@@ -209,12 +216,12 @@ class B200:
         self._pending_own = True    # latest step output lives in self.buf (not yet in a rollout row)
         if self.host_buffers:
             self._host = namespace(
-                observations=torch.zeros((num_envs, *obs_shape), dtype=self._obs_torch_dtype).pin_memory(),
-                rewards=torch.zeros(num_envs, dtype=torch.float32).pin_memory(),
-                terminals=torch.zeros(num_envs, dtype=torch.bool).pin_memory(),
-                truncations=torch.zeros(num_envs, dtype=torch.bool).pin_memory(),
-                masks=torch.ones(num_envs, dtype=torch.bool).pin_memory(),
-                actions=torch.zeros(num_envs, dtype=torch.int64).pin_memory(),
+                observations=torch.zeros((rows, *obs_shape), dtype=self._obs_torch_dtype).pin_memory(),
+                rewards=torch.zeros(rows, dtype=torch.float32).pin_memory(),
+                terminals=torch.zeros(rows, dtype=torch.bool).pin_memory(),
+                truncations=torch.zeros(rows, dtype=torch.bool).pin_memory(),
+                masks=torch.ones(rows, dtype=torch.bool).pin_memory(),
+                actions=torch.zeros(rows, dtype=torch.int64).pin_memory(),
             )
             self._host_np = namespace(**{k: v.numpy() for k, v in self._host.items()})
             with torch.cuda.device(self.device):
@@ -241,6 +248,7 @@ class B200:
         """pb_env_out for rollout row `row`, or for the vecenv's own buffers when row is None; `lo` = first env of the
         shard the outputs belong to."""
         b = self.buf
+        lo *= self.agents_per_env     # its first agent row
         if row is None:
             return _native.EnvOut(obs=b.observations.data_ptr() + lo * self.obs_bytes, obs_stride=self.obs_bytes,
                                   rewards=b.rewards.data_ptr() + lo * 4, terminals=b.terminals.data_ptr() + lo,
@@ -258,7 +266,7 @@ class B200:
             # list form of make_seeds (vector.py:639-650) -- what Multiprocessing hands each worker is the slice
             # [seed + lo, ..., seed + hi - 1] (:424-428).  Env i is seeded with seed + i on the device, so a list is
             # accepted when it is such a run of consecutive integers; arbitrary per-env seeds have no device form.
-            seeds = make_seeds(seed, self.num_agents)
+            seeds = make_seeds(seed, self._envs)
             if not all(isinstance(x, (int, np.integer)) for x in seeds) or \
                     any(int(seeds[i]) != int(seeds[0]) + i for i in range(len(seeds))):
                 raise APIUsageError(f'seed {seed} must be an integer or a list of consecutive integers')
@@ -294,8 +302,8 @@ class B200:
                 row = self._cursor + 1
             for handle, lo, _ in self._shards:
                 out = self._env_out(row, lo)
-                _native.check(_native.lib().pb_env_step(handle, C.c_void_p(a.data_ptr() + 8 * lo), C.byref(out),
-                                                        _native.stream_ptr()))
+                a_shard = C.c_void_p(a.data_ptr() + 8 * lo * self.agents_per_env)     # the shard's first agent row
+                _native.check(_native.lib().pb_env_step(handle, a_shard, C.byref(out), _native.stream_ptr()))
             if self._rollout is not None:
                 if row is None:
                     self._pending_own = True
@@ -343,7 +351,7 @@ class B200:
                                    + 4 * self.num_agents + 2 * self.num_agents)
                 self._device_view = (obs, rewards, b.terminals, b.truncations, [], self.agent_ids, b.masks)
                 return self.host_sync() if not _device else self._device_view
-            infos = self._collect_infos() if self.exact_infos else []
+            infos = self._collect_infos(rewards=rewards) if self.exact_infos else []
             self.infos = infos
         return (obs, rewards, b.terminals, b.truncations, infos, self.agent_ids, b.masks)
 
@@ -402,7 +410,7 @@ class B200:
                 self._act_pending = False
         hn = self._host_np
         # the terminal flags are on the host already: no second D2H for the info dicts
-        infos = self._collect_infos(hn.terminals) if self.exact_infos else []
+        infos = self._collect_infos(hn.terminals, hn.rewards) if self.exact_infos else []
         self.infos = infos
         return (hn.observations, hn.rewards, hn.terminals, hn.truncations, infos, self.agent_ids, hn.masks)
 
@@ -449,10 +457,12 @@ class B200:
                 return self._host[k]
         return torch.as_tensor(array)
 
-    def _collect_infos(self, term=None):
+    def _collect_infos(self, term=None, rewards=None):
         """Per-env info dicts for rows that just ended an episode (EpisodeStats, postprocess.py:36-52), in env
         order like Serial.send (vector.py:153-154).  Costs one D2H of the terminal flags per recv unless the caller
-        already has them on the host (``term``)."""
+        already has them on the host (``term``).  ``rewards``: this step's reward rows (read by the multi-agent kinds)."""
+        if self.agents_per_env > 1:
+            return self._collect_agent_infos(term, rewards)
         if term is None:
             term = self.buf.terminals.cpu().numpy()
             self.d2h_bytes += term.nbytes
@@ -490,10 +500,41 @@ class B200:
         return [{'episode_return': float(ret[i]), 'episode_length': int(length[i]), 'score': float(score[i])}
                 for i in idx]
 
+    def _collect_agent_infos(self, term, rewards):
+        """Multi-agent kinds: for every env whose rows are terminal after this send, in env order, the env's own step
+        info {1: {'score': r1}, 2: {'score': r2}} with python ints (ocean.py:201-204; MultiagentEpisodeStats passes it
+        through unchanged, postprocess.py:147-179).  An agent's score is its reward on that row, so the dicts are built
+        from the reward and terminal rows; a reset-send yields none.  Without ``term`` both rows come to the host in one
+        device->host copy."""
+        n, a_per = self.num_agents, self.agents_per_env
+        if term is None:
+            stage = torch.empty(5 * n, dtype=torch.uint8, device=self.buf.terminals.device)
+            stage[:4 * n].view(torch.float32).copy_(rewards)
+            stage[4 * n:].copy_(self.buf.terminals.view(torch.uint8))
+            host = stage.cpu().numpy()
+            rewards, term = host[:4 * n].view(np.float32), host[4 * n:].view(np.bool_)
+            self.d2h_bytes += 5 * n
+        ended = np.asarray(term).reshape(-1, a_per).all(axis=1)
+        r = np.asarray(rewards).reshape(-1, a_per)
+        return [{a + 1: {'score': int(r[e, a])} for a in range(a_per)} for e in np.nonzero(ended)[0]]
+
     def episode_stats(self, clear=True):
         """Device-side EpisodeStats reduction: {episode_return, episode_length, score} means over the episodes
-        finished since the last call, plus their count (one 32-byte D2H)."""
+        finished since the last call, plus their count (one 32-byte D2H).  Multi-agent kinds: {'1/score', '2/score'}
+        means over the env steps since the last call (the keys the reference's evaluate builds from the per-agent infos
+        with unroll_nested_dict, clean_pufferl.py:119-121), plus that count."""
         out = [0.0] * 4
+        if self.agents_per_env > 1:
+            with torch.cuda.device(self.device):
+                for handle, _, _ in self._shards:
+                    part = (C.c_double * 4)()
+                    _native.check(_native.lib().pb_env_agent_stats_read(handle, part, int(clear), _native.stream_ptr()))
+                    out = [a + b for a, b in zip(out, part)]
+                    self.d2h_bytes += 32
+            cnt = out[0]
+            if cnt <= 0:
+                return {}, 0
+            return {f'{a + 1}/score': out[1 + a] / cnt for a in range(self.agents_per_env)}, int(cnt)
         with torch.cuda.device(self.device):
             for handle, _, _ in self._shards:
                 part = (C.c_double * 4)()
@@ -557,10 +598,12 @@ class B200Pool:
         self.host_buffers, self.exact_infos = first.host_buffers, first.exact_infos
         self.single_observation_space, self.single_action_space = first.single_observation_space, first.single_action_space
         self.emulated, self.driver_env, self.obs_bytes = first.emulated, first.driver_env, first.obs_bytes
-        self.agents_per_batch, self.num_agents = b, num_envs
+        # batch_size counts envs (vector.py:258-259): a group returns b * A agent rows
+        self.agents_per_env = a_per = first.agents_per_env
+        self.agents_per_batch, self.num_agents = b * a_per, num_envs * a_per
         self.action_space, self.observation_space = first.action_space, first.observation_space
-        self.agent_ids = np.arange(num_envs)
-        self._ids = [np.arange(i * b, (i + 1) * b) for i in range(g)]
+        self.agent_ids = np.arange(num_envs * a_per)
+        self._ids = [np.arange(i * b * a_per, (i + 1) * b * a_per) for i in range(g)]
         self.initialized = False
         self.flag = RESET
         self.infos = []

@@ -191,7 +191,8 @@ int pb_gae(const float* rewards, const float* values, const float* dones, float*
  * (pb_gae_time_major_supported). */
 int pb_gae_time_major_supported(int64_t num_envs, int64_t horizon);
 /* Tile-kernel variant for A/B measurements: 0 (default) chosen by horizon, 2 double-buffered tiles + coalesced outputs,
- * 3 single-buffered tiles, 1 the kernel of round 1.  Results are bit-identical. */
+ * 3 single-buffered tiles, 1 the kernel of round 1.  The variants share the element maps and the scan; results agree
+ * up to the order in which the tile look-back composes, which depends on timing (1e-6 in practice). */
 int pb_gae_set_variant(int32_t variant);
 int pb_gae_tm(const float* rewards, const float* values, const float* dones, float* advantages, float* returns_sorted,
               float* advantages_time_major, int64_t num_envs, int64_t horizon, float gamma, float gae_lambda,

@@ -19,6 +19,8 @@
 // HBM traffic = 12 B read + 4 (or 8 with returns) B written per agent-step.
 #include <stdlib.h>
 
+#include <algorithm>
+
 #include "pb_common.cuh"
 
 namespace {
@@ -41,7 +43,7 @@ struct GaeParams {
     const float* d;
     float* adv;
     float* ret;
-    float* adv_tm;     // optional: advantages in arrival (time-major) order [H][N] as well (fast path only)
+    float* adv_tm;     // optional: advantages in arrival (time-major) order [H][N] as well (32-env tile kernels only)
     int64_t N, H, B;
     float gamma, gl;
     int E, logE;       // envs per tile (power of two) or 0 in flat mode
@@ -73,6 +75,13 @@ __device__ __forceinline__ void compose(float& a, float& b, float a2, float b2) 
     // (a,b) o (a2,b2): first apply the later map (a2,b2), then this one
     a = fmaf(b, a2, a);
     b = b * b2;
+}
+
+// The map (a_f, b_f) of one element from its own value v0 and the step after it (r1, v1, d1).  c_gae.pyx:28-29
+// association, no FMA contraction inside an element.  The caller applies A[B-1] = 0.
+__device__ __forceinline__ float2 element_map(float r1, float v1, float d1, float v0, float gamma, float gl) {
+    const float nnt = __fsub_rn(1.0f, d1);
+    return make_float2(__fsub_rn(__fadd_rn(r1, __fmul_rn(__fmul_rn(gamma, v1), nnt)), v0), __fmul_rn(gl, nnt));
 }
 
 __device__ __forceinline__ float tile_lookback(GaeStatus* st, int tile, int numTiles, float tP, float tQ, int lane) {
@@ -119,8 +128,31 @@ __device__ __forceinline__ float tile_lookback(GaeStatus* st, int tile, int numT
     return carry;
 }
 
+// Self-cleaning workspace: the last block to leave zeroes the header and every status word, so the next call finds
+// the workspace as the caller first zero-filled it.  `s_flag` is any shared int the block no longer needs.
+template <int THREADS>
+__device__ __forceinline__ void release_workspace(const GaeParams& p, int* s_flag) {
+    const int tid = threadIdx.x;
+    if (tid == 0) {
+        __threadfence();
+        const uint32_t prev = atomicAdd(&p.hdr->exited, 1u);
+        *s_flag = (prev == gridDim.x - 1u) ? 1 : 0;
+    }
+    __syncthreads();
+    if (*s_flag) {
+        for (int j = tid; j < p.numTiles; j += THREADS) {
+            p.status[j].P = 0.f; p.status[j].Q = 0.f; p.status[j].X = 0.f; p.status[j].flag = 0u;
+        }
+        if (tid == 0) { p.hdr->ticket = 0u; p.hdr->exited = 0u; }
+    }
+}
+
 __device__ __forceinline__ void cp_async4(float* dst_smem, const float* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src)
+                 : "memory");
+}
+__device__ __forceinline__ void cp_async16(float* dst_smem, const float* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src)
                  : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
@@ -264,11 +296,9 @@ __global__ void __launch_bounds__(GAE_THREADS) k_gae(GaeParams p) {
                 } else {
                     r1 = halo[0]; v1 = halo[1]; d1 = halo[2];
                 }
-                const float v0 = sV[sp0];
-                const float nnt = __fsub_rn(1.0f, d1);
-                // c_gae.pyx:28-29 association, no FMA contraction inside an element
-                a[k] = __fsub_rn(__fadd_rn(r1, __fmul_rn(__fmul_rn(p.gamma, v1), nnt)), v0);
-                b[k] = __fmul_rn(p.gl, nnt);
+                const float2 m = element_map(r1, v1, d1, sV[sp0], p.gamma, p.gl);
+                a[k] = m.x;
+                b[k] = m.y;
                 if (f0 + i == p.B - 1) {  // A[B-1] = 0
                     a[k] = 0.f;
                     b[k] = 0.f;
@@ -338,43 +368,137 @@ __global__ void __launch_bounds__(GAE_THREADS) k_gae(GaeParams p) {
         ticket = next_ticket;
         cur ^= 1;
     }
-
-    // ---- self-cleaning workspace: the last block to leave zeroes the header and every status word
-    if (tid == 0) {
-        __threadfence();
-        const uint32_t prev = atomicAdd(&p.hdr->exited, 1u);
-        s_ticket[0] = (prev == gridDim.x - 1u) ? 1 : 0;
-    }
-    __syncthreads();
-    if (s_ticket[0]) {
-        for (int j = tid; j < p.numTiles; j += GAE_THREADS) {
-            p.status[j].P = 0.f; p.status[j].Q = 0.f; p.status[j].X = 0.f; p.status[j].flag = 0u;
-        }
-        if (tid == 0) { p.hdr->ticket = 0u; p.hdr->exited = 0u; }
-    }
+    release_workspace<GAE_THREADS>(p, s_ticket);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Fast path (N > 1, N % 4 == 0, H in {128, 256, 512}): tile = 32 whole envs, 256 threads.
-//   * loads: every time row of the tile is one 128-byte run (32 envs), copied global->shared with 16-byte cp.async
-//     (LDGSTS.128): 12*KC async copies per thread, no register staging, no transposition -- shared layout is [t][32];
-//   * pass 1: thread (env = lane, chunk) composes its 16 consecutive steps SERIALLY in registers (2 FMAs per element
-//     instead of a 5-step shuffle scan); a warp's 32 lanes read 32 consecutive floats: conflict-free;
-//   * pass 2 (one warp): chunk carries inside each env, a 5-step shuffle suffix over the 32 env aggregates, then the
-//     decoupled look-back; pass 3: apply carries, 64 B of output per thread-chunk.
-// ~40 thread-instructions per element instead of ~180 for the generic kernel.
+// 32-env tile kernels (N > 1, N % 4 == 0, H in {128, 256, 512}): tile = 32 whole envs, one warp per 16-step chunk
+// slot.  Both kernels are built from the same blocks and do the same arithmetic:
+//   * loads (load_env_tile): every time row of the tile is one 128-byte run (32 envs), copied global->shared with
+//     16-byte cp.async (LDGSTS.128), no register staging, no transposition -- shared layout is [t][32];
+//   * pass 1 (scan_chunks): thread (env = lane, chunk) composes its 16 consecutive steps SERIALLY in registers (2 FMAs
+//     per element instead of a 5-step shuffle scan); a warp's 32 lanes read 32 consecutive floats: conflict-free;
+//   * pass 2 (scan_tile, one warp): chunk carries inside each env, a 5-step shuffle suffix over the 32 env aggregates,
+//     then the decoupled look-back;
+//   * pass 3: apply the carries to each chunk's maps and store the outputs -- the part in which the kernels differ.
+// ~40 thread-instructions per element instead of ~180 for k_gae.
 constexpr int FE = 32;            // envs per tile
 constexpr int FC = 16;            // steps per chunk
-constexpr int FAST_THREADS = 256; // 32 envs x 8 chunk slots
+constexpr int FAST_THREADS = 256; // k_gae_fast: 32 envs x 8 chunk slots
 
-__device__ __forceinline__ void cp_async16(float* dst_smem, const float* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src)
-                 : "memory");
+// Async loads of the tile of envs [e0, e0 + Et) (Et % 4 == 0): time row t = floats [t*N + e0, +Et) goes to row t of
+// [H][32], THREADS / 8 rows per sweep.  `halo` gets the element after the tile.  The caller commits the group.
+template <int H, int THREADS>
+__device__ __forceinline__ void load_env_tile(const GaeParams& p, int64_t e0, int Et, float* sR, float* sV, float* sD,
+                                              float* halo) {
+    const int tid = threadIdx.x;
+    const int quad = tid & 7, t0 = tid >> 3;         // 8 float4 per row, THREADS / 8 rows per sweep
+    if (4 * quad < Et) {
+        const int64_t g0 = (int64_t)t0 * p.N + e0 + 4 * quad;
+        const int64_t gstep = (int64_t)(THREADS / 8) * p.N;
+        const float* pr = p.r + g0;
+        const float* pv = p.v + g0;
+        const float* pd = p.d + g0;
+        int sp = t0 * FE + 4 * quad;
+#pragma unroll
+        for (int k = 0; k < H / (THREADS / 8); ++k) {
+            cp_async16(sR + sp, pr);
+            cp_async16(sV + sp, pv);
+            cp_async16(sD + sp, pd);
+            pr += gstep; pv += gstep; pd += gstep;
+            sp += (THREADS / 8) * FE;
+        }
+    }
+    if (tid == 0) {
+        const int64_t en = e0 + Et;                  // first env after the tile; its t = 0 row entry
+        if (en < p.N) {
+            cp_async4(halo + 0, p.r + en);
+            cp_async4(halo + 1, p.v + en);
+            cp_async4(halo + 2, p.d + en);
+        } else {
+            halo[0] = 0.f; halo[1] = 0.f; halo[2] = 1.f;
+        }
+    }
 }
 
+// Pass 1: chunk c = warp + kc * NW of env `lane`, composed serially in suffix order.  The element maps stay in a / b,
+// the chunk aggregate goes to s_cagg[c][lane]; lanes past the tile's Et envs hold identity maps.
+template <int KC, int NW>
+__device__ __forceinline__ void scan_chunks(const GaeParams& p, const float* sR, const float* sV, const float* sD,
+                                            const float* halo, int64_t e0, int Et, float (&a)[KC][FC],
+                                            float (&b)[KC][FC], float2 (*s_cagg)[FE]) {
+    constexpr int CE = NW * KC;                         // chunks per env
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+    for (int kc = 0; kc < KC; ++kc) {
+        const int c = warp + kc * NW;                   // chunk index; env = lane
+        float P = 0.f, Q = 1.f;
+        if (lane < Et) {
+            const int base = c * FC * FE + lane;
+            // the element after the chunk: next step of the env, next env's first step, or the tile halo
+            float rn, vn, dn;
+            if (c < CE - 1) { rn = sR[base + FC * FE]; vn = sV[base + FC * FE]; dn = sD[base + FC * FE]; }
+            else if (lane + 1 < Et) { rn = sR[lane + 1]; vn = sV[lane + 1]; dn = sD[lane + 1]; }
+            else { rn = halo[0]; vn = halo[1]; dn = halo[2]; }
+            const bool last_of_batch = (e0 + lane == p.N - 1) && (c == CE - 1);
+#pragma unroll
+            for (int j = FC - 1; j >= 0; --j) {
+                const float r0 = sR[base + j * FE], v0 = sV[base + j * FE], d0 = sD[base + j * FE];
+                const float2 m = element_map(rn, vn, dn, v0, p.gamma, p.gl);
+                float aj = m.x, bj = m.y;
+                if (last_of_batch && j == FC - 1) { aj = 0.f; bj = 0.f; }   // A[B-1] = 0
+                a[kc][j] = aj;
+                b[kc][j] = bj;
+                P = fmaf(bj, P, aj);     // (aj,bj) o (P,Q)
+                Q = bj * Q;
+                rn = r0; vn = v0; dn = d0;
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < FC; ++j) { a[kc][j] = 0.f; b[kc][j] = 1.f; }
+        }
+        s_cagg[c][lane] = make_float2(P, Q);
+    }
+}
+
+// Pass 2 (warp 0): s_cagg becomes each chunk's carry map w.r.t. its env's right end, s_eagg each env's carry map
+// w.r.t. the tile's right end; then the look-back, whose carry (A just after the tile) goes to s_carry.
+template <int CE>
+__device__ __forceinline__ void scan_tile(const GaeParams& p, int tile, float2 (*s_cagg)[FE], float2* s_eagg,
+                                          float* s_carry) {
+    const int lane = (int)threadIdx.x & 31;
+    float cP = 0.f, cQ = 1.f;                    // composition of the chunks to the right, w.r.t. the env end
+#pragma unroll
+    for (int c = CE - 1; c >= 0; --c) {
+        const float2 g = s_cagg[c][lane];
+        s_cagg[c][lane] = make_float2(cP, cQ);   // carry map entering chunk c from the right
+        const float nP = fmaf(g.y, cP, g.x), nQ = g.y * cQ;
+        cP = nP; cQ = nQ;
+    }
+    // inclusive suffix over the 32 env aggregates (missing envs are the identity)
+    float x = cP, y = cQ;
+#pragma unroll
+    for (int off = 1; off < FE; off <<= 1) {
+        const float x2 = __shfl_down_sync(0xffffffffu, x, off);
+        const float y2 = __shfl_down_sync(0xffffffffu, y, off);
+        if (lane + off < FE) compose(x, y, x2, y2);
+    }
+    const float tP = __shfl_sync(0xffffffffu, x, 0), tQ = __shfl_sync(0xffffffffu, y, 0);
+    // exclusive: map from the tile's right end to env `lane`'s right end
+    float exP = __shfl_down_sync(0xffffffffu, x, 1), exQ = __shfl_down_sync(0xffffffffu, y, 1);
+    if (lane == FE - 1) { exP = 0.f; exQ = 1.f; }
+    s_eagg[lane] = make_float2(exP, exQ);
+    const float carry = tile_lookback(p.status, tile, p.numTiles, tP, tQ, lane);
+    if (lane == 0) *s_carry = carry;
+}
+
+// The round-1 kernel: 256 threads, one tile buffer.  The next ticket is claimed while the tile loads, and pass 3
+// stores straight from registers, 64 B per thread-chunk (full sectors).  The only form that writes sorted returns and
+// time-major advantages in one call: the time-major output is staged in the reward tile, which is dead after pass 1.
 template <int KC>   // chunks per thread: H = 128 * KC
 __global__ void __launch_bounds__(FAST_THREADS) k_gae_fast(GaeParams p) {
-    constexpr int H = 128 * KC;
+    constexpr int NW = FAST_THREADS / 32;
+    constexpr int H = FC * NW * KC;
     constexpr int CE = H / FC;                 // chunks per env
     constexpr int ARR = H * FE;                // floats per array
     extern __shared__ __align__(16) float smem[];   // {r, v, d} x [H][32]
@@ -398,104 +522,17 @@ __global__ void __launch_bounds__(FAST_THREADS) k_gae_fast(GaeParams p) {
         const int64_t e0 = (int64_t)tile * FE;
         const int Et = (int)min((int64_t)FE, p.N - e0);     // multiple of 4 (N % 4 == 0)
 
-        // ---- async loads: row t of the tile = floats [t*N + e0, +Et)
-        {
-            const int quad = tid & 7, t0 = tid >> 3;         // 8 float4 per row, 32 rows per sweep
-            if (4 * quad < Et) {
-                const int64_t g0 = (int64_t)t0 * p.N + e0 + 4 * quad;
-                const int64_t gstep = 32 * p.N;
-                const float* pr = p.r + g0;
-                const float* pv = p.v + g0;
-                const float* pd = p.d + g0;
-                int sp = t0 * FE + 4 * quad;
-#pragma unroll
-                for (int k = 0; k < H / 32; ++k) {
-                    cp_async16(sR + sp, pr);
-                    cp_async16(sV + sp, pv);
-                    cp_async16(sD + sp, pd);
-                    pr += gstep; pv += gstep; pd += gstep;
-                    sp += 32 * FE;
-                }
-            }
-            if (tid == 0) {
-                const int64_t en = e0 + Et;                  // first env after the tile; its t = 0 row entry
-                if (en < p.N) {
-                    cp_async4(&s_halo[0], p.r + en);
-                    cp_async4(&s_halo[1], p.v + en);
-                    cp_async4(&s_halo[2], p.d + en);
-                } else {
-                    s_halo[0] = 0.f; s_halo[1] = 0.f; s_halo[2] = 1.f;
-                }
-                // claim the next tile now; the value is only read at the end of this iteration (latency hidden)
-                s_ticket[1] = (int)atomicAdd(&p.hdr->ticket, 1u);
-            }
-            cp_async_commit();
-            cp_async_wait<0>();
-        }
+        load_env_tile<H, FAST_THREADS>(p, e0, Et, sR, sV, sD, s_halo);
+        // claim the next tile now; the value is only read at the end of this iteration (latency hidden)
+        if (tid == 0) s_ticket[1] = (int)atomicAdd(&p.hdr->ticket, 1u);
+        cp_async_commit();
+        cp_async_wait<0>();
         __syncthreads();
 
-        // ---- pass 1: per-chunk serial composition (suffix order), element maps kept in registers
         float a[KC][FC], b[KC][FC];
-#pragma unroll
-        for (int kc = 0; kc < KC; ++kc) {
-            const int c = warp + kc * (FAST_THREADS / 32);      // chunk index; env = lane
-            float P = 0.f, Q = 1.f;
-            if (lane < Et) {
-                const int base = c * FC * FE + lane;
-                // the element after the chunk: next step of the env, next env's first step, or the tile halo
-                float rn, vn, dn;
-                if (c < CE - 1) { rn = sR[base + FC * FE]; vn = sV[base + FC * FE]; dn = sD[base + FC * FE]; }
-                else if (lane + 1 < Et) { rn = sR[lane + 1]; vn = sV[lane + 1]; dn = sD[lane + 1]; }
-                else { rn = s_halo[0]; vn = s_halo[1]; dn = s_halo[2]; }
-                const bool last_of_batch = (e0 + lane == p.N - 1) && (c == CE - 1);
-#pragma unroll
-                for (int j = FC - 1; j >= 0; --j) {
-                    const float r0 = sR[base + j * FE], v0 = sV[base + j * FE], d0 = sD[base + j * FE];
-                    const float nnt = __fsub_rn(1.0f, dn);
-                    // c_gae.pyx:28-29 association, no FMA contraction inside an element
-                    float aj = __fsub_rn(__fadd_rn(rn, __fmul_rn(__fmul_rn(p.gamma, vn), nnt)), v0);
-                    float bj = __fmul_rn(p.gl, nnt);
-                    if (last_of_batch && j == FC - 1) { aj = 0.f; bj = 0.f; }   // A[B-1] = 0
-                    a[kc][j] = aj;
-                    b[kc][j] = bj;
-                    P = fmaf(bj, P, aj);     // (aj,bj) o (P,Q)
-                    Q = bj * Q;
-                    rn = r0; vn = v0; dn = d0;
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < FC; ++j) { a[kc][j] = 0.f; b[kc][j] = 1.f; }
-            }
-            s_cagg[c][lane] = make_float2(P, Q);
-        }
+        scan_chunks<KC, NW>(p, sR, sV, sD, s_halo, e0, Et, a, b, s_cagg);
         __syncthreads();
-
-        // ---- pass 2 (warp 0): chunk carries inside each env, env carries inside the tile, then the look-back
-        if (warp == 0) {
-            float cP = 0.f, cQ = 1.f;                    // composition of the chunks to the right, w.r.t. the env end
-#pragma unroll
-            for (int c = CE - 1; c >= 0; --c) {
-                const float2 g = s_cagg[c][lane];
-                s_cagg[c][lane] = make_float2(cP, cQ);   // carry map entering chunk c from the right
-                const float nP = fmaf(g.y, cP, g.x), nQ = g.y * cQ;
-                cP = nP; cQ = nQ;
-            }
-            // inclusive suffix over the 32 env aggregates (missing envs are the identity)
-            float x = cP, y = cQ;
-#pragma unroll
-            for (int off = 1; off < FE; off <<= 1) {
-                const float x2 = __shfl_down_sync(0xffffffffu, x, off);
-                const float y2 = __shfl_down_sync(0xffffffffu, y, off);
-                if (lane + off < FE) compose(x, y, x2, y2);
-            }
-            const float tP = __shfl_sync(0xffffffffu, x, 0), tQ = __shfl_sync(0xffffffffu, y, 0);
-            // exclusive: map from the tile's right end to env `lane`'s right end
-            float exP = __shfl_down_sync(0xffffffffu, x, 1), exQ = __shfl_down_sync(0xffffffffu, y, 1);
-            if (lane == FE - 1) { exP = 0.f; exQ = 1.f; }
-            s_eagg[lane] = make_float2(exP, exQ);
-            const float carry = tile_lookback(p.status, tile, p.numTiles, tP, tQ, lane);
-            if (lane == 0) s_carry = carry;
-        }
+        if (warp == 0) scan_tile<CE>(p, tile, s_cagg, s_eagg, &s_carry);
         __syncthreads();
 
         // ---- pass 3: apply carries, write outputs in sorted order (64 B per thread-chunk, full sectors)
@@ -505,7 +542,7 @@ __global__ void __launch_bounds__(FAST_THREADS) k_gae_fast(GaeParams p) {
             const float a_env_end = fmaf(em.y, C, em.x);                // A just after this env
 #pragma unroll
             for (int kc = 0; kc < KC; ++kc) {
-                const int c = warp + kc * (FAST_THREADS / 32);
+                const int c = warp + kc * NW;
                 const float2 cm = s_cagg[c][lane];
                 float A = fmaf(cm.y, a_env_end, cm.x);                  // A just after this chunk
                 const int64_t f = (e0 + lane) * (int64_t)H + c * FC;
@@ -542,40 +579,25 @@ __global__ void __launch_bounds__(FAST_THREADS) k_gae_fast(GaeParams p) {
             if (lane < Et) {
                 float* dst = p.adv_tm + e0 + lane;
 #pragma unroll 4
-                for (int t = warp; t < H; t += FAST_THREADS / 32) __stcs(dst + (int64_t)t * p.N, sR[t * FE + lane]);
+                for (int t = warp; t < H; t += NW) __stcs(dst + (int64_t)t * p.N, sR[t * FE + lane]);
             }
         }
         __syncthreads();          // the tile buffers, s_cagg / s_eagg / s_carry are free again
         ticket = s_ticket[1];
         __syncthreads();          // everyone has read s_ticket[1] before thread 0 overwrites it next iteration
     }
-
-    if (tid == 0) {
-        __threadfence();
-        const uint32_t prev = atomicAdd(&p.hdr->exited, 1u);
-        s_ticket[0] = (prev == gridDim.x - 1u) ? 1 : 0;
-    }
-    __syncthreads();
-    if (s_ticket[0]) {
-        for (int j = tid; j < p.numTiles; j += FAST_THREADS) {
-            p.status[j].P = 0.f; p.status[j].Q = 0.f; p.status[j].X = 0.f; p.status[j].flag = 0u;
-        }
-        if (tid == 0) { p.hdr->ticket = 0u; p.hdr->exited = 0u; }
-    }
+    release_workspace<FAST_THREADS>(p, s_ticket);
 }
 
-
-// ---------------------------------------------------------------------------------------------------------------
-// Tile kernel v2 (same shapes as k_gae_fast: N % 4 == 0, H in {128, 256, 512}; same arithmetic, bit-identical results).
-// What changes is how the bytes move:
-//   * DOUBLE-BUFFERED tiles: the cp.async loads of the next tile (claimed by ticket at the top of the iteration) are in
-//     flight while this tile is scanned and written out, so DRAM does not idle during the scan (NBUF = 2 where 2 tiles
-//     fit in shared memory: 96 KB at H = 128 -> 2 CTAs / SM, 192 KB at H = 256 -> 1 CTA / SM);
+// The staged-output kernel, THREADS = 32 * (warps per tile), H = 16 * THREADS / 32 * KC.  What differs from k_gae_fast
+// is how the bytes move:
+//   * NBUF = 2: DOUBLE-BUFFERED tiles, the cp.async loads of the next tile (claimed by ticket at the top of the
+//     iteration) are in flight while this tile is scanned and written out, so DRAM does not idle during the scan;
 //   * COALESCED OUTPUTS: pass 3 stages its results in the tile arrays that are dead after pass 1 -- sorted order
 //     ([env][t], 16-byte chunks XOR-swizzled by env & 7: conflict-free for the lane = env writes and for the row reads)
 //     or arrival order ([t][32]) -- and the block then writes whole 512-byte env rows / 128-byte time rows, instead of
-//     32 scattered 16-byte pieces per store instruction;
-//   * one warp per 16-step chunk of all 32 envs (THREADS = 32 * min(H / 16, 16)): H = 256 runs 16 warps.
+//     32 scattered 16-byte pieces per store instruction.  Two outputs can be staged: advantages + (returns or
+//     time-major advantages).
 template <int KC, int NBUF, int THREADS>
 __global__ void __launch_bounds__(THREADS) k_gae_tile(GaeParams p) {
     constexpr int NW = THREADS / 32;
@@ -593,37 +615,8 @@ __global__ void __launch_bounds__(THREADS) k_gae_tile(GaeParams p) {
 
     auto issue_loads = [&](int tile, int b) {
         float* sR = smem + (size_t)b * 3 * ARR;
-        float* sV = sR + ARR;
-        float* sD = sR + 2 * ARR;
         const int64_t e0 = (int64_t)tile * FE;
-        const int Et = (int)min((int64_t)FE, p.N - e0);
-        const int quad = tid & 7, t0 = tid >> 3;         // 8 float4 per row, THREADS / 8 rows per sweep
-        if (4 * quad < Et) {
-            const int64_t g0 = (int64_t)t0 * p.N + e0 + 4 * quad;
-            const int64_t gstep = (int64_t)(THREADS / 8) * p.N;
-            const float* pr = p.r + g0;
-            const float* pv = p.v + g0;
-            const float* pd = p.d + g0;
-            int sp = t0 * FE + 4 * quad;
-#pragma unroll
-            for (int k = 0; k < H / (THREADS / 8); ++k) {
-                cp_async16(sR + sp, pr);
-                cp_async16(sV + sp, pv);
-                cp_async16(sD + sp, pd);
-                pr += gstep; pv += gstep; pd += gstep;
-                sp += (THREADS / 8) * FE;
-            }
-        }
-        if (tid == 0) {
-            const int64_t en = e0 + Et;                  // first env after the tile; its t = 0 row entry
-            if (en < p.N) {
-                cp_async4(&s_halo[b][0], p.r + en);
-                cp_async4(&s_halo[b][1], p.v + en);
-                cp_async4(&s_halo[b][2], p.d + en);
-            } else {
-                s_halo[b][0] = 0.f; s_halo[b][1] = 0.f; s_halo[b][2] = 1.f;
-            }
-        }
+        load_env_tile<H, THREADS>(p, e0, (int)min((int64_t)FE, p.N - e0), sR, sR + ARR, sR + 2 * ARR, s_halo[b]);
         cp_async_commit();
     };
 
@@ -655,64 +648,10 @@ __global__ void __launch_bounds__(THREADS) k_gae_tile(GaeParams p) {
         }
         __syncthreads();
 
-        // ---- pass 1: per-chunk serial composition (suffix order), element maps kept in registers
         float a[KC][FC], b[KC][FC];
-#pragma unroll
-        for (int kc = 0; kc < KC; ++kc) {
-            const int c = warp + kc * NW;                       // chunk index; env = lane
-            float P = 0.f, Q = 1.f;
-            if (lane < Et) {
-                const int base = c * FC * FE + lane;
-                float rn, vn, dn;
-                if (c < CE - 1) { rn = sR[base + FC * FE]; vn = sV[base + FC * FE]; dn = sD[base + FC * FE]; }
-                else if (lane + 1 < Et) { rn = sR[lane + 1]; vn = sV[lane + 1]; dn = sD[lane + 1]; }
-                else { rn = halo[0]; vn = halo[1]; dn = halo[2]; }
-                const bool last_of_batch = (e0 + lane == p.N - 1) && (c == CE - 1);
-#pragma unroll
-                for (int j = FC - 1; j >= 0; --j) {
-                    const float r0 = sR[base + j * FE], v0 = sV[base + j * FE], d0 = sD[base + j * FE];
-                    const float nnt = __fsub_rn(1.0f, dn);
-                    float aj = __fsub_rn(__fadd_rn(rn, __fmul_rn(__fmul_rn(p.gamma, vn), nnt)), v0);
-                    float bj = __fmul_rn(p.gl, nnt);
-                    if (last_of_batch && j == FC - 1) { aj = 0.f; bj = 0.f; }   // A[B-1] = 0
-                    a[kc][j] = aj;
-                    b[kc][j] = bj;
-                    P = fmaf(bj, P, aj);
-                    Q = bj * Q;
-                    rn = r0; vn = v0; dn = d0;
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < FC; ++j) { a[kc][j] = 0.f; b[kc][j] = 1.f; }
-            }
-            s_cagg[c][lane] = make_float2(P, Q);
-        }
+        scan_chunks<KC, NW>(p, sR, sV, sD, halo, e0, Et, a, b, s_cagg);
         __syncthreads();
-
-        // ---- pass 2 (warp 0): chunk carries inside each env, env carries inside the tile, then the look-back
-        if (warp == 0) {
-            float cP = 0.f, cQ = 1.f;
-#pragma unroll
-            for (int c = CE - 1; c >= 0; --c) {
-                const float2 g = s_cagg[c][lane];
-                s_cagg[c][lane] = make_float2(cP, cQ);
-                const float nP = fmaf(g.y, cP, g.x), nQ = g.y * cQ;
-                cP = nP; cQ = nQ;
-            }
-            float x = cP, y = cQ;
-#pragma unroll
-            for (int off = 1; off < FE; off <<= 1) {
-                const float x2 = __shfl_down_sync(0xffffffffu, x, off);
-                const float y2 = __shfl_down_sync(0xffffffffu, y, off);
-                if (lane + off < FE) compose(x, y, x2, y2);
-            }
-            const float tP = __shfl_sync(0xffffffffu, x, 0), tQ = __shfl_sync(0xffffffffu, y, 0);
-            float exP = __shfl_down_sync(0xffffffffu, x, 1), exQ = __shfl_down_sync(0xffffffffu, y, 1);
-            if (lane == FE - 1) { exP = 0.f; exQ = 1.f; }
-            s_eagg[lane] = make_float2(exP, exQ);
-            const float carry = tile_lookback(p.status, tile, p.numTiles, tP, tQ, lane);
-            if (lane == 0) s_carry = carry;
-        }
+        if (warp == 0) scan_tile<CE>(p, tile, s_cagg, s_eagg, &s_carry);
         __syncthreads();
 
         // ---- pass 3: apply carries; results staged in the dead tile arrays:
@@ -786,32 +725,16 @@ __global__ void __launch_bounds__(THREADS) k_gae_tile(GaeParams p) {
         if (NBUF == 2) cur ^= 1;
         else if (ticket < p.numTiles) issue_loads(p.numTiles - 1 - ticket, 0);
     }
-
-    if (tid == 0) {
-        __threadfence();
-        const uint32_t prev = atomicAdd(&p.hdr->exited, 1u);
-        s_ticket[0] = (prev == gridDim.x - 1u) ? 1 : 0;
-    }
-    __syncthreads();
-    if (s_ticket[0]) {
-        for (int j = tid; j < p.numTiles; j += THREADS) {
-            p.status[j].P = 0.f; p.status[j].Q = 0.f; p.status[j].X = 0.f; p.status[j].flag = 0u;
-        }
-        if (tid == 0) { p.hdr->ticket = 0u; p.hdr->exited = 0u; }
-    }
+    release_workspace<THREADS>(p, s_ticket);
 }
 
-// 0: by horizon -- 2 at H <= 128, 3 above (H100 80GB HBM3 at 700 W, bench.py: C2 H = 128 23.7 us double- vs 25.0 us
-// single-buffered; C3 H = 256 162 us single- vs 177 us double-buffered); 2 / 3: k_gae_tile double- / single-buffered;
-// 1: k_gae_fast
-int g_gae_variant = 0;
+int g_gae_variant = 0;   // pb_gae_set_variant
 
 struct GaePlan {
-    int fastKC;   // > 0: k_gae_fast<fastKC, nbuf>
-    int nbuf;
+    int fastKC;   // > 0: a 32-env tile kernel, H = 128 * fastKC
     int E, logE, L, pitch, numTiles, RW;
     uint32_t magicH;
-    size_t smem;
+    size_t smem;  // dynamic shared memory per tile buffer
 };
 
 GaePlan gae_plan(int64_t N, int64_t H) {
@@ -820,7 +743,6 @@ GaePlan gae_plan(int64_t N, int64_t H) {
     const int Ltarget = 2048, Lmax = 4096;
     if (N > 1 && N % 4 == 0 && (H == 128 || H == 256 || H == 512)) {
         g.fastKC = (int)(H / 128);
-        g.nbuf = 1;
         g.E = FE; g.logE = 5; g.L = FE * (int)H; g.pitch = FE; g.magicH = 0;
         g.numTiles = (int)pb_ceil_div(N, FE);
         g.smem = (size_t)3 * FE * H * sizeof(float);
@@ -853,6 +775,41 @@ GaePlan gae_plan(int64_t N, int64_t H) {
     return g;
 }
 
+struct GaeKernel {
+    void (*fn)(GaeParams);
+    int threads;
+    int nbuf;     // tile buffers in dynamic shared memory
+};
+template <int KC>
+GaeKernel round1() { return {k_gae_fast<KC>, FAST_THREADS, 1}; }
+template <int KC, int NBUF, int THREADS>
+GaeKernel staged() { return {k_gae_tile<KC, NBUF, THREADS>, THREADS, NBUF}; }
+
+// The 32-env tile kernel for H = 128 * fastKC.  Variant 0 picks by horizon: double-buffered at H = 128, single-buffered
+// above (H100 80GB HBM3 at 700 W, bench.py: C2 H = 128 23.7 us double- vs 25.0 us single-buffered; C3 H = 256 162 us
+// single- vs 177 us double-buffered).  Two buffers do not fit at H = 512.  k_gae_fast serves variant 1 and every call
+// the staged kernel cannot: sorted returns and time-major advantages together.
+GaeKernel tile_kernel(int variant, int fastKC, bool staged_ok) {
+    if (variant == 0) variant = fastKC == 1 ? 2 : 3;
+    if (variant == 1 || !staged_ok)  // H = 128        H = 256                H = 512
+        return fastKC == 1 ? round1<1>() : fastKC == 2 ? round1<2>() : round1<4>();
+    if (variant == 2)
+        return fastKC == 1 ? staged<1, 2, 256>() : fastKC == 2 ? staged<1, 2, 512>() : staged<2, 1, 512>();
+    return fastKC == 1 ? staged<1, 1, 256>() : fastKC == 2 ? staged<2, 1, 256>() : staged<2, 1, 512>();
+}
+
+// Persistent launch: every resident slot of the chip, never more blocks than tiles (one wave, no tail).
+int launch_persistent(void (*kernel)(GaeParams), int threads, size_t smem, const GaeParams& p, cudaStream_t s) {
+    PB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+    PB_REQUIRE(per_sm >= 1, PB_ERR_CUDA, "pb_gae: kernel does not fit on an SM (smem %zu)", smem);
+    const int grid = std::min(per_sm * PB_NUM_SMS, p.numTiles);
+    kernel<<<grid, threads, smem, s>>>(p);
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
+
 }  // namespace
 
 extern "C" size_t pb_gae_workspace_bytes(int64_t num_envs, int64_t horizon) {
@@ -879,11 +836,11 @@ extern "C" int pb_gae_tm(const float* rewards, const float* values, const float*
     PB_REQUIRE(num_envs >= 0 && horizon >= 0, PB_ERR_INVALID, "pb_gae: negative size");
     if (num_envs == 0 || horizon == 0) return PB_OK;
     PB_REQUIRE(rewards && values && dones && (advantages || advantages_time_major), PB_ERR_INVALID, "pb_gae: null pointer");
-    PB_REQUIRE(!advantages_time_major || gae_plan(num_envs, horizon).fastKC > 0, PB_ERR_UNSUPPORTED,
+    const GaePlan g = gae_plan(num_envs, horizon);
+    PB_REQUIRE(!advantages_time_major || g.fastKC > 0, PB_ERR_UNSUPPORTED,
                "pb_gae_tm: the time-major output needs the tile kernel (horizon in {128, 256, 512}, num_envs %% 4 == 0)");
-    PB_REQUIRE(advantages || gae_plan(num_envs, horizon).fastKC > 0, PB_ERR_INVALID, "pb_gae: null advantages");
+    PB_REQUIRE(advantages || g.fastKC > 0, PB_ERR_INVALID, "pb_gae: null advantages");
     PB_REQUIRE(num_envs * horizon < (1ll << 40), PB_ERR_INVALID, "pb_gae: batch too large");
-    GaePlan g = gae_plan(num_envs, horizon);
     const size_t need = sizeof(GaeHeader) + (size_t)g.numTiles * sizeof(GaeStatus);
     PB_REQUIRE(workspace && workspace_bytes >= need, PB_ERR_INVALID,
                "pb_gae: workspace too small (%zu < %zu)", workspace_bytes, need);
@@ -896,65 +853,19 @@ extern "C" int pb_gae_tm(const float* rewards, const float* values, const float*
     p.hdr = (GaeHeader*)workspace;
     p.status = (GaeStatus*)((char*)workspace + sizeof(GaeHeader));
     cudaStream_t s = (cudaStream_t)stream;
-    // persistent grid: every resident slot of the chip, never more blocks than tiles (one wave, no tail)
-    int per_sm = 0;
     if (g.fastKC > 0) {
         PB_REQUIRE((!advantages || ((uintptr_t)advantages & 15) == 0) && (!returns_sorted || ((uintptr_t)returns_sorted & 15) == 0),
                    PB_ERR_INVALID, "pb_gae: advantages / returns must be 16-byte aligned");
         PB_REQUIRE(((uintptr_t)rewards & 15) == 0 && ((uintptr_t)values & 15) == 0 && ((uintptr_t)dones & 15) == 0,
                    PB_ERR_INVALID, "pb_gae: rewards / values / dones must be 16-byte aligned");
-#define PB_GAE_FAST(KC)                                                                                               \
-    {                                                                                                                 \
-        PB_CUDA(cudaFuncSetAttribute(k_gae_fast<KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));     \
-        PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gae_fast<KC>, FAST_THREADS, g.smem));       \
-        PB_REQUIRE(per_sm >= 1, PB_ERR_CUDA, "pb_gae: kernel does not fit on an SM (smem %zu)", g.smem);              \
-        int grid = per_sm * PB_NUM_SMS;                                                                               \
-        if (grid > g.numTiles) grid = g.numTiles;                                                                     \
-        k_gae_fast<KC><<<grid, FAST_THREADS, g.smem, s>>>(p);                                                         \
+        const GaeKernel k = tile_kernel(g_gae_variant, g.fastKC, !(returns_sorted && advantages_time_major));
+        return launch_persistent(k.fn, k.threads, k.nbuf * g.smem, p, s);
     }
-#define PB_GAE_TILE(KC, NBUF, THREADS)                                                                                \
-    {                                                                                                                 \
-        const size_t smem2 = (size_t)NBUF * g.smem;                                                                   \
-        PB_CUDA(cudaFuncSetAttribute(k_gae_tile<KC, NBUF, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize,      \
-                                     (int)smem2));                                                                    \
-        PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gae_tile<KC, NBUF, THREADS>, THREADS, smem2)); \
-        PB_REQUIRE(per_sm >= 1, PB_ERR_CUDA, "pb_gae: kernel does not fit on an SM (smem %zu)", smem2);               \
-        int grid = per_sm * PB_NUM_SMS;                                                                               \
-        if (grid > g.numTiles) grid = g.numTiles;                                                                     \
-        k_gae_tile<KC, NBUF, THREADS><<<grid, THREADS, smem2, s>>>(p);                                                \
-    }
-        const bool v2_ok = !(returns_sorted && advantages_time_major);   // v2 stages two outputs: adv + (ret | adv_tm)
-        const int variant = g_gae_variant ? g_gae_variant : (g.fastKC == 1 ? 2 : 3);   // double-buffered tiles for H = 128, single-buffered above
-        if (variant == 2 && v2_ok) {
-            if (g.fastKC == 1) PB_GAE_TILE(1, 2, 256) else if (g.fastKC == 2) PB_GAE_TILE(1, 2, 512) else PB_GAE_TILE(2, 1, 512)
-        } else if (variant == 3 && v2_ok) {   // single-buffered tiles (more CTAs per SM), coalesced outputs
-            if (g.fastKC == 1) PB_GAE_TILE(1, 1, 256) else if (g.fastKC == 2) PB_GAE_TILE(2, 1, 256) else PB_GAE_TILE(2, 1, 512)
-        } else {
-            if (g.fastKC == 1) PB_GAE_FAST(1) else if (g.fastKC == 2) PB_GAE_FAST(2) else PB_GAE_FAST(4)
-        }
-#undef PB_GAE_TILE
-#undef PB_GAE_FAST
-        PB_LAUNCH_CHECK();
-        return PB_OK;
-    }
-    if (g.RW == 16) {
-        PB_CUDA(cudaFuncSetAttribute(k_gae<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
-        PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gae<16>, GAE_THREADS, g.smem));
-    } else {
-        PB_CUDA(cudaFuncSetAttribute(k_gae<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
-        PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gae<32>, GAE_THREADS, g.smem));
-    }
-    PB_REQUIRE(per_sm >= 1, PB_ERR_CUDA, "pb_gae: kernel does not fit on an SM (smem %zu)", g.smem);
-    int grid = per_sm * PB_NUM_SMS;
-    if (grid > g.numTiles) grid = g.numTiles;
-    if (g.RW == 16) k_gae<16><<<grid, GAE_THREADS, g.smem, s>>>(p);
-    else k_gae<32><<<grid, GAE_THREADS, g.smem, s>>>(p);
-    PB_LAUNCH_CHECK();
-    return PB_OK;
+    return launch_persistent(g.RW == 16 ? k_gae<16> : k_gae<32>, GAE_THREADS, g.smem, p, s);
 }
 
-// 0 (default): chosen by horizon; 2: k_gae_tile (double-buffered tiles, coalesced outputs); 3: k_gae_tile single-buffered;
-// 1: the round-1 k_gae_fast.  For A/B measurements.
+// 0 (default): chosen by horizon; 2: k_gae_tile double-buffered where two tiles fit; 3: k_gae_tile single-buffered;
+// 1: the round-1 k_gae_fast.  For A/B measurements; see tile_kernel.
 extern "C" int pb_gae_set_variant(int32_t variant) {
     PB_REQUIRE(variant >= 0 && variant <= 3, PB_ERR_INVALID, "pb_gae_set_variant: 0 .. 3");
     g_gae_variant = variant;

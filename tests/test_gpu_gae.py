@@ -171,19 +171,55 @@ def test_gae_time_major_output_and_slab_statistics(h, n):
 
 @pytest.mark.parametrize('h,n', [(128, 64), (128, 36), (128, 16384), (256, 96), (256, 4096), (512, 40), (512, 1000)])
 def test_gae_tile_kernel_variants_agree(h, n):
-    """k_gae_tile (double-buffered, coalesced outputs; default) and the round-1 k_gae_fast are the same arithmetic: the
-    element maps are identical, only the tile look-back may compose in a different order run to run -> compare to 1e-6."""
+    """Every pb_gae_set_variant value (0 by horizon, 1 the round-1 k_gae_fast, 2 / 3 k_gae_tile double- / single-
+    buffered) computes the same element maps and scan; only the tile look-back may compose in a different order run to
+    run -> compare to 1e-6, and each against the oracle."""
     from pufferlib_b200 import _native
     lib = _native.lib()
     r, v, d = make_inputs(h, n, seed=3 * h + n, p_done=0.02)
     out = {}
     try:
-        for variant in (1, 2):
+        for variant in (0, 1, 2, 3):
             _native.check(lib.pb_gae_set_variant(variant))
             out[variant] = gae_device(r, v, d, 0.99, 0.95)
     finally:
         lib.pb_gae_set_variant(0)
-    for k in (0, 1):
-        assert np.allclose(out[1][k], out[2][k], rtol=1e-6, atol=1e-6)
     rs, vs, ds = (sorted_from_time_major(x) for x in (r, v, d))
-    gae_tolerance_check(out[2][0], ogae.compute_gae(ds, vs, rs, 0.99, 0.95), ogae.compute_gae_f64(ds, vs, rs, 0.99, 0.95))
+    ref32, ref64 = ogae.compute_gae(ds, vs, rs, 0.99, 0.95), ogae.compute_gae_f64(ds, vs, rs, 0.99, 0.95)
+    for variant in (0, 1, 3):
+        for k in (0, 1):
+            assert np.allclose(out[variant][k], out[2][k], rtol=1e-6, atol=1e-6), variant
+    for variant in (0, 1, 2, 3):
+        gae_tolerance_check(out[variant][0], ref32, ref64)
+
+
+@pytest.mark.parametrize('h,n', [(128, 64), (128, 36), (256, 96), (512, 40), (512, 1000)])
+def test_gae_sorted_returns_and_time_major_in_one_call(h, n):
+    """pb_gae_tm with advantages, returns and time-major advantages at once: the staged k_gae_tile epilogue holds only
+    two outputs, so every variant runs the round-1 k_gae_fast for this call.  Within the one call the returns are the
+    advantages plus the values and the time-major output is the sorted advantages transposed, bit for bit."""
+    import ctypes as C
+    import torch
+    from pufferlib_b200 import _native
+    lib = _native.lib()
+    r, v, d = make_inputs(h, n, seed=5 * h + n, p_done=0.02)
+    rs, vs, ds = (sorted_from_time_major(x) for x in (r, v, d))
+    ref32, ref64 = ogae.compute_gae(ds, vs, rs, 0.99, 0.95), ogae.compute_gae_f64(ds, vs, rs, 0.99, 0.95)
+    dev = torch.device('cuda')
+    tr, tv, td = (torch.as_tensor(x, device=dev) for x in (r, v, d))
+    ws = torch.zeros(lib.pb_gae_workspace_bytes(n, h), dtype=torch.uint8, device=dev)
+    try:
+        for variant in (0, 1, 2, 3):
+            _native.check(lib.pb_gae_set_variant(variant))
+            adv, ret, adv_tm = (torch.full((n * h,), float('nan'), device=dev) for _ in range(3))
+            _native.check(lib.pb_gae_tm(_native.ptr(tr), _native.ptr(tv), _native.ptr(td), _native.ptr(adv), _native.ptr(ret),
+                                        _native.ptr(adv_tm), n, h, C.c_float(0.99), C.c_float(0.95), _native.ptr(ws),
+                                        ws.numel(), _native.stream_ptr()))
+            torch.cuda.synchronize()
+            a, rt, atm = (x.cpu().numpy() for x in (adv, ret, adv_tm))
+            assert np.array_equal(rt.view(np.uint32), (a + vs).view(np.uint32)), variant
+            assert np.array_equal(atm.reshape(h, n).view(np.uint32), a.reshape(n, h).T.view(np.uint32)), variant
+            gae_tolerance_check(a, ref32, ref64)
+            assert int(ws.to(torch.int32).abs().sum()) == 0, 'workspace must be left zeroed'
+    finally:
+        lib.pb_gae_set_variant(0)

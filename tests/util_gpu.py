@@ -31,6 +31,63 @@ def rna(t):
     return ((bits + 0x1000) & ~0x1FFF).view(torch.float32).double()
 
 
+def trunc_tf32(t):
+    """The TF32 value a tensor core reads from the fp32 value of t (low 13 mantissa bits dropped), as fp64."""
+    bits = t.detach().float().contiguous().view(torch.int32)
+    return (bits & ~0x1FFF).view(torch.float32).double()
+
+
+# Rounding model of the fp32 accumulation in k_breakout_rollout's tensor-core products (wgmma for the encoder, mma.sync for
+# the heads).  The TF32 operand products are exact in fp32 (11 x 11 significant bits), so every error comes from the K = 128
+# additions of the products plus the one fp32 add of the bias: each addition loses at most one fp32 ulp of a partial sum
+# (2^-23 of it: the adder may truncate rather than round), times 2 because the tensor core aligns a group of addends to the
+# largest exponent before it sums them.  Every partial sum is bounded by S = sum_k |x_k w_k| + |b|, so
+#     |out_kernel - out_fp64| <= ACC_F32 * S,   ACC_F32 = 2 * (K + 1) * 2^-23.
+# This is a worst-case bound: typical errors are about sqrt(K) * 2^-24 * S, some twenty times smaller.
+ACC_F32 = 2 * 129 * 2.0 ** -23
+
+
+def rollout_encoder_ref(x, model):
+    """fp64 pre-activation of k_breakout_rollout's encoder for observations x [M, 128]: obs . trunc_tf32(W_enc)^T + b_enc
+    (the observations are exact in TF32) -> (pre, bound) with |pre_kernel - pre| <= bound elementwise."""
+    w = trunc_tf32(model.encoder.weight)
+    b = model.encoder.bias.detach().double()
+    x = x.double()
+    return x @ w.t() + b, ACC_F32 * (x.abs() @ w.abs().t() + b.abs())
+
+
+def rollout_heads_ref(hidden, w_cat, b_cat):
+    """fp64 head outputs [M, 8] of k_breakout_rollout from fp32 relu(h) [M, 128]: the mma.sync reads relu(h) truncated to
+    TF32 and W_heads rounded to TF32 (cvt.rna), and the bias is added in fp32 -> (out, bound), as rollout_encoder_ref."""
+    h, w, b = trunc_tf32(hidden), rna(w_cat), b_cat.detach().double()
+    return h @ w.t() + b, ACC_F32 * (h.abs() @ w.abs().t() + b.abs())
+
+
+def check_rollout_dump(dbg_hidden, dbg_out, x0, model, exact_encoder=False):
+    """The step-0 dump of k_breakout_rollout (pb_rollout_debug_buffers) checked stage by stage, each stage from the
+    kernel's own previous one: relu(h) against the fp64 encoder on the stored step-0 observations x0, then the head
+    outputs against fp64 heads recomputed from the dumped relu(h).  Both within the ACC_F32 bound; the padding rows of the
+    8-row head matrix are zero, so their outputs must be exactly 0.  exact_encoder: every partial sum of the encoder product
+    is exact in fp32 (weights on a coarse grid), so relu(h) must equal fl(sum + b_enc) bit for bit.
+    -> (max |err| relu(h), largest bound, max |err| heads, largest bound)."""
+    with torch.no_grad():
+        pre, bound_h = rollout_encoder_ref(x0, model)
+        ref_h = torch.relu(pre)
+        err_h = (dbg_hidden.double() - ref_h).abs()
+        assert bool((err_h <= bound_h).all()), \
+            f'relu(h) at step 0: max err {float(err_h.max()):.3e}, {int((err_h > bound_h).sum())} elements past the bound'
+        if exact_encoder:
+            off = int((dbg_hidden != ref_h.float()).sum())
+            assert off == 0, f'relu(h) at step 0: {off} elements differ from fl(exact sum + b_enc)'
+        w_cat, b_cat = model.head_matrix()
+        out, bound_o = rollout_heads_ref(dbg_hidden, w_cat, b_cat)
+        err_o = (dbg_out.double() - out).abs()
+        assert bool((err_o <= bound_o).all()), \
+            f'head outputs at step 0: max err per column {[f"{float(v):.2e}" for v in err_o.max(0).values]}, ' \
+            f'bound {[f"{float(v):.2e}" for v in bound_o.max(0).values]}'
+    return float(err_h.max()), float(bound_h.max()), float(err_o.max()), float(bound_o.max())
+
+
 def restated_draw(probs, u, window):
     """The inverse-CDF draw of pb_sample_row restated on fp64 probabilities [n, A] (numpy) and the uniforms u [n]:
     -> (actions: the first k with u < cdf_k, near: rows whose u lies within `window` of an inner boundary cdf_k,

@@ -287,6 +287,11 @@ def test_train_fused_update_matches_cudnn_update(env, n, h, bptt, monkeypatch):
     value-head bias; the value head of a freshly initialised policy fits near-zero returns, so its gradient is a nearly
     cancelling mean), state 1.5e-4, parameters 2.5e-5, value loss 2 % apart (7.47e-4 vs 7.62e-4); squared gradients within
     3.4e-4."""
+    check_fused_update_matches_cudnn(env, n, h, bptt, monkeypatch)
+
+
+def check_fused_update_matches_cudnn(env, n, h, bptt, monkeypatch):
+    """The body of test_train_fused_update_matches_cudnn_update for env kind `env`, n envs, h steps, bptt horizon bptt."""
     vec = pvec.make(ocean.env_creator(env), num_envs=n, backend=pvec.B200)
     torch.manual_seed(0)
     net = models.LSTMWrapper(vec.driver_env, models.Default(vec.driver_env), input_size=128, hidden_size=128)

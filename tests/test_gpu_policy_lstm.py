@@ -163,8 +163,23 @@ def test_fused_recurrent_rollout_replays(env, n, h):
     the fp64 recurrence on the stored observations gives the stored values / logprobs and the final lstm_h / lstm_c, the
     actions are the inverse CDF of each step's uniforms, and train() afterwards gives finite losses.  Largest errors
     observed (H100 80GB HBM3): value 9.9e-5, logprob 1.5e-5, lstm_h 1.5e-5, lstm_c 2.4e-5; bound TOL_ROLLOUT = 5e-4."""
+    check_recurrent_rollout_replays(env, n, h)
+
+
+def rollout_oracle(env, n):
+    """The oracle vectoriser of env kind `env` over n envs."""
     from oracle.envs import OracleVec
+    from oracle.ocean import OceanSerial
     from oracle.squared import SquaredSerial
+    if env == 'squared':
+        return SquaredSerial(n)
+    if env == 'breakout':
+        return OracleVec('breakout', n)
+    return OceanSerial(env, n)
+
+
+def check_recurrent_rollout_replays(env, n, h):
+    """The body of test_fused_recurrent_rollout_replays for env kind `env`, n envs, h steps."""
     vec = pvec.make(ocean.env_creator(env), num_envs=n, backend=pvec.B200)
     torch.manual_seed(0)
     net = models.LSTMWrapper(vec.driver_env, models.Default(vec.driver_env), input_size=128, hidden_size=128)
@@ -174,7 +189,7 @@ def test_fused_recurrent_rollout_replays(env, n, h):
     assert data.fused_rows
     clean_pufferl.evaluate(data)
     exp = data.experience
-    ora = SquaredSerial(n) if env == 'squared' else OracleVec('breakout', n)
+    ora = rollout_oracle(env, n)
     ora.async_reset(1)
     obs_shape = tuple(vec.single_observation_space.shape)
     acts, obs = cpu(exp.actions).reshape(h, n), cpu(exp.obs).reshape(h, n, *obs_shape)

@@ -90,7 +90,9 @@ __device__ __forceinline__ void pb_peer_allreduce_slice(const pb_peer_comm& c, f
     __syncthreads();
     const uint64_t e = s_epoch;
     const int64_t chunk = ((n + PB_PEER_SLICES - 1) / PB_PEER_SLICES + 3) & ~(int64_t)3;
-    const int64_t lo = (int64_t)b * chunk, hi = lo + chunk < n ? lo + chunk : n;
+    // a short buffer leaves the trailing slices empty: lo = hi = n (an unclamped lo > n would put hi4 below hi when n % 4 != 0,
+    // and this CTA would then sum the last n % 4 elements a second time)
+    const int64_t lo = (int64_t)b * chunk < n ? (int64_t)b * chunk : n, hi = lo + chunk < n ? lo + chunk : n;
     const int64_t slot_off = PB_PEER_HEADER_BYTES / 4 + (int64_t)(e & 1) * c.capacity;
     float* mine = reinterpret_cast<float*>(c.base[c.rank]) + slot_off;
     // 128-bit accesses where the layout allows (slices start at multiples of 4 floats): one peer load per thread and rank,

@@ -33,7 +33,7 @@ def log(rank, *a):
 def check_allreduce(rank, world):
     comm = pdist.PeerComm(20000)
     torch.manual_seed(100 + rank)
-    for n in (1, 17157, 20000):
+    for n in (1, 5, 514, 17157, 20000):
         x = torch.randn(n, device='cuda')
         ref = x.clone()
         dist.all_reduce(ref)

@@ -77,7 +77,6 @@ def build_lib(src_root, out_dir, phases):
     lib.pb_mlp_update_fused.restype = C.c_int
     lib.pb_mlp_update_fused.argtypes = _native.lib().pb_mlp_update_fused.argtypes
     lib.pb_mlp_update_workspace_bytes.restype = C.c_size_t
-    lib.pb_mlp_update_set_variant.argtypes = [C.c_int32]
     lib.pb_phase_lib_error.restype = C.c_char_p
     return lib
 

@@ -412,15 +412,13 @@ int pb_mlp_tail_backward_ex(const float* dout, int64_t dout_stride, const float*
  *   returns      nullable: advantages (raw) + old_values is used (clean_pufferl.py:476-481)
  *   grad_flat    [128*128 + 8*128 + 128 + 8]: dW_enc | dW_heads | db_enc | db_heads  (what pb_clip_adam consumes)
  *   stats8       the six loss sums of pb_ppo_loss (zeroed here)
- *   dpre_out     null: dW_enc = dPre^T x is accumulated inside the kernel (wgmma with x^T fragments in registers and
- *                dPre^T in shared memory).  Non-null: dPre
- *                [M][128] (slab-major rows) is written there instead and the dW_enc part of grad_flat is left to the caller
- *   dbg_*        nullable dumps of relu(h) [M][128], dPre [M][128], dOut [M][8] for validation. */
+ *   dpre_out     must be NULL (PB_ERR_INVALID before any launch otherwise): dW_enc = dPre^T x is accumulated inside the
+ *                kernel (wgmma with x^T fragments in registers and dPre^T in shared memory)
+ *   dbg_*        nullable dumps of relu(h) [M][128], dPre [M][128], dOut [M][8] for validation.
+ * The head, dPre and dW_heads products take TF32 operands on mma.sync with fp32 accumulation. */
 size_t pb_mlp_update_workspace_bytes(void);
-/* epilogue products: 1 = fp32 head / dPre products, 2 = TF32 mma.sync products (default) */
-int pb_mlp_update_set_variant(int32_t variant);
 /* the reduce step of pb_mlp_update_fused also leaves the sum of squares of the gradient it wrote as pb_mlp_update_sumsq_parts()
- * doubles at byte pb_mlp_update_sumsq_offset() of the workspace (dW-in-kernel mode): input of pb_clip_adam_parts */
+ * doubles at byte pb_mlp_update_sumsq_offset() of the workspace: input of pb_clip_adam_parts */
 size_t pb_mlp_update_sumsq_offset(void);
 int32_t pb_mlp_update_sumsq_parts(void);
 int pb_mlp_update_fused(const float* x, int64_t ldx, int64_t slab_rows, int64_t slab_stride_rows, int32_t n_slabs,

@@ -10,8 +10,6 @@
 // their 512-byte observation rows cooperatively -- per row each lane builds one float4 (lane 0-1: the 8 header
 // scalars, lanes 2-31: 4 bricks each from the shuffled bitmap) so every row is ONE fully coalesced 512 B warp store
 // (4 x 128 B lines).  Reward / flag / done rows are [N]-contiguous.
-#include <cuda.h>
-
 #include "env_common.cuh"
 #include "policy_sample.cuh"
 #include "tma.cuh"
@@ -234,20 +232,6 @@ struct RolloutParams {
     float* dbg_out;             // validation only: head outputs of step 0, [N][8]
 };
 
-__device__ __forceinline__ void ro_tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-            smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-        : "memory");
-}
-__device__ __forceinline__ void ro_tma_store_2d(const CUtensorMap* map, int c0, int c1, const void* src) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%1, %2}], [%3];" ::"l"(
-                     reinterpret_cast<uint64_t>(map)),
-                 "r"(c0), "r"(c1), "r"(smem_u32(src))
-                 : "memory");
-}
-
 // the observation row of one env (same values as k_breakout's cooperative row write) into row r of a SW128 K-major tile
 __device__ __forceinline__ void ro_write_obs(uint8_t* tile, int r, int px, int bx, int by, int vx, int vy, int lives,
                                              int in_play, const uint4& bricks) {
@@ -264,19 +248,6 @@ __device__ __forceinline__ void ro_write_obs(uint8_t* tile, int r, int px, int b
         }
         *reinterpret_cast<float4*>(tile + (c >> 3) * RO_KBLK_BYTES + r * 128 + ((((c & 7) ^ (r & 7))) << 4)) = v;
     }
-}
-
-// mma.sync m16n8k8 TF32 (fp32 accumulate): a0 (g, t)  a1 (g + 8, t)  a2 (g, t + 4)  a3 (g + 8, t + 4);  b0 (k = t, n = g)  b1 (k = t + 4, n = g);
-// c0 c1 (g, 2t + {0,1})  c2 c3 (g + 8, 2t + {0,1})      [g = lane >> 2, t = lane & 3]
-__device__ __forceinline__ void ro_mma_tf32(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t ro_to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return r;
 }
 
 template <bool DBG>      // DBG: step-0 dumps for the validation hook (pb_rollout_debug_buffers); compiled out of the product path
@@ -305,7 +276,7 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
         // ================= TMA issue (one thread) =================
         if (lane == 0) {
             mbar_expect_tx(w_full, RO_TILE_BYTES);
-            for (int kb = 0; kb < 4; ++kb) ro_tma_load_2d(smem + RO_SMEM_W + kb * RO_KBLK_BYTES, &map_w, kb * 32, 0, w_full);
+            for (int kb = 0; kb < 4; ++kb) tma_load_2d(smem + RO_SMEM_W + kb * RO_KBLK_BYTES, &map_w, kb * 32, 0, w_full);
             for (int t = 0; t <= H; ++t) {
                 const int s = t & 1;
                 uint8_t* tile = smem + RO_SMEM_X + s * RO_TILE_BYTES;
@@ -317,7 +288,7 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
                 // the same tile goes to HBM: rollout row t, or the vecenv's own observation buffer for the closing step
                 const CUtensorMap* map = t < H ? &map_obs : &map_carry;
                 const int row0 = t < H ? t * p.n + e0 : e0;
-                for (int kb = 0; kb < 4; ++kb) ro_tma_store_2d(map, kb * 32, row0, tile + kb * RO_KBLK_BYTES);
+                for (int kb = 0; kb < 4; ++kb) tma_store_2d(map, kb * 32, row0, tile + kb * RO_KBLK_BYTES);
                 tma_commit();
             }
             tma_wait_all<0>();
@@ -354,8 +325,8 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
         float benc[16][2];                            // b_enc of the accumulator columns 8j + 2tq + {0, 1}
 #pragma unroll
         for (int kb = 0; kb < 16; ++kb) {
-            hb[kb][0] = ro_to_tf32(c_ro_wh[g * 128 + 8 * kb + 2 * tq]);
-            hb[kb][1] = ro_to_tf32(c_ro_wh[g * 128 + 8 * kb + 2 * tq + 1]);
+            hb[kb][0] = to_tf32(c_ro_wh[g * 128 + 8 * kb + 2 * tq]);
+            hb[kb][1] = to_tf32(c_ro_wh[g * 128 + 8 * kb + 2 * tq + 1]);
             benc[kb][0] = c_ro_benc[8 * kb + 2 * tq];
             benc[kb][1] = c_ro_benc[8 * kb + 2 * tq + 1];
         }
@@ -407,8 +378,10 @@ k_breakout_rollout(const __grid_constant__ CUtensorMap map_obs, const __grid_con
                 for (int kb = 0; kb < 16; ++kb) {
                     const float4 lo = *reinterpret_cast<const float4*>(a_lo + kb * 1024);
                     const float4 hi = *reinterpret_cast<const float4*>(a_hi + kb * 1024);
-                    ro_mma_tf32(hp[0], __float_as_uint(lo.x), __float_as_uint(lo.y), __float_as_uint(hi.x), __float_as_uint(hi.y), hb[kb][0], hb[kb][1]);
-                    ro_mma_tf32(hp[1], __float_as_uint(lo.z), __float_as_uint(lo.w), __float_as_uint(hi.z), __float_as_uint(hi.w), hb[kb][0], hb[kb][1]);
+                    const uint32_t a0[4] = {__float_as_uint(lo.x), __float_as_uint(lo.y), __float_as_uint(hi.x), __float_as_uint(hi.y)};
+                    const uint32_t a1[4] = {__float_as_uint(lo.z), __float_as_uint(lo.w), __float_as_uint(hi.z), __float_as_uint(hi.w)};
+                    mma_tf32(hp[0], a0, hb[kb][0], hb[kb][1]);
+                    mma_tf32(hp[1], a1, hb[kb][0], hb[kb][1]);
                 }
                 __syncwarp();        // all fragment loads done: the head of the block becomes the [32 rows][10] redistribution scratch
                 float* scr = reinterpret_cast<float*>(blk);
@@ -510,22 +483,6 @@ __global__ void k_counter_add(uint64_t* c, uint64_t v) { *c += v; }
 float* g_ro_dbg_hidden = nullptr;
 float* g_ro_dbg_out = nullptr;
 
-typedef CUresult (*RoEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int ro_make_map(RoEncodeTiledFn fn, CUtensorMap* map, const float* base, int64_t rows, int64_t row_stride_floats) {
-    const cuuint64_t dims[2] = {128, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)row_stride_floats * 4};
-    const cuuint32_t box[2] = {32, (cuuint32_t)RO_ENVS};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    PB_REQUIRE(r == CUDA_SUCCESS, PB_ERR_CUDA, "cuTensorMapEncodeTiled failed: %d", (int)r);
-    return PB_OK;
-}
-
 int breakout_launch(pb_env* env, int mode, const int64_t* actions, const pb_env_out* out, cudaStream_t s) {
     BreakoutState* st = (BreakoutState*)env->kind;
     const int n = env->cfg.num_envs;
@@ -605,15 +562,10 @@ extern "C" int pb_rollout_breakout_mlp(pb_env* env, int32_t horizon, float* obs,
                    ((uintptr_t)w_enc & 15) == 0,
                PB_ERR_INVALID, "pb_rollout_breakout_mlp: 16-byte aligned, densely packed observation rows required");
     PB_CUDA(cudaSetDevice(env->cfg.device));
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qr;
-    PB_REQUIRE(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) == cudaSuccess && fn &&
-                   qr == cudaDriverEntryPointSuccess,
-               PB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
     alignas(64) CUtensorMap map_obs, map_carry, map_w;
-    int rc = ro_make_map((RoEncodeTiledFn)fn, &map_obs, obs, (int64_t)horizon * n, 128);
-    if (rc == PB_OK) rc = ro_make_map((RoEncodeTiledFn)fn, &map_carry, (const float*)carry->obs, n, 128);
-    if (rc == PB_OK) rc = ro_make_map((RoEncodeTiledFn)fn, &map_w, w_enc, 128, 128);
+    int rc = pb_tma_map_128(&map_obs, obs, (int64_t)horizon * n, 128, RO_ENVS);
+    if (rc == PB_OK) rc = pb_tma_map_128(&map_carry, (const float*)carry->obs, n, 128, RO_ENVS);
+    if (rc == PB_OK) rc = pb_tma_map_128(&map_w, w_enc, 128, 128, RO_ENVS);
     if (rc != PB_OK) return rc;
     BreakoutState* st = (BreakoutState*)env->kind;
     cudaStream_t s = (cudaStream_t)stream;

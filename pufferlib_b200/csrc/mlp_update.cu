@@ -29,16 +29,14 @@
 // [dW_enc (hid x feat) | dW_heads (8 x hid) | db_enc | db_heads] of clean_pufferl._DefaultMLPUpdate, leaving per-block
 // sums of squares for pb_clip_adam_parts.
 //
-// Epilogue precision (pb_mlp_update_set_variant): variant 2 (default) takes the head, g^T and dW_heads products on mma.sync
-// with TF32 operands and fp32 accumulation -- the precision class of torch.set_float32_matmul_precision('high'), which
-// clean_pufferl sets; variant 1 forms the head and g^T products with fp32 FFMAs.  The dPre-to-HBM mode (dW_enc by the
-// caller) runs the variant-1 epilogue.  Every mbarrier wait is bounded (tma.cuh: __trap instead of a hang).
+// Epilogue precision: the head, g^T and dW_heads products run on mma.sync with TF32 operands and fp32 accumulation -- the
+// precision class of torch.set_float32_matmul_precision('high'), which clean_pufferl sets.  Every mbarrier wait is bounded
+// (tma.cuh: __trap instead of a hang).
 //
 // Built with -DPB_UPDATE_PHASES (bench_update.py builds such a library of its own), lane 0 of each warpgroup records
 // clock64() at the phase boundaries of the first PH_TILES tiles of its CTA into a buffer set by
 // pb_mlp_update_set_phase_buffer; pb_mlp_update_phase_names names the phases.  Without the macro none of that code
 // exists (the SASS of the library is the same with and without it).
-#include <cuda.h>
 #include <stdlib.h>
 
 #include "pb_common.cuh"
@@ -87,7 +85,6 @@ struct FusedParams {
     float* part_dw;            // [grid][FEAT][HID]
     float* part_tail;          // [grid][TAIL]
     double* stats;             // [8]
-    float* dpre_out;           // DW_KERNEL = false: dPre [m][128] (slab-major rows) for the caller's dW GEMM
     float* dbg_hidden;         // nullable [m][128]
     float* dbg_dpre;           // nullable [m][128]
     float* dbg_dout;           // nullable [m][8]
@@ -108,28 +105,6 @@ constexpr int PH_TILES = 32, PH_N = 8;                 // [grid][warpgroups][PH_
 #else
 #define PB_PHASE(k, idx) do {} while (0)
 #endif
-
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-            smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-        : "memory");
-}
-
-__device__ __forceinline__ uint32_t to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return r;
-}
-
-// mma.sync m16n8k8 TF32: a0 (g, t)  a1 (g + 8, t)  a2 (g, t + 4)  a3 (g + 8, t + 4);  b0 (k = t, n = g)  b1 (k = t + 4, n = g);
-// c0 c1 (g, 2t + {0,1})  c2 c3 (g + 8, 2t + {0,1})      [g = lane >> 2, t = lane & 3]
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 // byte offset of element (hidden unit n, tile row l) in the relu(h)^T / dPre^T buffer: two K-major SWIZZLE_128B blocks of
 // [128 hidden units][32 rows] (rows 0..31, 32..63) -- the layout of a wgmma B operand with N = hidden units, K = rows
@@ -208,10 +183,7 @@ __device__ __forceinline__ RowStats ppo_row_sub(float z_lo, float z_hi, int sub,
     return s;
 }
 
-// TF32_EPI  : head / g^T / dW_heads products on mma.sync with TF32 operands (variant 2); else fp32 FFMAs for the head and
-//             g^T products and TF32 (round-to-nearest operands) for dW_heads (variant 1)
-// DW_KERNEL : dW_enc^T accumulated on the tensor core; else dPre goes to HBM (p.dpre_out) and the caller forms dW_enc
-template <bool TF32_EPI, bool DW_KERNEL>
+// The head, g^T and dW_heads products take TF32 operands on mma.sync; dW_enc^T is accumulated on the tensor core (wgmma)
 __global__ void __launch_bounds__(THREADS, 1)
 k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const FusedParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -254,9 +226,8 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
     const int lr = tid >> 2, sub = tid & 3;
     const float bh_lo = p.b_heads[sub], bh_hi = p.b_heads[sub + 4];
     // W_heads operands, resident in registers
-    uint32_t hb[8][2], ga[4];            // TF32_EPI: heads B fragments (hidden half warp >> 2), g^T A fragment
-    float whr[2][NO];                    // fp32 epilogue: W_heads[a][hr0], W_heads[a][hr1]
-    if (TF32_EPI) {
+    uint32_t hb[8][2], ga[4];            // heads B fragments (hidden half warp >> 2), g^T A fragment
+    {
         const int hh = warp >> 2;
 #pragma unroll
         for (int ks = 0; ks < 8; ++ks) {
@@ -267,12 +238,6 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
         ga[1] = to_tf32(wh[t * HID + hr1]);
         ga[2] = to_tf32(wh[(t + 4) * HID + hr0]);
         ga[3] = to_tf32(wh[(t + 4) * HID + hr1]);
-    } else {
-#pragma unroll
-        for (int a = 0; a < NO; ++a) {
-            whr[0][a] = wh[a * HID + hr0];
-            whr[1][a] = wh[a * HID + hr1];
-        }
     }
 
     float dwacc[64];                     // dW_enc^T [feature 64wg + 16wq + g (+8)][hidden unit 8j + 2t (+1)]; the first
@@ -334,7 +299,7 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
         PB_PHASE(it, 0);
         const uint8_t* xs = smem + SM_X + s * X_TILE_BYTES;
         // the forward of this tile is done; the dW_enc product of the previous tile (committed after it) may still run
-        if (DW_KERNEL && it > 0) wgmma_wait<1>();
+        if (it > 0) wgmma_wait<1>();
         else wgmma_wait<0>();
         wgmma_fence_acc(h);
         float hv[32];                            // the epilogue works on a copy: h stays the forward's accumulator only
@@ -367,7 +332,7 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
         PB_PHASE(it, 2);
 
         // ---- 3. head products: out[row][a] = relu(h)[row] . W_heads[a]
-        if (TF32_EPI) {      // warp: rows 16(warp & 3) .. +15, hidden half warp >> 2; partial sums of the two halves to outp
+        {                    // warp: rows 16(warp & 3) .. +15, hidden half warp >> 2; partial sums of the two halves to outp
             const int l0 = 16 * (warp & 3) + g, hh = warp >> 2;
             float c[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -381,18 +346,6 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
             }
             *reinterpret_cast<float2*>(outp + (hh * TILE_M + l0) * NO + 2 * t) = make_float2(c[0], c[1]);
             *reinterpret_cast<float2*>(outp + (hh * TILE_M + l0 + 8) * NO + 2 * t) = make_float2(c[2], c[3]);
-        } else {             // thread = (row, pair of heads), fp32 FFMAs over all 128 hidden units
-            const int l = tid & (TILE_M - 1), a0 = 2 * (tid >> 6);
-            float o0 = 0.f, o1 = 0.f;
-            if (a0 <= p.n_act) {
-#pragma unroll 8
-                for (int n = 0; n < HID; ++n) {
-                    const float rh = *reinterpret_cast<const float*>(gbuf + g_off(n, l));
-                    o0 = fmaf(rh, wh[a0 * HID + n], o0);
-                    o1 = fmaf(rh, wh[(a0 + 1) * HID + n], o1);
-                }
-            }
-            *reinterpret_cast<float2*>(outp + l * NO + a0) = make_float2(o0, o1);
         }
         __syncthreads();
         PB_PHASE(it, 3);
@@ -400,10 +353,8 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
         // ---- 4. the loss row math -> dOut of the tile
         {
             float z_lo = bh_lo + outp[lr * NO + sub], z_hi = bh_hi + outp[lr * NO + sub + 4];
-            if (TF32_EPI) {
-                z_lo += outp[(TILE_M + lr) * NO + sub];
-                z_hi += outp[(TILE_M + lr) * NO + sub + 4];
-            }
+            z_lo += outp[(TILE_M + lr) * NO + sub];
+            z_hi += outp[(TILE_M + lr) * NO + sub + 4];
             const float r_ = p.returns ? ret : adv + old_v;       // returns = raw advantages + old values (:476-481)
             const float a_ = (adv - adv_mean) * adv_rstd;
             float g_lo, g_hi;
@@ -430,39 +381,17 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
         float dp[32];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            if (TF32_EPI) {
-                float c[4] = {0.f, 0.f, 0.f, 0.f};
-                mma_tf32(c, ga, __float_as_uint(dos[(8 * j + g) * NO + t]), __float_as_uint(dos[(8 * j + g) * NO + t + 4]));
-                dp[4 * j] = c[0]; dp[4 * j + 1] = c[1]; dp[4 * j + 2] = c[2]; dp[4 * j + 3] = c[3];
-            } else {
-                const int l = 8 * j + 2 * t;
-                const float4 d0a = *reinterpret_cast<const float4*>(dos + l * NO), d0b = *reinterpret_cast<const float4*>(dos + l * NO + 4);
-                const float4 d1a = *reinterpret_cast<const float4*>(dos + (l + 1) * NO), d1b = *reinterpret_cast<const float4*>(dos + (l + 1) * NO + 4);
-                const float d0[8] = {d0a.x, d0a.y, d0a.z, d0a.w, d0b.x, d0b.y, d0b.z, d0b.w};
-                const float d1[8] = {d1a.x, d1a.y, d1a.z, d1a.w, d1b.x, d1b.y, d1b.z, d1b.w};
-                float s00 = 0.f, s01 = 0.f, s10 = 0.f, s11 = 0.f;
-#pragma unroll
-                for (int a = 0; a < NO; ++a) {
-                    s00 = fmaf(d0[a], whr[0][a], s00);
-                    s01 = fmaf(d1[a], whr[0][a], s01);
-                    s10 = fmaf(d0[a], whr[1][a], s10);
-                    s11 = fmaf(d1[a], whr[1][a], s11);
-                }
-                dp[4 * j] = s00; dp[4 * j + 1] = s01; dp[4 * j + 2] = s10; dp[4 * j + 3] = s11;
-            }
+            float c[4] = {0.f, 0.f, 0.f, 0.f};
+            mma_tf32(c, ga, __float_as_uint(dos[(8 * j + g) * NO + t]), __float_as_uint(dos[(8 * j + g) * NO + t + 4]));
+            dp[4 * j] = c[0]; dp[4 * j + 1] = c[1]; dp[4 * j + 2] = c[2]; dp[4 * j + 3] = c[3];
 #pragma unroll
             for (int e = 0; e < 4; ++e) dp[4 * j + e] = hv[4 * j + e] > 0.f ? dp[4 * j + e] : 0.f;
             be_acc[0] += dp[4 * j] + dp[4 * j + 1];
             be_acc[1] += dp[4 * j + 2] + dp[4 * j + 3];
             const float b0 = dos[(8 * j + 2 * t) * NO + g], b1 = dos[(8 * j + 2 * t + 1) * NO + g];
-            if (TF32_EPI) {
-                const uint32_t a[4] = {__float_as_uint(hv[4 * j]), __float_as_uint(hv[4 * j + 2]), __float_as_uint(hv[4 * j + 1]),
-                                       __float_as_uint(hv[4 * j + 3])};
-                mma_tf32(dwh, a, __float_as_uint(b0), __float_as_uint(b1));
-            } else {
-                const uint32_t a[4] = {to_tf32(hv[4 * j]), to_tf32(hv[4 * j + 2]), to_tf32(hv[4 * j + 1]), to_tf32(hv[4 * j + 3])};
-                mma_tf32(dwh, a, to_tf32(b0), to_tf32(b1));
-            }
+            const uint32_t a[4] = {__float_as_uint(hv[4 * j]), __float_as_uint(hv[4 * j + 2]), __float_as_uint(hv[4 * j + 1]),
+                                   __float_as_uint(hv[4 * j + 3])};
+            mma_tf32(dwh, a, __float_as_uint(b0), __float_as_uint(b1));
             const int l = 8 * j + 2 * t;
             if (p.dbg_dpre) {
 #pragma unroll
@@ -471,86 +400,60 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
                     if (le < rows_left) p.dbg_dpre[(i0 + le) * HID + he] = dp[4 * j + e];
                 }
             }
-            // dPre^T over relu(h)^T (every read of relu(h)^T, step 3, is behind the last barrier): TF32 rounded to nearest as
-            // the operand of the dW product, or exact for the row writes of the dPre-to-HBM mode
-            if (DW_KERNEL) {
-                *reinterpret_cast<uint2*>(gbuf + g_off(hr0, l)) = make_uint2(to_tf32(dp[4 * j]), to_tf32(dp[4 * j + 1]));
-                *reinterpret_cast<uint2*>(gbuf + g_off(hr1, l)) = make_uint2(to_tf32(dp[4 * j + 2]), to_tf32(dp[4 * j + 3]));
-            } else {
-                *reinterpret_cast<float2*>(gbuf + g_off(hr0, l)) = make_float2(dp[4 * j], dp[4 * j + 1]);
-                *reinterpret_cast<float2*>(gbuf + g_off(hr1, l)) = make_float2(dp[4 * j + 2], dp[4 * j + 3]);
-            }
+            // dPre^T over relu(h)^T (every read of relu(h)^T, step 3, is behind the last barrier), TF32 rounded to nearest as
+            // the operand of the dW product
+            *reinterpret_cast<uint2*>(gbuf + g_off(hr0, l)) = make_uint2(to_tf32(dp[4 * j]), to_tf32(dp[4 * j + 1]));
+            *reinterpret_cast<uint2*>(gbuf + g_off(hr1, l)) = make_uint2(to_tf32(dp[4 * j + 2]), to_tf32(dp[4 * j + 3]));
         }
 
         // ---- 6. dW_enc^T [64wg .. 64wg + 63][128] += x^T . dPre  (M = features, N = hidden units, K = 64 rows).  Both
         //         operands are rounded to nearest TF32 (truncation would bias a sum over the whole minibatch)
         PB_PHASE(it, 5);
-        if (DW_KERNEL) {
-            fence_proxy_async_smem();            // dPre^T written by the generic proxy, read by the tensor core
-            wgmma_wait<0>();                     // the previous tile's dW_enc product: its A registers and buffer are free
+        fence_proxy_async_smem();                // dPre^T written by the generic proxy, read by the tensor core
+        wgmma_wait<0>();                         // the previous tile's dW_enc product: its A registers and buffer are free
 #pragma unroll
-            for (int ks = 0; ks < 8; ++ks)
+        for (int ks = 0; ks < 8; ++ks)
 #pragma unroll
-                for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
-            __syncthreads();                     // dPre^T of both warpgroups is in the buffer
-            if (it + 1 < n_my) forward(it + 1);
-            const int f0 = 64 * wg + 16 * wq + g;
+            for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
+        __syncthreads();                         // dPre^T of both warpgroups is in the buffer
+        if (it + 1 < n_my) forward(it + 1);
+        const int f0 = 64 * wg + 16 * wq + g;
 #pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {
-                const int r0 = 8 * ks + t;
-                xa[ks][0] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0)));
-                xa[ks][1] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0 + 8)));
-                xa[ks][2] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0)));
-                xa[ks][3] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0 + 8)));
-            }
-            wgmma_fence();
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)
-                wgmma_m64n128k8_rs(dwacc, xa[ks], wgmma_desc_sw128(g_addr + (ks >> 2) * G_KBLK_BYTES + (ks & 3) * 32),
-                                   (it | ks) ? 1 : 0);
-            wgmma_commit();
-            PB_PHASE(it, 6);
-        } else {
-            // ---- 6'. dPre rows to HBM: warp w writes rows 8w .. 8w + 7, one whole 512-byte row per store instruction
-            __syncthreads();
-#pragma unroll
-            for (int k = 0; k < TILE_M / 8; ++k) {
-                const int l = 8 * warp + k;
-                if (l < rows_left) {
-                    const int n = 4 * lane;
-                    const float4 v = make_float4(*reinterpret_cast<const float*>(gbuf + g_off(n, l)),
-                                                 *reinterpret_cast<const float*>(gbuf + g_off(n + 1, l)),
-                                                 *reinterpret_cast<const float*>(gbuf + g_off(n + 2, l)),
-                                                 *reinterpret_cast<const float*>(gbuf + g_off(n + 3, l)));
-                    __stcs(reinterpret_cast<float4*>(p.dpre_out + (i0 + l) * HID + n), v);
-                }
-            }
-            if (it + 1 < n_my) forward(it + 1);
+        for (int ks = 0; ks < 8; ++ks) {
+            const int r0 = 8 * ks + t;
+            xa[ks][0] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0)));
+            xa[ks][1] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0 + 8)));
+            xa[ks][2] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0)));
+            xa[ks][3] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0 + 8)));
         }
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)
+            wgmma_m64n128k8_rs(dwacc, xa[ks], wgmma_desc_sw128(g_addr + (ks >> 2) * G_KBLK_BYTES + (ks & 3) * 32),
+                               (it | ks) ? 1 : 0);
+        wgmma_commit();
+        PB_PHASE(it, 6);
         __syncthreads();                         // every read of x stage s is done
         if (tid == 0 && it + NSTAGE < n_my) {
             fence_proxy_async_smem();
             issue(it + NSTAGE);
         }
     }
-    if (DW_KERNEL) {                             // the last tile's dW_enc product
-        wgmma_wait<0>();
-        wgmma_fence_acc(dwacc);
+    // the last tile's dW_enc product
+    wgmma_wait<0>();
+    wgmma_fence_acc(dwacc);
 #pragma unroll
-        for (int ks = 0; ks < 8; ++ks)
+    for (int ks = 0; ks < 8; ++ks)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
-    }
+        for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
 
     // ================= per-CTA partials =================
-    if (DW_KERNEL) {
-        float* pd = p.part_dw + (int64_t)blockIdx.x * FEAT * HID;
-        const int f0 = 64 * wg + 16 * wq + g;
+    const int f0 = 64 * wg + 16 * wq + g;
+    float* pd = p.part_dw + (int64_t)blockIdx.x * FEAT * HID;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            *reinterpret_cast<float2*>(pd + f0 * HID + 8 * j + 2 * t) = make_float2(dwacc[4 * j], dwacc[4 * j + 1]);
-            *reinterpret_cast<float2*>(pd + (f0 + 8) * HID + 8 * j + 2 * t) = make_float2(dwacc[4 * j + 2], dwacc[4 * j + 3]);
-        }
+    for (int j = 0; j < 16; ++j) {
+        *reinterpret_cast<float2*>(pd + f0 * HID + 8 * j + 2 * t) = make_float2(dwacc[4 * j], dwacc[4 * j + 1]);
+        *reinterpret_cast<float2*>(pd + (f0 + 8) * HID + 8 * j + 2 * t) = make_float2(dwacc[4 * j + 2], dwacc[4 * j + 3]);
     }
     float* pt = p.part_tail + (int64_t)blockIdx.x * TAIL;
     pt[(2 * t) * HID + hr0] = dwh[0];
@@ -599,10 +502,6 @@ __global__ void __launch_bounds__(256) k_update_reduce(const float* __restrict__
     const int e = blockIdx.x * 64 + (threadIdx.x & 63), grp = threadIdx.x >> 6;
     constexpr int NDW = FEAT * HID;
     float s = 0.f;
-    if (e < NDW && !part_dw) {                // dW_enc is formed by the caller (dPre went to HBM); whole blocks: NDW % 64 == 0
-        if (threadIdx.x == 0) sumsq_part[blockIdx.x] = 0.0;
-        return;
-    }
     if (e < NDW + TAIL) {
         const float* src = e < NDW ? part_dw + e : part_tail + (e - NDW);
         const int64_t stride = e < NDW ? NDW : TAIL;
@@ -629,26 +528,7 @@ __global__ void __launch_bounds__(256) k_update_reduce(const float* __restrict__
     if (threadIdx.x == 0) sumsq_part[blockIdx.x] = sq[0] + sq[1];
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// 2-D map of a [rows][128] fp32 matrix (row stride in floats), boxes of [box_rows][32 floats] with the 128-byte swizzle
-int make_map2(EncodeTiledFn fn, CUtensorMap* map, const float* base, int64_t rows, int64_t row_stride_floats, int box_rows) {
-    const cuuint64_t dims[2] = {(cuuint64_t)FEAT, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)row_stride_floats * 4};
-    const cuuint32_t box[2] = {(cuuint32_t)KBLK, (cuuint32_t)box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    PB_REQUIRE(r == CUDA_SUCCESS, PB_ERR_CUDA, "cuTensorMapEncodeTiled failed: %d", (int)r);
-    return PB_OK;
-}
-
 int num_sms() { return pb_num_sms(); }
-
-int g_update_variant = 2;     // 1 = fp32 head / g^T products, 2 = TF32 mma.sync epilogue
 
 #ifdef PB_UPDATE_PHASES
 unsigned long long* g_phases = nullptr;
@@ -677,12 +557,6 @@ extern "C" const char* pb_mlp_update_phase_names(void) {
 }
 #endif
 
-extern "C" int pb_mlp_update_set_variant(int32_t variant) {
-    PB_REQUIRE(variant == 1 || variant == 2, PB_ERR_INVALID, "pb_mlp_update_set_variant: 1 or 2");
-    g_update_variant = variant;
-    return PB_OK;
-}
-
 constexpr int REDUCE_BLOCKS = (FEAT * HID + TAIL + 63) / 64;
 
 // workspace: per-CTA partials [SMs][FEAT * HID + TAIL] floats | REDUCE_BLOCKS doubles (sums of squares of the gradient)
@@ -705,6 +579,7 @@ extern "C" int pb_mlp_update_fused(const float* x, int64_t ldx, int64_t slab_row
     PB_REQUIRE(x && w_enc && b_enc && w_heads && b_heads && actions && old_logprobs && advantages && grad_flat && stats8 &&
                    workspace && (returns || old_values),
                PB_ERR_INVALID, "pb_mlp_update_fused: null pointer");
+    PB_REQUIRE(!dpre_out, PB_ERR_INVALID, "pb_mlp_update_fused: dpre_out must be null (dW_enc is formed in the kernel)");
     PB_REQUIRE(n_slabs == 1 || row_slab_stride >= slab_rows, PB_ERR_INVALID, "pb_mlp_update_fused: row slabs overlap");
     PB_REQUIRE(slab_rows >= 1 && n_slabs >= 1 && n_act >= 1 && n_act <= 7 && (!clip_vloss || old_values), PB_ERR_INVALID,
                "pb_mlp_update_fused: bad sizes (slab_rows %lld, n_slabs %d, n_act %d)", (long long)slab_rows, n_slabs, n_act);
@@ -713,18 +588,13 @@ extern "C" int pb_mlp_update_fused(const float* x, int64_t ldx, int64_t slab_row
     PB_REQUIRE(n_slabs == 1 || slab_stride_rows >= slab_rows, PB_ERR_INVALID, "pb_mlp_update_fused: slabs overlap");
     PB_REQUIRE(workspace_bytes >= pb_mlp_update_workspace_bytes(), PB_ERR_INVALID, "pb_mlp_update_fused: workspace too small");
     PB_REQUIRE(!dbg_hidden || dbg_dpre, PB_ERR_INVALID, "pb_mlp_update_fused: dbg_hidden needs dbg_dpre");
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qr;
-    PB_REQUIRE(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) == cudaSuccess && fn &&
-                   qr == cudaDriverEntryPointSuccess,
-               PB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
     const int64_t tiles_per_slab = (slab_rows + TILE_M - 1) / TILE_M;
     const int64_t n_tiles = tiles_per_slab * n_slabs;
     const int64_t map_rows = (int64_t)(n_slabs - 1) * slab_stride_rows + slab_rows;
     PB_REQUIRE(n_tiles <= 0x7FFFFFFF && map_rows <= 0x7FFFFFFF, PB_ERR_UNSUPPORTED, "pb_mlp_update_fused: too many rows");
     alignas(64) CUtensorMap map_x, map_w;
-    int rc = make_map2((EncodeTiledFn)fn, &map_x, x, map_rows, ldx, TILE_M);
-    if (rc == PB_OK) rc = make_map2((EncodeTiledFn)fn, &map_w, w_enc, HID, FEAT, HID);
+    int rc = pb_tma_map_128(&map_x, x, map_rows, ldx, TILE_M);
+    if (rc == PB_OK) rc = pb_tma_map_128(&map_w, w_enc, HID, FEAT, HID);
     if (rc != PB_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     const int grid = n_tiles < num_sms() ? (int)n_tiles : num_sms();
@@ -736,23 +606,19 @@ extern "C" int pb_mlp_update_fused(const float* x, int64_t ldx, int64_t slab_row
     p.clip = clip_coef; p.vclip = vf_clip_coef; p.vf_coef = vf_coef; p.ent_coef = ent_coef; p.clip_vloss = clip_vloss;
     p.part_dw = (float*)workspace; p.part_tail = (float*)workspace + (size_t)num_sms() * FEAT * HID;
     p.w_heads = w_heads; p.b_enc = b_enc; p.b_heads = b_heads;
-    p.stats = stats8; p.dpre_out = dpre_out; p.dbg_hidden = dbg_hidden; p.dbg_dpre = dbg_dpre; p.dbg_dout = dbg_dout;
+    p.stats = stats8; p.dbg_hidden = dbg_hidden; p.dbg_dpre = dbg_dpre; p.dbg_dout = dbg_dout;
 #ifdef PB_UPDATE_PHASES
     p.phases = g_phases;
 #endif
     PB_CUDA(cudaMemsetAsync(stats8, 0, 8 * sizeof(double), s));
     static bool attr_set = false;
     if (!attr_set) {
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-        PB_CUDA(cudaFuncSetAttribute(k_mlp_update<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
+        PB_CUDA(cudaFuncSetAttribute(k_mlp_update, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
         attr_set = true;
     }
-    if (dpre_out) k_mlp_update<false, false><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_w, p);
-    else if (g_update_variant == 2) k_mlp_update<true, true><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_w, p);
-    else k_mlp_update<false, true><<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_w, p);
+    k_mlp_update<<<grid, THREADS, SMEM_TOTAL, s>>>(map_x, map_w, p);
     PB_LAUNCH_CHECK();
-    k_update_reduce<<<REDUCE_BLOCKS, 256, 0, s>>>(dpre_out ? nullptr : p.part_dw, p.part_tail, grid, grad_flat,
+    k_update_reduce<<<REDUCE_BLOCKS, 256, 0, s>>>(p.part_dw, p.part_tail, grid, grad_flat,
                                                   reinterpret_cast<double*>((char*)workspace + pb_mlp_update_sumsq_offset()));
     PB_LAUNCH_CHECK();
     return PB_OK;

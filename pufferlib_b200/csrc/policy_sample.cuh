@@ -1,6 +1,5 @@
 // policy_sample.cuh -- pieces shared by every kernel that samples actions (policy_mlp.cu, policy_lstm.cu, sample.cu and
-// the persistent rollout kernel of env_breakout.cu):
-//   * to_tf32 / mma_tf32: round-to-nearest TF32 conversion (cvt.rna) and the mma.sync m16n8k8 TF32 tile product;
+// the persistent rollout kernel of env_breakout.cu), with the tensor-core helpers of wgmma.cuh (to_tf32, mma_tf32):
 //   * pb_policy_uniform: the counter-based uniform of a row, u = mix(seed, step counter, row) in [0, 1), 24 bits;
 //   * pb_sample_row<NC>: one row's sampling epilogue over NC padded head outputs z[0..NC) = n_act logits | value | pad
 //     (reference frameworks/cleanrl.py:25-47): lse = max z + log sum exp(z - max z), the probabilities
@@ -16,17 +15,7 @@
 //     finite as there).
 #pragma once
 #include "pb_common.cuh"
-
-__device__ __forceinline__ uint32_t to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return r;
-}
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
+#include "wgmma.cuh"
 
 __device__ __forceinline__ float pb_policy_uniform(uint64_t seed, uint64_t offset, int64_t row) {
     const uint32_t rnd = pb_mix32(seed * 0x9E3779B97F4A7C15ull + offset * 0xD1B54A32D192ED03ull +

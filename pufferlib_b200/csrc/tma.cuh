@@ -1,9 +1,13 @@
-// tma.cuh -- 1-D bulk async copies (TMA engine, SASS UBLKCP) + mbarrier helpers, inline PTX for sm_90a.
-// Used to stage whole image-observation rows through shared memory: global -> shared (mbarrier complete_tx),
-// shared -> global (bulk_group).  Addresses and sizes must be multiples of 16 bytes.
+// tma.cuh -- bulk async copies (TMA engine, SASS UBLKCP) + mbarrier helpers, inline PTX for sm_90a.
+// 1-D copies stage whole image-observation rows through shared memory: global -> shared (mbarrier complete_tx),
+// shared -> global (bulk_group).  Addresses and sizes must be multiples of 16 bytes.  2-D copies move boxes of a tensor
+// map; pb_tma_map_128 builds the map of the fp32 [rows][128] matrices that the wgmma kernels tile.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "pb_common.cuh"
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -49,6 +53,21 @@ __device__ __forceinline__ void tma_store_1d(void* dst_gmem, const void* src_sme
                  "r"(bytes)
                  : "memory");
 }
+// global -> shared: the box of `map` at coordinates (c0 innermost, c1), completion signalled on an mbarrier
+__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+            smem_u32(dst)),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+        : "memory");
+}
+// shared -> global: one box of `map`, tracked by the bulk async-group of the issuing thread
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, int c0, int c1, const void* src) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%1, %2}], [%3];" ::"l"(
+                     reinterpret_cast<uint64_t>(map)),
+                 "r"(c0), "r"(c1), "r"(smem_u32(src))
+                 : "memory");
+}
 __device__ __forceinline__ void tma_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_wait_read() {  // shared-memory sources of all but the N newest groups are free
@@ -60,3 +79,26 @@ __device__ __forceinline__ void tma_wait_all() {
 }
 // make generic-proxy writes to shared memory visible to the async proxy (before a bulk store reads them)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// Host: the 2-D tensor map of a [rows][128] fp32 matrix whose rows are row_stride floats apart, in boxes of [box_rows][32
+// floats] with the 128-byte swizzle (the K-major SWIZZLE_128B tiles of wgmma.cuh).  PB_OK, or PB_ERR_CUDA with the message
+// set when the driver entry point is missing or refuses the map.
+inline int pb_tma_map_128(CUtensorMap* map, const float* base, int64_t rows, int64_t row_stride, int box_rows) {
+    typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                      const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                      CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qr;
+    PB_REQUIRE(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) == cudaSuccess && fn &&
+                   qr == cudaDriverEntryPointSuccess,
+               PB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+    const cuuint64_t dims[2] = {128, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)row_stride * 4};
+    const cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
+    const cuuint32_t estr[2] = {1, 1};
+    const CUresult r = ((EncodeTiledFn)fn)(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides,
+                                           box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    PB_REQUIRE(r == CUDA_SUCCESS, PB_ERR_CUDA, "cuTensorMapEncodeTiled failed: %d", (int)r);
+    return PB_OK;
+}

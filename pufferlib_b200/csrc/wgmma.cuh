@@ -1,4 +1,5 @@
-// wgmma.cuh -- Hopper warpgroup MMA (wgmma.mma_async, sm_90a) wrappers for TF32 operands with fp32 accumulation.
+// wgmma.cuh -- tensor-core helpers for TF32 operands with fp32 accumulation: round-to-nearest TF32 conversion, the warp-level
+// mma.sync m16n8k8 tile product, and the Hopper warpgroup MMA (wgmma.mma_async, sm_90a) wrappers.
 //
 // A warpgroup (4 consecutive warps, the first one a multiple of 4) computes D[64][N] += A[64][8] . B[8][N]^T per instruction.
 // Fragment layouts (PTX ISA, "wgmma .tf32" register fragments), g = lane >> 2, t = lane & 3, warp w of the warpgroup:
@@ -10,6 +11,21 @@
 // The accumulator and A registers are in flight between an MMA and wgmma_wait: every caller waits before touching them.
 #pragma once
 #include <stdint.h>
+
+// fp32 -> TF32 rounded to nearest (cvt.rna), for operands the tensor core would otherwise truncate
+__device__ __forceinline__ uint32_t to_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r;
+}
+
+// mma.sync m16n8k8 TF32: a0 (g, t)  a1 (g + 8, t)  a2 (g, t + 4)  a3 (g + 8, t + 4);  b0 (k = t, n = g)  b1 (k = t + 4, n = g);
+// c0 c1 (g, 2t + {0,1})  c2 c3 (g + 8, 2t + {0,1})      [g = lane >> 2, t = lane & 3]
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
 
 // shared-memory matrix descriptor, SWIZZLE_128B K-major: start >> 4 | LBO (unused for swizzled K-major: 1) << 16 |
 // SBO = 1024 B between 8-row groups << 32 | layout type 1 (128-byte swizzle) << 62.  Advancing K by 8 floats inside a

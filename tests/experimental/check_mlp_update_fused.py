@@ -2,7 +2,7 @@
 stage, end to end against float64 autograd, the sums of squares of the reduce step), then timing at the bench minibatch.  Not
 collected by pytest (tests/test_gpu_update_kernel.py runs the same cases); run by hand on an H100 under a timeout:
 
-    timeout 200 python tests/experimental/check_mlp_update_fused.py [--variant 1|2]
+    timeout 200 python tests/experimental/check_mlp_update_fused.py
 """
 import os
 import sys
@@ -30,15 +30,12 @@ def timing():
     act = torch.randint(0, n_act, (m,), device=dev)
     olp = -torch.rand(m, device=dev) - 0.5
     adv, ret, oval = torch.randn(m, device=dev), torch.randn(m, device=dev), torch.randn(m, device=dev)
-    dpre_t = torch.empty(m, 128, device=dev)
     ws = workspace(dev)
-    for name, (rows, slabs, stride, dpo) in (('1 slab of 524288 rows, dW in kernel', (m, 1, m, None)),
-                                             ('2 slabs of 262144 rows, dW in kernel', (m // 2, 2, 2 * m, None)),
-                                             ('2 slabs of 262144 rows, dPre to HBM', (m // 2, 2, 2 * m, dpre_t))):
+    for name, (rows, slabs, stride) in (('1 slab of 524288 rows', (m, 1, m)), ('2 slabs of 262144 rows', (m // 2, 2, 2 * m))):
         def fn(k):
             off = (k % 4) * (m // 2) if slabs == 2 else (k % 4) * m
             return fused(xbuf[off:], 128, rows, stride, slabs, w_enc, b_enc, w_cat, b_cat, act, olp, adv, ret, oval, n_act, False,
-                         dpre_out=dpo, ws=ws)
+                         ws=ws)
         for k in range(3):
             fn(k)
         torch.cuda.synchronize()
@@ -53,17 +50,12 @@ def timing():
 
 
 def main():
-    variant = int(sys.argv[sys.argv.index('--variant') + 1]) if '--variant' in sys.argv else 2
-    print('update kernel variant', variant, flush=True)
     ok = True
     for args in SHAPES:
-        ok &= case(*args, variant=variant)
+        ok &= case(*args)
     for *args, nm in DIRECT:
-        ok &= case(*args, variant=variant, nm=nm, returns=False, adv_norm=True)
+        ok &= case(*args, nm=nm, returns=False, adv_norm=True)
     print('ALL OK' if ok else 'SOME MISMATCH', flush=True)
-    if variant != 2:
-        from pufferlib_b200 import _native
-        _native.check(_native.lib().pb_mlp_update_set_variant(variant))
     timing()
     print('done')
 

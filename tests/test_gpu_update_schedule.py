@@ -3,7 +3,7 @@ a ring of NSTAGE x tiles), with the stage-by-stage checks of tests/util_update.p
   * an odd number of tiles on every CTA;
   * slabs shorter than one tile (every tile ragged) and slabs whose row count is not a multiple of the tile;
   * enough tiles per CTA that every x stage goes round several times;
-and that the same launch twice gives a bitwise-equal gradient and the same per-block sums of squares (the loss statistics are
+each with the benchmark's loss coefficients and with clip_vloss off and other coefficients (util_update.CFG_ALT); and that the same launch twice gives a bitwise-equal gradient and the same per-block sums of squares (the loss statistics are
 left out: their fp64 atomicAdds land in no fixed order)."""
 import pytest
 import torch
@@ -25,10 +25,10 @@ def schedule_shapes():
             'many_tiles_per_cta': (8192, 8, 8192, 3, 24)}
 
 
-@pytest.mark.parametrize('variant', [2, 1])
+@pytest.mark.parametrize('coefs', ['bench', 'alt'])
 @pytest.mark.parametrize('shape', ['odd_tiles_per_cta', 'slabs_shorter_than_a_tile', 'ragged_slabs', 'many_tiles_per_cta'])
-def test_update_schedule_boundaries(shape, variant):
-    assert uu.case(*schedule_shapes()[shape], variant=variant)
+def test_update_schedule_boundaries(shape, coefs):
+    assert uu.case(*schedule_shapes()[shape], cfg=uu.CFG if coefs == 'bench' else uu.CFG_ALT)
 
 
 @pytest.mark.parametrize('slab_rows,n_slabs,slab_stride', [(4096 * 4 + 17, 4, 4096 * 8), (96, 1, 96)])

@@ -263,7 +263,8 @@ int pb_ppo_loss(const float* logits, int64_t logits_stride, const float* value, 
                 float* grad_value, int64_t grad_value_stride, double* stats8, void* stream);
 
 /* -- fused rollout-time policy step --------------------------------------------------------------------------------
- * For models.Default with 128 input features and 128 hidden units (pufferlib/models.py:12-62): encoder Linear + ReLU,
+ * For models.Default with 128 input features and 128, 256, 384 or 512 hidden units (pufferlib/models.py:12-62;
+ * PB_ERR_UNSUPPORTED before any launch otherwise): encoder Linear + ReLU,
  * both heads, sample_logits (frameworks/cleanrl.py:25-47) and the value / logprob / action row stores of
  * Experience.store (clean_pufferl.py:443-446) in ONE launch per env step; the hidden layer never leaves the SM
  * (mma.sync TF32 tensor-core tiles, fp32 accumulate).  w_heads / b_heads: the 8- or 16-row padded head matrix
@@ -385,7 +386,8 @@ int pb_rollout_debug_buffers(float* hidden, float* out);
  *   dpre[m][H]      = (dout[m][0..R-1] @ w_heads[R][H]) * (hidden > 0)                (heads dX + ReLU backward)
  *   grads_out       = [ dW_heads (R*H) | db_enc (H) = column sums of dpre | db_heads (R) = column sums of dout ]
  * dout holds the loss gradient w.r.t. the R padded head outputs (n_act logits, the value, zero padding) of the 8- or
- * 16-row padded head matrix w_heads, row stride dout_stride floats.  Deterministic (two-stage partial sums).  H = 128.
+ * 16-row padded head matrix w_heads, row stride dout_stride floats.  Deterministic (two-stage partial sums).
+ * H = 128, 256, 384 or 512 (PB_ERR_UNSUPPORTED before any launch otherwise).
  * Pointers 16-byte aligned.  pb_mlp_tail_workspace_bytes / pb_mlp_tail_backward: R = 8 (n_act <= 7); the _ex forms take
  * R = head_rows, 8 or 16 (16 for 8 <= n_act <= 15). */
 size_t pb_mlp_tail_workspace_bytes(int64_t m, int32_t hidden_size);

@@ -206,7 +206,8 @@ class _DefaultMLPUpdate:
         encoder GEMM (+bias+ReLU epilogue, one per slab) -> R-column head GEMM -> pb_ppo_loss (loss statistics +
         analytic dLoss/dOut) -> pb_mlp_tail_backward_ex (dPre, dW_heads, db_heads, db_enc) -> split-K dW_enc GEMM + sum
         [-> gradient all-reduce over ONE flat buffer when world_size > 1] -> pb_clip_adam -> pb_pack_heads,
-    with R = 8 head rows for n_act <= 7 and 16 for 8 <= n_act <= 15 (models.Default.head_matrix).
+    with R = 8 head rows for n_act <= 7 and 16 for 8 <= n_act <= 15 (models.Default.head_matrix), for 128 to 512 hidden
+    units (models.FAST_HIDDEN).
     train() passes each minibatch as Experience.minibatch() to forward_backward; where _fused_ok holds (update_plan asks
     it once per train() and sets used_fused; <= 7 actions) the chain is ONE kernel, pb_mlp_update_fused.
     Same math as the autograd path (tests/test_gpu_experience.py::test_manual_update_matches_autograd_update); the
@@ -222,7 +223,7 @@ class _DefaultMLPUpdate:
         if config.target_kl is not None or not getattr(data, 'own_optimizer', False):
             return False
         n_act, hid = model.decoder.weight.shape
-        if hid != 128 or n_act > 15 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
+        if hid not in models.FAST_HIDDEN or n_act > 15 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
             return False
         g = opt.param_groups[0]
         if len(opt.param_groups) != 1 or g.get('amsgrad') or g.get('weight_decay') or g.get('maximize'):
@@ -327,8 +328,8 @@ class _DefaultMLPUpdate:
 
     def _fused_ok(self, x, config):
         """pb_mlp_update_fused (csrc/mlp_update.cu): fp32 observations with exactly 128 features in equally spaced row
-        slabs and <= 7 actions (the 8-row head matrix) -- the C2 / C5 workload.  Everything else takes the kernel chain
-        below."""
+        slabs, 128 hidden units and <= 7 actions (the 8-row head matrix) -- the C2 / C5 workload.  Everything else
+        (256 to 512 hidden units included) takes the kernel chain below."""
         return (bool(getattr(config, 'fused_update', FUSED_UPDATE_DEFAULT)) and x.dtype == torch.float32 and x.shape[2] == 128
                 and self.hid == 128 and self.head_rows == 8 and x.stride(2) == 1 and x.stride(1) % 4 == 0 and x.data_ptr() % 16 == 0
                 and (x.shape[0] == 1 or (x.stride(0) % x.stride(1) == 0 and x.stride(0) >= x.shape[1] * x.stride(1))))

@@ -247,6 +247,188 @@ __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd_tma(const float* __
     }
 }
 
+// ---- H = 256, 384, 512: the same per-row plan over 128-column slices of the hidden layer, slice s = blockIdx.y.
+// Every output but db_heads is per hidden column, so a CTA of slice s reads columns [128s, 128s + 128) of its rows
+// (row stride H), reads each row's dOut once, and writes its columns of the block's [NO*H | H | NO] partial row; slice 0
+// also writes db_heads.  A slice's accumulators are those of the H = 128 kernels, so the registers, the reduction
+// buffer and the dynamic shared memory are theirs too.  The H = 128 kernels above are kept as they are.
+
+// index in the [NO*H | H | NO] partial row of entry j of a slice's [NO*128 | 128 | NO] accumulators
+template <int NO>
+__device__ __forceinline__ int64_t slice_partial_index(int j, int h, int col0) {
+    if (j < NO * 128) return (int64_t)(j >> 7) * h + col0 + (j & 127);
+    if (j < NO * 128 + 128) return (int64_t)NO * h + col0 + (j - NO * 128);
+    return (int64_t)NO * h + h + (j - NO * 128 - 128);
+}
+
+template <int NO>
+__global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd_slices(const float* __restrict__ dout, int64_t dout_stride,
+                                                                   const float* __restrict__ w_heads,   // [NO][h]
+                                                                   const float* __restrict__ hidden,    // [M][h]
+                                                                   float* __restrict__ dpre,            // [M][h]
+                                                                   float* __restrict__ partials, int64_t m, int h) {
+    constexpr int RSTRIDE = 8 * 128 + 128 + NO;   // NO / 8 passes of 8 dW rows, as k_mlp_tail_bwd<128, NO>
+    __shared__ float s_red[MT_WARPS][RSTRIDE];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int col0 = 128 * (int)blockIdx.y;
+    const float* hcol = hidden + col0 + 4 * lane;
+    float* dcol = dpre + col0 + 4 * lane;
+
+    float4 w[NO], acc_w[NO], acc_b = make_float4(0.f, 0.f, 0.f, 0.f);
+    float acc_o[NO];
+#pragma unroll
+    for (int k = 0; k < NO; ++k) {
+        w[k] = *reinterpret_cast<const float4*>(w_heads + (int64_t)k * h + col0 + 4 * lane);
+        acc_w[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        acc_o[k] = 0.f;
+    }
+    const int64_t row0 = (int64_t)blockIdx.x * ROWS_PER_BLOCK;
+    const int64_t row_end = min(row0 + ROWS_PER_BLOCK, m);
+#pragma unroll 2
+    for (int64_t r = row0 + warp; r < row_end; r += MT_WARPS) {
+        float d[NO];
+        tail_load_dout<NO>(dout + r * dout_stride, d);
+        const float4 hv = __ldcs(reinterpret_cast<const float4*>(hcol + r * h));
+        float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int k = 0; k < NO; ++k) {
+            acc_o[k] += d[k];
+            g.x = fmaf(d[k], w[k].x, g.x); g.y = fmaf(d[k], w[k].y, g.y);
+            g.z = fmaf(d[k], w[k].z, g.z); g.w = fmaf(d[k], w[k].w, g.w);
+            acc_w[k].x = fmaf(d[k], hv.x, acc_w[k].x); acc_w[k].y = fmaf(d[k], hv.y, acc_w[k].y);
+            acc_w[k].z = fmaf(d[k], hv.z, acc_w[k].z); acc_w[k].w = fmaf(d[k], hv.w, acc_w[k].w);
+        }
+        g.x = hv.x > 0.f ? g.x : 0.f; g.y = hv.y > 0.f ? g.y : 0.f;
+        g.z = hv.z > 0.f ? g.z : 0.f; g.w = hv.w > 0.f ? g.w : 0.f;
+        acc_b.x += g.x; acc_b.y += g.y; acc_b.z += g.z; acc_b.w += g.w;
+        __stcs(reinterpret_cast<float4*>(dcol + r * h), g);
+    }
+    // pass p: dW rows 8p..8p+7 at s_red[.][0, 1024); pass 0 also db_enc at [1024, 1152) and db_heads at [1152, 1152 + NO)
+    float* mine = s_red[warp];
+    float* out = partials + (int64_t)blockIdx.x * (NO * h + h + NO);
+#pragma unroll
+    for (int pass = 0; pass < NO / 8; ++pass) {
+        if (pass > 0) __syncthreads();
+#pragma unroll
+        for (int k = 0; k < 8; ++k) *reinterpret_cast<float4*>(mine + k * 128 + 4 * lane) = acc_w[8 * pass + k];
+        if (pass == 0) {
+            *reinterpret_cast<float4*>(mine + 8 * 128 + 4 * lane) = acc_b;
+            if (lane == 0)
+#pragma unroll
+                for (int k = 0; k < NO; ++k) mine[9 * 128 + k] = acc_o[k];
+        }
+        __syncthreads();
+        const int n = pass == 0 ? (blockIdx.y == 0 ? RSTRIDE : 9 * 128) : 8 * 128;
+        for (int j = threadIdx.x; j < n; j += MT_THREADS) {
+            float s = 0.f;
+#pragma unroll
+            for (int wq = 0; wq < MT_WARPS; ++wq) s += s_red[wq][j];
+            out[slice_partial_index<NO>(j < 8 * 128 ? 8 * 128 * pass + j : (NO - 8) * 128 + j, h, col0)] = s;
+        }
+    }
+}
+
+// TMA-staged slices (dout contiguous [M][NO]): the ring of k_mlp_tail_bwd_tma, filled with one 512-byte bulk copy per
+// row (the slice's columns of the row; lane l of warp 0 copies row l of the chunk) plus the chunk's dOut rows.
+template <int NO>
+__global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd_tma_slices(const float* __restrict__ dout,      // [M][NO]
+                                                                       const float* __restrict__ w_heads,   // [NO][h]
+                                                                       const float* __restrict__ hidden,    // [M][h]
+                                                                       float* __restrict__ dpre,            // [M][h]
+                                                                       float* __restrict__ partials, int64_t m, int h) {
+    constexpr int PS = NO * 128 + 128 + NO;   // a slice's accumulators
+    constexpr uint32_t H_BYTES = TT_CHUNK * 128 * 4, D_BYTES = TT_CHUNK * NO * 4;
+    extern __shared__ __align__(128) unsigned char dyn[];
+    float* s_h = reinterpret_cast<float*>(dyn);                                   // [STAGES][CHUNK][128]
+    float* s_d = reinterpret_cast<float*>(dyn + (size_t)TT_STAGES * H_BYTES);     // [STAGES][CHUNK][NO]
+    float* s_red = reinterpret_cast<float*>(dyn + (size_t)TT_STAGES * (H_BYTES + D_BYTES));   // [WARPS][PS]
+    __shared__ uint64_t bars[TT_STAGES];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int col0 = 128 * (int)blockIdx.y;
+
+    const int64_t row0 = (int64_t)blockIdx.x * ROWS_PER_BLOCK;
+    const int64_t row_end = min(row0 + ROWS_PER_BLOCK, m);
+    const int n_chunks = (int)((row_end - row0 + TT_CHUNK - 1) / TT_CHUNK);
+    auto issue = [&](int c) {   // warp 0; lane 0 arrives with the byte count before any lane copies
+        const int st = c % TT_STAGES;
+        const int64_t r = row0 + (int64_t)c * TT_CHUNK;
+        const uint32_t rows = (uint32_t)min((int64_t)TT_CHUNK, row_end - r);
+        if (lane == 0) {
+            mbar_expect_tx(&bars[st], rows * (128 * 4 + NO * 4));
+            tma_load_1d(s_d + (size_t)st * TT_CHUNK * NO, dout + r * NO, rows * NO * 4, &bars[st]);
+        }
+        __syncwarp();
+        if ((uint32_t)lane < rows)
+            tma_load_1d(s_h + ((size_t)st * TT_CHUNK + lane) * 128, hidden + (r + lane) * h + col0, 128 * 4, &bars[st]);
+    };
+    if (threadIdx.x == 0) {
+        for (int st = 0; st < TT_STAGES; ++st) mbar_init(&bars[st], 1);
+        mbar_fence_init();
+    }
+    __syncthreads();   // barriers initialised before warp 0 copies and anyone waits on them
+    if (warp == 0)
+        for (int c = 0; c < TT_STAGES && c < n_chunks; ++c) issue(c);
+
+    float4 w[NO], acc_w[NO], acc_b = make_float4(0.f, 0.f, 0.f, 0.f);
+    float acc_o[NO];
+#pragma unroll
+    for (int k = 0; k < NO; ++k) {
+        w[k] = *reinterpret_cast<const float4*>(w_heads + (int64_t)k * h + col0 + 4 * lane);
+        acc_o[k] = 0.f;
+        acc_w[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    float* dcol = dpre + col0 + 4 * lane;
+
+    for (int c = 0; c < n_chunks; ++c) {
+        const int st = c % TT_STAGES;
+        mbar_wait(&bars[st], (uint32_t)((c / TT_STAGES) & 1));
+        const int64_t r0 = row0 + (int64_t)c * TT_CHUNK;
+        const int rows = (int)min((int64_t)TT_CHUNK, row_end - r0);
+        const float* ch = s_h + (size_t)st * TT_CHUNK * 128;
+        const float* cd = s_d + (size_t)st * TT_CHUNK * NO;
+#pragma unroll
+        for (int i = 0; i < TT_CHUNK / MT_WARPS; ++i) {
+            const int rl = warp + i * MT_WARPS;
+            if (rl < rows) {
+                float d[NO];
+                tail_load_dout<NO>(cd + rl * NO, d);
+                const float4 hv = *reinterpret_cast<const float4*>(ch + rl * 128 + 4 * lane);
+                float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+                for (int k = 0; k < NO; ++k) {
+                    acc_o[k] += d[k];
+                    g.x = fmaf(d[k], w[k].x, g.x); g.y = fmaf(d[k], w[k].y, g.y);
+                    g.z = fmaf(d[k], w[k].z, g.z); g.w = fmaf(d[k], w[k].w, g.w);
+                    acc_w[k].x = fmaf(d[k], hv.x, acc_w[k].x); acc_w[k].y = fmaf(d[k], hv.y, acc_w[k].y);
+                    acc_w[k].z = fmaf(d[k], hv.z, acc_w[k].z); acc_w[k].w = fmaf(d[k], hv.w, acc_w[k].w);
+                }
+                g.x = hv.x > 0.f ? g.x : 0.f; g.y = hv.y > 0.f ? g.y : 0.f;
+                g.z = hv.z > 0.f ? g.z : 0.f; g.w = hv.w > 0.f ? g.w : 0.f;
+                acc_b.x += g.x; acc_b.y += g.y; acc_b.z += g.z; acc_b.w += g.w;
+                __stcs(reinterpret_cast<float4*>(dcol + (r0 + rl) * h), g);
+            }
+        }
+        __syncthreads();                                   // everyone is done reading stage st
+        if (warp == 0 && c + TT_STAGES < n_chunks) issue(c + TT_STAGES);
+    }
+    float* mine = s_red + (size_t)warp * PS;
+#pragma unroll
+    for (int k = 0; k < NO; ++k) *reinterpret_cast<float4*>(mine + k * 128 + 4 * lane) = acc_w[k];
+    *reinterpret_cast<float4*>(mine + NO * 128 + 4 * lane) = acc_b;
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < NO; ++k) mine[NO * 128 + 128 + k] = acc_o[k];
+    __syncthreads();
+    float* out = partials + (int64_t)blockIdx.x * (NO * h + h + NO);
+    const int n = blockIdx.y == 0 ? PS : NO * 128 + 128;
+    for (int j = threadIdx.x; j < n; j += MT_THREADS) {
+        float sum = 0.f;
+#pragma unroll
+        for (int wq = 0; wq < MT_WARPS; ++wq) sum += s_red[(size_t)wq * PS + j];
+        out[slice_partial_index<NO>(j, h, col0)] = sum;
+    }
+}
+
 // deterministic second stage: out[j] = sum over blocks of partials[b][j].  One warp per output element: lane l sums
 // blocks l, l+32, ... in order, then a fixed shuffle tree combines the 32 lane sums (same order every run).
 __global__ void __launch_bounds__(256) k_reduce_partials(const float* __restrict__ partials, int n_blocks, int pstride,
@@ -276,6 +458,21 @@ int launch_tail(const float* dout, int64_t dout_stride, const float* w_heads, co
     return PB_OK;
 }
 
+template <int NO>
+int launch_tail_slices(const float* dout, int64_t dout_stride, const float* w_heads, const float* hidden, int64_t m, int h,
+                       float* dpre, float* workspace, int blocks, cudaStream_t s) {
+    const dim3 grid((unsigned)blocks, (unsigned)(h / 128));
+    if (dout_stride == NO) {
+        const size_t smem = (size_t)TT_STAGES * (TT_CHUNK * 128 * 4 + TT_CHUNK * NO * 4) + (size_t)MT_WARPS * (NO * 128 + 128 + NO) * 4;
+        PB_CUDA(cudaFuncSetAttribute(k_mlp_tail_bwd_tma_slices<NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_mlp_tail_bwd_tma_slices<NO><<<grid, MT_THREADS, smem, s>>>(dout, w_heads, hidden, dpre, workspace, m, h);
+    } else {
+        k_mlp_tail_bwd_slices<NO><<<grid, MT_THREADS, 0, s>>>(dout, dout_stride, w_heads, hidden, dpre, workspace, m, h);
+    }
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
+
 }  // namespace
 
 extern "C" size_t pb_mlp_tail_workspace_bytes_ex(int64_t m, int32_t hidden, int32_t head_rows) {
@@ -292,8 +489,8 @@ extern "C" int pb_mlp_tail_backward_ex(const float* dout, int64_t dout_stride, c
                                        int64_t m, int32_t hidden_size, float* dpre, float* grads_out, void* workspace,
                                        size_t workspace_bytes, int32_t head_rows, void* stream) {
     PB_REQUIRE(m >= 1, PB_ERR_INVALID, "pb_mlp_tail_backward: m must be positive");
-    PB_REQUIRE(hidden_size == 128, PB_ERR_UNSUPPORTED, "pb_mlp_tail_backward: hidden size %d (only 128 is built)",
-               hidden_size);
+    PB_REQUIRE(hidden_size >= 128 && hidden_size <= 512 && hidden_size % 128 == 0, PB_ERR_UNSUPPORTED,
+               "pb_mlp_tail_backward: hidden size %d (128, 256, 384 and 512 are built)", hidden_size);
     PB_REQUIRE(head_rows == 8 || head_rows == 16, PB_ERR_UNSUPPORTED,
                "pb_mlp_tail_backward: head_rows %d (8 and 16 are built)", head_rows);
     PB_REQUIRE(dout && w_heads && hidden && dpre && grads_out && workspace, PB_ERR_INVALID,
@@ -307,8 +504,13 @@ extern "C" int pb_mlp_tail_backward_ex(const float* dout, int64_t dout_stride, c
     const int blocks = (int)pb_ceil_div(m, ROWS_PER_BLOCK);
     const int pstride = head_rows * hidden_size + hidden_size + head_rows;
     cudaStream_t s = (cudaStream_t)stream;
-    const int rc = head_rows == 8 ? launch_tail<8>(dout, dout_stride, w_heads, hidden, m, dpre, (float*)workspace, blocks, s)
-                                  : launch_tail<16>(dout, dout_stride, w_heads, hidden, m, dpre, (float*)workspace, blocks, s);
+    float* ws = (float*)workspace;
+    const int rc =
+        hidden_size == 128
+            ? (head_rows == 8 ? launch_tail<8>(dout, dout_stride, w_heads, hidden, m, dpre, ws, blocks, s)
+                              : launch_tail<16>(dout, dout_stride, w_heads, hidden, m, dpre, ws, blocks, s))
+            : (head_rows == 8 ? launch_tail_slices<8>(dout, dout_stride, w_heads, hidden, m, hidden_size, dpre, ws, blocks, s)
+                              : launch_tail_slices<16>(dout, dout_stride, w_heads, hidden, m, hidden_size, dpre, ws, blocks, s));
     if (rc != PB_OK) return rc;
     k_reduce_partials<<<(pstride * 32 + 255) / 256, 256, 0, s>>>((const float*)workspace, blocks, pstride, grads_out);
     PB_LAUNCH_CHECK();

@@ -163,11 +163,148 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
     }
 }
 
+// ---- hidden = 256, 384, 512: the hidden layer in 128-unit chunks.  Chunk c is W_enc rows [128c, 128c + 128) (64 KB),
+//      streamed by one 512-byte bulk copy per row into a two-stage ring on mbarriers; per chunk a warp computes its 16
+//      rows x 128 hidden units with the fragments of k_policy_mlp_sample, applies bias, ReLU and cvt.rna, and adds the
+//      chunk's share of the NC head columns into the same head accumulators (second mma).  The head bias is added once,
+//      after the last chunk.  Shared memory: x tile 34 KB + ring 136 KB + heads / encoder bias up to 34 KB -> one
+//      128-thread CTA per SM.
+constexpr int PW_HMAX = 512;
+
 template <int NC>
-int launch(const PolicyParams& p, cudaStream_t stream) {
-    const size_t smem = (size_t)(PM_ROWS + PM_H) * PM_PITCH * sizeof(float);
-    PB_CUDA(cudaFuncSetAttribute(k_policy_mlp_sample<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_policy_mlp_sample<NC><<<(unsigned)pb_ceil_div(p.m, PM_ROWS), PM_THREADS, smem, stream>>>(p);
+__global__ void __launch_bounds__(PM_THREADS, 1) k_policy_mlp_sample_wide(PolicyParams p, int hid) {
+    extern __shared__ __align__(128) float smem[];
+    float* sX = smem;                              // [64][136]
+    float* sW = smem + PM_ROWS * PM_PITCH;         // [2][128][136]: ring stage s holds chunk c with c % 2 == s
+    __shared__ float sWh[NC][PW_HMAX];
+    __shared__ float sBe[PW_HMAX];
+    __shared__ float sBh[NC];
+    __shared__ __align__(8) uint64_t bars[3];      // [0]: obs tile, [1 + s]: ring stage s
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    const int n_chunks = hid >> 7;
+    const int64_t row0 = (int64_t)blockIdx.x * PM_ROWS;
+    const int valid = (int)((p.m - row0) < PM_ROWS ? (p.m - row0) : PM_ROWS);
+    const uint64_t offset = p.counter ? *p.counter : 0ull;
+    constexpr uint32_t CHUNK_BYTES = 128u * PM_K * 4u;
+
+    if (tid == 0) {
+        for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+        mbar_fence_init();
+        mbar_expect_tx(&bars[0], (uint32_t)valid * PM_K * 4u);
+        mbar_expect_tx(&bars[1], CHUNK_BYTES);
+        mbar_expect_tx(&bars[2], CHUNK_BYTES);      // n_chunks >= 2
+    }
+    if (tid >= valid && tid < PM_ROWS) {
+#pragma unroll 8
+        for (int q = 0; q < PM_K / 4; ++q) *reinterpret_cast<float4*>(sX + tid * PM_PITCH + 4 * q) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    for (int i = tid; i < NC * hid; i += PM_THREADS) sWh[i / hid][i % hid] = p.w_heads[i];
+    for (int i = tid; i < hid; i += PM_THREADS) sBe[i] = p.b_enc[i];
+    if (tid < NC) sBh[tid] = p.b_heads[tid];
+    __syncthreads();
+    if (tid < valid) tma_load_1d(sX + tid * PM_PITCH, p.obs + (row0 + tid) * p.obs_stride, PM_K * 4u, &bars[0]);
+#pragma unroll
+    for (int s = 0; s < 2; ++s)
+        tma_load_1d(sW + (s * 128 + tid) * PM_PITCH, p.w_enc + (int64_t)(128 * s + tid) * PM_K, PM_K * 4u, &bars[1 + s]);
+
+    float out[NC / 8][4];
+#pragma unroll
+    for (int q8 = 0; q8 < NC / 8; ++q8) { out[q8][0] = out[q8][1] = out[q8][2] = out[q8][3] = 0.f; }
+    const float* xa = sX + (16 * warp + g) * PM_PITCH + 2 * t;
+    mbar_wait(&bars[0], 0);
+#pragma unroll 1
+    for (int c = 0; c < n_chunks; ++c) {
+        const int s = c & 1;
+        mbar_wait(&bars[1 + s], (uint32_t)(c >> 1) & 1u);
+        float acc[16][4];
+#pragma unroll
+        for (int nt = 0; nt < 16; ++nt) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }
+        const float* wbase = sW + (s * 128 + g) * PM_PITCH + 2 * t;
+#pragma unroll 4
+        for (int ks = 0; ks < 16; ++ks) {
+            const float2 x0 = *reinterpret_cast<const float2*>(xa + 8 * ks);
+            const float2 x1 = *reinterpret_cast<const float2*>(xa + 8 * PM_PITCH + 8 * ks);
+            const uint32_t a[4] = {to_tf32(x0.x), to_tf32(x1.x), to_tf32(x0.y), to_tf32(x1.y)};
+#pragma unroll
+            for (int nt = 0; nt < 16; ++nt) {
+                const float2 w = *reinterpret_cast<const float2*>(wbase + 8 * nt * PM_PITCH + 8 * ks);
+                mma_tf32(acc[nt], a, __float_as_uint(w.x), __float_as_uint(w.y));
+            }
+        }
+        // stage s is free once every warp has read it: refill it with chunk c + 2 (tid 0 arrives with the byte count
+        // before the barrier, so the copies can only complete the phase after it)
+        if (c + 2 < n_chunks && tid == 0) mbar_expect_tx(&bars[1 + s], CHUNK_BYTES);
+        __syncthreads();
+        if (c + 2 < n_chunks)
+            tma_load_1d(sW + (s * 128 + tid) * PM_PITCH, p.w_enc + (int64_t)(128 * (c + 2) + tid) * PM_K, PM_K * 4u,
+                        &bars[1 + s]);
+#pragma unroll
+        for (int nt = 0; nt < 16; ++nt) {
+            const int c0 = 128 * c + 8 * nt + 2 * t;
+            const float b0 = sBe[c0], b1 = sBe[c0 + 1];
+            uint32_t a[4];
+            a[0] = to_tf32(fmaxf(acc[nt][0] + b0, 0.f));
+            a[1] = to_tf32(fmaxf(acc[nt][2] + b0, 0.f));
+            a[2] = to_tf32(fmaxf(acc[nt][1] + b1, 0.f));
+            a[3] = to_tf32(fmaxf(acc[nt][3] + b1, 0.f));
+#pragma unroll
+            for (int q8 = 0; q8 < NC / 8; ++q8)
+                mma_tf32(out[q8], a, to_tf32(sWh[8 * q8 + g][c0]), to_tf32(sWh[8 * q8 + g][c0 + 1]));
+        }
+    }
+    float rowv[2][NC];
+#pragma unroll
+    for (int q8 = 0; q8 < NC / 8; ++q8) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int src = (lane & ~3) | q, k = 8 * q8 + 2 * q;
+            const float v0 = __shfl_sync(0xffffffffu, out[q8][0], src), v1 = __shfl_sync(0xffffffffu, out[q8][1], src);
+            const float v2 = __shfl_sync(0xffffffffu, out[q8][2], src), v3 = __shfl_sync(0xffffffffu, out[q8][3], src);
+            rowv[0][k] = v0 + sBh[k]; rowv[0][k + 1] = v1 + sBh[k + 1];
+            rowv[1][k] = v2 + sBh[k]; rowv[1][k + 1] = v3 + sBh[k + 1];
+        }
+    }
+    if (t < 2) {
+        const int64_t r = row0 + 16 * warp + g + 8 * t;
+        if (r < p.m) {
+            float z[NC];
+#pragma unroll
+            for (int k = 0; k < NC; ++k) z[k] = t ? rowv[1][k] : rowv[0][k];
+            int a;
+            float lp, ent, value;
+            pb_sample_row<NC>(z, p.n_act, pb_policy_uniform(p.seed, offset, r), a, lp, ent, value);
+            p.actions[r] = a;
+            p.logprobs[r] = lp;
+            p.values[r] = value;
+            if (p.entropies) p.entropies[r] = ent;
+        }
+    }
+    if (p.ticket) {
+        __syncthreads();
+        if (tid == 0) {
+            __threadfence();
+            if (atomicAdd(p.ticket, 1u) == gridDim.x - 1) {
+                *p.ticket = 0u;
+                *p.counter = offset + 1ull;
+                __threadfence();
+            }
+        }
+    }
+}
+
+template <int NC>
+int launch(const PolicyParams& p, int hid, cudaStream_t stream) {
+    const unsigned grid = (unsigned)pb_ceil_div(p.m, PM_ROWS);
+    if (hid == PM_H) {
+        const size_t smem = (size_t)(PM_ROWS + PM_H) * PM_PITCH * sizeof(float);
+        PB_CUDA(cudaFuncSetAttribute(k_policy_mlp_sample<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_policy_mlp_sample<NC><<<grid, PM_THREADS, smem, stream>>>(p);
+    } else {
+        const size_t smem = (size_t)(PM_ROWS + 2 * 128) * PM_PITCH * sizeof(float);
+        PB_CUDA(cudaFuncSetAttribute(k_policy_mlp_sample_wide<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_policy_mlp_sample_wide<NC><<<grid, PM_THREADS, smem, stream>>>(p, hid);
+    }
     PB_LAUNCH_CHECK();
     return PB_OK;
 }
@@ -180,9 +317,10 @@ extern "C" int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const 
                                     uint32_t* ticket_dev, int64_t* actions, float* logprobs, float* values, float* entropies, void* stream) {
     PB_REQUIRE(m >= 0, PB_ERR_INVALID, "pb_policy_mlp_sample: negative m");
     if (m == 0) return PB_OK;
-    PB_REQUIRE(in_features == PM_K && hidden_size == PM_H, PB_ERR_UNSUPPORTED,
-               "pb_policy_mlp_sample: built for 128 input features and 128 hidden units (got %d, %d)", in_features,
-               hidden_size);
+    PB_REQUIRE(in_features == PM_K && hidden_size >= PM_H && hidden_size <= PW_HMAX && hidden_size % PM_H == 0,
+               PB_ERR_UNSUPPORTED,
+               "pb_policy_mlp_sample: built for 128 input features and 128, 256, 384 or 512 hidden units (got %d, %d)",
+               in_features, hidden_size);
     PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "pb_policy_mlp_sample: n_act must be in [1, 15]");
     PB_REQUIRE(obs && w_enc && b_enc && w_heads && b_heads && actions && logprobs && values, PB_ERR_INVALID,
                "pb_policy_mlp_sample: null pointer");
@@ -192,5 +330,5 @@ extern "C" int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const 
     PolicyParams p{obs, obs_stride, w_enc, b_enc, w_heads, b_heads, m, n_act, seed, counter_dev, ticket_dev,
                    actions, logprobs, values, entropies};
     // w_heads / b_heads: the head matrix of models.Default.head_matrix, 8 rows for n_act <= 7, else 16
-    return n_act + 1 <= 8 ? launch<8>(p, (cudaStream_t)stream) : launch<16>(p, (cudaStream_t)stream);
+    return n_act + 1 <= 8 ? launch<8>(p, hidden_size, (cudaStream_t)stream) : launch<16>(p, hidden_size, (cudaStream_t)stream);
 }

@@ -8,7 +8,7 @@ import ctypes as C
 
 import torch
 
-from pufferlib_b200 import _native
+from pufferlib_b200 import _native, models
 
 
 def log_prob(logits, value):
@@ -64,7 +64,8 @@ class Policy(torch.nn.Module):
         return action, logprob, ent, value
 
     def _policy_step_fused(self, x, out=None):
-        """models.Default with 128 fp32 features / 128 hidden / <= 15 actions: the whole rollout-time policy step (encoder,
+        """models.Default with 128 fp32 features / 128, 256, 384 or 512 hidden (models.FAST_HIDDEN) / <= 15 actions: the
+        whole rollout-time policy step (encoder,
         ReLU, heads, sampling, row stores) as ONE kernel (pb_policy_mlp_sample).  Returns None if it does not apply."""
         model = self.policy
         if not (hasattr(model, 'head_matrix') and getattr(model, 'fast_path', False) and x.is_cuda
@@ -72,7 +73,7 @@ class Policy(torch.nn.Module):
             return None
         x2 = x.view(x.shape[0], -1)
         n_act, hid = model.decoder.weight.shape
-        if x2.shape[1] != 128 or hid != 128 or n_act > 15 or x2.stride(1) != 1 or x2.stride(0) % 4 != 0:
+        if x2.shape[1] != 128 or hid not in models.FAST_HIDDEN or n_act > 15 or x2.stride(1) != 1 or x2.stride(0) % 4 != 0:
             return None
         n, dev = x2.shape[0], x2.device
         if out is None:

@@ -69,6 +69,10 @@ class _DefaultMLPFunction(torch.autograd.Function):
                 db_cat[n_act:n_act + 1], None)
 
 
+# hidden sizes the hand-written kernels are built for (pb_policy_mlp_sample, pb_mlp_tail_backward_ex): 128 * k, k <= 4
+FAST_HIDDEN = (128, 256, 384, 512)
+
+
 def _slab_split(g_, r_, split=64):
     """K-slices per slab in the slab form of _gemm_tn: split / G, halved until they divide R."""
     sp = max(1, split // g_)
@@ -187,7 +191,7 @@ class Default(nn.Module):
         self.encoder = nn.Linear(int(np.prod(env.single_observation_space.shape)), hidden_size)
         self.decoder = layer_init(nn.Linear(hidden_size, env.single_action_space.n), std=0.01)
         self.value_head = nn.Linear(hidden_size, 1)
-        self.fast_path = True     # fused forward epilogues + pb_mlp_tail_backward (CUDA, hidden 128, <= 15 actions)
+        self.fast_path = True     # fused forward epilogues + pb_mlp_tail_backward (CUDA, FAST_HIDDEN, <= 15 actions)
         self._head_cache = {}
 
     def invalidate_cache(self):
@@ -231,7 +235,7 @@ class Default(nn.Module):
 
     def _fast_ok(self, x):
         n_act, hid = self.decoder.weight.shape
-        return self.fast_path and x.is_cuda and hid == 128 and n_act + 1 <= 16 and not x.requires_grad
+        return self.fast_path and x.is_cuda and hid in FAST_HIDDEN and n_act + 1 <= 16 and not x.requires_grad
 
     def forward_packed(self, observations):
         """-> (out [M, R], n_act) with logits = out[:, :n_act], value = out[:, n_act] (zero padding after; R = 8 for

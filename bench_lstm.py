@@ -2,13 +2,14 @@
 """bench_lstm.py -- the recurrent policy on the device path: RecurrentPolicy(LSTMWrapper(Default), fused_sample=True).
 
     python bench_lstm.py [--env breakout|squared] [--num-envs N] [--horizon H] [--steps K] [--warmup W] [--fused-update]
+                         [--hidden 128|256]
 
 Prints one JSON line with
   * agent-steps/s of the PPO loop (CUDA-graphed rollout; recurrent update on cuDNN autograd, or with --fused-update on
     the BPTT kernels pb_lstm_bptt_forward / _backward + pb_ppo_loss), the same step definition as bench.py;
   * `policy_step`: the rollout-time policy step, fused (pb_policy_lstm_sample: one kernel) vs unfused
     (fused_sample=False), measured in the same process on the rollout's own observation rows;
-  * `roofline_kernels.policy_lstm_step`: algorithmic HBM bytes 4F + 2048 + 16 per row over the fused step time, against
+  * `roofline_kernels.policy_lstm_step`: algorithmic HBM bytes 4F + 16H + 16 per row over the fused step time, against
     the H100 SXM data-sheet 3.35 TB/s; the packed weights each CTA streams from L2 are reported separately;
   * `update`: forward + loss + backward of one training minibatch ([B segments, T = 16 steps] of the rollout), fused
     (forward_packed_seq on the minibatch form train() used: the segment view of the rollout buffer, or the gathered
@@ -19,6 +20,7 @@ Prints one JSON line with
     the same way in one process and alternated, CUDA events around each call, median; the project's kernel launches per
     train() (pb_launch_count), the peak memory each kind of call allocates beyond what was allocated before it, and the
     observation bytes the segment view no longer gathers.
+--hidden sets H = LSTM input size = hidden size = the inner Default's hidden size (default 128).
 Shared pieces (PPO config, timed steps, card name and power limit) come from bench.py.  Writes nothing to the tree.
 """
 import argparse
@@ -44,6 +46,8 @@ def parse_args():
     ap.add_argument('--fused-update', action='store_true', help='train() on the fused BPTT kernels')
     ap.add_argument('--update-reps', type=int, default=10, help='timed minibatch updates per path')
     ap.add_argument('--train-reps', type=int, default=10, help='timed train() calls per trainer (captured, eager)')
+    ap.add_argument('--hidden', type=int, default=128, choices=[128, 256],
+                    help='LSTM input size = hidden size = the inner Default\'s hidden size')
     return ap.parse_args()
 
 
@@ -115,13 +119,14 @@ def policy_step_times(data, reps=256):
     return res
 
 
-def update_cost_per_row(feats, n_out, steps):
+def update_cost_per_row(feats, n_out, steps, H=128):
     """Algorithmic HBM bytes and TF32 tensor-core FLOPs per minibatch row of the fused update (forward kernel, loss
-    kernel, backward kernel, weight-gradient GEMMs and column sums), from the shapes.  n_out = R head columns."""
-    H, G = 128, 512
+    kernel, backward kernel, weight-gradient GEMMs and column sums), from the shapes.  n_out = R head columns, H the
+    LSTM size."""
+    G = 4 * H
     state = 4 * 4 * H / steps                                   # h0, c0 read and h_T, c_T written, once per segment
     nbytes = {
-        'forward': 4 * feats + 4 * 1024 + 4 * n_out + state,     # x; saved row written; out written
+        'forward': 4 * feats + 4 * 8 * H + 4 * n_out + state,    # x; saved row (8H) written; out written
         'loss': 4 * n_out + 28 + 4 * n_out,                     # out + 7 per-row scalars read; dOut written
         'backward': 4 * n_out + 4 * (H + 4 * H + H) + 4 * G + 4 * H,   # dOut, e, activations, c read; dz, dPre written
         'weight_grads': 2 * 4 * G + 4 * 2 * H + 2 * 4 * H + 4 * feats + 2 * 4 * n_out + 4 * H,
@@ -195,8 +200,8 @@ def make_trainer(args, train_graph):
     n, h = args.num_envs, args.horizon
     vec = pvec.make(ocean.env_creator(args.env), num_envs=n, backend=pvec.B200.options(exact_infos=False))
     torch.manual_seed(1)
-    net = models.LSTMWrapper(vec.driver_env, models.Default(vec.driver_env, hidden_size=128), input_size=128,
-                             hidden_size=128)
+    net = models.LSTMWrapper(vec.driver_env, models.Default(vec.driver_env, hidden_size=args.hidden),
+                             input_size=args.hidden, hidden_size=args.hidden)
     policy = cleanrl.RecurrentPolicy(net, fused_sample=True, seed=1, fused_update=args.fused_update).cuda()
     cfg = ppo_config(n, h, 'cuda', seed=1, cuda_graph=not args.no_graph, minibatches=args.minibatches,
                      epochs=args.epochs, env=args.env)
@@ -261,19 +266,20 @@ def main(args):
     upd, (seg, bptt), form = update_times(data, args.update_reps)
     n_act = vec.single_action_space.n
     n_out = -(-(n_act + 1) // 8) * 8
-    # algorithmic HBM bytes of one fused step: x (4F), h and c read and written (4 x 512), value + logprob + action (16)
+    # algorithmic HBM bytes of one fused step: x (4F), h and c read and written (4 x 4H), value + logprob + action (16)
+    H = args.hidden
     feats = int(np.prod(vec.single_observation_space.shape))
-    step_bytes = n * (4 * feats + 2048 + 16)
+    step_bytes = n * (4 * feats + 16 * H + 16)
     peak_gbs = 3350.0
     bound_s = step_bytes / (peak_gbs * 1e9)
     t_f, t_u = times['fused']['seconds'], times['unfused']['seconds']
-    ctas = -(-n // 128)
+    ctas = -(-n // (128 if H == 128 else 64))       # rows per CTA of k_policy_lstm_sample / _256
     # packed operands one CTA reads from L2 (W_enc, gate weights, biases, 16-row head matrix): not HBM traffic per step
-    weight_bytes = 4 * (128 * 136 + 16 * 32 * 264 + 128 + 512 + 16 * 128 + 16)
+    weight_bytes = 4 * (H * 136 + H // 8 * 32 * (2 * H + 8) + H + 4 * H + 16 * H + 16)
     line = {
         'metric': METRIC, 'value': n * h * args.steps / (ms * 1e-3), 'unit': UNIT, 'n_gpus': 1, 'steps': args.steps,
         'warmup': max(args.warmup, 2), 'ms_per_step': ms / args.steps, 'higher_is_better': True,
-        'config': {'workload': f'{args.env} num_envs={n} horizon={h} RecurrentPolicy(LSTMWrapper(Default)) hidden=128 '
+        'config': {'workload': f'{args.env} num_envs={n} horizon={h} RecurrentPolicy(LSTMWrapper(Default)) hidden={H} '
                                'fused_sample=True', 'global_batch': n * h, 'minibatch_size': n * h // args.minibatches,
                    'update_epochs': args.epochs, 'bptt_horizon': 16, 'cuda_graph_rollout': not args.no_graph,
                    'update': 'fused BPTT kernels' if args.fused_update else 'cuDNN LSTM autograd',
@@ -285,13 +291,13 @@ def main(args):
             'unfused_eager_us': round(times['unfused']['eager_seconds'] * 1e6, 2),
             'method': {k: v['method'] for k, v in times.items()}},
         'roofline_kernels': {'policy_lstm_step': {
-            'kernel': 'k_policy_lstm_sample', 'algorithmic_bytes_per_launch': step_bytes,
-            'bytes_per_row': 4 * feats + 2048 + 16, 'hbm_bound_us': round(bound_s * 1e6, 2),
+            'kernel': 'k_policy_lstm_sample' + ('' if H == 128 else '_256'), 'algorithmic_bytes_per_launch': step_bytes,
+            'bytes_per_row': 4 * feats + 16 * H + 16, 'hbm_bound_us': round(bound_s * 1e6, 2),
             'peak': peak_gbs, 'peak_source': 'H100 SXM5 HBM3 data sheet (3.35 TB/s), not measured',
             'avg_launch_us': round(t_f * 1e6, 2), 'achieved': round(step_bytes / t_f / 1e9, 1),
             'frac': round(bound_s / t_f, 4), 'launches_per_step': h,
             'l2_weight_bytes_per_cta': weight_bytes, 'l2_weight_bytes_per_launch': weight_bytes * ctas}},
-        'update': dict(update_section(upd, seg, bptt, feats, n_out), fused_minibatch_form=form),
+        'update': dict(update_section(upd, seg, bptt, feats, n_out, H), fused_minibatch_form=form),
         'train': train_section(args, data, warm_peaks, feats),
         'gpu': gpu_info(0), 'profile_s': prof, 'env_stats': {k: float(v) for k, v in data.stats.items()},
     }
@@ -352,9 +358,9 @@ def train_section(args, data, warm_peaks, feats):
     }
 
 
-def update_section(upd, seg, bptt, feats, n_out):
+def update_section(upd, seg, bptt, feats, n_out, H=128):
     rows = seg * bptt
-    nbytes, flops = update_cost_per_row(feats, n_out, bptt)
+    nbytes, flops = update_cost_per_row(feats, n_out, bptt, H)
     b_row, f_row = sum(nbytes.values()), sum(flops.values())
     peak_gbs, peak_tflops = 3350.0, 495.0
     t_bytes, t_flops = rows * b_row / (peak_gbs * 1e9), rows * f_row / (peak_tflops * 1e12)

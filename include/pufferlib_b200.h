@@ -278,14 +278,15 @@ int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const float* w_en
                          float* logprobs, float* values, float* entropies, void* stream);
 
 /* -- fused rollout-time recurrent policy step ------------------------------------------------------------------------
- * For LSTMWrapper(models.Default) with one LSTM layer of input and hidden size 128 (pufferlib/models.py:64-111, the
+ * For LSTMWrapper(models.Default) with one LSTM layer of input size = hidden size = H, H = 128 or 256, over a Default
+ * with an H-unit encoder (pufferlib/models.py:64-111, the
  * recurrent wrapper of cleanrl.py:69-93) at rollout time (clean_pufferl.py:100-117): encoder Linear + ReLU, the LSTM cell,
  * both heads, sample_logits (frameworks/cleanrl.py:25-47), the value / logprob / action row stores and the in-place
  * lstm_h / lstm_c update in ONE launch per env step (mma.sync TF32 tensor-core tiles, fp32 accumulate; the gates never
  * leave the SM).  Per row r < m:
  *   e = relu(x W_enc^T + b_enc);  z = e W_ih^T + h W_hh^T + b_ih + b_hh  (gate order i, f, g, o);
  *   c' = sigmoid(f) c + sigmoid(i) tanh(g);  h' = sigmoid(o) tanh(c');  out = h' W_cat^T + b_cat.
- * obs: [m] rows of in_features (<= 128) fp32, obs_stride floats apart (no alignment needed).  h, c: [m][128] fp32,
+ * obs: [m] rows of in_features (<= 128) fp32, obs_stride floats apart (no alignment needed).  h, c: [m][H] fp32,
  * h_stride / c_stride floats apart (even, 8-byte aligned), read and then overwritten in place; the state is not reset on
  * done (as clean_pufferl.py:100-105).  Packed operands (models.LSTMWrapper.fused_operands builds them):
  *   w_enc   [128][136]        W_enc rounded to TF32 (cvt.rna), columns past in_features zero;
@@ -295,9 +296,14 @@ int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const float* w_en
  *                             256..263 zero; rounded to TF32 (cvt.rna); 16-byte aligned;
  *   b_gates [16][32]          b_ih + b_hh in the same chunk order;
  *   w_heads [n_out][128], b_heads [n_out]: n_act logit rows | value row | zero rows, n_out = n_act + 1 rounded up to 8.
+ * At H = 256 the same packs with K = 512:
+ *   w_enc   [256][136];  b_enc [256];
+ *   w_gates [32][32][520]     chunk ch, row 8j + u = row 256j + 8ch + u of [W_ih | W_hh], columns 0..255 from W_ih,
+ *                             256..511 from W_hh, 512..519 zero; TF32; 16-byte aligned;
+ *   b_gates [32][32] (1024)   chunk order;  w_heads [n_out][256].
  * Sampling: the counter-based inverse CDF of pb_policy_mlp_sample on (seed, *counter_dev, row); with a non-null ticket_dev
  * the last CTA advances *counter_dev by 1.  Rows >= m are never read or written.  PB_ERR_UNSUPPORTED for in_features > 128,
- * input_size or hidden_size != 128, n_act > 15. */
+ * input_size != hidden_size, hidden_size other than 128 or 256, n_act > 15. */
 int pb_policy_lstm_sample(const float* obs, int64_t obs_stride, int32_t in_features, const float* w_enc,
                           const float* b_enc, const float* w_gates, const float* b_gates, const float* w_heads,
                           const float* b_heads, float* h, int64_t h_stride, float* c, int64_t c_stride, int64_t m,
@@ -310,22 +316,23 @@ int pb_policy_lstm_sample(const float* obs, int64_t obs_stride, int32_t in_featu
  * *obs] minibatch of clean_pufferl.py:188-191), same model envelope and packed operands as pb_policy_lstm_sample.
  * Rows are in (b, t) order: row b*T + t.
  * pb_lstm_bptt_forward: obs row b*T + t at obs + (b*T + t) * obs_stride (in_features <= 128 fp32, no alignment needed);
- *   h0, c0 [B][128] or null (zeros).  Per step the formula of pb_policy_lstm_sample (same rounding: T = 1 computes what
+ *   h0, c0 [B][H] or null (zeros).  Per step the formula of pb_policy_lstm_sample (same rounding: T = 1 computes what
  *   the rollout step computes).  Writes
  *   out   [B*T][R] fp32, R = 8 for n_act <= 7, else 16: n_act logits | value | the head bias of the zero rows;
- *   h_out, c_out [B][128]: the state after step T - 1;
- *   saved [B*T][1024] fp32 (4096 B per row): [e | h_prev | sigmoid(i) | sigmoid(f) | tanh(g) | sigmoid(o) | c | h],
- *         128 floats each (gates unit-major), e = relu(x W_enc^T + b_enc), h_prev = the state the step started from.
+ *   h_out, c_out [B][H]: the state after step T - 1;
+ *   saved [B*T][8H] fp32 (32H B per row): [e | h_prev | sigmoid(i) | sigmoid(f) | tanh(g) | sigmoid(o) | c | h],
+ *         H floats each (gates unit-major), e = relu(x W_enc^T + b_enc), h_prev = the state the step started from.
  * pb_lstm_bptt_backward: dout [B*T][R] (the loss gradient w.r.t. out, R as above), saved and c0 of the forward,
- *   w_gates_t [16][256][40] (models.LSTMWrapper.gate_weights_transposed: chunk ch, row n, column 8j + u = row 128j +
+ *   w_gates_t [H/8][2H][40] (models.LSTMWrapper.gate_weights_transposed: chunk ch, row n, column 8j + u = row Hj +
  *   8ch + u, column n of [W_ih | W_hh], rounded to TF32; columns 32..39 zero; 16-byte aligned), w_heads as in the
  *   forward.  The final state gets no gradient.  Writes
- *   dz   [B*T][512]: dLoss/d(gate pre-activations), nn.LSTM order i | f | g | o, unit-major;
- *   dpre [B*T][128]: dLoss/d(encoder pre-activation).
+ *   dz   [B*T][4H]: dLoss/d(gate pre-activations), nn.LSTM order i | f | g | o, unit-major;
+ *   dpre [B*T][H]: dLoss/d(encoder pre-activation).  At H = 256 the kernel also keeps dc of step t - 1 in dpre row
+ *        (b, t - 1) until that row receives its value, so dpre must not alias another buffer.
  *   The weight gradients follow by GEMMs: dW_ih | dW_hh = dz^T [e | h_prev], db_ih = db_hh = column sums of dz,
  *   dW_enc = dpre^T x, db_enc = column sums of dpre, dW_cat = dout^T h, db_cat = column sums of dout.
- * Segments >= B are never read or written.  PB_ERR_UNSUPPORTED (before any launch) for in_features > 128, input_size or
- * hidden_size != 128, n_act > 15.  Pointers 8-byte aligned unless stated otherwise. */
+ * Segments >= B are never read or written.  PB_ERR_UNSUPPORTED (before any launch) for in_features > 128, input_size !=
+ * hidden_size, hidden_size other than 128 or 256, n_act > 15.  Pointers 8-byte aligned unless stated otherwise. */
 int pb_lstm_bptt_forward(const float* obs, int64_t obs_stride, int32_t in_features, int64_t batch, int32_t steps,
                          const float* h0, const float* c0, const float* w_enc, const float* b_enc, const float* w_gates,
                          const float* b_gates, const float* w_heads, const float* b_heads, int32_t input_size,
@@ -342,12 +349,12 @@ int pb_lstm_bptt_backward(const float* dout, const float* saved, const float* c0
  *   dense (b, t) order of pb_lstm_bptt_forward, which is the case groups = 1, stride_e = T * obs_stride,
  *   stride_t = obs_stride.
  * pb_lstm_bptt_backward_rows: dpre row (b, t) at dpre + (b / groups) * dpre_stride_e + (b % groups) * dpre_stride_g +
- *   t * dpre_stride_t; those strides even and >= 128 (dpre_stride_g only checked when groups > 1).  dz keeps row b*T + t.
- *   pb_lstm_bptt_backward is the case groups = 1, dpre_stride_e = 128 T, dpre_stride_t = 128.
+ *   t * dpre_stride_t; those strides even and >= H (dpre_stride_g only checked when groups > 1).  dz keeps row b*T + t.
+ *   pb_lstm_bptt_backward is the case groups = 1, dpre_stride_e = H T, dpre_stride_t = H.
  * The segment view of Experience.segment_obs: minibatch mb of the reference (segments r = e*G + g, G = S / n_mb time
  * windows of T = bptt steps per env, S = horizon / bptt, n_mb | S) read from the arrival-order obs [horizon][N][F]:
  *   obs + mb*T*N*F, groups = G, stride_e = F, stride_g = n_mb*T*N*F, stride_t = N*F.
- * With dpre_stride_e = 128, dpre_stride_g = 128 T N, dpre_stride_t = 128 N, dPre row (b, t) lands at ((b % G) T + t) N
+ * With dpre_stride_e = H, dpre_stride_g = H T N, dpre_stride_t = H N, dPre row (b, t) lands at ((b % G) T + t) N
  * + b / G: G slabs of T*N rows in the order of the observation slabs obs + (g*n_mb + mb)*T*N*F, so that
  * dW_enc = sum_g dPre_g^T x_g.  Both compute bitwise what the dense entry points compute on the gathered copy (only the
  * load and store addresses differ).  PB_ERR_INVALID (before any launch) for groups < 1, batch % groups != 0, strides

@@ -40,6 +40,8 @@
 // tanh(g) | sigmoid(o) (4 x 128, unit-major) | c_t (128) | h_t (128)]; [e | h_prev] is the operand of dW_ih | dW_hh,
 // h_t that of dW_cat.  At B*T = 524 288 rows (breakout's minibatch) that is 2.1 GB.
 //
+// LSTM size 256: k_lstm_bptt_fwd_256 / k_lstm_bptt_bwd_256 below (64 segments per CTA; their own layout notes).
+//
 // Tile choice.  128 segments per CTA, one CTA per SM (shared memory): every CTA streams the 528 KB of gate weights per
 // step from L2, so fewer, fuller CTAs stream less.  At the headline shape B = 32 768 that is 256 CTAs = 1.94 waves on
 // 132 SMs, both waves nearly full (124 CTAs in the second); 64-segment CTAs would give 512 CTAs = 3.88 waves and twice
@@ -410,10 +412,332 @@ __global__ void __launch_bounds__(BT_THREADS, 1) k_lstm_bptt_bwd(BwdParams p) {
     }
 }
 
+// ---- H = 256 (LSTMWrapper(Default(hidden_size=256), 256, 256)).  Saved row 2048 floats: [e (256) | h_prev (256) |
+// sigmoid(i) | sigmoid(f) | tanh(g) | sigmoid(o) (4 x 256) | c_t (256) | h_t (256)]; dz rows [1024], dPre rows [256].
+constexpr int SV2 = 2048;
+constexpr int SV2_E = 0, SV2_HP = 256, SV2_ACT = 512, SV2_C = 1536, SV2_H = 1792;
+// backward: [2 stages][512][40] transposed ring (80 KB per chunk) and the dh fragments [chunk][row group][lane]
+constexpr int BW2_CHUNK = 2 * PW_H * BW_P;
+constexpr uint32_t BW2_CHUNK_BYTES = BW2_CHUNK * 4u;
+constexpr int FRAG2 = PW_CHUNKS * 4 * 32 * 4;
+constexpr int SB2_DH = 2 * BW2_CHUNK;
+constexpr size_t BWD2_SMEM = (size_t)(SB2_DH + FRAG2) * sizeof(float);
+static_assert(BWD2_SMEM <= 227 * 1024, "shared memory over the sm_90 per-CTA limit");
+
+// The forward at H = 256: 64 segments per CTA, 4 warps, the shared-memory plan of pb_policy_lstm_sample's H = 256 step
+// (lstm_cell.cuh, PW_*).  Phase 1 runs the encoder for all T steps with W_enc and the x tile over the ring and h tile.
+// Phase 2 walks the steps: at each step every warp reloads its 16 rows of the h tile from h_{t-1} (the saved rows it
+// wrote, or h0); the state it needs per (row, unit) -- h_prev for the saved row and c_prev -- comes back from the saved
+// row of step t-1 that the same thread wrote (or h0 / c0), so c and h round-trip through L2 / HBM once per step
+// (2 KB per segment, against the 8 KB saved row written) instead of occupying 128 KB of shared memory.
+template <int NC>
+__global__ void __launch_bounds__(128, 1) k_lstm_bptt_fwd_256(FwdParams p) {
+    extern __shared__ __align__(128) float smem[];
+    float* sX = smem + SW_X;
+    float* sWe = smem + SW_WE;
+    float* sWg = smem + SW_WG;
+    float* sHt = smem + SW_HT;
+    float* sWh = smem + SW_WH;
+    float* sBe = smem + SW_BE;
+    float* sBg = smem + SW_BG;
+    float* sBh = smem + SW_BH;
+    __shared__ __align__(8) uint64_t bars[3];      // [0]: W_enc, [1 + s]: gate-weight ring stage s
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    const int T = p.steps, F = p.in_features;
+    const int64_t b0 = (int64_t)blockIdx.x * PW_ROWS;
+    const int valid = (int)((p.batch - b0) < PW_ROWS ? (p.batch - b0) : PW_ROWS);
+    const int items = T * PW_CHUNKS;
+
+    if (tid == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        mbar_init(&bars[2], 1);
+        mbar_fence_init();
+        mbar_expect_tx(&bars[0], PW_WENC_BYTES);
+        tma_load_1d(sWe, p.w_enc, PW_WENC_BYTES, &bars[0]);
+    }
+    for (int i = tid; i < PW_H; i += 128) sBe[i] = p.b_enc[i];
+    for (int i = tid; i < 4 * PW_H; i += 128) sBg[i] = p.b_gates[i];
+    for (int i = tid; i < NC * PW_H; i += 128) sWh[(i >> 8) * PW_HP + (i & (PW_H - 1))] = p.w_heads[i];
+    if (tid < NC) sBh[tid] = p.b_heads[tid];
+    if (tid < PW_ROWS) {
+        const int64_t b = b0 + tid;
+        *xrow(sX, tid) = (b / p.groups) * p.s_e + (b % p.groups) * p.s_g;
+    }
+
+    const int lr = 16 * warp + g;
+    const bool va = lr < valid, vb = lr + 8 < valid;
+    const int64_t ra0 = (b0 + lr) * T, rb0 = ra0 + 8 * (int64_t)T;
+
+    // ---- phase 1: e = relu(x W_enc^T + b_enc) for every step, to the saved rows
+#pragma unroll 1
+    for (int st = 0; st < T; ++st) {
+        __syncthreads();
+        for (int i = tid; i < PW_ROWS * PL_F; i += 128) {
+            const int r = i >> 7, k = i & (PL_F - 1);
+            sX[r * PL_XP + k] = (r < valid && k < F) ? p.obs[*xrow(sX, r) + st * p.s_t + k] : 0.f;
+        }
+        __syncthreads();
+        if (st == 0) mbar_wait(&bars[0], 0);
+        float acc[32][4];
+        lstm_encoder(acc, sX + lr * PL_XP + 2 * t, sWe + g * PL_XP + 2 * t, F);
+        lstm_encoder_relu(acc, sBe, t);
+        float* sa = p.saved + (ra0 + st) * SV2 + SV2_E + 2 * t;
+        float* sb = p.saved + (rb0 + st) * SV2 + SV2_E + 2 * t;
+#pragma unroll
+        for (int nt = 0; nt < 32; ++nt) {
+            if (va) st2(sa + 8 * nt, acc[nt][0], acc[nt][1]);
+            if (vb) st2(sb + 8 * nt, acc[nt][2], acc[nt][3]);
+        }
+    }
+    fence_proxy_async_smem();                      // the x tile's generic writes before the ring's bulk copies
+    __syncthreads();                               // x tile and W_enc are dead: the region becomes ring | h tile
+    if (tid == 0) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {              // items >= 32 > 2
+            mbar_expect_tx(&bars[1 + s], PW_CHUNK_BYTES);
+            tma_load_1d(sWg + s * PW_CHUNK, p.w_gates + (int64_t)s * PW_CHUNK, PW_CHUNK_BYTES, &bars[1 + s]);
+        }
+    }
+
+    // ---- phase 2: the recurrence
+    const float* wlane = sWg + g * PW_GP + 2 * t;
+    const float* hs = sHt + lr * PW_HP + 2 * t;
+    int it = 0;
+#pragma unroll 1
+    for (int st = 0; st < T; ++st) {
+        const int64_t ra = ra0 + st, rb = rb0 + st;
+        float* sa = p.saved + ra * SV2;
+        float* sb = p.saved + rb * SV2;
+        // h_{t-1} (or h0): the previous step's last stores of this warp's lanes are ordered before the reload
+        __syncwarp();
+        lstm_load_h_tile(sHt, 16 * warp, lane, [&](int r) -> const float* {
+            const int lrow = 16 * warp + r;
+            if (lrow >= valid) return nullptr;
+            if (st > 0) return p.saved + ((b0 + lrow) * T + st - 1) * SV2 + SV2_H;
+            return p.h0 ? p.h0 + (b0 + lrow) * PW_H : nullptr;
+        });
+        __syncwarp();
+        // h_prev and c_prev of this thread's (row, unit) pairs: the saved row of step t-1 it wrote, or h0 / c0
+        const float* hpa = st > 0 ? sa - SV2 + SV2_H : (p.h0 ? p.h0 + (b0 + lr) * PW_H : nullptr);
+        const float* hpb = st > 0 ? sb - SV2 + SV2_H : (p.h0 ? p.h0 + (b0 + lr + 8) * PW_H : nullptr);
+        const float* cpa = st > 0 ? sa - SV2 + SV2_C : (p.c0 ? p.c0 + (b0 + lr) * PW_H : nullptr);
+        const float* cpb = st > 0 ? sb - SV2 + SV2_C : (p.c0 ? p.c0 + (b0 + lr + 8) * PW_H : nullptr);
+        uint32_t eA[32][4];
+#pragma unroll
+        for (int k = 0; k < 32; ++k) {
+            const float2 e0 = ld2(sa + SV2_E + 8 * k + 2 * t, va), e1 = ld2(sb + SV2_E + 8 * k + 2 * t, vb);
+            lstm_a_frag(eA[k], e0.x, e0.y, e1.x, e1.y);
+        }
+        float out[NC / 8][4];
+#pragma unroll
+        for (int q = 0; q < NC / 8; ++q) { out[q][0] = out[q][1] = out[q][2] = out[q][3] = 0.f; }
+#pragma unroll 1
+        for (int ch = 0; ch < PW_CHUNKS; ++ch, ++it) {
+            const int s = it & 1;
+            const int u0 = 8 * ch + 2 * t;
+            const float2 ha = ld2(hpa + u0, va && hpa), hb = ld2(hpb + u0, vb && hpb);
+            const float2 ca = ld2(cpa + u0, va && cpa), cb = ld2(cpb + u0, vb && cpb);
+            float gacc[4][4];
+            mbar_wait(&bars[1 + s], (uint32_t)(it >> 1) & 1u);
+            lstm_gate_chunk_256(gacc, eA, hs, wlane + s * PW_CHUNK);
+            __syncthreads();                       // every warp is done with stage s: refill it with item it + 2
+            if (tid == 0 && it + 2 < items) {
+                mbar_expect_tx(&bars[1 + s], PW_CHUNK_BYTES);
+                tma_load_1d(sWg + s * PW_CHUNK, p.w_gates + (int64_t)((it + 2) % PW_CHUNKS) * PW_CHUNK, PW_CHUNK_BYTES,
+                            &bars[1 + s]);
+            }
+            const float cp[4] = {ca.x, ca.y, cb.x, cb.y};
+            float act[4][4], cn[4], hn[4];
+            lstm_cell(gacc, sBg + 32 * ch + 2 * t, cp, act, cn, hn);
+            if (va) {
+                st2(sa + SV2_HP + u0, ha.x, ha.y);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) st2(sa + SV2_ACT + PW_H * j + u0, act[j][0], act[j][1]);
+                st2(sa + SV2_C + u0, cn[0], cn[1]);
+                st2(sa + SV2_H + u0, hn[0], hn[1]);
+            }
+            if (vb) {
+                st2(sb + SV2_HP + u0, hb.x, hb.y);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) st2(sb + SV2_ACT + PW_H * j + u0, act[j][2], act[j][3]);
+                st2(sb + SV2_C + u0, cn[2], cn[3]);
+                st2(sb + SV2_H + u0, hn[2], hn[3]);
+            }
+            if (st == T - 1) {
+                if (va) {
+                    st2(p.h_out + (b0 + lr) * PW_H + u0, hn[0], hn[1]);
+                    st2(p.c_out + (b0 + lr) * PW_H + u0, cn[0], cn[1]);
+                }
+                if (vb) {
+                    st2(p.h_out + (b0 + lr + 8) * PW_H + u0, hn[2], hn[3]);
+                    st2(p.c_out + (b0 + lr + 8) * PW_H + u0, cn[2], cn[3]);
+                }
+            }
+            lstm_head_chunk<NC, PW_HP>(out, hn, sWh, g, u0);
+        }
+#pragma unroll
+        for (int q = 0; q < NC / 8; ++q) {
+            const int k = 8 * q + 2 * t;
+            if (va) st2(p.out + ra * NC + k, out[q][0] + sBh[k], out[q][1] + sBh[k + 1]);
+            if (vb) st2(p.out + rb * NC + k, out[q][2] + sBh[k], out[q][3] + sBh[k + 1]);
+        }
+    }
+}
+
+// The backward at H = 256: 64 segments per CTA, 8 warps.  Warp w takes row group w & 3 (16 segments) and output half
+// w >> 2 of the product [de | dh_{t-1}] = dz [W_ih | W_hh]: half 0 accumulates de (256 columns, 128 registers), half 1
+// dh_{t-1}, whose C fragment of n-tile ch is exactly the chunk-ch fragment the next (earlier) step needs.  Both halves
+// compute the cell backward of every chunk (the same values: the A fragments of their product); half 0 writes dz.
+// dh_t goes through shared memory (half 1 adds W_cat^T dOut_t and publishes it); dc_{t-1} is kept in the dPre row of step
+// t-1, which only receives its dPre value after its own step has read dc back (half 0 writes both, each read is
+// separated from the next write by a CTA barrier).  Shared memory: ring 2 x 80 KB + dh 64 KB = 224 KB; W_cat is read
+// through L1.  The transposed gate weights stream from L2 at 2.6 MB per CTA per step (41 KB per segment).
+template <int NC>
+__global__ void __launch_bounds__(256, 1) k_lstm_bptt_bwd_256(BwdParams p) {
+    extern __shared__ __align__(128) float smem[];
+    float* sWt = smem;
+    float* sDH = smem + SB2_DH;
+    __shared__ __align__(8) uint64_t bars[2];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3, rg = warp & 3, half = warp >> 2;
+    const int T = p.steps;
+    const int64_t b0 = (int64_t)blockIdx.x * PW_ROWS;
+    const int valid = (int)((p.batch - b0) < PW_ROWS ? (p.batch - b0) : PW_ROWS);
+    const int items = T * PW_CHUNKS;
+
+    if (tid == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        mbar_fence_init();
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            mbar_expect_tx(&bars[s], BW2_CHUNK_BYTES);
+            tma_load_1d(sWt + s * BW2_CHUNK, p.w_gates_t + (int64_t)s * BW2_CHUNK, BW2_CHUNK_BYTES, &bars[s]);
+        }
+    }
+    __syncthreads();                               // barrier inits are visible
+
+    const int lr = 16 * rg + g;
+    const bool va = lr < valid, vb = lr + 8 < valid;
+    const int64_t ra0 = (b0 + lr) * T, rb0 = ra0 + 8 * (int64_t)T;
+    const int64_t ba = b0 + lr, bb = ba + 8;
+    float* const dpa = p.dpre + (ba / p.groups) * p.d_e + (ba % p.groups) * p.d_g;
+    float* const dpb = p.dpre + (bb / p.groups) * p.d_e + (bb % p.groups) * p.d_g;
+    const float* wlane = sWt + (PW_H * half + g) * BW_P + 2 * t;
+    float acc[32][4];
+#pragma unroll
+    for (int nt = 0; nt < 32; ++nt) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }   // dh_T = 0
+    int it = 0;
+#pragma unroll 1
+    for (int st = T - 1; st >= 0; --st) {
+        const int64_t ra = ra0 + st, rb = rb0 + st;
+        const float* sa = p.saved + ra * SV2;
+        const float* sb = p.saved + rb * SV2;
+        // ---- dh_t = (recurrent part, half 1's accumulators) + W_cat^T dOut_t, to the dh fragments
+        if (half == 1) {
+            float da[NC], db[NC];
+#pragma unroll
+            for (int k = 0; k < NC; k += 2) {
+                const float2 x0 = ld2(p.dout + ra * NC + k, va), x1 = ld2(p.dout + rb * NC + k, vb);
+                da[k] = x0.x; da[k + 1] = x0.y; db[k] = x1.x; db[k + 1] = x1.y;
+            }
+#pragma unroll
+            for (int ch = 0; ch < PW_CHUNKS; ++ch) {
+                float d[4] = {acc[ch][0], acc[ch][1], acc[ch][2], acc[ch][3]};
+#pragma unroll
+                for (int k = 0; k < NC; ++k) {
+                    if (k <= p.n_act) {
+                        const float2 w = __ldg(reinterpret_cast<const float2*>(p.w_heads + k * PW_H + 8 * ch + 2 * t));
+                        d[0] += da[k] * w.x; d[1] += da[k] * w.y; d[2] += db[k] * w.x; d[3] += db[k] * w.y;
+                    }
+                }
+                reinterpret_cast<float4*>(sDH)[(ch * 4 + rg) * 32 + lane] = make_float4(d[0], d[1], d[2], d[3]);
+            }
+        }
+#pragma unroll
+        for (int nt = 0; nt < 32; ++nt) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }
+        __syncthreads();                           // dh_t is visible to both halves
+        const float* cpa = st > 0 ? sa - SV2 + SV2_C : (p.c0 ? p.c0 + (b0 + lr) * PW_H : nullptr);
+        const float* cpb = st > 0 ? sb - SV2 + SV2_C : (p.c0 ? p.c0 + (b0 + lr + 8) * PW_H : nullptr);
+        const bool carry = st < T - 1;             // dc_t in the dPre row of step t (zero at t = T - 1)
+#pragma unroll 1
+        for (int ch = 0; ch < PW_CHUNKS; ++ch, ++it) {
+            const int s = it & 1;
+            const int u0 = 8 * ch + 2 * t;
+            const float4 dhv = reinterpret_cast<const float4*>(sDH)[(ch * 4 + rg) * 32 + lane];
+            const float2 dca = ld2(dpa + st * p.d_t + u0, va && carry), dcb = ld2(dpb + st * p.d_t + u0, vb && carry);
+            const float dh[4] = {dhv.x, dhv.y, dhv.z, dhv.w}, dc0[4] = {dca.x, dca.y, dcb.x, dcb.y};
+            float act[4][4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float2 x0 = ld2(sa + SV2_ACT + PW_H * j + u0, va), x1 = ld2(sb + SV2_ACT + PW_H * j + u0, vb);
+                act[j][0] = x0.x; act[j][1] = x0.y; act[j][2] = x1.x; act[j][3] = x1.y;
+            }
+            const float2 c0a = ld2(sa + SV2_C + u0, va), c0b = ld2(sb + SV2_C + u0, vb);
+            const float2 c1a = ld2(cpa + u0, va && cpa), c1b = ld2(cpb + u0, vb && cpb);
+            const float ct[4] = {c0a.x, c0a.y, c0b.x, c0b.y}, cprev[4] = {c1a.x, c1a.y, c1b.x, c1b.y};
+            float dz[4][4], dcn[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float si = act[0][e], sf = act[1][e], tg = act[2][e], so = act[3][e];
+                const float tc = tanhf(ct[e]);
+                const float dc = dc0[e] + dh[e] * so * (1.f - tc * tc);
+                dz[0][e] = dc * tg * si * (1.f - si);
+                dz[1][e] = dc * cprev[e] * sf * (1.f - sf);
+                dz[2][e] = dc * si * (1.f - tg * tg);
+                dz[3][e] = dh[e] * tc * so * (1.f - so);
+                dcn[e] = dc * sf;
+            }
+            uint32_t zA[4][4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) lstm_a_frag(zA[j], dz[j][0], dz[j][1], dz[j][2], dz[j][3]);
+            if (half == 0) {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    if (va) st2(p.dz + ra * (4 * PW_H) + PW_H * j + u0, dz[j][0], dz[j][1]);
+                    if (vb) st2(p.dz + rb * (4 * PW_H) + PW_H * j + u0, dz[j][2], dz[j][3]);
+                }
+                if (st > 0) {                      // dc_{t-1} to the dPre row of step t - 1
+                    if (va) st2(dpa + (st - 1) * p.d_t + u0, dcn[0], dcn[1]);
+                    if (vb) st2(dpb + (st - 1) * p.d_t + u0, dcn[2], dcn[3]);
+                }
+            }
+            mbar_wait(&bars[s], (uint32_t)(it >> 1) & 1u);
+            const float* wc = wlane + s * BW2_CHUNK;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                for (int nt = 0; nt < 32; ++nt) {
+                    const float2 w = *reinterpret_cast<const float2*>(wc + 8 * nt * BW_P + 8 * j);
+                    mma_tf32(acc[nt], zA[j], __float_as_uint(w.x), __float_as_uint(w.y));
+                }
+            }
+            __syncthreads();                       // every warp is done with stage s (and with dc_t of chunk ch)
+            if (tid == 0 && it + 2 < items) {
+                mbar_expect_tx(&bars[s], BW2_CHUNK_BYTES);
+                tma_load_1d(sWt + s * BW2_CHUNK, p.w_gates_t + (int64_t)((it + 2) % PW_CHUNKS) * BW2_CHUNK,
+                            BW2_CHUNK_BYTES, &bars[s]);
+            }
+        }
+        // ---- dPre_enc = de * (e > 0), over the carried dc_t (every read of it was before the last barrier)
+        if (half == 0) {
+#pragma unroll
+            for (int nt = 0; nt < 32; ++nt) {
+                const int k = 8 * nt + 2 * t;
+                const float2 ea = ld2(sa + SV2_E + k, va), eb = ld2(sb + SV2_E + k, vb);
+                if (va) st2(dpa + st * p.d_t + k, ea.x > 0.f ? acc[nt][0] : 0.f, ea.y > 0.f ? acc[nt][1] : 0.f);
+                if (vb) st2(dpb + st * p.d_t + k, eb.x > 0.f ? acc[nt][2] : 0.f, eb.y > 0.f ? acc[nt][3] : 0.f);
+            }
+        }
+    }
+}
+
 template <typename K, typename P>
-int launch(K kernel, const P& p, size_t smem, cudaStream_t stream) {
+int launch(K kernel, const P& p, size_t smem, cudaStream_t stream, int rows = BT_ROWS, int threads = BT_THREADS) {
     PB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<(unsigned)pb_ceil_div(p.batch, BT_ROWS), BT_THREADS, smem, stream>>>(p);
+    kernel<<<(unsigned)pb_ceil_div(p.batch, rows), threads, smem, stream>>>(p);
     PB_LAUNCH_CHECK();
     return PB_OK;
 }
@@ -431,8 +755,9 @@ int forward_rows(const char* fn, const float* obs, int32_t in_features, int64_t 
                fn, groups, (long long)batch);
     PB_REQUIRE(in_features >= 1 && in_features <= PL_F, PB_ERR_UNSUPPORTED,
                "%s: observation features must be in [1, %d] (got %d)", fn, PL_F, in_features);
-    PB_REQUIRE(input_size == PL_H && hidden_size == PL_H, PB_ERR_UNSUPPORTED,
-               "%s: built for LSTM input and hidden size %d (got %d, %d)", fn, PL_H, input_size, hidden_size);
+    PB_REQUIRE(input_size == hidden_size && (hidden_size == PL_H || hidden_size == PW_H), PB_ERR_UNSUPPORTED,
+               "%s: built for LSTM input size = hidden size = %d or %d (got %d, %d)", fn, PL_H, PW_H, input_size,
+               hidden_size);
     PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "%s: n_act must be in [1, 15]", fn);
     if (batch == 0) return PB_OK;
     PB_REQUIRE(obs && w_enc && b_enc && w_gates && b_gates && w_heads && b_heads && out && h_out && c_out && saved,
@@ -447,6 +772,9 @@ int forward_rows(const char* fn, const float* obs, int32_t in_features, int64_t 
     FwdParams p{obs, s_e, s_g, s_t, groups, in_features, batch, steps, h0, c0, w_enc, b_enc, w_gates, b_gates, w_heads,
                 b_heads, out, h_out, c_out, saved};
     cudaStream_t s = (cudaStream_t)stream;
+    if (hidden_size == PW_H)
+        return n_act + 1 <= 8 ? launch(k_lstm_bptt_fwd_256<8>, p, PW_SMEM, s, PW_ROWS, 128)
+                              : launch(k_lstm_bptt_fwd_256<16>, p, PW_SMEM, s, PW_ROWS, 128);
     return n_act + 1 <= 8 ? launch(k_lstm_bptt_fwd<8>, p, FWD_SMEM, s) : launch(k_lstm_bptt_fwd<16>, p, FWD_SMEM, s);
 }
 
@@ -458,20 +786,24 @@ int backward_rows(const char* fn, const float* dout, const float* saved, const f
     PB_REQUIRE(batch >= 0 && steps >= 1, PB_ERR_INVALID, "%s: need batch >= 0 and steps >= 1", fn);
     PB_REQUIRE(groups >= 1 && batch % groups == 0, PB_ERR_INVALID, "%s: need groups >= 1 dividing batch (got %d, %lld)",
                fn, groups, (long long)batch);
-    PB_REQUIRE(input_size == PL_H && hidden_size == PL_H, PB_ERR_UNSUPPORTED,
-               "%s: built for LSTM input and hidden size %d (got %d, %d)", fn, PL_H, input_size, hidden_size);
+    PB_REQUIRE(input_size == hidden_size && (hidden_size == PL_H || hidden_size == PW_H), PB_ERR_UNSUPPORTED,
+               "%s: built for LSTM input size = hidden size = %d or %d (got %d, %d)", fn, PL_H, PW_H, input_size,
+               hidden_size);
     PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "%s: n_act must be in [1, 15]", fn);
     if (batch == 0) return PB_OK;
     PB_REQUIRE(dout && saved && w_gates_t && w_heads && dz && dpre, PB_ERR_INVALID, "%s: null pointer", fn);
-    PB_REQUIRE(d_e >= PL_H && d_t >= PL_H && (groups == 1 || d_g >= PL_H) && d_e % 2 == 0 && d_g % 2 == 0 &&
-                   d_t % 2 == 0,
-               PB_ERR_INVALID, "%s: dPre strides must be even and at least %d floats", fn, PL_H);
+    PB_REQUIRE(d_e >= hidden_size && d_t >= hidden_size && (groups == 1 || d_g >= hidden_size) && d_e % 2 == 0 &&
+                   d_g % 2 == 0 && d_t % 2 == 0,
+               PB_ERR_INVALID, "%s: dPre strides must be even and at least %d floats", fn, hidden_size);
     PB_REQUIRE(aligned(w_gates_t, 16), PB_ERR_INVALID, "%s: w_gates_t must be 16-byte aligned", fn);
     PB_REQUIRE(aligned(dout, 8) && aligned(saved, 8) && aligned(c0, 8) && aligned(w_heads, 8) && aligned(dz, 8) &&
                    aligned(dpre, 8),
                PB_ERR_INVALID, "%s: dout / saved / c0 / w_heads / dz / dpre must be 8-byte aligned", fn);
     BwdParams p{dout, saved, c0, w_gates_t, w_heads, batch, steps, n_act, dz, dpre, groups, d_e, d_g, d_t};
     cudaStream_t s = (cudaStream_t)stream;
+    if (hidden_size == PW_H)
+        return n_act + 1 <= 8 ? launch(k_lstm_bptt_bwd_256<8>, p, BWD2_SMEM, s, PW_ROWS, 256)
+                              : launch(k_lstm_bptt_bwd_256<16>, p, BWD2_SMEM, s, PW_ROWS, 256);
     return n_act + 1 <= 8 ? launch(k_lstm_bptt_bwd<8>, p, BWD_SMEM, s) : launch(k_lstm_bptt_bwd<16>, p, BWD_SMEM, s);
 }
 
@@ -503,9 +835,9 @@ extern "C" int pb_lstm_bptt_forward_rows(const float* obs, int32_t in_features, 
 extern "C" int pb_lstm_bptt_backward(const float* dout, const float* saved, const float* c0, const float* w_gates_t,
                                      const float* w_heads, int64_t batch, int32_t steps, int32_t input_size,
                                      int32_t hidden_size, int32_t n_act, float* dz, float* dpre, void* stream) {
-    // dPre dense [B*T][128] in row order b*T + t
+    // dPre dense [B*T][H] in row order b*T + t
     return backward_rows("pb_lstm_bptt_backward", dout, saved, c0, w_gates_t, w_heads, batch, steps, input_size,
-                         hidden_size, n_act, 1, (int64_t)steps * PL_H, 0, PL_H, dz, dpre, stream);
+                         hidden_size, n_act, 1, (int64_t)steps * hidden_size, 0, hidden_size, dz, dpre, stream);
 }
 
 extern "C" int pb_lstm_bptt_backward_rows(const float* dout, const float* saved, const float* c0,

@@ -9,6 +9,7 @@
 //   * the cell update of a thread's 2 rows x 2 units, and the head product accumulated chunk by chunk.
 // Fragment element order of a chunk, e = 0..3: (row g, unit u0), (row g, u0 + 1), (row g + 8, u0), (row g + 8, u0 + 1)
 // with u0 = 8 ch + 2t -- the C fragment of n-tile j of the chunk is gate j of those four (row, unit) pairs.
+// Two sizes H = input size = hidden size: 128 (PL_*) and 256 (PW_*, the geometry of the H = 256 kernels below).
 #pragma once
 #include "policy_sample.cuh"
 
@@ -23,11 +24,37 @@ constexpr uint32_t PL_WENC_BYTES = PL_H * PL_XP * 4u;
 
 __device__ __forceinline__ float pb_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 
-// acc[nt] += x[16 rows][F] W_enc^T for n-tile nt (hidden units 8nt..8nt+7).  xa = sX + lr * PL_XP + 2t,
+// H = 256: one CTA owns 64 rows (4 warps x 16).  e stays in registers as the A fragments of k-steps 0..31 (128
+// registers, as [e | h] at H = 128); h_prev is read as A fragments from the h tile [64][264] (TF32, 64-bit loads of the
+// k-slot trick, conflict-free at pitch 264).  Shared memory, in floats: the ring and the h tile, which first hold W_enc
+// and the x tile for the encoder, then the heads and the biases (PW_SMEM = 222 784 B).
+constexpr int PW_H = 256;
+constexpr int PW_ROWS = 64;                        // rows (segments) per CTA
+constexpr int PW_HP = PW_H + 8;                    // 264: h tile / W_heads pitch
+constexpr int PW_GP = 2 * PW_H + 8;                // 520: gate-weight row pitch, K = [e (256) | h (256)] + pad
+constexpr int PW_CHUNKS = PW_H / 8;                // 32 chunks of 8 units
+constexpr int PW_CHUNK = 32 * PW_GP;               // floats per chunk (66560 B)
+constexpr uint32_t PW_CHUNK_BYTES = PW_CHUNK * 4u;
+constexpr uint32_t PW_WENC_BYTES = PW_H * PL_XP * 4u;
+constexpr int SW_WG = 0;                           // [2][32][520] gate-weight ring
+constexpr int SW_HT = SW_WG + 2 * PW_CHUNK;        // [64][264] h_prev tile, TF32
+constexpr int SW_WE = 0;                           // [256][136] W_enc (encoder phase, over the ring)
+constexpr int SW_X = SW_WE + PW_H * PL_XP;         // [64][136] x tile (encoder phase, over the h tile)
+constexpr int SW_WH = SW_HT + PW_ROWS * PW_HP;     // [16][264] head matrix
+constexpr int SW_BE = SW_WH + 16 * PW_HP;          // [256] b_enc
+constexpr int SW_BG = SW_BE + PW_H;                // [32][32] b_ih + b_hh, chunk order
+constexpr int SW_BH = SW_BG + 4 * PW_H;            // [16] head bias
+constexpr size_t PW_SMEM = (size_t)(SW_BH + 16) * sizeof(float);
+static_assert(SW_X + PW_ROWS * PL_XP <= SW_WH, "W_enc and the x tile must fit in the ring and h tile");
+static_assert(PW_SMEM <= 227 * 1024, "shared memory over the sm_90 per-CTA limit");
+static_assert((SW_HT * 4) % 16 == 0 && (SW_X * 4) % 16 == 0 && PW_CHUNK_BYTES % 16 == 0, "bulk copy alignment");
+
+// acc[nt] += x[16 rows][F] W_enc^T for n-tile nt (hidden units 8nt..8nt+7), NT = H / 8.  xa = sX + lr * PL_XP + 2t,
 // wb = sWe + g * PL_XP + 2t; K = F rounded up to 8 (the tile is zero past F).
-__device__ __forceinline__ void lstm_encoder(float (&acc)[16][4], const float* xa, const float* wb, int F) {
+template <int NT>
+__device__ __forceinline__ void lstm_encoder(float (&acc)[NT][4], const float* xa, const float* wb, int F) {
 #pragma unroll
-    for (int nt = 0; nt < 16; ++nt) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }
+    for (int nt = 0; nt < NT; ++nt) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }
     const int ksteps = (F + 7) >> 3;
 #pragma unroll 2
     for (int ks = 0; ks < ksteps; ++ks) {
@@ -35,7 +62,7 @@ __device__ __forceinline__ void lstm_encoder(float (&acc)[16][4], const float* x
         const float2 x1 = *reinterpret_cast<const float2*>(xa + 8 * PL_XP + 8 * ks);
         const uint32_t a[4] = {to_tf32(x0.x), to_tf32(x1.x), to_tf32(x0.y), to_tf32(x1.y)};
 #pragma unroll
-        for (int nt = 0; nt < 16; ++nt) {
+        for (int nt = 0; nt < NT; ++nt) {
             const float2 w = *reinterpret_cast<const float2*>(wb + 8 * nt * PL_XP + 8 * ks);   // B[k][n] = W[n][k]
             mma_tf32(acc[nt], a, __float_as_uint(w.x), __float_as_uint(w.y));
         }
@@ -43,9 +70,10 @@ __device__ __forceinline__ void lstm_encoder(float (&acc)[16][4], const float* x
 }
 
 // relu(acc + b) in place: C fragment of n-tile nt = columns 8nt + {2t, 2t+1} of rows {g, g+8}
-__device__ __forceinline__ void lstm_encoder_relu(float (&acc)[16][4], const float* sBe, int t) {
+template <int NT>
+__device__ __forceinline__ void lstm_encoder_relu(float (&acc)[NT][4], const float* sBe, int t) {
 #pragma unroll
-    for (int nt = 0; nt < 16; ++nt) {
+    for (int nt = 0; nt < NT; ++nt) {
         const int c0 = 8 * nt + 2 * t;
         const float b0 = sBe[c0], b1 = sBe[c0 + 1];
         acc[nt][0] = fmaxf(acc[nt][0] + b0, 0.f);
@@ -77,6 +105,47 @@ __device__ __forceinline__ void lstm_gate_chunk(float (&gacc)[4][4], const uint3
     }
 }
 
+// the H = 256 chunk: gacc[j] = [e | h_prev] x gate j, e (k-steps 0..31) from registers, h_prev (k-steps 32..63) from
+// this warp's rows of the TF32 h tile.  hs = tile + lr * PW_HP + 2t, wc = stage base + g * PW_GP + 2t
+__device__ __forceinline__ void lstm_gate_chunk_256(float (&gacc)[4][4], const uint32_t (&eA)[32][4], const float* hs,
+                                                    const float* wc) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { gacc[j][0] = gacc[j][1] = gacc[j][2] = gacc[j][3] = 0.f; }
+#pragma unroll
+    for (int ks = 0; ks < 32; ++ks) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 w = *reinterpret_cast<const float2*>(wc + 8 * j * PW_GP + 8 * ks);
+            mma_tf32(gacc[j], eA[ks], __float_as_uint(w.x), __float_as_uint(w.y));
+        }
+    }
+#pragma unroll
+    for (int ks = 0; ks < 32; ++ks) {
+        const float2 x0 = *reinterpret_cast<const float2*>(hs + 8 * ks);
+        const float2 x1 = *reinterpret_cast<const float2*>(hs + 8 * PW_HP + 8 * ks);
+        const uint32_t a[4] = {__float_as_uint(x0.x), __float_as_uint(x1.x), __float_as_uint(x0.y), __float_as_uint(x1.y)};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 w = *reinterpret_cast<const float2*>(wc + 8 * j * PW_GP + 8 * (32 + ks));
+            mma_tf32(gacc[j], a, __float_as_uint(w.x), __float_as_uint(w.y));
+        }
+    }
+}
+
+// this warp's 16 rows of the H = 256 h tile from rows src(r) (fp32, 256 floats each; null = zeros), rounded to TF32
+// (cvt.rna) on the way in.  rows: this warp's first tile row; src(r) for r = 0..15.
+template <typename Src>
+__device__ __forceinline__ void lstm_load_h_tile(float* sHt, int rows, int lane, Src src) {
+#pragma unroll 4
+    for (int i = lane; i < 16 * (PW_H / 2); i += 32) {
+        const int r = i / (PW_H / 2), k = 2 * (i % (PW_H / 2));
+        const float* p = src(r);
+        const float2 v = p ? *reinterpret_cast<const float2*>(p + k) : make_float2(0.f, 0.f);
+        *reinterpret_cast<float2*>(sHt + (rows + r) * PW_HP + k) =
+            make_float2(__uint_as_float(to_tf32(v.x)), __uint_as_float(to_tf32(v.y)));
+    }
+}
+
 // the cell update of the four (row, unit) elements: bg = sBg + 32 ch + 2t (b_ih + b_hh in chunk order), cp = c_prev;
 // act[j][e] = sigmoid(i), sigmoid(f), tanh(g), sigmoid(o)
 __device__ __forceinline__ void lstm_cell(const float (&gacc)[4][4], const float* bg, const float (&cp)[4],
@@ -95,15 +164,15 @@ __device__ __forceinline__ void lstm_cell(const float (&gacc)[4][4], const float
     }
 }
 
-// heads: chunk ch is k-step ch of h' W_cat^T (slots t <-> unit u0, t + 4 <-> unit u0 + 1); sWh pitch PL_XP
-template <int NC>
+// heads: chunk ch is k-step ch of h' W_cat^T (slots t <-> unit u0, t + 4 <-> unit u0 + 1); sWh pitch P
+template <int NC, int P = PL_XP>
 __device__ __forceinline__ void lstm_head_chunk(float (&out)[NC / 8][4], const float (&hn)[4], const float* sWh, int g,
                                                 int u0) {
     uint32_t a[4];
     lstm_a_frag(a, hn[0], hn[1], hn[2], hn[3]);
 #pragma unroll
     for (int q = 0; q < NC / 8; ++q) {
-        const float* wh = sWh + (8 * q + g) * PL_XP + u0;
+        const float* wh = sWh + (8 * q + g) * P + u0;
         mma_tf32(out[q], a, to_tf32(wh[0]), to_tf32(wh[1]));
     }
 }

@@ -36,6 +36,8 @@
 // the time at every size.  Shortening that chain (wgmma, a deeper ring in the dead x-tile region, 2-CTA multicast of
 // the weight stream) is where further speed is; none of it is measured yet.
 //
+// k_policy_lstm_sample_256 (below) is the same step at LSTM size 256, with e in registers and h_prev in a shared tile.
+//
 // Operand rounding: every tensor-core operand is rounded to nearest TF32 (cvt.rna: ties away from zero): x, relu(e + b),
 // h_prev and h' in the kernel, W_enc and the gate weights on the host (models.LSTMWrapper.fused_operands), W_cat in the
 // kernel.  Accumulation, biases, the cell update and the sampler are fp32.
@@ -73,6 +75,55 @@ struct LstmParams {
     uint64_t seed; uint64_t* counter; unsigned int* ticket;
     int64_t* actions; float* logprobs; float* values; float* entropies;
 };
+
+// The sampling epilogue of a warp's 16 rows for the H = 256 kernel (k_policy_lstm_sample keeps the same code inline,
+// which leaves its compiled code as it was): out[q] = (row g, cols 8q + 2t, +1), (row g + 8, same) of h' W_cat^T;
+// gather the NC columns of a row across its quad, add the head bias, sample, store the row; then the last CTA to leave
+// advances the stream counter (every CTA read it before its ticket).  lr: the warp's local row of fragment row g.
+template <int NC>
+__device__ __forceinline__ void sample_rows(const float (&out)[NC / 8][4], const float* sBh, const LstmParams& p,
+                                            int64_t row0, int lr, int lane, int tid, uint64_t offset) {
+    const int t = lane & 3;
+    float rowv[2][NC];
+#pragma unroll
+    for (int q8 = 0; q8 < NC / 8; ++q8) {
+#pragma unroll
+        for (int qq = 0; qq < 4; ++qq) {
+            const int src = (lane & ~3) | qq, k = 8 * q8 + 2 * qq;
+            const float v0 = __shfl_sync(0xffffffffu, out[q8][0], src), v1 = __shfl_sync(0xffffffffu, out[q8][1], src);
+            const float v2 = __shfl_sync(0xffffffffu, out[q8][2], src), v3 = __shfl_sync(0xffffffffu, out[q8][3], src);
+            rowv[0][k] = v0 + sBh[k]; rowv[0][k + 1] = v1 + sBh[k + 1];
+            rowv[1][k] = v2 + sBh[k]; rowv[1][k + 1] = v3 + sBh[k + 1];
+        }
+    }
+    // lane t == 0 finishes row g, lane t == 1 finishes row g + 8
+    if (t < 2) {
+        const int64_t r = row0 + lr + 8 * t;
+        if (r < p.m) {
+            float z[NC];
+#pragma unroll
+            for (int k = 0; k < NC; ++k) z[k] = t ? rowv[1][k] : rowv[0][k];
+            int a;
+            float lp, ent, value;
+            pb_sample_row<NC>(z, p.n_act, pb_policy_uniform(p.seed, offset, r), a, lp, ent, value);
+            p.actions[r] = a;
+            p.logprobs[r] = lp;
+            p.values[r] = value;
+            if (p.entropies) p.entropies[r] = ent;
+        }
+    }
+    if (p.ticket) {
+        __syncthreads();
+        if (tid == 0) {
+            __threadfence();
+            if (atomicAdd(p.ticket, 1u) == gridDim.x - 1) {
+                *p.ticket = 0u;
+                *p.counter = offset + 1ull;
+                __threadfence();
+            }
+        }
+    }
+}
 
 template <int NC>
 __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams p) {
@@ -220,10 +271,129 @@ __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams
     }
 }
 
+// The H = 256 step (LSTMWrapper(Default(hidden_size=256), 256, 256)): the same function with the geometry of
+// lstm_cell.cuh's PW_* block.  A CTA owns 64 rows, 4 warps x 16 rows (256 CTAs at N = 16384: 1.94 waves on 132 SMs).
+//   * encoder: W_enc [256][136] (one 136 KB bulk copy) and the x tile [64][136] sit where the gate-weight ring and the h
+//     tile go later; a warp's 16 x 256 accumulator becomes eA, the A fragments of k-steps 0..31 (128 registers).
+//   * then the ring's first two stages are requested and each warp loads its 16 rows of h_prev into the h tile
+//     [64][264] (TF32); k-steps 32..63 of every chunk read their A fragments from there (64-bit loads).
+//   * gates: 32 chunks of 8 units from the packed [32][32][520] weights (2.1 MB per CTA per step from L2, 33 KB per
+//     row) through a 2-stage ring of 65 KB bulk copies; cell update, state stores and heads as at H = 128.
+template <int NC>
+__global__ void __launch_bounds__(128, 1) k_policy_lstm_sample_256(LstmParams p) {
+    extern __shared__ __align__(128) float smem[];
+    float* sX = smem + SW_X;
+    float* sWe = smem + SW_WE;
+    float* sWg = smem + SW_WG;
+    float* sHt = smem + SW_HT;
+    float* sWh = smem + SW_WH;
+    float* sBe = smem + SW_BE;
+    float* sBg = smem + SW_BG;
+    float* sBh = smem + SW_BH;
+    __shared__ __align__(8) uint64_t bars[3];      // [0]: W_enc, [1 + s]: gate-weight ring stage s
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    const int64_t row0 = (int64_t)blockIdx.x * PW_ROWS;
+    const int valid = (int)((p.m - row0) < PW_ROWS ? (p.m - row0) : PW_ROWS);
+    const uint64_t offset = p.counter ? *p.counter : 0ull;
+
+    if (tid == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        mbar_init(&bars[2], 1);
+        mbar_fence_init();
+        mbar_expect_tx(&bars[0], PW_WENC_BYTES);
+        tma_load_1d(sWe, p.w_enc, PW_WENC_BYTES, &bars[0]);
+    }
+    const int F = p.in_features;
+    for (int i = tid; i < PW_ROWS * PL_F; i += 128) {
+        const int r = i >> 7, k = i & (PL_F - 1);
+        sX[r * PL_XP + k] = (r < valid && k < F) ? p.obs[(row0 + r) * p.obs_stride + k] : 0.f;
+    }
+    for (int i = tid; i < PW_H; i += 128) sBe[i] = p.b_enc[i];
+    for (int i = tid; i < 4 * PW_H; i += 128) sBg[i] = p.b_gates[i];
+    for (int i = tid; i < NC * PW_H; i += 128) sWh[(i >> 8) * PW_HP + (i & (PW_H - 1))] = p.w_heads[i];
+    if (tid < NC) sBh[tid] = p.b_heads[tid];
+    __syncthreads();
+
+    const int lr = 16 * warp + g;
+    const bool va = lr < valid, vb = lr + 8 < valid;
+    uint32_t eA[32][4];
+    {
+        float acc[32][4];
+        mbar_wait(&bars[0], 0);
+        lstm_encoder(acc, sX + lr * PL_XP + 2 * t, sWe + g * PL_XP + 2 * t, F);
+        lstm_encoder_relu(acc, sBe, t);
+#pragma unroll
+        for (int nt = 0; nt < 32; ++nt) lstm_a_frag(eA[nt], acc[nt][0], acc[nt][1], acc[nt][2], acc[nt][3]);
+    }
+    fence_proxy_async_smem();                      // the x tile's generic writes before the ring's bulk copies
+    __syncthreads();                               // W_enc and the x tile are consumed: ring and h tile from here
+    if (tid == 0) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            mbar_expect_tx(&bars[1 + s], PW_CHUNK_BYTES);
+            tma_load_1d(sWg + s * PW_CHUNK, p.w_gates + (int64_t)s * PW_CHUNK, PW_CHUNK_BYTES, &bars[1 + s]);
+        }
+    }
+    float* h_a = p.h + (row0 + lr) * p.h_stride;
+    float* h_b = h_a + 8 * p.h_stride;
+    float* c_a = p.c + (row0 + lr) * p.c_stride;
+    float* c_b = c_a + 8 * p.c_stride;
+    // h_prev of this warp's rows into the h tile before any of them is overwritten (only this warp reads them)
+    lstm_load_h_tile(sHt, 16 * warp, lane, [&](int r) -> const float* {
+        return 16 * warp + r < valid ? p.h + (row0 + 16 * warp + r) * p.h_stride : nullptr;
+    });
+    __syncwarp();
+
+    float out[NC / 8][4];
+#pragma unroll
+    for (int q = 0; q < NC / 8; ++q) { out[q][0] = out[q][1] = out[q][2] = out[q][3] = 0.f; }
+    const float* wlane = sWg + g * PW_GP + 2 * t;
+    const float* hs = sHt + lr * PW_HP + 2 * t;
+#pragma unroll 1
+    for (int ch = 0; ch < PW_CHUNKS; ++ch) {
+        const int s = ch & 1;
+        const int u0 = 8 * ch + 2 * t;
+        const float2 ca = va ? *reinterpret_cast<const float2*>(c_a + u0) : make_float2(0.f, 0.f);
+        const float2 cb = vb ? *reinterpret_cast<const float2*>(c_b + u0) : make_float2(0.f, 0.f);
+        float gacc[4][4];
+        mbar_wait(&bars[1 + s], (uint32_t)(ch >> 1) & 1u);
+        lstm_gate_chunk_256(gacc, eA, hs, wlane + s * PW_CHUNK);
+        __syncthreads();                           // every warp is done with stage s: refill it with chunk ch + 2
+        if (tid == 0 && ch + 2 < PW_CHUNKS) {
+            mbar_expect_tx(&bars[1 + s], PW_CHUNK_BYTES);
+            tma_load_1d(sWg + s * PW_CHUNK, p.w_gates + (int64_t)(ch + 2) * PW_CHUNK, PW_CHUNK_BYTES, &bars[1 + s]);
+        }
+        const float cp[4] = {ca.x, ca.y, cb.x, cb.y};
+        float act[4][4], cn[4], hn[4];
+        lstm_cell(gacc, sBg + 32 * ch + 2 * t, cp, act, cn, hn);
+        if (va) {
+            *reinterpret_cast<float2*>(c_a + u0) = make_float2(cn[0], cn[1]);
+            *reinterpret_cast<float2*>(h_a + u0) = make_float2(hn[0], hn[1]);
+        }
+        if (vb) {
+            *reinterpret_cast<float2*>(c_b + u0) = make_float2(cn[2], cn[3]);
+            *reinterpret_cast<float2*>(h_b + u0) = make_float2(hn[2], hn[3]);
+        }
+        lstm_head_chunk<NC, PW_HP>(out, hn, sWh, g, u0);
+    }
+    sample_rows<NC>(out, sBh, p, row0, lr, lane, tid, offset);
+}
+
 template <int NC>
 int launch(const LstmParams& p, cudaStream_t stream) {
     PB_CUDA(cudaFuncSetAttribute(k_policy_lstm_sample<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PL_SMEM));
     k_policy_lstm_sample<NC><<<(unsigned)pb_ceil_div(p.m, PL_ROWS), PL_THREADS, PL_SMEM, stream>>>(p);
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
+
+template <int NC>
+int launch_256(const LstmParams& p, cudaStream_t stream) {
+    PB_CUDA(cudaFuncSetAttribute(k_policy_lstm_sample_256<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)PW_SMEM));
+    k_policy_lstm_sample_256<NC><<<(unsigned)pb_ceil_div(p.m, PW_ROWS), 128, PW_SMEM, stream>>>(p);
     PB_LAUNCH_CHECK();
     return PB_OK;
 }
@@ -240,19 +410,23 @@ extern "C" int pb_policy_lstm_sample(const float* obs, int64_t obs_stride, int32
     if (m == 0) return PB_OK;
     PB_REQUIRE(in_features >= 1 && in_features <= PL_F, PB_ERR_UNSUPPORTED,
                "pb_policy_lstm_sample: observation features must be in [1, %d] (got %d)", PL_F, in_features);
-    PB_REQUIRE(input_size == PL_H && hidden_size == PL_H, PB_ERR_UNSUPPORTED,
-               "pb_policy_lstm_sample: built for LSTM input and hidden size %d (got %d, %d)", PL_H, input_size, hidden_size);
+    PB_REQUIRE(input_size == hidden_size && (hidden_size == PL_H || hidden_size == PW_H), PB_ERR_UNSUPPORTED,
+               "pb_policy_lstm_sample: built for LSTM input size = hidden size = %d or %d (got %d, %d)", PL_H, PW_H,
+               input_size, hidden_size);
     PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "pb_policy_lstm_sample: n_act must be in [1, 15]");
     PB_REQUIRE(obs && w_enc && b_enc && w_gates && b_gates && w_heads && b_heads && h && c && actions && logprobs && values,
                PB_ERR_INVALID, "pb_policy_lstm_sample: null pointer");
     PB_REQUIRE(obs_stride >= in_features, PB_ERR_INVALID, "pb_policy_lstm_sample: obs_stride < in_features");
     PB_REQUIRE(((uintptr_t)w_enc & 15) == 0 && ((uintptr_t)w_gates & 15) == 0, PB_ERR_INVALID,
                "pb_policy_lstm_sample: w_enc / w_gates must be 16-byte aligned");
-    PB_REQUIRE(((uintptr_t)h & 7) == 0 && ((uintptr_t)c & 7) == 0 && h_stride >= PL_H && c_stride >= PL_H &&
-                   h_stride % 2 == 0 && c_stride % 2 == 0,
-               PB_ERR_INVALID, "pb_policy_lstm_sample: h / c must be 8-byte aligned with even row strides >= %d", PL_H);
+    PB_REQUIRE(((uintptr_t)h & 7) == 0 && ((uintptr_t)c & 7) == 0 && h_stride >= hidden_size &&
+                   c_stride >= hidden_size && h_stride % 2 == 0 && c_stride % 2 == 0,
+               PB_ERR_INVALID, "pb_policy_lstm_sample: h / c must be 8-byte aligned with even row strides >= %d",
+               hidden_size);
     PB_REQUIRE(!ticket_dev || counter_dev, PB_ERR_INVALID, "pb_policy_lstm_sample: ticket_dev needs counter_dev");
     LstmParams p{obs, obs_stride, in_features, w_enc, b_enc, w_gates, b_gates, w_heads, b_heads, h, h_stride, c, c_stride,
                  m, n_act, seed, counter_dev, ticket_dev, actions, logprobs, values, entropies};
+    if (hidden_size == PW_H)
+        return n_act + 1 <= 8 ? launch_256<8>(p, (cudaStream_t)stream) : launch_256<16>(p, (cudaStream_t)stream);
     return n_act + 1 <= 8 ? launch<8>(p, (cudaStream_t)stream) : launch<16>(p, (cudaStream_t)stream);
 }

@@ -175,11 +175,12 @@ class RecurrentPolicy(torch.nn.Module):
         x2 = x.reshape(n, -1)
         if x2.stride(1) != 1:
             return None
+        hid = model.recurrent.hidden_size
         if state is None:
-            state = (torch.zeros(1, n, 128, device=dev), torch.zeros(1, n, 128, device=dev))
+            state = (torch.zeros(1, n, hid, device=dev), torch.zeros(1, n, hid, device=dev))
         h, c = state
-        for s in (h, c):     # [1, n, 128] fp32 rows (a slice lstm_h[:, lo:hi] of the rollout state is fine)
-            if not (s.dim() == 3 and tuple(s.shape) == (1, n, 128) and s.dtype == torch.float32 and s.device == dev
+        for s in (h, c):     # [1, n, H] fp32 rows (a slice lstm_h[:, lo:hi] of the rollout state is fine)
+            if not (s.dim() == 3 and tuple(s.shape) == (1, n, hid) and s.dtype == torch.float32 and s.device == dev
                     and s.stride(2) == 1 and s.stride(1) % 2 == 0 and s.data_ptr() % 8 == 0):
                 return None
         if out is None:
@@ -198,7 +199,7 @@ class RecurrentPolicy(torch.nn.Module):
         _native.check(_native.lib().pb_policy_lstm_sample(
             _native.ptr(x2), x2.stride(0), x2.shape[1], _native.ptr(w_enc), _native.ptr(b_enc), _native.ptr(w_gates),
             _native.ptr(b_gates), _native.ptr(w_cat), _native.ptr(b_cat), _native.ptr(h), h.stride(1), _native.ptr(c),
-            c.stride(1), n, 128, 128, n_act, C.c_uint64(self._seed), _native.ptr(self._counter), _native.ptr(self._ticket),
+            c.stride(1), n, hid, hid, n_act, C.c_uint64(self._seed), _native.ptr(self._counter), _native.ptr(self._ticket),
             _native.ptr(actions), _native.ptr(logprob), _native.ptr(value), _native.ptr(ent), _native.stream_ptr()))
         return actions, logprob, ent, value, (h, c)
 

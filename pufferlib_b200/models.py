@@ -71,6 +71,9 @@ class _DefaultMLPFunction(torch.autograd.Function):
 
 # hidden sizes the hand-written kernels are built for (pb_policy_mlp_sample, pb_mlp_tail_backward_ex): 128 * k, k <= 4
 FAST_HIDDEN = (128, 256, 384, 512)
+# LSTM sizes H (input size = hidden size = the inner Default's hidden size) of the fused recurrent kernels
+# (pb_policy_lstm_sample, pb_lstm_bptt_*)
+FUSED_LSTM_HIDDEN = (128, 256)
 
 
 def _slab_split(g_, r_, split=64):
@@ -106,8 +109,8 @@ class _LSTMBPTTFunction(torch.autograd.Function):
     """LSTMWrapper(models.Default) over a minibatch of bptt segments as one autograd node (the fused recurrent update).
 
     forward : pb_lstm_bptt_forward -- encoder, LSTM cell over the T steps and both heads; returns the packed head output
-              out [B*T, R] (n_act logits | value | zero pad, rows b*T + t) and the final state (h_T, c_T) [B, 128], and
-              keeps the saved-activation rows [B*T, 1024] for the backward.
+              out [B*T, R] (n_act logits | value | zero pad, rows b*T + t) and the final state (h_T, c_T) [B, H], and
+              keeps the saved-activation rows [B*T, 8H] for the backward (H = 128 or 256: LSTMWrapper.fused_supported).
     backward: pb_lstm_bptt_backward -- dz (the gate pre-activations) and dPre (the encoder pre-activation) in reverse
               time; the weight gradients are library GEMMs on those buffers (_gemm_tn).  The observations and the initial
               state get no gradient; neither does the final state (train() hands it on detached).
@@ -120,22 +123,22 @@ class _LSTMBPTTFunction(torch.autograd.Function):
     def forward(ctx, x, h0, c0, ops, w_enc, b_enc, w_ih, w_hh, b_ih, b_hh, w_dec, b_dec, w_val, b_val):
         from pufferlib_b200 import _native
         w_enc_p, b_enc_p, w_gates, b_gates, w_cat, b_cat, w_gates_t = ops
-        n_act, seg = w_dec.shape[0], x.dim() == 4
+        n_act, seg, hid = w_dec.shape[0], x.dim() == 4, w_hh.shape[1]
         bsz, steps, feats = (x.shape[0] * x.shape[1],) + tuple(x.shape[2:]) if seg else x.shape
         m = bsz * steps
         out = x.new_empty(m, w_cat.shape[0])
-        h_out, c_out = x.new_empty(bsz, 128), x.new_empty(bsz, 128)
-        saved = x.new_empty(m, 1024)
+        h_out, c_out = x.new_empty(bsz, hid), x.new_empty(bsz, hid)
+        saved = x.new_empty(m, 8 * hid)
         P, lib = _native.ptr, _native.lib()
         if seg:
             _native.check(lib.pb_lstm_bptt_forward_rows(
                 P(x), feats, bsz, steps, x.shape[1], x.stride(0), x.stride(1), x.stride(2), P(h0), P(c0), P(w_enc_p),
-                P(b_enc_p), P(w_gates), P(b_gates), P(w_cat), P(b_cat), 128, 128, n_act, P(out), P(h_out), P(c_out),
+                P(b_enc_p), P(w_gates), P(b_gates), P(w_cat), P(b_cat), hid, hid, n_act, P(out), P(h_out), P(c_out),
                 P(saved), _native.stream_ptr()))
         else:
             _native.check(lib.pb_lstm_bptt_forward(
                 P(x), x.stride(1), feats, bsz, steps, P(h0), P(c0), P(w_enc_p), P(b_enc_p), P(w_gates), P(b_gates),
-                P(w_cat), P(b_cat), 128, 128, n_act, P(out), P(h_out), P(c_out), P(saved), _native.stream_ptr()))
+                P(w_cat), P(b_cat), hid, hid, n_act, P(out), P(h_out), P(c_out), P(saved), _native.stream_ptr()))
         ctx.save_for_backward(x, c0, saved, w_gates_t, w_cat)
         ctx.n_act = n_act
         ctx.mark_non_differentiable(h_out, c_out)
@@ -145,31 +148,31 @@ class _LSTMBPTTFunction(torch.autograd.Function):
     def backward(ctx, dout, _dh, _dc):
         from pufferlib_b200 import _native
         x, c0, saved, w_gates_t, w_cat = ctx.saved_tensors
-        n_act, seg = ctx.n_act, x.dim() == 4
+        n_act, seg, hid = ctx.n_act, x.dim() == 4, saved.shape[1] // 8
         bsz, steps, feats = (x.shape[0] * x.shape[1],) + tuple(x.shape[2:]) if seg else x.shape
         m = bsz * steps
         dout = dout.contiguous()
-        dz = x.new_empty(m, 512)
-        dpre = x.new_empty(m, 128)
+        dz = x.new_empty(m, 4 * hid)
+        dpre = x.new_empty(m, hid)
         P, lib = _native.ptr, _native.lib()
         if seg:       # dPre row (e, g, t) -> (g*T + t)*E + e: slab g holds the rows of observation slab g, (t, e) order
             e_, g_ = x.shape[:2]
             _native.check(lib.pb_lstm_bptt_backward_rows(
-                P(dout), P(saved), P(c0), P(w_gates_t), P(w_cat), bsz, steps, 128, 128, n_act, g_, 128, 128 * steps * e_,
-                128 * e_, P(dz), P(dpre), _native.stream_ptr()))
+                P(dout), P(saved), P(c0), P(w_gates_t), P(w_cat), bsz, steps, hid, hid, n_act, g_, hid, hid * steps * e_,
+                hid * e_, P(dz), P(dpre), _native.stream_ptr()))
             x_rows = x.permute(1, 2, 0, 3).view(g_, steps * e_, feats)     # [G, T*E, F] slabs, a view (forward_packed_seq)
         else:
             _native.check(lib.pb_lstm_bptt_backward(
-                P(dout), P(saved), P(c0), P(w_gates_t), P(w_cat), bsz, steps, 128, 128, n_act, P(dz), P(dpre),
+                P(dout), P(saved), P(c0), P(w_gates_t), P(w_cat), bsz, steps, hid, hid, n_act, P(dz), P(dpre),
                 _native.stream_ptr()))
             x_rows = x.reshape(m, feats)
-        dw_gates = _gemm_tn(dz, saved[:, :256])            # dz^T [e | h_prev] = [dW_ih | dW_hh]
+        dw_gates = _gemm_tn(dz, saved[:, :2 * hid])        # dz^T [e | h_prev] = [dW_ih | dW_hh]
         db_gates = dz.sum(0)
         dw_enc = _gemm_tn(dpre, x_rows)
-        dw_cat = _gemm_tn(dout, saved[:, 896:])             # dOut^T h
+        dw_cat = _gemm_tn(dout, saved[:, 7 * hid:])         # dOut^T h
         db_cat = dout.sum(0)
         # b_ih and b_hh get the same gradient, as separate tensors (their .grad must not alias)
-        return (None, None, None, None, dw_enc, dpre.sum(0), dw_gates[:, :128], dw_gates[:, 128:], db_gates,
+        return (None, None, None, None, dw_enc, dpre.sum(0), dw_gates[:, :hid], dw_gates[:, hid:], db_gates,
                 db_gates.clone(), dw_cat[:n_act], db_cat[:n_act], dw_cat[n_act:n_act + 1], db_cat[n_act:n_act + 1])
 
 
@@ -312,22 +315,23 @@ class LSTMWrapper(nn.Module):
             self.policy.invalidate_cache()
 
     def fused_supported(self, x):
-        """Can pb_policy_lstm_sample run this model on observations x?  One LSTM layer with bias, input and hidden size
-        128, a models.Default inner policy with a 128-unit encoder and <= 15 actions, fp32 CUDA observations of <= 128
-        features."""
+        """Can pb_policy_lstm_sample run this model on observations x?  One LSTM layer with bias, input size = hidden
+        size = H with H in FUSED_LSTM_HIDDEN, a models.Default inner policy with an H-unit encoder and <= 15 actions,
+        fp32 CUDA observations of <= 128 features."""
         rnn, inner = self.recurrent, self.policy
-        if not (isinstance(inner, Default) and rnn.num_layers == 1 and rnn.bias and rnn.input_size == 128
-                and rnn.hidden_size == 128 and getattr(rnn, 'proj_size', 0) == 0):
+        H = rnn.hidden_size
+        if not (isinstance(inner, Default) and rnn.num_layers == 1 and rnn.bias and H in FUSED_LSTM_HIDDEN
+                and rnn.input_size == H and getattr(rnn, 'proj_size', 0) == 0):
             return False
         n_act, hid = inner.decoder.weight.shape
         feats = int(np.prod(self.obs_shape))
-        return (tuple(inner.encoder.weight.shape) == (128, feats) and hid == 128 and n_act <= 15 and feats <= 128
+        return (tuple(inner.encoder.weight.shape) == (H, feats) and hid == H and n_act <= 15 and feats <= 128
                 and x.is_cuda and x.dtype == torch.float32 and rnn.weight_ih_l0.dtype == torch.float32)
 
     def fused_operands(self):
-        """The packed operands of pb_policy_lstm_sample (layouts in include/pufferlib_b200.h):
-        (w_enc [128, 136] TF32, b_enc [128], w_gates [16 * 32, 264] TF32 in chunk order, b_gates [16 * 32] = b_ih + b_hh
-        in chunk order, w_cat [8 or 16, 128], b_cat).  Cached under no_grad, keyed like Default.head_matrix."""
+        """The packed operands of pb_policy_lstm_sample (layouts in include/pufferlib_b200.h), for H = hidden size:
+        (w_enc [H, 136] TF32, b_enc [H], w_gates [H/8 * 32, 2H + 8] TF32 in chunk order, b_gates [4H] = b_ih + b_hh
+        in chunk order, w_cat [8 or 16, H], b_cat).  Cached under no_grad, keyed like Default.head_matrix."""
         cache = self._fused_cache
         rnn, inner = self.recurrent, self.policy
         key = (inner.encoder.weight.data_ptr(), rnn.weight_ih_l0.data_ptr(), rnn.weight_hh_l0.data_ptr(),
@@ -335,15 +339,15 @@ class LSTMWrapper(nn.Module):
         if not torch.is_grad_enabled() and cache.get('key') == key:
             return cache['ops']
         with torch.no_grad():
-            w = inner.encoder.weight
-            w_enc = w.new_zeros(128, 136)
+            w, H = inner.encoder.weight, rnn.hidden_size
+            w_enc = w.new_zeros(H, 136)
             w_enc[:, :w.shape[1]] = _round_tf32(w)
-            # chunk ch, row 8j + u <- gate j of unit 8ch + u = row 128j + 8ch + u of [W_ih | W_hh]
+            # chunk ch, row 8j + u <- gate j of unit 8ch + u = row Hj + 8ch + u of [W_ih | W_hh]
             dev = w.device
-            order = (torch.arange(4, device=dev)[None, :, None] * 128 + torch.arange(16, device=dev)[:, None, None] * 8
+            order = (torch.arange(4, device=dev)[None, :, None] * H + torch.arange(H // 8, device=dev)[:, None, None] * 8
                      + torch.arange(8, device=dev)[None, None, :]).reshape(-1)
-            w_gates = w.new_zeros(16 * 32, 264)
-            w_gates[:, :256] = _round_tf32(torch.cat([rnn.weight_ih_l0, rnn.weight_hh_l0], dim=1)[order])
+            w_gates = w.new_zeros(H // 8 * 32, 2 * H + 8)
+            w_gates[:, :2 * H] = _round_tf32(torch.cat([rnn.weight_ih_l0, rnn.weight_hh_l0], dim=1)[order])
             b_gates = (rnn.bias_ih_l0 + rnn.bias_hh_l0)[order].contiguous()
             w_cat, b_cat = inner.head_matrix()
             ops = (w_enc, inner.encoder.bias.detach(), w_gates, b_gates, w_cat, b_cat)
@@ -352,8 +356,8 @@ class LSTMWrapper(nn.Module):
         return ops
 
     def gate_weights_transposed(self):
-        """The gate weights for the backward product of pb_lstm_bptt_backward: [16 * 256, 40] TF32 (cvt.rna); chunk ch,
-        row n, column 8j + u = row 128j + 8ch + u, column n of [W_ih | W_hh]; columns 32..39 zero.  Cached under
+        """The gate weights for the backward product of pb_lstm_bptt_backward: [H/8 * 2H, 40] TF32 (cvt.rna); chunk ch,
+        row n, column 8j + u = row Hj + 8ch + u, column n of [W_ih | W_hh]; columns 32..39 zero.  Cached under
         no_grad, keyed like fused_operands."""
         cache = self._fused_cache
         rnn = self.recurrent
@@ -361,11 +365,12 @@ class LSTMWrapper(nn.Module):
         if not torch.is_grad_enabled() and cache.get('tkey') == key:
             return cache['wt']
         with torch.no_grad():
-            w = _round_tf32(torch.cat([rnn.weight_ih_l0, rnn.weight_hh_l0], dim=1))      # [512, 256]
-            wt = w.new_zeros(16, 256, 40)
-            # w.view(4, 16, 8, 256)[j, ch, u, n] = row 128j + 8ch + u -> [ch, n, 8j + u]
-            wt[:, :, :32] = w.view(4, 16, 8, 256).permute(1, 3, 0, 2).reshape(16, 256, 32)
-            wt = wt.view(16 * 256, 40)
+            H = rnn.hidden_size
+            w = _round_tf32(torch.cat([rnn.weight_ih_l0, rnn.weight_hh_l0], dim=1))      # [4H, 2H]
+            wt = w.new_zeros(H // 8, 2 * H, 40)
+            # w.view(4, H/8, 8, 2H)[j, ch, u, n] = row Hj + 8ch + u -> [ch, n, 8j + u]
+            wt[:, :, :32] = w.view(4, H // 8, 8, 2 * H).permute(1, 3, 0, 2).reshape(H // 8, 2 * H, 32)
+            wt = wt.view(H // 8 * 2 * H, 40)
         if not torch.is_grad_enabled():
             cache['tkey'], cache['wt'] = key, wt
         return wt
@@ -373,8 +378,8 @@ class LSTMWrapper(nn.Module):
     def forward_packed_seq(self, x, state=None):
         """The training forward over bptt segments on the fused kernels (pb_lstm_bptt_forward / _backward):
         x [B, T, *obs], or the strided segment view [E, G, T, *obs] of Experience.segment_obs with segment b = e*G + g
-        (B = E*G; read in place, pb_lstm_bptt_forward_rows / _backward_rows); state (h, c) of shape [1, B, 128] (detached)
-        or None (zeros).  -> (out [B*T, R], n_act, (h_T, c_T) [1, B, 128]) with logits = out[:, :n_act],
+        (B = E*G; read in place, pb_lstm_bptt_forward_rows / _backward_rows); state (h, c) of shape [1, B, H] (detached)
+        or None (zeros), H the hidden size.  -> (out [B*T, R], n_act, (h_T, c_T) [1, B, H]) with logits = out[:, :n_act],
         value = out[:, n_act], rows b*T + t in both cases; or None when the fast path does not apply (fused_supported
         fails, the inner Default's fast_path is off, or the layout is not one the kernel reads).  The packed operands are
         rebuilt on every call that records gradients."""
@@ -403,7 +408,7 @@ class LSTMWrapper(nn.Module):
         if state is not None:
             h0, c0 = state
             for s in (h0, c0):
-                if (tuple(s.shape) != (1, bsz, 128) or s.dtype != torch.float32 or s.device != x.device
+                if (tuple(s.shape) != (1, bsz, self.recurrent.hidden_size) or s.dtype != torch.float32 or s.device != x.device
                         or s.requires_grad):
                     return None
             h0, c0 = h0[0].contiguous(), c0[0].contiguous()

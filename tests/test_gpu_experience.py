@@ -385,8 +385,6 @@ def test_direct_slab_update_replays_through_gathered_minibatches(n, bptt, nm, kw
     B: R = 1024, raw advantages, no clipping.  With breakout's 4 actions, one 128-byte line of the value-head weight is
     updated by two CTAs of pb_clip_adam_parts (asserted below): a head matrix rebuilt from a stale copy of that line would
     change the next minibatch."""
-    import ctypes as C
-    import util_update as uu
     from pufferlib_b200 import models
     from pufferlib_b200.frameworks import cleanrl
     h = 128
@@ -395,8 +393,26 @@ def test_direct_slab_update_replays_through_gathered_minibatches(n, bptt, nm, kw
     pol = cleanrl.Policy(models.Default(vec.driver_env), fused_sample=True, seed=7).cuda()
     cfg = make_config(n, h, env='breakout', bptt_horizon=bptt, minibatch_size=n * h // nm, **kw)
     data = clean_pufferl.create(cfg, vec, pol)
+    norms = replay_direct_update(data)
+    if cfg.max_grad_norm < 1:
+        assert min(norms) > cfg.max_grad_norm, norms          # every step clipped
+    else:
+        assert max(norms) < cfg.max_grad_norm, norms
+    clean_pufferl.close(data)
+
+
+def replay_direct_update(data, exp_avg_tol=1e-4):
+    """The body of test_direct_slab_update_replays_through_gathered_minibatches for a breakout `data` (models.Default,
+    config.update_epochs x num_minibatches steps): evaluate + train once, evaluate, snapshot, train() on the 'direct' path,
+    then the replay and its checks (exp_avg_tol: the bound on the first Adam moments, relative to each one's maximum).
+    Returns the gradient norms the replay's pb_clip_adam computed, one per step."""
+    import ctypes as C
+    import util_update as uu
+    cfg, pol = data.config, data.policy
     clean_pufferl.evaluate(data)
-    clean_pufferl.train(data)                    # the Adam state exists and the learning rate is annealed once
+    n = data.experience.num_envs
+    h, nm, bptt = cfg.batch_size // n, cfg.batch_size // cfg.minibatch_size, cfg.bptt_horizon
+    clean_pufferl.train(data)                  # the Adam state exists and the learning rate is annealed once
     assert data.train_minibatch_path == 'direct'
     clean_pufferl.evaluate(data)
     exp, model, opt = data.experience, pol.policy, data.optimizer
@@ -454,10 +470,6 @@ def test_direct_slab_update_replays_through_gathered_minibatches(n, bptt, nm, kw
             norms.append(float(norm_out))
     torch.cuda.synchronize()
     n_steps = cfg.update_epochs * nm
-    if cfg.max_grad_norm < 1:
-        assert min(norms) > cfg.max_grad_norm, norms          # every step clipped
-    else:
-        assert max(norms) < cfg.max_grad_norm, norms
     errs = {}
     for k, p in enumerate(params):
         errs[f'param{k}'] = float((p.detach() - mine[k]).abs().max())
@@ -468,7 +480,7 @@ def test_direct_slab_update_replays_through_gathered_minibatches(n, bptt, nm, kw
     for k in range(6):
         # one Adam step moves a parameter by at most ~lr; the two sides agree to 1e-3 of that per step
         assert errs[f'param{k}'] <= 1e-3 * lr * n_steps, errs
-        assert errs[f'exp_avg{k}'] <= 1e-4 and errs[f'exp_avg_sq{k}'] <= 1e-4, errs
+        assert errs[f'exp_avg{k}'] <= exp_avg_tol and errs[f'exp_avg_sq{k}'] <= 1e-4, errs
     # the head matrix train() leaves is the packed form of its own parameters, bit for bit, and the replay's up to the above
     mu = data.manual_update
     w_ref, b_ref = torch.full_like(w_cat, 9.0), torch.full_like(b_cat, 9.0)
@@ -485,4 +497,4 @@ def test_direct_slab_update_replays_through_gathered_minibatches(n, bptt, nm, kw
     # move it by ~1e-7 of a term
     assert abs(got[0] - tot[0]) <= 1e-6, (got, tot)
     assert np.allclose(got[1:], tot[1:], rtol=1e-4, atol=0), (got, tot)
-    clean_pufferl.close(data)
+    return norms

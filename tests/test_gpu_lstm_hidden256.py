@@ -367,9 +367,11 @@ def test_backward_matches_fp64_autograd(feats, n_act, bsz, steps, init):
     assert all(e < TOL_GRAD for e in errs.values()), errs
 
 
-def reference_grads_h(net, x, h0, c0, dout):
+def reference_grads_h(net, x, h0, c0, dout, pre_grads=None):
     """reference_grads of test_gpu_lstm_bptt.py at the net's hidden size: fp64 autograd with the kernels' operand
-    rounding (TF32 leaves for x, W_enc, the gate weights and W_cat; e, h_prev and h' rounded with identity gradient)."""
+    rounding (TF32 leaves for x, W_enc, the gate weights and W_cat; e, h_prev and h' rounded with identity gradient).
+    pre_grads: a dict that also receives the gradients pb_lstm_bptt_backward writes, rows b*T + t: 'dz' [B*T, 4H] of the gate
+    pre-activations (i, f, g, o) and 'dpre' [B*T, H] of the encoder pre-activation."""
     inner, rnn = net.policy, net.recurrent
     bsz, steps, _ = x.shape
     hid = rnn.hidden_size
@@ -392,16 +394,25 @@ def reference_grads_h(net, x, h0, c0, dout):
     z0 = torch.zeros(bsz, hid, dtype=torch.float64, device='cuda')
     h = z0 if h0 is None else h0.double()
     c = z0 if c0 is None else c0.double()
-    outs = []
+    outs, pres, zs = [], [], []
     for t in range(steps):
-        e = torch.relu(rna(x[:, t]) @ p['encoder.weight'].t() + p['encoder.bias'])
+        pre = rna(x[:, t]) @ p['encoder.weight'].t() + p['encoder.bias']
+        e = torch.relu(pre)
         zz = ste(e) @ p['weight_ih_l0'].t() + ste(h) @ p['weight_hh_l0'].t() + p['bias_ih_l0'] + p['bias_hh_l0']
+        if pre_grads is not None:
+            pre.retain_grad()
+            zz.retain_grad()
+            pres.append(pre)
+            zs.append(zz)
         i, f, g, o = zz.chunk(4, 1)
         c = torch.sigmoid(f) * c + torch.sigmoid(i) * torch.tanh(g)
         h = torch.sigmoid(o) * torch.tanh(c)
         outs.append(ste(h) @ w_cat.t() + b_cat)
     out = torch.stack(outs, 1).reshape(bsz * steps, R)
     (out * dout.double()).sum().backward()
+    if pre_grads is not None:
+        pre_grads['dz'] = torch.stack([z.grad for z in zs], 1).reshape(bsz * steps, 4 * hid)
+        pre_grads['dpre'] = torch.stack([q.grad for q in pres], 1).reshape(bsz * steps, hid)
     return {k: v.grad for k, v in p.items()}
 
 

@@ -155,25 +155,30 @@ def clip_offsets(n, dev):
 
 
 def case(slab_rows, n_slabs, slab_stride, n_act, seed, nm=None, returns=True, old_values=True, adv_norm=False, cfg=CFG,
-         ws=None):
+         ws=None, mb=None, x_tail=64):
     """One minibatch of `n_slabs` slabs of `slab_rows` rows whose x rows start `slab_stride` rows apart.
 
-    nm (arrival-order rows, as Experience.minibatch 'direct'): the per-row arrays live in buffers of n_slabs * nm slabs, the
-    minibatch's slab s at slab s * nm + 1, and the kernel gets the pointer offset by one slab and row_slab_stride = nm * R;
-    every other element is NaN.  Otherwise they are contiguous, slab-major.  returns=False: the kernel forms raw advantages +
-    old values; old_values=False (needs returns and clip_vloss = 0): no old values at all; adv_norm: the kernel normalises
-    the advantages with device constants (mean, 1 / (std + 1e-8)).  ws: a workspace to reuse (else a fresh NaN one)."""
+    nm (arrival-order rows, as Experience.minibatch 'direct'): the per-row arrays live in buffers of exactly n_slabs * nm
+    slabs, the minibatch's slab s at slab s * nm + mb (mb: which of the nm minibatches, default 1), and the kernel gets the
+    pointer offset by mb slabs and row_slab_stride = nm * R; every other element is NaN.  Otherwise they are contiguous,
+    slab-major.  x_tail: rows of X_GAP after the minibatch's last x slab (0 with mb = nm - 1: the x rows and the per-row
+    arrays end flush with their allocations, as the last minibatch of train()'s rollout does).  returns=False: the kernel
+    forms raw advantages + old values; old_values=False (needs returns and clip_vloss = 0): no old values at all; adv_norm:
+    the kernel normalises the advantages with device constants (mean, 1 / (std + 1e-8)).  ws: a workspace to reuse (else a
+    fresh NaN one)."""
     assert (returns or old_values) and (old_values or not cfg[1])
     dev = torch.device('cuda')
     torch.manual_seed(seed)
     m = slab_rows * n_slabs
-    mb = 1 if nm else 0                                           # the minibatch under test (arrival-order layout)
+    if mb is None:
+        mb = 1 if nm else 0                                       # the minibatch under test (arrival-order layout)
+    assert (0 <= mb < nm) if nm else mb == 0
     if nm:
         assert slab_stride == nm * slab_rows
     total_rows = (n_slabs - 1) * slab_stride + slab_rows
     # x rows outside the minibatch are large and finite: the last tile of a ragged slab loads rows past the slab end into
     # masked rows (0 * x there must stay 0), and a misindexed slab would show up in every gradient
-    xbuf = torch.full((mb * slab_rows + total_rows + 64, 128), X_GAP, device=dev)
+    xbuf = torch.full((mb * slab_rows + total_rows + x_tail, 128), X_GAP, device=dev)
     x = torch.randn(m, 128, device=dev)                           # slab-major rows
     for s in range(n_slabs):
         xbuf[mb * slab_rows + s * slab_stride:][:slab_rows] = x[s * slab_rows:(s + 1) * slab_rows]
@@ -235,7 +240,7 @@ def case(slab_rows, n_slabs, slab_stride, n_act, seed, nm=None, returns=True, ol
     if ws is None:
         ws = workspace(dev)
     print(f'case slab_rows={slab_rows} n_slabs={n_slabs} stride={slab_stride} n_act={n_act} (M={m}) '
-          f'nm={nm} returns={returns} old_values={old_values} adv_norm={adv_norm} cfg={cfg}', flush=True)
+          f'nm={nm} mb={mb} x_tail={x_tail} returns={returns} old_values={old_values} adv_norm={adv_norm} cfg={cfg}', flush=True)
 
     def launch(debug, dpre_out=None, gflat=None):
         return fused(xv, 128, slab_rows, slab_stride, n_slabs, w_enc, b_enc, w_cat, b_cat, k_act, k_olp, k_adv, k_ret, k_oval,

@@ -253,8 +253,8 @@ int pb_sample_logits(const float* logits, int64_t logits_stride, int64_t n, int3
  * and the analytic gradients of  loss = mean(pg) - ent_coef*mean(entropy) + vf_coef*0.5*mean(v)  with respect to the
  * logits [m][n_act] and the value [m] (already scaled by 1/m), following ATen's tie rules for maximum / clamp.
  * `advantages` are the (already normalised, clean_pufferl.py:211-213) minibatch advantages.  Strides in floats.
- * Packed rows: when logits, value and both gradients share one 8- or 16-row padded head output [m][W] (W = 8 with
- * n_act <= 7, W = 16 with n_act <= 15; all four strides W, value = logits + n_act, grad_value = grad_logits + n_act,
+ * Packed rows: when logits, value and both gradients share one 8-, 16- or 32-row padded head output [m][W] (W = 8 with
+ * n_act <= 7, W = 16 with n_act <= 15, W = 32 with n_act <= 31; all four strides W, value = logits + n_act, grad_value = grad_logits + n_act,
  * logits and grad_logits 16-byte aligned), every gradient row is written whole, zero padding included. */
 int pb_ppo_loss(const float* logits, int64_t logits_stride, const float* value, int64_t value_stride,
                 const int64_t* actions, const float* old_logprobs, const float* advantages, const float* returns,
@@ -267,8 +267,9 @@ int pb_ppo_loss(const float* logits, int64_t logits_stride, const float* value, 
  * PB_ERR_UNSUPPORTED before any launch otherwise): encoder Linear + ReLU,
  * both heads, sample_logits (frameworks/cleanrl.py:25-47) and the value / logprob / action row stores of
  * Experience.store (clean_pufferl.py:443-446) in ONE launch per env step; the hidden layer never leaves the SM
- * (mma.sync TF32 tensor-core tiles, fp32 accumulate).  w_heads / b_heads: the 8- or 16-row padded head matrix
- * (n_act logits | value | zeros; 8 rows for n_act <= 7, 16 for 8 <= n_act <= 15).  w_enc is consumed as TF32: the tensor core ignores the low 13 mantissa bits, so pass
+ * (mma.sync TF32 tensor-core tiles, fp32 accumulate).  w_heads / b_heads: the 8-, 16- or 32-row padded head matrix
+ * (n_act logits | value | zeros; 8 rows for n_act <= 7, 16 for 8 <= n_act <= 15, 32 for 16 <= n_act <= 31; n_act > 31:
+ * PB_ERR_UNSUPPORTED; with more than 15 actions w_heads must be 16-byte aligned).  w_enc is consumed as TF32: the tensor core ignores the low 13 mantissa bits, so pass
  * it pre-rounded (cvt.rna) for round-to-nearest products.  Sampling: counter-based inverse CDF on (seed, *counter_dev, row).  With a non-null
  * ticket_dev (one zero-initialised uint32 owned by the caller) the last CTA to finish advances *counter_dev by 1, so a
  * captured rollout graph needs no separate counter update per env step. */
@@ -392,11 +393,11 @@ int pb_rollout_debug_buffers(float* hidden, float* out);
  * backward pass after the encoder GEMM, in ONE pass over the hidden layer instead of five ATen launches:
  *   dpre[m][H]      = (dout[m][0..R-1] @ w_heads[R][H]) * (hidden > 0)                (heads dX + ReLU backward)
  *   grads_out       = [ dW_heads (R*H) | db_enc (H) = column sums of dpre | db_heads (R) = column sums of dout ]
- * dout holds the loss gradient w.r.t. the R padded head outputs (n_act logits, the value, zero padding) of the 8- or
- * 16-row padded head matrix w_heads, row stride dout_stride floats.  Deterministic (two-stage partial sums).
+ * dout holds the loss gradient w.r.t. the R padded head outputs (n_act logits, the value, zero padding) of the 8-, 16-
+ * or 32-row padded head matrix w_heads, row stride dout_stride floats.  Deterministic (two-stage partial sums).
  * H = 128, 256, 384 or 512 (PB_ERR_UNSUPPORTED before any launch otherwise).
  * Pointers 16-byte aligned.  pb_mlp_tail_workspace_bytes / pb_mlp_tail_backward: R = 8 (n_act <= 7); the _ex forms take
- * R = head_rows, 8 or 16 (16 for 8 <= n_act <= 15). */
+ * R = head_rows, 8, 16 or 32 (16 for 8 <= n_act <= 15, 32 for 16 <= n_act <= 31; other values: PB_ERR_UNSUPPORTED). */
 size_t pb_mlp_tail_workspace_bytes(int64_t m, int32_t hidden_size);
 int pb_mlp_tail_backward(const float* dout, int64_t dout_stride, const float* w_heads, const float* hidden, int64_t m,
                          int32_t hidden_size, float* dpre, float* grads_out, void* workspace, size_t workspace_bytes,
@@ -517,8 +518,8 @@ int pb_clip_adam_peer(const pb_adam_tensor* tensors, int32_t n_tensors, float ma
                       const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
                       const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, void* stream);
 
-/* The 8- or 16-row padded head matrix of models.Default (pufferlib/models.py:33-38: decoder rows | value_head row | zero
- * padding; 8 rows for n_act <= 7, 16 for 8 <= n_act <= 15), its bias, and (optionally) the encoder weight rounded to
+/* The 8-, 16- or 32-row padded head matrix of models.Default (pufferlib/models.py:33-38: decoder rows | value_head row |
+ * zero padding; 8 rows for n_act <= 7, 16 for 8 <= n_act <= 15, 32 for 16 <= n_act <= 31), its bias, and (optionally) the encoder weight rounded to
  * TF32, in one launch: the operands pb_policy_mlp_sample, pb_mlp_tail_backward(_ex) and the head GEMM consume. */
 int pb_pack_heads(const float* w_dec, const float* b_dec, const float* w_val, const float* b_val, int32_t n_act,
                   int32_t hidden_size, float* w_cat, float* b_cat, const float* w_enc, float* w_enc_tf32,

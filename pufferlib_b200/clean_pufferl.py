@@ -100,8 +100,8 @@ class _FusedPPOLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, value, actions, old_logprobs, adv, returns, old_values, cfg, packed_n_act):
         """packed_n_act > 0: `logits` is the packed head output [M, R] (logits | value | zero pad; R = 8 for
-        n_act <= 7, 16 for n_act <= 15) and `value` is ignored; the gradient comes back as ONE [M, R] tensor (no
-        slice/cat nodes in the autograd graph)."""
+        n_act <= 7, 16 for n_act <= 15, 32 for n_act <= 31) and `value` is ignored; the gradient comes back as ONE
+        [M, R] tensor (no slice/cat nodes in the autograd graph)."""
         clip_coef, clip_vloss, vf_clip_coef, vf_coef, ent_coef = cfg
         dev = logits.device
         if packed_n_act:
@@ -110,8 +110,9 @@ class _FusedPPOLoss(torch.autograd.Function):
             assert out.stride(1) == 1 and out.dtype == torch.float32
             l_ptr, l_stride = out.data_ptr(), out.stride(0)
             v_ptr, v_stride = out.data_ptr() + 4 * n_act, out.stride(0)
-            # [M, 8] and [M, 16] rows: the kernel writes whole rows (zero padding included); other widths need the memset
-            grad = torch.empty_like(out) if out.shape[1] in (8, 16) and n_act < out.shape[1] else torch.zeros_like(out)
+            # [M, 8], [M, 16] and [M, 32] rows: the kernel writes whole rows (zero padding included); other widths need
+            # the memset
+            grad = torch.empty_like(out) if out.shape[1] in (8, 16, 32) and n_act < out.shape[1] else torch.zeros_like(out)
             gl_ptr, gl_stride, gv_ptr, gv_stride = grad.data_ptr(), grad.stride(0), grad.data_ptr() + 4 * n_act, grad.stride(0)
             ctx.packed = True
             ctx.save_for_backward(grad)
@@ -163,7 +164,7 @@ def fused_ppo_loss(logits, value, actions, old_logprobs, adv, returns, old_value
 
 def fused_ppo_loss_packed(out, n_act, actions, old_logprobs, adv, returns, old_values, config):
     """Same, on the packed head output [M, R] of models.Default.forward_packed or models.LSTMWrapper.forward_packed_seq
-    (R = 8 for n_act <= 7, 16 for n_act <= 15): one [M, R] gradient back."""
+    (R = 8 for n_act <= 7, 16 for n_act <= 15, 32 for n_act <= 31): one [M, R] gradient back."""
     return _FusedPPOLoss.apply(out, None, actions, old_logprobs, adv, returns, old_values, _loss_cfg(config), int(n_act))
 
 
@@ -206,8 +207,8 @@ class _DefaultMLPUpdate:
         encoder GEMM (+bias+ReLU epilogue, one per slab) -> R-column head GEMM -> pb_ppo_loss (loss statistics +
         analytic dLoss/dOut) -> pb_mlp_tail_backward_ex (dPre, dW_heads, db_heads, db_enc) -> split-K dW_enc GEMM + sum
         [-> gradient all-reduce over ONE flat buffer when world_size > 1] -> pb_clip_adam -> pb_pack_heads,
-    with R = 8 head rows for n_act <= 7 and 16 for 8 <= n_act <= 15 (models.Default.head_matrix), for 128 to 512 hidden
-    units (models.FAST_HIDDEN).
+    with R = 8 head rows for n_act <= 7, 16 for 8 <= n_act <= 15 and 32 for 16 <= n_act <= 31 (models.Default.head_matrix),
+    for 128 to 512 hidden units (models.FAST_HIDDEN).
     train() passes each minibatch as Experience.minibatch() to forward_backward; where _fused_ok holds (update_plan asks
     it once per train() and sets used_fused; <= 7 actions) the chain is ONE kernel, pb_mlp_update_fused.
     Same math as the autograd path (tests/test_gpu_experience.py::test_manual_update_matches_autograd_update); the
@@ -223,7 +224,7 @@ class _DefaultMLPUpdate:
         if config.target_kl is not None or not getattr(data, 'own_optimizer', False):
             return False
         n_act, hid = model.decoder.weight.shape
-        if hid not in models.FAST_HIDDEN or n_act > 15 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
+        if hid not in models.FAST_HIDDEN or n_act > 31 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
             return False
         g = opt.param_groups[0]
         if len(opt.param_groups) != 1 or g.get('amsgrad') or g.get('weight_decay') or g.get('maximize'):
@@ -239,7 +240,7 @@ class _DefaultMLPUpdate:
         dev = model.encoder.weight.device
         self.n_act, self.hid = model.decoder.weight.shape
         self.features = model.encoder.weight.shape[1]
-        self.head_rows = 8 if self.n_act + 1 <= 8 else 16
+        self.head_rows = next(r for r in (8, 16, 32) if self.n_act + 1 <= r)
         hid, f_, n_act, rows = self.hid, self.features, self.n_act, self.head_rows
         z = dict(dtype=torch.float32, device=dev)
         # ONE flat gradient buffer: dW_enc | dW_heads (R x hid) | db_enc | db_heads (R)  (also the all-reduce bucket)

@@ -8,7 +8,7 @@
 // This kernel does all five reading `hidden` ONCE and writing dPre once (2 * 4H + 4 NO B per row).  The dense H x H
 // encoder GEMMs (forward, and dW_enc = dPre^T @ obs) stay on cuBLAS tensor cores.
 // NO = the padded head rows: 8 for n_act <= 7, 16 for 8 <= n_act <= 15 (models.Default.head_matrix); both kernels are
-// templates on it.
+// templates on it.  32 rows (16 <= n_act <= 31) take the half-width kernels further down (k_mlp_tail_bwd(_tma)_half).
 // A warp owns rows; lane l owns columns 4l..4l+3 (one float4 per row per lane, 512 B coalesced for H = 128); the
 // head weights live in registers (NO x 4 per lane); per-lane accumulators (dW: NO x 4, db_enc: 4) are reduced over
 // the block's warps in shared memory and written as ONE partial row per block; a second tiny kernel sums the
@@ -429,6 +429,164 @@ __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd_tma_slices(const fl
     }
 }
 
+// ---- 32 head rows (16 <= n_act <= 31), any H = 128 k.  With one float4 per lane the head weights and dW accumulators
+// alone would take 256 registers per lane, so here a lane owns ONE float2 of a row: a warp covers 64 columns and the grid
+// runs over 64-column slices of the hidden layer, slice s = blockIdx.y (H / 64 of them, 2 at H = 128).  w and acc_w are
+// then 64 registers each.  `hidden` is still read once and dPre written once; every slice re-reads the row's 128-byte
+// dOut (+12 % bytes at H = 128).  db_heads: lane l sums column l of dOut (one 4-byte load per row and lane) instead of
+// holding 32 sums; slice 0 writes it.  The partial row, k_reduce_partials and the workspace are those of the kernels above.
+constexpr int HS_W = 64;                           // columns per slice
+constexpr int HS_NO = 32;                          // head rows
+constexpr int HS_RSTRIDE = 8 * HS_W + HS_W + HS_NO;   // reduction row: 8 dW rows | db_enc | db_heads (4 passes)
+
+// one row of a slice: dPre's two columns of the lane (returned), and the lane's accumulators
+__device__ __forceinline__ float2 half_slice_row(const float (&d)[HS_NO], float2 hv, const float2 (&w)[HS_NO],
+                                                 float2 (&acc_w)[HS_NO], float2& acc_b) {
+    float2 g = make_float2(0.f, 0.f);
+#pragma unroll
+    for (int k = 0; k < HS_NO; ++k) {
+        g.x = fmaf(d[k], w[k].x, g.x); g.y = fmaf(d[k], w[k].y, g.y);
+        acc_w[k].x = fmaf(d[k], hv.x, acc_w[k].x); acc_w[k].y = fmaf(d[k], hv.y, acc_w[k].y);
+    }
+    g.x = hv.x > 0.f ? g.x : 0.f; g.y = hv.y > 0.f ? g.y : 0.f;
+    acc_b.x += g.x; acc_b.y += g.y;
+    return g;
+}
+
+// the block's sum of every warp's accumulators into its [32 H | H | 32] partial row, in 4 passes of 8 dW rows through
+// s_red [WARPS][HS_RSTRIDE]; pass 0 also carries db_enc and (slice 0) db_heads
+__device__ __forceinline__ void half_slice_reduce(const float2 (&acc_w)[HS_NO], float2 acc_b, float acc_o,
+                                                  float (*s_red)[HS_RSTRIDE], float* out, int h, int col0) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* mine = s_red[warp];
+#pragma unroll
+    for (int pass = 0; pass < HS_NO / 8; ++pass) {
+        if (pass > 0) __syncthreads();   // the previous pass has been summed
+#pragma unroll
+        for (int k = 0; k < 8; ++k) *reinterpret_cast<float2*>(mine + k * HS_W + 2 * lane) = acc_w[8 * pass + k];
+        if (pass == 0) {
+            *reinterpret_cast<float2*>(mine + 8 * HS_W + 2 * lane) = acc_b;
+            mine[9 * HS_W + lane] = acc_o;
+        }
+        __syncthreads();
+        const int n = pass == 0 ? (col0 == 0 ? HS_RSTRIDE : 9 * HS_W) : 8 * HS_W;
+        for (int j = threadIdx.x; j < n; j += MT_THREADS) {
+            float s = 0.f;
+#pragma unroll
+            for (int wq = 0; wq < MT_WARPS; ++wq) s += s_red[wq][j];
+            int64_t idx;
+            if (j < 8 * HS_W) idx = (int64_t)(8 * pass + j / HS_W) * h + col0 + j % HS_W;     // dW_heads
+            else if (j < 9 * HS_W) idx = (int64_t)HS_NO * h + col0 + (j - 8 * HS_W);          // db_enc
+            else idx = (int64_t)HS_NO * h + h + (j - 9 * HS_W);                               // db_heads
+            out[idx] = s;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd_half(const float* __restrict__ dout, int64_t dout_stride,
+                                                                 const float* __restrict__ w_heads,   // [32][h]
+                                                                 const float* __restrict__ hidden,    // [M][h]
+                                                                 float* __restrict__ dpre,            // [M][h]
+                                                                 float* __restrict__ partials, int64_t m, int h) {
+    __shared__ float s_red[MT_WARPS][HS_RSTRIDE];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int col0 = HS_W * (int)blockIdx.y;
+    const float* hcol = hidden + col0 + 2 * lane;
+    float* dcol = dpre + col0 + 2 * lane;
+
+    float2 w[HS_NO], acc_w[HS_NO], acc_b = make_float2(0.f, 0.f);
+    float acc_o = 0.f;
+#pragma unroll
+    for (int k = 0; k < HS_NO; ++k) {
+        w[k] = *reinterpret_cast<const float2*>(w_heads + (int64_t)k * h + col0 + 2 * lane);
+        acc_w[k] = make_float2(0.f, 0.f);
+    }
+    const int64_t row0 = (int64_t)blockIdx.x * ROWS_PER_BLOCK;
+    const int64_t row_end = min(row0 + ROWS_PER_BLOCK, m);
+    for (int64_t r = row0 + warp; r < row_end; r += MT_WARPS) {
+        const float* drow = dout + r * dout_stride;
+        float d[HS_NO];
+        tail_load_dout<HS_NO>(drow, d);
+        acc_o += drow[lane];
+        const float2 hv = __ldcs(reinterpret_cast<const float2*>(hcol + r * h));
+        __stcs(reinterpret_cast<float2*>(dcol + r * h), half_slice_row(d, hv, w, acc_w, acc_b));
+    }
+    half_slice_reduce(acc_w, acc_b, acc_o, s_red, partials + (int64_t)blockIdx.x * (HS_NO * h + h + HS_NO), h, col0);
+}
+
+// TMA-staged (dout contiguous [M][32]): the 4-stage ring of k_mlp_tail_bwd_tma_slices, 32 rows per stage, filled with one
+// 256-byte bulk copy per row (the slice's columns; lane l of warp 0 copies row l of the chunk) plus the chunk's dOut
+// rows: 12 KB per stage, 48 KB of dynamic shared memory.
+__global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd_tma_half(const float* __restrict__ dout,      // [M][32]
+                                                                     const float* __restrict__ w_heads,   // [32][h]
+                                                                     const float* __restrict__ hidden,    // [M][h]
+                                                                     float* __restrict__ dpre,            // [M][h]
+                                                                     float* __restrict__ partials, int64_t m, int h) {
+    constexpr uint32_t H_BYTES = TT_CHUNK * HS_W * 4;
+    extern __shared__ __align__(128) unsigned char dyn[];
+    float* s_h = reinterpret_cast<float*>(dyn);                                   // [STAGES][CHUNK][64]
+    float* s_d = reinterpret_cast<float*>(dyn + (size_t)TT_STAGES * H_BYTES);     // [STAGES][CHUNK][32]
+    __shared__ float s_red[MT_WARPS][HS_RSTRIDE];
+    __shared__ uint64_t bars[TT_STAGES];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int col0 = HS_W * (int)blockIdx.y;
+
+    const int64_t row0 = (int64_t)blockIdx.x * ROWS_PER_BLOCK;
+    const int64_t row_end = min(row0 + ROWS_PER_BLOCK, m);
+    const int n_chunks = (int)((row_end - row0 + TT_CHUNK - 1) / TT_CHUNK);
+    auto issue = [&](int c) {   // warp 0; lane 0 arrives with the byte count before any lane copies
+        const int st = c % TT_STAGES;
+        const int64_t r = row0 + (int64_t)c * TT_CHUNK;
+        const uint32_t rows = (uint32_t)min((int64_t)TT_CHUNK, row_end - r);
+        if (lane == 0) {
+            mbar_expect_tx(&bars[st], rows * (HS_W * 4 + HS_NO * 4));
+            tma_load_1d(s_d + (size_t)st * TT_CHUNK * HS_NO, dout + r * HS_NO, rows * HS_NO * 4, &bars[st]);
+        }
+        __syncwarp();
+        if ((uint32_t)lane < rows)
+            tma_load_1d(s_h + ((size_t)st * TT_CHUNK + lane) * HS_W, hidden + (r + lane) * h + col0, HS_W * 4, &bars[st]);
+    };
+    if (threadIdx.x == 0) {
+        for (int st = 0; st < TT_STAGES; ++st) mbar_init(&bars[st], 1);
+        mbar_fence_init();
+    }
+    __syncthreads();   // barriers initialised before warp 0 copies and anyone waits on them
+    if (warp == 0)
+        for (int c = 0; c < TT_STAGES && c < n_chunks; ++c) issue(c);
+
+    float2 w[HS_NO], acc_w[HS_NO], acc_b = make_float2(0.f, 0.f);
+    float acc_o = 0.f;
+#pragma unroll
+    for (int k = 0; k < HS_NO; ++k) {
+        w[k] = *reinterpret_cast<const float2*>(w_heads + (int64_t)k * h + col0 + 2 * lane);
+        acc_w[k] = make_float2(0.f, 0.f);
+    }
+    float* dcol = dpre + col0 + 2 * lane;
+
+    for (int c = 0; c < n_chunks; ++c) {
+        const int st = c % TT_STAGES;
+        mbar_wait(&bars[st], (uint32_t)((c / TT_STAGES) & 1));
+        const int64_t r0 = row0 + (int64_t)c * TT_CHUNK;
+        const int rows = (int)min((int64_t)TT_CHUNK, row_end - r0);
+        const float* ch = s_h + (size_t)st * TT_CHUNK * HS_W;
+        const float* cd = s_d + (size_t)st * TT_CHUNK * HS_NO;
+#pragma unroll
+        for (int i = 0; i < TT_CHUNK / MT_WARPS; ++i) {
+            const int rl = warp + i * MT_WARPS;
+            if (rl < rows) {
+                float d[HS_NO];
+                tail_load_dout<HS_NO>(cd + rl * HS_NO, d);
+                acc_o += cd[rl * HS_NO + lane];
+                const float2 hv = *reinterpret_cast<const float2*>(ch + rl * HS_W + 2 * lane);
+                __stcs(reinterpret_cast<float2*>(dcol + (r0 + rl) * h), half_slice_row(d, hv, w, acc_w, acc_b));
+            }
+        }
+        __syncthreads();                                   // everyone is done reading stage st
+        if (warp == 0 && c + TT_STAGES < n_chunks) issue(c + TT_STAGES);
+    }
+    half_slice_reduce(acc_w, acc_b, acc_o, s_red, partials + (int64_t)blockIdx.x * (HS_NO * h + h + HS_NO), h, col0);
+}
+
 // deterministic second stage: out[j] = sum over blocks of partials[b][j].  One warp per output element: lane l sums
 // blocks l, l+32, ... in order, then a fixed shuffle tree combines the 32 lane sums (same order every run).
 __global__ void __launch_bounds__(256) k_reduce_partials(const float* __restrict__ partials, int n_blocks, int pstride,
@@ -473,10 +631,24 @@ int launch_tail_slices(const float* dout, int64_t dout_stride, const float* w_he
     return PB_OK;
 }
 
+int launch_tail_half(const float* dout, int64_t dout_stride, const float* w_heads, const float* hidden, int64_t m, int h,
+                     float* dpre, float* workspace, int blocks, cudaStream_t s) {
+    const dim3 grid((unsigned)blocks, (unsigned)(h / HS_W));
+    if (dout_stride == HS_NO) {
+        const size_t smem = (size_t)TT_STAGES * TT_CHUNK * (HS_W + HS_NO) * 4;
+        PB_CUDA(cudaFuncSetAttribute(k_mlp_tail_bwd_tma_half, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_mlp_tail_bwd_tma_half<<<grid, MT_THREADS, smem, s>>>(dout, w_heads, hidden, dpre, workspace, m, h);
+    } else {
+        k_mlp_tail_bwd_half<<<grid, MT_THREADS, 0, s>>>(dout, dout_stride, w_heads, hidden, dpre, workspace, m, h);
+    }
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
+
 }  // namespace
 
 extern "C" size_t pb_mlp_tail_workspace_bytes_ex(int64_t m, int32_t hidden, int32_t head_rows) {
-    if (m <= 0 || hidden <= 0 || (head_rows != 8 && head_rows != 16)) return 16;
+    if (m <= 0 || hidden <= 0 || (head_rows != 8 && head_rows != 16 && head_rows != 32)) return 16;
     const int64_t blocks = pb_ceil_div(m, ROWS_PER_BLOCK);
     return (size_t)blocks * (size_t)(head_rows * hidden + hidden + head_rows) * sizeof(float);
 }
@@ -491,8 +663,8 @@ extern "C" int pb_mlp_tail_backward_ex(const float* dout, int64_t dout_stride, c
     PB_REQUIRE(m >= 1, PB_ERR_INVALID, "pb_mlp_tail_backward: m must be positive");
     PB_REQUIRE(hidden_size >= 128 && hidden_size <= 512 && hidden_size % 128 == 0, PB_ERR_UNSUPPORTED,
                "pb_mlp_tail_backward: hidden size %d (128, 256, 384 and 512 are built)", hidden_size);
-    PB_REQUIRE(head_rows == 8 || head_rows == 16, PB_ERR_UNSUPPORTED,
-               "pb_mlp_tail_backward: head_rows %d (8 and 16 are built)", head_rows);
+    PB_REQUIRE(head_rows == 8 || head_rows == 16 || head_rows == 32, PB_ERR_UNSUPPORTED,
+               "pb_mlp_tail_backward: head_rows %d (8, 16 and 32 are built)", head_rows);
     PB_REQUIRE(dout && w_heads && hidden && dpre && grads_out && workspace, PB_ERR_INVALID,
                "pb_mlp_tail_backward: null pointer");
     PB_REQUIRE(dout_stride >= head_rows && dout_stride % 4 == 0 && ((uintptr_t)dout & 15) == 0 &&
@@ -506,7 +678,8 @@ extern "C" int pb_mlp_tail_backward_ex(const float* dout, int64_t dout_stride, c
     cudaStream_t s = (cudaStream_t)stream;
     float* ws = (float*)workspace;
     const int rc =
-        hidden_size == 128
+        head_rows == HS_NO ? launch_tail_half(dout, dout_stride, w_heads, hidden, m, hidden_size, dpre, ws, blocks, s)
+        : hidden_size == 128
             ? (head_rows == 8 ? launch_tail<8>(dout, dout_stride, w_heads, hidden, m, dpre, ws, blocks, s)
                               : launch_tail<16>(dout, dout_stride, w_heads, hidden, m, dpre, ws, blocks, s))
             : (head_rows == 8 ? launch_tail_slices<8>(dout, dout_stride, w_heads, hidden, m, hidden_size, dpre, ws, blocks, s)

@@ -8,7 +8,7 @@
 // bias corrections of torch.optim.Adam(capturable=True): step counters, moments and parameters are the optimizer's
 // own state tensors, updated in place, so state_dict() and a later fall-back to optimizer.step() stay valid.
 //
-// pb_pack_heads builds the 8- or 16-row head matrix (n_act logit rows | value row | zero pad) that the fused forward, the
+// pb_pack_heads builds the 8-, 16- or 32-row head matrix (n_act logit rows | value row | zero pad) that the fused forward, the
 // rollout-time policy kernel and pb_mlp_tail_backward consume, plus the TF32-rounded encoder weight, in one launch
 // (the ATen formulation is 2 fills + 4 strided copies + 3 elementwise kernels per optimizer step).
 #include "pb_common.cuh"
@@ -213,7 +213,7 @@ __global__ void __launch_bounds__(CAP_THREADS) k_clip_adam_parts(AdamArgs a, con
     }
 }
 
-// R = 8 head rows for n_act <= 7, 16 for 8 <= n_act <= 15 (models.Default.head_matrix)
+// R = 8 head rows for n_act <= 7, 16 for 8 <= n_act <= 15, 32 for 16 <= n_act <= 31 (models.Default.head_matrix)
 template <int R>
 __global__ void __launch_bounds__(256) k_pack_heads(const float* __restrict__ w_dec, const float* __restrict__ b_dec,
                                                     const float* __restrict__ w_val, const float* __restrict__ b_val,
@@ -379,9 +379,9 @@ extern "C" int pb_pack_heads(const float* w_dec, const float* b_dec, const float
                              int32_t n_act, int32_t hidden_size, float* w_cat, float* b_cat, const float* w_enc,
                              float* w_enc_tf32, int64_t enc_numel, void* stream) {
     PB_REQUIRE(w_dec && b_dec && w_val && b_val && w_cat && b_cat, PB_ERR_INVALID, "pb_pack_heads: null pointer");
-    PB_REQUIRE(n_act >= 1 && n_act <= 15 && hidden_size >= 1, PB_ERR_INVALID, "pb_pack_heads: n_act in [1,15], hidden >= 1");
+    PB_REQUIRE(n_act >= 1 && n_act <= 31 && hidden_size >= 1, PB_ERR_INVALID, "pb_pack_heads: n_act in [1,31], hidden >= 1");
     PB_REQUIRE(!w_enc_tf32 || (w_enc && enc_numel >= 1), PB_ERR_INVALID, "pb_pack_heads: w_enc_tf32 needs w_enc");
-    const int rows = n_act + 1 <= 8 ? 8 : 16;
+    const int rows = n_act + 1 <= 8 ? 8 : (n_act + 1 <= 16 ? 16 : 32);
     const int64_t work = w_enc_tf32 ? (enc_numel > rows * (int64_t)hidden_size ? enc_numel : rows * (int64_t)hidden_size)
                                     : rows * (int64_t)hidden_size;
     int64_t blocks = pb_ceil_div(work, 256);
@@ -389,8 +389,11 @@ extern "C" int pb_pack_heads(const float* w_dec, const float* b_dec, const float
     if (rows == 8)
         k_pack_heads<8><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w_dec, b_dec, w_val, b_val, n_act, hidden_size,
                                                                             w_cat, b_cat, w_enc, w_enc_tf32, enc_numel);
-    else
+    else if (rows == 16)
         k_pack_heads<16><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w_dec, b_dec, w_val, b_val, n_act, hidden_size,
+                                                                             w_cat, b_cat, w_enc, w_enc_tf32, enc_numel);
+    else
+        k_pack_heads<32><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w_dec, b_dec, w_val, b_val, n_act, hidden_size,
                                                                              w_cat, b_cat, w_enc, w_enc_tf32, enc_numel);
     PB_LAUNCH_CHECK();
     return PB_OK;

@@ -9,9 +9,9 @@
 //     (cp.async.bulk, one per row, two mbarriers);
 //   * hidden = relu(X W^T + b) on the tensor cores (mma.sync m16n8k8 TF32, fp32 accumulate; a warp owns 16 rows x 128
 //     columns, accumulators stay in registers -- `hidden` is never written to memory);
-//   * the two heads (n_act logits + value, padded to NC = 8 columns for n_act <= 7, 16 for n_act <= 15) are a second
-//     mma whose A operand is the accumulator fragment itself (the k order of the second product is permuted to match the
-//     C-fragment layout); NC = 16 is two n8 blocks on the same A fragments;
+//   * the two heads (n_act logits + value, padded to NC = 8 columns for n_act <= 7, 16 for n_act <= 15, 32 for
+//     n_act <= 31) are a second mma whose A operand is the accumulator fragment itself (the k order of the second product
+//     is permuted to match the C-fragment layout); NC = 16 and 32 are two and four n8 blocks on the same A fragments;
 //   * a quad shuffle gathers each row's NC outputs, one lane per row does logsumexp / inverse-CDF sampling / logprob /
 //     entropy and writes action, logprob, value straight into the rollout rows.
 // Tensor-core path note: this is a 128x128x128 tile per CTA, far below the size where a wgmma pipeline pays; the large
@@ -36,16 +36,19 @@ struct PolicyParams {
 };
 
 // 64 rows per CTA, one warp per 16 rows: 128 threads, 104 KB shared (+ 4 KB more head rows at NC = 16) -> 2 CTAs per
-// SM, 256 CTAs at 16384 rows
+// SM, 256 CTAs at 16384 rows.  NC = 32: a static [32][128] head copy (16 KB) would leave room for one CTA per SM only, so
+// the head rows are read into registers (8 float4 per thread) before the hidden product and written over sW once every
+// warp is done with W_enc: the shared memory, and the two CTAs per SM, stay those of NC = 16.
 constexpr int PM_ROWS = 64;
 constexpr int PM_THREADS = 2 * PM_ROWS;
 
 template <int NC>
 __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p) {
+    constexpr bool HEADS_IN_SW = NC > 16;
     extern __shared__ __align__(128) float smem[];
     float* sX = smem;                              // [64][136]
     float* sW = smem + PM_ROWS * PM_PITCH;         // [128][136]  (row = hidden unit, col = input feature)
-    __shared__ float sWh[NC][PM_H];
+    __shared__ float sWh[HEADS_IN_SW ? 1 : NC][PM_H];
     __shared__ float sBe[PM_H];
     __shared__ float sBh[NC];
     __shared__ __align__(8) uint64_t bars[2];      // [0]: obs tile + W rows 0..63, [1]: W rows 64..127
@@ -68,7 +71,14 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
 #pragma unroll 8
         for (int q = 0; q < PM_K / 4; ++q) *reinterpret_cast<float4*>(sX + tid * PM_PITCH + 4 * q) = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    for (int i = tid; i < NC * PM_H; i += PM_THREADS) sWh[i >> 7][i & 127] = p.w_heads[i];
+    float4 wh[HEADS_IN_SW ? NC * PM_H / 4 / PM_THREADS : 1];   // NC = 32: float4 i = tid + 128 j of w_heads
+    if constexpr (HEADS_IN_SW) {
+#pragma unroll
+        for (int j = 0; j < NC * PM_H / 4 / PM_THREADS; ++j)
+            wh[j] = *reinterpret_cast<const float4*>(p.w_heads + 4 * (tid + PM_THREADS * j));
+    } else {
+        for (int i = tid; i < NC * PM_H; i += PM_THREADS) sWh[i >> 7][i & 127] = p.w_heads[i];
+    }
     if (tid < PM_H) sBe[tid] = p.b_enc[tid];
     if (tid < NC) sBh[tid] = p.b_heads[tid];
     __syncthreads();
@@ -100,6 +110,15 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
             }
         }
     }
+    if constexpr (HEADS_IN_SW) {   // every warp is done with W_enc: head row r -> sW row r (same 136-float pitch)
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < NC * PM_H / 4 / PM_THREADS; ++j) {
+            const int i = tid + PM_THREADS * j;
+            *reinterpret_cast<float4*>(sW + (i >> 5) * PM_PITCH + 4 * (i & 31)) = wh[j];
+        }
+        __syncthreads();
+    }
     // ---- bias + ReLU on the accumulators; heads = hidden @ Wh^T as a second mma with A = the C fragments:
     //      C fragment of n-tile nt holds columns 8nt + {2t, 2t+1} of rows {g, g+8}; use them as k slots {t, t+4};
     //      head block q8 (columns 8q8..8q8+7) takes B from head rows 8q8 + g
@@ -116,8 +135,14 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
         a[2] = to_tf32(fmaxf(acc[nt][1] + b1, 0.f));      // (g,   col c0+1) -> k slot t+4
         a[3] = to_tf32(fmaxf(acc[nt][3] + b1, 0.f));      // (g+8, col c0+1) -> k slot t+4
 #pragma unroll
-        for (int q8 = 0; q8 < NC / 8; ++q8)   // B[k slot][n = g]
-            mma_tf32(out[q8], a, to_tf32(sWh[8 * q8 + g][c0]), to_tf32(sWh[8 * q8 + g][c0 + 1]));
+        for (int q8 = 0; q8 < NC / 8; ++q8) {   // B[k slot][n = g]
+            if constexpr (HEADS_IN_SW) {
+                const float2 hw = *reinterpret_cast<const float2*>(sW + (8 * q8 + g) * PM_PITCH + c0);
+                mma_tf32(out[q8], a, to_tf32(hw.x), to_tf32(hw.y));
+            } else {
+                mma_tf32(out[q8], a, to_tf32(sWh[8 * q8 + g][c0]), to_tf32(sWh[8 * q8 + g][c0 + 1]));
+            }
+        }
     }
     // out[q8]: (row g, cols 8q8 + 2t, +1), (row g+8, same).  Gather the NC columns of a row across its quad.
     float rowv[2][NC];
@@ -169,14 +194,19 @@ __global__ void __launch_bounds__(PM_THREADS) k_policy_mlp_sample(PolicyParams p
 //      chunk's share of the NC head columns into the same head accumulators (second mma).  The head bias is added once,
 //      after the last chunk.  Shared memory: x tile 34 KB + ring 136 KB + heads / encoder bias up to 34 KB -> one
 //      128-thread CTA per SM.
+//      NC = 32: the whole [32][512] head matrix (64 KB) does not fit beside the ring, so each ring stage also carries
+//      the chunk's 128 columns of the 32 head rows (one more 512-byte bulk copy per head row, 17 KB per stage): 204 KB
+//      of dynamic shared memory.  A stage is then refilled after the chunk's head product, not before it.
 constexpr int PW_HMAX = 512;
 
 template <int NC>
 __global__ void __launch_bounds__(PM_THREADS, 1) k_policy_mlp_sample_wide(PolicyParams p, int hid) {
+    constexpr bool RING_HEADS = NC > 16;
+    constexpr int STAGE_ROWS = RING_HEADS ? 128 + NC : 128;   // W_enc rows of the chunk (| its head columns)
     extern __shared__ __align__(128) float smem[];
     float* sX = smem;                              // [64][136]
-    float* sW = smem + PM_ROWS * PM_PITCH;         // [2][128][136]: ring stage s holds chunk c with c % 2 == s
-    __shared__ float sWh[NC][PW_HMAX];
+    float* sW = smem + PM_ROWS * PM_PITCH;         // [2][STAGE_ROWS][136]: ring stage s holds chunk c with c % 2 == s
+    __shared__ float sWh[RING_HEADS ? 1 : NC][PW_HMAX];
     __shared__ float sBe[PW_HMAX];
     __shared__ float sBh[NC];
     __shared__ __align__(8) uint64_t bars[3];      // [0]: obs tile, [1 + s]: ring stage s
@@ -186,7 +216,7 @@ __global__ void __launch_bounds__(PM_THREADS, 1) k_policy_mlp_sample_wide(Policy
     const int64_t row0 = (int64_t)blockIdx.x * PM_ROWS;
     const int valid = (int)((p.m - row0) < PM_ROWS ? (p.m - row0) : PM_ROWS);
     const uint64_t offset = p.counter ? *p.counter : 0ull;
-    constexpr uint32_t CHUNK_BYTES = 128u * PM_K * 4u;
+    constexpr uint32_t CHUNK_BYTES = (uint32_t)STAGE_ROWS * PM_K * 4u;
 
     if (tid == 0) {
         for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
@@ -199,14 +229,19 @@ __global__ void __launch_bounds__(PM_THREADS, 1) k_policy_mlp_sample_wide(Policy
 #pragma unroll 8
         for (int q = 0; q < PM_K / 4; ++q) *reinterpret_cast<float4*>(sX + tid * PM_PITCH + 4 * q) = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    for (int i = tid; i < NC * hid; i += PM_THREADS) sWh[i / hid][i % hid] = p.w_heads[i];
+    if constexpr (!RING_HEADS)
+        for (int i = tid; i < NC * hid; i += PM_THREADS) sWh[i / hid][i % hid] = p.w_heads[i];
     for (int i = tid; i < hid; i += PM_THREADS) sBe[i] = p.b_enc[i];
     if (tid < NC) sBh[tid] = p.b_heads[tid];
     __syncthreads();
     if (tid < valid) tma_load_1d(sX + tid * PM_PITCH, p.obs + (row0 + tid) * p.obs_stride, PM_K * 4u, &bars[0]);
 #pragma unroll
-    for (int s = 0; s < 2; ++s)
-        tma_load_1d(sW + (s * 128 + tid) * PM_PITCH, p.w_enc + (int64_t)(128 * s + tid) * PM_K, PM_K * 4u, &bars[1 + s]);
+    for (int s = 0; s < 2; ++s) {
+        tma_load_1d(sW + (s * STAGE_ROWS + tid) * PM_PITCH, p.w_enc + (int64_t)(128 * s + tid) * PM_K, PM_K * 4u, &bars[1 + s]);
+        if (RING_HEADS && tid < NC)
+            tma_load_1d(sW + (s * STAGE_ROWS + 128 + tid) * PM_PITCH, p.w_heads + (int64_t)tid * hid + 128 * s, PM_H * 4u,
+                        &bars[1 + s]);
+    }
 
     float out[NC / 8][4];
 #pragma unroll
@@ -220,7 +255,7 @@ __global__ void __launch_bounds__(PM_THREADS, 1) k_policy_mlp_sample_wide(Policy
         float acc[16][4];
 #pragma unroll
         for (int nt = 0; nt < 16; ++nt) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }
-        const float* wbase = sW + (s * 128 + g) * PM_PITCH + 2 * t;
+        const float* wbase = sW + (s * STAGE_ROWS + g) * PM_PITCH + 2 * t;
 #pragma unroll 4
         for (int ks = 0; ks < 16; ++ks) {
             const float2 x0 = *reinterpret_cast<const float2*>(xa + 8 * ks);
@@ -234,11 +269,13 @@ __global__ void __launch_bounds__(PM_THREADS, 1) k_policy_mlp_sample_wide(Policy
         }
         // stage s is free once every warp has read it: refill it with chunk c + 2 (tid 0 arrives with the byte count
         // before the barrier, so the copies can only complete the phase after it)
-        if (c + 2 < n_chunks && tid == 0) mbar_expect_tx(&bars[1 + s], CHUNK_BYTES);
-        __syncthreads();
-        if (c + 2 < n_chunks)
-            tma_load_1d(sW + (s * 128 + tid) * PM_PITCH, p.w_enc + (int64_t)(128 * (c + 2) + tid) * PM_K, PM_K * 4u,
-                        &bars[1 + s]);
+        if constexpr (!RING_HEADS) {
+            if (c + 2 < n_chunks && tid == 0) mbar_expect_tx(&bars[1 + s], CHUNK_BYTES);
+            __syncthreads();
+            if (c + 2 < n_chunks)
+                tma_load_1d(sW + (s * 128 + tid) * PM_PITCH, p.w_enc + (int64_t)(128 * (c + 2) + tid) * PM_K, PM_K * 4u,
+                            &bars[1 + s]);
+        }
 #pragma unroll
         for (int nt = 0; nt < 16; ++nt) {
             const int c0 = 128 * c + 8 * nt + 2 * t;
@@ -249,8 +286,26 @@ __global__ void __launch_bounds__(PM_THREADS, 1) k_policy_mlp_sample_wide(Policy
             a[2] = to_tf32(fmaxf(acc[nt][1] + b1, 0.f));
             a[3] = to_tf32(fmaxf(acc[nt][3] + b1, 0.f));
 #pragma unroll
-            for (int q8 = 0; q8 < NC / 8; ++q8)
-                mma_tf32(out[q8], a, to_tf32(sWh[8 * q8 + g][c0]), to_tf32(sWh[8 * q8 + g][c0 + 1]));
+            for (int q8 = 0; q8 < NC / 8; ++q8) {
+                if constexpr (RING_HEADS) {   // the chunk's columns of head row 8 q8 + g, from the ring stage
+                    const float2 hw = *reinterpret_cast<const float2*>(
+                        sW + (s * STAGE_ROWS + 128 + 8 * q8 + g) * PM_PITCH + 8 * nt + 2 * t);
+                    mma_tf32(out[q8], a, to_tf32(hw.x), to_tf32(hw.y));
+                } else {
+                    mma_tf32(out[q8], a, to_tf32(sWh[8 * q8 + g][c0]), to_tf32(sWh[8 * q8 + g][c0 + 1]));
+                }
+            }
+        }
+        if constexpr (RING_HEADS) {   // stage s (W_enc rows and head columns) is free: refill it with chunk c + 2
+            if (c + 2 < n_chunks && tid == 0) mbar_expect_tx(&bars[1 + s], CHUNK_BYTES);
+            __syncthreads();
+            if (c + 2 < n_chunks) {
+                tma_load_1d(sW + (s * STAGE_ROWS + tid) * PM_PITCH, p.w_enc + (int64_t)(128 * (c + 2) + tid) * PM_K,
+                            PM_K * 4u, &bars[1 + s]);
+                if (tid < NC)
+                    tma_load_1d(sW + (s * STAGE_ROWS + 128 + tid) * PM_PITCH, p.w_heads + (int64_t)tid * hid + 128 * (c + 2),
+                                PM_H * 4u, &bars[1 + s]);
+            }
         }
     }
     float rowv[2][NC];
@@ -301,7 +356,7 @@ int launch(const PolicyParams& p, int hid, cudaStream_t stream) {
         PB_CUDA(cudaFuncSetAttribute(k_policy_mlp_sample<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         k_policy_mlp_sample<NC><<<grid, PM_THREADS, smem, stream>>>(p);
     } else {
-        const size_t smem = (size_t)(PM_ROWS + 2 * 128) * PM_PITCH * sizeof(float);
+        const size_t smem = (size_t)(PM_ROWS + 2 * (NC > 16 ? 128 + NC : 128)) * PM_PITCH * sizeof(float);
         PB_CUDA(cudaFuncSetAttribute(k_policy_mlp_sample_wide<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         k_policy_mlp_sample_wide<NC><<<grid, PM_THREADS, smem, stream>>>(p, hid);
     }
@@ -321,14 +376,17 @@ extern "C" int pb_policy_mlp_sample(const float* obs, int64_t obs_stride, const 
                PB_ERR_UNSUPPORTED,
                "pb_policy_mlp_sample: built for 128 input features and 128, 256, 384 or 512 hidden units (got %d, %d)",
                in_features, hidden_size);
-    PB_REQUIRE(n_act >= 1 && n_act <= 15, PB_ERR_UNSUPPORTED, "pb_policy_mlp_sample: n_act must be in [1, 15]");
+    PB_REQUIRE(n_act >= 1 && n_act <= 31, PB_ERR_UNSUPPORTED, "pb_policy_mlp_sample: n_act must be in [1, 31]");
     PB_REQUIRE(obs && w_enc && b_enc && w_heads && b_heads && actions && logprobs && values, PB_ERR_INVALID,
                "pb_policy_mlp_sample: null pointer");
     PB_REQUIRE(obs_stride >= PM_K && obs_stride % 4 == 0 && ((uintptr_t)obs & 15) == 0 && ((uintptr_t)w_enc & 15) == 0,
                PB_ERR_INVALID, "pb_policy_mlp_sample: obs / w_enc must be 16-byte aligned, stride a multiple of 4");
     PB_REQUIRE(!ticket_dev || counter_dev, PB_ERR_INVALID, "pb_policy_mlp_sample: ticket_dev needs counter_dev");
+    PB_REQUIRE(n_act + 1 <= 16 || ((uintptr_t)w_heads & 15) == 0, PB_ERR_INVALID,
+               "pb_policy_mlp_sample: w_heads must be 16-byte aligned for more than 15 actions");
     PolicyParams p{obs, obs_stride, w_enc, b_enc, w_heads, b_heads, m, n_act, seed, counter_dev, ticket_dev,
                    actions, logprobs, values, entropies};
-    // w_heads / b_heads: the head matrix of models.Default.head_matrix, 8 rows for n_act <= 7, else 16
-    return n_act + 1 <= 8 ? launch<8>(p, hidden_size, (cudaStream_t)stream) : launch<16>(p, hidden_size, (cudaStream_t)stream);
+    // w_heads / b_heads: the head matrix of models.Default.head_matrix, 8 rows for n_act <= 7, 16 for n_act <= 15, else 32
+    cudaStream_t s = (cudaStream_t)stream;
+    return n_act + 1 <= 8 ? launch<8>(p, hidden_size, s) : n_act + 1 <= 16 ? launch<16>(p, hidden_size, s) : launch<32>(p, hidden_size, s);
 }

@@ -38,7 +38,7 @@ struct PpoParams {
     int clip_vloss;
 };
 
-// PW = 0: separate logits / value / gradient buffers, any strides.  PW = 8 or 16: logits / value / grads all live in
+// PW = 0: separate logits / value / gradient buffers, any strides.  PW = 8, 16 or 32: logits / value / grads all live in
 // [m][PW] rows (n_act logits | value | zero pad): PW / 4 128-bit accesses per row, every row written whole
 template <int PW>
 __global__ void __launch_bounds__(PL_THREADS) k_ppo_loss(PpoParams p) {
@@ -183,8 +183,8 @@ extern "C" int pb_ppo_loss(const float* logits, int64_t logits_stride, const flo
     PpoParams p{logits, logits_stride, value, value_stride, actions, old_logprobs, advantages, returns, old_values,
                 grad_logits, grad_logits_stride, grad_value, grad_value_stride, stats8, m, n_act, clip_coef, vf_clip_coef,
                 vf_coef, ent_coef, clip_vloss};
-    // packed rows: logits, value, and both gradients share [m][W] buffers, W = 8 (n_act <= 7) or 16 (n_act <= 15), with
-    // the value at column n_act of the logits rows
+    // packed rows: logits, value, and both gradients share [m][W] buffers, W = 8 (n_act <= 7), 16 (n_act <= 15) or 32
+    // (n_act <= 31), with the value at column n_act of the logits rows
     auto packed = [&](int w) {
         return logits_stride == w && grad_logits_stride == w && n_act <= w - 1 && value == logits + n_act &&
                value_stride == w && grad_value == grad_logits + n_act && grad_value_stride == w &&
@@ -193,6 +193,7 @@ extern "C" int pb_ppo_loss(const float* logits, int64_t logits_stride, const flo
     const unsigned grid = (unsigned)pb_ceil_div(m, PL_THREADS);
     if (packed(8)) k_ppo_loss<8><<<grid, PL_THREADS, 0, s>>>(p);
     else if (packed(16)) k_ppo_loss<16><<<grid, PL_THREADS, 0, s>>>(p);
+    else if (packed(32)) k_ppo_loss<32><<<grid, PL_THREADS, 0, s>>>(p);
     else k_ppo_loss<0><<<grid, PL_THREADS, 0, s>>>(p);
     PB_LAUNCH_CHECK();
     return PB_OK;

@@ -64,7 +64,7 @@ class Policy(torch.nn.Module):
         return action, logprob, ent, value
 
     def _policy_step_fused(self, x, out=None):
-        """models.Default with 128 fp32 features / 128, 256, 384 or 512 hidden (models.FAST_HIDDEN) / <= 15 actions: the
+        """models.Default with 128 fp32 features / 128, 256, 384 or 512 hidden (models.FAST_HIDDEN) / <= 31 actions: the
         whole rollout-time policy step (encoder,
         ReLU, heads, sampling, row stores) as ONE kernel (pb_policy_mlp_sample).  Returns None if it does not apply."""
         model = self.policy
@@ -73,7 +73,7 @@ class Policy(torch.nn.Module):
             return None
         x2 = x.view(x.shape[0], -1)
         n_act, hid = model.decoder.weight.shape
-        if x2.shape[1] != 128 or hid not in models.FAST_HIDDEN or n_act > 15 or x2.stride(1) != 1 or x2.stride(0) % 4 != 0:
+        if x2.shape[1] != 128 or hid not in models.FAST_HIDDEN or n_act > 31 or x2.stride(1) != 1 or x2.stride(0) % 4 != 0:
             return None
         n, dev = x2.shape[0], x2.device
         if out is None:

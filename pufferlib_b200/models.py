@@ -16,7 +16,8 @@ class _DefaultMLPFunction(torch.autograd.Function):
 
     forward : hidden = relu(x @ W_enc^T + b_enc)  -- bias + ReLU fused into the cuBLASLt GEMM epilogue;
               out    = hidden @ W_cat^T + b_cat    -- both heads in ONE R-column GEMM (n_act logits, value, zero pad;
-                                                      R = 8 for n_act <= 7, 16 for n_act <= 15: Default.head_matrix).
+                                                      R = 8 for n_act <= 7, 16 for n_act <= 15, 32 for n_act <= 31:
+                                                      Default.head_matrix).
     backward: pb_mlp_tail_backward_ex reads `hidden` once and produces dPre (heads dX + ReLU backward), dW_heads,
               db_heads and db_enc; the dense dW_enc = dPre^T @ x stays on cuBLAS tensor cores.  x (the observations) has
               no grad.
@@ -194,7 +195,7 @@ class Default(nn.Module):
         self.encoder = nn.Linear(int(np.prod(env.single_observation_space.shape)), hidden_size)
         self.decoder = layer_init(nn.Linear(hidden_size, env.single_action_space.n), std=0.01)
         self.value_head = nn.Linear(hidden_size, 1)
-        self.fast_path = True     # fused forward epilogues + pb_mlp_tail_backward (CUDA, FAST_HIDDEN, <= 15 actions)
+        self.fast_path = True     # fused forward epilogues + pb_mlp_tail_backward (CUDA, FAST_HIDDEN, <= 31 actions)
         self._head_cache = {}
 
     def invalidate_cache(self):
@@ -203,16 +204,17 @@ class Default(nn.Module):
         self._head_cache.clear()
 
     def head_matrix(self, cache=None):
-        """(w_cat [R, H], b_cat [R]): n_act logit rows | value row | zero padding up to R = the next multiple of 8 rows
-        (8 for n_act <= 7, 16 for n_act <= 15).  Cached until invalidate_cache() when `cache` is true (default: under no_grad); built anew
-        otherwise, since fused optimizers do not bump tensor._version and the cache cannot see an optimizer step."""
+        """(w_cat [R, H], b_cat [R]): n_act logit rows | value row | zero padding up to R = 8 rows for n_act <= 7, 16 for
+        n_act <= 15, 32 for n_act <= 31 (the row counts the kernels are built for), the next multiple of 8 past that.
+        Cached until invalidate_cache() when `cache` is true (default: under no_grad); built anew otherwise, since fused
+        optimizers do not bump tensor._version and the cache cannot see an optimizer step."""
         if cache is None:
             cache = not torch.is_grad_enabled()
         key = (self.decoder.weight.data_ptr(), torch.cuda.is_current_stream_capturing())
         if cache and self._head_cache.get('key') == key:
             return self._head_cache['w'], self._head_cache['b']
         n_act, hid = self.decoder.weight.shape
-        rows = -(-(n_act + 1) // 8) * 8
+        rows = next((r for r in (8, 16, 32) if n_act + 1 <= r), -(-(n_act + 1) // 8) * 8)
         with torch.no_grad():
             w_cat = self.decoder.weight.new_zeros(rows, hid)
             w_cat[:n_act] = self.decoder.weight
@@ -238,12 +240,12 @@ class Default(nn.Module):
 
     def _fast_ok(self, x):
         n_act, hid = self.decoder.weight.shape
-        return self.fast_path and x.is_cuda and hid in FAST_HIDDEN and n_act + 1 <= 16 and not x.requires_grad
+        return self.fast_path and x.is_cuda and hid in FAST_HIDDEN and n_act + 1 <= 32 and not x.requires_grad
 
     def forward_packed(self, observations):
         """-> (out [M, R], n_act) with logits = out[:, :n_act], value = out[:, n_act] (zero padding after; R = 8 for
-        n_act <= 7, 16 for n_act <= 15), or None when the fast path does not apply.  Lets the fused PPO loss hand back
-        ONE [M, R] gradient."""
+        n_act <= 7, 16 for n_act <= 15, 32 for n_act <= 31), or None when the fast path does not apply.  Lets the fused
+        PPO loss hand back ONE [M, R] gradient."""
         x = observations.view(observations.shape[0], -1)
         if not self._fast_ok(x):
             return None

@@ -129,14 +129,14 @@ class _FusedPPOLoss(torch.autograd.Function):
             ctx.save_for_backward(grad_logits, grad_value)
             ctx.value_shape = value.shape
         stats = torch.empty(8, dtype=torch.float64, device=dev)
+        # the per-row arrays as contiguous tensors held until the launch: a copy made inside the call's argument list
+        # would go back to the caching allocator as soon as its address is taken, and the next copy could reuse it
+        rows = [t.reshape(-1).contiguous() for t in (actions, old_logprobs, adv, returns, old_values)]
         cp = C.c_void_p
         _native.check(_native.lib().pb_ppo_loss(
-            cp(l_ptr), l_stride, cp(v_ptr), v_stride,
-            _native.ptr(actions.reshape(-1).contiguous()), _native.ptr(old_logprobs.reshape(-1).contiguous()),
-            _native.ptr(adv.reshape(-1).contiguous()), _native.ptr(returns.reshape(-1).contiguous()),
-            _native.ptr(old_values.reshape(-1).contiguous()), m, n_act, C.c_float(clip_coef), int(bool(clip_vloss)),
-            C.c_float(vf_clip_coef), C.c_float(vf_coef), C.c_float(ent_coef), cp(gl_ptr), gl_stride, cp(gv_ptr),
-            gv_stride, _native.ptr(stats), _native.stream_ptr()))
+            cp(l_ptr), l_stride, cp(v_ptr), v_stride, *[_native.ptr(t) for t in rows], m, n_act, C.c_float(clip_coef),
+            int(bool(clip_vloss)), C.c_float(vf_clip_coef), C.c_float(vf_coef), C.c_float(ent_coef), cp(gl_ptr), gl_stride,
+            cp(gv_ptr), gv_stride, _native.ptr(stats), _native.stream_ptr()))
         means = stats[:6] / m
         means[1] *= 0.5                                  # v_loss = 0.5 * mean(max(...))
         loss = (means[0] - ent_coef * means[2] + vf_coef * means[1]).float()
@@ -150,6 +150,10 @@ class _FusedPPOLoss(torch.autograd.Function):
         grad_logits, grad_value = ctx.saved_tensors
         return (g_loss * grad_logits, (g_loss * grad_value).view(ctx.value_shape), None, None, None, None, None, None,
                 None)
+
+
+# the most actions pb_ppo_loss takes (csrc/ppo_loss.cu, PL_MAX_ACT); update_plan sends larger heads to the reference loss
+PPO_LOSS_MAX_ACTIONS = 32
 
 
 def _loss_cfg(config):
@@ -952,7 +956,8 @@ def update_plan(data):
         'model'      autograd through model(obs) + fused_ppo_loss (Convolutional; Default with fast_path=False)
         'bptt'       LSTMWrapper.forward_packed_seq (the fused BPTT kernels) + fused_ppo_loss_packed
         'cudnn'      the policy's recurrent forward (cuDNN LSTM) + the reference loss
-        'reference'  the policy's forward + the reference loss (fused_loss=False)
+        'reference'  the policy's forward + the reference loss (fused_loss=False, or more than PPO_LOSS_MAX_ACTIONS
+                     actions)
     form, the layout Experience.prepare builds: 'direct' (the fused kernel reads the arrival-order rollout tensors in
     place), 'slabs' (order-free loss: per-row tensors copied slab-major, obs a view), 'segments' (the BPTT kernels on bptt
     segment views of obs) or 'gathered' (the reference layout: b_obs and the b_* tensors).  capture: 'whole' (ONE graph),
@@ -988,7 +993,7 @@ def update_plan(data):
         engine = 'mlp_fused' if manual._fused_ok(x, config) else 'mlp_chain'
         form = 'gathered' if not zero_copy else \
             'direct' if engine == 'mlp_fused' and _native.lib().pb_gae_time_major_supported(n, h) else 'slabs'
-    elif data.fused_loss:
+    elif data.fused_loss and int(getattr(data.vecenv.single_action_space, 'n', 0)) <= PPO_LOSS_MAX_ACTIONS:
         default = hasattr(model, 'forward_packed_slabs')
         engine = 'packed' if default and model._fast_ok(exp.obs) else 'model'
         form = 'slabs' if zero_copy and default else 'gathered'

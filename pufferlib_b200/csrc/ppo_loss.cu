@@ -75,15 +75,24 @@ __global__ void __launch_bounds__(PL_THREADS) k_ppo_loss(PpoParams p) {
         const float lse = mx + logf(sum);
         int a = (int)p.actions[i];
         a = a < 0 ? 0 : (a >= p.n_act ? p.n_act - 1 : a);
-        float ent = 0.f, nl_a = 0.f;
+        // p_k = exp(z_k - lse) sums to T = 1 up to a few ulps for logits of ordinary size; when they share a large offset
+        // C, lse lies on the grid of ulp(C) and T misses 1 by up to ulp(C)/2, so past |T - 1| > 2^-20 the probabilities
+        // are divided by T (the rule of pb_sample_row; rows below it keep inv = 1 and the same bits).  -inf logits (masked
+        // actions) have p_k = 0 and enter the entropy as max(z_k - lse, -FLT_MAX), as cleanrl.entropy clamps them
+        float nl_a = 0.f, tot = 0.f;
 #pragma unroll
         for (int k = 0; k < PL_MAX_ACT; ++k)
             if (k < p.n_act) {
-                const float nl = z[k] - lse, pk = expf(nl);
-                ent -= pk * nl;
+                const float nl = z[k] - lse;
+                tot += expf(nl);
                 if (k == a) nl_a = nl;
                 z[k] = nl;   // keep the normalised logit
             }
+        const float inv = fabsf(tot - 1.f) > 0x1p-20f ? 1.f / tot : 1.f;
+        float ent = 0.f;
+#pragma unroll
+        for (int k = 0; k < PL_MAX_ACT; ++k)
+            if (k < p.n_act) ent -= expf(z[k]) * inv * fmaxf(z[k], -3.4028234663852886e38f);
         const float logratio = nl_a - p.old_logprobs[i];
         const float ratio = expf(logratio);
         const float adv = p.adv[i];
@@ -120,7 +129,8 @@ __global__ void __launch_bounds__(PL_THREADS) k_ppo_loss(PpoParams p) {
         }
         const float gv_out = 0.5f * p.vf_coef * g_v * inv_m;
         if (!PACKED) p.grad_value[i * p.gvstride] = gv_out;
-        // d loss / d logits_j = g_nlp * (delta_ja - p_j) + ent_coef/M * p_j * (nl_j + H)
+        // d loss / d logits_j = g_nlp * (delta_ja - p_j) + ent_coef/M * p_j * (nl_j + H); the entropy term is 0 where p_j = 0
+        // (0 * -inf would be NaN for a masked action; autograd gives exactly 0 there)
         const float g_ent = p.ent_coef * inv_m;
         float gro[PW ? PW : 4];
 #pragma unroll
@@ -128,8 +138,8 @@ __global__ void __launch_bounds__(PL_THREADS) k_ppo_loss(PpoParams p) {
 #pragma unroll
         for (int k = 0; k < PL_MAX_ACT; ++k)
             if (k < p.n_act) {
-                const float pk = expf(z[k]);
-                const float gk = g_nlp * ((k == a ? 1.f : 0.f) - pk) + g_ent * pk * (z[k] + ent);
+                const float pk = expf(z[k]) * inv;
+                const float gk = g_nlp * ((k == a ? 1.f : 0.f) - pk) + (pk > 0.f ? g_ent * pk * (z[k] + ent) : 0.f);
                 if (PACKED) { if (k < PW) gro[k] = gk; }
                 else p.grad_logits[i * p.glstride + k] = gk;
             }

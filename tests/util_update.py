@@ -155,7 +155,7 @@ def clip_offsets(n, dev):
 
 
 def case(slab_rows, n_slabs, slab_stride, n_act, seed, nm=None, returns=True, old_values=True, adv_norm=False, cfg=CFG,
-         ws=None, mb=None, x_tail=64):
+         ws=None, mb=None, x_tail=64, logit_offset=0.0):
     """One minibatch of `n_slabs` slabs of `slab_rows` rows whose x rows start `slab_stride` rows apart.
 
     nm (arrival-order rows, as Experience.minibatch 'direct'): the per-row arrays live in buffers of exactly n_slabs * nm
@@ -165,7 +165,8 @@ def case(slab_rows, n_slabs, slab_stride, n_act, seed, nm=None, returns=True, ol
     arrays end flush with their allocations, as the last minibatch of train()'s rollout does).  returns=False: the kernel
     forms raw advantages + old values; old_values=False (needs returns and clip_vloss = 0): no old values at all; adv_norm:
     the kernel normalises the advantages with device constants (mean, 1 / (std + 1e-8)).  ws: a workspace to reuse (else a
-    fresh NaN one)."""
+    fresh NaN one).  logit_offset: a constant C added to the logit rows of b_cat (C = 1e3: every logit near C, where the
+    log-sum-exp lies on the grid of ulp(C) and the unnormalised probabilities miss a sum of 1 by up to ulp(C)/2)."""
     assert (returns or old_values) and (old_values or not cfg[1])
     dev = torch.device('cuda')
     torch.manual_seed(seed)
@@ -189,6 +190,7 @@ def case(slab_rows, n_slabs, slab_stride, n_act, seed, nm=None, returns=True, ol
     w_cat[:n_act + 1] = torch.randn(n_act + 1, 128, device=dev) * 0.1
     b_cat = torch.zeros(8, device=dev)
     b_cat[:n_act + 1] = torch.randn(n_act + 1, device=dev) * 0.1
+    b_cat[:n_act] += logit_offset
     act = torch.randint(0, n_act, (m,), device=dev)
     # old log-probabilities and old values relative to the float64 policy: rows below, inside and above both clip ranges
     with torch.no_grad():
@@ -240,7 +242,8 @@ def case(slab_rows, n_slabs, slab_stride, n_act, seed, nm=None, returns=True, ol
     if ws is None:
         ws = workspace(dev)
     print(f'case slab_rows={slab_rows} n_slabs={n_slabs} stride={slab_stride} n_act={n_act} (M={m}) '
-          f'nm={nm} mb={mb} x_tail={x_tail} returns={returns} old_values={old_values} adv_norm={adv_norm} cfg={cfg}', flush=True)
+          f'nm={nm} mb={mb} x_tail={x_tail} logit_offset={logit_offset} returns={returns} old_values={old_values} '
+          f'adv_norm={adv_norm} cfg={cfg}', flush=True)
 
     def launch(debug, dpre_out=None, gflat=None):
         return fused(xv, 128, slab_rows, slab_stride, n_slabs, w_enc, b_enc, w_cat, b_cat, k_act, k_olp, k_adv, k_ret, k_oval,

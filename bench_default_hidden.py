@@ -132,7 +132,7 @@ def tail_section(args, m=524288, rows=8):
     t = alternate({'tail': lambda: _native.check(lib.pb_mlp_tail_backward_ex(*a))}, args.kernel_reps)['tail']
     bytes_per_row = 2 * 4 * hid + 4 * rows * (hid // 128)
     bw = bytes_per_row * m / t
-    return dict(rows=m, hidden=hid, head_rows=rows, kernel='k_mlp_tail_bwd_tma_slices + k_reduce_partials',
+    return dict(rows=m, hidden=hid, head_rows=rows, kernel='k_mlp_tail_bwd<8, TMA> + k_reduce_partials',
                 bytes_per_row=bytes_per_row, us=t * 1e6, tb_per_s=bw / 1e12, share_of_hbm_peak=bw / HBM_PEAK,
                 launches_per_window=args.kernel_reps, windows=5, statistic='median')
 

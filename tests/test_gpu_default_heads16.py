@@ -13,6 +13,7 @@ from pufferlib_b200 import _native, clean_pufferl, models
 from pufferlib_b200.environments import ocean
 from pufferlib_b200.frameworks import cleanrl
 from test_gpu_experience import make_config
+from test_gpu_mlp_tail import check_tail, tail, tail_inputs
 from test_gpu_policy_lstm import fake_env
 from test_gpu_ppo_loss import reference_loss
 
@@ -60,47 +61,6 @@ def test_ppo_loss_packed_rows_16(m, n_act, clip_vloss):
     assert torch.equal(grad, a.grad)
 
 
-def _tail_inputs(m, n_act, rows, seed):
-    torch.manual_seed(seed)
-    hidden = torch.relu(torch.randn(m, 128, device=DEV))
-    dout = torch.randn(m, rows, device=DEV) / max(m, 1) ** 0.5
-    dout[:, n_act + 1:] = 0
-    w = torch.randn(rows, 128, device=DEV)
-    w[n_act + 1:] = 0
-    return hidden, dout, w
-
-
-def _tail(dout, w, hidden, rows, legacy=False, ws=None):
-    m = hidden.shape[0]
-    lib = _native.lib()
-    dpre = torch.full_like(hidden, float('nan'))
-    grads = torch.full((rows * 128 + 128 + rows,), float('nan'), device=DEV)
-    if legacy:
-        ws = torch.empty(lib.pb_mlp_tail_workspace_bytes(m, 128), dtype=torch.uint8, device=DEV)
-        _native.check(lib.pb_mlp_tail_backward(_native.ptr(dout), dout.stride(0), _native.ptr(w), _native.ptr(hidden), m,
-                                               128, _native.ptr(dpre), _native.ptr(grads), _native.ptr(ws), ws.numel(),
-                                               _native.stream_ptr()))
-    else:
-        if ws is None:
-            ws = torch.empty(lib.pb_mlp_tail_workspace_bytes_ex(m, 128, rows), dtype=torch.uint8, device=DEV)
-        _native.check(lib.pb_mlp_tail_backward_ex(_native.ptr(dout), dout.stride(0), _native.ptr(w), _native.ptr(hidden),
-                                                  m, 128, _native.ptr(dpre), _native.ptr(grads), _native.ptr(ws),
-                                                  ws.numel(), rows, _native.stream_ptr()))
-    return dpre, grads
-
-
-def _check_tail(dpre, grads, hidden, dout, w, rows, n_act):
-    h64, d64, w64 = hidden.double(), dout.double(), w.double()
-    ref_dpre = (d64 @ w64) * (h64 > 0)
-    refs = {'dpre': (dpre, ref_dpre), 'dW_heads': (grads[:rows * 128].view(rows, 128), d64.t() @ h64),
-            'db_enc': (grads[rows * 128:(rows + 1) * 128], ref_dpre.sum(0)), 'db_heads': (grads[(rows + 1) * 128:], d64.sum(0))}
-    for name, (got, ref) in refs.items():
-        err = float((got.double() - ref).abs().max())      # NaN (a row or an entry never written) fails too
-        assert err <= 1e-5 * float(ref.abs().max()) + 1e-30, (name, err, float(ref.abs().max()))
-    assert float(grads[:rows * 128].view(rows, 128)[n_act + 1:].abs().sum()) == 0.0
-    assert float(grads[(rows + 1) * 128:][n_act + 1:].abs().sum()) == 0.0
-
-
 TAIL_HEADS = [(8, 1), (8, 4), (8, 7), (16, 8), (16, 15)]
 
 
@@ -113,13 +73,9 @@ def test_mlp_tail_backward_matches_fp64(m, head_rows, n_act, strided):
     take the generic kernel, contiguous [M, head_rows] rows the TMA-staged one.  M runs over the edges of its 32-row TMA
     chunks and 512-row CTAs; dPre and the gradients start as NaN, so a row the kernel skips fails.  The padding rows of
     dW_heads and db_heads are exactly 0."""
-    hidden, dout, w = _tail_inputs(m, n_act, head_rows, m + n_act)
-    if strided:
-        wide = torch.zeros(m, head_rows + 4, device=DEV)
-        wide[:, :head_rows] = dout
-        dout = wide[:, :head_rows]
-    dpre, grads = _tail(dout, w, hidden, head_rows)
-    _check_tail(dpre, grads, hidden, dout, w, head_rows, n_act)
+    hidden, dout, w = tail_inputs(m, 128, n_act, head_rows, m + n_act, strided)
+    dpre, grads = tail(dout, w, hidden, head_rows)
+    check_tail(dpre, grads, hidden, dout, w, head_rows, n_act)
 
 
 @pytest.mark.parametrize('head_rows,n_act', [(8, 5), (16, 11)])
@@ -131,25 +87,17 @@ def test_mlp_tail_backward_small_launch_on_a_large_workspace(head_rows, n_act, s
     big, small = 524288 + 17, 513
     ws = torch.empty(lib.pb_mlp_tail_workspace_bytes_ex(big, 128, head_rows), dtype=torch.uint8, device=DEV)
     for m in (big, small):
-        hidden, dout, w = _tail_inputs(m, n_act, head_rows, m)
-        if strided:
-            wide = torch.zeros(m, head_rows + 4, device=DEV)
-            wide[:, :head_rows] = dout
-            dout = wide[:, :head_rows]
-        dpre, grads = _tail(dout, w, hidden, head_rows, ws=ws)
-    _check_tail(dpre, grads, hidden, dout, w, head_rows, n_act)
+        hidden, dout, w = tail_inputs(m, 128, n_act, head_rows, m, strided)
+        dpre, grads = tail(dout, w, hidden, head_rows, ws=ws)
+    check_tail(dpre, grads, hidden, dout, w, head_rows, n_act)
 
 
 @pytest.mark.parametrize('m', [37, 524288 + 17])
 @pytest.mark.parametrize('strided', [False, True])
 def test_mlp_tail_backward_ex_8_rows_is_the_existing_entry_point(m, strided):
-    hidden, dout, w = _tail_inputs(m, 5, 8, 3)
-    if strided:
-        wide = torch.zeros(m, 12, device=DEV)
-        wide[:, :8] = dout
-        dout = wide[:, :8]
-    a = _tail(dout, w, hidden, 8)
-    b = _tail(dout, w, hidden, 8, legacy=True)
+    hidden, dout, w = tail_inputs(m, 128, 5, 8, 3, strided)
+    a = tail(dout, w, hidden, 8)
+    b = tail(dout, w, hidden, 8, legacy=True)
     assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1])
 
 

@@ -1,6 +1,6 @@
 """models.Default with 16 to 31 actions on the hand-written kernels: the 32-row padded head matrix (n_act logit rows |
-value row | zero rows, models.Default.head_matrix) through pb_ppo_loss's packed rows, pb_mlp_tail_backward_ex's
-half-width kernels, pb_pack_heads, pb_policy_mlp_sample's four n8 head blocks and the _DefaultMLPUpdate chain of train().
+value row | zero rows, models.Default.head_matrix) through pb_ppo_loss's packed rows, pb_mlp_tail_backward_ex,
+pb_pack_heads, pb_policy_mlp_sample's four n8 head blocks and the _DefaultMLPUpdate chain of train().
 More than 31 actions keeps the plain modules; LSTMWrapper(Default) with more than 15 actions keeps the cuDNN path."""
 import copy
 import ctypes as C
@@ -16,8 +16,9 @@ from pufferlib_b200 import _native, clean_pufferl, models
 from pufferlib_b200.environments import ocean
 from pufferlib_b200.frameworks import cleanrl
 from test_gpu_default_heads16 import _loss_inputs
-from test_gpu_default_hidden import check_tail, make_default, policy_step_abi, tail, tail_inputs
+from test_gpu_default_hidden import make_default, policy_step_abi
 from test_gpu_experience import make_config
+from test_gpu_mlp_tail import check_tail, tail, tail_inputs
 from test_gpu_peer_staged import Engine, TorchAdam, assert_same_bits, default_parameters, round4, step_gradients
 from test_gpu_policy_lstm import fake_env
 from test_gpu_ppo_loss import reference_loss
@@ -65,7 +66,7 @@ def test_ppo_loss_packed_rows_32(m, n_act, clip_vloss):
 # tail backward
 
 @pytest.mark.parametrize('m', [1, 31, 32, 33, 511, 512, 513, 4096, 524288 + 17])
-@pytest.mark.parametrize('hid', [128, 256, 512])
+@pytest.mark.parametrize('hid', [128, 256, 384, 512])
 @pytest.mark.parametrize('strided', [False, True])
 def test_mlp_tail_32_rows_matches_fp64(m, hid, strided):
     """pb_mlp_tail_backward_ex(head_rows=32) vs fp64 torch: dPre, dW_heads, db_enc, db_heads within 1e-5 of each output's
@@ -78,7 +79,7 @@ def test_mlp_tail_32_rows_matches_fp64(m, hid, strided):
     check_tail(dpre, grads, hidden, dout, w, 32, n_act)
 
 
-@pytest.mark.parametrize('hid', [128, 256, 512])
+@pytest.mark.parametrize('hid', [128, 256, 384, 512])
 @pytest.mark.parametrize('strided', [False, True])
 def test_mlp_tail_32_rows_small_launch_on_a_large_workspace(hid, strided):
     """513 rows on the workspace a 524 305-row launch just filled: the reduction reads only the small launch's

@@ -13,6 +13,7 @@ from pufferlib_b200 import _native, clean_pufferl, models
 from pufferlib_b200.environments import ocean
 from pufferlib_b200.frameworks import cleanrl
 from test_gpu_experience import make_config
+from test_gpu_mlp_tail import check_tail, tail, tail_inputs
 from test_gpu_policy_lstm import fake_env
 from test_gpu_sampling import G, TIE, check_mlp_outputs, mlp_reference
 from util_gpu import restated_draw, softmax64, uniforms
@@ -140,60 +141,21 @@ def test_policy_mlp_wide_tf32_tie_in_second_chunk(n_act):
 # ---------------------------------------------------------------------------------------------------------------------
 # tail backward
 
-def tail_inputs(m, hid, n_act, rows, seed, strided):
-    torch.manual_seed(seed)
-    hidden = torch.relu(torch.randn(m, hid, device=DEV))
-    dout = torch.randn(m, rows, device=DEV) / max(m, 1) ** 0.5
-    dout[:, n_act + 1:] = 0
-    w = torch.randn(rows, hid, device=DEV)
-    w[n_act + 1:] = 0
-    if strided:            # rows head_rows + 4 floats apart: the generic kernel
-        wide = torch.zeros(m, rows + 4, device=DEV)
-        wide[:, :rows] = dout
-        dout = wide[:, :rows]
-    return hidden, dout, w
-
-
-def tail(dout, w, hidden, rows, ws=None):
-    m, hid = hidden.shape
-    lib = _native.lib()
-    dpre = torch.full_like(hidden, float('nan'))
-    grads = torch.full((rows * hid + hid + rows,), float('nan'), device=DEV)
-    if ws is None:
-        ws = torch.empty(lib.pb_mlp_tail_workspace_bytes_ex(m, hid, rows), dtype=torch.uint8, device=DEV)
-    _native.check(lib.pb_mlp_tail_backward_ex(P(dout), dout.stride(0), P(w), P(hidden), m, hid, P(dpre), P(grads), P(ws),
-                                              ws.numel(), rows, _native.stream_ptr()))
-    return dpre, grads
-
-
-def check_tail(dpre, grads, hidden, dout, w, rows, n_act):
-    hid = hidden.shape[1]
-    h64, d64, w64 = hidden.double(), dout.double(), w.double()
-    ref_dpre = (d64 @ w64) * (h64 > 0)
-    refs = {'dpre': (dpre, ref_dpre), 'dW_heads': (grads[:rows * hid].view(rows, hid), d64.t() @ h64),
-            'db_enc': (grads[rows * hid:(rows + 1) * hid], ref_dpre.sum(0)), 'db_heads': (grads[(rows + 1) * hid:], d64.sum(0))}
-    for name, (got, ref) in refs.items():
-        err = float((got.double() - ref).abs().max())      # NaN (an entry never written) fails too
-        assert err <= 1e-5 * float(ref.abs().max()) + 1e-30, (name, err, float(ref.abs().max()))
-    assert float(grads[:rows * hid].view(rows, hid)[n_act + 1:].abs().sum()) == 0.0
-    assert float(grads[(rows + 1) * hid:][n_act + 1:].abs().sum()) == 0.0
-
-
 @pytest.mark.parametrize('m', [1, 31, 32, 33, 511, 512, 513, 4096, 524288 + 17])
 @pytest.mark.parametrize('rows,n_act', [(8, 5), (16, 12)])
-@pytest.mark.parametrize('hid', [256, 512])
+@pytest.mark.parametrize('hid', WIDE)
 @pytest.mark.parametrize('strided', [False, True])
 def test_mlp_tail_slices_match_fp64(m, rows, n_act, hid, strided):
-    """pb_mlp_tail_backward_ex at H = 256 and 512 vs fp64 torch: dPre, dW_heads, db_enc, db_heads within 1e-5 of each
-    output's maximum; dPre and the gradients start as NaN, so an entry no slice writes fails; the padding rows of dW_heads
-    and db_heads are exactly 0.  M runs over the edges of the 32-row TMA chunks and the 512-row CTAs."""
+    """pb_mlp_tail_backward_ex at H = 256, 384 and 512 vs fp64 torch: dPre, dW_heads, db_enc, db_heads within 1e-5 of
+    each output's maximum; dPre and the gradients start as NaN, so an entry no slice writes fails; the padding rows of
+    dW_heads and db_heads are exactly 0.  M runs over the edges of the 32-row TMA chunks and the 512-row CTAs."""
     hidden, dout, w = tail_inputs(m, hid, n_act, rows, m + hid, strided)
     dpre, grads = tail(dout, w, hidden, rows)
     check_tail(dpre, grads, hidden, dout, w, rows, n_act)
 
 
 @pytest.mark.parametrize('rows,n_act', [(8, 5), (16, 11)])
-@pytest.mark.parametrize('hid', [256, 512])
+@pytest.mark.parametrize('hid', WIDE)
 @pytest.mark.parametrize('strided', [False, True])
 def test_mlp_tail_slices_small_launch_on_a_large_workspace(rows, n_act, hid, strided):
     """513 rows on the workspace a 524 305-row launch just filled: the reduction reads only the small launch's

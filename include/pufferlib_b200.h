@@ -525,6 +525,37 @@ int pb_pack_heads(const float* w_dec, const float* b_dec, const float* w_val, co
                   int32_t hidden_size, float* w_cat, float* b_cat, const float* w_enc, float* w_enc_tf32,
                   int64_t enc_numel, void* stream);
 
+/* -- PPO early stop (target_kl, clean_pufferl.py:256-258) on the device, and conditional graph nodes ----------------------
+ * pb_kl_stop (one thread) takes the last minibatch's approx_kl of epoch `epoch` from exactly one source: approx_kl, an fp32
+ * device scalar (stats[4] of fused_ppo_loss / the reference loss), or kl_sum / rows, an fp64 row sum and its row count
+ * (the approx_kl column of a pb_ppo_loss / pb_mlp_update_fused statistics row), rounded once to fp32 -- the value
+ * fused_ppo_loss returns for those rows.  stop = approx_kl > target_kl in fp32, as torch compares a 0-dim fp32 tensor with
+ * a Python float (target_kl: a device fp32 scalar holding that float rounded to fp32, so a captured graph reads the
+ * current value); a NaN approx_kl never stops.  state (device int32[2]):
+ * epoch 0 starts a new train() call; then state[0] = stop and state[1] = the epochs the call runs if no later decision
+ * stops it (epoch + 1 if stop, else epoch + 2).  With epoch > 0 and state[0] already set nothing changes (the flag stays
+ * set for the rest of the call).  use_handle != 0: also cudaGraphSetConditional(cond_handle, !stopped), from inside a
+ * graph launch; use_handle = 0 (eager): only state is written. */
+int pb_kl_stop(const float* approx_kl, const double* kl_sum, int64_t rows, const float* target_kl, int32_t epoch,
+               int32_t* state, uint64_t cond_handle, int32_t use_handle, void* stream);
+/* IF nodes in a stream capture.  pb_graph_cond_create: a conditional handle of the graph `stream` is capturing, set to
+ * default_value at every launch (cudaGraphCondAssignDefault).  A handle serves one IF node (CUDA allows one conditional
+ * node per handle) and must be created on the graph that holds that node: create the handles of IF nodes added on
+ * `stream` from `stream`, not from a body stream (a body stream captures the child graph of an IF node).  A chain of IF
+ * nodes with default 0 whose bodies each set the next node's handle runs up to the first body that does not.
+ * pb_graph_if_begin: an IF node on cond_handle after the
+ * capture's current dependencies; the capture of `stream` continues after it, and body_stream (a second stream, not
+ * capturing) starts capturing the node's body graph until pb_graph_if_end(body_stream).  Work enqueued on body_stream in
+ * between runs in a launch only while the handle is non-zero.  Without an active capture (PB_ERR_STATE) or with bad
+ * arguments (PB_ERR_INVALID) nothing is added and nothing is launched. */
+int pb_graph_cond_create(void* stream, uint32_t default_value, uint64_t* handle_out);
+int pb_graph_if_begin(uint64_t cond_handle, void* stream, void* body_stream);
+int pb_graph_if_end(void* body_stream);
+/* A non-blocking stream of the caller's own (cudaStreamCreateWithFlags), e.g. the body stream of the IF nodes: unlike
+ * torch's pooled streams it is never handed to another component. */
+int pb_stream_create(void** stream_out);
+int pb_stream_destroy(void* stream);
+
 /* -- structured observation pack / unpack (SURVEY §8 row a-4) --------------------------------------------------------
  * Replaces, for N samples at once, `emulate` / `nativize` (pufferlib/extensions.pyx:19-30, 32-49): leaf tensors
  * [N][nbytes[k]] <-> C-aligned records [N][record_bytes] whose layout is `np.dtype(..., align=True)` of the space

@@ -137,6 +137,13 @@ SIGNATURES = {
     'pb_peer_free': (C.c_int, [C.c_void_p]),
     'pb_peer_allreduce': (C.c_int, [C.POINTER(PeerComm), C.c_void_p, C.c_int64, C.c_void_p]),
     'pb_pack_heads': (C.c_int, [C.c_void_p] * 4 + [C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p]),
+    'pb_kl_stop': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_int32,
+                             C.c_void_p]),
+    'pb_graph_cond_create': (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64)]),
+    'pb_stream_create': (C.c_int, [C.POINTER(C.c_void_p)]),
+    'pb_stream_destroy': (C.c_int, [C.c_void_p]),
+    'pb_graph_if_begin': (C.c_int, [C.c_uint64, C.c_void_p, C.c_void_p]),
+    'pb_graph_if_end': (C.c_int, [C.c_void_p]),
     'pb_struct_pack': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
     'pb_struct_unpack': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
 }

@@ -3,6 +3,8 @@
     python -m pufferlib_b200.build [--force] [--verbose]
 
 The shared library has a plain C ABI (include/pufferlib_b200.h) and links only cudart: no torch, no pybind.
+cudaGraphSetConditional (csrc/graph_cond.cu) is a device-runtime builtin that needs neither relocatable device code nor
+cudadevrt, so cudart stays the only library linked.
 It is written next to this file, so the package imports from the source tree.
 """
 import glob

@@ -17,6 +17,7 @@ Mirrors reference clean_pufferl.py: ``create`` (:30-73), ``evaluate`` (:75-154),
 The policy stays a torch ``nn.Module`` with the reference's call convention
 (``policy(obs) -> actions, logprob, entropy, value``; ``policy(obs, action=a)`` in train).
 """
+import contextlib
 import ctypes as C
 import random
 import time
@@ -225,7 +226,8 @@ class _DefaultMLPUpdate:
             return False
         if not (hasattr(model, 'forward_packed_slabs') and getattr(model, 'fast_path', False)):
             return False
-        if config.target_kl is not None or not getattr(data, 'own_optimizer', False):
+        # several ranks with target_kl keep the autograd path (each rank would stop on its own approx_kl)
+        if (config.target_kl is not None and data.grad_bucket is not None) or not getattr(data, 'own_optimizer', False):
             return False
         n_act, hid = model.decoder.weight.shape
         if hid not in models.FAST_HIDDEN or n_act > 31 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
@@ -839,6 +841,7 @@ def create(config, vecenv, policy, optimizer=None, wandb=None):
         msg=msg, last_log_time=0, utilization=None, grad_bucket=grad_bucket,
         io=pufferlib_b200.namespace(h2d=0, d2h=0), graph_state=0, rollout_graph=None, graph_steps=0,
         graph_launches=0, graph_replays=0, train_graph_state=0, train_graph=None, train_result=None, train_graph_launches=0, train_graph_replays=0, train_segments=None, train_acc=None, own_optimizer=own_optimizer, manual_update=None, train_minibatch_path=None, train_recurrent_path=None,
+        train_epochs_run=None, train_kl_stop=None,
         fused_rows=bool(getattr(policy, 'fused_sample', False)) and hasattr(vecenv, 'bind_rollout'),
         # one-kernel PPO loss (pb_ppo_loss) where the update engine has one (update_plan): needs a wrapper exposing the
         # model as .policy, one Discrete head
@@ -1001,8 +1004,9 @@ def update_plan(data):
         engine, form = 'reference', 'gathered'
 
     capture = None
-    if bool(getattr(config, 'cuda_graph_train', getattr(config, 'cuda_graph', False))) and config.target_kl is None \
-            and data.train_graph_state >= 0:
+    # target_kl on one GPU: the stop is decided on the device and skips the later epochs through IF nodes (_KLStop)
+    if bool(getattr(config, 'cuda_graph_train', getattr(config, 'cuda_graph', False))) and \
+            (config.target_kl is None or data.grad_bucket is None) and data.train_graph_state >= 0:
         # an NCCL call inside the update loop (autograd path on several ranks, or the hand-written update without peer
         # memory) keeps the update out of ONE graph -- capturing it hung on this stack (torch 2.11 / NCCL 2.28) -- so it
         # is captured in segments around an ordinary all-reduce call; with the peer all-reduce fused into
@@ -1095,6 +1099,93 @@ def evaluate(data):
     return data.stats, infos
 
 
+class _KLStop:
+    """The early stop of clean_pufferl.py:256-258 (`if approx_kl > target_kl: break` after each epoch) decided on the
+    device by pb_kl_stop, so that eager and captured train() decide alike and the captured one stays ONE graph.  After
+    every epoch but the last, pb_kl_stop reads the last minibatch's approx_kl and writes state = (stopped, epochs run).
+    Eager, the host reads the flag (one sync per epoch, as the reference's .item()).  Captured, every epoch is the body of
+    an IF node with a conditional handle of its own (CUDA ties a handle to one node), all created on the root graph by
+    begin(): epoch 0's handle is 1 at every launch, the others 0 until the previous epoch's pb_kl_stop sets them, so after
+    a stop, or after a skipped body whose pb_kl_stop did not run, no later body runs.  Every epoch's work is captured on
+    one body stream (this object's own, never shared) that is torch's current stream meanwhile -- autograd included, so
+    no autograd node of one epoch belongs to another stream than the next -- with its allocations (cuBLAS workspace
+    included) in the train graph's pool."""
+
+    def __init__(self, device):
+        self.state = torch.zeros(2, dtype=torch.int32, device=device)   # stopped, epochs run
+        self.target = torch.zeros(1, device=device)     # fp32(target_kl), set by train() before it runs or replays
+        raw = C.c_void_p()
+        _native.check(_native.lib().pb_stream_create(C.byref(raw)))
+        self._raw_body = raw.value
+        self.body = torch.cuda.ExternalStream(raw.value, device=device)
+        self.pool = None            # memory pool of the train graph being captured (train() sets it)
+        self.main = None            # the capture stream (captures only)
+        self.handles = None         # handles[e]: conditional handle of epoch e's IF node (captures only)
+
+    def close(self):
+        if self._raw_body is not None:
+            torch.cuda.synchronize(self.state.device)
+            _native.check(_native.lib().pb_stream_destroy(C.c_void_p(self._raw_body)))
+            self._raw_body = self.body = None
+
+    def begin(self, epochs):
+        """At the top of train()'s device part.  A capture creates the handles of all its IF nodes here, on the root
+        graph that will hold them (a handle must belong to the graph of its node, not to the body graph in which the
+        pb_kl_stop that sets it is captured)."""
+        self.main, self.handles = None, None
+        if torch.cuda.is_current_stream_capturing():
+            self.main = torch.cuda.current_stream()
+            self.handles = []
+            for e in range(epochs):
+                h = C.c_uint64()
+                _native.check(_native.lib().pb_graph_cond_create(_native.stream_ptr(self.main), int(e == 0), C.byref(h)))
+                self.handles.append(h.value)
+
+    @property
+    def capturing(self):
+        return self.handles is not None
+
+    def decide(self, epoch, approx_kl=None, stats=None, row=0, rows=0):
+        """pb_kl_stop after `epoch` on an fp32 approx_kl tensor, or on row `row` of a [*, 8] fp64 statistics tensor;
+        captured, it sets the handle of epoch + 1's IF node."""
+        handle = self.handles[epoch + 1] if self.capturing else None
+        kl_sum = None if stats is None else C.c_void_p(stats.data_ptr() + 64 * row + 8 * 4)
+        if approx_kl is not None and approx_kl.dtype != torch.float32:
+            approx_kl = approx_kl.float()
+        _native.check(_native.lib().pb_kl_stop(
+            _native.ptr(approx_kl), kl_sum, rows, _native.ptr(self.target), epoch, _native.ptr(self.state),
+            handle or 0, int(handle is not None), _native.stream_ptr()))
+
+    def stopped(self):
+        return bool(self.state[0].item())
+
+    @contextlib.contextmanager
+    def if_body(self, epoch):
+        """Work inside runs in a graph launch only if epoch's handle is set (epoch 0: always; later epochs: if the
+        pb_kl_stop of the epoch before let them)."""
+        dev, lib = self.state.device.index, _native.lib()
+        assert torch.cuda.current_stream() == self.main and self.body != self.main
+        _native.check(lib.pb_graph_if_begin(self.handles[epoch], _native.stream_ptr(self.main),
+                                            _native.stream_ptr(self.body)))
+        # the caching allocator serves a pool to one filter at a time: hand the train graph's pool from the capture
+        # stream to the body stream and back (begin takes a pool reference, release gives it back).  The filter put
+        # back matches the capture stream only, where torch.cuda.graph's matched every stream of the capture: no torch
+        # side stream is forked into this capture after the first IF node (the captured part runs on these two streams)
+        torch._C._cuda_endAllocateToPool(dev, self.pool)
+        try:
+            with torch.cuda.stream(self.body):
+                torch._C._cuda_beginAllocateCurrentStreamToPool(dev, self.pool)
+                try:
+                    yield
+                finally:
+                    torch._C._cuda_endAllocateToPool(dev, self.pool)
+                    torch._C._cuda_releasePool(dev, self.pool)
+        finally:
+            torch._C._cuda_beginAllocateCurrentStreamToPool(dev, self.pool)
+            torch._C._cuda_releasePool(dev, self.pool)
+            _native.check(lib.pb_graph_if_end(_native.stream_ptr(self.body)))
+
+
 class _SegmentGraphs:
     """Per-segment CUDA graphs for the multi-GPU update loop: each (forward + loss + backward) minibatch segment and the
     (clip + Adam) segment is captured once and replayed; the NCCL all-reduce between them stays an ordinary call."""
@@ -1175,6 +1266,11 @@ def _train_device_part(data, plan, seg=None):
     if manual is not None:
         manual.pack_heads()                      # the parameters may have changed since the last train() (checkpoints)
     n_stats = config.update_epochs * n_mb
+    kl_stop = _kl_stop(data)
+    if kl_stop is not None:
+        kl_stop.begin(config.update_epochs)
+        if manual is not None and manual.stats is not None:
+            manual.stats.zero_()                 # rows of epochs that do not run must add nothing to loss_means
 
     def forward_backward(mb, k=0):              # k = epoch * n_mb + mb: the manual path's statistics row
         b = experience.minibatch(mb)
@@ -1222,7 +1318,9 @@ def _train_device_part(data, plan, seg=None):
 
         with profile.train_misc, torch.no_grad():
             acc.add_(st / n_mb)
-        carry['approx_kl'] = st[4]
+        # detached: the stop decision must not keep this minibatch's autograd graph (and the streams its nodes were
+        # created on) alive into the next epoch
+        carry['approx_kl'] = st[4].detach()
 
     def optimizer_step():
         with profile.learn:
@@ -1232,7 +1330,7 @@ def _train_device_part(data, plan, seg=None):
             torch.nn.utils.clip_grad_norm_(data.policy.parameters(), config.max_grad_norm)
             data.optimizer.step()
 
-    for epoch in range(config.update_epochs):
+    def run_epoch(epoch):
         carry['lstm_state'] = None
         for mb in range(n_mb):
             if seg is not None:       # the manual path writes its statistics to a per-(epoch, minibatch) row
@@ -1250,10 +1348,27 @@ def _train_device_part(data, plan, seg=None):
                 seg.run('opt', optimizer_step)
             else:
                 optimizer_step()
+        if kl_stop is not None and epoch < config.update_epochs - 1:
+            if manual is not None:
+                kl_stop.decide(epoch, stats=manual.stats, row=epoch * n_mb + n_mb - 1, rows=manual.mb_rows)
+            else:
+                kl_stop.decide(epoch, approx_kl=carry['approx_kl'])
 
-        if config.target_kl is not None:
-            if carry['approx_kl'].item() > config.target_kl:
-                break
+    for epoch in range(config.update_epochs):
+        if kl_stop is not None and kl_stop.capturing:
+            with kl_stop.if_body(epoch):
+                run_epoch(epoch)
+        elif kl_stop is None or epoch == 0:
+            run_epoch(epoch)
+        elif kl_stop.stopped():
+            break
+        else:
+            run_epoch(epoch)
+        data.train_epochs_run = epoch + 1
+        # several ranks: the reference's host-side check, each rank on its own approx_kl (one epoch: nothing to skip)
+        if kl_stop is None and config.target_kl is not None and data.grad_bucket is not None and \
+                carry['approx_kl'].item() > config.target_kl:
+            break
 
     with profile.train_misc:
         # explained variance on the device, same quantities as clean_pufferl.py:266-270
@@ -1262,20 +1377,37 @@ def _train_device_part(data, plan, seg=None):
         ev = 1 - (y_true - y_pred).var(unbiased=False) / var_y
         if manual is not None:
             acc = manual.loss_means(n_mb)
-        return torch.cat([acc, torch.stack([ev, var_y])])
+        out = [acc, torch.stack([ev, var_y])]
+        if kl_stop is not None:
+            out.append(kl_stop.state[1:].float())      # epochs run
+        return torch.cat(out)
+
+
+def _kl_stop(data):
+    """The device-side target_kl stop of this train() (_KLStop), or None: no target_kl, one epoch, or several ranks."""
+    config = data.config
+    if config.target_kl is None or config.update_epochs < 2 or data.grad_bucket is not None:
+        return None
+    if getattr(data, 'train_kl_stop', None) is None:
+        data.train_kl_stop = _KLStop(data.experience.device)
+    return data.train_kl_stop
 
 
 def train(data):
-    """One PPO update (reference: clean_pufferl.py:156-292).  With ``config.cuda_graph`` (no target_kl; recurrent
-    policies only on one GPU with the fused BPTT update) the device part is captured once -- after an eager first call
-    that initialises the optimizer state -- and replayed as ONE graph launch; the learning rate lives in a device tensor
-    so annealing works under replay."""
+    """One PPO update (reference: clean_pufferl.py:156-292).  With ``config.cuda_graph`` (recurrent policies only on one
+    GPU with the fused BPTT update; target_kl only on one GPU) the device part is captured once -- after an eager first
+    call that initialises the optimizer state -- and replayed as ONE graph launch; the learning rate lives in a device
+    tensor so annealing works under replay, and the target_kl stop is decided on the device (_KLStop).
+    data.train_epochs_run: the epochs this call ran."""
     config, profile, experience = data.config, data.profile, data.experience
     data.losses = make_losses()
     losses = data.losses
     with profile.train_misc:
         experience.sort_training_data()        # host-side bookkeeping only (clean_pufferl.py:452-464)
         plan = update_plan(data)
+        kl_stop = _kl_stop(data)
+        if kl_stop is not None:                # a device scalar, like the learning rate: replays read the current value
+            kl_stop.target.fill_(float(config.target_kl))
     if plan.capture == 'segments' and data.train_graph_state >= 1:
         if data.train_segments is None:
             data.train_segments = _SegmentGraphs()
@@ -1290,7 +1422,10 @@ def train(data):
                 torch.cuda.synchronize()
                 launches0 = _native.lib().pb_launch_count()
                 graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
+                pool = None
+                if kl_stop is not None:       # its IF bodies allocate from this graph's pool, so the id must be known
+                    pool = kl_stop.pool = torch.cuda.graph_pool_handle()
+                with torch.cuda.graph(graph, pool=pool):
                     data.train_result = _train_device_part(data, plan)
                 data.train_graph = graph
                 data.train_graph_launches = _native.lib().pb_launch_count() - launches0
@@ -1318,6 +1453,8 @@ def train(data):
         losses.policy_loss, losses.value_loss, losses.entropy = float(host[0]), float(host[1]), float(host[2])
         losses.old_approx_kl, losses.approx_kl, losses.clipfrac = float(host[3]), float(host[4]), float(host[5])
         losses.explained_variance = float('nan') if host[7] == 0 else float(host[6])
+        if host.size > 8:                      # device-side target_kl stop: the epochs it ran
+            data.train_epochs_run = int(host[8])
         data.epoch += 1
         profile.update(data)
         interval = getattr(config, 'checkpoint_interval', None)        # clean_pufferl.py:288-290
@@ -1366,6 +1503,8 @@ def try_load_checkpoint(data):
 
 
 def close(data):
+    if getattr(data, 'train_kl_stop', None) is not None:
+        data.train_kl_stop.close()
     mu = getattr(data, 'manual_update', None)
     if mu is not None and getattr(mu, 'peer', None) is not None:
         mu.peer.close()            # collective: every rank closes (unmaps the peers' buffers, then frees its own)

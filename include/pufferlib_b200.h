@@ -517,6 +517,22 @@ int pb_clip_adam_peer_parts(const pb_adam_tensor* tensors, int32_t n_tensors, fl
 int pb_clip_adam_peer(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm, float grad_scale, float lr,
                       const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
                       const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, void* stream);
+/* The same two exchanges carrying one fp64 payload per rank beside the gradient: the KL row sum for the PPO early stop
+ * agreed across ranks (pb_kl_stop with kl_sum = *kl_out, rows = world * rows per minibatch).  *kl_in is this rank's value;
+ * it travels in 4 reserved floats of the exchange slot right after the gradient, floats [round4(n), round4(n) + 4) with
+ * n = grad_flat_numel, as the 32-bit words (low half, high half, 0, 0), and *kl_out (device fp64) receives the payloads of
+ * all ranks added in rank order starting from 0.0, so every rank gets the same bits.  The payload is outside the
+ * gradient's sum of squares, the clip and Adam.  kl_in and kl_out are both null (then these are pb_clip_adam_peer /
+ * pb_clip_adam_peer_parts, which leave the payload floats untouched) or both 8-byte aligned device pointers; with them the
+ * communicator has 2 or more ranks and capacity >= round4(n) + 4.  Otherwise PB_ERR_INVALID and nothing is launched. */
+int pb_clip_adam_peer_ex(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm, float grad_scale, float lr,
+                         const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
+                         const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, const double* kl_in,
+                         double* kl_out, void* stream);
+int pb_clip_adam_peer_parts_ex(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm, float grad_scale,
+                               float lr, const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
+                               const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, double* sumsq_scratch,
+                               const pb_head_pack* pack, const double* kl_in, double* kl_out, void* stream);
 
 /* The 8-, 16- or 32-row padded head matrix of models.Default (pufferlib/models.py:33-38: decoder rows | value_head row |
  * zero padding; 8 rows for n_act <= 7, 16 for 8 <= n_act <= 15, 32 for 16 <= n_act <= 31), its bias, and (optionally) the encoder weight rounded to
@@ -529,7 +545,8 @@ int pb_pack_heads(const float* w_dec, const float* b_dec, const float* w_val, co
  * pb_kl_stop (one thread) takes the last minibatch's approx_kl of epoch `epoch` from exactly one source: approx_kl, an fp32
  * device scalar (stats[4] of fused_ppo_loss / the reference loss), or kl_sum / rows, an fp64 row sum and its row count
  * (the approx_kl column of a pb_ppo_loss / pb_mlp_update_fused statistics row), rounded once to fp32 -- the value
- * fused_ppo_loss returns for those rows.  stop = approx_kl > target_kl in fp32, as torch compares a 0-dim fp32 tensor with
+ * fused_ppo_loss returns for those rows.  Several ranks decide once for all: kl_sum is the ranks' row sums added (the
+ * kl_out of pb_clip_adam_peer_ex / _parts_ex, or an all-reduce) and rows = world * rows per minibatch.  stop = approx_kl > target_kl in fp32, as torch compares a 0-dim fp32 tensor with
  * a Python float (target_kl: a device fp32 scalar holding that float rounded to fp32, so a captured graph reads the
  * current value); a NaN approx_kl never stops.  state (device int32[2]):
  * epoch 0 starts a new train() call; then state[0] = stop and state[1] = the epochs the call runs if no later decision

@@ -126,6 +126,12 @@ SIGNATURES = {
     'pb_clip_adam_peer_parts': (C.c_int, [C.POINTER(AdamTensor), C.c_int32, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_float,
                                           C.c_float, C.c_float, C.c_void_p, C.POINTER(PeerComm), C.c_void_p, C.c_int64, C.c_void_p,
                                           C.POINTER(HeadPack), C.c_void_p]),
+    'pb_clip_adam_peer_ex': (C.c_int, [C.POINTER(AdamTensor), C.c_int32, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_float,
+                                       C.c_float, C.c_float, C.c_void_p, C.POINTER(PeerComm), C.c_void_p, C.c_int64,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
+    'pb_clip_adam_peer_parts_ex': (C.c_int, [C.POINTER(AdamTensor), C.c_int32, C.c_float, C.c_float, C.c_float, C.c_void_p,
+                                             C.c_float, C.c_float, C.c_float, C.c_void_p, C.POINTER(PeerComm), C.c_void_p,
+                                             C.c_int64, C.c_void_p, C.POINTER(HeadPack), C.c_void_p, C.c_void_p, C.c_void_p]),
     'pb_peer_allreduce_parts': (C.c_int, [C.POINTER(PeerComm), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     'pb_peer_slices': (C.c_int32, []),
     'pb_mlp_update_sumsq_offset': (C.c_size_t, []),

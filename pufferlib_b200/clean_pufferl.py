@@ -226,8 +226,7 @@ class _DefaultMLPUpdate:
             return False
         if not (hasattr(model, 'forward_packed_slabs') and getattr(model, 'fast_path', False)):
             return False
-        # several ranks with target_kl keep the autograd path (each rank would stop on its own approx_kl)
-        if (config.target_kl is not None and data.grad_bucket is not None) or not getattr(data, 'own_optimizer', False):
+        if not getattr(data, 'own_optimizer', False):
             return False
         n_act, hid = model.decoder.weight.shape
         if hid not in models.FAST_HIDDEN or n_act > 31 or model.encoder.weight.dtype != torch.float32 or not model.encoder.weight.is_cuda:
@@ -278,7 +277,9 @@ class _DefaultMLPUpdate:
         self.world = torch.distributed.get_world_size() if (torch.distributed.is_available() and
                                                             torch.distributed.is_initialized()) else 1
         # multi-GPU: the gradient sum is fused into pb_clip_adam_peer over NVLink peer memory (distributed.PeerComm); the
-        # NCCL all-reduce is only the fallback when peer mapping is unavailable (config.peer_allreduce=False, or IPC failed)
+        # NCCL all-reduce is only the fallback when peer mapping is unavailable (config.peer_allreduce=False, or IPC failed).
+        # The slot always has room for the 4-float KL payload after the gradient (pb_clip_adam_peer_ex): target_kl may be
+        # set on a later call
         self.peer = None
         self.peer_parts = None
         self.head_pack = None
@@ -286,7 +287,7 @@ class _DefaultMLPUpdate:
             from pufferlib_b200.distributed import PeerComm
             ok = torch.ones(1, device=dev)
             try:
-                self.peer = PeerComm(self.gflat.numel())
+                self.peer = PeerComm((self.gflat.numel() + 3) // 4 * 4 + 4)
             except Exception as e:           # every rank must take the same path: agree on it below
                 data.msg = f'peer all-reduce unavailable ({type(e).__name__}: {e}); using NCCL'
                 ok.zero_()
@@ -400,12 +401,15 @@ class _DefaultMLPUpdate:
             torch.distributed.all_reduce(self.gflat)
 
     @torch.no_grad()
-    def optimizer_step(self, config):
+    def optimizer_step(self, config, kl_row=None, kl_out=None):
+        """kl_row (several ranks with peers only): the exchange also carries the KL column of statistics row kl_row and
+        leaves its sum over the ranks in kl_out, a device fp64 scalar (pb_clip_adam_peer_ex / _parts_ex)."""
         g = self.opt.param_groups[0]
         lr = g['lr']
         lr_dev = _native.ptr(lr) if isinstance(lr, torch.Tensor) else None
         b1, b2 = g['betas']
         lib = _native.lib()
+        kl = (None, None) if kl_row is None else (C.c_void_p(self.stats.data_ptr() + 64 * kl_row + 8 * 4), _native.ptr(kl_out))
         hyper = (C.c_float(float(config.max_grad_norm)), C.c_float(1.0 / self.world),
                  C.c_float(0.0 if lr_dev is not None else float(lr)), lr_dev, C.c_float(b1), C.c_float(b2), C.c_float(g['eps']), None)
         if self.used_fused and (self.world == 1 or self.peer is not None):
@@ -419,18 +423,18 @@ class _DefaultMLPUpdate:
             if self.peer is not None:       # exchange + clip + Adam: one kernel
                 if self.peer_parts is None:
                     self.peer_parts = torch.zeros(lib.pb_peer_slices(), dtype=torch.float64, device=self.gflat.device)
-                _native.check(lib.pb_clip_adam_peer_parts(
+                _native.check(lib.pb_clip_adam_peer_parts_ex(
                     self.tensors, len(self.tensors), *hyper, C.byref(self.peer.struct), _native.ptr(self.gflat), self.gflat.numel(),
-                    _native.ptr(self.peer_parts), C.byref(self.head_pack), _native.stream_ptr()))
+                    _native.ptr(self.peer_parts), C.byref(self.head_pack), *kl, _native.stream_ptr()))
             else:
                 parts = C.c_void_p(self.fused_ws.data_ptr() + lib.pb_mlp_update_sumsq_offset())
                 _native.check(lib.pb_clip_adam_parts(self.tensors, len(self.tensors), *hyper, parts, lib.pb_mlp_update_sumsq_parts(),
                                                      None, C.byref(self.head_pack), _native.stream_ptr()))
             return
         else:
-            _native.check(lib.pb_clip_adam_peer(
+            _native.check(lib.pb_clip_adam_peer_ex(
                 self.tensors, len(self.tensors), *hyper, C.byref(self.peer.struct) if self.peer is not None else None,
-                _native.ptr(self.gflat), self.gflat.numel(), _native.stream_ptr()))
+                _native.ptr(self.gflat), self.gflat.numel(), *kl, _native.stream_ptr()))
         self.pack_heads()
 
     def loss_means(self, n_mb):
@@ -1004,9 +1008,11 @@ def update_plan(data):
         engine, form = 'reference', 'gathered'
 
     capture = None
-    # target_kl on one GPU: the stop is decided on the device and skips the later epochs through IF nodes (_KLStop)
+    # target_kl: the stop is decided on the device and skips the later epochs through IF nodes (_KLStop).  On several ranks
+    # only the peer exchange carries the KL sum inside the graph; the NCCL plans all-reduce it eagerly between epochs
+    kl_ranks = config.target_kl is not None and data.grad_bucket is not None
     if bool(getattr(config, 'cuda_graph_train', getattr(config, 'cuda_graph', False))) and \
-            (config.target_kl is None or data.grad_bucket is None) and data.train_graph_state >= 0:
+            (not kl_ranks or (manual is not None and manual.peer is not None)) and data.train_graph_state >= 0:
         # an NCCL call inside the update loop (autograd path on several ranks, or the hand-written update without peer
         # memory) keeps the update out of ONE graph -- capturing it hung on this stack (torch 2.11 / NCCL 2.28) -- so it
         # is captured in segments around an ordinary all-reduce call; with the peer all-reduce fused into
@@ -1109,11 +1115,16 @@ class _KLStop:
     a stop, or after a skipped body whose pb_kl_stop did not run, no later body runs.  Every epoch's work is captured on
     one body stream (this object's own, never shared) that is torch's current stream meanwhile -- autograd included, so
     no autograd node of one epoch belongs to another stream than the next -- with its allocations (cuBLAS workspace
-    included) in the train graph's pool."""
+    included) in the train graph's pool.
+    Several ranks: every rank decides on the KL sum over all ranks' rows of the epoch's last minibatch (kl_sum), divided
+    by world * rows per minibatch, so all ranks see the same bits and stop after the same epoch.  The peer exchange of that
+    minibatch's optimizer step carries the sum (pb_clip_adam_peer_ex / _parts_ex); the NCCL plans all-reduce it."""
 
-    def __init__(self, device):
+    def __init__(self, device, ranks=False):
         self.state = torch.zeros(2, dtype=torch.int32, device=device)   # stopped, epochs run
         self.target = torch.zeros(1, device=device)     # fp32(target_kl), set by train() before it runs or replays
+        # several ranks: the KL row sum over all ranks
+        self.kl_sum = torch.zeros(1, dtype=torch.float64, device=device) if ranks else None
         raw = C.c_void_p()
         _native.check(_native.lib().pb_stream_create(C.byref(raw)))
         self._raw_body = raw.value
@@ -1145,11 +1156,14 @@ class _KLStop:
     def capturing(self):
         return self.handles is not None
 
-    def decide(self, epoch, approx_kl=None, stats=None, row=0, rows=0):
-        """pb_kl_stop after `epoch` on an fp32 approx_kl tensor, or on row `row` of a [*, 8] fp64 statistics tensor;
-        captured, it sets the handle of epoch + 1's IF node."""
+    def decide(self, epoch, approx_kl=None, stats=None, row=0, rows=0, kl_sum=None):
+        """pb_kl_stop after `epoch` on an fp32 approx_kl tensor, on row `row` of a [*, 8] fp64 statistics tensor, or on an
+        fp64 KL row sum kl_sum (a one-element tensor) of `rows` rows; captured, it sets the handle of epoch + 1's IF node."""
         handle = self.handles[epoch + 1] if self.capturing else None
-        kl_sum = None if stats is None else C.c_void_p(stats.data_ptr() + 64 * row + 8 * 4)
+        if kl_sum is not None:
+            kl_sum = _native.ptr(kl_sum)
+        elif stats is not None:
+            kl_sum = C.c_void_p(stats.data_ptr() + 64 * row + 8 * 4)
         if approx_kl is not None and approx_kl.dtype != torch.float32:
             approx_kl = approx_kl.float()
         _native.check(_native.lib().pb_kl_stop(
@@ -1322,10 +1336,14 @@ def _train_device_part(data, plan, seg=None):
         # created on) alive into the next epoch
         carry['approx_kl'] = st[4].detach()
 
-    def optimizer_step():
+    world = manual.world if manual is not None else (data.grad_bucket.world if data.grad_bucket is not None else 1)
+    # several ranks with peers: the exchange of each epoch's last optimizer step carries the KL row sum (_KLStop)
+    kl_peer = kl_stop is not None and world > 1 and manual is not None and manual.peer is not None
+
+    def optimizer_step(kl_row=None):
         with profile.learn:
             if manual is not None:
-                manual.optimizer_step(config)
+                manual.optimizer_step(config, kl_row, kl_stop.kl_sum if kl_row is not None else None)
                 return
             torch.nn.utils.clip_grad_norm_(data.policy.parameters(), config.max_grad_norm)
             data.optimizer.step()
@@ -1346,13 +1364,28 @@ def _train_device_part(data, plan, seg=None):
                     data.grad_bucket.all_reduce_mean()          # ONE NCCL all-reduce per optimizer step
             if seg is not None:
                 seg.run('opt', optimizer_step)
+            elif kl_peer and mb == n_mb - 1 and epoch < config.update_epochs - 1:
+                optimizer_step(kl_row=epoch * n_mb + mb)
             else:
                 optimizer_step()
         if kl_stop is not None and epoch < config.update_epochs - 1:
-            if manual is not None:
-                kl_stop.decide(epoch, stats=manual.stats, row=epoch * n_mb + n_mb - 1, rows=manual.mb_rows)
-            else:
+            last = epoch * n_mb + n_mb - 1
+            if world == 1 and manual is not None:
+                kl_stop.decide(epoch, stats=manual.stats, row=last, rows=manual.mb_rows)
+            elif world == 1:
                 kl_stop.decide(epoch, approx_kl=carry['approx_kl'])
+            else:
+                # one decision for all ranks on the KL sum over their rows; without peers an NCCL all-reduce of this
+                # rank's fp64 row sum (the fused loss's fp32 mean times the rows, for autograd) forms it
+                rows = manual.mb_rows if manual is not None else experience.minibatch_size
+                if not kl_peer:
+                    with torch.no_grad():
+                        if manual is not None:
+                            kl_stop.kl_sum.copy_(manual.stats[last, 4:5])
+                        else:
+                            kl_stop.kl_sum.copy_(carry['approx_kl'].double() * rows)
+                    torch.distributed.all_reduce(kl_stop.kl_sum)
+                kl_stop.decide(epoch, kl_sum=kl_stop.kl_sum, rows=world * rows)
 
     for epoch in range(config.update_epochs):
         if kl_stop is not None and kl_stop.capturing:
@@ -1365,10 +1398,6 @@ def _train_device_part(data, plan, seg=None):
         else:
             run_epoch(epoch)
         data.train_epochs_run = epoch + 1
-        # several ranks: the reference's host-side check, each rank on its own approx_kl (one epoch: nothing to skip)
-        if kl_stop is None and config.target_kl is not None and data.grad_bucket is not None and \
-                carry['approx_kl'].item() > config.target_kl:
-            break
 
     with profile.train_misc:
         # explained variance on the device, same quantities as clean_pufferl.py:266-270
@@ -1384,20 +1413,21 @@ def _train_device_part(data, plan, seg=None):
 
 
 def _kl_stop(data):
-    """The device-side target_kl stop of this train() (_KLStop), or None: no target_kl, one epoch, or several ranks."""
+    """The device-side target_kl stop of this train() (_KLStop), or None: no target_kl, or one epoch."""
     config = data.config
-    if config.target_kl is None or config.update_epochs < 2 or data.grad_bucket is not None:
+    if config.target_kl is None or config.update_epochs < 2:
         return None
     if getattr(data, 'train_kl_stop', None) is None:
-        data.train_kl_stop = _KLStop(data.experience.device)
+        data.train_kl_stop = _KLStop(data.experience.device, ranks=data.grad_bucket is not None)
     return data.train_kl_stop
 
 
 def train(data):
     """One PPO update (reference: clean_pufferl.py:156-292).  With ``config.cuda_graph`` (recurrent policies only on one
-    GPU with the fused BPTT update; target_kl only on one GPU) the device part is captured once -- after an eager first
-    call that initialises the optimizer state -- and replayed as ONE graph launch; the learning rate lives in a device
-    tensor so annealing works under replay, and the target_kl stop is decided on the device (_KLStop).
+    GPU with the fused BPTT update; target_kl on several GPUs only with the peer exchange) the device part is captured
+    once -- after an eager first call that initialises the optimizer state -- and replayed as ONE graph launch; the
+    learning rate lives in a device tensor so annealing works under replay, and the target_kl stop is decided on the
+    device (_KLStop), on several ranks once for all of them.
     data.train_epochs_run: the epochs this call ran."""
     config, profile, experience = data.config, data.profile, data.experience
     data.losses = make_losses()

@@ -29,6 +29,8 @@ struct AdamArgs {
     pb_peer_comm peer;      // world <= 1: no exchange
     float* flat;            // the flat gradient buffer all `grad` pointers lie in (peer exchange only)
     int64_t flat_n;
+    const double* kl_in;    // nullable: the exchange's fp64 payload (peer.cuh), summed over the ranks into *kl_out
+    double* kl_out;
 };
 
 __global__ void __launch_bounds__(CA_THREADS) k_clip_adam(AdamArgs a) {
@@ -38,7 +40,7 @@ __global__ void __launch_bounds__(CA_THREADS) k_clip_adam(AdamArgs a) {
     const int tid = threadIdx.x;
 
     // ---- multi-GPU: sum the flat gradient buffer over all ranks through NVLink peer memory (peer.cuh)
-    if (a.peer.world > 1) pb_peer_allreduce_sum(a.peer, a.flat, a.flat_n);
+    if (a.peer.world > 1) pb_peer_allreduce_sum(a.peer, a.flat, a.flat_n, a.kl_in, a.kl_out);
 
     // ---- pass 1: global L2 norm of the (scaled) gradients
     float ss = 0.f;
@@ -116,7 +118,8 @@ __global__ void __launch_bounds__(CAP_THREADS) k_clip_adam_parts(AdamArgs a, con
     __shared__ int s_last;
     __shared__ double s_red[CAP_THREADS / 32];
     if (PEER) {
-        pb_peer_allreduce_slice(a.peer, a.flat, a.flat_n, peer_parts);       // flat slice summed over the ranks + its sum of squares
+        // flat slice summed over the ranks + its sum of squares (and the payload, in the last slice's CTA)
+        pb_peer_allreduce_slice(a.peer, a.flat, a.flat_n, peer_parts, a.kl_in, a.kl_out);
         __syncthreads();
         if (threadIdx.x == 0) {          // grid barrier: every slice and every partial sum is in global memory
             __threadfence();
@@ -244,9 +247,24 @@ extern "C" int pb_clip_adam(const pb_adam_tensor* tensors, int32_t n_tensors, fl
                              nullptr, nullptr, 0, stream);
 }
 
-extern "C" int pb_clip_adam_peer(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm, float grad_scale,
-                                 float lr, const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
-                                 const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, void* stream) {
+// The checks shared by the _ex forms: both or neither of kl_in / kl_out, 8-byte aligned; with them the communicator has
+// >= 2 ranks and the slot has room for the 4 payload floats after round4(n) gradient floats.
+static int check_payload(const char* who, const pb_peer_comm* comm, int64_t n, const double* kl_in, const double* kl_out) {
+    PB_REQUIRE((kl_in == nullptr) == (kl_out == nullptr), PB_ERR_INVALID, "%s: give both kl_in and kl_out, or neither", who);
+    PB_REQUIRE((uintptr_t)kl_in % 8 == 0 && (uintptr_t)kl_out % 8 == 0, PB_ERR_INVALID, "%s: misaligned kl_in or kl_out", who);
+    if (kl_in) {
+        PB_REQUIRE(comm && comm->world >= 2, PB_ERR_INVALID, "%s: a KL payload needs a communicator of 2 or more ranks", who);
+        PB_REQUIRE(((n + 3) & ~(int64_t)3) + 4 <= comm->capacity, PB_ERR_INVALID,
+                   "%s: no room for the KL payload (round4(%lld) + 4 floats > capacity %lld)", who, (long long)n,
+                   (long long)comm->capacity);
+    }
+    return PB_OK;
+}
+
+static int clip_adam_peer(const char* who, const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm,
+                          float grad_scale, float lr, const float* lr_dev, float beta1, float beta2, float eps,
+                          float* total_norm_out, const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel,
+                          const double* kl_in, double* kl_out, void* stream) {
     PB_REQUIRE(tensors && n_tensors >= 1 && n_tensors <= CA_MAX_TENSORS, PB_ERR_INVALID,
                "pb_clip_adam: 1..%d tensors", CA_MAX_TENSORS);
     AdamArgs a{};
@@ -274,18 +292,37 @@ extern "C" int pb_clip_adam_peer(const pb_adam_tensor* tensors, int32_t n_tensor
     if (comm && comm->world > 1) {
         PB_REQUIRE(comm->world <= PB_PEER_MAX_RANKS && comm->rank >= 0 && comm->rank < comm->world && comm->epoch &&
                        grad_flat && grad_flat_numel >= 1 && grad_flat_numel <= comm->capacity,
-                   PB_ERR_INVALID, "pb_clip_adam_peer: bad communicator or flat gradient buffer");
-        for (int r = 0; r < comm->world; ++r) PB_REQUIRE(comm->base[r], PB_ERR_INVALID, "pb_clip_adam_peer: peer %d not mapped", r);
+                   PB_ERR_INVALID, "%s: bad communicator or flat gradient buffer", who);
+        for (int r = 0; r < comm->world; ++r) PB_REQUIRE(comm->base[r], PB_ERR_INVALID, "%s: peer %d not mapped", who, r);
         for (int k = 0; k < n_tensors; ++k)
             PB_REQUIRE(tensors[k].grad >= grad_flat && tensors[k].grad + tensors[k].numel <= grad_flat + grad_flat_numel,
-                       PB_ERR_INVALID, "pb_clip_adam_peer: gradient %d lies outside the flat buffer", k);
+                       PB_ERR_INVALID, "%s: gradient %d lies outside the flat buffer", who, k);
         a.peer = *comm;
         a.flat = grad_flat;
         a.flat_n = grad_flat_numel;
     }
+    const int rc = check_payload(who, comm, grad_flat_numel, kl_in, kl_out);
+    if (rc) return rc;
+    a.kl_in = kl_in;
+    a.kl_out = kl_out;
     k_clip_adam<<<1, CA_THREADS, 0, (cudaStream_t)stream>>>(a);
     PB_LAUNCH_CHECK();
     return PB_OK;
+}
+
+extern "C" int pb_clip_adam_peer(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm, float grad_scale,
+                                 float lr, const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
+                                 const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, void* stream) {
+    return clip_adam_peer("pb_clip_adam_peer", tensors, n_tensors, max_grad_norm, grad_scale, lr, lr_dev, beta1, beta2, eps,
+                          total_norm_out, comm, grad_flat, grad_flat_numel, nullptr, nullptr, stream);
+}
+
+extern "C" int pb_clip_adam_peer_ex(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm, float grad_scale,
+                                    float lr, const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
+                                    const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, const double* kl_in,
+                                    double* kl_out, void* stream) {
+    return clip_adam_peer("pb_clip_adam_peer_ex", tensors, n_tensors, max_grad_norm, grad_scale, lr, lr_dev, beta1, beta2, eps,
+                          total_norm_out, comm, grad_flat, grad_flat_numel, kl_in, kl_out, stream);
 }
 
 // pb_clip_adam for callers that hold the sum of squares of the (already summed over ranks, unscaled) gradient as n_parts
@@ -329,27 +366,28 @@ extern "C" int pb_clip_adam_parts(const pb_adam_tensor* tensors, int32_t n_tenso
 
 // The same with the gradient all-reduce over NVLink peer memory in front, in ONE kernel (pb_peer_slices() CTAs): replaces the
 // pair pb_peer_allreduce_parts + pb_clip_adam_parts.  sumsq_scratch: pb_peer_slices() doubles of device memory.
-extern "C" int pb_clip_adam_peer_parts(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm, float grad_scale,
-                                       float lr, const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
-                                       const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, double* sumsq_scratch,
-                                       const pb_head_pack* pack, void* stream) {
+static int clip_adam_peer_parts(const char* who, const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm,
+                                float grad_scale, float lr, const float* lr_dev, float beta1, float beta2, float eps,
+                                float* total_norm_out, const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel,
+                                double* sumsq_scratch, const pb_head_pack* pack, const double* kl_in, double* kl_out,
+                                void* stream) {
     PB_REQUIRE(tensors && n_tensors >= 1 && n_tensors <= CA_MAX_TENSORS && comm && grad_flat && sumsq_scratch, PB_ERR_INVALID,
-               "pb_clip_adam_peer_parts: bad arguments");
+               "%s: bad arguments", who);
     PB_REQUIRE(comm->world >= 2 && comm->world <= PB_PEER_MAX_RANKS && comm->rank >= 0 && comm->rank < comm->world && comm->epoch &&
                    grad_flat_numel >= 1 && grad_flat_numel <= comm->capacity,
-               PB_ERR_INVALID, "pb_clip_adam_peer_parts: bad communicator or flat gradient buffer");
-    for (int r = 0; r < comm->world; ++r) PB_REQUIRE(comm->base[r], PB_ERR_INVALID, "pb_clip_adam_peer_parts: peer %d not mapped", r);
+               PB_ERR_INVALID, "%s: bad communicator or flat gradient buffer", who);
+    for (int r = 0; r < comm->world; ++r) PB_REQUIRE(comm->base[r], PB_ERR_INVALID, "%s: peer %d not mapped", who, r);
     AdamArgs a{};
     for (int k = 0; k < n_tensors; ++k) {
         const pb_adam_tensor& t = tensors[k];
         PB_REQUIRE(t.param && t.exp_avg && t.exp_avg_sq && t.step && t.grad && t.numel >= 1, PB_ERR_INVALID,
-                   "pb_clip_adam_peer_parts: tensor %d has a null pointer or no elements", k);
+                   "%s: tensor %d has a null pointer or no elements", who, k);
         PB_REQUIRE(t.grad >= grad_flat && t.grad + t.numel <= grad_flat + grad_flat_numel, PB_ERR_INVALID,
-                   "pb_clip_adam_peer_parts: gradient %d lies outside the flat buffer", k);
+                   "%s: gradient %d lies outside the flat buffer", who, k);
         a.t[k] = t;
     }
     PB_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f && grad_scale > 0.f,
-               PB_ERR_INVALID, "pb_clip_adam_peer_parts: bad hyper-parameters");
+               PB_ERR_INVALID, "%s: bad hyper-parameters", who);
     a.n = n_tensors;
     a.max_norm = max_grad_norm;
     a.grad_scale = grad_scale;
@@ -366,13 +404,36 @@ extern "C" int pb_clip_adam_peer_parts(const pb_adam_tensor* tensors, int32_t n_
     if (pack) {
         PB_REQUIRE(pack->w_dec && pack->b_dec && pack->w_val && pack->b_val && pack->w_cat && pack->b_cat && pack->n_act >= 1 &&
                        pack->n_act <= 7 && pack->hid >= 1,
-                   PB_ERR_INVALID, "pb_clip_adam_peer_parts: bad head-pack arguments");
+                   PB_ERR_INVALID, "%s: bad head-pack arguments", who);
         hp = *pack;
     }
+    const int rc = check_payload(who, comm, grad_flat_numel, kl_in, kl_out);
+    if (rc) return rc;
+    a.kl_in = kl_in;
+    a.kl_out = kl_out;
     k_clip_adam_parts<512, true><<<PB_PEER_SLICES, 512, 0, (cudaStream_t)stream>>>(
         a, nullptr, 0, reinterpret_cast<unsigned long long*>(comm->epoch), hp, sumsq_scratch);
     PB_LAUNCH_CHECK();
     return PB_OK;
+}
+
+extern "C" int pb_clip_adam_peer_parts(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm, float grad_scale,
+                                       float lr, const float* lr_dev, float beta1, float beta2, float eps, float* total_norm_out,
+                                       const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel, double* sumsq_scratch,
+                                       const pb_head_pack* pack, void* stream) {
+    return clip_adam_peer_parts("pb_clip_adam_peer_parts", tensors, n_tensors, max_grad_norm, grad_scale, lr, lr_dev, beta1,
+                                beta2, eps, total_norm_out, comm, grad_flat, grad_flat_numel, sumsq_scratch, pack, nullptr,
+                                nullptr, stream);
+}
+
+extern "C" int pb_clip_adam_peer_parts_ex(const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm,
+                                          float grad_scale, float lr, const float* lr_dev, float beta1, float beta2, float eps,
+                                          float* total_norm_out, const pb_peer_comm* comm, float* grad_flat,
+                                          int64_t grad_flat_numel, double* sumsq_scratch, const pb_head_pack* pack,
+                                          const double* kl_in, double* kl_out, void* stream) {
+    return clip_adam_peer_parts("pb_clip_adam_peer_parts_ex", tensors, n_tensors, max_grad_norm, grad_scale, lr, lr_dev, beta1,
+                                beta2, eps, total_norm_out, comm, grad_flat, grad_flat_numel, sumsq_scratch, pack, kl_in,
+                                kl_out, stream);
 }
 
 extern "C" int pb_pack_heads(const float* w_dec, const float* b_dec, const float* w_val, const float* b_val,

@@ -27,8 +27,31 @@ __device__ __forceinline__ float4 pb_ld_relaxed_sys_f32x4(const float* p) {
     return v;
 }
 
+// The optional fp64 payload of an exchange (the KL row sum of pb_clip_adam_peer_ex / _parts_ex): 4 reserved floats of the
+// slot right after the gradient, at round4(n), as 32-bit words (lo, hi, 0, 0) -- word stores, so a slot of any alignment
+// holds it.  Written by one thread before its CTA's flag store, read by one thread after the CTA's flag waits.
+__device__ __forceinline__ int64_t pb_peer_payload_offset(int64_t n) { return (n + 3) & ~(int64_t)3; }
+__device__ __forceinline__ void pb_peer_payload_put(float* slot_payload, double v) {
+    uint32_t* w = reinterpret_cast<uint32_t*>(slot_payload);
+    w[0] = (uint32_t)__double2loint(v);
+    w[1] = (uint32_t)__double2hiint(v);
+    w[2] = 0u;
+    w[3] = 0u;
+}
+// sum over ranks of the payloads in slot offset `off`, in rank order from 0.0: the same bits on every rank
+__device__ __forceinline__ double pb_peer_payload_sum(const pb_peer_comm& c, int64_t off) {
+    double s = 0.0;
+    for (int r = 0; r < c.world; ++r) {
+        const float* p = reinterpret_cast<const float*>(c.base[r]) + off;
+        s += __hiloint2double(__float_as_int(pb_ld_relaxed_sys_f32(p + 1)), __float_as_int(pb_ld_relaxed_sys_f32(p)));
+    }
+    return s;
+}
+
 // One CTA (any size that is a multiple of 32): flat[0..n) <- sum over ranks, in rank order (bit-identical everywhere).
-__device__ __forceinline__ void pb_peer_allreduce_sum(const pb_peer_comm& c, float* flat, int64_t n) {
+// kl_in (nullable, then kl_out too): this rank's payload; *kl_out <- the ranks' payloads summed in rank order.
+__device__ __forceinline__ void pb_peer_allreduce_sum(const pb_peer_comm& c, float* flat, int64_t n, const double* kl_in = nullptr,
+                                                      double* kl_out = nullptr) {
     if (c.world <= 1) return;
     __shared__ uint64_t s_epoch;
     const int tid = threadIdx.x, nt = blockDim.x;
@@ -43,6 +66,7 @@ __device__ __forceinline__ void pb_peer_allreduce_sum(const pb_peer_comm& c, flo
     const int64_t n4 = vec ? n >> 2 : 0;
     for (int64_t i = tid; i < n4; i += nt) reinterpret_cast<float4*>(mine)[i] = reinterpret_cast<const float4*>(flat)[i];
     for (int64_t i = 4 * n4 + tid; i < n; i += nt) mine[i] = flat[i];
+    if (kl_in && tid == 0) pb_peer_payload_put(mine + pb_peer_payload_offset(n), *kl_in);
     __threadfence_system();
     __syncthreads();
     if (tid < c.world) {   // raise my flag in every rank's buffer (mine included)
@@ -73,6 +97,7 @@ __device__ __forceinline__ void pb_peer_allreduce_sum(const pb_peer_comm& c, flo
         for (int r = 0; r < c.world; ++r) s += pb_ld_relaxed_sys_f32(reinterpret_cast<const float*>(c.base[r]) + slot_off + i);
         flat[i] = s;
     }
+    if (kl_in && tid == 0) *kl_out = pb_peer_payload_sum(c, slot_off + pb_peer_payload_offset(n));
     __syncthreads();
     if (tid == 0) *c.epoch = e;
 }
@@ -82,7 +107,10 @@ constexpr int PB_PEER_SLICES = 16;           // flags of source rank r, slice b 
 // Multi-CTA form: CTA b (of PB_PEER_SLICES) sums slice b over all ranks.  Slices are independent (own flag per rank and
 // slice), so there is no grid-wide barrier; the epoch counter is NOT advanced here (every CTA reads it at its start): the
 // kernel that follows in the stream does it (pb_clip_adam_parts).  sumsq[b] = sum of squares of the summed slice.
-__device__ __forceinline__ void pb_peer_allreduce_slice(const pb_peer_comm& c, float* flat, int64_t n, double* sumsq) {
+// kl_in / kl_out: the payload, as in pb_peer_allreduce_sum, owned by the CTA of the last slice (the payload follows the
+// gradient's tail) and carried by that CTA's own flags.
+__device__ __forceinline__ void pb_peer_allreduce_slice(const pb_peer_comm& c, float* flat, int64_t n, double* sumsq,
+                                                        const double* kl_in = nullptr, double* kl_out = nullptr) {
     __shared__ uint64_t s_epoch;
     __shared__ double s_sq[32];
     const int tid = threadIdx.x, nt = blockDim.x, b = blockIdx.x;
@@ -102,6 +130,8 @@ __device__ __forceinline__ void pb_peer_allreduce_slice(const pb_peer_comm& c, f
     for (int64_t i = lo + 4 * tid; i < hi4; i += 4 * nt)
         *reinterpret_cast<float4*>(mine + i) = *reinterpret_cast<const float4*>(flat + i);
     for (int64_t i = hi4 + tid; i < hi; i += nt) mine[i] = flat[i];
+    const bool payload = kl_in && b == PB_PEER_SLICES - 1;
+    if (payload && tid == 0) pb_peer_payload_put(mine + pb_peer_payload_offset(n), *kl_in);
     __syncthreads();
     if (tid < c.world) {
         __threadfence_system();      // (cumulative: the CTA barrier ordered every thread's slot writes before this thread)
@@ -114,6 +144,7 @@ __device__ __forceinline__ void pb_peer_allreduce_slice(const pb_peer_comm& c, f
         }
     }
     __syncthreads();
+    if (payload && tid == 0) *kl_out = pb_peer_payload_sum(c, slot_off + pb_peer_payload_offset(n));
     double sq = 0.0;
     for (int64_t i = lo + 4 * tid; i < hi4; i += 4 * nt) {
         float4 v[PB_PEER_MAX_RANKS];

@@ -11,7 +11,7 @@
 //   z   = e W_ih^T + h W_hh^T + (b_ih + b_hh)           [512], PyTorch gate order i, f, g, o
 //   c'  = sigmoid(f) c + sigmoid(i) tanh(g),  h' = sigmoid(o) tanh(c')     (h, c overwritten in place)
 //   out = h' W_cat^T + b_cat                            n_act logits | value | zero pad (8 or 16 columns)
-//   then the sampling epilogue of pb_policy_mlp_sample (policy_sample.cuh) and the value / logprob / action row stores.
+//   then the sampling epilogue and row stores that pb_policy_mlp_sample uses too (pb_sample_epilogue, policy_sample.cuh).
 // The state is not reset on done, like the reference and the unfused path.
 //
 // Layout.  A CTA owns 128 rows, 8 warps x 16 rows, 1 CTA per SM (128 CTAs at N = 16384: one wave on 132 SMs).
@@ -71,59 +71,8 @@ struct LstmParams {
     const float* w_gates; const float* b_gates;    // [16][32][264] TF32, [16][32]
     const float* w_heads; const float* b_heads;    // [NC][128], [NC]
     float* h; int64_t h_stride; float* c; int64_t c_stride;   // [m][128] each, read then overwritten
-    int64_t m; int n_act;
-    uint64_t seed; uint64_t* counter; unsigned int* ticket;
-    int64_t* actions; float* logprobs; float* values; float* entropies;
+    PbSampleOut sample;
 };
-
-// The sampling epilogue of a warp's 16 rows for the H = 256 kernel (k_policy_lstm_sample keeps the same code inline,
-// which leaves its compiled code as it was): out[q] = (row g, cols 8q + 2t, +1), (row g + 8, same) of h' W_cat^T;
-// gather the NC columns of a row across its quad, add the head bias, sample, store the row; then the last CTA to leave
-// advances the stream counter (every CTA read it before its ticket).  lr: the warp's local row of fragment row g.
-template <int NC>
-__device__ __forceinline__ void sample_rows(const float (&out)[NC / 8][4], const float* sBh, const LstmParams& p,
-                                            int64_t row0, int lr, int lane, int tid, uint64_t offset) {
-    const int t = lane & 3;
-    float rowv[2][NC];
-#pragma unroll
-    for (int q8 = 0; q8 < NC / 8; ++q8) {
-#pragma unroll
-        for (int qq = 0; qq < 4; ++qq) {
-            const int src = (lane & ~3) | qq, k = 8 * q8 + 2 * qq;
-            const float v0 = __shfl_sync(0xffffffffu, out[q8][0], src), v1 = __shfl_sync(0xffffffffu, out[q8][1], src);
-            const float v2 = __shfl_sync(0xffffffffu, out[q8][2], src), v3 = __shfl_sync(0xffffffffu, out[q8][3], src);
-            rowv[0][k] = v0 + sBh[k]; rowv[0][k + 1] = v1 + sBh[k + 1];
-            rowv[1][k] = v2 + sBh[k]; rowv[1][k + 1] = v3 + sBh[k + 1];
-        }
-    }
-    // lane t == 0 finishes row g, lane t == 1 finishes row g + 8
-    if (t < 2) {
-        const int64_t r = row0 + lr + 8 * t;
-        if (r < p.m) {
-            float z[NC];
-#pragma unroll
-            for (int k = 0; k < NC; ++k) z[k] = t ? rowv[1][k] : rowv[0][k];
-            int a;
-            float lp, ent, value;
-            pb_sample_row<NC>(z, p.n_act, pb_policy_uniform(p.seed, offset, r), a, lp, ent, value);
-            p.actions[r] = a;
-            p.logprobs[r] = lp;
-            p.values[r] = value;
-            if (p.entropies) p.entropies[r] = ent;
-        }
-    }
-    if (p.ticket) {
-        __syncthreads();
-        if (tid == 0) {
-            __threadfence();
-            if (atomicAdd(p.ticket, 1u) == gridDim.x - 1) {
-                *p.ticket = 0u;
-                *p.counter = offset + 1ull;
-                __threadfence();
-            }
-        }
-    }
-}
 
 template <int NC>
 __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams p) {
@@ -139,8 +88,8 @@ __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
     const int64_t row0 = (int64_t)blockIdx.x * PL_ROWS;
-    const int valid = (int)((p.m - row0) < PL_ROWS ? (p.m - row0) : PL_ROWS);
-    const uint64_t offset = p.counter ? *p.counter : 0ull;   // every CTA reads it before taking its exit ticket
+    const int valid = (int)((p.sample.m - row0) < PL_ROWS ? (p.sample.m - row0) : PL_ROWS);
+    const uint64_t offset = p.sample.counter ? *p.sample.counter : 0ull;   // read by every CTA before its exit ticket
 
     // ---- weights by bulk copy: W_enc and the first two gate chunks are in flight while x, h and the small operands load
     if (tid == 0) {
@@ -228,47 +177,7 @@ __global__ void __launch_bounds__(PL_THREADS, 1) k_policy_lstm_sample(LstmParams
         lstm_head_chunk<NC>(out, hn, sWh, g, u0);
     }
 
-    // ---- out[q]: (row g, cols 8q + 2t, +1), (row g + 8, same).  Gather the NC columns of a row across its quad.
-    float rowv[2][NC];
-#pragma unroll
-    for (int q8 = 0; q8 < NC / 8; ++q8) {
-#pragma unroll
-        for (int qq = 0; qq < 4; ++qq) {
-            const int src = (lane & ~3) | qq, k = 8 * q8 + 2 * qq;
-            const float v0 = __shfl_sync(0xffffffffu, out[q8][0], src), v1 = __shfl_sync(0xffffffffu, out[q8][1], src);
-            const float v2 = __shfl_sync(0xffffffffu, out[q8][2], src), v3 = __shfl_sync(0xffffffffu, out[q8][3], src);
-            rowv[0][k] = v0 + sBh[k]; rowv[0][k + 1] = v1 + sBh[k + 1];
-            rowv[1][k] = v2 + sBh[k]; rowv[1][k + 1] = v3 + sBh[k + 1];
-        }
-    }
-    // lane t == 0 finishes row g, lane t == 1 finishes row g + 8
-    if (t < 2) {
-        const int64_t r = row0 + lr + 8 * t;
-        if (r < p.m) {
-            float z[NC];
-#pragma unroll
-            for (int k = 0; k < NC; ++k) z[k] = t ? rowv[1][k] : rowv[0][k];
-            int a;
-            float lp, ent, value;
-            pb_sample_row<NC>(z, p.n_act, pb_policy_uniform(p.seed, offset, r), a, lp, ent, value);
-            p.actions[r] = a;
-            p.logprobs[r] = lp;
-            p.values[r] = value;
-            if (p.entropies) p.entropies[r] = ent;
-        }
-    }
-    // ---- the last CTA to leave advances the stream counter (every CTA read it before its ticket)
-    if (p.ticket) {
-        __syncthreads();
-        if (tid == 0) {
-            __threadfence();
-            if (atomicAdd(p.ticket, 1u) == gridDim.x - 1) {
-                *p.ticket = 0u;
-                *p.counter = offset + 1ull;
-                __threadfence();
-            }
-        }
-    }
+    pb_sample_epilogue<NC>(out, sBh, p.sample, row0 + lr, offset);
 }
 
 // The H = 256 step (LSTMWrapper(Default(hidden_size=256), 256, 256)): the same function with the geometry of
@@ -294,8 +203,8 @@ __global__ void __launch_bounds__(128, 1) k_policy_lstm_sample_256(LstmParams p)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
     const int64_t row0 = (int64_t)blockIdx.x * PW_ROWS;
-    const int valid = (int)((p.m - row0) < PW_ROWS ? (p.m - row0) : PW_ROWS);
-    const uint64_t offset = p.counter ? *p.counter : 0ull;
+    const int valid = (int)((p.sample.m - row0) < PW_ROWS ? (p.sample.m - row0) : PW_ROWS);
+    const uint64_t offset = p.sample.counter ? *p.sample.counter : 0ull;
 
     if (tid == 0) {
         mbar_init(&bars[0], 1);
@@ -378,13 +287,13 @@ __global__ void __launch_bounds__(128, 1) k_policy_lstm_sample_256(LstmParams p)
         }
         lstm_head_chunk<NC, PW_HP>(out, hn, sWh, g, u0);
     }
-    sample_rows<NC>(out, sBh, p, row0, lr, lane, tid, offset);
+    pb_sample_epilogue<NC>(out, sBh, p.sample, row0 + lr, offset);
 }
 
 template <int NC>
 int launch(const LstmParams& p, cudaStream_t stream) {
     PB_CUDA(cudaFuncSetAttribute(k_policy_lstm_sample<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PL_SMEM));
-    k_policy_lstm_sample<NC><<<(unsigned)pb_ceil_div(p.m, PL_ROWS), PL_THREADS, PL_SMEM, stream>>>(p);
+    k_policy_lstm_sample<NC><<<(unsigned)pb_ceil_div(p.sample.m, PL_ROWS), PL_THREADS, PL_SMEM, stream>>>(p);
     PB_LAUNCH_CHECK();
     return PB_OK;
 }
@@ -393,7 +302,7 @@ template <int NC>
 int launch_256(const LstmParams& p, cudaStream_t stream) {
     PB_CUDA(cudaFuncSetAttribute(k_policy_lstm_sample_256<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)PW_SMEM));
-    k_policy_lstm_sample_256<NC><<<(unsigned)pb_ceil_div(p.m, PW_ROWS), 128, PW_SMEM, stream>>>(p);
+    k_policy_lstm_sample_256<NC><<<(unsigned)pb_ceil_div(p.sample.m, PW_ROWS), 128, PW_SMEM, stream>>>(p);
     PB_LAUNCH_CHECK();
     return PB_OK;
 }
@@ -425,7 +334,7 @@ extern "C" int pb_policy_lstm_sample(const float* obs, int64_t obs_stride, int32
                hidden_size);
     PB_REQUIRE(!ticket_dev || counter_dev, PB_ERR_INVALID, "pb_policy_lstm_sample: ticket_dev needs counter_dev");
     LstmParams p{obs, obs_stride, in_features, w_enc, b_enc, w_gates, b_gates, w_heads, b_heads, h, h_stride, c, c_stride,
-                 m, n_act, seed, counter_dev, ticket_dev, actions, logprobs, values, entropies};
+                 {m, n_act, seed, counter_dev, ticket_dev, actions, logprobs, values, entropies}};
     if (hidden_size == PW_H)
         return n_act + 1 <= 8 ? launch_256<8>(p, (cudaStream_t)stream) : launch_256<16>(p, (cudaStream_t)stream);
     return n_act + 1 <= 8 ? launch<8>(p, (cudaStream_t)stream) : launch<16>(p, (cudaStream_t)stream);

@@ -13,6 +13,8 @@
 //     A zero-probability action is never drawn.  logprob = z_a - lse (the reference's normalized[a]);
 //     entropy = -sum (p_k/T) * max(z_k - lse, -FLT_MAX) (cleanrl.entropy of softmax(normalized), -inf logits kept
 //     finite as there).
+//   * PbSampleOut and pb_sample_epilogue<NC>: the row outputs of the fused policy steps (policy_mlp.cu, policy_lstm.cu)
+//     and the epilogue that fills them from a warp's head-product fragments and advances the stream counter.
 #pragma once
 #include "pb_common.cuh"
 #include "wgmma.cuh"
@@ -63,4 +65,61 @@ __device__ __forceinline__ void pb_sample_row(const float (&z)[NC], int n_act, f
     logprob = lp;
     entropy = ent;
     value = v;
+}
+
+// What a fused policy step writes: rows [0, m) of actions / logprobs / values (/ entropies), drawn with
+// pb_policy_uniform(seed, *counter, row); with a ticket, the last CTA to leave advances *counter by one.
+struct PbSampleOut {
+    int64_t m; int n_act;
+    uint64_t seed; uint64_t* counter; unsigned int* ticket;               // counter may be null (offset 0), ticket too
+    int64_t* actions; float* logprobs; float* values; float* entropies;   // [m] each (entropies may be null)
+};
+
+// The sampling epilogue of a warp's 16 rows, called by every thread of the CTA.  out[q8] = (row g, cols 8q8 + 2t, +1),
+// (row g + 8, same) of the head product, without its bias sBh[NC]; row = the global row of fragment row g; offset = the
+// *counter every CTA read before it got here.  The NC columns of a row are gathered across its quad, lane t == 0
+// finishes row g and lane t == 1 row g + 8.  Then the last CTA to leave advances the stream counter, so the host needs
+// no separate "counter += 1" launch per env step.
+template <int NC>
+__device__ __forceinline__ void pb_sample_epilogue(const float (&out)[NC / 8][4], const float* sBh, const PbSampleOut& o,
+                                                   int64_t row, uint64_t offset) {
+    const int lane = threadIdx.x & 31, t = lane & 3;
+    float rowv[2][NC];
+#pragma unroll
+    for (int q8 = 0; q8 < NC / 8; ++q8) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int src = (lane & ~3) | q, k = 8 * q8 + 2 * q;
+            const float v0 = __shfl_sync(0xffffffffu, out[q8][0], src), v1 = __shfl_sync(0xffffffffu, out[q8][1], src);
+            const float v2 = __shfl_sync(0xffffffffu, out[q8][2], src), v3 = __shfl_sync(0xffffffffu, out[q8][3], src);
+            rowv[0][k] = v0 + sBh[k]; rowv[0][k + 1] = v1 + sBh[k + 1];
+            rowv[1][k] = v2 + sBh[k]; rowv[1][k + 1] = v3 + sBh[k + 1];
+        }
+    }
+    if (t < 2) {
+        const int64_t r = row + 8 * t;
+        if (r < o.m) {
+            float z[NC];
+#pragma unroll
+            for (int k = 0; k < NC; ++k) z[k] = t ? rowv[1][k] : rowv[0][k];
+            int a;
+            float lp, ent, value;
+            pb_sample_row<NC>(z, o.n_act, pb_policy_uniform(o.seed, offset, r), a, lp, ent, value);
+            o.actions[r] = a;
+            o.logprobs[r] = lp;
+            o.values[r] = value;
+            if (o.entropies) o.entropies[r] = ent;
+        }
+    }
+    if (o.ticket) {
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            __threadfence();
+            if (atomicAdd(o.ticket, 1u) == gridDim.x - 1) {
+                *o.ticket = 0u;
+                *o.counter = offset + 1ull;
+                __threadfence();
+            }
+        }
+    }
 }

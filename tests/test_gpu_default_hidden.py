@@ -1,5 +1,5 @@
 """models.Default with 256, 384 and 512 hidden units on the hand-written kernels: pb_policy_mlp_sample's chunked
-rollout step (k_policy_mlp_sample_wide), pb_mlp_tail_backward_ex over 128-column slices of the hidden layer (both the
+rollout step (the W_enc ring of k_policy_mlp_sample), pb_mlp_tail_backward_ex over 128-column slices of the hidden layer (both the
 TMA-staged and the strided kernel), the fast-path forward / backward, and the _DefaultMLPUpdate chain of train().
 The H = 128 kernels are covered by test_gpu_sampling, test_gpu_default_heads16 and test_gpu_ppo_loss."""
 import ctypes as C
@@ -136,6 +136,43 @@ def test_policy_mlp_wide_tf32_tie_in_second_chunk(n_act):
     v_trunc = (trunc(h_t) @ trunc(w_cat).t() + b_cat.double())[:, n_act]
     assert float((out64[:, n_act] - v_trunc).abs().min()) >= 4.8e-4        # the probe separates the roundings
     check_mlp_outputs(out64, n_act, a, lp, ent, v, 3, 0, f'second-chunk tie n_act={n_act}')
+
+
+@pytest.mark.parametrize('n_act', [5, 12, 24])
+@pytest.mark.parametrize('hid', WIDE)
+def test_policy_mlp_wide_zero_units_match_hidden_128(hid, n_act):
+    """Every hidden size runs one arithmetic: a Default at H = 256, 384, 512 whose encoder rows, encoder bias and head
+    columns past unit 128 are zero gives, bit for bit, the actions, logprobs, values, entropies, counter and ticket of the
+    H = 128 Default made of its first 128 units (the extra chunks add exact zeros).  n_act 5, 12, 24 take the 8-, 16- and
+    32-row heads; 20001 rows end in a partial CTA; observation rows are 132 floats apart."""
+    m, start, seed = 20001, 2 ** 33 + 5, 9
+    wide = make_default(hid, n_act, seed=hid + n_act)
+    narrow = make_default(128, n_act)
+    with torch.no_grad():
+        wide.encoder.weight[128:] = 0
+        wide.encoder.bias[128:] = 0
+        wide.decoder.weight[:, 128:] = 0
+        wide.value_head.weight[:, 128:] = 0
+        for a, b in ((narrow.encoder.weight, wide.encoder.weight[:128]), (narrow.encoder.bias, wide.encoder.bias[:128]),
+                     (narrow.decoder.weight, wide.decoder.weight[:, :128]), (narrow.decoder.bias, wide.decoder.bias),
+                     (narrow.value_head.weight, wide.value_head.weight[:, :128]),
+                     (narrow.value_head.bias, wide.value_head.bias)):
+            a.copy_(b)
+    wide.invalidate_cache()
+    narrow.invalidate_cache()
+    x = (torch.rand(m, 132, device=DEV, generator=torch.Generator(device=DEV).manual_seed(n_act)) * 2 - 1)[:, :128]
+    outs = []
+    for net in (wide, narrow):
+        counter = torch.tensor([start], dtype=torch.int64, device=DEV)
+        ticket = torch.zeros(1, dtype=torch.int32, device=DEV)
+        acts = torch.full((m,), -7, dtype=torch.int64, device=DEV)
+        lp, val, ent = (torch.full((m,), 7.0, device=DEV) for _ in range(3))
+        _native.check(policy_step_abi(net, x, 132, counter, ticket, acts, lp, val, ent, seed))
+        outs.append((acts, lp, val, ent, counter, ticket))
+    torch.cuda.synchronize()
+    assert int(outs[0][4][0]) == start + 1
+    for name, a, b in zip(('actions', 'logprobs', 'values', 'entropies', 'counter', 'ticket'), *outs):
+        assert torch.equal(a, b), f'H={hid} n_act={n_act}: {name} differs from the H = 128 model'
 
 
 # ---------------------------------------------------------------------------------------------------------------------

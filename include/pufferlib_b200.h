@@ -473,7 +473,8 @@ int pb_clip_adam(const pb_adam_tensor* tensors, int32_t n_tensors, float max_gra
  * in every peer's buffer, wait for all flags, add all ranks' slots in rank order with direct NVLink loads (identical
  * bits on every rank).  No host involvement per call: it can be captured in a CUDA graph.  pb_clip_adam_peer is
  * pb_clip_adam with that all-reduce of the flat gradient buffer fused in front (all `grad` pointers of the tensors must
- * lie inside grad_flat[0..grad_flat_numel)); pass grad_scale = 1/world for the mean. */
+ * lie inside grad_flat[0..grad_flat_numel)); pass grad_scale = 1/world for the mean.  Callers that keep their own
+ * optimizer step (the recurrent update, whose clip + Adam stay torch's) take the mean alone from pb_peer_allreduce_mean. */
 #define PB_PEER_MAX_RANKS 8
 typedef struct pb_peer_comm {
     int32_t world, rank;
@@ -494,6 +495,14 @@ int pb_peer_allreduce(const pb_peer_comm* comm, float* flat, int64_t n, void* st
  * step may be in flight per device at a time (device-wide ticket counters). */
 int pb_peer_allreduce_parts(const pb_peer_comm* comm, float* flat, int64_t n, double* sumsq_parts, void* stream);
 int32_t pb_peer_slices(void);
+/* The gradient mean of a caller that keeps its own clip + optimizer step (the recurrent update's GradBucket): flat[0..n) <-
+ * (sum over the ranks in rank order) * (1.f / world), with the reciprocal rounded to fp32 first -- bitwise what an all-reduce
+ * sum followed by torch's flat.div_(world) gives for the same rank-order sum.  pb_peer_slices() CTAs on the protocol of
+ * pb_peer_allreduce_parts; unlike it, this call advances the communicator's epoch counter itself (once), so it stands alone
+ * in a stream or a CUDA graph.  kl_in / kl_out: the optional fp64 payload with the layout and rules of
+ * pb_clip_adam_peer_parts_ex (below): *kl_out <- the ranks' *kl_in added in rank order from 0.0, not scaled.  Bad arguments:
+ * PB_ERR_INVALID and nothing is launched. */
+int pb_peer_allreduce_mean(const pb_peer_comm* comm, float* flat, int64_t n, const double* kl_in, double* kl_out, void* stream);
 typedef struct pb_head_pack {   /* optional tail of pb_clip_adam_parts: pb_pack_heads (without the encoder copy) on the updated parameters */
     const float* w_dec;
     const float* b_dec;

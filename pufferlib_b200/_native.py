@@ -134,6 +134,7 @@ SIGNATURES = {
                                              C.c_int64, C.c_void_p, C.POINTER(HeadPack), C.c_void_p, C.c_void_p, C.c_void_p]),
     'pb_peer_allreduce_parts': (C.c_int, [C.POINTER(PeerComm), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     'pb_peer_slices': (C.c_int32, []),
+    'pb_peer_allreduce_mean': (C.c_int, [C.POINTER(PeerComm), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     'pb_mlp_update_sumsq_offset': (C.c_size_t, []),
     'pb_mlp_update_sumsq_parts': (C.c_int32, []),
     'pb_peer_buffer_bytes': (C.c_size_t, [C.c_int64]),

@@ -284,18 +284,10 @@ class _DefaultMLPUpdate:
         self.peer_parts = None
         self.head_pack = None
         if self.world > 1 and bool(getattr(data.config, 'peer_allreduce', True)):
-            from pufferlib_b200.distributed import PeerComm
-            ok = torch.ones(1, device=dev)
-            try:
-                self.peer = PeerComm((self.gflat.numel() + 3) // 4 * 4 + 4)
-            except Exception as e:           # every rank must take the same path: agree on it below
-                data.msg = f'peer all-reduce unavailable ({type(e).__name__}: {e}); using NCCL'
-                ok.zero_()
-            torch.distributed.all_reduce(ok, op=torch.distributed.ReduceOp.MIN)
-            if float(ok.item()) == 0.0:
-                if self.peer is not None:
-                    self.peer.close()
-                self.peer = None
+            from pufferlib_b200.distributed import open_peer_comm
+            self.peer, msg = open_peer_comm((self.gflat.numel() + 3) // 4 * 4 + 4, dev)
+            if msg is not None:
+                data.msg = msg
 
     def _current_state_ptrs(self):
         out = []
@@ -970,6 +962,8 @@ def update_plan(data):
     segment views of obs) or 'gathered' (the reference layout: b_obs and the b_* tensors).  capture: 'whole' (ONE graph),
     'segments' (per-segment graphs around an NCCL all-reduce, _SegmentGraphs) or None (eager).  manual: this call's
     _DefaultMLPUpdate (built here, and rebuilt when optimizer.load_state_dict() replaced the Adam state it holds), or None.
+    bptt_peer: the 'bptt' engine on several ranks takes its gradient mean from the peer exchange of data.grad_bucket
+    (GradBucket.open_peer, tried once here) rather than from NCCL.
     Sets data.manual_update, train_minibatch_path, train_recurrent_path and manual.used_fused."""
     config, exp, model = data.config, data.experience, getattr(data.policy, 'policy', None)
     if data.manual_update is not None and data.manual_update.stale():
@@ -1007,12 +1001,21 @@ def update_plan(data):
     else:
         engine, form = 'reference', 'gathered'
 
+    bucket = data.grad_bucket
+    if engine == 'bptt' and bucket is not None and not bucket.peer_tried and bool(getattr(config, 'peer_allreduce', True)):
+        # the recurrent update on several ranks: its gradient mean over NVLink peer memory (pb_peer_allreduce_mean) instead
+        # of NCCL, so that it can be ONE graph like the MLP update's; NCCL stays the fallback (on every rank alike)
+        msg = bucket.open_peer()
+        if msg is not None:
+            data.msg = msg
+    bptt_peer = engine == 'bptt' and bucket is not None and bucket.peer is not None
+
     capture = None
     # target_kl: the stop is decided on the device and skips the later epochs through IF nodes (_KLStop).  On several ranks
     # only the peer exchange carries the KL sum inside the graph; the NCCL plans all-reduce it eagerly between epochs
     kl_ranks = config.target_kl is not None and data.grad_bucket is not None
     if bool(getattr(config, 'cuda_graph_train', getattr(config, 'cuda_graph', False))) and \
-            (not kl_ranks or (manual is not None and manual.peer is not None)) and data.train_graph_state >= 0:
+            (not kl_ranks or (manual is not None and manual.peer is not None) or bptt_peer) and data.train_graph_state >= 0:
         # an NCCL call inside the update loop (autograd path on several ranks, or the hand-written update without peer
         # memory) keeps the update out of ONE graph -- capturing it hung on this stack (torch 2.11 / NCCL 2.28) -- so it
         # is captured in segments around an ordinary all-reduce call; with the peer all-reduce fused into
@@ -1020,14 +1023,14 @@ def update_plan(data):
         nccl_call = data.grad_bucket is not None and (manual is None or manual.peer is None)
         if exp.lstm_h is None:
             capture = 'segments' if nccl_call else 'whole'
-        elif engine == 'bptt' and data.grad_bucket is None:
-            capture = 'whole'           # the cuDNN path and recurrent updates on several ranks stay eager
+        elif engine == 'bptt' and (data.grad_bucket is None or bptt_peer):
+            capture = 'whole'           # the cuDNN path and recurrent updates on several ranks over NCCL stay eager
 
     data.train_minibatch_path = form
     data.train_recurrent_path = {'bptt': 'fused', 'cudnn': 'cudnn'}.get(engine)
     if manual is not None:
         manual.used_fused = engine == 'mlp_fused'
-    return pufferlib_b200.namespace(engine=engine, form=form, capture=capture, manual=manual)
+    return pufferlib_b200.namespace(engine=engine, form=form, capture=capture, manual=manual, bptt_peer=bptt_peer)
 
 
 def _invalidate_policy_cache(data):
@@ -1338,7 +1341,7 @@ def _train_device_part(data, plan, seg=None):
 
     world = manual.world if manual is not None else (data.grad_bucket.world if data.grad_bucket is not None else 1)
     # several ranks with peers: the exchange of each epoch's last optimizer step carries the KL row sum (_KLStop)
-    kl_peer = kl_stop is not None and world > 1 and manual is not None and manual.peer is not None
+    kl_peer = kl_stop is not None and world > 1 and ((manual is not None and manual.peer is not None) or plan.bptt_peer)
 
     def optimizer_step(kl_row=None):
         with profile.learn:
@@ -1356,15 +1359,22 @@ def _train_device_part(data, plan, seg=None):
                         lambda: forward_backward(mb, epoch * n_mb + mb))
             else:
                 forward_backward(mb, epoch * n_mb + mb)
+            last_kl = kl_peer and mb == n_mb - 1 and epoch < config.update_epochs - 1
             if manual is not None:
                 with profile.learn:
                     manual.all_reduce()                         # ONE NCCL all-reduce (sum; 1/world folded into the step)
+            elif plan.bptt_peer:
+                with profile.learn, torch.no_grad():
+                    # ONE peer-exchange kernel per optimizer step; the epoch's last carries this rank's KL row sum, the value
+                    # the NCCL plan all-reduces
+                    kl_in = carry['approx_kl'].double() * experience.minibatch_size if last_kl else None
+                    data.grad_bucket.peer_all_reduce_mean(kl_in, kl_stop.kl_sum if last_kl else None)
             elif data.grad_bucket is not None:
                 with profile.learn:
                     data.grad_bucket.all_reduce_mean()          # ONE NCCL all-reduce per optimizer step
             if seg is not None:
                 seg.run('opt', optimizer_step)
-            elif kl_peer and mb == n_mb - 1 and epoch < config.update_epochs - 1:
+            elif last_kl and manual is not None:
                 optimizer_step(kl_row=epoch * n_mb + mb)
             else:
                 optimizer_step()
@@ -1423,8 +1433,9 @@ def _kl_stop(data):
 
 
 def train(data):
-    """One PPO update (reference: clean_pufferl.py:156-292).  With ``config.cuda_graph`` (recurrent policies only on one
-    GPU with the fused BPTT update; target_kl on several GPUs only with the peer exchange) the device part is captured
+    """One PPO update (reference: clean_pufferl.py:156-292).  With ``config.cuda_graph`` (recurrent policies only with the
+    fused BPTT update, on several GPUs only with its peer exchange; target_kl on several GPUs only with the peer
+    exchange) the device part is captured
     once -- after an eager first call that initialises the optimizer state -- and replayed as ONE graph launch; the
     learning rate lives in a device tensor so annealing works under replay, and the target_kl stop is decided on the
     device (_KLStop), on several ranks once for all of them.
@@ -1529,6 +1540,8 @@ def try_load_checkpoint(data):
     _invalidate_policy_cache(data)
     if data.train_graph_state > 0:      # captured updates hold the old optimizer-state addresses: capture again
         data.train_graph, data.train_segments, data.train_graph_state = None, None, 0
+    if data.grad_bucket is not None and data.grad_bucket.peer is not None:
+        data.grad_bucket.close_peer()   # collective, like the hand-written update's: the next train() maps a fresh one
     print(f'Loaded checkpoint {resume_state["model_name"]}')
 
 
@@ -1539,4 +1552,6 @@ def close(data):
     if mu is not None and getattr(mu, 'peer', None) is not None:
         mu.peer.close()            # collective: every rank closes (unmaps the peers' buffers, then frees its own)
         mu.peer = None
+    if getattr(data, 'grad_bucket', None) is not None:
+        data.grad_bucket.close_peer()
     data.vecenv.close()

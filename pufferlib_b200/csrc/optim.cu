@@ -247,20 +247,6 @@ extern "C" int pb_clip_adam(const pb_adam_tensor* tensors, int32_t n_tensors, fl
                              nullptr, nullptr, 0, stream);
 }
 
-// The checks shared by the _ex forms: both or neither of kl_in / kl_out, 8-byte aligned; with them the communicator has
-// >= 2 ranks and the slot has room for the 4 payload floats after round4(n) gradient floats.
-static int check_payload(const char* who, const pb_peer_comm* comm, int64_t n, const double* kl_in, const double* kl_out) {
-    PB_REQUIRE((kl_in == nullptr) == (kl_out == nullptr), PB_ERR_INVALID, "%s: give both kl_in and kl_out, or neither", who);
-    PB_REQUIRE((uintptr_t)kl_in % 8 == 0 && (uintptr_t)kl_out % 8 == 0, PB_ERR_INVALID, "%s: misaligned kl_in or kl_out", who);
-    if (kl_in) {
-        PB_REQUIRE(comm && comm->world >= 2, PB_ERR_INVALID, "%s: a KL payload needs a communicator of 2 or more ranks", who);
-        PB_REQUIRE(((n + 3) & ~(int64_t)3) + 4 <= comm->capacity, PB_ERR_INVALID,
-                   "%s: no room for the KL payload (round4(%lld) + 4 floats > capacity %lld)", who, (long long)n,
-                   (long long)comm->capacity);
-    }
-    return PB_OK;
-}
-
 static int clip_adam_peer(const char* who, const pb_adam_tensor* tensors, int32_t n_tensors, float max_grad_norm,
                           float grad_scale, float lr, const float* lr_dev, float beta1, float beta2, float eps,
                           float* total_norm_out, const pb_peer_comm* comm, float* grad_flat, int64_t grad_flat_numel,
@@ -301,7 +287,7 @@ static int clip_adam_peer(const char* who, const pb_adam_tensor* tensors, int32_
         a.flat = grad_flat;
         a.flat_n = grad_flat_numel;
     }
-    const int rc = check_payload(who, comm, grad_flat_numel, kl_in, kl_out);
+    const int rc = pb_peer_check_payload(who, comm, grad_flat_numel, kl_in, kl_out);
     if (rc) return rc;
     a.kl_in = kl_in;
     a.kl_out = kl_out;
@@ -407,7 +393,7 @@ static int clip_adam_peer_parts(const char* who, const pb_adam_tensor* tensors, 
                    PB_ERR_INVALID, "%s: bad head-pack arguments", who);
         hp = *pack;
     }
-    const int rc = check_payload(who, comm, grad_flat_numel, kl_in, kl_out);
+    const int rc = pb_peer_check_payload(who, comm, grad_flat_numel, kl_in, kl_out);
     if (rc) return rc;
     a.kl_in = kl_in;
     a.kl_out = kl_out;

@@ -61,7 +61,50 @@ __global__ void __launch_bounds__(1024) k_peer_allreduce(pb_peer_comm c, float* 
 __global__ void __launch_bounds__(512) k_peer_allreduce_slices(pb_peer_comm c, float* flat, int64_t n, double* sumsq) {
     pb_peer_allreduce_slice(c, flat, n, sumsq);
 }
+
+// (one exchange in flight per device: the ticket and the sums of squares nobody reads are module-wide)
+__device__ unsigned int g_mean_ticket = 0;
+__device__ double g_mean_sumsq[PB_PEER_SLICES];
+
+// The sliced exchange, then flat[slice] *= 1/world in the CTA that summed the slice, then the epoch advanced by the last CTA
+// to finish (each read it at its start).  inv_world is 1.f / world rounded on the host: ATen's div_ by a scalar multiplies
+// by that reciprocal, so this is bitwise GradBucket.all_reduce_mean on the same rank-order sum.
+__global__ void __launch_bounds__(512) k_peer_allreduce_mean(pb_peer_comm c, float* flat, int64_t n, float inv_world,
+                                                             const double* kl_in, double* kl_out) {
+    pb_peer_allreduce_slice(c, flat, n, g_mean_sumsq, kl_in, kl_out);
+    __syncthreads();             // this CTA's stores of its summed slice are visible to all its threads
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const int64_t chunk = ((n + PB_PEER_SLICES - 1) / PB_PEER_SLICES + 3) & ~(int64_t)3;   // pb_peer_allreduce_slice's bounds
+    const int64_t lo = (int64_t)blockIdx.x * chunk < n ? (int64_t)blockIdx.x * chunk : n, hi = lo + chunk < n ? lo + chunk : n;
+    for (int64_t i = lo + tid; i < hi; i += nt) flat[i] = __fmul_rn(flat[i], inv_world);
+    if (tid == 0) {
+        __threadfence();
+        if (atomicAdd(&g_mean_ticket, 1u) == gridDim.x - 1) {
+            g_mean_ticket = 0;
+            *c.epoch += 1;
+        }
+    }
+}
 }  // namespace
+
+// In-place MEAN of flat[0..n) over all ranks (every rank must call it the same number of times): the sliced exchange of
+// pb_peer_allreduce_parts (pb_peer_slices() CTAs), scaled by 1/world, advancing the epoch counter itself.  kl_in / kl_out:
+// the optional fp64 payload of pb_clip_adam_peer_parts_ex, summed (not averaged) over the ranks.
+extern "C" int pb_peer_allreduce_mean(const pb_peer_comm* comm, float* flat, int64_t n, const double* kl_in, double* kl_out,
+                                      void* stream) {
+    PB_REQUIRE(comm && flat && n >= 1, PB_ERR_INVALID, "pb_peer_allreduce_mean: bad arguments");
+    PB_REQUIRE(comm->world >= 1 && comm->world <= PB_PEER_MAX_RANKS && comm->rank >= 0 && comm->rank < comm->world &&
+                   comm->epoch && n <= comm->capacity,
+               PB_ERR_INVALID, "pb_peer_allreduce_mean: bad communicator (world %d rank %d capacity %lld, n %lld)", comm->world,
+               comm->rank, (long long)comm->capacity, (long long)n);
+    for (int r = 0; r < comm->world; ++r) PB_REQUIRE(comm->base[r], PB_ERR_INVALID, "pb_peer_allreduce_mean: peer %d not mapped", r);
+    const int rc = pb_peer_check_payload("pb_peer_allreduce_mean", comm, n, kl_in, kl_out);
+    if (rc) return rc;
+    const float inv_world = 1.0f / (float)comm->world;
+    k_peer_allreduce_mean<<<PB_PEER_SLICES, 512, 0, (cudaStream_t)stream>>>(*comm, flat, n, inv_world, kl_in, kl_out);
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
 
 // Sliced form: PB_PEER_SLICES CTAs, each sums one slice over all ranks and leaves the slice's sum of squares in
 // sumsq_parts[0..16).  The epoch counter is advanced by the pb_clip_adam_parts call that must follow in the same stream.

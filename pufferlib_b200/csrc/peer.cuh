@@ -6,6 +6,22 @@
 
 constexpr int PB_PEER_HEADER_BYTES = 1024;   // 8 flag lines of 128 B
 
+// Host check shared by every entry point that takes the optional fp64 payload: both or neither of kl_in / kl_out, 8-byte
+// aligned; with them the communicator has >= 2 ranks and the slot has room for the 4 payload floats after round4(n) gradient
+// floats.
+static inline int pb_peer_check_payload(const char* who, const pb_peer_comm* comm, int64_t n, const double* kl_in,
+                                        const double* kl_out) {
+    PB_REQUIRE((kl_in == nullptr) == (kl_out == nullptr), PB_ERR_INVALID, "%s: give both kl_in and kl_out, or neither", who);
+    PB_REQUIRE((uintptr_t)kl_in % 8 == 0 && (uintptr_t)kl_out % 8 == 0, PB_ERR_INVALID, "%s: misaligned kl_in or kl_out", who);
+    if (kl_in) {
+        PB_REQUIRE(comm && comm->world >= 2, PB_ERR_INVALID, "%s: a KL payload needs a communicator of 2 or more ranks", who);
+        PB_REQUIRE(((n + 3) & ~(int64_t)3) + 4 <= comm->capacity, PB_ERR_INVALID,
+                   "%s: no room for the KL payload (round4(%lld) + 4 floats > capacity %lld)", who, (long long)n,
+                   (long long)comm->capacity);
+    }
+    return PB_OK;
+}
+
 #ifdef __CUDACC__
 __device__ __forceinline__ void pb_st_release_sys_u64(uint64_t* p, uint64_t v) {
     asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");

@@ -7,7 +7,9 @@ gradients are averaged with a single NCCL all-reduce over one flat fp32 bucket (
 is tens of KB for the MLP, 6.7 MB for NatureCNN -- latency-bound, so exactly one collective, no bucketing).
 
 For the hand-written update (clean_pufferl._DefaultMLPUpdate) the exchange is fused into the optimizer kernel over NVLink
-peer memory (``PeerComm`` / csrc/peer.cu): no NCCL call per step, so the update is ONE CUDA graph at any world size.
+peer memory (``PeerComm`` / csrc/peer.cu): no NCCL call per step, so the update is ONE CUDA graph at any world size.  The
+fused recurrent update keeps torch's clip + Adam and takes the gradient mean alone over the same kind of peer memory
+(``GradBucket.open_peer`` / ``peer_all_reduce_mean``, pb_peer_allreduce_mean), so it too is ONE graph on every rank.
 """
 import ctypes as C
 import os
@@ -57,6 +59,21 @@ class GradBucket:
             off += n
         self.params = params
         self.world = dist.get_world_size() if dist.is_initialized() else 1
+        # PeerComm for the flat buffer (open_peer), or None: all_reduce_mean's NCCL call.  peer_tried: open_peer has run
+        self.peer, self.peer_tried = None, False
+
+    def open_peer(self):
+        """Map a PeerComm over the flat buffer, with room for the 4-float KL payload after it (pb_peer_allreduce_mean), on
+        every rank or on none.  Collective; once until close_peer.  -> None, or why peers are unavailable (NCCL then)."""
+        self.peer_tried = True
+        self.peer, msg = open_peer_comm((self.flat.numel() + 3) // 4 * 4 + 4, self.flat.device)
+        return msg
+
+    def close_peer(self):
+        """Collective, like open_peer; the next open_peer maps a fresh communicator."""
+        if self.peer is not None:
+            self.peer.close()
+        self.peer, self.peer_tried = None, False
 
     def zero(self):
         self.rebind()
@@ -79,6 +96,15 @@ class GradBucket:
         if self.world > 1:
             dist.all_reduce(self.flat, op=dist.ReduceOp.SUM)
             self.flat.div_(self.world)
+
+    def peer_all_reduce_mean(self, kl_in=None, kl_out=None):
+        """all_reduce_mean over the peer buffers (open_peer): ONE kernel, no host call, so it can be captured; the same bits
+        as all_reduce_mean on the same rank-order sum.  kl_in / kl_out (both or neither): device fp64 one-element tensors;
+        kl_out <- kl_in summed over the ranks in rank order, carried by the same exchange."""
+        from pufferlib_b200 import _native
+        self.rebind()
+        _native.check(_native.lib().pb_peer_allreduce_mean(C.byref(self.peer.struct), _native.ptr(self.flat), self.flat.numel(),
+                                                           _native.ptr(kl_in), _native.ptr(kl_out), _native.stream_ptr()))
 
 
 def broadcast_parameters(module, src=0):
@@ -145,3 +171,21 @@ class PeerComm:
                 dist.barrier()             # nobody still has the buffer mapped / in use
             lib.pb_peer_free(self._own)
             self._own = None
+
+
+def open_peer_comm(capacity_floats, device):
+    """PeerComm(capacity_floats) on every rank, or None on every rank: all ranks agree through one all-reduce, and those
+    that mapped their peers close them again when any rank could not.  -> (comm or None, why this rank failed or None)."""
+    ok = torch.ones(1, device=device)
+    comm, msg = None, None
+    try:
+        comm = PeerComm(capacity_floats)
+    except Exception as e:           # every rank must take the same path: agree on it below
+        msg = f'peer all-reduce unavailable ({type(e).__name__}: {e}); using NCCL'
+        ok.zero_()
+    dist.all_reduce(ok, op=dist.ReduceOp.MIN)
+    if float(ok.item()) == 0.0:
+        if comm is not None:
+            comm.close()
+        comm = None
+    return comm, msg

@@ -407,6 +407,24 @@ int pb_mlp_tail_backward_ex(const float* dout, int64_t dout_stride, const float*
                             int32_t hidden_size, float* dpre, float* grads_out, void* workspace, size_t workspace_bytes,
                             int32_t head_rows, void* stream);
 
+/* -- NatureCNN conv1 on uint8 frame stacks -----------------------------------------------------------------------------
+ * The first layer of models.Convolutional (pufferlib/models.py:113-157): Conv2d(4, 32, 8, stride=4) + ReLU on
+ * (4, 84, 84) uint8 observations scaled by 1/255, read in place (no fp32 copy of the frames).
+ *   x        m rows of uint8 [4][84][84], row_stride bytes apart (>= 28 224, a multiple of 16; x 16-byte aligned)
+ *   w, b     fp32 [32][256] (k = c*64 + ky*8 + kx; consumed as TF32, rounded with cvt.rna) and [32]
+ *   y        fp32 [m][32][20][20] contiguous: relu(S / 255 + b), S = conv(x, w) on TF32 tensor cores, fp32 accumulation
+ * pb_conv1_u8_wgrad: dz = dy * (y > 0) (threshold_backward), dw [32][256] = sum over rows and pixels of dz * x / 255,
+ * db [32] = sum of dz; dz enters the tensor core as TF32 (cvt.rna), x exactly.  No input gradient.  The row sums are
+ * split over a fixed number of CTAs into fp32 partials in `workspace` (pb_conv1_u8_wgrad_workspace_bytes(m) bytes,
+ * 16-byte aligned) and summed in a fixed order: deterministic.  y and dy 16-byte aligned.
+ * Both: no allocation and no host synchronisation (capturable); PB_ERR_INVALID before any launch for a null or
+ * misaligned pointer, a bad row_stride or a short workspace; m = 0 returns PB_OK without a launch. */
+int pb_conv1_u8_forward(const uint8_t* x, int64_t row_stride, int64_t m, const float* w, const float* b, float* y,
+                        void* stream);
+size_t pb_conv1_u8_wgrad_workspace_bytes(int64_t m);
+int pb_conv1_u8_wgrad(const uint8_t* x, int64_t row_stride, int64_t m, const float* y, const float* dy, float* dw,
+                      float* db, void* workspace, size_t workspace_bytes, void* stream);
+
 /* -- fused minibatch update (forward + PPO loss + backward) -------------------------------------------------------------
  * One minibatch of clean_pufferl.train (clean_pufferl.py:186-244) for models.Default (pufferlib/models.py:12-62) with
  * 128 fp32 input features, 128 hidden units and <= 7 actions, up to and including the gradients, in ONE persistent

@@ -101,6 +101,9 @@ SIGNATURES = {
     'pb_mlp_tail_workspace_bytes_ex': (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32]),
     'pb_mlp_tail_backward_ex': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_size_t, C.c_int32, C.c_void_p]),
+    'pb_conv1_u8_forward': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 3 + [C.c_void_p]),
+    'pb_conv1_u8_wgrad_workspace_bytes': (C.c_size_t, [C.c_int64]),
+    'pb_conv1_u8_wgrad': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]),
     'pb_rollout_breakout_mlp': (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 6 + [C.POINTER(EnvOut)] + [C.c_void_p] * 4 +
                                 [C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
     'pb_rollout_debug_buffers': (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -21,6 +21,7 @@
 #include <type_traits>
 
 #include "pb_common.cuh"
+#include "reduce_partials.cuh"
 #include "tma.cuh"
 
 namespace {
@@ -226,20 +227,6 @@ __global__ void __launch_bounds__(MT_THREADS) k_mlp_tail_bwd(const float* __rest
     tail_reduce<R, VEC, RSTRIDE>(acc_w, acc_b, acc_d, s_red, partials + (int64_t)blockIdx.x * (R * h + h + R), h, col0);
 }
 
-// deterministic second stage: out[j] = sum over blocks of partials[b][j].  One warp per output element: lane l sums
-// blocks l, l+32, ... in order, then a fixed shuffle tree combines the 32 lane sums (same order every run).
-__global__ void __launch_bounds__(256) k_reduce_partials(const float* __restrict__ partials, int n_blocks, int pstride,
-                                                        float* __restrict__ out) {
-    const int lane = threadIdx.x & 31;
-    const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (j >= pstride) return;
-    float s = 0.f;
-    for (int b = lane; b < n_blocks; b += 32) s += partials[(int64_t)b * pstride + j];
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-    if (lane == 0) out[j] = s;
-}
-
 template <int R>
 int launch_tail(const float* dout, int64_t dout_stride, const float* w_heads, const float* hidden, int64_t m, int h,
                 float* dpre, float* workspace, int blocks, cudaStream_t s) {
@@ -295,7 +282,8 @@ extern "C" int pb_mlp_tail_backward_ex(const float* dout, int64_t dout_stride, c
     default: rc = launch_tail<32>(dout, dout_stride, w_heads, hidden, m, hidden_size, dpre, ws, blocks, s); break;
     }
     if (rc != PB_OK) return rc;
-    k_reduce_partials<<<(pstride * 32 + 255) / 256, 256, 0, s>>>((const float*)workspace, blocks, pstride, grads_out);
+    k_reduce_partials<<<(pstride * 32 + 255) / 256, 256, 0, s>>>((const float*)workspace, blocks, pstride, pstride,
+                                                                 grads_out);
     PB_LAUNCH_CHECK();
     return PB_OK;
 }

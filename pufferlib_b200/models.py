@@ -438,12 +438,44 @@ class LSTMWrapper(nn.Module):
         return logits, value, state
 
 
+class _Conv1U8Function(torch.autograd.Function):
+    """relu(conv1(x / 255) + b) of NatureCNN (Conv2d(4, 32, 8, stride=4) on (4, 84, 84) uint8 frame stacks) as one
+    autograd node: pb_conv1_u8_forward reads the uint8 rows in place and writes y [M, 32, 20, 20]; the backward
+    (pb_conv1_u8_wgrad) takes the ReLU's gradient rule and the weight and bias gradients from y, dy and the same bytes.
+    x gets no gradient (conv1 is the first layer), so only y is saved beside it."""
+
+    @staticmethod
+    def forward(ctx, x, w, b):
+        from pufferlib_b200 import _native
+        m = x.shape[0]
+        y = torch.empty(m, 32, 20, 20, dtype=torch.float32, device=x.device)
+        _native.check(_native.lib().pb_conv1_u8_forward(_native.ptr(x), x.stride(0), m, _native.ptr(w), _native.ptr(b),
+                                                        _native.ptr(y), _native.stream_ptr()))
+        ctx.save_for_backward(x, y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from pufferlib_b200 import _native
+        x, y = ctx.saved_tensors
+        dy = dy.contiguous()
+        m, lib = x.shape[0], _native.lib()
+        dw = torch.empty(32, 4, 8, 8, dtype=torch.float32, device=x.device)
+        db = torch.empty(32, dtype=torch.float32, device=x.device)
+        ws = torch.empty(lib.pb_conv1_u8_wgrad_workspace_bytes(m), dtype=torch.uint8, device=x.device)
+        _native.check(lib.pb_conv1_u8_wgrad(_native.ptr(x), x.stride(0), m, _native.ptr(y), _native.ptr(dy),
+                                            _native.ptr(dw), _native.ptr(db), _native.ptr(ws), ws.numel(),
+                                            _native.stream_ptr()))
+        return None, dw, db
+
+
 class Convolutional(nn.Module):
     def __init__(self, env, *args, framestack=4, flat_size=64 * 7 * 7, input_size=512, hidden_size=512,
                  output_size=512, channels_last=False, downsample=1, **kwargs):
         super().__init__()
         self.channels_last = channels_last
         self.downsample = downsample
+        self.fast_path = True     # conv1 + ReLU on the uint8 frames in place (_Conv1U8Function) where _conv1_u8_ok holds
         self.network = nn.Sequential(
             layer_init(nn.Conv2d(framestack, 32, 8, stride=4)), nn.ReLU(),
             layer_init(nn.Conv2d(32, 64, 4, stride=2)), nn.ReLU(),
@@ -458,11 +490,31 @@ class Convolutional(nn.Module):
         hidden, lookup = self.encode_observations(observations)
         return self.decode_actions(hidden, lookup)
 
+    def _conv1_u8_ok(self, x):
+        """Can pb_conv1_u8_forward run the first layer on x?  CUDA uint8 [M, 4, 84, 84] with every row one contiguous
+        frame stack (rows 16-byte aligned), channels-first frames at full resolution, and the stock
+        Conv2d(4, 32, 8, stride=4) + ReLU with fp32 parameters first."""
+        conv = self.network[0]
+        if not (self.fast_path and not self.channels_last and self.downsample == 1 and x.is_cuda
+                and x.dtype == torch.uint8 and x.dim() == 4 and tuple(x.shape[1:]) == (4, 84, 84)
+                and tuple(x.stride()[1:]) == (7056, 84, 1) and x.stride(0) % 16 == 0 and x.data_ptr() % 16 == 0):
+            return False
+        return (type(conv) is nn.Conv2d and type(self.network[1]) is nn.ReLU and conv.in_channels == 4
+                and conv.out_channels == 32 and conv.kernel_size == (8, 8) and conv.stride == (4, 4)
+                and conv.padding == (0, 0) and conv.dilation == (1, 1) and conv.groups == 1
+                and conv.padding_mode == 'zeros' and conv.bias is not None
+                and conv.weight.dtype == conv.bias.dtype == torch.float32 and conv.weight.is_contiguous()
+                and conv.weight.data_ptr() % 16 == 0)
+
     def encode_observations(self, observations):
         if self.channels_last:
             observations = observations.permute(0, 3, 1, 2)
         if self.downsample > 1:
             observations = observations[:, :, ::self.downsample, ::self.downsample]
+        if observations.shape[0] > 0 and self._conv1_u8_ok(observations):
+            conv = self.network[0]
+            y1 = _Conv1U8Function.apply(observations, conv.weight, conv.bias)
+            return self.network[2:](y1), None
         return self.network(observations.float() / 255.0), None
 
     def decode_actions(self, flat_hidden, lookup, concat=None):

@@ -21,9 +21,11 @@
 //     from shared memory as the K-major B operand); the accumulator stays in registers across all tiles of the CTA.
 // The tensor core works one tile ahead of the epilogue: at the end of tile it, the forward product of tile it + 1 is issued
 // first and the dW_enc product of tile it after it; tile it + 1 waits only for its forward (wgmma_wait<1>), so the dW_enc
-// product runs under the epilogue of tile it + 1 and is retired just before the next one is issued.  That takes two
+// product runs under the epilogue of tile it + 1 and is retired after that tile's head products.  That takes two
 // relu(h)^T / dPre^T buffers (tile it uses buffer it & 1) and keeps the x^T fragments of the product in flight in
-// registers; the x ring has two stages so that shared memory still fits.  Neither accumulator is written by anything but
+// registers; the x ring has two stages so that shared memory still fits.  The x^T fragments of tile it + 1 are loaded
+// right after that retirement, under the loss row math, so the barrier before the products is also the last one before
+// the x stage is refilled: a tile has five CTA-wide barriers.  Neither accumulator is written by anything but
 // wgmma between issue and wait (the first product into each has scale-d 0), so ptxas keeps the products asynchronous.
 // Per-CTA partials go to a workspace and k_update_reduce sums them deterministically into the flat gradient buffer
 // [dW_enc (hid x feat) | dW_heads (8 x hid) | db_enc | db_heads] of clean_pufferl._DefaultMLPUpdate, leaving per-block
@@ -96,10 +98,10 @@ struct FusedParams {
 #endif
 };
 #ifdef PB_UPDATE_PHASES
-constexpr int PH_TILES = 32, PH_N = 8;                 // [grid][warpgroups][PH_TILES][PH_N] clock64 stamps
+constexpr int PH_TILES = 32, PH_N = 11;                // [grid][warpgroups][PH_TILES][PH_N] clock64 stamps
 #define PB_PHASE(k, idx)                                                                                               \
     do {                                                                                                               \
-        if (p.phases && (tid & 127) == 0 && (k) < PH_TILES)                                                            \
+        if (p.phases && (tid & 127) == 0 && (k) >= 0 && (k) < PH_TILES)                                                \
             p.phases[(((int64_t)blockIdx.x * (THREADS / 128) + (tid >> 7)) * PH_TILES + (k)) * PH_N + (idx)] = clock64(); \
     } while (0)
 #else
@@ -252,11 +254,12 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
 
     // ---- 1. hidden^T = W_enc[64wg .. 64wg + 63] . x^T  (M = hidden units, N = 64 rows, K = 128 features), issued one
     //         tile ahead: the forward of tile it + 1 goes to the tensor core before the dW_enc product of tile it, and
-    //         that product completes under the epilogue of tile it + 1 (retired by the wgmma_wait<0> of step 6)
+    //         that product completes under the epilogue of tile it + 1 (retired by the wgmma_wait<0> after its heads)
     float h[32];
     auto forward = [&](int it) {
         const int s = it % NSTAGE;
         mbar_wait(&x_full[s], (uint32_t)((it / NSTAGE) & 1));
+        PB_PHASE(it - 1, 8);             // stamped for the tile whose step 6 issues this forward (none for tile 0)
         const uint32_t x_addr = smem_u32(smem + SM_X + s * X_TILE_BYTES);
         wgmma_fence();                   // the first wgmma has scale-d 0: h needs no zeroing
 #pragma unroll
@@ -350,6 +353,27 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
         __syncthreads();
         PB_PHASE(it, 3);
 
+        // ---- x^T fragments of this tile's dW_enc product (step 6), loaded here so that their latency hides under the
+        //      loss row math, and so that every read of x stage s is done before the barrier of step 6.  The previous
+        //      tile's dW_enc product (issued at the end of that tile, long finished) is retired first: its A registers
+        //      are overwritten here and its relu(h)^T / dPre^T buffer is the one the next tile writes.  Both operands are
+        //      rounded to nearest TF32 (truncation would bias a sum over the whole minibatch).
+        wgmma_wait<0>();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
+        const int f0 = 64 * wg + 16 * wq + g;
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks) {
+            const int r0 = 8 * ks + t;
+            xa[ks][0] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0)));
+            xa[ks][1] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0 + 8)));
+            xa[ks][2] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0)));
+            xa[ks][3] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0 + 8)));
+        }
+        PB_PHASE(it, 4);
+
         // ---- 4. the loss row math -> dOut of the tile
         {
             float z_lo = bh_lo + outp[lr * NO + sub], z_hi = bh_hi + outp[lr * NO + sub + 4];
@@ -373,7 +397,7 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
             }
         }
         __syncthreads();
-        PB_PHASE(it, 4);
+        PB_PHASE(it, 5);
 
         // ---- 5. g^T = W_heads^T dOut^T (same fragment layout as hidden^T), dPre^T = g^T where relu(h) > 0, db_enc, and
         //         dW_heads^T += relu(h)^T dOut with the hidden^T registers as the A fragments (k = t <-> row 8j + 2t,
@@ -406,38 +430,25 @@ k_mlp_update(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
             *reinterpret_cast<uint2*>(gbuf + g_off(hr1, l)) = make_uint2(to_tf32(dp[4 * j + 2]), to_tf32(dp[4 * j + 3]));
         }
 
-        // ---- 6. dW_enc^T [64wg .. 64wg + 63][128] += x^T . dPre  (M = features, N = hidden units, K = 64 rows).  Both
-        //         operands are rounded to nearest TF32 (truncation would bias a sum over the whole minibatch)
-        PB_PHASE(it, 5);
+        // ---- 6. dW_enc^T [64wg .. 64wg + 63][128] += x^T . dPre  (M = features, N = hidden units, K = 64 rows)
+        PB_PHASE(it, 6);
         fence_proxy_async_smem();                // dPre^T written by the generic proxy, read by the tensor core
-        wgmma_wait<0>();                         // the previous tile's dW_enc product: its A registers and buffer are free
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks)
-#pragma unroll
-            for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(xa[ks][i])::"memory");
-        __syncthreads();                         // dPre^T of both warpgroups is in the buffer
-        if (it + 1 < n_my) forward(it + 1);
-        const int f0 = 64 * wg + 16 * wq + g;
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {
-            const int r0 = 8 * ks + t;
-            xa[ks][0] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0)));
-            xa[ks][1] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0, f0 + 8)));
-            xa[ks][2] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0)));
-            xa[ks][3] = to_tf32(*reinterpret_cast<const float*>(xs + x_off(r0 + 4, f0 + 8)));
+        __syncthreads();                         // dPre^T of both warpgroups is in the buffer; every read of x stage s
+                                                 // (the forward of tile it, the x^T fragments) is done
+        if (tid == 0 && it + NSTAGE < n_my) {
+            fence_proxy_async_smem();
+            issue(it + NSTAGE);
         }
+        PB_PHASE(it, 7);
+        if (it + 1 < n_my) forward(it + 1);
+        PB_PHASE(it, 9);
         wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < 8; ++ks)
             wgmma_m64n128k8_rs(dwacc, xa[ks], wgmma_desc_sw128(g_addr + (ks >> 2) * G_KBLK_BYTES + (ks & 3) * 32),
                                (it | ks) ? 1 : 0);
         wgmma_commit();
-        PB_PHASE(it, 6);
-        __syncthreads();                         // every read of x stage s is done
-        if (tid == 0 && it + NSTAGE < n_my) {
-            fence_proxy_async_smem();
-            issue(it + NSTAGE);
-        }
+        PB_PHASE(it, 10);
     }
     // the last tile's dW_enc product
     wgmma_wait<0>();
@@ -549,9 +560,9 @@ extern "C" int32_t pb_mlp_update_phase_layout(int32_t* tiles, int32_t* n) {
 // what each warpgroup's stamps delimit (one comma-separated list per warpgroup, ';' between warpgroups): phase i runs from
 // stamp i to stamp i + 1, the last one to the next tile's stamp 0
 extern "C" const char* pb_mlp_update_phase_names(void) {
-#define PB_PHASE_NAMES "forward wgmma wait,bias + ReLU store + barrier,head products + barrier,loss rows + barrier," \
-                       "g^T / dPre^T / dW_heads,previous dW_enc wait + barrier + next forward + dW_enc issue," \
-                       "barrier + refill + next row loads"
+#define PB_PHASE_NAMES "forward wgmma wait,bias + ReLU store + barrier,head products + barrier," \
+                       "previous dW_enc wait + x^T fragment loads,loss rows + barrier,g^T / dPre^T / dW_heads," \
+                       "barrier + refill,next x wait,next forward issue,dW_enc issue,next row loads"
     return PB_PHASE_NAMES ";" PB_PHASE_NAMES;
 #undef PB_PHASE_NAMES
 }

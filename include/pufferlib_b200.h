@@ -53,7 +53,10 @@ enum {
     /* the reference's ocean test envs (environments/ocean/ocean.py; creators environment.py:33-46, 67-70) */
     PB_ENV_MEMORY = 4, PB_ENV_PASSWORD = 5, PB_ENV_STOCHASTIC = 6, PB_ENV_BANDIT = 7,
     /* two PettingZoo agents per env (ocean.py:149-208 behind PettingZooPufferEnv, emulation.py:236-420) */
-    PB_ENV_MULTIAGENT = 8
+    PB_ENV_MULTIAGENT = 8,
+    /* breakout (PB_ENV_BREAKOUT's game) seen as the reference's Atari breakout is: a (4, 84, 84) uint8 frame stack,
+       oldest frame first, for the NatureCNN (environments/atari/environment.py:37-39, atari/torch.py:8-10) */
+    PB_ENV_BREAKOUT_PIXELS = 9
 };
 enum { PB_DTYPE_F32 = 0, PB_DTYPE_U8 = 1 };
 
@@ -76,7 +79,8 @@ typedef struct {
                                  STOCHASTIC: no iparam; p is dparam[0]; episodes are 100 steps  ocean.py:529-582
                                  BANDIT  : [0]=num_actions in [1, 32768] (default 10)   ocean.py:8-62
                                  MULTIAGENT: no parameters (any non-zero iparam or any dparam is refused)
-                                                                                        ocean.py:149-208 */
+                                                                                        ocean.py:149-208
+                                 BREAKOUT_PIXELS: [0]=max_ticks (default 4096), as BREAKOUT */
 } pb_env_config;
 
 typedef struct {

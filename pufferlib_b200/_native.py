@@ -13,7 +13,7 @@ SO_PATH = os.environ.get('PUFFERLIB_B200_SO', os.path.join(HERE, 'libpuffer_b200
 
 PB_OK, PB_ERR_INVALID, PB_ERR_CUDA, PB_ERR_STATE, PB_ERR_UNSUPPORTED = 0, -1, -2, -3, -4
 ENV_KINDS = {'squared': 0, 'breakout': 1, 'snake': 2, 'pong': 3, 'memory': 4, 'password': 5, 'stochastic': 6, 'bandit': 7,
-             'multiagent': 8}
+             'multiagent': 8, 'breakout_pixels': 9}
 DTYPE_F32, DTYPE_U8 = 0, 1
 
 

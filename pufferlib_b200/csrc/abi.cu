@@ -69,7 +69,7 @@ extern "C" int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_h
     PB_REQUIRE(n_dparam >= 0 && (n_dparam == 0 || dparam_host), PB_ERR_INVALID, "pb_env_create_ex: bad dparam");
     *out = nullptr;
     PB_REQUIRE(cfg->num_envs >= 1, PB_ERR_INVALID, "num_envs must be at least 1");  // vector.py:578-579
-    PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_MULTIAGENT, PB_ERR_INVALID, "unknown env kind %d",
+    PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_BREAKOUT_PIXELS, PB_ERR_INVALID, "unknown env kind %d",
                cfg->kind);
     int ndev = 0;
     PB_CUDA(cudaGetDeviceCount(&ndev));
@@ -87,6 +87,7 @@ extern "C" int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_h
             case PB_ENV_BREAKOUT: rc = pb_breakout_create(env); break;
             case PB_ENV_SNAKE: rc = pb_snake_create(env); break;
             case PB_ENV_PONG: rc = pb_pong_create(env); break;
+            case PB_ENV_BREAKOUT_PIXELS: rc = pb_breakout_pixels_create(env); break;
             default: rc = pb_ocean_create(env, dparam_host, n_dparam); break;
         }
     }

@@ -50,6 +50,7 @@ int pb_squared_create(pb_env* env);
 int pb_breakout_create(pb_env* env);
 int pb_snake_create(pb_env* env);
 int pb_pong_create(pb_env* env);
+int pb_breakout_pixels_create(pb_env* env);
 int pb_ocean_create(pb_env* env, const double* dparam, int n_dparam);   // memory, password, stochastic, bandit,
                                                                          // multiagent
 

@@ -5,20 +5,12 @@
 // environments/test/mock_environments.py:211) and so are the vectoriser / EpisodeStats conventions
 // (vector.py:147-151, emulation.py:187-192, postprocess.py:22-54).  Bit-exact against oracle/csrc/envs.c.
 //
-// The 28,224-byte observation row is moved by the TMA engine, never by the LSU: per env one cp.async.bulk pulls
-// the three surviving frames of row t-1 (21,168 B) into a shared-memory stage while the CTA renders the new 84x84
-// frame into the same stage (zero fill + 52 pixel stores), then ONE cp.async.bulk pushes the whole 28,224 B row to
-// row t.  A ring of 4 stages per CTA keeps 4 envs in flight; 2 CTAs per SM.  Per-env state is 12 B of SoA.
+// The 28,224-byte observation rows are written by the TMA frame-stack ring of frame_stack.cuh; this file is the game:
+// the integer dynamics and the renderer (zero fill + 52 pixel stores).  Per-env state is 12 B of SoA.
 #include "env_common.cuh"
-#include "tma.cuh"
+#include "frame_stack.cuh"
 
 namespace {
-
-constexpr int PG_STAGES = 4;
-constexpr uint32_t FRAME = 84 * 84;        // 7056 = 441 * 16
-constexpr uint32_t ROW = 4 * FRAME;        // 28224
-constexpr uint32_t STAGE_BYTES = 28672;    // ROW rounded up to 1 KiB
-constexpr int PG_THREADS = 128;
 
 struct PongState {
     uint32_t* s0;   // ly(8) | ry(8)<<8 | (bx+2)(8)<<16 | (by)(8)<<24
@@ -26,17 +18,6 @@ struct PongState {
     uint32_t* ctr;
     uint64_t seed;
     int max_score, max_ticks;
-};
-
-struct PgOut {
-    unsigned char* obs;
-    int64_t stride;
-    float* rewards;
-    uint8_t* terminals;
-    uint8_t* truncations;
-    uint8_t* masks;
-    float* dones_f32;
-    bool write_const;
 };
 
 struct PongEnv {
@@ -52,85 +33,49 @@ __device__ __forceinline__ void pong_serve(PongEnv& s, uint64_t seed_e) {
     s.vy = (int)((r >> 1) % 5u) - 2;
 }
 
-// MODE 0: async_reset;  MODE 1: vectoriser send
-template <int MODE>
-__global__ void __launch_bounds__(PG_THREADS) k_pong(PongState st, int n, const int64_t* __restrict__ actions,
-                                                    uint8_t* done, const unsigned char* __restrict__ prev,
-                                                    int64_t prev_stride, PgOut out, EpisodeAcc acc) {
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ uint64_t bars[PG_STAGES];
-    const int tid = threadIdx.x;
-    const int64_t step = gridDim.x;
-    uint32_t phase[PG_STAGES] = {0, 0, 0, 0};
+// the game behind the frame-stack ring (frame_stack.cuh)
+struct PongGame {
+    using State = PongState;
+    using Env = PongEnv;
 
-    auto needs_load = [&](int64_t e) -> bool { return MODE == 1 && done[e] == 0; };
-    auto issue_load = [&](int s, int64_t e) {  // thread 0 only
-        if (needs_load(e)) {
-            mbar_expect_tx(&bars[s], 3 * FRAME);
-            tma_load_1d(smem + (size_t)s * STAGE_BYTES, prev + e * prev_stride + FRAME, 3 * FRAME, &bars[s]);
-        }
-    };
-
-    if (tid == 0) {
-        for (int s = 0; s < PG_STAGES; ++s) mbar_init(&bars[s], 1);
-        mbar_fence_init();
-        int64_t e = blockIdx.x;
-        for (int s = 0; s < PG_STAGES && e < n; ++s, e += step) issue_load(s, e);
+    static __device__ __forceinline__ void reset(const State& st, int64_t e, uint64_t seed_e, bool keep_ctr, Env& p) {
+        p.ctr = keep_ctr ? st.ctr[e] : 0u;
+        p.ly = 36; p.ry = 36; p.score_l = 0; p.score_r = 0; p.tick = 0;
+        pong_serve(p, seed_e);
     }
-    __syncthreads();
 
-    int it = 0;
-    for (int64_t e = blockIdx.x; e < n; e += step, ++it) {
-        const int s = it % PG_STAGES;
-        unsigned char* buf = smem + (size_t)s * STAGE_BYTES;
-        unsigned char* frame = buf + 3 * FRAME;
-        // refill the stage that was stored one iteration ago: by now its bulk store has long read shared memory, so
-        // this wait does not stall, and the load gets PG_STAGES - 1 iterations of lead time
-        if (tid == 0 && it > 0) {
-            const int64_t e_next = e + step * (PG_STAGES - 1);
-            if (e_next < n) {
-                tma_wait_read<0>();
-                issue_load((it - 1) % PG_STAGES, e_next);
-            }
+    static __device__ __forceinline__ void step(const State& st, int64_t e, int64_t action, uint64_t seed_e, Env& p,
+                                                float& reward, bool& terminal, float& score) {
+        const uint32_t a0 = st.s0[e], a1 = st.s1[e];
+        p.ly = a0 & 0xff; p.ry = (a0 >> 8) & 0xff; p.bx = (int)((a0 >> 16) & 0xff) - 2; p.by = (a0 >> 24) & 0xff;
+        p.vx = (int)(a1 & 7) - 2; p.vy = (int)((a1 >> 3) & 7) - 2;
+        p.score_l = (a1 >> 6) & 15; p.score_r = (a1 >> 10) & 15; p.tick = a1 >> 16;
+        p.ctr = st.ctr[e];
+        int a = (int)action;
+        a = a < 0 ? 0 : (a > 5 ? 5 : a);
+        // dy+3 per action, 3 bits each: NOOP, FIRE -> 0; UP(2,4) -> -3; DOWN(3,5) -> +3   (oracle/SPEC.md §Pong)
+        p.ry = min(max(p.ry + (int)((0x30C1Bu >> (3 * a)) & 7u) - 3, 0), 72);
+        const int tgt = min(max(p.by - 5, 0), 72);
+        if (p.ly < tgt) p.ly = min(p.ly + 2, tgt);
+        else if (p.ly > tgt) p.ly = max(p.ly - 2, tgt);
+        p.bx += p.vx; p.by += p.vy;
+        if (p.by < 0) { p.by = -p.by; p.vy = -p.vy; }
+        if (p.by > 82) { p.by = 164 - p.by; p.vy = -p.vy; }
+        if (p.vx > 0 && p.bx >= 76 && p.bx <= 78 && p.by + 2 > p.ry && p.by < p.ry + 12) {
+            p.vx = -2; p.bx = 76; p.vy = (p.by + 1 - p.ry - 6) / 3;
+        } else if (p.vx < 0 && p.bx >= 4 && p.bx <= 6 && p.by + 2 > p.ly && p.by < p.ly + 12) {
+            p.vx = 2; p.bx = 6; p.vy = (p.by + 1 - p.ly - 6) / 3;
         }
-        // ---- integer physics, computed redundantly by every thread (same inputs: broadcast loads)
-        const uint64_t seed_e = st.seed + (uint64_t)e;
-        PongEnv p;
-        float reward = 0.f;
-        bool terminal = false;
-        const bool loaded = needs_load(e);     // false -> this row is a reset row
-        if (!loaded) {
-            p.ctr = (MODE == 1) ? st.ctr[e] : 0u;
-            p.ly = 36; p.ry = 36; p.score_l = 0; p.score_r = 0; p.tick = 0;
-            pong_serve(p, seed_e);
-        } else {
-            const uint32_t a0 = st.s0[e], a1 = st.s1[e];
-            p.ly = a0 & 0xff; p.ry = (a0 >> 8) & 0xff; p.bx = (int)((a0 >> 16) & 0xff) - 2; p.by = (a0 >> 24) & 0xff;
-            p.vx = (int)(a1 & 7) - 2; p.vy = (int)((a1 >> 3) & 7) - 2;
-            p.score_l = (a1 >> 6) & 15; p.score_r = (a1 >> 10) & 15; p.tick = a1 >> 16;
-            p.ctr = st.ctr[e];
-            int a = (int)actions[e];
-            a = a < 0 ? 0 : (a > 5 ? 5 : a);
-            // dy+3 per action, 3 bits each: NOOP, FIRE -> 0; UP(2,4) -> -3; DOWN(3,5) -> +3   (oracle/SPEC.md §Pong)
-            p.ry = min(max(p.ry + (int)((0x30C1Bu >> (3 * a)) & 7u) - 3, 0), 72);
-            const int tgt = min(max(p.by - 5, 0), 72);
-            if (p.ly < tgt) p.ly = min(p.ly + 2, tgt);
-            else if (p.ly > tgt) p.ly = max(p.ly - 2, tgt);
-            p.bx += p.vx; p.by += p.vy;
-            if (p.by < 0) { p.by = -p.by; p.vy = -p.vy; }
-            if (p.by > 82) { p.by = 164 - p.by; p.vy = -p.vy; }
-            if (p.vx > 0 && p.bx >= 76 && p.bx <= 78 && p.by + 2 > p.ry && p.by < p.ry + 12) {
-                p.vx = -2; p.bx = 76; p.vy = (p.by + 1 - p.ry - 6) / 3;
-            } else if (p.vx < 0 && p.bx >= 4 && p.bx <= 6 && p.by + 2 > p.ly && p.by < p.ly + 12) {
-                p.vx = 2; p.bx = 6; p.vy = (p.by + 1 - p.ly - 6) / 3;
-            }
-            if (p.bx < 0) { p.score_r += 1; reward = 1.f; pong_serve(p, seed_e); }
-            else if (p.bx > 82) { p.score_l += 1; reward = -1.f; pong_serve(p, seed_e); }
-            p.tick += 1;
-            terminal = p.score_l >= st.max_score || p.score_r >= st.max_score || p.tick >= st.max_ticks;
-        }
-        // ---- render the new frame into the stage: zero fill, then opponent paddle, agent paddle, ball
-        for (int k = tid; k < (int)(FRAME / 16); k += PG_THREADS) reinterpret_cast<uint4*>(frame)[k] = make_uint4(0, 0, 0, 0);
+        if (p.bx < 0) { p.score_r += 1; reward = 1.f; pong_serve(p, seed_e); }
+        else if (p.bx > 82) { p.score_l += 1; reward = -1.f; pong_serve(p, seed_e); }
+        p.tick += 1;
+        terminal = p.score_l >= st.max_score || p.score_r >= st.max_score || p.tick >= st.max_ticks;
+        score = (float)(p.score_r - p.score_l);
+    }
+
+    // zero fill, then opponent paddle, agent paddle, ball
+    static __device__ __forceinline__ void render(const Env& p, unsigned char* frame, int tid) {
+        for (int k = tid; k < (int)(FS_FRAME / 16); k += FS_THREADS) reinterpret_cast<uint4*>(frame)[k] = make_uint4(0, 0, 0, 0);
         __syncthreads();
         if (tid < 24) frame[(p.ly + (tid >> 1)) * 84 + 4 + (tid & 1)] = 128;
         else if (tid < 48) frame[(p.ry + ((tid - 24) >> 1)) * 84 + 78 + (tid & 1)] = 192;
@@ -139,71 +84,26 @@ __global__ void __launch_bounds__(PG_THREADS) k_pong(PongState st, int n, const 
             const int x = p.bx + (tid & 1), y = p.by + (tid >> 1);
             if (x >= 0 && x < 84 && y >= 0 && y < 84) frame[y * 84 + x] = 255;
         }
-        fence_proxy_async_smem();
-        __syncthreads();
-        // ---- thread 0: bookkeeping + the bulk stores
-        if (tid == 0) {
-            st.s0[e] = (uint32_t)p.ly | ((uint32_t)p.ry << 8) | ((uint32_t)(p.bx + 2) << 16) | ((uint32_t)p.by << 24);
-            st.s1[e] = (uint32_t)(p.vx + 2) | ((uint32_t)(p.vy + 2) << 3) | ((uint32_t)p.score_l << 6) |
-                       ((uint32_t)p.score_r << 10) | ((uint32_t)p.tick << 16);
-            st.ctr[e] = p.ctr;
-            done[e] = terminal ? 1 : 0;
-            out.rewards[e] = reward;
-            out.terminals[e] = terminal ? 1 : 0;
-            if (out.write_const) out.truncations[e] = 0;
-            if (out.write_const) out.masks[e] = 1;
-            if (out.dones_f32) out.dones_f32[e] = terminal ? 1.f : 0.f;
-            // EpisodeStats (postprocess.py:22-54), scalar form
-            if (!loaded) { acc.ep_return[e] = 0.0; acc.ep_length[e] = 0; }
-            else {
-                const double ret = acc.ep_return[e] + (double)reward;
-                const int len = acc.ep_length[e] + 1;
-                acc.ep_return[e] = ret; acc.ep_length[e] = len;
-                if (terminal) {
-                    const float score = (float)(p.score_r - p.score_l);
-                    acc.row_return[e] = ret; acc.row_length[e] = len; acc.row_score[e] = score;
-                    double* slot = acc.stats + 4 * (blockIdx.x & (PB_STAT_SLOTS - 1));
-                    atomicAdd(slot + 0, 1.0); atomicAdd(slot + 1, ret);
-                    atomicAdd(slot + 2, (double)len); atomicAdd(slot + 3, (double)score);
-                }
-            }
-            unsigned char* row = out.obs + e * out.stride;
-            if (loaded) {
-                mbar_wait(&bars[s], phase[s]);     // the three old frames have landed
-                tma_store_1d(row, buf, ROW);
-            } else {
-                for (int k = 0; k < 4; ++k) tma_store_1d(row + (size_t)k * FRAME, frame, FRAME);
-            }
-            tma_commit();
-        }
-        if (loaded) phase[s] ^= 1;
-        // no trailing barrier: the next iteration uses another stage; this stage is refilled by thread 0 at the top of
-        // the next iteration (after wait_read) and rendered into PG_STAGES iterations later, behind block barriers
     }
-    if (tid == 0) tma_wait_all<0>();
+
+    static __device__ __forceinline__ void store(const State& st, int64_t e, const Env& p) {
+        st.s0[e] = (uint32_t)p.ly | ((uint32_t)p.ry << 8) | ((uint32_t)(p.bx + 2) << 16) | ((uint32_t)p.by << 24);
+        st.s1[e] = (uint32_t)(p.vx + 2) | ((uint32_t)(p.vy + 2) << 3) | ((uint32_t)p.score_l << 6) |
+                   ((uint32_t)p.score_r << 10) | ((uint32_t)p.tick << 16);
+        st.ctr[e] = p.ctr;
+    }
+};
+
+// MODE 0: async_reset;  MODE 1: vectoriser send
+template <int MODE>
+__global__ void __launch_bounds__(FS_THREADS) k_pong(PongState st, int n, const int64_t* __restrict__ actions,
+                                                    uint8_t* done, const unsigned char* __restrict__ prev,
+                                                    int64_t prev_stride, FsOut out, EpisodeAcc acc) {
+    frame_stack_run<MODE, PongGame>(st, n, actions, done, prev, prev_stride, out, acc);
 }
 
 int pong_launch(pb_env* env, int mode, const int64_t* actions, const pb_env_out* out, cudaStream_t s) {
-    PongState* st = (PongState*)env->kind;
-    const int n = env->cfg.num_envs;
-    PB_REQUIRE(out->obs_stride % 16 == 0 && ((uintptr_t)out->obs & 15) == 0, PB_ERR_INVALID,
-               "pong: obs pointer/stride must be 16-byte aligned");
-    PgOut o{(unsigned char*)out->obs, out->obs_stride, out->rewards, out->terminals, out->truncations, out->masks,
-            out->dones_f32,
-            env->write_const};
-    int grid = PB_NUM_SMS * 2;
-    if (grid > n) grid = n;
-    const size_t smem = (size_t)PG_STAGES * STAGE_BYTES;
-    if (mode == 0) {
-        PB_CUDA(cudaFuncSetAttribute(k_pong<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_pong<0><<<grid, PG_THREADS, smem, s>>>(*st, n, actions, env->d_done, nullptr, 0, o, pb_episode_acc(env));
-    } else {
-        PB_CUDA(cudaFuncSetAttribute(k_pong<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_pong<1><<<grid, PG_THREADS, smem, s>>>(*st, n, actions, env->d_done, (const unsigned char*)env->cur_obs,
-                                                 env->cur_obs_stride, o, pb_episode_acc(env));
-    }
-    PB_LAUNCH_CHECK();
-    return PB_OK;
+    return fs_launch(env, mode, *(PongState*)env->kind, actions, out, s, k_pong<0>, k_pong<1>, "pong");
 }
 
 int pong_reset(pb_env* env, uint64_t seed, const pb_env_out* out, cudaStream_t s) {
@@ -248,7 +148,7 @@ int pb_pong_create(pb_env* env) {
     env->info.obs_shape[0] = 4;
     env->info.obs_shape[1] = 84;
     env->info.obs_shape[2] = 84;
-    env->info.obs_bytes = ROW;
+    env->info.obs_bytes = FS_ROW;
     env->info.num_actions = 6;
     env->info.obs_low = 0.f;
     env->info.obs_high = 255.f;

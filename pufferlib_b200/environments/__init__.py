@@ -16,7 +16,7 @@ from pufferlib_b200.exceptions import APIUsageError
 
 KNOWN_BY_NAME = {'make_squared': 'squared', 'make_breakout': 'breakout', 'make_snake': 'snake', 'make_pong': 'pong',
                  'make_memory': 'memory', 'make_password': 'password', 'make_stochastic': 'stochastic',
-                 'make_bandit': 'bandit', 'make_multiagent': 'multiagent'}
+                 'make_bandit': 'bandit', 'make_multiagent': 'multiagent', 'make_breakout_pixels': 'breakout_pixels'}
 
 # Kinds whose reference env draws from a process-global RNG stream (CPython's `random` for squared, numpy's
 # `np.random` for memory and bandit): their results depend on which envs share a process, so the B200 backend gives
@@ -92,6 +92,11 @@ def resolve_config(creator, args, kwargs):
         iparam[0] = int(kwargs.pop('max_ticks', 0))
     elif kind == 'snake':
         iparam[0] = int(kwargs.pop('max_ticks', 0))
+    elif kind == 'breakout_pixels':
+        if args:
+            raise APIUsageError(f'breakout_pixels: takes max_ticks as a keyword only, got args {list(args)}')
+        if 'max_ticks' in kwargs:      # the tick counter is 16 bits of the packed state
+            iparam[0] = _int_in(kind, 'max_ticks', kwargs.pop('max_ticks'), 1, 65535)
     elif kind == 'pong':
         iparam[0] = int(kwargs.pop('max_score', 0))
         iparam[1] = int(kwargs.pop('max_ticks', 0))

@@ -429,6 +429,30 @@ size_t pb_conv1_u8_wgrad_workspace_bytes(int64_t m);
 int pb_conv1_u8_wgrad(const uint8_t* x, int64_t row_stride, int64_t m, const float* y, const float* dy, float* dw,
                       float* db, void* workspace, size_t workspace_bytes, void* stream);
 
+/* -- NatureCNN conv2 and conv3 -----------------------------------------------------------------------------------------
+ * The second and third layers of models.Convolutional, each Conv2d + ReLU on fp32 NCHW rows, `layer` = 2 or 3:
+ *   layer 2: x [m][32][20][20] (conv1's y), w [64][32][4][4], stride 2 -> y [m][64][9][9]
+ *   layer 3: x [m][64][9][9],              w [64][64][3][3], stride 1 -> y [m][64][7][7]
+ * Every tensor contiguous; w in the stock [64][C_in][KS][KS] order (k = c * KS^2 + ky * KS + kx), b [64].
+ * pb_nature_conv_forward: y = relu(conv(x, w) + b); x and w enter TF32 tensor cores rounded with cvt.rna, fp32
+ *   accumulation, then the bias and the ReLU in fp32.
+ * pb_nature_conv_dgrad: dz = dy * (y > 0) (threshold_backward, never written), dx = conv_transpose(dz, w) [m][C_in][H][H];
+ *   dz and w rounded to TF32 (cvt.rna), fp32 accumulation; every dx element written once (no atomics).
+ * pb_nature_conv_wgrad: dw [64][C_in][KS][KS] = sum over rows and pixels of dz * im2col(x), db [64] = sum of dz; dz and x
+ *   enter the tensor cores as TF32 (cvt.rna), db sums fp32 dz.  The rows are split over a fixed number of CTAs into fp32
+ *   partials in `workspace` (pb_nature_conv_wgrad_workspace_bytes(layer, m) bytes; 0 for a bad layer) and summed in a
+ *   fixed order: deterministic.
+ * All: no allocation and no host synchronisation (capturable); PB_ERR_INVALID before any launch for a bad layer, a
+ * negative m, a null or misaligned pointer (x, y, dy, dx, w, workspace 16-byte aligned; b, dw, db 4-byte aligned) or a
+ * short workspace; m = 0 returns PB_OK without a launch. */
+int pb_nature_conv_forward(int32_t layer, const float* x, int64_t m, const float* w, const float* b, float* y,
+                           void* stream);
+int pb_nature_conv_dgrad(int32_t layer, const float* y, const float* dy, const float* w, int64_t m, float* dx,
+                         void* stream);
+size_t pb_nature_conv_wgrad_workspace_bytes(int32_t layer, int64_t m);
+int pb_nature_conv_wgrad(int32_t layer, const float* x, const float* y, const float* dy, int64_t m, float* dw, float* db,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 /* -- fused minibatch update (forward + PPO loss + backward) -------------------------------------------------------------
  * One minibatch of clean_pufferl.train (clean_pufferl.py:186-244) for models.Default (pufferlib/models.py:12-62) with
  * 128 fp32 input features, 128 hidden units and <= 7 actions, up to and including the gradients, in ONE persistent

@@ -274,6 +274,26 @@ class Default(nn.Module):
         hidden, lookup = self.encode_observations(observations)
         return self.decode_actions(hidden, lookup)
 
+    def _trunk_ok(self):
+        """Can _ConvReLUTF32Function run network[2:6] (after conv1 ran on the uint8 frames)?  Only where torch would let
+        cuDNN run these convolutions in TF32 (torch.backends.cudnn.allow_tf32): with it off the user asked for fp32
+        convolutions and gets them.  network[2:6] must be the stock Conv2d(32, 64, 4, stride=2), ReLU,
+        Conv2d(64, 64, 3, stride=1), ReLU with bias, no padding, fp32 contiguous 16-byte aligned weights."""
+        if not torch.backends.cudnn.allow_tf32:
+            return False
+        net = self.network
+        if not (type(net[3]) is nn.ReLU and type(net[5]) is nn.ReLU):
+            return False
+        for conv, cin, ks, stride in ((net[2], 32, 4, 2), (net[4], 64, 3, 1)):
+            if not (type(conv) is nn.Conv2d and conv.in_channels == cin and conv.out_channels == 64
+                    and conv.kernel_size == (ks, ks) and conv.stride == (stride, stride) and conv.padding == (0, 0)
+                    and conv.dilation == (1, 1) and conv.groups == 1 and conv.padding_mode == 'zeros'
+                    and conv.bias is not None and conv.weight.dtype == conv.bias.dtype == torch.float32
+                    and conv.weight.is_cuda and conv.weight.is_contiguous() and conv.bias.is_contiguous()
+                    and conv.weight.data_ptr() % 16 == 0 and conv.bias.data_ptr() % 4 == 0):
+                return False
+        return True
+
     def encode_observations(self, observations):
         batch_size = observations.shape[0]
         observations = observations.view(batch_size, -1)
@@ -469,13 +489,53 @@ class _Conv1U8Function(torch.autograd.Function):
         return None, dw, db
 
 
+class _ConvReLUTF32Function(torch.autograd.Function):
+    """relu(conv(x, w) + b) of NatureCNN's conv2 (layer 2: Conv2d(32, 64, 4, stride=2) on [M, 32, 20, 20]) or conv3
+    (layer 3: Conv2d(64, 64, 3, stride=1) on [M, 64, 9, 9]) as one autograd node on TF32 tensor cores
+    (pb_nature_conv_forward).  The backward takes the ReLU's gradient rule from y and returns dx
+    (pb_nature_conv_dgrad) and dw, db (pb_nature_conv_wgrad), each only when autograd asks for it.  x and y are saved:
+    for conv2, x is conv1's y, which _Conv1U8Function keeps anyway."""
+
+    SHAPES = {2: ((32, 20, 20), (64, 9, 9)), 3: ((64, 9, 9), (64, 7, 7))}
+
+    @staticmethod
+    def forward(ctx, x, w, b, layer):
+        from pufferlib_b200 import _native
+        m = x.shape[0]
+        y = torch.empty(m, *_ConvReLUTF32Function.SHAPES[layer][1], dtype=torch.float32, device=x.device)
+        _native.check(_native.lib().pb_nature_conv_forward(layer, _native.ptr(x), m, _native.ptr(w), _native.ptr(b),
+                                                           _native.ptr(y), _native.stream_ptr()))
+        ctx.layer = layer
+        ctx.save_for_backward(x, w, y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from pufferlib_b200 import _native
+        x, w, y = ctx.saved_tensors
+        dy = dy.contiguous()
+        m, lib, layer, P = x.shape[0], _native.lib(), ctx.layer, _native.ptr
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty_like(x)
+            _native.check(lib.pb_nature_conv_dgrad(layer, P(y), P(dy), P(w), m, P(dx), _native.stream_ptr()))
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            dw = torch.empty_like(w)
+            db = torch.empty(w.shape[0], dtype=torch.float32, device=x.device)
+            ws = torch.empty(lib.pb_nature_conv_wgrad_workspace_bytes(layer, m), dtype=torch.uint8, device=x.device)
+            _native.check(lib.pb_nature_conv_wgrad(layer, P(x), P(y), P(dy), m, P(dw), P(db), P(ws), ws.numel(),
+                                                   _native.stream_ptr()))
+        return (dx, dw if ctx.needs_input_grad[1] else None, db if ctx.needs_input_grad[2] else None, None)
+
+
 class Convolutional(nn.Module):
     def __init__(self, env, *args, framestack=4, flat_size=64 * 7 * 7, input_size=512, hidden_size=512,
                  output_size=512, channels_last=False, downsample=1, **kwargs):
         super().__init__()
         self.channels_last = channels_last
         self.downsample = downsample
-        self.fast_path = True     # conv1 + ReLU on the uint8 frames in place (_Conv1U8Function) where _conv1_u8_ok holds
+        self.fast_path = True     # conv1 + ReLU on the uint8 frames in place (_Conv1U8Function) where _conv1_u8_ok holds,
+                                  # then conv2, conv3 (_ConvReLUTF32Function) where _trunk_ok holds too
         self.network = nn.Sequential(
             layer_init(nn.Conv2d(framestack, 32, 8, stride=4)), nn.ReLU(),
             layer_init(nn.Conv2d(32, 64, 4, stride=2)), nn.ReLU(),
@@ -506,6 +566,26 @@ class Convolutional(nn.Module):
                 and conv.weight.dtype == conv.bias.dtype == torch.float32 and conv.weight.is_contiguous()
                 and conv.weight.data_ptr() % 16 == 0)
 
+    def _trunk_ok(self):
+        """Can _ConvReLUTF32Function run network[2:6] (after conv1 ran on the uint8 frames)?  Only where torch would let
+        cuDNN run these convolutions in TF32 (torch.backends.cudnn.allow_tf32): with it off the user asked for fp32
+        convolutions and gets them.  network[2:6] must be the stock Conv2d(32, 64, 4, stride=2), ReLU,
+        Conv2d(64, 64, 3, stride=1), ReLU with bias, no padding, fp32 contiguous 16-byte aligned weights."""
+        if not torch.backends.cudnn.allow_tf32:
+            return False
+        net = self.network
+        if not (type(net[3]) is nn.ReLU and type(net[5]) is nn.ReLU):
+            return False
+        for conv, cin, ks, stride in ((net[2], 32, 4, 2), (net[4], 64, 3, 1)):
+            if not (type(conv) is nn.Conv2d and conv.in_channels == cin and conv.out_channels == 64
+                    and conv.kernel_size == (ks, ks) and conv.stride == (stride, stride) and conv.padding == (0, 0)
+                    and conv.dilation == (1, 1) and conv.groups == 1 and conv.padding_mode == 'zeros'
+                    and conv.bias is not None and conv.weight.dtype == conv.bias.dtype == torch.float32
+                    and conv.weight.is_cuda and conv.weight.is_contiguous() and conv.bias.is_contiguous()
+                    and conv.weight.data_ptr() % 16 == 0 and conv.bias.data_ptr() % 4 == 0):
+                return False
+        return True
+
     def encode_observations(self, observations):
         if self.channels_last:
             observations = observations.permute(0, 3, 1, 2)
@@ -514,6 +594,10 @@ class Convolutional(nn.Module):
         if observations.shape[0] > 0 and self._conv1_u8_ok(observations):
             conv = self.network[0]
             y1 = _Conv1U8Function.apply(observations, conv.weight, conv.bias)
+            if self._trunk_ok():
+                y2 = _ConvReLUTF32Function.apply(y1, self.network[2].weight, self.network[2].bias, 2)
+                y3 = _ConvReLUTF32Function.apply(y2, self.network[4].weight, self.network[4].bias, 3)
+                return self.network[6:](y3), None
             return self.network[2:](y1), None
         return self.network(observations.float() / 255.0), None
 

@@ -429,6 +429,25 @@ size_t pb_conv1_u8_wgrad_workspace_bytes(int64_t m);
 int pb_conv1_u8_wgrad(const uint8_t* x, int64_t row_stride, int64_t m, const float* y, const float* dy, float* dw,
                       float* db, void* workspace, size_t workspace_bytes, void* stream);
 
+/* The same two kernels on frame stacks read in place from the rollout buffer as bptt segments, for the training forward
+ * and backward of LSTMWrapper(Convolutional) (pufferlib/models.py:64-111 over :113-157; environments/atari/torch.py:
+ * Recurrent), whose minibatches are [rows, bptt] segments (clean_pufferl.py:188-191).  Segment b of the batch is
+ * (e, g) = (b / groups, b % groups); its step t is the row at x + e * stride_e + g * stride_g + t * stride_t (bytes).
+ * y (forward) and dy (wgrad) stay dense in row order b*T + t, m = batch * steps rows; the workspace is
+ * pb_conv1_u8_wgrad_workspace_bytes(batch * steps).  The dense entry points are the case groups = 1,
+ * stride_e = T * row_stride, stride_t = row_stride: only the address a row is read from differs, so both compute
+ * bitwise what the dense entry points compute on a gathered copy (the weight gradient's CTA split is over b*T + t).
+ * Experience.segment_obs (minibatch mb of n_mb, G = S / n_mb windows of T = bptt steps per env, N envs, R = 28 224):
+ *   x = obs + mb*T*N*R, groups = G, stride_e = R, stride_g = n_mb*T*N*R, stride_t = N*R.
+ * PB_ERR_INVALID before any launch for batch < 0, steps < 1, groups < 1, batch % groups != 0, any of the three strides
+ * below 28 224 or not a multiple of 16, and the pointer and workspace conditions above; batch = 0 returns PB_OK without
+ * a launch.  No allocation and no host synchronisation (capturable). */
+int pb_conv1_u8_forward_rows(const uint8_t* x, int64_t batch, int32_t steps, int32_t groups, int64_t stride_e,
+                             int64_t stride_g, int64_t stride_t, const float* w, const float* b, float* y, void* stream);
+int pb_conv1_u8_wgrad_rows(const uint8_t* x, int64_t batch, int32_t steps, int32_t groups, int64_t stride_e,
+                           int64_t stride_g, int64_t stride_t, const float* y, const float* dy, float* dw, float* db,
+                           void* workspace, size_t workspace_bytes, void* stream);
+
 /* -- NatureCNN conv2 and conv3 -----------------------------------------------------------------------------------------
  * The second and third layers of models.Convolutional, each Conv2d + ReLU on fp32 NCHW rows, `layer` = 2 or 3:
  *   layer 2: x [m][32][20][20] (conv1's y), w [64][32][4][4], stride 2 -> y [m][64][9][9]

@@ -954,13 +954,15 @@ def update_plan(data):
         'packed'     autograd through Default.forward_packed(_slabs) + fused_ppo_loss_packed
         'model'      autograd through model(obs) + fused_ppo_loss (Convolutional; Default with fast_path=False)
         'bptt'       LSTMWrapper.forward_packed_seq (the fused BPTT kernels) + fused_ppo_loss_packed
+        'cudnn_conv' LSTMWrapper(Convolutional) (cuDNN LSTM, conv1 on the uint8 frames: forward_segments on the
+                     segment views, or forward on b_obs) + fused_ppo_loss
         'cudnn'      the policy's recurrent forward (cuDNN LSTM) + the reference loss
         'reference'  the policy's forward + the reference loss (fused_loss=False, or more than PPO_LOSS_MAX_ACTIONS
                      actions)
     form, the layout Experience.prepare builds: 'direct' (the fused kernel reads the arrival-order rollout tensors in
-    place), 'slabs' (order-free loss: per-row tensors copied slab-major, obs a view), 'segments' (the BPTT kernels on bptt
-    segment views of obs) or 'gathered' (the reference layout: b_obs and the b_* tensors).  capture: 'whole' (ONE graph),
-    'segments' (per-segment graphs around an NCCL all-reduce, _SegmentGraphs) or None (eager).  manual: this call's
+    place), 'slabs' (order-free loss: per-row tensors copied slab-major, obs a view), 'segments' ('bptt' and 'cudnn_conv'
+    on bptt segment views of obs) or 'gathered' (the reference layout: b_obs and the b_* tensors).  capture: 'whole' (ONE
+    graph), 'segments' (per-segment graphs around an NCCL all-reduce, _SegmentGraphs) or None (eager).  manual: this call's
     _DefaultMLPUpdate (built here, and rebuilt when optimizer.load_state_dict() replaced the Adam state it holds), or None.
     bptt_peer: the 'bptt' engine on several ranks takes its gradient mean from the peer exchange of data.grad_bucket
     (GradBucket.open_peer, tried once here) rather than from NCCL.
@@ -986,7 +988,16 @@ def update_plan(data):
         bptt = (data.fused_loss and bool(getattr(data.policy, 'fused_update', False))
                 and hasattr(model, 'forward_packed_seq') and model.fused_supported(exp.obs)
                 and bool(getattr(model.policy, 'fast_path', False)))
-        engine, form = ('bptt', 'segments' if zero_copy else 'gathered') if bptt else ('cudnn', 'gathered')
+        if bptt:
+            engine = 'bptt'
+        elif data.fused_loss and int(getattr(data.vecenv.single_action_space, 'n', 0)) <= PPO_LOSS_MAX_ACTIONS and \
+                hasattr(model, 'forward_segments') and isinstance(model.policy, models.Convolutional) and \
+                model.policy._conv1_u8_ok(exp.obs):
+            # the Atari LSTM policy: its minibatch frames read where the rollout left them (or from b_obs), the fused loss
+            engine = 'cudnn_conv'
+        else:
+            engine = 'cudnn'
+        form = 'segments' if zero_copy and engine != 'cudnn' else 'gathered'
     elif manual is not None:
         # every minibatch of a form is this view shifted by whole minibatches of rows, and the observations _fused_ok
         # accepts have 512-byte rows (128 fp32 features): minibatch 0 answers for all of them
@@ -1023,11 +1034,12 @@ def update_plan(data):
         nccl_call = data.grad_bucket is not None and (manual is None or manual.peer is None)
         if exp.lstm_h is None:
             capture = 'segments' if nccl_call else 'whole'
-        elif engine == 'bptt' and (data.grad_bucket is None or bptt_peer):
+        elif (engine == 'bptt' and (data.grad_bucket is None or bptt_peer)) or \
+                (engine == 'cudnn_conv' and data.grad_bucket is None):
             capture = 'whole'           # the cuDNN path and recurrent updates on several ranks over NCCL stay eager
 
     data.train_minibatch_path = form
-    data.train_recurrent_path = {'bptt': 'fused', 'cudnn': 'cudnn'}.get(engine)
+    data.train_recurrent_path = {'bptt': 'fused', 'cudnn': 'cudnn', 'cudnn_conv': 'cudnn'}.get(engine)
     if manual is not None:
         manual.used_fused = engine == 'mlp_fused'
     return pufferlib_b200.namespace(engine=engine, form=form, capture=capture, manual=manual, bptt_peer=bptt_peer)
@@ -1312,6 +1324,16 @@ def _train_device_part(data, plan, seg=None):
                     carry['lstm_state'] = (packed[2][0].detach(), packed[2][1].detach())
             elif engine == 'model':
                 logits, newvalue = model(obs.reshape(-1, *obs_shape))
+            elif engine == 'cudnn_conv':         # rows b*T + t, as the b_* per-row tensors
+                if plan.form == 'segments':
+                    out = model.forward_segments(obs, carry['lstm_state'])
+                    if out is None:
+                        raise RuntimeError(f'the {engine} engine refused minibatch {mb} of form {plan.form}: update_plan '
+                                           'and the model disagree on what its kernels cover')
+                else:
+                    out = model(obs, carry['lstm_state'])
+                logits, newvalue, st_ = out
+                carry['lstm_state'] = (st_[0].detach(), st_[1].detach())
             elif engine == 'cudnn':
                 _, newlogprob, entropy, newvalue, st_ = data.policy(obs, state=carry['lstm_state'], action=atn)
                 carry['lstm_state'] = (st_[0].detach(), st_[1].detach())
@@ -1321,7 +1343,7 @@ def _train_device_part(data, plan, seg=None):
         with profile.train_misc:
             if engine in ('packed', 'bptt'):
                 loss, st = fused_ppo_loss_packed(packed[0], packed[1], atn, log_probs, adv, ret, val, config)
-            elif engine == 'model':
+            elif engine in ('model', 'cudnn_conv'):
                 loss, st = fused_ppo_loss(logits, newvalue, atn, log_probs, adv, ret, val, config)
             else:
                 loss, st = _ppo_loss(newlogprob, entropy, newvalue, log_probs, adv, ret, val, config)
@@ -1434,7 +1456,8 @@ def _kl_stop(data):
 
 def train(data):
     """One PPO update (reference: clean_pufferl.py:156-292).  With ``config.cuda_graph`` (recurrent policies only with the
-    fused BPTT update, on several GPUs only with its peer exchange; target_kl on several GPUs only with the peer
+    fused BPTT update, on several GPUs only with its peer exchange, or LSTMWrapper(Convolutional) on one GPU (the
+    'cudnn_conv' engine); target_kl on several GPUs only with the peer
     exchange) the device part is captured
     once -- after an eager first call that initialises the optimizer state -- and replayed as ONE graph launch; the
     learning rate lives in a device tensor so annealing works under replay, and the target_kl stop is decided on the

@@ -69,14 +69,31 @@ __device__ __forceinline__ uint32_t byte_f32(uint32_t w, int j) {
 // byte offset of output pixel p's receptive field (row 4 oy, column 4 ox of channel 0) in a frame stack
 __device__ __forceinline__ int pix_base(int p) { return (p / 20) * (4 * 84) + (p % 20) * 4; }
 
-__device__ __forceinline__ void issue_row(unsigned char* dst, uint64_t* bar, const unsigned char* x, int64_t row,
-                                         int64_t row_stride) {
+// Where row r (the r-th frame stack the kernels process, the r-th row of y and dy) is read from.  Both kernels are
+// templates over this, and it is the only thing that differs between the dense and the segment entry points.
+struct DenseRows {            // row r at x + r * stride
+    const unsigned char* x;
+    int64_t stride;
+    __device__ __forceinline__ const unsigned char* operator()(int64_t r) const { return x + r * stride; }
+};
+
+struct SegmentRows {          // row r = b*T + t, segment b = (e, g) = (b / groups, b % groups): x + e*se + g*sg + t*st
+    const unsigned char* x;
+    int64_t se, sg, st;
+    int32_t steps, groups;
+    __device__ __forceinline__ const unsigned char* operator()(int64_t r) const {
+        const int64_t b = r / steps, e = b / groups;
+        return x + e * se + (b - e * groups) * sg + (r - b * steps) * st;
+    }
+};
+
+__device__ __forceinline__ void issue_row(unsigned char* dst, uint64_t* bar, const unsigned char* src) {
     mbar_expect_tx(bar, C1_ROW);
-    tma_load_1d(dst, x + row * row_stride, C1_ROW, bar);
+    tma_load_1d(dst, src, C1_ROW, bar);
 }
 
-__global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(const unsigned char* __restrict__ x, int64_t row_stride,
-                                                             int64_t m, const float* __restrict__ w,
+template <class Rows>
+__global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(Rows rows, int64_t m, const float* __restrict__ w,
                                                              const float* __restrict__ b, float* __restrict__ y) {
     extern __shared__ __align__(128) unsigned char dyn[];
     FwdSmem& s = *reinterpret_cast<FwdSmem*>(dyn);
@@ -89,7 +106,7 @@ __global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(const unsigned char
     __syncthreads();
     if (threadIdx.x == 0)
         for (int i = 0; i < C1_STAGES && i < n_rows; ++i)
-            issue_row(s.x[i], &s.bar[i], x, blockIdx.x + (int64_t)i * gridDim.x, row_stride);
+            issue_row(s.x[i], &s.bar[i], rows(blockIdx.x + (int64_t)i * gridDim.x));
     // W in B-fragment order (the header comment), rounded to TF32
     for (int e = threadIdx.x; e < 16 * 4 * 32; e += FW_THREADS) {
         const int p = e >> 7, nt = (e >> 5) & 3, l = e & 31, lg = l >> 2, lt = l & 3;
@@ -147,7 +164,7 @@ __global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(const unsigned char
         }
         __syncthreads();   // every warp is done with stage st: refill it with the row after next
         if (threadIdx.x == 0 && i + C1_STAGES < n_rows)
-            issue_row(s.x[st], &s.bar[st], x, row + (int64_t)C1_STAGES * gridDim.x, row_stride);
+            issue_row(s.x[st], &s.bar[st], rows(row + (int64_t)C1_STAGES * gridDim.x));
         float* yrow = y + row * C1_Y;
 #pragma unroll
         for (int a = 0; a < FW_MT; ++a) {
@@ -171,8 +188,8 @@ __global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(const unsigned char
     }
 }
 
-__global__ void __launch_bounds__(WG_THREADS, 2) k_conv1_wgrad(const unsigned char* __restrict__ x, int64_t row_stride,
-                                                               int64_t m, const float* __restrict__ y,
+template <class Rows>
+__global__ void __launch_bounds__(WG_THREADS, 2) k_conv1_wgrad(Rows rows, int64_t m, const float* __restrict__ y,
                                                                const float* __restrict__ dy, float* __restrict__ partials) {
     extern __shared__ __align__(128) unsigned char dyn[];
     WgSmem& s = *reinterpret_cast<WgSmem*>(dyn);
@@ -185,7 +202,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) k_conv1_wgrad(const unsigned ch
     __syncthreads();
     if (threadIdx.x == 0)
         for (int i = 0; i < C1_STAGES && i < n_rows; ++i)
-            issue_row(s.x[i], &s.bar[i], x, blockIdx.x + (int64_t)i * gridDim.x, row_stride);
+            issue_row(s.x[i], &s.bar[i], rows(blockIdx.x + (int64_t)i * gridDim.x));
 
     // warp w: channel c = w >> 1, kernel rows 4 (w & 1) .. +3.  n-tile j, column n <-> kernel row 4 (w & 1) + (n >> 1),
     // kx = 4 (n & 1) + j: lane g reads the bytes of all four n-tiles as one word
@@ -240,7 +257,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) k_conv1_wgrad(const unsigned ch
         }
         __syncthreads();   // dz and stage st are free
         if (threadIdx.x == 0 && i + C1_STAGES < n_rows)
-            issue_row(s.x[st], &s.bar[st], x, row + (int64_t)C1_STAGES * gridDim.x, row_stride);
+            issue_row(s.x[st], &s.bar[st], rows(row + (int64_t)C1_STAGES * gridDim.x));
     }
     // this CTA's partial row: dW / 255 in k order, then db
     float* part = partials + (int64_t)blockIdx.x * WG_PSTRIDE;
@@ -271,21 +288,70 @@ int check_rows(const void* x, int64_t row_stride, int64_t m, const char* who) {
     return PB_OK;
 }
 
+// The segment entry points' checks: batch segments of `steps` rows, every stride (bytes) a whole aligned row or more
+int check_segments(const void* x, int64_t batch, int32_t steps, int32_t groups, int64_t se, int64_t sg, int64_t st,
+                   const char* who) {
+    PB_REQUIRE(batch >= 0 && steps >= 1, PB_ERR_INVALID, "%s: need batch >= 0 and steps >= 1", who);
+    PB_REQUIRE(groups >= 1 && batch % groups == 0, PB_ERR_INVALID, "%s: need groups >= 1 dividing batch (got %d, %lld)",
+               who, groups, (long long)batch);
+    PB_REQUIRE(x && ((uintptr_t)x & 15) == 0, PB_ERR_INVALID, "%s: x must be a 16-byte aligned device pointer", who);
+    for (const int64_t stride : {se, sg, st})
+        PB_REQUIRE(stride >= C1_ROW && stride % 16 == 0, PB_ERR_INVALID,
+                   "%s: stride %lld must be >= %d and a multiple of 16", who, (long long)stride, C1_ROW);
+    return PB_OK;
+}
+
+template <class Rows>
+int forward(const char* who, Rows rows, int64_t m, const float* w, const float* b, float* y, void* stream) {
+    PB_REQUIRE(w && b && y && ((uintptr_t)w & 15) == 0 && ((uintptr_t)b & 3) == 0 && ((uintptr_t)y & 15) == 0,
+               PB_ERR_INVALID, "%s: w and y must be 16-byte aligned, b 4-byte aligned", who);
+    if (m == 0) return PB_OK;
+    const int smem = (int)sizeof(FwdSmem);
+    PB_CUDA(cudaFuncSetAttribute(k_conv1_fwd<Rows>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const int grid = (int)(m < 2 * (int64_t)PB_NUM_SMS ? m : 2 * (int64_t)PB_NUM_SMS);
+    k_conv1_fwd<<<grid, FW_THREADS, smem, (cudaStream_t)stream>>>(rows, m, w, b, y);
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
+
+template <class Rows>
+int wgrad(const char* who, Rows rows, int64_t m, const float* y, const float* dy, float* dw, float* db, void* workspace,
+          size_t workspace_bytes, void* stream) {
+    PB_REQUIRE(y && dy && dw && db && workspace && ((uintptr_t)y & 15) == 0 && ((uintptr_t)dy & 15) == 0 &&
+                   ((uintptr_t)dw & 3) == 0 && ((uintptr_t)db & 3) == 0 && ((uintptr_t)workspace & 15) == 0,
+               PB_ERR_INVALID, "%s: y, dy and workspace must be 16-byte aligned, dw and db 4-byte aligned", who);
+    PB_REQUIRE(workspace_bytes >= pb_conv1_u8_wgrad_workspace_bytes(m), PB_ERR_INVALID, "%s: workspace too small", who);
+    if (m == 0) return PB_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int smem = (int)sizeof(WgSmem);
+    PB_CUDA(cudaFuncSetAttribute(k_conv1_wgrad<Rows>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const int ctas = (int)(m < WG_CTAS ? m : WG_CTAS);
+    float* part = (float*)workspace;
+    k_conv1_wgrad<<<ctas, WG_THREADS, smem, s>>>(rows, m, y, dy, part);
+    PB_LAUNCH_CHECK();
+    k_reduce_partials<<<(C1_CO * C1_K * 32 + 255) / 256, 256, 0, s>>>(part, ctas, WG_PSTRIDE, C1_CO * C1_K, dw);
+    PB_LAUNCH_CHECK();
+    k_reduce_partials<<<(C1_CO * 32 + 255) / 256, 256, 0, s>>>(part + C1_CO * C1_K, ctas, WG_PSTRIDE, C1_CO, db);
+    PB_LAUNCH_CHECK();
+    return PB_OK;
+}
+
 }  // namespace
 
 extern "C" int pb_conv1_u8_forward(const uint8_t* x, int64_t row_stride, int64_t m, const float* w, const float* b, float* y,
                                    void* stream) {
     const int rc = check_rows(x, row_stride, m, "pb_conv1_u8_forward");
     if (rc != PB_OK) return rc;
-    PB_REQUIRE(w && b && y && ((uintptr_t)w & 15) == 0 && ((uintptr_t)b & 3) == 0 && ((uintptr_t)y & 15) == 0,
-               PB_ERR_INVALID, "pb_conv1_u8_forward: w and y must be 16-byte aligned, b 4-byte aligned");
-    if (m == 0) return PB_OK;
-    const int smem = (int)sizeof(FwdSmem);
-    PB_CUDA(cudaFuncSetAttribute(k_conv1_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    const int grid = (int)(m < 2 * (int64_t)PB_NUM_SMS ? m : 2 * (int64_t)PB_NUM_SMS);
-    k_conv1_fwd<<<grid, FW_THREADS, smem, (cudaStream_t)stream>>>(x, row_stride, m, w, b, y);
-    PB_LAUNCH_CHECK();
-    return PB_OK;
+    return forward("pb_conv1_u8_forward", DenseRows{x, row_stride}, m, w, b, y, stream);
+}
+
+extern "C" int pb_conv1_u8_forward_rows(const uint8_t* x, int64_t batch, int32_t steps, int32_t groups, int64_t stride_e,
+                                        int64_t stride_g, int64_t stride_t, const float* w, const float* b, float* y,
+                                        void* stream) {
+    const char* who = "pb_conv1_u8_forward_rows";
+    const int rc = check_segments(x, batch, steps, groups, stride_e, stride_g, stride_t, who);
+    if (rc != PB_OK) return rc;
+    return forward(who, SegmentRows{x, stride_e, stride_g, stride_t, steps, groups}, batch * steps, w, b, y, stream);
 }
 
 extern "C" size_t pb_conv1_u8_wgrad_workspace_bytes(int64_t m) {
@@ -297,22 +363,15 @@ extern "C" int pb_conv1_u8_wgrad(const uint8_t* x, int64_t row_stride, int64_t m
                                  float* db, void* workspace, size_t workspace_bytes, void* stream) {
     const int rc = check_rows(x, row_stride, m, "pb_conv1_u8_wgrad");
     if (rc != PB_OK) return rc;
-    PB_REQUIRE(y && dy && dw && db && workspace && ((uintptr_t)y & 15) == 0 && ((uintptr_t)dy & 15) == 0 &&
-                   ((uintptr_t)dw & 3) == 0 && ((uintptr_t)db & 3) == 0 && ((uintptr_t)workspace & 15) == 0,
-               PB_ERR_INVALID, "pb_conv1_u8_wgrad: y, dy and workspace must be 16-byte aligned, dw and db 4-byte aligned");
-    PB_REQUIRE(workspace_bytes >= pb_conv1_u8_wgrad_workspace_bytes(m), PB_ERR_INVALID,
-               "pb_conv1_u8_wgrad: workspace too small");
-    if (m == 0) return PB_OK;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int smem = (int)sizeof(WgSmem);
-    PB_CUDA(cudaFuncSetAttribute(k_conv1_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    const int ctas = (int)(m < WG_CTAS ? m : WG_CTAS);
-    float* part = (float*)workspace;
-    k_conv1_wgrad<<<ctas, WG_THREADS, smem, s>>>(x, row_stride, m, y, dy, part);
-    PB_LAUNCH_CHECK();
-    k_reduce_partials<<<(C1_CO * C1_K * 32 + 255) / 256, 256, 0, s>>>(part, ctas, WG_PSTRIDE, C1_CO * C1_K, dw);
-    PB_LAUNCH_CHECK();
-    k_reduce_partials<<<(C1_CO * 32 + 255) / 256, 256, 0, s>>>(part + C1_CO * C1_K, ctas, WG_PSTRIDE, C1_CO, db);
-    PB_LAUNCH_CHECK();
-    return PB_OK;
+    return wgrad("pb_conv1_u8_wgrad", DenseRows{x, row_stride}, m, y, dy, dw, db, workspace, workspace_bytes, stream);
+}
+
+extern "C" int pb_conv1_u8_wgrad_rows(const uint8_t* x, int64_t batch, int32_t steps, int32_t groups, int64_t stride_e,
+                                      int64_t stride_g, int64_t stride_t, const float* y, const float* dy, float* dw,
+                                      float* db, void* workspace, size_t workspace_bytes, void* stream) {
+    const char* who = "pb_conv1_u8_wgrad_rows";
+    const int rc = check_segments(x, batch, steps, groups, stride_e, stride_g, stride_t, who);
+    if (rc != PB_OK) return rc;
+    return wgrad(who, SegmentRows{x, stride_e, stride_g, stride_t, steps, groups}, batch * steps, y, dy, dw, db,
+                 workspace, workspace_bytes, stream);
 }

@@ -274,26 +274,6 @@ class Default(nn.Module):
         hidden, lookup = self.encode_observations(observations)
         return self.decode_actions(hidden, lookup)
 
-    def _trunk_ok(self):
-        """Can _ConvReLUTF32Function run network[2:6] (after conv1 ran on the uint8 frames)?  Only where torch would let
-        cuDNN run these convolutions in TF32 (torch.backends.cudnn.allow_tf32): with it off the user asked for fp32
-        convolutions and gets them.  network[2:6] must be the stock Conv2d(32, 64, 4, stride=2), ReLU,
-        Conv2d(64, 64, 3, stride=1), ReLU with bias, no padding, fp32 contiguous 16-byte aligned weights."""
-        if not torch.backends.cudnn.allow_tf32:
-            return False
-        net = self.network
-        if not (type(net[3]) is nn.ReLU and type(net[5]) is nn.ReLU):
-            return False
-        for conv, cin, ks, stride in ((net[2], 32, 4, 2), (net[4], 64, 3, 1)):
-            if not (type(conv) is nn.Conv2d and conv.in_channels == cin and conv.out_channels == 64
-                    and conv.kernel_size == (ks, ks) and conv.stride == (stride, stride) and conv.padding == (0, 0)
-                    and conv.dilation == (1, 1) and conv.groups == 1 and conv.padding_mode == 'zeros'
-                    and conv.bias is not None and conv.weight.dtype == conv.bias.dtype == torch.float32
-                    and conv.weight.is_cuda and conv.weight.is_contiguous() and conv.bias.is_contiguous()
-                    and conv.weight.data_ptr() % 16 == 0 and conv.bias.data_ptr() % 4 == 0):
-                return False
-        return True
-
     def encode_observations(self, observations):
         batch_size = observations.shape[0]
         observations = observations.view(batch_size, -1)
@@ -450,6 +430,29 @@ class LSTMWrapper(nn.Module):
         if state is not None:
             assert state[0].shape[1] == state[1].shape[1] == batch
         hidden, lookup = self.policy.encode_observations(x.reshape(batch * steps, *self.obs_shape))
+        return self._recur(hidden, lookup, batch, steps, state)
+
+    def forward_segments(self, x, state):
+        """forward for the training minibatch read in place: x the segment view [E, G, T, *obs] of
+        Experience.segment_obs (segment b = e*G + g, B = E*G segments of T steps), state (h, c) [1, B, H] or None.
+        The inner policy's encode_segments reads the view (models.Convolutional: conv1's kernel on the frame stacks where
+        they lie); the LSTM and the heads are those of forward.  -> (logits, value, state) with rows b*T + t, what
+        forward gives for the gathered copy [B, T, *obs]; None when the inner policy cannot encode the view.  The view
+        is never reshaped (that would copy the observations)."""
+        nd = len(self.obs_shape)
+        encode = getattr(self.policy, 'encode_segments', None)
+        if encode is None or x.dim() != nd + 3 or tuple(x.shape[3:]) != self.obs_shape:
+            return None
+        batch, steps = x.shape[0] * x.shape[1], x.shape[2]
+        if state is not None:
+            assert state[0].shape[1] == state[1].shape[1] == batch
+        hidden = encode(x)
+        if hidden is None:
+            return None
+        return self._recur(hidden, None, batch, steps, state)
+
+    def _recur(self, hidden, lookup, batch, steps, state):
+        """The LSTM over hidden [B*T, input_size] (rows b*T + t) from state, then the inner policy's heads."""
         assert hidden.shape == (batch * steps, self.input_size)
         seq = hidden.reshape(batch, steps, self.input_size).transpose(0, 1)       # [T, B, F] for nn.LSTM
         seq, state = self.recurrent(seq, state)
@@ -458,19 +461,37 @@ class LSTMWrapper(nn.Module):
         return logits, value, state
 
 
+_CONV1_ROW = 4 * 84 * 84     # bytes of one (4, 84, 84) uint8 frame stack
+
+
 class _Conv1U8Function(torch.autograd.Function):
     """relu(conv1(x / 255) + b) of NatureCNN (Conv2d(4, 32, 8, stride=4) on (4, 84, 84) uint8 frame stacks) as one
     autograd node: pb_conv1_u8_forward reads the uint8 rows in place and writes y [M, 32, 20, 20]; the backward
     (pb_conv1_u8_wgrad) takes the ReLU's gradient rule and the weight and bias gradients from y, dy and the same bytes.
-    x gets no gradient (conv1 is the first layer), so only y is saved beside it."""
+    x gets no gradient (conv1 is the first layer), so only y is saved beside it.
+    x is either rows [M, 4, 84, 84] or the segment view [E, G, T, 4, 84, 84] of Experience.segment_obs (segment
+    b = e*G + g; pb_conv1_u8_forward_rows / _wgrad_rows), whose y rows are b*T + t.  The view itself is saved, not a copy."""
+
+    @staticmethod
+    def _segments(x):
+        """(batch, steps, groups, stride_e, stride_g, stride_t) of a segment view, in bytes.  A dimension of size 1 is
+        never stepped over, so its stride is whatever torch reports; it is passed as one row, which the kernel accepts."""
+        e_, g_, steps = x.shape[:3]
+        st = [x.stride(i) if x.shape[i] > 1 else _CONV1_ROW for i in range(3)]
+        return e_ * g_, steps, g_, st[0], st[1], st[2]
 
     @staticmethod
     def forward(ctx, x, w, b):
         from pufferlib_b200 import _native
-        m = x.shape[0]
+        P, lib = _native.ptr, _native.lib()
+        seg = x.dim() == 6
+        m = x.shape[0] * x.shape[1] * x.shape[2] if seg else x.shape[0]
         y = torch.empty(m, 32, 20, 20, dtype=torch.float32, device=x.device)
-        _native.check(_native.lib().pb_conv1_u8_forward(_native.ptr(x), x.stride(0), m, _native.ptr(w), _native.ptr(b),
-                                                        _native.ptr(y), _native.stream_ptr()))
+        if seg:
+            _native.check(lib.pb_conv1_u8_forward_rows(P(x), *_Conv1U8Function._segments(x), P(w), P(b), P(y),
+                                                       _native.stream_ptr()))
+        else:
+            _native.check(lib.pb_conv1_u8_forward(P(x), x.stride(0), m, P(w), P(b), P(y), _native.stream_ptr()))
         ctx.save_for_backward(x, y)
         return y
 
@@ -479,13 +500,16 @@ class _Conv1U8Function(torch.autograd.Function):
         from pufferlib_b200 import _native
         x, y = ctx.saved_tensors
         dy = dy.contiguous()
-        m, lib = x.shape[0], _native.lib()
+        m, lib, P = y.shape[0], _native.lib(), _native.ptr
         dw = torch.empty(32, 4, 8, 8, dtype=torch.float32, device=x.device)
         db = torch.empty(32, dtype=torch.float32, device=x.device)
         ws = torch.empty(lib.pb_conv1_u8_wgrad_workspace_bytes(m), dtype=torch.uint8, device=x.device)
-        _native.check(lib.pb_conv1_u8_wgrad(_native.ptr(x), x.stride(0), m, _native.ptr(y), _native.ptr(dy),
-                                            _native.ptr(dw), _native.ptr(db), _native.ptr(ws), ws.numel(),
-                                            _native.stream_ptr()))
+        if x.dim() == 6:
+            _native.check(lib.pb_conv1_u8_wgrad_rows(P(x), *_Conv1U8Function._segments(x), P(y), P(dy), P(dw), P(db),
+                                                     P(ws), ws.numel(), _native.stream_ptr()))
+        else:
+            _native.check(lib.pb_conv1_u8_wgrad(P(x), x.stride(0), m, P(y), P(dy), P(dw), P(db), P(ws), ws.numel(),
+                                                _native.stream_ptr()))
         return None, dw, db
 
 
@@ -554,10 +578,21 @@ class Convolutional(nn.Module):
         """Can pb_conv1_u8_forward run the first layer on x?  CUDA uint8 [M, 4, 84, 84] with every row one contiguous
         frame stack (rows 16-byte aligned), channels-first frames at full resolution, and the stock
         Conv2d(4, 32, 8, stride=4) + ReLU with fp32 parameters first."""
+        return x.dim() == 4 and x.stride(0) % 16 == 0 and self._frames_ok(x)
+
+    def _conv1_segments_ok(self, x):
+        """The same for a segment view [E, G, T, 4, 84, 84] (Experience.segment_obs) and pb_conv1_u8_forward_rows: every
+        frame stack contiguous, and each of E, G, T that is stepped over (size > 1) a multiple of 16 bytes and at least
+        one frame stack apart."""
+        return (x.dim() == 6 and self._frames_ok(x)
+                and all(x.stride(i) % 16 == 0 and x.stride(i) >= _CONV1_ROW for i in range(3) if x.shape[i] > 1))
+
+    def _frames_ok(self, x):
+        """_conv1_u8_ok's conditions on the trailing (4, 84, 84) dimensions of x and on the module."""
         conv = self.network[0]
         if not (self.fast_path and not self.channels_last and self.downsample == 1 and x.is_cuda
-                and x.dtype == torch.uint8 and x.dim() == 4 and tuple(x.shape[1:]) == (4, 84, 84)
-                and tuple(x.stride()[1:]) == (7056, 84, 1) and x.stride(0) % 16 == 0 and x.data_ptr() % 16 == 0):
+                and x.dtype == torch.uint8 and tuple(x.shape[-3:]) == (4, 84, 84)
+                and tuple(x.stride()[-3:]) == (7056, 84, 1) and x.data_ptr() % 16 == 0):
             return False
         return (type(conv) is nn.Conv2d and type(self.network[1]) is nn.ReLU and conv.in_channels == 4
                 and conv.out_channels == 32 and conv.kernel_size == (8, 8) and conv.stride == (4, 4)
@@ -593,13 +628,27 @@ class Convolutional(nn.Module):
             observations = observations[:, :, ::self.downsample, ::self.downsample]
         if observations.shape[0] > 0 and self._conv1_u8_ok(observations):
             conv = self.network[0]
-            y1 = _Conv1U8Function.apply(observations, conv.weight, conv.bias)
-            if self._trunk_ok():
-                y2 = _ConvReLUTF32Function.apply(y1, self.network[2].weight, self.network[2].bias, 2)
-                y3 = _ConvReLUTF32Function.apply(y2, self.network[4].weight, self.network[4].bias, 3)
-                return self.network[6:](y3), None
-            return self.network[2:](y1), None
+            return self._after_conv1(_Conv1U8Function.apply(observations, conv.weight, conv.bias)), None
         return self.network(observations.float() / 255.0), None
+
+    def encode_segments(self, view):
+        """encode_observations for the bptt segments of a training minibatch read in place: the segment view
+        [E, G, T, 4, 84, 84] of Experience.segment_obs (segment b = e*G + g) -> hidden [E*G*T, 512] in row order b*T + t,
+        what encode_observations gives for the gathered copy [E*G*T, 4, 84, 84] of the same rows, bit for bit.  None when
+        conv1's kernel cannot read the view (_conv1_segments_ok) or it is empty; the view is never reshaped (that would
+        copy it)."""
+        if view.dim() != 6 or view.numel() == 0 or not self._conv1_segments_ok(view):
+            return None
+        conv = self.network[0]
+        return self._after_conv1(_Conv1U8Function.apply(view, conv.weight, conv.bias))
+
+    def _after_conv1(self, y1):
+        """network[2:] on conv1's output y1 [M, 32, 20, 20]: conv2 and conv3 on _ConvReLUTF32Function where _trunk_ok."""
+        if self._trunk_ok():
+            y2 = _ConvReLUTF32Function.apply(y1, self.network[2].weight, self.network[2].bias, 2)
+            y3 = _ConvReLUTF32Function.apply(y2, self.network[4].weight, self.network[4].bias, 3)
+            return self.network[6:](y3)
+        return self.network[2:](y1)
 
     def decode_actions(self, flat_hidden, lookup, concat=None):
         return self.actor(flat_hidden), self.value_fn(flat_hidden)

@@ -80,7 +80,18 @@ typedef struct {
                                  BANDIT  : [0]=num_actions in [1, 32768] (default 10)   ocean.py:8-62
                                  MULTIAGENT: no parameters (any non-zero iparam or any dparam is refused)
                                                                                         ocean.py:149-208
-                                 BREAKOUT_PIXELS: [0]=max_ticks (default 4096), as BREAKOUT */
+                                 BREAKOUT_PIXELS: [0]=max_ticks (default 4096), as BREAKOUT
+                                 PONG and BREAKOUT_PIXELS, the Atari preprocessing (oracle/SPEC_PIXEL_PREPROCESSING.md):
+                                   [2]=frameskip in [1, 8] (0 = default 1): ticks per step, rewards summed, the frame
+                                       the pixel-wise max of the last two ticks' frames; above 1 it needs
+                                       max_ticks >= 4 * frameskip
+                                   [3]=noop_max in [0, 30] and < max_ticks (default 0): a real reset is followed by
+                                       1 + draw % noop_max NOOP ticks; PONG with noop_max > 0 needs max_score >= 2
+                                   [4]=episodic_life 0 / 1 (BREAKOUT_PIXELS only): a lost life is a terminal row,
+                                       the next send runs a NOOP step instead of a reset
+                                   [5]=clip_rewards 0 / 1: the row reward is the sign of the step's reward sum
+                                 All zero is the plain game, one tick per step.  Values out of range are refused
+                                 with PB_ERR_INVALID by pb_env_create before anything is allocated. */
 } pb_env_config;
 
 typedef struct {
@@ -159,6 +170,11 @@ int pb_env_stats_read(pb_env* env, double* out4_host, int clear, void* stream);
 /* The score of pb_env_episode_rows in fp64, for the kinds whose score is a python float that fp32 does not hold
  * (STOCHASTIC: 1 - (p - frac)**2); *score = NULL for the kinds without one (their fp32 score is exact). */
 int pb_env_episode_score_f64(pb_env* env, const double** score);
+/* Where the most recent step ENDED a game, for a BREAKOUT_PIXELS env with episodic_life (iparam[4]): a device array
+ * [N] of 0 / 1, owned by the handle, overwritten by the next step.  With episodic_life a terminal row may be a lost
+ * life only; pb_env_episode_rows is valid where this is 1.  *ended = NULL for every other env, where each terminal row
+ * ends a game. */
+int pb_env_game_ended(pb_env* env, const uint8_t** ended);
 /* Per-agent statistics of the multi-agent kinds (MultiagentEpisodeStats, postprocess.py:147-179, which computes
  * episode_return / episode_length and then drops them: only the env's own per-agent info values are kept):
  * out4_host = {env steps, sum of agent 1's score, sum of agent 2's score, 0} accumulated on the device since the last

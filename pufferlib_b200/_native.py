@@ -57,6 +57,7 @@ SIGNATURES = {
     'pb_env_create': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(C.c_void_p)]),
     'pb_env_create_ex': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(C.c_double), C.c_int32, C.POINTER(C.c_void_p)]),
     'pb_env_episode_score_f64': (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
+    'pb_env_game_ended': (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     'pb_env_destroy': (C.c_int, [C.c_void_p]),
     'pb_env_get_info': (C.c_int, [C.c_void_p, C.POINTER(EnvInfo)]),
     'pb_env_agents_per_env': (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),

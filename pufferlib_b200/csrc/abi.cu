@@ -4,6 +4,7 @@
 #include <string.h>
 
 #include "env_common.cuh"
+#include "frame_stack.cuh"
 
 static thread_local char g_err[512] = "";
 
@@ -71,6 +72,10 @@ extern "C" int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_h
     PB_REQUIRE(cfg->num_envs >= 1, PB_ERR_INVALID, "num_envs must be at least 1");  // vector.py:578-579
     PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_BREAKOUT_PIXELS, PB_ERR_INVALID, "unknown env kind %d",
                cfg->kind);
+    if (cfg->kind == PB_ENV_PONG || cfg->kind == PB_ENV_BREAKOUT_PIXELS) {
+        const int rc = fs_pre_check(cfg);   // the Atari preprocessing options, refused before anything is allocated
+        if (rc != PB_OK) return rc;
+    }
     int ndev = 0;
     PB_CUDA(cudaGetDeviceCount(&ndev));
     PB_REQUIRE(cfg->device >= 0 && cfg->device < ndev, PB_ERR_CUDA, "CUDA device %d not available (%d devices)",
@@ -182,6 +187,12 @@ extern "C" int pb_env_episode_rows(pb_env* env, const double** episode_return, c
 extern "C" int pb_env_episode_score_f64(pb_env* env, const double** score) {
     PB_REQUIRE(env && score, PB_ERR_INVALID, "pb_env_episode_score_f64: null pointer");
     *score = env->d_row_score64;
+    return PB_OK;
+}
+
+extern "C" int pb_env_game_ended(pb_env* env, const uint8_t** ended) {
+    PB_REQUIRE(env && ended, PB_ERR_INVALID, "pb_env_game_ended: null pointer");
+    *ended = env->d_ended;
     return PB_OK;
 }
 

@@ -63,6 +63,19 @@ __device__ __forceinline__ uint32_t bkp_pixel(const BkEnv& p, const BkRowView& v
     return 0u;
 }
 
+// frame pixel (r, c) of the union of two states' objects (render2): `va` is the row view of a with the OR of both brick
+// bitmaps, `vb` that of b (only its ball test is read)
+__device__ __forceinline__ uint32_t bkp_pixel2(const BkEnv& a, const BkEnv& b, const BkRowView& va, const BkRowView& vb,
+                                               int c) {
+    const int x0 = (160 * c) / 84, x1 = (160 * (c + 1)) / 84;
+    if ((va.ball && a.bx < x1 && a.bx + 2 > x0) || (vb.ball && b.bx < x1 && b.bx + 2 > x0)) return 255u;
+    if (va.paddle && ((a.px < x1 && a.px + 24 > x0) || (b.px < x1 && b.px + 24 > x0))) return 192u;
+    const uint32_t cols = (1u << (x0 >> 3)) | (1u << ((x1 - 1) >> 3));
+    if (va.bits_a & cols) return va.gray_a;
+    if (va.bits_b & cols) return va.gray_b;
+    return 0u;
+}
+
 // the game behind the frame-stack ring (frame_stack.cuh)
 struct BreakoutPixelsGame {
     using State = BreakoutState;
@@ -74,20 +87,37 @@ struct BreakoutPixelsGame {
         p.bricks = make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0x00ffffffu);
     }
 
-    static __device__ __forceinline__ void step(const State& st, int64_t e, int64_t action, uint64_t seed_e, Env& p,
-                                                float& reward, bool& terminal, float& score) {
+    static constexpr int NOOP = 0;
+    static constexpr bool kLives = true;
+
+    static __device__ __forceinline__ int lives(const Env& p) { return p.lives; }
+
+    static __device__ __forceinline__ void load(const State& st, int64_t e, Env& p) {
+        p.ctr = st.ctr[e];
+        bk_unpack(st.s0[e], st.s1[e], p.px, p.lives, p.in_play, p.wait, p.vx, p.vy, p.bx, p.by, p.tick);
+        p.bricks = st.bricks[e];
+    }
+
+    static __device__ __forceinline__ void tick(const State& st, Env& p, int64_t action, uint64_t seed_e, float& reward,
+                                                bool& terminal, float& score) {
         // the game on plain locals (bk_physics picks the bitmap word by pointer: on a struct member that would put the
         // whole Env in local memory)
-        uint32_t ctr = st.ctr[e];
-        int px, lives, in_play, wait, vx, vy, bx, by, tick;
-        bk_unpack(st.s0[e], st.s1[e], px, lives, in_play, wait, vx, vy, bx, by, tick);
-        uint4 bricks = st.bricks[e];
+        uint32_t ctr = p.ctr;
+        int px = p.px, lives = p.lives, in_play = p.in_play, wait = p.wait, vx = p.vx, vy = p.vy, bx = p.bx, by = p.by,
+            tick = p.tick;
+        uint4 bricks = p.bricks;
         int r = 0;
         bk_physics(px, lives, in_play, wait, vx, vy, bx, by, tick, bricks, ctr, (int)action, seed_e, st.max_ticks, r, terminal,
                    score);
         reward = (float)r;
         p.px = px; p.lives = lives; p.in_play = in_play; p.wait = wait; p.vx = vx; p.vy = vy; p.bx = bx; p.by = by;
         p.tick = tick; p.bricks = bricks; p.ctr = ctr;
+    }
+
+    static __device__ __forceinline__ void step(const State& st, int64_t e, int64_t action, uint64_t seed_e, Env& p,
+                                                float& reward, bool& terminal, float& score) {
+        load(st, e, p);
+        tick(st, p, action, seed_e, reward, terminal, score);
     }
 
     // thread k builds the 16-byte runs k, k + 128, ...: frame bytes 16k .. 16k + 15 span frame rows r0 and r0 + 1 at most
@@ -100,6 +130,27 @@ struct BreakoutPixelsGame {
             for (int j = 0; j < 16; ++j) {
                 const int c = c0 + j;
                 const uint32_t px = c < 84 ? bkp_pixel(p, v0, c) : bkp_pixel(p, v1, c - 84);
+                w[j >> 2] |= px << (8 * (j & 3));
+            }
+            reinterpret_cast<uint4*>(frame)[k] = make_uint4(w[0], w[1], w[2], w[3]);
+        }
+    }
+
+    // render's rule over the objects of both states: two balls, two paddles, the OR of the brick bitmaps (each frame pixel
+    // is a max over objects, so this is the pixel-wise max of the two frames)
+    static __device__ __forceinline__ void render2(const Env& a, const Env& b, unsigned char* frame, int tid) {
+        Env u = a;
+        u.bricks = make_uint4(a.bricks.x | b.bricks.x, a.bricks.y | b.bricks.y, a.bricks.z | b.bricks.z,
+                              a.bricks.w | b.bricks.w);
+        for (int k = tid; k < (int)(FS_FRAME / 16); k += FS_THREADS) {
+            const int r0 = (16 * k) / 84, c0 = 16 * k - 84 * r0;
+            const BkRowView a0 = bkp_row_view(u, r0), a1 = bkp_row_view(u, r0 + 1);
+            const BkRowView b0 = bkp_row_view(b, r0), b1 = bkp_row_view(b, r0 + 1);
+            uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int c = c0 + j;
+                const uint32_t px = c < 84 ? bkp_pixel2(u, b, a0, b0, c) : bkp_pixel2(u, b, a1, b1, c - 84);
                 w[j >> 2] |= px << (8 * (j & 3));
             }
             reinterpret_cast<uint4*>(frame)[k] = make_uint4(w[0], w[1], w[2], w[3]);
@@ -122,13 +173,27 @@ __global__ void __launch_bounds__(FS_THREADS) k_breakout_pixels(BreakoutState st
     frame_stack_run<MODE, BreakoutPixelsGame>(st, n, actions, done, prev, prev_stride, out, acc);
 }
 
+// the same with the Atari preprocessing layer (oracle/SPEC_PIXEL_PREPROCESSING.md)
+template <int MODE>
+__global__ void __launch_bounds__(FS_THREADS, 2) k_breakout_pixels_pp(BreakoutState st, int n, const int64_t* __restrict__ actions,
+                                                                  uint8_t* done, const unsigned char* __restrict__ prev,
+                                                                  int64_t prev_stride, FsOut out, EpisodeAcc acc, FsPre pre) {
+    frame_stack_run<MODE, BreakoutPixelsGame, true>(st, n, actions, done, prev, prev_stride, out, acc, pre);
+}
+
+struct BkpKind {
+    BreakoutState st;
+    FsPre pre;
+};
+
 int bkp_launch(pb_env* env, int mode, const int64_t* actions, const pb_env_out* out, cudaStream_t s) {
-    return fs_launch(env, mode, *(BreakoutState*)env->kind, actions, out, s, k_breakout_pixels<0>, k_breakout_pixels<1>,
-                     "breakout_pixels");
+    const BkpKind* k = (const BkpKind*)env->kind;
+    return fs_launch(env, mode, k->st, actions, out, s, k_breakout_pixels<0>, k_breakout_pixels<1>, k_breakout_pixels_pp<0>,
+                     k_breakout_pixels_pp<1>, k->pre, "breakout_pixels");
 }
 
 int bkp_reset(pb_env* env, uint64_t seed, const pb_env_out* out, cudaStream_t s) {
-    BreakoutState* st = (BreakoutState*)env->kind;
+    BreakoutState* st = &((BkpKind*)env->kind)->st;
     st->seed = seed + (uint64_t)env->cfg.env_index_offset;
     return bkp_launch(env, 0, nullptr, out, s);
 }
@@ -138,10 +203,11 @@ int bkp_step(pb_env* env, const int64_t* actions, const pb_env_out* out, cudaStr
 }
 
 void bkp_destroy(pb_env* env) {
-    BreakoutState* st = (BreakoutState*)env->kind;
-    if (!st) return;
-    cudaFree(st->s0); cudaFree(st->s1); cudaFree(st->bricks); cudaFree(st->ctr);
-    delete st;
+    BkpKind* k = (BkpKind*)env->kind;
+    if (!k) return;
+    cudaFree(k->st.s0); cudaFree(k->st.s1); cudaFree(k->st.bricks); cudaFree(k->st.ctr);
+    fs_pre_destroy(env, k->pre);
+    delete k;
     env->kind = nullptr;
 }
 
@@ -150,8 +216,9 @@ const pb_env_vtable BREAKOUT_PIXELS_VT = {bkp_reset, bkp_step, bkp_destroy};
 }  // namespace
 
 int pb_breakout_pixels_create(pb_env* env) {
-    BreakoutState* st = new BreakoutState();
-    env->kind = st;
+    BkpKind* k = new BkpKind();
+    BreakoutState* st = &k->st;
+    env->kind = k;
     env->vt = &BREAKOUT_PIXELS_VT;
     st->max_ticks = env->cfg.iparam[0] > 0 ? env->cfg.iparam[0] : 4096;
     PB_REQUIRE(st->max_ticks <= 65535, PB_ERR_INVALID, "breakout_pixels: max_ticks must be <= 65535");
@@ -164,6 +231,8 @@ int pb_breakout_pixels_create(pb_env* env) {
     PB_CUDA(cudaMemset(st->s1, 0, n * 4));
     PB_CUDA(cudaMemset(st->bricks, 0, n * 16));
     PB_CUDA(cudaMemset(st->ctr, 0, n * 4));
+    const int rc = fs_pre_create(env, k->pre);
+    if (rc != PB_OK) return rc;
     env->info.obs_dtype = PB_DTYPE_U8;
     env->info.obs_ndim = 3;
     env->info.obs_shape[0] = 4;

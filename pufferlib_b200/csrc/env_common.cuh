@@ -27,6 +27,8 @@ struct pb_env {
     int32_t* d_row_length;
     float* d_row_score;
     double* d_row_score64;   // optional [N]: the score in fp64, for kinds whose score is a python float (NULL otherwise)
+    uint8_t* d_ended;        // optional [N]: 1 where the most recent row ended a game, for kinds where a terminal row
+                             // may not (episodic_life); NULL when every terminal row ends one
     double* d_stats;         // [PB_STAT_SLOTS][4] episodes, sum return, sum length, sum score (slot = warp hash:
                              // same-address atomics serialise in L2, spreading them keeps the step kernel flat)
     double* h_stats_pinned;  // [PB_STAT_SLOTS][4] pinned staging for pb_env_stats_read

@@ -44,13 +44,19 @@ struct PongGame {
         pong_serve(p, seed_e);
     }
 
-    static __device__ __forceinline__ void step(const State& st, int64_t e, int64_t action, uint64_t seed_e, Env& p,
-                                                float& reward, bool& terminal, float& score) {
+    static constexpr int NOOP = 0;
+    static constexpr bool kLives = false;
+
+    static __device__ __forceinline__ void load(const State& st, int64_t e, Env& p) {
         const uint32_t a0 = st.s0[e], a1 = st.s1[e];
         p.ly = a0 & 0xff; p.ry = (a0 >> 8) & 0xff; p.bx = (int)((a0 >> 16) & 0xff) - 2; p.by = (a0 >> 24) & 0xff;
         p.vx = (int)(a1 & 7) - 2; p.vy = (int)((a1 >> 3) & 7) - 2;
         p.score_l = (a1 >> 6) & 15; p.score_r = (a1 >> 10) & 15; p.tick = a1 >> 16;
         p.ctr = st.ctr[e];
+    }
+
+    static __device__ __forceinline__ void tick(const State& st, Env& p, int64_t action, uint64_t seed_e, float& reward,
+                                                bool& terminal, float& score) {
         int a = (int)action;
         a = a < 0 ? 0 : (a > 5 ? 5 : a);
         // dy+3 per action, 3 bits each: NOOP, FIRE -> 0; UP(2,4) -> -3; DOWN(3,5) -> +3   (oracle/SPEC.md §Pong)
@@ -73,6 +79,12 @@ struct PongGame {
         score = (float)(p.score_r - p.score_l);
     }
 
+    static __device__ __forceinline__ void step(const State& st, int64_t e, int64_t action, uint64_t seed_e, Env& p,
+                                                float& reward, bool& terminal, float& score) {
+        load(st, e, p);
+        tick(st, p, action, seed_e, reward, terminal, score);
+    }
+
     // zero fill, then opponent paddle, agent paddle, ball
     static __device__ __forceinline__ void render(const Env& p, unsigned char* frame, int tid) {
         for (int k = tid; k < (int)(FS_FRAME / 16); k += FS_THREADS) reinterpret_cast<uint4*>(frame)[k] = make_uint4(0, 0, 0, 0);
@@ -82,6 +94,22 @@ struct PongGame {
         __syncthreads();   // ball is drawn last (it may overlap a paddle pixel)
         if (tid < 4) {
             const int x = p.bx + (tid & 1), y = p.by + (tid >> 1);
+            if (x >= 0 && x < 84 && y >= 0 && y < 84) frame[y * 84 + x] = 255;
+        }
+    }
+
+    // render's rule over the objects of both states (every pixel is the max over the objects covering it: 128 < 192 <
+    // 255, drawn in that order): four paddles, then two balls
+    static __device__ __forceinline__ void render2(const Env& a, const Env& b, unsigned char* frame, int tid) {
+        for (int k = tid; k < (int)(FS_FRAME / 16); k += FS_THREADS) reinterpret_cast<uint4*>(frame)[k] = make_uint4(0, 0, 0, 0);
+        __syncthreads();
+        const bool pa = tid < 48;                        // fields picked by value: a pointer pick puts Env in local memory
+        const int t = pa ? tid : tid - 48, ly = pa ? a.ly : b.ly, ry = pa ? a.ry : b.ry;
+        if (t < 24) frame[(ly + (t >> 1)) * 84 + 4 + (t & 1)] = 128;
+        else if (t < 48) frame[(ry + ((t - 24) >> 1)) * 84 + 78 + (t & 1)] = 192;
+        __syncthreads();
+        if (tid < 8) {
+            const int x = (tid < 4 ? a.bx : b.bx) + (tid & 1), y = (tid < 4 ? a.by : b.by) + ((tid >> 1) & 1);
             if (x >= 0 && x < 84 && y >= 0 && y < 84) frame[y * 84 + x] = 255;
         }
     }
@@ -102,12 +130,26 @@ __global__ void __launch_bounds__(FS_THREADS) k_pong(PongState st, int n, const 
     frame_stack_run<MODE, PongGame>(st, n, actions, done, prev, prev_stride, out, acc);
 }
 
+// the same with the Atari preprocessing layer (oracle/SPEC_PIXEL_PREPROCESSING.md)
+template <int MODE>
+__global__ void __launch_bounds__(FS_THREADS, 2) k_pong_pp(PongState st, int n, const int64_t* __restrict__ actions,
+                                                       uint8_t* done, const unsigned char* __restrict__ prev,
+                                                       int64_t prev_stride, FsOut out, EpisodeAcc acc, FsPre pre) {
+    frame_stack_run<MODE, PongGame, true>(st, n, actions, done, prev, prev_stride, out, acc, pre);
+}
+
+struct PongKind {
+    PongState st;
+    FsPre pre;
+};
+
 int pong_launch(pb_env* env, int mode, const int64_t* actions, const pb_env_out* out, cudaStream_t s) {
-    return fs_launch(env, mode, *(PongState*)env->kind, actions, out, s, k_pong<0>, k_pong<1>, "pong");
+    const PongKind* k = (const PongKind*)env->kind;
+    return fs_launch(env, mode, k->st, actions, out, s, k_pong<0>, k_pong<1>, k_pong_pp<0>, k_pong_pp<1>, k->pre, "pong");
 }
 
 int pong_reset(pb_env* env, uint64_t seed, const pb_env_out* out, cudaStream_t s) {
-    PongState* st = (PongState*)env->kind;
+    PongState* st = &((PongKind*)env->kind)->st;
     st->seed = seed + (uint64_t)env->cfg.env_index_offset;
     return pong_launch(env, 0, nullptr, out, s);
 }
@@ -117,10 +159,11 @@ int pong_step(pb_env* env, const int64_t* actions, const pb_env_out* out, cudaSt
 }
 
 void pong_destroy(pb_env* env) {
-    PongState* st = (PongState*)env->kind;
-    if (!st) return;
-    cudaFree(st->s0); cudaFree(st->s1); cudaFree(st->ctr);
-    delete st;
+    PongKind* k = (PongKind*)env->kind;
+    if (!k) return;
+    cudaFree(k->st.s0); cudaFree(k->st.s1); cudaFree(k->st.ctr);
+    fs_pre_destroy(env, k->pre);
+    delete k;
     env->kind = nullptr;
 }
 
@@ -129,8 +172,9 @@ const pb_env_vtable PONG_VT = {pong_reset, pong_step, pong_destroy};
 }  // namespace
 
 int pb_pong_create(pb_env* env) {
-    PongState* st = new PongState();
-    env->kind = st;
+    PongKind* k = new PongKind();
+    PongState* st = &k->st;
+    env->kind = k;
     env->vt = &PONG_VT;
     st->max_score = env->cfg.iparam[0] > 0 ? env->cfg.iparam[0] : 5;
     st->max_ticks = env->cfg.iparam[1] > 0 ? env->cfg.iparam[1] : 4096;
@@ -143,6 +187,8 @@ int pb_pong_create(pb_env* env) {
     PB_CUDA(cudaMemset(st->s0, 0, n * 4));
     PB_CUDA(cudaMemset(st->s1, 0, n * 4));
     PB_CUDA(cudaMemset(st->ctr, 0, n * 4));
+    const int rc = fs_pre_create(env, k->pre);
+    if (rc != PB_OK) return rc;
     env->info.obs_dtype = PB_DTYPE_U8;
     env->info.obs_ndim = 3;
     env->info.obs_shape[0] = 4;

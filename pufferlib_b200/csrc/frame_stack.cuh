@@ -14,6 +14,12 @@
 //   G::step(st, e, action, seed_e, p, reward, terminal, score)   load state and run one step of the dynamics
 //   G::render(p, frame, tid)                           all FS_THREADS threads draw the 84x84 frame into shared memory
 //   G::store(st, e, p)                                 thread 0 writes the state back
+// and, for the Atari preprocessing layer (oracle/SPEC_PIXEL_PREPROCESSING.md), which runs only in the FsPre instances:
+//   G::load(st, e, p)                                  load one env's state
+//   G::tick(st, p, action, seed_e, reward, terminal, score)   one tick of the dynamics on loaded state (reward: 0 on entry)
+//   G::render2(a, b, frame, tid)                       the frame drawn from the objects of both states: the pixel-wise
+//                                                      max of render(a) and render(b), in one pass
+//   G::NOOP, G::kLives (and G::lives(p) where kLives)  the no-op action; whether the game has lives
 // Every thread runs reset / step redundantly on the same inputs (broadcast loads), so no barrier is needed before render.
 #pragma once
 #include "env_common.cuh"
@@ -42,13 +48,80 @@ static inline FsOut fs_out(const pb_env* env, const pb_env_out* out) {
                  out->dones_f32, env->write_const};
 }
 
+// The Atari preprocessing options of the pixel kinds (pb_env_config.iparam[2..5]; oracle/SPEC_PIXEL_PREPROCESSING.md).
+// `word` [N] is the wrapper's per-env word: bit 31 = a soft reset (episodic life) is pending, bits 0..30 = real resets
+// since async_reset (the key of the no-op draw).  `ended` [N] = 1 where the row ended a game (only with episodic_life,
+// where a terminal row may not have); it is pb_env.d_ended.
+struct FsPre {
+    uint32_t* word;
+    uint8_t* ended;
+    int frameskip, noop_max, episodic_life, clip_rewards;
+};
+constexpr uint32_t FS_SOFT = 0x80000000u;
+
+static inline bool fs_pre_on(const FsPre& p) {
+    return p.frameskip > 1 || p.noop_max > 0 || p.episodic_life || p.clip_rewards;
+}
+
+// Range check of iparam[2..5] for PONG / BREAKOUT_PIXELS, before anything is allocated.  A skipping game lasts at least
+// four full agent steps, one per frame-stack slot: max_ticks >= 4 * frameskip.  No-ops must not end a game:
+// noop_max < max_ticks, and pong needs max_score >= 2 (a point takes at least 21 ticks from the serve, so 30 no-op ticks
+// hold at most one).
+static inline int fs_pre_check(const pb_env_config* cfg) {
+    const bool pong = cfg->kind == PB_ENV_PONG;
+    const int* ip = cfg->iparam;
+    const int max_ticks = ip[pong ? 1 : 0] > 0 ? ip[pong ? 1 : 0] : 4096;
+    const int max_score = ip[0] > 0 ? ip[0] : 5;
+    PB_REQUIRE(ip[2] >= 0 && ip[2] <= 8, PB_ERR_INVALID, "frameskip must be in [1, 8], got %d", ip[2]);
+    PB_REQUIRE(ip[2] <= 1 || max_ticks >= 4 * ip[2], PB_ERR_INVALID, "frameskip %d needs max_ticks >= %d, got %d", ip[2],
+               4 * ip[2], max_ticks);
+    PB_REQUIRE(ip[3] >= 0 && ip[3] <= 30 && ip[3] < max_ticks, PB_ERR_INVALID,
+               "noop_max must be in [0, 30] and below max_ticks %d, got %d", max_ticks, ip[3]);
+    PB_REQUIRE(ip[4] == 0 || (ip[4] == 1 && !pong), PB_ERR_INVALID,
+               "episodic_life must be 0 or 1, and 0 for pong (no lives), got %d", ip[4]);
+    PB_REQUIRE(ip[5] == 0 || ip[5] == 1, PB_ERR_INVALID, "clip_rewards must be 0 or 1, got %d", ip[5]);
+    PB_REQUIRE(!pong || ip[3] == 0 || max_score >= 2, PB_ERR_INVALID, "pong: noop_max needs max_score >= 2");
+    return PB_OK;
+}
+
+// Reads the (checked) options; allocates the per-env word, and pb_env.d_ended with episodic_life, when any is set.
+static inline int fs_pre_create(pb_env* env, FsPre& pre) {
+    const int* ip = env->cfg.iparam;
+    pre = FsPre{nullptr, nullptr, ip[2] > 0 ? ip[2] : 1, ip[3], ip[4], ip[5]};
+    if (!fs_pre_on(pre)) return PB_OK;
+    const size_t n = (size_t)env->cfg.num_envs;
+    PB_CUDA(cudaMalloc(&pre.word, n * 4));
+    PB_CUDA(cudaMemset(pre.word, 0, n * 4));
+    if (pre.episodic_life) {
+        PB_CUDA(cudaMalloc(&env->d_ended, n));
+        PB_CUDA(cudaMemset(env->d_ended, 0, n));
+        pre.ended = env->d_ended;
+    }
+    return PB_OK;
+}
+
+static inline void fs_pre_destroy(pb_env* env, FsPre& pre) {
+    cudaFree(pre.word);
+    cudaFree(env->d_ended);
+    pre.word = nullptr;
+    env->d_ended = nullptr;
+}
+
 #ifdef __CUDACC__
+// The no-op count draw of a real reset: its own key, so the game's counter stream is untouched; k = real resets of env
+// e since async_reset.
+__device__ __forceinline__ int fs_noops(uint64_t seed_e, uint32_t k, int noop_max) {
+    const uint32_t r = pb_mix32((seed_e ^ 0x6E6F6F705F726E64ull) * 0x9E3779B97F4A7C15ull +
+                                (uint64_t)k * 0xD1B54A32D192ED03ull);
+    return 1 + (int)(r % (uint32_t)noop_max);
+}
+
 // MODE 0: async_reset;  MODE 1: vectoriser send.  The body of a __launch_bounds__(FS_THREADS) kernel with FS_SMEM bytes of
-// dynamic shared memory.
-template <int MODE, class G>
+// dynamic shared memory.  PP: the Atari preprocessing layer (`pre`); PP = false is the plain game, one tick per step.
+template <int MODE, class G, bool PP = false>
 __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int n, const int64_t* __restrict__ actions,
                                                 uint8_t* done, const unsigned char* __restrict__ prev, int64_t prev_stride,
-                                                const FsOut& out, const EpisodeAcc& acc) {
+                                                const FsOut& out, const EpisodeAcc& acc, FsPre pre = FsPre{}) {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bars[FS_STAGES];
     const int tid = threadIdx.x;
@@ -90,11 +163,54 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
         typename G::Env p;
         float reward = 0.f, score = 0.f;
         bool terminal = false;
-        const bool loaded = needs_load(e);     // false -> this row is a reset row
-        if (!loaded) G::reset(st, e, seed_e, MODE == 1, p);
-        else G::step(st, e, actions[e], seed_e, p, reward, terminal, score);
-        // ---- render the new frame into the stage
-        G::render(p, frame, tid);
+        const bool loaded = needs_load(e);     // false -> this row is a reset row (PP: a real or a soft reset)
+        // PP: `raw` / `ticks` = the unclipped reward sum / the game ticks of this row, `ended` = the game ended,
+        // `fresh` = a real reset, `word` = the wrapper word to store
+        float raw = 0.f;
+        int ticks = 0;
+        bool ended = false, fresh = !loaded;
+        uint32_t word = 0u;
+        if constexpr (!PP) {
+            if (!loaded) G::reset(st, e, seed_e, MODE == 1, p);
+            else G::step(st, e, actions[e], seed_e, p, reward, terminal, score);
+            // ---- render the new frame into the stage
+            G::render(p, frame, tid);
+        } else {
+            const uint32_t w = MODE == 1 ? pre.word[e] : 0u;
+            fresh = !loaded && !(w & FS_SOFT);
+            typename G::Env q;                 // the state after the second-to-last tick (max-pooling)
+            if (fresh) {
+                // reset, then 1 + draw % noop_max ticks of NOOP; the frame is the last tick's
+                G::reset(st, e, seed_e, MODE == 1, p);
+                const int noops = pre.noop_max > 0 ? fs_noops(seed_e, w, pre.noop_max) : 0;
+                for (; ticks < noops; ++ticks) {
+                    float r = 0.f;
+                    G::tick(st, p, G::NOOP, seed_e, r, ended, score);
+                    raw += r;
+                }
+                q = p;
+                word = (w + 1u) & ~FS_SOFT;
+            } else {
+                // an agent step, or (soft reset) a NOOP step: up to frameskip ticks, stopping where the game ends
+                G::load(st, e, p);
+                const int a = loaded ? (int)actions[e] : G::NOOP;
+                int lives0 = 0;
+                if constexpr (G::kLives) lives0 = G::lives(p);
+                for (ticks = 0; ticks < pre.frameskip && !ended; ++ticks) {
+                    q = p;
+                    float r = 0.f;
+                    G::tick(st, p, a, seed_e, r, ended, score);
+                    raw += r;
+                }
+                if (ticks == 1) q = p;
+                bool life_lost = false;
+                if constexpr (G::kLives) life_lost = loaded && pre.episodic_life && G::lives(p) < lives0 && G::lives(p) > 0;
+                terminal = ended || life_lost;
+                if (loaded) reward = pre.clip_rewards ? (float)((raw > 0.f) - (raw < 0.f)) : raw;
+                word = (w & ~FS_SOFT) | (life_lost && !ended ? FS_SOFT : 0u);
+            }
+            G::render2(q, p, frame, tid);
+        }
         fence_proxy_async_smem();
         __syncthreads();
         // ---- thread 0: bookkeeping + the bulk stores
@@ -106,13 +222,18 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
             if (out.write_const) out.truncations[e] = 0;
             if (out.write_const) out.masks[e] = 1;
             if (out.dones_f32) out.dones_f32[e] = terminal ? 1.f : 0.f;
-            // EpisodeStats (postprocess.py:22-54), scalar form
-            if (!loaded) { acc.ep_return[e] = 0.0; acc.ep_length[e] = 0; }
+            if constexpr (PP) {
+                pre.word[e] = word;
+                if (pre.ended) pre.ended[e] = ended ? 1 : 0;
+            }
+            // EpisodeStats (postprocess.py:22-54), scalar form; PP: over every tick of the game, raw rewards, reported
+            // where the game ends
+            if (!PP && !loaded) { acc.ep_return[e] = 0.0; acc.ep_length[e] = 0; }
             else {
-                const double ret = acc.ep_return[e] + (double)reward;
-                const int len = acc.ep_length[e] + 1;
+                const double ret = PP ? (fresh ? 0.0 : acc.ep_return[e]) + (double)raw : acc.ep_return[e] + (double)reward;
+                const int len = PP ? (fresh ? 0 : acc.ep_length[e]) + ticks : acc.ep_length[e] + 1;
                 acc.ep_return[e] = ret; acc.ep_length[e] = len;
-                if (terminal) {
+                if (PP ? ended : terminal) {
                     acc.row_return[e] = ret; acc.row_length[e] = len; acc.row_score[e] = score;
                     double* slot = acc.stats + 4 * (blockIdx.x & (PB_STAT_SLOTS - 1));
                     atomicAdd(slot + 0, 1.0); atomicAdd(slot + 1, ret);
@@ -136,17 +257,28 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
 }
 
 // The obs pointer / stride check and the launch: 2 CTAs per SM, at most one per env.  `k0` / `k1` are the game's MODE 0 / 1
-// kernels (__global__ wrappers of frame_stack_run).
-template <class State, class K0, class K1>
+// kernels (__global__ wrappers of frame_stack_run), `p0` / `p1` its preprocessing instances, launched when `pre` sets
+// any option.
+template <class State, class K0, class K1, class P0, class P1>
 int fs_launch(pb_env* env, int mode, const State& st, const int64_t* actions, const pb_env_out* out, cudaStream_t s,
-              K0* k0, K1* k1, const char* who) {
+              K0* k0, K1* k1, P0* p0, P1* p1, const FsPre& pre, const char* who) {
     const int n = env->cfg.num_envs;
     PB_REQUIRE(out->obs_stride % 16 == 0 && ((uintptr_t)out->obs & 15) == 0, PB_ERR_INVALID,
                "%s: obs pointer/stride must be 16-byte aligned", who);
     const FsOut o = fs_out(env, out);
     int grid = PB_NUM_SMS * 2;
     if (grid > n) grid = n;
-    if (mode == 0) {
+    if (fs_pre_on(pre)) {
+        const unsigned char* prev = mode == 0 ? nullptr : (const unsigned char*)env->cur_obs;
+        const int64_t prev_stride = mode == 0 ? 0 : env->cur_obs_stride;
+        if (mode == 0) {
+            PB_CUDA(cudaFuncSetAttribute(p0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_SMEM));
+            p0<<<grid, FS_THREADS, FS_SMEM, s>>>(st, n, actions, env->d_done, prev, prev_stride, o, pb_episode_acc(env), pre);
+        } else {
+            PB_CUDA(cudaFuncSetAttribute(p1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_SMEM));
+            p1<<<grid, FS_THREADS, FS_SMEM, s>>>(st, n, actions, env->d_done, prev, prev_stride, o, pb_episode_acc(env), pre);
+        }
+    } else if (mode == 0) {
         PB_CUDA(cudaFuncSetAttribute(k0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_SMEM));
         k0<<<grid, FS_THREADS, FS_SMEM, s>>>(st, n, actions, env->d_done, nullptr, 0, o, pb_episode_acc(env));
     } else {

@@ -12,6 +12,8 @@ A kind may have several agents per env (multiagent: two); the backend reads that
 import math
 import operator
 
+import numpy as np
+
 from pufferlib_b200.exceptions import APIUsageError
 
 KNOWN_BY_NAME = {'make_squared': 'squared', 'make_breakout': 'breakout', 'make_snake': 'snake', 'make_pong': 'pong',
@@ -64,6 +66,37 @@ def _finite(kind, name, v):
     return v
 
 
+def _flag(kind, name, v):
+    if not isinstance(v, (bool, np.bool_)):
+        raise APIUsageError(f'{kind}: {name} must be a bool, got {v!r}')
+    return int(bool(v))
+
+
+def _atari_options(kind, kwargs, iparam, max_ticks, max_score=None):
+    """The Atari preprocessing keywords of the pixel kinds (oracle/SPEC_PIXEL_PREPROCESSING.md) -> iparam[2..5].
+    Every default is the plain game; no-ops must not be able to end a game, and a skipping game must last at least four
+    full agent steps."""
+    for name in ('frameskip', 'noop_max'):
+        if isinstance(kwargs.get(name), (bool, np.bool_)):
+            raise APIUsageError(f'{kind}: {name} must be an integer, got {kwargs[name]!r}')
+    if 'frameskip' in kwargs:
+        iparam[2] = _int_in(kind, 'frameskip', kwargs.pop('frameskip'), 1, 8)
+        if iparam[2] > 1 and max_ticks < 4 * iparam[2]:     # a game of at least 4 skipped steps, one per stack slot
+            raise APIUsageError(f'{kind}: frameskip {iparam[2]} needs max_ticks >= {4 * iparam[2]}, got {max_ticks}')
+    if 'noop_max' in kwargs:
+        iparam[3] = _int_in(kind, 'noop_max', kwargs.pop('noop_max'), 0, 30)
+        if iparam[3] >= max_ticks:
+            raise APIUsageError(f'{kind}: noop_max must be below max_ticks {max_ticks}, got {iparam[3]}')
+        if iparam[3] and max_score is not None and max_score < 2:   # a point takes >= 21 ticks: two never fit in 30
+            raise APIUsageError(f'{kind}: noop_max needs max_score >= 2, or no-ops could end a game')
+    if 'episodic_life' in kwargs:
+        iparam[4] = _flag(kind, 'episodic_life', kwargs.pop('episodic_life'))
+        if iparam[4] and kind == 'pong':
+            raise APIUsageError('pong: has no lives, so episodic_life is refused')
+    if 'clip_rewards' in kwargs:
+        iparam[5] = _flag(kind, 'clip_rewards', kwargs.pop('clip_rewards'))
+
+
 def resolve(creator, args, kwargs):
     """-> (kind name, iparam list of 8 ints) for pb_env_config."""
     kind, iparam, _ = resolve_config(creator, args, kwargs)
@@ -97,9 +130,13 @@ def resolve_config(creator, args, kwargs):
             raise APIUsageError(f'breakout_pixels: takes max_ticks as a keyword only, got args {list(args)}')
         if 'max_ticks' in kwargs:      # the tick counter is 16 bits of the packed state
             iparam[0] = _int_in(kind, 'max_ticks', kwargs.pop('max_ticks'), 1, 65535)
+        _atari_options(kind, kwargs, iparam, iparam[0] or 4096)
     elif kind == 'pong':
+        if args:
+            raise APIUsageError(f'pong: takes keywords only, got args {list(args)}')
         iparam[0] = int(kwargs.pop('max_score', 0))
         iparam[1] = int(kwargs.pop('max_ticks', 0))
+        _atari_options(kind, kwargs, iparam, iparam[1] if iparam[1] > 0 else 4096, iparam[0] if iparam[0] > 0 else 5)
     elif kind == 'multiagent':
         if args or kwargs:      # make_multiagent() takes no arguments (ocean/environment.py:69-72)
             raise APIUsageError(f'multiagent: takes no arguments, got args {list(args or ())} kwargs {sorted(kwargs)}')

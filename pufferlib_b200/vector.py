@@ -463,7 +463,10 @@ class B200:
         already has them on the host (``term``).  ``rewards``: this step's reward rows (read by the multi-agent kinds)."""
         if self.agents_per_env > 1:
             return self._collect_agent_infos(term, rewards)
-        if term is None:
+        ended = self._game_ended()
+        if ended is not None:       # episodic_life: a terminal row may be a lost life, which ends no episode
+            term = ended
+        elif term is None:
             term = self.buf.terminals.cpu().numpy()
             self.d2h_bytes += term.nbytes
         idx = np.nonzero(term)[0]
@@ -499,6 +502,24 @@ class B200:
             self.d2h_bytes += n * 8
         return [{'episode_return': float(ret[i]), 'episode_length': int(length[i]), 'score': float(score[i])}
                 for i in idx]
+
+    def _game_ended(self):
+        """The device's per-env 'this row ended a game' bytes (pb_env_game_ended) in one device->host copy, or None when
+        every terminal row ends a game (the env has no such array)."""
+        lib = _native.lib()
+        ptrs = []
+        for handle, lo, cnt in self._shards:
+            p = C.c_void_p()
+            _native.check(lib.pb_env_game_ended(handle, C.byref(p)))
+            ptrs.append((p.value, lo, cnt))
+        if not all(p for p, _, _ in ptrs):
+            return None
+        stage = torch.empty(self.num_agents, dtype=torch.uint8, device=self.buf.terminals.device)
+        for p, lo, cnt in ptrs:
+            _native.check(lib.pb_copy_rows(C.c_void_p(p), cnt, C.c_void_p(stage.data_ptr() + lo), cnt, cnt, 1,
+                                           _native.stream_ptr()))
+        self.d2h_bytes += self.num_agents
+        return stage.cpu().numpy().view(np.bool_)
 
     def _collect_agent_infos(self, term, rewards):
         """Multi-agent kinds: for every env whose rows are terminal after this send, in env order, the env's own step

@@ -90,8 +90,11 @@ typedef struct {
                                    [4]=episodic_life 0 / 1 (BREAKOUT_PIXELS only): a lost life is a terminal row,
                                        the next send runs a NOOP step instead of a reset
                                    [5]=clip_rewards 0 / 1: the row reward is the sign of the step's reward sum
-                                 All zero is the plain game, one tick per step.  Values out of range are refused
-                                 with PB_ERR_INVALID by pb_env_create before anything is allocated. */
+                                 PONG and BREAKOUT_PIXELS, the frame stack:
+                                   [6]=framestack 1 or 4 (0 = default 4): frames per observation row, obs_shape
+                                       (S, 84, 84), obs_bytes S * 7056, oldest frame first; 1 is the newest frame alone
+                                 All zero is the plain game, one tick per step, four frames per row.  Values out of
+                                 range are refused with PB_ERR_INVALID by pb_env_create before anything is allocated. */
 } pb_env_config;
 
 typedef struct {
@@ -463,6 +466,24 @@ int pb_conv1_u8_forward_rows(const uint8_t* x, int64_t batch, int32_t steps, int
 int pb_conv1_u8_wgrad_rows(const uint8_t* x, int64_t batch, int32_t steps, int32_t groups, int64_t stride_e,
                            int64_t stride_g, int64_t stride_t, const float* y, const float* dy, float* dw, float* db,
                            void* workspace, size_t workspace_bytes, void* stream);
+
+/* The four entry points above for Conv2d(frames, 32, 8, stride=4) on (frames, 84, 84) rows, frames = 1 (the one-frame
+ * observation of framestack=1, models.Convolutional(framestack=1)) or 4 (what the entry points above are: they are these
+ * with frames = 4, bit for bit).  A row is R = frames * 7056 bytes: row_stride and each stepped stride must be >= R and a
+ * multiple of 16; w is [32][64 * frames] and dw the same; y, dy and the workspace as above
+ * (pb_conv1_u8_wgrad_workspace_bytes covers both values).  frames = 1: K = 64, and the weight gradient keeps the fixed
+ * CTA split and the fixed-order sum, so it is deterministic too.  PB_ERR_INVALID before any launch for frames other
+ * than 1 or 4 and every condition above. */
+int pb_conv1_u8_forward_ex(int32_t frames, const uint8_t* x, int64_t row_stride, int64_t m, const float* w,
+                           const float* b, float* y, void* stream);
+int pb_conv1_u8_wgrad_ex(int32_t frames, const uint8_t* x, int64_t row_stride, int64_t m, const float* y,
+                         const float* dy, float* dw, float* db, void* workspace, size_t workspace_bytes, void* stream);
+int pb_conv1_u8_forward_rows_ex(int32_t frames, const uint8_t* x, int64_t batch, int32_t steps, int32_t groups,
+                                int64_t stride_e, int64_t stride_g, int64_t stride_t, const float* w, const float* b,
+                                float* y, void* stream);
+int pb_conv1_u8_wgrad_rows_ex(int32_t frames, const uint8_t* x, int64_t batch, int32_t steps, int32_t groups,
+                              int64_t stride_e, int64_t stride_g, int64_t stride_t, const float* y, const float* dy,
+                              float* dw, float* db, void* workspace, size_t workspace_bytes, void* stream);
 
 /* -- NatureCNN conv2 and conv3 -----------------------------------------------------------------------------------------
  * The second and third layers of models.Convolutional, each Conv2d + ReLU on fp32 NCHW rows, `layer` = 2 or 3:

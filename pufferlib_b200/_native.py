@@ -109,6 +109,13 @@ SIGNATURES = {
                                  + [C.c_void_p] * 3 + [C.c_void_p]),
     'pb_conv1_u8_wgrad_rows': (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32] + [C.c_int64] * 3
                                + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]),
+    'pb_conv1_u8_forward_ex': (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 3 + [C.c_void_p]),
+    'pb_conv1_u8_wgrad_ex': (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 5
+                             + [C.c_size_t, C.c_void_p]),
+    'pb_conv1_u8_forward_rows_ex': (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32] + [C.c_int64] * 3
+                                    + [C.c_void_p] * 3 + [C.c_void_p]),
+    'pb_conv1_u8_wgrad_rows_ex': (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32] + [C.c_int64] * 3
+                                  + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]),
     'pb_nature_conv_forward': (C.c_int, [C.c_int32, C.c_void_p, C.c_int64] + [C.c_void_p] * 3 + [C.c_void_p]),
     'pb_nature_conv_dgrad': (C.c_int, [C.c_int32] + [C.c_void_p] * 3 + [C.c_int64, C.c_void_p, C.c_void_p]),
     'pb_nature_conv_wgrad_workspace_bytes': (C.c_size_t, [C.c_int32, C.c_int64]),

@@ -1,4 +1,5 @@
-// env_breakout_pixels.cu -- N Breakout instances seen as (4,84,84) uint8 frame stacks (oracle/SPEC_BREAKOUT_PIXELS.md),
+// env_breakout_pixels.cu -- N Breakout instances seen as (4,84,84) (or, framestack=1, (1,84,84)) uint8 frame stacks
+// (oracle/SPEC_BREAKOUT_PIXELS.md),
 // sm_90a: the policy input of the reference's Atari breakout (atari/environment.py:37-39, NatureCNN at atari/torch.py).
 //
 // The game is breakout's, step for step: bk_physics and the 28 B of SoA state from env_breakout.cuh, the same RNG,
@@ -166,30 +167,34 @@ struct BreakoutPixelsGame {
 };
 
 // MODE 0: async_reset;  MODE 1: vectoriser send
-template <int MODE>
+template <int MODE, int S>
 __global__ void __launch_bounds__(FS_THREADS) k_breakout_pixels(BreakoutState st, int n, const int64_t* __restrict__ actions,
                                                                uint8_t* done, const unsigned char* __restrict__ prev,
                                                                int64_t prev_stride, FsOut out, EpisodeAcc acc) {
-    frame_stack_run<MODE, BreakoutPixelsGame>(st, n, actions, done, prev, prev_stride, out, acc);
+    frame_stack_run<MODE, BreakoutPixelsGame, false, S>(st, n, actions, done, prev, prev_stride, out, acc);
 }
 
 // the same with the Atari preprocessing layer (oracle/SPEC_PIXEL_PREPROCESSING.md)
-template <int MODE>
+template <int MODE, int S>
 __global__ void __launch_bounds__(FS_THREADS, 2) k_breakout_pixels_pp(BreakoutState st, int n, const int64_t* __restrict__ actions,
                                                                   uint8_t* done, const unsigned char* __restrict__ prev,
                                                                   int64_t prev_stride, FsOut out, EpisodeAcc acc, FsPre pre) {
-    frame_stack_run<MODE, BreakoutPixelsGame, true>(st, n, actions, done, prev, prev_stride, out, acc, pre);
+    frame_stack_run<MODE, BreakoutPixelsGame, true, S>(st, n, actions, done, prev, prev_stride, out, acc, pre);
 }
 
 struct BkpKind {
     BreakoutState st;
     FsPre pre;
+    int frames;   // S, 4 or 1
 };
 
 int bkp_launch(pb_env* env, int mode, const int64_t* actions, const pb_env_out* out, cudaStream_t s) {
     const BkpKind* k = (const BkpKind*)env->kind;
-    return fs_launch(env, mode, k->st, actions, out, s, k_breakout_pixels<0>, k_breakout_pixels<1>, k_breakout_pixels_pp<0>,
-                     k_breakout_pixels_pp<1>, k->pre, "breakout_pixels");
+    if (k->frames == 1)
+        return fs_launch<1>(env, mode, k->st, actions, out, s, k_breakout_pixels<0, 1>, k_breakout_pixels<1, 1>,
+                            k_breakout_pixels_pp<0, 1>, k_breakout_pixels_pp<1, 1>, k->pre, "breakout_pixels");
+    return fs_launch<4>(env, mode, k->st, actions, out, s, k_breakout_pixels<0, 4>, k_breakout_pixels<1, 4>,
+                        k_breakout_pixels_pp<0, 4>, k_breakout_pixels_pp<1, 4>, k->pre, "breakout_pixels");
 }
 
 int bkp_reset(pb_env* env, uint64_t seed, const pb_env_out* out, cudaStream_t s) {
@@ -233,12 +238,13 @@ int pb_breakout_pixels_create(pb_env* env) {
     PB_CUDA(cudaMemset(st->ctr, 0, n * 4));
     const int rc = fs_pre_create(env, k->pre);
     if (rc != PB_OK) return rc;
+    k->frames = fs_frames(&env->cfg);
     env->info.obs_dtype = PB_DTYPE_U8;
     env->info.obs_ndim = 3;
-    env->info.obs_shape[0] = 4;
+    env->info.obs_shape[0] = k->frames;
     env->info.obs_shape[1] = 84;
     env->info.obs_shape[2] = 84;
-    env->info.obs_bytes = FS_ROW;
+    env->info.obs_bytes = k->frames * FS_FRAME;
     env->info.num_actions = 4;
     env->info.obs_low = 0.f;
     env->info.obs_high = 255.f;

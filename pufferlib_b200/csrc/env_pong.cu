@@ -1,4 +1,4 @@
-// env_pong.cu -- N Pong instances with (4,84,84) uint8 frame-stack observations (oracle/SPEC.md §Pong), sm_90a.
+// env_pong.cu -- N Pong instances with (4,84,84) (or, framestack=1, (1,84,84)) uint8 frame-stack observations (oracle/SPEC.md §Pong), sm_90a.
 //
 // Dynamics are the builder's spec (the reference's pong is ALE behind third-party wrappers: SURVEY.md §0); the
 // observation layout (4,84,84) uint8 NCHW, oldest frame first, is the reference's (atari/environment.py:37-39,
@@ -122,30 +122,35 @@ struct PongGame {
     }
 };
 
-// MODE 0: async_reset;  MODE 1: vectoriser send
-template <int MODE>
+// MODE 0: async_reset;  MODE 1: vectoriser send;  S frames per row
+template <int MODE, int S>
 __global__ void __launch_bounds__(FS_THREADS) k_pong(PongState st, int n, const int64_t* __restrict__ actions,
                                                     uint8_t* done, const unsigned char* __restrict__ prev,
                                                     int64_t prev_stride, FsOut out, EpisodeAcc acc) {
-    frame_stack_run<MODE, PongGame>(st, n, actions, done, prev, prev_stride, out, acc);
+    frame_stack_run<MODE, PongGame, false, S>(st, n, actions, done, prev, prev_stride, out, acc);
 }
 
 // the same with the Atari preprocessing layer (oracle/SPEC_PIXEL_PREPROCESSING.md)
-template <int MODE>
+template <int MODE, int S>
 __global__ void __launch_bounds__(FS_THREADS, 2) k_pong_pp(PongState st, int n, const int64_t* __restrict__ actions,
                                                        uint8_t* done, const unsigned char* __restrict__ prev,
                                                        int64_t prev_stride, FsOut out, EpisodeAcc acc, FsPre pre) {
-    frame_stack_run<MODE, PongGame, true>(st, n, actions, done, prev, prev_stride, out, acc, pre);
+    frame_stack_run<MODE, PongGame, true, S>(st, n, actions, done, prev, prev_stride, out, acc, pre);
 }
 
 struct PongKind {
     PongState st;
     FsPre pre;
+    int frames;   // S, 4 or 1
 };
 
 int pong_launch(pb_env* env, int mode, const int64_t* actions, const pb_env_out* out, cudaStream_t s) {
     const PongKind* k = (const PongKind*)env->kind;
-    return fs_launch(env, mode, k->st, actions, out, s, k_pong<0>, k_pong<1>, k_pong_pp<0>, k_pong_pp<1>, k->pre, "pong");
+    if (k->frames == 1)
+        return fs_launch<1>(env, mode, k->st, actions, out, s, k_pong<0, 1>, k_pong<1, 1>, k_pong_pp<0, 1>, k_pong_pp<1, 1>,
+                            k->pre, "pong");
+    return fs_launch<4>(env, mode, k->st, actions, out, s, k_pong<0, 4>, k_pong<1, 4>, k_pong_pp<0, 4>, k_pong_pp<1, 4>,
+                        k->pre, "pong");
 }
 
 int pong_reset(pb_env* env, uint64_t seed, const pb_env_out* out, cudaStream_t s) {
@@ -189,12 +194,13 @@ int pb_pong_create(pb_env* env) {
     PB_CUDA(cudaMemset(st->ctr, 0, n * 4));
     const int rc = fs_pre_create(env, k->pre);
     if (rc != PB_OK) return rc;
+    k->frames = fs_frames(&env->cfg);
     env->info.obs_dtype = PB_DTYPE_U8;
     env->info.obs_ndim = 3;
-    env->info.obs_shape[0] = 4;
+    env->info.obs_shape[0] = k->frames;
     env->info.obs_shape[1] = 84;
     env->info.obs_shape[2] = 84;
-    env->info.obs_bytes = FS_ROW;
+    env->info.obs_bytes = k->frames * FS_FRAME;
     env->info.num_actions = 6;
     env->info.obs_low = 0.f;
     env->info.obs_high = 255.f;

@@ -1,11 +1,14 @@
-// frame_stack.cuh -- the TMA ring that writes (4,84,84) uint8 frame-stack observation rows, shared by the pixel env
-// kinds (pong: env_pong.cu, breakout_pixels: env_breakout_pixels.cu).  The game is a template parameter; the ring, its
-// mbarrier phases, the store / refill order, the reward / flag rows and EpisodeStats are this one body.
+// frame_stack.cuh -- the TMA ring that writes (S,84,84) uint8 frame-stack observation rows, S = 4 (the default) or 1,
+// shared by the pixel env kinds (pong: env_pong.cu, breakout_pixels: env_breakout_pixels.cu).  The game is a template
+// parameter; the ring, its mbarrier phases, the store / refill order, the reward / flag rows and EpisodeStats are this
+// one body.
 //
 // The 28,224-byte observation row is moved by the TMA engine, never by the LSU: per env one cp.async.bulk pulls the
 // three surviving frames of row t-1 (21,168 B) into a shared-memory stage while the CTA renders the new 84x84 frame
 // into the same stage, then ONE cp.async.bulk pushes the whole 28,224 B row to row t.  A reset row is one rendered
 // frame stored to all 4 slots.  A ring of FS_STAGES stages per CTA keeps 4 envs in flight; 2 CTAs per SM.
+// S = 1 (pb_env_config.iparam[6] = 1, the one-frame observation of a recurrent policy) loads nothing: every row is the
+// rendered frame, 7,056 B, stored by one cp.async.bulk.
 //
 // A game G provides
 //   G::State                                           per-env SoA state in HBM (passed by value to the kernel)
@@ -30,7 +33,11 @@ constexpr uint32_t FS_FRAME = 84 * 84;      // 7056 = 441 * 16
 constexpr uint32_t FS_ROW = 4 * FS_FRAME;   // 28224
 constexpr uint32_t FS_STAGE_BYTES = 28672;  // FS_ROW rounded up to 1 KiB
 constexpr int FS_THREADS = 128;
-constexpr size_t FS_SMEM = (size_t)FS_STAGES * FS_STAGE_BYTES;
+// the stage and the ring of an S-frame row: a stage is S frames rounded up to 1 KiB
+template <int S>
+constexpr uint32_t FS_STAGE_OF = S == 4 ? FS_STAGE_BYTES : 7168u;
+template <int S>
+constexpr size_t FS_SMEM_OF = (size_t)FS_STAGES * FS_STAGE_OF<S>;
 
 struct FsOut {
     unsigned char* obs;
@@ -70,6 +77,7 @@ static inline bool fs_pre_on(const FsPre& p) {
 static inline int fs_pre_check(const pb_env_config* cfg) {
     const bool pong = cfg->kind == PB_ENV_PONG;
     const int* ip = cfg->iparam;
+    PB_REQUIRE(ip[6] == 0 || ip[6] == 1 || ip[6] == 4, PB_ERR_INVALID, "framestack must be 1 or 4, got %d", ip[6]);
     const int max_ticks = ip[pong ? 1 : 0] > 0 ? ip[pong ? 1 : 0] : 4096;
     const int max_score = ip[0] > 0 ? ip[0] : 5;
     PB_REQUIRE(ip[2] >= 0 && ip[2] <= 8, PB_ERR_INVALID, "frameskip must be in [1, 8], got %d", ip[2]);
@@ -83,6 +91,9 @@ static inline int fs_pre_check(const pb_env_config* cfg) {
     PB_REQUIRE(!pong || ip[3] == 0 || max_score >= 2, PB_ERR_INVALID, "pong: noop_max needs max_score >= 2");
     return PB_OK;
 }
+
+// The frames per observation row, S, of a checked config: iparam[6], 0 = the default 4.
+static inline int fs_frames(const pb_env_config* cfg) { return cfg->iparam[6] == 1 ? 1 : 4; }
 
 // Reads the (checked) options; allocates the per-env word, and pb_env.d_ended with episodic_life, when any is set.
 static inline int fs_pre_create(pb_env* env, FsPre& pre) {
@@ -116,9 +127,10 @@ __device__ __forceinline__ int fs_noops(uint64_t seed_e, uint32_t k, int noop_ma
     return 1 + (int)(r % (uint32_t)noop_max);
 }
 
-// MODE 0: async_reset;  MODE 1: vectoriser send.  The body of a __launch_bounds__(FS_THREADS) kernel with FS_SMEM bytes of
-// dynamic shared memory.  PP: the Atari preprocessing layer (`pre`); PP = false is the plain game, one tick per step.
-template <int MODE, class G, bool PP = false>
+// MODE 0: async_reset;  MODE 1: vectoriser send.  The body of a __launch_bounds__(FS_THREADS) kernel with FS_SMEM_OF<S>
+// bytes of dynamic shared memory.  PP: the Atari preprocessing layer (`pre`); PP = false is the plain game, one tick per
+// step.  S: frames per row, 4 or 1.
+template <int MODE, class G, bool PP = false, int S = 4>
 __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int n, const int64_t* __restrict__ actions,
                                                 uint8_t* done, const unsigned char* __restrict__ prev, int64_t prev_stride,
                                                 const FsOut& out, const EpisodeAcc& acc, FsPre pre = FsPre{}) {
@@ -128,11 +140,13 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
     const int64_t step = gridDim.x;
     uint32_t phase[FS_STAGES] = {0, 0, 0, 0};
 
+    static_assert(S == 4 || S == 1, "frame stacks of 4 or 1 frames");
+    constexpr uint32_t STAGE = FS_STAGE_OF<S>;
     auto needs_load = [&](int64_t e) -> bool { return MODE == 1 && done[e] == 0; };
     auto issue_load = [&](int s, int64_t e) {  // thread 0 only
-        if (needs_load(e)) {
+        if (S == 4 && needs_load(e)) {
             mbar_expect_tx(&bars[s], 3 * FS_FRAME);
-            tma_load_1d(smem + (size_t)s * FS_STAGE_BYTES, prev + e * prev_stride + FS_FRAME, 3 * FS_FRAME, &bars[s]);
+            tma_load_1d(smem + (size_t)s * STAGE, prev + e * prev_stride + FS_FRAME, 3 * FS_FRAME, &bars[s]);
         }
     };
 
@@ -147,11 +161,18 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
     int it = 0;
     for (int64_t e = blockIdx.x; e < n; e += step, ++it) {
         const int s = it % FS_STAGES;
-        unsigned char* buf = smem + (size_t)s * FS_STAGE_BYTES;
-        unsigned char* frame = buf + 3 * FS_FRAME;
+        unsigned char* buf = smem + (size_t)s * STAGE;
+        unsigned char* frame = buf + (S - 1) * FS_FRAME;
+        if constexpr (S == 1) {
+            // no refill load waits for the bulk store that last read this stage (FS_STAGES iterations ago, the oldest of
+            // the groups this thread committed): wait for it here, and let the barrier hold every thread back from
+            // rendering into the stage until it has
+            if (tid == 0 && it >= FS_STAGES) tma_wait_read<FS_STAGES - 1>();
+            __syncthreads();
+        }
         // refill the stage that was stored one iteration ago: by now its bulk store has long read shared memory, so
         // this wait does not stall, and the load gets FS_STAGES - 1 iterations of lead time
-        if (tid == 0 && it > 0) {
+        if (S == 4 && tid == 0 && it > 0) {
             const int64_t e_next = e + step * (FS_STAGES - 1);
             if (e_next < n) {
                 tma_wait_read<0>();
@@ -241,7 +262,9 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
                 }
             }
             unsigned char* row = out.obs + e * out.stride;
-            if (loaded) {
+            if (S == 1) {
+                tma_store_1d(row, frame, FS_FRAME);
+            } else if (loaded) {
                 mbar_wait(&bars[s], phase[s]);     // the three old frames have landed
                 tma_store_1d(row, buf, FS_ROW);
             } else {
@@ -249,7 +272,7 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
             }
             tma_commit();
         }
-        if (loaded) phase[s] ^= 1;
+        if (S == 4 && loaded) phase[s] ^= 1;
         // no trailing barrier: the next iteration uses another stage; this stage is refilled by thread 0 at the top of
         // the next iteration (after wait_read) and rendered into FS_STAGES iterations later, behind block barriers
     }
@@ -257,33 +280,34 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
 }
 
 // The obs pointer / stride check and the launch: 2 CTAs per SM, at most one per env.  `k0` / `k1` are the game's MODE 0 / 1
-// kernels (__global__ wrappers of frame_stack_run), `p0` / `p1` its preprocessing instances, launched when `pre` sets
-// any option.
-template <class State, class K0, class K1, class P0, class P1>
+// kernels (__global__ wrappers of frame_stack_run) for S frames per row, `p0` / `p1` its preprocessing instances,
+// launched when `pre` sets any option.
+template <int S, class State, class K0, class K1, class P0, class P1>
 int fs_launch(pb_env* env, int mode, const State& st, const int64_t* actions, const pb_env_out* out, cudaStream_t s,
               K0* k0, K1* k1, P0* p0, P1* p1, const FsPre& pre, const char* who) {
     const int n = env->cfg.num_envs;
     PB_REQUIRE(out->obs_stride % 16 == 0 && ((uintptr_t)out->obs & 15) == 0, PB_ERR_INVALID,
                "%s: obs pointer/stride must be 16-byte aligned", who);
     const FsOut o = fs_out(env, out);
+    constexpr size_t SMEM = FS_SMEM_OF<S>;
     int grid = PB_NUM_SMS * 2;
     if (grid > n) grid = n;
     if (fs_pre_on(pre)) {
         const unsigned char* prev = mode == 0 ? nullptr : (const unsigned char*)env->cur_obs;
         const int64_t prev_stride = mode == 0 ? 0 : env->cur_obs_stride;
         if (mode == 0) {
-            PB_CUDA(cudaFuncSetAttribute(p0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_SMEM));
-            p0<<<grid, FS_THREADS, FS_SMEM, s>>>(st, n, actions, env->d_done, prev, prev_stride, o, pb_episode_acc(env), pre);
+            PB_CUDA(cudaFuncSetAttribute(p0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+            p0<<<grid, FS_THREADS, SMEM, s>>>(st, n, actions, env->d_done, prev, prev_stride, o, pb_episode_acc(env), pre);
         } else {
-            PB_CUDA(cudaFuncSetAttribute(p1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_SMEM));
-            p1<<<grid, FS_THREADS, FS_SMEM, s>>>(st, n, actions, env->d_done, prev, prev_stride, o, pb_episode_acc(env), pre);
+            PB_CUDA(cudaFuncSetAttribute(p1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+            p1<<<grid, FS_THREADS, SMEM, s>>>(st, n, actions, env->d_done, prev, prev_stride, o, pb_episode_acc(env), pre);
         }
     } else if (mode == 0) {
-        PB_CUDA(cudaFuncSetAttribute(k0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_SMEM));
-        k0<<<grid, FS_THREADS, FS_SMEM, s>>>(st, n, actions, env->d_done, nullptr, 0, o, pb_episode_acc(env));
+        PB_CUDA(cudaFuncSetAttribute(k0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+        k0<<<grid, FS_THREADS, SMEM, s>>>(st, n, actions, env->d_done, nullptr, 0, o, pb_episode_acc(env));
     } else {
-        PB_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_SMEM));
-        k1<<<grid, FS_THREADS, FS_SMEM, s>>>(st, n, actions, env->d_done, (const unsigned char*)env->cur_obs,
+        PB_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+        k1<<<grid, FS_THREADS, SMEM, s>>>(st, n, actions, env->d_done, (const unsigned char*)env->cur_obs,
                                              env->cur_obs_stride, o, pb_episode_acc(env));
     }
     PB_LAUNCH_CHECK();

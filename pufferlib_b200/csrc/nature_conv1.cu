@@ -1,5 +1,7 @@
-// nature_conv1.cu -- the first convolution of models.Convolutional (NatureCNN: Conv2d(4, 32, 8, stride=4) + ReLU on
-// (4, 84, 84) uint8 frame stacks, pufferlib/models.py:113-157) read straight from the uint8 rows (sm_90a).
+// nature_conv1.cu -- the first convolution of models.Convolutional (NatureCNN: Conv2d(C, 32, 8, stride=4) + ReLU on
+// (C, 84, 84) uint8 frame stacks, C = framestack = 4 or 1, pufferlib/models.py:113-157) read straight from the uint8 rows
+// (sm_90a).  Both kernels are templates over C; what follows describes C = 4, and C = 1 is the same with K = 64 (4
+// k-pairs), 7 056-byte rows and the weight gradient's warps split as noted there.
 //
 // The stock path runs `network(x.float() / 255)`: two fp32 copies of every frame stack (4 bytes per pixel) before cuDNN
 // reads one, and autograd keeps the scaled copy alive for the weight gradient.  Here the bytes are read once, in place.
@@ -15,6 +17,8 @@
 // k_conv1_wgrad dW[co][k] = sum over rows and pixels of dz * x_col / 255 and db = sum dz, with dz = dy * (y > 0)
 //               (threshold_backward) formed in registers and never written.  Per row: dz -> shared memory (TF32, cvt.rna),
 //               x staged as in the forward; GEMM M = 32 channels, N = 256 k, K = 400 pixels, warp w owning 32 k columns.
+//               C = 1 has 64 k columns: warp w owns columns 32 (w & 1) .. +31 over every fourth 8-pixel k-step from
+//               w >> 1, and the four warps of a column half are summed in shared memory, in warp order, at the end.
 //               Rows are split over a fixed number of CTAs (WG_CTAS, independent of the device) into fp32 partial rows,
 //               summed in a fixed order by k_reduce_partials: two launches on the same inputs give the same bits.
 //
@@ -29,11 +33,13 @@
 
 namespace {
 
-constexpr int C1_ROW = 4 * 84 * 84;     // bytes of one frame stack
 constexpr int C1_PLANE = 84 * 84;
+template <int C>
+constexpr int C1_ROW = C * C1_PLANE;    // bytes of one frame stack
+template <int C>
+constexpr int C1_K = 64 * C;
 constexpr int C1_PIX = 400;             // 20 x 20 output pixels
 constexpr int C1_CO = 32;
-constexpr int C1_K = 256;
 constexpr int C1_Y = C1_CO * C1_PIX;   // floats of one output row
 constexpr int C1_STAGES = 2;
 constexpr float C1_INV255 = 1.0f / 255.0f;
@@ -46,17 +52,20 @@ constexpr int FW_OLD = 20;             // output tile row stride (floats): 16 pi
 constexpr int WG_THREADS = 256;
 constexpr int WG_CTAS = 264;           // row split of the weight gradient: fixed, so the summation order is too
 constexpr int WG_DZLD = 404;           // dz row stride (floats): 400 + 4, conflict-free A-fragment loads
-constexpr int WG_PSTRIDE = C1_CO * C1_K + C1_CO;   // partial row: dW [32][256] | db [32]
+template <int C>
+constexpr int WG_PSTRIDE = C1_CO * C1_K<C> + C1_CO;   // partial row: dW [32][64 C] | db [32]
 
+template <int C>
 struct FwdSmem {
-    unsigned char x[C1_STAGES][C1_ROW];
-    uint4 w[16][4][32];                       // [k-pair][n-tile][lane]: (b0, b1) of both k-steps, TF32 bits
+    unsigned char x[C1_STAGES][C1_ROW<C>];
+    uint4 w[4 * C][4][32];                    // [k-pair][n-tile][lane]: (b0, b1) of both k-steps, TF32 bits
     float out[FW_WARPS][C1_CO][FW_OLD];
     uint64_t bar[C1_STAGES];
 };
 
+template <int C>
 struct WgSmem {
-    unsigned char x[C1_STAGES][C1_ROW];
+    unsigned char x[C1_STAGES][C1_ROW<C>];
     float dz[C1_CO][WG_DZLD];                 // TF32 bits of dz
     uint64_t bar[C1_STAGES];
 };
@@ -87,16 +96,17 @@ struct SegmentRows {          // row r = b*T + t, segment b = (e, g) = (b / grou
     }
 };
 
+template <int C>
 __device__ __forceinline__ void issue_row(unsigned char* dst, uint64_t* bar, const unsigned char* src) {
-    mbar_expect_tx(bar, C1_ROW);
-    tma_load_1d(dst, src, C1_ROW, bar);
+    mbar_expect_tx(bar, C1_ROW<C>);
+    tma_load_1d(dst, src, C1_ROW<C>, bar);
 }
 
-template <class Rows>
+template <int C, class Rows>
 __global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(Rows rows, int64_t m, const float* __restrict__ w,
                                                              const float* __restrict__ b, float* __restrict__ y) {
     extern __shared__ __align__(128) unsigned char dyn[];
-    FwdSmem& s = *reinterpret_cast<FwdSmem*>(dyn);
+    FwdSmem<C>& s = *reinterpret_cast<FwdSmem<C>*>(dyn);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const int64_t n_rows = (m - blockIdx.x + gridDim.x - 1) / gridDim.x;   // rows blockIdx.x + i * gridDim.x
     if (threadIdx.x == 0) {
@@ -106,12 +116,12 @@ __global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(Rows rows, int64_t 
     __syncthreads();
     if (threadIdx.x == 0)
         for (int i = 0; i < C1_STAGES && i < n_rows; ++i)
-            issue_row(s.x[i], &s.bar[i], rows(blockIdx.x + (int64_t)i * gridDim.x));
+            issue_row<C>(s.x[i], &s.bar[i], rows(blockIdx.x + (int64_t)i * gridDim.x));
     // W in B-fragment order (the header comment), rounded to TF32
-    for (int e = threadIdx.x; e < 16 * 4 * 32; e += FW_THREADS) {
+    for (int e = threadIdx.x; e < 4 * C * 4 * 32; e += FW_THREADS) {
         const int p = e >> 7, nt = (e >> 5) & 3, l = e & 31, lg = l >> 2, lt = l & 3;
         const float4 v = __ldg(reinterpret_cast<const float4*>(
-            w + (8 * nt + lg) * C1_K + (p >> 2) * 64 + (2 * (p & 3) + (lt >> 1)) * 8 + 4 * (lt & 1)));
+            w + (8 * nt + lg) * C1_K<C> + (p >> 2) * 64 + (2 * (p & 3) + (lt >> 1)) * 8 + 4 * (lt & 1)));
         s.w[p][nt][l] = make_uint4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w));
     }
     float bias[4][2];
@@ -144,7 +154,7 @@ __global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(Rows rows, int64_t 
 #pragma unroll
                 for (int e = 0; e < 4; ++e) acc[a][nt][e] = 0.f;
 #pragma unroll 2
-        for (int p = 0; p < 16; ++p) {   // k-steps 2p, 2p + 1: channel p >> 2, kernel rows 2 (p & 3) + 0 / 1
+        for (int p = 0; p < 4 * C; ++p) {   // k-steps 2p, 2p + 1: channel p >> 2, kernel rows 2 (p & 3) + 0 / 1
             const int koff = (p >> 2) * C1_PLANE + 2 * (p & 3) * 84 + toff;
             uint4 bf[4];
 #pragma unroll
@@ -164,7 +174,7 @@ __global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(Rows rows, int64_t 
         }
         __syncthreads();   // every warp is done with stage st: refill it with the row after next
         if (threadIdx.x == 0 && i + C1_STAGES < n_rows)
-            issue_row(s.x[st], &s.bar[st], rows(row + (int64_t)C1_STAGES * gridDim.x));
+            issue_row<C>(s.x[st], &s.bar[st], rows(row + (int64_t)C1_STAGES * gridDim.x));
         float* yrow = y + row * C1_Y;
 #pragma unroll
         for (int a = 0; a < FW_MT; ++a) {
@@ -188,11 +198,11 @@ __global__ void __launch_bounds__(FW_THREADS, 2) k_conv1_fwd(Rows rows, int64_t 
     }
 }
 
-template <class Rows>
+template <int C, class Rows>
 __global__ void __launch_bounds__(WG_THREADS, 2) k_conv1_wgrad(Rows rows, int64_t m, const float* __restrict__ y,
                                                                const float* __restrict__ dy, float* __restrict__ partials) {
     extern __shared__ __align__(128) unsigned char dyn[];
-    WgSmem& s = *reinterpret_cast<WgSmem*>(dyn);
+    WgSmem<C>& s = *reinterpret_cast<WgSmem<C>*>(dyn);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const int64_t n_rows = (m - blockIdx.x + gridDim.x - 1) / gridDim.x;
     if (threadIdx.x == 0) {
@@ -202,11 +212,14 @@ __global__ void __launch_bounds__(WG_THREADS, 2) k_conv1_wgrad(Rows rows, int64_
     __syncthreads();
     if (threadIdx.x == 0)
         for (int i = 0; i < C1_STAGES && i < n_rows; ++i)
-            issue_row(s.x[i], &s.bar[i], rows(blockIdx.x + (int64_t)i * gridDim.x));
+            issue_row<C>(s.x[i], &s.bar[i], rows(blockIdx.x + (int64_t)i * gridDim.x));
 
     // warp w: channel c = w >> 1, kernel rows 4 (w & 1) .. +3.  n-tile j, column n <-> kernel row 4 (w & 1) + (n >> 1),
-    // kx = 4 (n & 1) + j: lane g reads the bytes of all four n-tiles as one word
-    const int xoff = (warp >> 1) * C1_PLANE + (4 * (warp & 1) + (g >> 1)) * 84 + 4 * (g & 1);
+    // kx = 4 (n & 1) + j: lane g reads the bytes of all four n-tiles as one word.  C = 1: channel 0, and the k-steps of
+    // pixels 8 (w >> 1) + 32 i
+    const int xoff = (C == 4 ? warp >> 1 : 0) * C1_PLANE + (4 * (warp & 1) + (g >> 1)) * 84 + 4 * (g & 1);
+    const int p_first = C == 4 ? 0 : 8 * (warp >> 1);
+    constexpr int P_STEP = C == 4 ? 8 : 32;
     float acc[2][4][4] = {};
     float dbs[4] = {};   // db of channels warp + 8q, this lane's pixels
     for (int64_t i = 0; i < n_rows; ++i) {
@@ -234,8 +247,8 @@ __global__ void __launch_bounds__(WG_THREADS, 2) k_conv1_wgrad(Rows rows, int64_
         __syncthreads();   // dz staged
         mbar_wait(&s.bar[st], (uint32_t)((i / C1_STAGES) & 1));
         const unsigned char* xs = s.x[st] + xoff;
-#pragma unroll 2
-        for (int p0 = 0; p0 < C1_PIX; p0 += 8) {
+#pragma unroll (C == 4 ? 2 : 1)
+        for (int p0 = p_first; p0 < C1_PIX; p0 += P_STEP) {
             const uint32_t w0 = *reinterpret_cast<const uint32_t*>(xs + pix_base(p0 + t));
             const uint32_t w1 = *reinterpret_cast<const uint32_t*>(xs + pix_base(p0 + t + 4));
             uint32_t fa[2][4];
@@ -257,64 +270,95 @@ __global__ void __launch_bounds__(WG_THREADS, 2) k_conv1_wgrad(Rows rows, int64_
         }
         __syncthreads();   // dz and stage st are free
         if (threadIdx.x == 0 && i + C1_STAGES < n_rows)
-            issue_row(s.x[st], &s.bar[st], rows(row + (int64_t)C1_STAGES * gridDim.x));
+            issue_row<C>(s.x[st], &s.bar[st], rows(row + (int64_t)C1_STAGES * gridDim.x));
     }
     // this CTA's partial row: dW / 255 in k order, then db
-    float* part = partials + (int64_t)blockIdx.x * WG_PSTRIDE;
-    const int kbase = (warp >> 1) * 64 + (4 * (warp & 1)) * 8;
+    float* part = partials + (int64_t)blockIdx.x * WG_PSTRIDE<C>;
+    const int kbase = (C == 4 ? warp >> 1 : 0) * 64 + (4 * (warp & 1)) * 8;
+    if constexpr (C == 1) {
+        // the four pixel quarters of each column half, summed in warp order by warps 0 and 1 (dz is free: the last
+        // iteration ended on a barrier)
+        float* red = &s.dz[0][0] + warp * 32 * 32 + lane;   // [8 warps][32 values][32 lanes]
 #pragma unroll
-    for (int mi = 0; mi < 2; ++mi)
+        for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
+            for (int j = 0; j < 4; ++j)
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int co = 16 * mi + g + 8 * (e >> 1), n = 2 * t + (e & 1);
-                part[co * C1_K + kbase + (n >> 1) * 8 + 4 * (n & 1) + j] = acc[mi][j][e] * C1_INV255;
-            }
+                for (int e = 0; e < 4; ++e) red[(16 * mi + 4 * j + e) * 32] = acc[mi][j][e];
+        __syncthreads();
+        if (warp < 2) {
+#pragma unroll
+            for (int q = 1; q < 4; ++q)
+#pragma unroll
+                for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j)
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) acc[mi][j][e] += red[(2 * q * 32 + 16 * mi + 4 * j + e) * 32];
+        }
+    }
+    if (C == 4 || warp < 2) {
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int co = 16 * mi + g + 8 * (e >> 1), n = 2 * t + (e & 1);
+                    part[co * C1_K<C> + kbase + (n >> 1) * 8 + 4 * (n & 1) + j] = acc[mi][j][e] * C1_INV255;
+                }
+    }
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
         float v = dbs[q];
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-        if (lane == 0) part[C1_CO * C1_K + warp + 8 * q] = v;
+        if (lane == 0) part[C1_CO * C1_K<C> + warp + 8 * q] = v;
     }
 }
 
-int check_rows(const void* x, int64_t row_stride, int64_t m, const char* who) {
+int check_frames(int frames, const char* who) {
+    PB_REQUIRE(frames == 1 || frames == 4, PB_ERR_INVALID, "%s: frames must be 1 or 4, got %d", who, frames);
+    return PB_OK;
+}
+
+int check_rows(int frames, const void* x, int64_t row_stride, int64_t m, const char* who) {
+    const int row = frames * C1_PLANE;
     PB_REQUIRE(m >= 0, PB_ERR_INVALID, "%s: m must not be negative", who);
     PB_REQUIRE(x && ((uintptr_t)x & 15) == 0, PB_ERR_INVALID, "%s: x must be a 16-byte aligned device pointer", who);
-    PB_REQUIRE(row_stride >= C1_ROW && row_stride % 16 == 0, PB_ERR_INVALID,
-               "%s: row_stride %lld must be >= %d and a multiple of 16", who, (long long)row_stride, C1_ROW);
+    PB_REQUIRE(row_stride >= row && row_stride % 16 == 0, PB_ERR_INVALID,
+               "%s: row_stride %lld must be >= %d and a multiple of 16", who, (long long)row_stride, row);
     return PB_OK;
 }
 
 // The segment entry points' checks: batch segments of `steps` rows, every stride (bytes) a whole aligned row or more
-int check_segments(const void* x, int64_t batch, int32_t steps, int32_t groups, int64_t se, int64_t sg, int64_t st,
-                   const char* who) {
+int check_segments(int frames, const void* x, int64_t batch, int32_t steps, int32_t groups, int64_t se, int64_t sg,
+                   int64_t st, const char* who) {
+    const int row = frames * C1_PLANE;
     PB_REQUIRE(batch >= 0 && steps >= 1, PB_ERR_INVALID, "%s: need batch >= 0 and steps >= 1", who);
     PB_REQUIRE(groups >= 1 && batch % groups == 0, PB_ERR_INVALID, "%s: need groups >= 1 dividing batch (got %d, %lld)",
                who, groups, (long long)batch);
     PB_REQUIRE(x && ((uintptr_t)x & 15) == 0, PB_ERR_INVALID, "%s: x must be a 16-byte aligned device pointer", who);
     for (const int64_t stride : {se, sg, st})
-        PB_REQUIRE(stride >= C1_ROW && stride % 16 == 0, PB_ERR_INVALID,
-                   "%s: stride %lld must be >= %d and a multiple of 16", who, (long long)stride, C1_ROW);
+        PB_REQUIRE(stride >= row && stride % 16 == 0, PB_ERR_INVALID,
+                   "%s: stride %lld must be >= %d and a multiple of 16", who, (long long)stride, row);
     return PB_OK;
 }
 
-template <class Rows>
+template <int C, class Rows>
 int forward(const char* who, Rows rows, int64_t m, const float* w, const float* b, float* y, void* stream) {
     PB_REQUIRE(w && b && y && ((uintptr_t)w & 15) == 0 && ((uintptr_t)b & 3) == 0 && ((uintptr_t)y & 15) == 0,
                PB_ERR_INVALID, "%s: w and y must be 16-byte aligned, b 4-byte aligned", who);
     if (m == 0) return PB_OK;
-    const int smem = (int)sizeof(FwdSmem);
-    PB_CUDA(cudaFuncSetAttribute(k_conv1_fwd<Rows>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const int smem = (int)sizeof(FwdSmem<C>);
+    PB_CUDA(cudaFuncSetAttribute(k_conv1_fwd<C, Rows>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const int grid = (int)(m < 2 * (int64_t)PB_NUM_SMS ? m : 2 * (int64_t)PB_NUM_SMS);
-    k_conv1_fwd<<<grid, FW_THREADS, smem, (cudaStream_t)stream>>>(rows, m, w, b, y);
+    k_conv1_fwd<C><<<grid, FW_THREADS, smem, (cudaStream_t)stream>>>(rows, m, w, b, y);
     PB_LAUNCH_CHECK();
     return PB_OK;
 }
 
-template <class Rows>
+template <int C, class Rows>
 int wgrad(const char* who, Rows rows, int64_t m, const float* y, const float* dy, float* dw, float* db, void* workspace,
           size_t workspace_bytes, void* stream) {
     PB_REQUIRE(y && dy && dw && db && workspace && ((uintptr_t)y & 15) == 0 && ((uintptr_t)dy & 15) == 0 &&
@@ -323,55 +367,114 @@ int wgrad(const char* who, Rows rows, int64_t m, const float* y, const float* dy
     PB_REQUIRE(workspace_bytes >= pb_conv1_u8_wgrad_workspace_bytes(m), PB_ERR_INVALID, "%s: workspace too small", who);
     if (m == 0) return PB_OK;
     cudaStream_t s = (cudaStream_t)stream;
-    const int smem = (int)sizeof(WgSmem);
-    PB_CUDA(cudaFuncSetAttribute(k_conv1_wgrad<Rows>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const int smem = (int)sizeof(WgSmem<C>);
+    PB_CUDA(cudaFuncSetAttribute(k_conv1_wgrad<C, Rows>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const int ctas = (int)(m < WG_CTAS ? m : WG_CTAS);
     float* part = (float*)workspace;
-    k_conv1_wgrad<<<ctas, WG_THREADS, smem, s>>>(rows, m, y, dy, part);
+    k_conv1_wgrad<C><<<ctas, WG_THREADS, smem, s>>>(rows, m, y, dy, part);
     PB_LAUNCH_CHECK();
-    k_reduce_partials<<<(C1_CO * C1_K * 32 + 255) / 256, 256, 0, s>>>(part, ctas, WG_PSTRIDE, C1_CO * C1_K, dw);
+    k_reduce_partials<<<(C1_CO * C1_K<C> * 32 + 255) / 256, 256, 0, s>>>(part, ctas, WG_PSTRIDE<C>, C1_CO * C1_K<C>, dw);
     PB_LAUNCH_CHECK();
-    k_reduce_partials<<<(C1_CO * 32 + 255) / 256, 256, 0, s>>>(part + C1_CO * C1_K, ctas, WG_PSTRIDE, C1_CO, db);
+    k_reduce_partials<<<(C1_CO * 32 + 255) / 256, 256, 0, s>>>(part + C1_CO * C1_K<C>, ctas, WG_PSTRIDE<C>, C1_CO, db);
     PB_LAUNCH_CHECK();
     return PB_OK;
+}
+
+// The entry points' bodies: the checks of an S-frame row (frames = S), then the C = frames instance.  Every refusal
+// returns before anything is launched.
+int dense_forward(const char* who, int frames, const uint8_t* x, int64_t row_stride, int64_t m, const float* w,
+                  const float* b, float* y, void* stream) {
+    int rc = check_frames(frames, who);
+    if (rc == PB_OK) rc = check_rows(frames, x, row_stride, m, who);
+    if (rc != PB_OK) return rc;
+    const DenseRows rows{x, row_stride};
+    return frames == 1 ? forward<1>(who, rows, m, w, b, y, stream) : forward<4>(who, rows, m, w, b, y, stream);
+}
+
+int segment_forward(const char* who, int frames, const uint8_t* x, int64_t batch, int32_t steps, int32_t groups,
+                    int64_t se, int64_t sg, int64_t st, const float* w, const float* b, float* y, void* stream) {
+    int rc = check_frames(frames, who);
+    if (rc == PB_OK) rc = check_segments(frames, x, batch, steps, groups, se, sg, st, who);
+    if (rc != PB_OK) return rc;
+    const SegmentRows rows{x, se, sg, st, steps, groups};
+    return frames == 1 ? forward<1>(who, rows, batch * steps, w, b, y, stream)
+                       : forward<4>(who, rows, batch * steps, w, b, y, stream);
+}
+
+int dense_wgrad(const char* who, int frames, const uint8_t* x, int64_t row_stride, int64_t m, const float* y,
+                const float* dy, float* dw, float* db, void* workspace, size_t workspace_bytes, void* stream) {
+    int rc = check_frames(frames, who);
+    if (rc == PB_OK) rc = check_rows(frames, x, row_stride, m, who);
+    if (rc != PB_OK) return rc;
+    const DenseRows rows{x, row_stride};
+    return frames == 1 ? wgrad<1>(who, rows, m, y, dy, dw, db, workspace, workspace_bytes, stream)
+                       : wgrad<4>(who, rows, m, y, dy, dw, db, workspace, workspace_bytes, stream);
+}
+
+int segment_wgrad(const char* who, int frames, const uint8_t* x, int64_t batch, int32_t steps, int32_t groups,
+                  int64_t se, int64_t sg, int64_t st, const float* y, const float* dy, float* dw, float* db,
+                  void* workspace, size_t workspace_bytes, void* stream) {
+    int rc = check_frames(frames, who);
+    if (rc == PB_OK) rc = check_segments(frames, x, batch, steps, groups, se, sg, st, who);
+    if (rc != PB_OK) return rc;
+    const SegmentRows rows{x, se, sg, st, steps, groups};
+    return frames == 1 ? wgrad<1>(who, rows, batch * steps, y, dy, dw, db, workspace, workspace_bytes, stream)
+                       : wgrad<4>(who, rows, batch * steps, y, dy, dw, db, workspace, workspace_bytes, stream);
 }
 
 }  // namespace
 
 extern "C" int pb_conv1_u8_forward(const uint8_t* x, int64_t row_stride, int64_t m, const float* w, const float* b, float* y,
                                    void* stream) {
-    const int rc = check_rows(x, row_stride, m, "pb_conv1_u8_forward");
-    if (rc != PB_OK) return rc;
-    return forward("pb_conv1_u8_forward", DenseRows{x, row_stride}, m, w, b, y, stream);
+    return dense_forward("pb_conv1_u8_forward", 4, x, row_stride, m, w, b, y, stream);
 }
 
 extern "C" int pb_conv1_u8_forward_rows(const uint8_t* x, int64_t batch, int32_t steps, int32_t groups, int64_t stride_e,
                                         int64_t stride_g, int64_t stride_t, const float* w, const float* b, float* y,
                                         void* stream) {
-    const char* who = "pb_conv1_u8_forward_rows";
-    const int rc = check_segments(x, batch, steps, groups, stride_e, stride_g, stride_t, who);
-    if (rc != PB_OK) return rc;
-    return forward(who, SegmentRows{x, stride_e, stride_g, stride_t, steps, groups}, batch * steps, w, b, y, stream);
+    return segment_forward("pb_conv1_u8_forward_rows", 4, x, batch, steps, groups, stride_e, stride_g, stride_t, w, b, y,
+                           stream);
 }
 
-extern "C" size_t pb_conv1_u8_wgrad_workspace_bytes(int64_t m) {
+extern "C" size_t pb_conv1_u8_wgrad_workspace_bytes(int64_t m) {   // both C: a C = 1 partial row is the shorter one
     const int64_t ctas = m < WG_CTAS ? m : WG_CTAS;
-    return ctas <= 0 ? 16 : (size_t)ctas * WG_PSTRIDE * sizeof(float);
+    return ctas <= 0 ? 16 : (size_t)ctas * WG_PSTRIDE<4> * sizeof(float);
 }
 
 extern "C" int pb_conv1_u8_wgrad(const uint8_t* x, int64_t row_stride, int64_t m, const float* y, const float* dy, float* dw,
                                  float* db, void* workspace, size_t workspace_bytes, void* stream) {
-    const int rc = check_rows(x, row_stride, m, "pb_conv1_u8_wgrad");
-    if (rc != PB_OK) return rc;
-    return wgrad("pb_conv1_u8_wgrad", DenseRows{x, row_stride}, m, y, dy, dw, db, workspace, workspace_bytes, stream);
+    return dense_wgrad("pb_conv1_u8_wgrad", 4, x, row_stride, m, y, dy, dw, db, workspace, workspace_bytes, stream);
 }
 
 extern "C" int pb_conv1_u8_wgrad_rows(const uint8_t* x, int64_t batch, int32_t steps, int32_t groups, int64_t stride_e,
                                       int64_t stride_g, int64_t stride_t, const float* y, const float* dy, float* dw,
                                       float* db, void* workspace, size_t workspace_bytes, void* stream) {
-    const char* who = "pb_conv1_u8_wgrad_rows";
-    const int rc = check_segments(x, batch, steps, groups, stride_e, stride_g, stride_t, who);
-    if (rc != PB_OK) return rc;
-    return wgrad(who, SegmentRows{x, stride_e, stride_g, stride_t, steps, groups}, batch * steps, y, dy, dw, db,
-                 workspace, workspace_bytes, stream);
+    return segment_wgrad("pb_conv1_u8_wgrad_rows", 4, x, batch, steps, groups, stride_e, stride_g, stride_t, y, dy, dw, db,
+                         workspace, workspace_bytes, stream);
+}
+
+extern "C" int pb_conv1_u8_forward_ex(int32_t frames, const uint8_t* x, int64_t row_stride, int64_t m, const float* w,
+                                      const float* b, float* y, void* stream) {
+    return dense_forward("pb_conv1_u8_forward_ex", frames, x, row_stride, m, w, b, y, stream);
+}
+
+extern "C" int pb_conv1_u8_forward_rows_ex(int32_t frames, const uint8_t* x, int64_t batch, int32_t steps, int32_t groups,
+                                           int64_t stride_e, int64_t stride_g, int64_t stride_t, const float* w,
+                                           const float* b, float* y, void* stream) {
+    return segment_forward("pb_conv1_u8_forward_rows_ex", frames, x, batch, steps, groups, stride_e, stride_g, stride_t, w,
+                           b, y, stream);
+}
+
+extern "C" int pb_conv1_u8_wgrad_ex(int32_t frames, const uint8_t* x, int64_t row_stride, int64_t m, const float* y,
+                                    const float* dy, float* dw, float* db, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+    return dense_wgrad("pb_conv1_u8_wgrad_ex", frames, x, row_stride, m, y, dy, dw, db, workspace, workspace_bytes, stream);
+}
+
+extern "C" int pb_conv1_u8_wgrad_rows_ex(int32_t frames, const uint8_t* x, int64_t batch, int32_t steps, int32_t groups,
+                                         int64_t stride_e, int64_t stride_g, int64_t stride_t, const float* y,
+                                         const float* dy, float* dw, float* db, void* workspace, size_t workspace_bytes,
+                                         void* stream) {
+    return segment_wgrad("pb_conv1_u8_wgrad_rows_ex", frames, x, batch, steps, groups, stride_e, stride_g, stride_t, y, dy,
+                         dw, db, workspace, workspace_bytes, stream);
 }

@@ -97,6 +97,21 @@ def _atari_options(kind, kwargs, iparam, max_ticks, max_score=None):
         iparam[5] = _flag(kind, 'clip_rewards', kwargs.pop('clip_rewards'))
 
 
+def _framestack(kind, kwargs, iparam):
+    """The pixel kinds' `framestack` keyword -> iparam[6]: frames per observation row, (S, 84, 84).  4 is the default
+    (iparam[6] = 0) and 1 the one-frame observation for a recurrent policy, the two the reference recommends
+    (models.Convolutional: 1 frame with an LSTM, 4 without)."""
+    if 'framestack' not in kwargs:
+        return
+    v = kwargs.pop('framestack')
+    if isinstance(v, (bool, np.bool_)):
+        raise APIUsageError(f'{kind}: framestack must be an integer, 1 or 4, got {v!r}')
+    v = _int_in(kind, 'framestack', v, 1, 4)
+    if v not in (1, 4):
+        raise APIUsageError(f'{kind}: framestack must be 1 (with an LSTM) or 4 (without), got {v}')
+    iparam[6] = v
+
+
 def resolve(creator, args, kwargs):
     """-> (kind name, iparam list of 8 ints) for pb_env_config."""
     kind, iparam, _ = resolve_config(creator, args, kwargs)
@@ -131,12 +146,14 @@ def resolve_config(creator, args, kwargs):
         if 'max_ticks' in kwargs:      # the tick counter is 16 bits of the packed state
             iparam[0] = _int_in(kind, 'max_ticks', kwargs.pop('max_ticks'), 1, 65535)
         _atari_options(kind, kwargs, iparam, iparam[0] or 4096)
+        _framestack(kind, kwargs, iparam)
     elif kind == 'pong':
         if args:
             raise APIUsageError(f'pong: takes keywords only, got args {list(args)}')
         iparam[0] = int(kwargs.pop('max_score', 0))
         iparam[1] = int(kwargs.pop('max_ticks', 0))
         _atari_options(kind, kwargs, iparam, iparam[1] if iparam[1] > 0 else 4096, iparam[0] if iparam[0] > 0 else 5)
+        _framestack(kind, kwargs, iparam)
     elif kind == 'multiagent':
         if args or kwargs:      # make_multiagent() takes no arguments (ocean/environment.py:69-72)
             raise APIUsageError(f'multiagent: takes no arguments, got args {list(args or ())} kwargs {sorted(kwargs)}')
@@ -152,6 +169,8 @@ def resolve_config(creator, args, kwargs):
         else:
             iparam[0] = _int_in(kind, 'num_actions', v['num_actions'], 1, 1 << 15)
             dparam = [_finite(kind, 'reward_scale', v['reward_scale']), _finite(kind, 'reward_noise', v['reward_noise'])]
+    if 'framestack' in kwargs:
+        raise APIUsageError(f'{kind}: framestack is an option of the pixel kinds (pong, breakout_pixels) only')
     if kwargs:
         raise APIUsageError(f'{kind}: unexpected env kwargs {sorted(kwargs)}')
     return kind, iparam, dparam

@@ -2,7 +2,7 @@
 
 Same architecture and call convention as the reference (adjacent to the hot path, not rewritten):
   Default        reference pufferlib/models.py:12-62   Linear(prod(obs)->hidden)+ReLU; heads hidden->n_act, ->1
-  Convolutional  reference pufferlib/models.py:113-157 NatureCNN for (4,84,84) uint8 (atari/torch.py:8-18)
+  Convolutional  reference pufferlib/models.py:113-157 NatureCNN for (S,84,84) uint8, S = framestack (atari/torch.py:8-18)
   layer_init     reference pufferlib/pytorch.py:193-199
 """
 import numpy as np
@@ -461,23 +461,27 @@ class LSTMWrapper(nn.Module):
         return logits, value, state
 
 
-_CONV1_ROW = 4 * 84 * 84     # bytes of one (4, 84, 84) uint8 frame stack
+_CONV1_FRAME = 84 * 84     # bytes of one 84 x 84 uint8 frame; a frame stack of S frames is S of them
+_CONV1_FRAMES = (1, 4)     # the frame-stack depths S conv1's kernels take (framestack=1 with an LSTM, 4 without)
 
 
 class _Conv1U8Function(torch.autograd.Function):
-    """relu(conv1(x / 255) + b) of NatureCNN (Conv2d(4, 32, 8, stride=4) on (4, 84, 84) uint8 frame stacks) as one
-    autograd node: pb_conv1_u8_forward reads the uint8 rows in place and writes y [M, 32, 20, 20]; the backward
-    (pb_conv1_u8_wgrad) takes the ReLU's gradient rule and the weight and bias gradients from y, dy and the same bytes.
-    x gets no gradient (conv1 is the first layer), so only y is saved beside it.
-    x is either rows [M, 4, 84, 84] or the segment view [E, G, T, 4, 84, 84] of Experience.segment_obs (segment
-    b = e*G + g; pb_conv1_u8_forward_rows / _wgrad_rows), whose y rows are b*T + t.  The view itself is saved, not a copy."""
+    """relu(conv1(x / 255) + b) of NatureCNN (Conv2d(S, 32, 8, stride=4) on (S, 84, 84) uint8 frame stacks, S = 1 or
+    4) as one autograd node: pb_conv1_u8_forward_ex reads the uint8 rows in place and writes y [M, 32, 20, 20]; the
+    backward (pb_conv1_u8_wgrad_ex) takes the ReLU's gradient rule and the weight and bias gradients from y, dy and the
+    same bytes.  x gets no gradient (conv1 is the first layer), so only y is saved beside it.
+    x is either rows [M, S, 84, 84] or the segment view [E, G, T, S, 84, 84] of Experience.segment_obs (segment
+    b = e*G + g; pb_conv1_u8_forward_rows_ex / _wgrad_rows_ex), whose y rows are b*T + t.  The view itself is saved, not
+    a copy."""
 
     @staticmethod
     def _segments(x):
         """(batch, steps, groups, stride_e, stride_g, stride_t) of a segment view, in bytes.  A dimension of size 1 is
-        never stepped over, so its stride is whatever torch reports; it is passed as one row, which the kernel accepts."""
+        never stepped over, so its stride is whatever torch reports; it is passed as one S-frame row, which the kernel
+        accepts."""
         e_, g_, steps = x.shape[:3]
-        st = [x.stride(i) if x.shape[i] > 1 else _CONV1_ROW for i in range(3)]
+        row = x.shape[3] * _CONV1_FRAME
+        st = [x.stride(i) if x.shape[i] > 1 else row for i in range(3)]
         return e_ * g_, steps, g_, st[0], st[1], st[2]
 
     @staticmethod
@@ -486,12 +490,14 @@ class _Conv1U8Function(torch.autograd.Function):
         P, lib = _native.ptr, _native.lib()
         seg = x.dim() == 6
         m = x.shape[0] * x.shape[1] * x.shape[2] if seg else x.shape[0]
+        frames = x.shape[-3]
         y = torch.empty(m, 32, 20, 20, dtype=torch.float32, device=x.device)
         if seg:
-            _native.check(lib.pb_conv1_u8_forward_rows(P(x), *_Conv1U8Function._segments(x), P(w), P(b), P(y),
-                                                       _native.stream_ptr()))
+            _native.check(lib.pb_conv1_u8_forward_rows_ex(frames, P(x), *_Conv1U8Function._segments(x), P(w), P(b), P(y),
+                                                          _native.stream_ptr()))
         else:
-            _native.check(lib.pb_conv1_u8_forward(P(x), x.stride(0), m, P(w), P(b), P(y), _native.stream_ptr()))
+            _native.check(lib.pb_conv1_u8_forward_ex(frames, P(x), x.stride(0), m, P(w), P(b), P(y),
+                                                     _native.stream_ptr()))
         ctx.save_for_backward(x, y)
         return y
 
@@ -501,15 +507,16 @@ class _Conv1U8Function(torch.autograd.Function):
         x, y = ctx.saved_tensors
         dy = dy.contiguous()
         m, lib, P = y.shape[0], _native.lib(), _native.ptr
-        dw = torch.empty(32, 4, 8, 8, dtype=torch.float32, device=x.device)
+        frames = x.shape[-3]
+        dw = torch.empty(32, frames, 8, 8, dtype=torch.float32, device=x.device)
         db = torch.empty(32, dtype=torch.float32, device=x.device)
         ws = torch.empty(lib.pb_conv1_u8_wgrad_workspace_bytes(m), dtype=torch.uint8, device=x.device)
         if x.dim() == 6:
-            _native.check(lib.pb_conv1_u8_wgrad_rows(P(x), *_Conv1U8Function._segments(x), P(y), P(dy), P(dw), P(db),
-                                                     P(ws), ws.numel(), _native.stream_ptr()))
+            _native.check(lib.pb_conv1_u8_wgrad_rows_ex(frames, P(x), *_Conv1U8Function._segments(x), P(y), P(dy), P(dw),
+                                                        P(db), P(ws), ws.numel(), _native.stream_ptr()))
         else:
-            _native.check(lib.pb_conv1_u8_wgrad(P(x), x.stride(0), m, P(y), P(dy), P(dw), P(db), P(ws), ws.numel(),
-                                                _native.stream_ptr()))
+            _native.check(lib.pb_conv1_u8_wgrad_ex(frames, P(x), x.stride(0), m, P(y), P(dy), P(dw), P(db), P(ws),
+                                                   ws.numel(), _native.stream_ptr()))
         return None, dw, db
 
 
@@ -575,26 +582,29 @@ class Convolutional(nn.Module):
         return self.decode_actions(hidden, lookup)
 
     def _conv1_u8_ok(self, x):
-        """Can pb_conv1_u8_forward run the first layer on x?  CUDA uint8 [M, 4, 84, 84] with every row one contiguous
+        """Can pb_conv1_u8_forward_ex run the first layer on x?  CUDA uint8 [M, S, 84, 84] with every row one contiguous
         frame stack (rows 16-byte aligned), channels-first frames at full resolution, and the stock
-        Conv2d(4, 32, 8, stride=4) + ReLU with fp32 parameters first."""
+        Conv2d(S, 32, 8, stride=4) + ReLU with fp32 parameters first, S = framestack = 1 or 4."""
         return x.dim() == 4 and x.stride(0) % 16 == 0 and self._frames_ok(x)
 
     def _conv1_segments_ok(self, x):
-        """The same for a segment view [E, G, T, 4, 84, 84] (Experience.segment_obs) and pb_conv1_u8_forward_rows: every
-        frame stack contiguous, and each of E, G, T that is stepped over (size > 1) a multiple of 16 bytes and at least
-        one frame stack apart."""
+        """The same for a segment view [E, G, T, S, 84, 84] (Experience.segment_obs) and pb_conv1_u8_forward_rows_ex:
+        every frame stack contiguous, and each of E, G, T that is stepped over (size > 1) a multiple of 16 bytes and at
+        least one frame stack (S * 7056 bytes) apart."""
         return (x.dim() == 6 and self._frames_ok(x)
-                and all(x.stride(i) % 16 == 0 and x.stride(i) >= _CONV1_ROW for i in range(3) if x.shape[i] > 1))
+                and all(x.stride(i) % 16 == 0 and x.stride(i) >= x.shape[3] * _CONV1_FRAME
+                        for i in range(3) if x.shape[i] > 1))
 
     def _frames_ok(self, x):
-        """_conv1_u8_ok's conditions on the trailing (4, 84, 84) dimensions of x and on the module."""
+        """_conv1_u8_ok's conditions on the trailing (S, 84, 84) dimensions of x, S = conv1's in_channels = 1 or 4, and
+        on the module."""
         conv = self.network[0]
         if not (self.fast_path and not self.channels_last and self.downsample == 1 and x.is_cuda
-                and x.dtype == torch.uint8 and tuple(x.shape[-3:]) == (4, 84, 84)
-                and tuple(x.stride()[-3:]) == (7056, 84, 1) and x.data_ptr() % 16 == 0):
+                and x.dtype == torch.uint8 and x.dim() >= 3 and x.shape[-3] in _CONV1_FRAMES
+                and tuple(x.shape[-2:]) == (84, 84) and tuple(x.stride()[-3:]) == (7056, 84, 1)
+                and x.data_ptr() % 16 == 0):
             return False
-        return (type(conv) is nn.Conv2d and type(self.network[1]) is nn.ReLU and conv.in_channels == 4
+        return (type(conv) is nn.Conv2d and type(self.network[1]) is nn.ReLU and conv.in_channels == x.shape[-3]
                 and conv.out_channels == 32 and conv.kernel_size == (8, 8) and conv.stride == (4, 4)
                 and conv.padding == (0, 0) and conv.dilation == (1, 1) and conv.groups == 1
                 and conv.padding_mode == 'zeros' and conv.bias is not None
@@ -633,8 +643,8 @@ class Convolutional(nn.Module):
 
     def encode_segments(self, view):
         """encode_observations for the bptt segments of a training minibatch read in place: the segment view
-        [E, G, T, 4, 84, 84] of Experience.segment_obs (segment b = e*G + g) -> hidden [E*G*T, 512] in row order b*T + t,
-        what encode_observations gives for the gathered copy [E*G*T, 4, 84, 84] of the same rows, bit for bit.  None when
+        [E, G, T, S, 84, 84] of Experience.segment_obs (segment b = e*G + g) -> hidden [E*G*T, 512] in row order b*T + t,
+        what encode_observations gives for the gathered copy [E*G*T, S, 84, 84] of the same rows, bit for bit.  None when
         conv1's kernel cannot read the view (_conv1_segments_ok) or it is empty; the view is never reshaped (that would
         copy it)."""
         if view.dim() != 6 or view.numel() == 0 or not self._conv1_segments_ok(view):

@@ -388,9 +388,34 @@ class _DefaultMLPUpdate:
                                                   _native.ptr(self.tail), _native.ptr(self.ws), self.ws.numel(), rows, s))
         self._dw_enc(self.dpre, x)
 
-    def all_reduce(self):
+    # train()'s minibatch loop drives this object as it drives _AutogradUpdate
+    def begin(self, data, kl_stop):
+        self.config, self.profile, self.experience, self.kl_stop = data.config, data.profile, data.experience, kl_stop
+        self.pack_heads()                        # the parameters may have changed since the last train() (checkpoints)
+        if kl_stop is not None and self.stats is not None:
+            self.stats.zero_()                   # rows of epochs that do not run must add nothing to loss_means
+
+    def graph_key(self, epoch, mb):
+        return 'fb', epoch, mb                   # each (epoch, minibatch) writes its own statistics row
+
+    def train_minibatch(self, epoch, mb):
+        n_mb, config = self.experience.num_minibatches, self.config
+        with self.profile.train_forward:
+            self.forward_backward(epoch * n_mb + mb, config.update_epochs * n_mb, self.experience.minibatch(mb), config)
+
+    def exchange(self, kl):
         if self.world > 1 and self.peer is None:
-            torch.distributed.all_reduce(self.gflat)
+            torch.distributed.all_reduce(self.gflat)         # ONE NCCL all-reduce (sum; 1/world folded into the step)
+
+    def step(self, epoch, mb, kl):               # with peers, the exchange before a stop decision carries the KL row sum
+        kl_row = epoch * self.experience.num_minibatches + mb if kl and self.peer is not None else None
+        self.optimizer_step(self.config, kl_row, self.kl_stop.kl_sum if kl_row is not None else None)
+
+    def kl_args(self, epoch):
+        last = (epoch + 1) * self.experience.num_minibatches - 1
+        if self.world == 1:
+            return dict(stats=self.stats, row=last, rows=self.mb_rows)
+        return _ranks_kl_args(self.kl_stop, self.world * self.mb_rows, self.stats[last, 4:5] if self.peer is None else None)
 
     @torch.no_grad()
     def optimizer_step(self, config, kl_row=None, kl_out=None):
@@ -948,7 +973,8 @@ def _rollout_loop(data, infos):
 
 def update_plan(data):
     """How this train() runs, decided on the host after sort_training_data and before anything is launched or captured.
-    Returns namespace(engine, form, capture, manual).  engine, what runs one minibatch's forward, loss and backward:
+    Returns namespace(engine, form, capture, manual, bptt_peer, update, kl_stop).  engine, what runs one minibatch's
+    forward, loss and backward:
         'mlp_fused'  _DefaultMLPUpdate on pb_mlp_update_fused (one kernel per minibatch)
         'mlp_chain'  _DefaultMLPUpdate's hand-written kernel chain
         'packed'     autograd through Default.forward_packed(_slabs) + fused_ppo_loss_packed
@@ -965,8 +991,9 @@ def update_plan(data):
     graph), 'segments' (per-segment graphs around an NCCL all-reduce, _SegmentGraphs) or None (eager).  manual: this call's
     _DefaultMLPUpdate (built here, and rebuilt when optimizer.load_state_dict() replaced the Adam state it holds), or None.
     bptt_peer: the 'bptt' engine on several ranks takes its gradient mean from the peer exchange of data.grad_bucket
-    (GradBucket.open_peer, tried once here) rather than from NCCL.
-    Sets data.manual_update, train_minibatch_path, train_recurrent_path and manual.used_fused."""
+    (GradBucket.open_peer, tried once here) rather than from NCCL.  update: what train()'s minibatch loop drives, manual or
+    an _AutogradUpdate for the engine.  kl_stop: the device-side target_kl stop (_KLStop), or None (no target_kl, or one
+    epoch).  Sets data.manual_update, train_minibatch_path, train_recurrent_path and manual.used_fused."""
     config, exp, model = data.config, data.experience, getattr(data.policy, 'policy', None)
     if data.manual_update is not None and data.manual_update.stale():
         # the hand-written update and any captured graph hold the old addresses: rebuild both (eager call now, capture
@@ -1038,11 +1065,16 @@ def update_plan(data):
                 (engine == 'cudnn_conv' and data.grad_bucket is None):
             capture = 'whole'           # the cuDNN path and recurrent updates on several ranks over NCCL stay eager
 
+    kl_stop = None
+    if config.target_kl is not None and config.update_epochs > 1:
+        kl_stop = data.train_kl_stop = data.train_kl_stop or _KLStop(exp.device, ranks=data.grad_bucket is not None)
     data.train_minibatch_path = form
     data.train_recurrent_path = {'bptt': 'fused', 'cudnn': 'cudnn', 'cudnn_conv': 'cudnn'}.get(engine)
     if manual is not None:
         manual.used_fused = engine == 'mlp_fused'
-    return pufferlib_b200.namespace(engine=engine, form=form, capture=capture, manual=manual, bptt_peer=bptt_peer)
+    update = manual if manual is not None else _AutogradUpdate(data, engine, form, bptt_peer)
+    return pufferlib_b200.namespace(engine=engine, form=form, capture=capture, manual=manual, bptt_peer=bptt_peer,
+                                    update=update, kl_stop=kl_stop)
 
 
 def _invalidate_policy_cache(data):
@@ -1223,6 +1255,7 @@ class _SegmentGraphs:
         self.graphs = {}
         self.launches = {}
         self.replays = 0
+        self.replayed_launches = 0
 
     def run(self, key, fn):
         g = self.graphs.get(key)
@@ -1237,7 +1270,7 @@ class _SegmentGraphs:
             self.launches[key] = _native.lib().pb_launch_count() - l0
         g.replay()
         self.replays += 1
-        self.replayed_launches = getattr(self, 'replayed_launches', 0) + self.launches[key]
+        self.replayed_launches += self.launches[key]
 
 
 def _ppo_loss(newlogprob, entropy, newvalue, log_probs, adv, ret, val, config):
@@ -1270,162 +1303,141 @@ def _ppo_loss(newlogprob, entropy, newvalue, log_probs, adv, ret, val, config):
     return loss, stats
 
 
-def _train_device_part(data, plan, seg=None):
-    """Everything of train() that runs on the device without touching the host: GAE, minibatch construction, the
-    update_epochs x num_minibatches optimizer steps, the loss statistics, the way `plan` (update_plan) says.  No
-    synchronisation inside, so the whole thing can be captured in ONE CUDA graph (single GPU, see train) or, with
-    ``seg``, as per-segment graphs around the gradient all-reduce (multi-GPU)."""
-    config, profile, experience = data.config, data.profile, data.experience
-    device = experience.device
-    _invalidate_policy_cache(data)     # nothing cached by the rollout (eager or captured) may leak into an update graph
-    manual, engine, model = plan.manual, plan.engine, getattr(data.policy, 'policy', None)
-    with profile.train_misc:
-        experience.prepare(plan.form, config)
+def _ranks_kl_args(kl_stop, rows, own_sum):
+    """_KLStop.decide's arguments on several ranks: the KL sum over all ranks' `rows` rows.  The peer exchange left it in
+    kl_stop.kl_sum (own_sum None); otherwise an NCCL all-reduce of this rank's fp64 row sum own_sum forms it."""
+    if own_sum is not None:
+        kl_stop.kl_sum.copy_(own_sum)
+        torch.distributed.all_reduce(kl_stop.kl_sum)
+    return dict(kl_sum=kl_stop.kl_sum, rows=rows)
 
-    n_mb = experience.num_minibatches
-    if seg is not None:                        # persistent accumulator: the segment graphs update it in place
-        if data.train_acc is None:
-            data.train_acc = torch.zeros(6, device=device)
-        acc = data.train_acc
-        acc.zero_()
-    else:
-        acc = torch.zeros(6, device=device)    # policy, value, entropy, old_kl, kl, clipfrac
-    obs_shape = data.vecenv.single_observation_space.shape
-    carry = {'lstm_state': None, 'approx_kl': None}
-    if manual is not None:
-        manual.pack_heads()                      # the parameters may have changed since the last train() (checkpoints)
-    n_stats = config.update_epochs * n_mb
-    kl_stop = _kl_stop(data)
-    if kl_stop is not None:
-        kl_stop.begin(config.update_epochs)
-        if manual is not None and manual.stats is not None:
-            manual.stats.zero_()                 # rows of epochs that do not run must add nothing to loss_means
 
-    def forward_backward(mb, k=0):              # k = epoch * n_mb + mb: the manual path's statistics row
-        b = experience.minibatch(mb)
-        if manual is not None:
-            with profile.train_forward:
-                manual.forward_backward(k, n_stats, b, config)
-            return
-        obs, atn, log_probs, val, adv, ret = b.obs, b.actions, b.logprobs, b.values, b.advantages, b.returns
+class _AutogradUpdate:
+    """The minibatch update of clean_pufferl.py:186-244 through autograd, for update_plan's other engines; train()'s loop
+    drives it through the same methods as _DefaultMLPUpdate.  It holds the engine's forward + loss, ENGINES[engine]:
+    (self, minibatch, LSTM state) -> (loss, stats, LSTM state), or None where the model's kernels refuse the minibatch;
+    the LSTM state carried from one minibatch to the next; the gradient mean over the ranks (GradBucket: NCCL, or its
+    peer exchange where `peer`); clip_grad_norm_ + optimizer.step()."""
 
-        with profile.train_forward:
-            if engine in ('packed', 'bptt'):     # the model's own kernels; the loss hands back ONE [M, R] gradient
-                if engine == 'bptt':             # clean_pufferl.py:188-191: [rows, bptt, *obs] segments
-                    packed = model.forward_packed_seq(obs, carry['lstm_state'])
-                elif b.slab_form:
-                    packed = model.forward_packed_slabs(obs)
-                else:
-                    packed = model.forward_packed(obs.reshape(-1, *obs_shape))
-                if packed is None:
-                    raise RuntimeError(f'the {engine} engine refused minibatch {mb} of form {plan.form}: update_plan '
-                                       'and the model disagree on what its kernels cover')
-                if engine == 'bptt':
-                    carry['lstm_state'] = (packed[2][0].detach(), packed[2][1].detach())
-            elif engine == 'model':
-                logits, newvalue = model(obs.reshape(-1, *obs_shape))
-            elif engine == 'cudnn_conv':         # rows b*T + t, as the b_* per-row tensors
-                if plan.form == 'segments':
-                    out = model.forward_segments(obs, carry['lstm_state'])
-                    if out is None:
-                        raise RuntimeError(f'the {engine} engine refused minibatch {mb} of form {plan.form}: update_plan '
-                                           'and the model disagree on what its kernels cover')
-                else:
-                    out = model(obs, carry['lstm_state'])
-                logits, newvalue, st_ = out
-                carry['lstm_state'] = (st_[0].detach(), st_[1].detach())
-            elif engine == 'cudnn':
-                _, newlogprob, entropy, newvalue, st_ = data.policy(obs, state=carry['lstm_state'], action=atn)
-                carry['lstm_state'] = (st_[0].detach(), st_[1].detach())
+    def __init__(self, data, engine, form, peer):
+        self.engine, self.form, self.peer, self.config = engine, form, peer, data.config
+        self.policy, self.model, self.optimizer = data.policy, getattr(data.policy, 'policy', None), data.optimizer
+        self.experience, self.obs_shape, self.bucket = data.experience, data.experience.obs_shape, data.grad_bucket
+        self.profile = data.profile
+
+    def _rows(self, b):
+        return b.logprobs, b.advantages, b.returns, b.values, self.config
+
+    def _packed(self, b, state):      # out: (head output [M, R], n_act); the loss hands back ONE [M, R] gradient
+        m = self.model
+        out = m.forward_packed_slabs(b.obs) if b.slab_form else m.forward_packed(b.obs.reshape(-1, *self.obs_shape))
+        return None if out is None else (*fused_ppo_loss_packed(*out, b.actions, *self._rows(b)), None)
+
+    def _bptt(self, b, state):        # clean_pufferl.py:188-191: [rows, bptt, *obs] segments
+        out = self.model.forward_packed_seq(b.obs, state)       # (head output [M, R], n_act, LSTM state)
+        return None if out is None else (*fused_ppo_loss_packed(*out[:2], b.actions, *self._rows(b)), out[2])
+
+    def _model(self, b, state):
+        logits, value = self.model(b.obs.reshape(-1, *self.obs_shape))
+        return (*fused_ppo_loss(logits, value, b.actions, *self._rows(b)), None)
+
+    def _cudnn_conv(self, b, state):  # out: (logits, value, LSTM state), rows b*T + t as the b_* per-row tensors
+        out = self.model.forward_segments(b.obs, state) if self.form == 'segments' else self.model(b.obs, state)
+        return None if out is None else (*fused_ppo_loss(*out[:2], b.actions, *self._rows(b)), out[2])
+
+    def _cudnn(self, b, state):
+        _, logprob, entropy, value, state = self.policy(b.obs, state=state, action=b.actions)
+        return (*_ppo_loss(logprob, entropy, value, *self._rows(b)), state)
+
+    def _reference(self, b, state):
+        _, logprob, entropy, value = self.policy(b.obs.reshape(-1, *self.obs_shape), action=b.actions)
+        return (*_ppo_loss(logprob, entropy, value, *self._rows(b)), None)
+
+    ENGINES = {'packed': _packed, 'bptt': _bptt, 'model': _model, 'cudnn_conv': _cudnn_conv, 'cudnn': _cudnn,
+               'reference': _reference}
+
+    def begin(self, data, kl_stop):
+        if data.train_acc is None:            # persistent: the segment graphs update it in place
+            data.train_acc = torch.zeros(6, device=self.experience.device)
+        self.acc, self.kl_stop = data.train_acc, kl_stop
+        self.acc.zero_()                      # policy, value, entropy, old_kl, kl, clipfrac
+
+    def graph_key(self, epoch, mb):
+        return 'fb', mb
+
+    def train_minibatch(self, epoch, mb):
+        b = self.experience.minibatch(mb)
+        with self.profile.train_forward:
+            out = self.ENGINES[self.engine](self, b, self.state if mb else None)  # every epoch starts from a zero state
+        if out is None:
+            raise RuntimeError(f'the {self.engine} engine refused minibatch {mb} of form {self.form}: update_plan and '
+                               'the model disagree on what its kernels cover')
+        loss, stats, state = out
+        self.state = None if state is None else (state[0].detach(), state[1].detach())     # outside this graph
+        with self.profile.learn:
+            if self.bucket is not None:
+                self.bucket.zero()            # grads are views into one flat buffer
             else:
-                _, newlogprob, entropy, newvalue = data.policy(obs.reshape(-1, *obs_shape), action=atn)
-
-        with profile.train_misc:
-            if engine in ('packed', 'bptt'):
-                loss, st = fused_ppo_loss_packed(packed[0], packed[1], atn, log_probs, adv, ret, val, config)
-            elif engine in ('model', 'cudnn_conv'):
-                loss, st = fused_ppo_loss(logits, newvalue, atn, log_probs, adv, ret, val, config)
-            else:
-                loss, st = _ppo_loss(newlogprob, entropy, newvalue, log_probs, adv, ret, val, config)
-
-        with profile.learn:
-            if data.grad_bucket is not None:
-                data.grad_bucket.zero()                     # grads are views into one flat buffer
-            else:
-                data.optimizer.zero_grad()
+                self.optimizer.zero_grad()
             loss.backward()
-
-        with profile.train_misc, torch.no_grad():
-            acc.add_(st / n_mb)
+        with self.profile.train_misc, torch.no_grad():
+            self.acc.add_(stats / self.experience.num_minibatches)
         # detached: the stop decision must not keep this minibatch's autograd graph (and the streams its nodes were
         # created on) alive into the next epoch
-        carry['approx_kl'] = st[4].detach()
+        self.approx_kl = stats[4].detach()
 
-    world = manual.world if manual is not None else (data.grad_bucket.world if data.grad_bucket is not None else 1)
-    # several ranks with peers: the exchange of each epoch's last optimizer step carries the KL row sum (_KLStop)
-    kl_peer = kl_stop is not None and world > 1 and ((manual is not None and manual.peer is not None) or plan.bptt_peer)
+    def exchange(self, kl):
+        if self.peer:                         # ONE peer-exchange kernel; with kl it carries this rank's KL row sum too
+            kl_in = self.approx_kl.double() * self.experience.minibatch_size if kl else None
+            self.bucket.peer_all_reduce_mean(kl_in, self.kl_stop.kl_sum if kl else None)
+        elif self.bucket is not None:
+            self.bucket.all_reduce_mean()     # ONE NCCL all-reduce per optimizer step
 
-    def optimizer_step(kl_row=None):
-        with profile.learn:
-            if manual is not None:
-                manual.optimizer_step(config, kl_row, kl_stop.kl_sum if kl_row is not None else None)
-                return
-            torch.nn.utils.clip_grad_norm_(data.policy.parameters(), config.max_grad_norm)
-            data.optimizer.step()
+    def step(self, epoch, mb, kl):
+        torch.nn.utils.clip_grad_norm_(self.policy.parameters(), self.config.max_grad_norm)
+        self.optimizer.step()
+
+    def kl_args(self, epoch):
+        if self.bucket is None:
+            return dict(approx_kl=self.approx_kl)
+        rows = self.experience.minibatch_size  # the fused loss's fp32 mean times the rows: this rank's row sum
+        return _ranks_kl_args(self.kl_stop, self.bucket.world * rows, None if self.peer else self.approx_kl.double() * rows)
+
+    def loss_means(self, n_mb):
+        return self.acc
+
+
+def _train_device_part(data, plan, seg=None):
+    """Everything of train() that runs on the device without touching the host: GAE, minibatch construction, the
+    update_epochs x num_minibatches optimizer steps of plan.update (update_plan), the loss statistics.  No
+    synchronisation inside, so the whole thing can be captured in ONE CUDA graph (single GPU, see train) or, with
+    ``seg``, as per-segment graphs around the gradient all-reduce (multi-GPU)."""
+    config, profile, experience, update = data.config, data.profile, data.experience, plan.update
+    _invalidate_policy_cache(data)     # nothing cached by the rollout (eager or captured) may leak into an update graph
+    with profile.train_misc:
+        experience.prepare(plan.form, config)
+    n_mb, epochs = experience.num_minibatches, config.update_epochs
+    kl_stop = plan.kl_stop
+    if kl_stop is not None:
+        kl_stop.begin(epochs)
+    update.begin(data, kl_stop)
+    run = seg.run if seg is not None else lambda key, fn: fn()
 
     def run_epoch(epoch):
-        carry['lstm_state'] = None
         for mb in range(n_mb):
-            if seg is not None:       # the manual path writes its statistics to a per-(epoch, minibatch) row
-                seg.run(('fb', mb) if manual is None else ('fb', epoch, mb),
-                        lambda: forward_backward(mb, epoch * n_mb + mb))
-            else:
-                forward_backward(mb, epoch * n_mb + mb)
-            last_kl = kl_peer and mb == n_mb - 1 and epoch < config.update_epochs - 1
-            if manual is not None:
-                with profile.learn:
-                    manual.all_reduce()                         # ONE NCCL all-reduce (sum; 1/world folded into the step)
-            elif plan.bptt_peer:
-                with profile.learn, torch.no_grad():
-                    # ONE peer-exchange kernel per optimizer step; the epoch's last carries this rank's KL row sum, the value
-                    # the NCCL plan all-reduces
-                    kl_in = carry['approx_kl'].double() * experience.minibatch_size if last_kl else None
-                    data.grad_bucket.peer_all_reduce_mean(kl_in, kl_stop.kl_sum if last_kl else None)
-            elif data.grad_bucket is not None:
-                with profile.learn:
-                    data.grad_bucket.all_reduce_mean()          # ONE NCCL all-reduce per optimizer step
-            if seg is not None:
-                seg.run('opt', optimizer_step)
-            elif last_kl and manual is not None:
-                optimizer_step(kl_row=epoch * n_mb + mb)
-            else:
-                optimizer_step()
-        if kl_stop is not None and epoch < config.update_epochs - 1:
-            last = epoch * n_mb + n_mb - 1
-            if world == 1 and manual is not None:
-                kl_stop.decide(epoch, stats=manual.stats, row=last, rows=manual.mb_rows)
-            elif world == 1:
-                kl_stop.decide(epoch, approx_kl=carry['approx_kl'])
-            else:
-                # one decision for all ranks on the KL sum over their rows; without peers an NCCL all-reduce of this
-                # rank's fp64 row sum (the fused loss's fp32 mean times the rows, for autograd) forms it
-                rows = manual.mb_rows if manual is not None else experience.minibatch_size
-                if not kl_peer:
-                    with torch.no_grad():
-                        if manual is not None:
-                            kl_stop.kl_sum.copy_(manual.stats[last, 4:5])
-                        else:
-                            kl_stop.kl_sum.copy_(carry['approx_kl'].double() * rows)
-                    torch.distributed.all_reduce(kl_stop.kl_sum)
-                kl_stop.decide(epoch, kl_sum=kl_stop.kl_sum, rows=world * rows)
+            run(update.graph_key(epoch, mb), lambda: update.train_minibatch(epoch, mb))
+            kl = kl_stop is not None and mb == n_mb - 1 and epoch < epochs - 1     # a stop decision follows this step
+            with profile.learn:
+                update.exchange(kl)
+                run('opt', lambda: update.step(epoch, mb, kl))
+        if kl_stop is not None and epoch < epochs - 1:
+            kl_stop.decide(epoch, **update.kl_args(epoch))
 
-    for epoch in range(config.update_epochs):
+    for epoch in range(epochs):
         if kl_stop is not None and kl_stop.capturing:
             with kl_stop.if_body(epoch):
                 run_epoch(epoch)
-        elif kl_stop is None or epoch == 0:
-            run_epoch(epoch)
-        elif kl_stop.stopped():
+        elif kl_stop is not None and epoch > 0 and kl_stop.stopped():
             break
         else:
             run_epoch(epoch)
@@ -1436,22 +1448,10 @@ def _train_device_part(data, plan, seg=None):
         y_pred, y_true = experience.values, experience.returns
         var_y = y_true.var(unbiased=False)
         ev = 1 - (y_true - y_pred).var(unbiased=False) / var_y
-        if manual is not None:
-            acc = manual.loss_means(n_mb)
-        out = [acc, torch.stack([ev, var_y])]
+        out = [update.loss_means(n_mb), torch.stack([ev, var_y])]
         if kl_stop is not None:
             out.append(kl_stop.state[1:].float())      # epochs run
         return torch.cat(out)
-
-
-def _kl_stop(data):
-    """The device-side target_kl stop of this train() (_KLStop), or None: no target_kl, or one epoch."""
-    config = data.config
-    if config.target_kl is None or config.update_epochs < 2:
-        return None
-    if getattr(data, 'train_kl_stop', None) is None:
-        data.train_kl_stop = _KLStop(data.experience.device, ranks=data.grad_bucket is not None)
-    return data.train_kl_stop
 
 
 def train(data):
@@ -1469,7 +1469,7 @@ def train(data):
     with profile.train_misc:
         experience.sort_training_data()        # host-side bookkeeping only (clean_pufferl.py:452-464)
         plan = update_plan(data)
-        kl_stop = _kl_stop(data)
+        kl_stop = plan.kl_stop
         if kl_stop is not None:                # a device scalar, like the learning rate: replays read the current value
             kl_stop.target.fill_(float(config.target_kl))
     if plan.capture == 'segments' and data.train_graph_state >= 1:

@@ -6,7 +6,7 @@
 For every configuration below the trainer is built from fixed seeds and `evaluate(); train()` runs three times.  Each
 train() records the minibatch form (data.train_minibatch_path), the recurrent path, whether the hand-written update ran
 and on the fused kernel, the train graph state, the project kernels launched from Python during the call
-(pb_launch_count) and those a captured update graph holds.  The final parameters, Adam moments and losses go to
+(pb_launch_count), those a captured update graph holds and the epochs run.  The final parameters, Adam moments and losses go to
 DIR/<name>.npz, the records to DIR/records.json.  --repo imports pufferlib_b200 from another checkout, so two versions
 can be run on the same machine and compared.
 
@@ -55,6 +55,17 @@ CASES = {
     'squared_heads16_graph': ('squared', 64, 64, 'mlp', {}, dict(cuda_graph=True)),      # Discrete(8): 16-row chain
     'lstm_cudnn_graph': ('squared', 64, 16, 'lstm', dict(fused_update=False, hidden=64),
                          dict(bptt_horizon=8, minibatch_size=64 * 16 // 2, cuda_graph=True)),
+    # LSTMWrapper(Convolutional, 512, 512), the Atari LSTM policy: the 'cudnn_conv' engine on segment views
+    'conv_lstm': ('pong', 64, 32, 'conv_lstm', {}, dict(bptt_horizon=8, minibatch_size=64 * 32 // 2)),
+    'conv_lstm_graph': ('pong', 64, 32, 'conv_lstm', {}, dict(bptt_horizon=8, minibatch_size=64 * 32 // 2, cuda_graph=True)),
+    # target_kl on the autograd engines; 1e-6 stops after the first epoch
+    'lstm_target_kl': ('breakout', 256, 64, 'lstm', {}, dict(minibatch_size=256 * 64 // 2, target_kl=0.02)),
+    'lstm_target_kl_stop_graph': ('breakout', 256, 64, 'lstm', {},
+                                  dict(minibatch_size=256 * 64 // 2, target_kl=1e-6, cuda_graph=True)),
+    'autograd_target_kl': ('breakout', 64, 128, 'mlp', {}, dict(manual_update=False, target_kl=0.02)),
+    'autograd_target_kl_stop_graph': ('breakout', 64, 128, 'mlp', {},
+                                      dict(manual_update=False, target_kl=1e-6, cuda_graph=True)),
+    'target_kl_stop_graph': ('breakout', 64, 128, 'mlp', {}, dict(target_kl=1e-6, cuda_graph=True)),
 }
 
 
@@ -66,7 +77,10 @@ def build(env, n, h, kind, pol_kw, cfg_kw):
     from pufferlib_b200.frameworks import cleanrl
     vec = pvec.make(ocean.env_creator(env), num_envs=n, backend=pvec.B200)
     torch.manual_seed(0)
-    if kind == 'lstm':
+    if kind == 'conv_lstm':             # as tests/test_gpu_conv_lstm.py builds it
+        net = models.LSTMWrapper(vec.driver_env, models.Convolutional(vec.driver_env), input_size=512, hidden_size=512)
+        pol = cleanrl.RecurrentPolicy(net, seed=3)
+    elif kind == 'lstm':
         hid = pol_kw.get('hidden', 128)
         net = models.LSTMWrapper(vec.driver_env, models.Default(vec.driver_env, hidden_size=hid), input_size=hid,
                                  hidden_size=hid)
@@ -95,7 +109,7 @@ def run_case(name, out_dir):
             minibatch_path=data.train_minibatch_path, recurrent_path=data.train_recurrent_path,
             manual_update=mu is not None, used_fused=bool(mu.used_fused) if mu is not None else None,
             train_graph_state=data.train_graph_state, launches_from_python=int(lib.pb_launch_count() - l0),
-            graph_launches=int(data.train_graph_launches)))
+            graph_launches=int(data.train_graph_launches), epochs_run=data.train_epochs_run))
     arrays = {f'param/{k}': v.detach().float().cpu().numpy() for k, v in data.policy.state_dict().items()}
     names = {id(p): k for k, p in data.policy.named_parameters()}
     for p, st in data.optimizer.state.items():
@@ -125,7 +139,7 @@ def compare(a, b):
         for k in worst:
             worst[k] = max(worst[k], diff[k])
         paths = [(r['minibatch_path'], r['recurrent_path'], r['manual_update'], r['used_fused'], r['train_graph_state'],
-                  r['launches_from_python'], r['graph_launches']) for r in ra[name]]
+                  r['launches_from_python'], r['graph_launches'], r['epochs_run']) for r in ra[name]]
         print(f'{name}: records identical {paths}; max |diff| param {diff["param"]:.3e} adam {diff["adam"]:.3e} '
               f'losses {diff["losses"]:.3e}')
     print(json.dumps({'records_identical': same, 'max_abs_diff': worst}))

@@ -18,7 +18,8 @@
  *     PB_ERR_CUDA.
  *   - One host thread per GPU drives a handle; the library creates no threads and is re-entrant per handle.
  *
- * Agent rows: a kind has A agents per env (pb_env_agents_per_env; A = 2 for MULTIAGENT, 1 for every other kind).
+ * Agent rows: a kind has A agents per env (pb_env_agents_per_env; A = 2 for MULTIAGENT and PONG_VERSUS, 1 for every
+ * other kind).
  * Agent a of env e is row e*A + a, the order of the reference's Serial._assign_buffers (vector.py:97-110).  Seeds,
  * env_index_offset and num_envs count envs; observations, rewards, flags and actions count agent rows (N*A of them).
  *
@@ -56,7 +57,11 @@ enum {
     PB_ENV_MULTIAGENT = 8,
     /* breakout (PB_ENV_BREAKOUT's game) seen as the reference's Atari breakout is: a (4, 84, 84) uint8 frame stack,
        oldest frame first, for the NatureCNN (environments/atari/environment.py:37-39, atari/torch.py:8-10) */
-    PB_ENV_BREAKOUT_PIXELS = 9
+    PB_ENV_BREAKOUT_PIXELS = 9,
+    /* two-player pong from pixels (oracle/SPEC_PONG_VERSUS.md): PONG's game with the scripted left paddle replaced by a
+       second agent, two agent rows per env.  Agent 0 is the right paddle and sees PONG's frame; agent 1 is the left
+       paddle and sees the field mirrored in x with the paddle values swapped.  Zero-sum rewards, shared done flags. */
+    PB_ENV_PONG_VERSUS = 10
 };
 enum { PB_DTYPE_F32 = 0, PB_DTYPE_U8 = 1 };
 
@@ -90,7 +95,10 @@ typedef struct {
                                    [4]=episodic_life 0 / 1 (BREAKOUT_PIXELS only): a lost life is a terminal row,
                                        the next send runs a NOOP step instead of a reset
                                    [5]=clip_rewards 0 / 1: the row reward is the sign of the step's reward sum
-                                 PONG and BREAKOUT_PIXELS, the frame stack:
+                                 PONG_VERSUS: [0]=max_score in [1, 15] (default 5) [1]=max_ticks in [1, 65535]
+                                           (default 4096) [6]=framestack as below; [2..5] and [7] must be 0 (the
+                                           Atari preprocessing options are single-agent)
+                                 PONG, BREAKOUT_PIXELS and PONG_VERSUS, the frame stack:
                                    [6]=framestack 1 or 4 (0 = default 4): frames per observation row, obs_shape
                                        (S, 84, 84), obs_bytes S * 7056, oldest frame first; 1 is the newest frame alone
                                  All zero is the plain game, one tick per step, four frames per row.  Values out of
@@ -143,7 +151,8 @@ int pb_env_create(const pb_env_config* cfg, pb_env** out);
 int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_host, int32_t n_dparam, pb_env** out);
 int pb_env_destroy(pb_env* env);
 int pb_env_get_info(const pb_env* env, pb_env_info* out);
-/* A, the agents per env (PettingZooPufferEnv.num_agents, emulation.py:262): 2 for MULTIAGENT, 1 otherwise.  The
+/* A, the agents per env (PettingZooPufferEnv.num_agents, emulation.py:262): 2 for MULTIAGENT and PONG_VERSUS, 1
+ * otherwise.  The
  * outputs of reset / step and the actions of a step have N*A rows in the "Agent rows" order above. */
 int pb_env_agents_per_env(const pb_env* env, int32_t* out);
 
@@ -181,8 +190,12 @@ int pb_env_game_ended(pb_env* env, const uint8_t** ended);
 /* Per-agent statistics of the multi-agent kinds (MultiagentEpisodeStats, postprocess.py:147-179, which computes
  * episode_return / episode_length and then drops them: only the env's own per-agent info values are kept):
  * out4_host = {env steps, sum of agent 1's score, sum of agent 2's score, 0} accumulated on the device since the last
- * read with clear != 0.  Copies 32 bytes to host memory and synchronises `stream` once.  PB_ERR_INVALID for kinds
- * with one agent per env (pb_env_stats_read serves those). */
+ * read with clear != 0.  PONG_VERSUS: {games ended, sum of agent 0's score, sum of agent 1's score, sum of the game
+ * lengths in ticks} (agents 0 and 1 are the info keys 1 and 2), a score being the agent's points minus the other's
+ * (negative sums are returned as such); its pb_env_episode_rows give per env, where a game ended, the length and
+ * agent 0's score.  Copies 32 bytes to host
+ * memory and synchronises `stream` once.  PB_ERR_INVALID for kinds with one agent per env (pb_env_stats_read serves
+ * those). */
 int pb_env_agent_stats_read(pb_env* env, double* out4_host, int clear, void* stream);
 
 /* -- rollout ---------------------------------------------------------------------------------------------------

@@ -70,10 +70,14 @@ extern "C" int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_h
     PB_REQUIRE(n_dparam >= 0 && (n_dparam == 0 || dparam_host), PB_ERR_INVALID, "pb_env_create_ex: bad dparam");
     *out = nullptr;
     PB_REQUIRE(cfg->num_envs >= 1, PB_ERR_INVALID, "num_envs must be at least 1");  // vector.py:578-579
-    PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_BREAKOUT_PIXELS, PB_ERR_INVALID, "unknown env kind %d",
+    PB_REQUIRE(cfg->kind >= PB_ENV_SQUARED && cfg->kind <= PB_ENV_PONG_VERSUS, PB_ERR_INVALID, "unknown env kind %d",
                cfg->kind);
     if (cfg->kind == PB_ENV_PONG || cfg->kind == PB_ENV_BREAKOUT_PIXELS) {
         const int rc = fs_pre_check(cfg);   // the Atari preprocessing options, refused before anything is allocated
+        if (rc != PB_OK) return rc;
+    }
+    if (cfg->kind == PB_ENV_PONG_VERSUS) {
+        const int rc = pb_pong_versus_check(cfg);
         if (rc != PB_OK) return rc;
     }
     int ndev = 0;
@@ -93,6 +97,7 @@ extern "C" int pb_env_create_ex(const pb_env_config* cfg, const double* dparam_h
             case PB_ENV_SNAKE: rc = pb_snake_create(env); break;
             case PB_ENV_PONG: rc = pb_pong_create(env); break;
             case PB_ENV_BREAKOUT_PIXELS: rc = pb_breakout_pixels_create(env); break;
+            case PB_ENV_PONG_VERSUS: rc = pb_pong_versus_create(env); break;
             default: rc = pb_ocean_create(env, dparam_host, n_dparam); break;
         }
     }
@@ -221,7 +226,8 @@ extern "C" int pb_env_agent_stats_read(pb_env* env, double* out4_host, int clear
     PB_CUDA(cudaMemcpyAsync(h, env->d_agent_stats, bytes, cudaMemcpyDeviceToHost, s));
     if (clear) PB_CUDA(cudaMemsetAsync(env->d_agent_stats, 0, bytes, s));
     PB_CUDA(cudaStreamSynchronize(s));
-    for (int k = 0; k < 4; ++k) out4_host[k] = (double)h[k];   // integer counts: exact below 2**53
+    // integer sums in two's complement (a score sum may be negative): exact below 2**53 in magnitude
+    for (int k = 0; k < 4; ++k) out4_host[k] = (double)(long long)h[k];
     return PB_OK;
 }
 

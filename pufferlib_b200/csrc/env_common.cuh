@@ -53,6 +53,8 @@ int pb_breakout_create(pb_env* env);
 int pb_snake_create(pb_env* env);
 int pb_pong_create(pb_env* env);
 int pb_breakout_pixels_create(pb_env* env);
+int pb_pong_versus_check(const pb_env_config* cfg);   // the parameters, checked before anything is allocated
+int pb_pong_versus_create(pb_env* env);
 int pb_ocean_create(pb_env* env, const double* dparam, int n_dparam);   // memory, password, stochastic, bandit,
                                                                          // multiagent
 

@@ -6,32 +6,13 @@
 // (vector.py:147-151, emulation.py:187-192, postprocess.py:22-54).  Bit-exact against oracle/csrc/envs.c.
 //
 // The 28,224-byte observation rows are written by the TMA frame-stack ring of frame_stack.cuh; this file is the game:
-// the integer dynamics and the renderer (zero fill + 52 pixel stores).  Per-env state is 12 B of SoA.
+// the scripted opponent and the renderer (zero fill + 52 pixel stores); the state and the rest of the dynamics are
+// pong_game.cuh's.
 #include "env_common.cuh"
 #include "frame_stack.cuh"
+#include "pong_game.cuh"
 
 namespace {
-
-struct PongState {
-    uint32_t* s0;   // ly(8) | ry(8)<<8 | (bx+2)(8)<<16 | (by)(8)<<24
-    uint32_t* s1;   // (vx+2)(3) | (vy+2)(3)<<3 | score_l(4)<<6 | score_r(4)<<10 | tick(16)<<16
-    uint32_t* ctr;
-    uint64_t seed;
-    int max_score, max_ticks;
-};
-
-struct PongEnv {
-    int ly, ry, bx, by, vx, vy, score_l, score_r, tick;
-    uint32_t ctr;
-};
-
-__device__ __forceinline__ void pong_serve(PongEnv& s, uint64_t seed_e) {
-    const uint32_t r = pb_mix32(seed_e * 0x9E3779B97F4A7C15ull + (uint64_t)s.ctr * 0xD1B54A32D192ED03ull);
-    s.ctr += 1;
-    s.bx = 41; s.by = 41;
-    s.vx = (r & 1u) ? 2 : -2;
-    s.vy = (int)((r >> 1) % 5u) - 2;
-}
 
 // the game behind the frame-stack ring (frame_stack.cuh)
 struct PongGame {
@@ -39,20 +20,14 @@ struct PongGame {
     using Env = PongEnv;
 
     static __device__ __forceinline__ void reset(const State& st, int64_t e, uint64_t seed_e, bool keep_ctr, Env& p) {
-        p.ctr = keep_ctr ? st.ctr[e] : 0u;
-        p.ly = 36; p.ry = 36; p.score_l = 0; p.score_r = 0; p.tick = 0;
-        pong_serve(p, seed_e);
+        pong_reset(st.ctr, e, seed_e, keep_ctr, p);
     }
 
     static constexpr int NOOP = 0;
     static constexpr bool kLives = false;
 
     static __device__ __forceinline__ void load(const State& st, int64_t e, Env& p) {
-        const uint32_t a0 = st.s0[e], a1 = st.s1[e];
-        p.ly = a0 & 0xff; p.ry = (a0 >> 8) & 0xff; p.bx = (int)((a0 >> 16) & 0xff) - 2; p.by = (a0 >> 24) & 0xff;
-        p.vx = (int)(a1 & 7) - 2; p.vy = (int)((a1 >> 3) & 7) - 2;
-        p.score_l = (a1 >> 6) & 15; p.score_r = (a1 >> 10) & 15; p.tick = a1 >> 16;
-        p.ctr = st.ctr[e];
+        pong_load(st, e, p);
     }
 
     static __device__ __forceinline__ void tick(const State& st, Env& p, int64_t action, uint64_t seed_e, float& reward,
@@ -64,19 +39,7 @@ struct PongGame {
         const int tgt = min(max(p.by - 5, 0), 72);
         if (p.ly < tgt) p.ly = min(p.ly + 2, tgt);
         else if (p.ly > tgt) p.ly = max(p.ly - 2, tgt);
-        p.bx += p.vx; p.by += p.vy;
-        if (p.by < 0) { p.by = -p.by; p.vy = -p.vy; }
-        if (p.by > 82) { p.by = 164 - p.by; p.vy = -p.vy; }
-        if (p.vx > 0 && p.bx >= 76 && p.bx <= 78 && p.by + 2 > p.ry && p.by < p.ry + 12) {
-            p.vx = -2; p.bx = 76; p.vy = (p.by + 1 - p.ry - 6) / 3;
-        } else if (p.vx < 0 && p.bx >= 4 && p.bx <= 6 && p.by + 2 > p.ly && p.by < p.ly + 12) {
-            p.vx = 2; p.bx = 6; p.vy = (p.by + 1 - p.ly - 6) / 3;
-        }
-        if (p.bx < 0) { p.score_r += 1; reward = 1.f; pong_serve(p, seed_e); }
-        else if (p.bx > 82) { p.score_l += 1; reward = -1.f; pong_serve(p, seed_e); }
-        p.tick += 1;
-        terminal = p.score_l >= st.max_score || p.score_r >= st.max_score || p.tick >= st.max_ticks;
-        score = (float)(p.score_r - p.score_l);
+        pong_ball(st, p, seed_e, reward, terminal, score);
     }
 
     static __device__ __forceinline__ void step(const State& st, int64_t e, int64_t action, uint64_t seed_e, Env& p,
@@ -115,10 +78,7 @@ struct PongGame {
     }
 
     static __device__ __forceinline__ void store(const State& st, int64_t e, const Env& p) {
-        st.s0[e] = (uint32_t)p.ly | ((uint32_t)p.ry << 8) | ((uint32_t)(p.bx + 2) << 16) | ((uint32_t)p.by << 24);
-        st.s1[e] = (uint32_t)(p.vx + 2) | ((uint32_t)(p.vy + 2) << 3) | ((uint32_t)p.score_l << 6) |
-                   ((uint32_t)p.score_r << 10) | ((uint32_t)p.tick << 16);
-        st.ctr[e] = p.ctr;
+        pong_store(st, e, p);
     }
 };
 

@@ -24,9 +24,27 @@
 //                                                      max of render(a) and render(b), in one pass
 //   G::NOOP, G::kLives (and G::lives(p) where kLives)  the no-op action; whether the game has lives
 // Every thread runs reset / step redundantly on the same inputs (broadcast loads), so no barrier is needed before render.
+//
+// A game with several agents per env (G::kAgents = A > 1; absent means 1, and the preprocessing layer is single-agent)
+// writes A observation rows per env, agent a of env e at row e * A + a, every output row array indexed the same way.
+// Its ring items are those rows: a CTA runs the A items of one env back to back, and the dynamics step once per env,
+// at item 0, from all A actions, before any of its rows renders; the later items render from the same registers.  So
+// no two items load and store one env's state.  Such a game provides, in place of step / render:
+//   G::step(st, e, acts, seed_e, p, reward, terminal, score)   acts = the env's A actions; reward is agent 0's
+//   G::render(p, frame, tid, a)                        agent a's frame
+//   G::seat_reward(reward, a)                          agent a's reward, from agent 0's
+//   G::game_over(st, length, score)                    thread 0, where a game ends: the per-agent statistics
 #pragma once
+#include <type_traits>
+
 #include "env_common.cuh"
 #include "tma.cuh"
+
+// A, the agents per env of a frame-stack game: G::kAgents, or 1 where the game has no such member
+template <class G, class = void>
+struct fs_agents : std::integral_constant<int, 1> {};
+template <class G>
+struct fs_agents<G, std::void_t<decltype(G::kAgents)>> : std::integral_constant<int, G::kAgents> {};
 
 constexpr int FS_STAGES = 4;
 constexpr uint32_t FS_FRAME = 84 * 84;      // 7056 = 441 * 16
@@ -141,12 +159,14 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
     uint32_t phase[FS_STAGES] = {0, 0, 0, 0};
 
     static_assert(S == 4 || S == 1, "frame stacks of 4 or 1 frames");
+    constexpr int A = fs_agents<G>::value;
+    static_assert(A == 1 || !PP, "the preprocessing layer is single-agent");
     constexpr uint32_t STAGE = FS_STAGE_OF<S>;
     auto needs_load = [&](int64_t e) -> bool { return MODE == 1 && done[e] == 0; };
-    auto issue_load = [&](int s, int64_t e) {  // thread 0 only
+    auto issue_load = [&](int s, int64_t e, int a) {  // thread 0 only; the item of agent a of env e
         if (S == 4 && needs_load(e)) {
             mbar_expect_tx(&bars[s], 3 * FS_FRAME);
-            tma_load_1d(smem + (size_t)s * STAGE, prev + e * prev_stride + FS_FRAME, 3 * FS_FRAME, &bars[s]);
+            tma_load_1d(smem + (size_t)s * STAGE, prev + (e * A + a) * prev_stride + FS_FRAME, 3 * FS_FRAME, &bars[s]);
         }
     };
 
@@ -154,127 +174,157 @@ __device__ __forceinline__ void frame_stack_run(const typename G::State& st, int
         for (int s = 0; s < FS_STAGES; ++s) mbar_init(&bars[s], 1);
         mbar_fence_init();
         int64_t e = blockIdx.x;
-        for (int s = 0; s < FS_STAGES && e < n; ++s, e += step) issue_load(s, e);
+        for (int s = 0; s < FS_STAGES && e < n; ++s) {   // item s: agent s % A of the (s / A)-th env
+            issue_load(s, e, s % A);
+            if ((s + 1) % A == 0) e += step;
+        }
     }
     __syncthreads();
 
     int it = 0;
-    for (int64_t e = blockIdx.x; e < n; e += step, ++it) {
-        const int s = it % FS_STAGES;
-        unsigned char* buf = smem + (size_t)s * STAGE;
-        unsigned char* frame = buf + (S - 1) * FS_FRAME;
-        if constexpr (S == 1) {
-            // no refill load waits for the bulk store that last read this stage (FS_STAGES iterations ago, the oldest of
-            // the groups this thread committed): wait for it here, and let the barrier hold every thread back from
-            // rendering into the stage until it has
-            if (tid == 0 && it >= FS_STAGES) tma_wait_read<FS_STAGES - 1>();
-            __syncthreads();
-        }
-        // refill the stage that was stored one iteration ago: by now its bulk store has long read shared memory, so
-        // this wait does not stall, and the load gets FS_STAGES - 1 iterations of lead time
-        if (S == 4 && tid == 0 && it > 0) {
-            const int64_t e_next = e + step * (FS_STAGES - 1);
-            if (e_next < n) {
-                tma_wait_read<0>();
-                issue_load((it - 1) % FS_STAGES, e_next);
-            }
-        }
-        // ---- integer dynamics, computed redundantly by every thread (same inputs: broadcast loads)
-        const uint64_t seed_e = st.seed + (uint64_t)e;
+    for (int64_t e = blockIdx.x; e < n; e += step) {
+        // the env's state, stepped at its first item; A > 1: its later items render from it
         typename G::Env p;
         float reward = 0.f, score = 0.f;
-        bool terminal = false;
-        const bool loaded = needs_load(e);     // false -> this row is a reset row (PP: a real or a soft reset)
-        // PP: `raw` / `ticks` = the unclipped reward sum / the game ticks of this row, `ended` = the game ended,
-        // `fresh` = a real reset, `word` = the wrapper word to store
-        float raw = 0.f;
-        int ticks = 0;
-        bool ended = false, fresh = !loaded;
-        uint32_t word = 0u;
-        if constexpr (!PP) {
-            if (!loaded) G::reset(st, e, seed_e, MODE == 1, p);
-            else G::step(st, e, actions[e], seed_e, p, reward, terminal, score);
-            // ---- render the new frame into the stage
-            G::render(p, frame, tid);
-        } else {
-            const uint32_t w = MODE == 1 ? pre.word[e] : 0u;
-            fresh = !loaded && !(w & FS_SOFT);
-            typename G::Env q;                 // the state after the second-to-last tick (max-pooling)
-            if (fresh) {
-                // reset, then 1 + draw % noop_max ticks of NOOP; the frame is the last tick's
-                G::reset(st, e, seed_e, MODE == 1, p);
-                const int noops = pre.noop_max > 0 ? fs_noops(seed_e, w, pre.noop_max) : 0;
-                for (; ticks < noops; ++ticks) {
-                    float r = 0.f;
-                    G::tick(st, p, G::NOOP, seed_e, r, ended, score);
-                    raw += r;
+        bool terminal = false, loaded_env = false;
+#pragma unroll
+        for (int seat = 0; seat < A; ++seat, ++it) {
+            const int s = it % FS_STAGES;
+            unsigned char* buf = smem + (size_t)s * STAGE;
+            unsigned char* frame = buf + (S - 1) * FS_FRAME;
+            if constexpr (S == 1) {
+                // no refill load waits for the bulk store that last read this stage (FS_STAGES iterations ago, the oldest of
+                // the groups this thread committed): wait for it here, and let the barrier hold every thread back from
+                // rendering into the stage until it has
+                if (tid == 0 && it >= FS_STAGES) tma_wait_read<FS_STAGES - 1>();
+                __syncthreads();
+            }
+            // refill the stage that was stored one iteration ago: by now its bulk store has long read shared memory, so
+            // this wait does not stall, and the load gets FS_STAGES - 1 iterations of lead time
+            if (S == 4 && tid == 0 && it > 0) {
+                const int k = seat + FS_STAGES - 1;   // the item FS_STAGES - 1 ahead: k / A envs on, agent k % A
+                const int64_t e_next = e + step * (k / A);
+                if (e_next < n) {
+                    tma_wait_read<0>();
+                    issue_load((it - 1) % FS_STAGES, e_next, k % A);
                 }
-                q = p;
-                word = (w + 1u) & ~FS_SOFT;
+            }
+            // ---- integer dynamics, computed redundantly by every thread (same inputs: broadcast loads)
+            const uint64_t seed_e = st.seed + (uint64_t)e;
+            // false -> this row is a reset row (PP: a real or a soft reset); read once per env, before its item 0
+            // writes done[e]
+            const bool loaded = (A == 1 || seat == 0) ? needs_load(e) : loaded_env;
+            loaded_env = loaded;
+            // PP: `raw` / `ticks` = the unclipped reward sum / the game ticks of this row, `ended` = the game ended,
+            // `fresh` = a real reset, `word` = the wrapper word to store
+            float raw = 0.f;
+            int ticks = 0;
+            bool ended = false, fresh = !loaded;
+            uint32_t word = 0u;
+            if constexpr (!PP) {
+                if (seat == 0) {
+                    if (!loaded) G::reset(st, e, seed_e, MODE == 1, p);
+                    else if constexpr (A == 1) G::step(st, e, actions[e], seed_e, p, reward, terminal, score);
+                    else G::step(st, e, actions + e * A, seed_e, p, reward, terminal, score);
+                }
+                // ---- render the new frame into the stage
+                if constexpr (A == 1) G::render(p, frame, tid);
+                else G::render(p, frame, tid, seat);
             } else {
-                // an agent step, or (soft reset) a NOOP step: up to frameskip ticks, stopping where the game ends
-                G::load(st, e, p);
-                const int a = loaded ? (int)actions[e] : G::NOOP;
-                int lives0 = 0;
-                if constexpr (G::kLives) lives0 = G::lives(p);
-                for (ticks = 0; ticks < pre.frameskip && !ended; ++ticks) {
+                const uint32_t w = MODE == 1 ? pre.word[e] : 0u;
+                fresh = !loaded && !(w & FS_SOFT);
+                typename G::Env q;                 // the state after the second-to-last tick (max-pooling)
+                if (fresh) {
+                    // reset, then 1 + draw % noop_max ticks of NOOP; the frame is the last tick's
+                    G::reset(st, e, seed_e, MODE == 1, p);
+                    const int noops = pre.noop_max > 0 ? fs_noops(seed_e, w, pre.noop_max) : 0;
+                    for (; ticks < noops; ++ticks) {
+                        float r = 0.f;
+                        G::tick(st, p, G::NOOP, seed_e, r, ended, score);
+                        raw += r;
+                    }
                     q = p;
-                    float r = 0.f;
-                    G::tick(st, p, a, seed_e, r, ended, score);
-                    raw += r;
+                    word = (w + 1u) & ~FS_SOFT;
+                } else {
+                    // an agent step, or (soft reset) a NOOP step: up to frameskip ticks, stopping where the game ends
+                    G::load(st, e, p);
+                    const int a = loaded ? (int)actions[e] : G::NOOP;
+                    int lives0 = 0;
+                    if constexpr (G::kLives) lives0 = G::lives(p);
+                    for (ticks = 0; ticks < pre.frameskip && !ended; ++ticks) {
+                        q = p;
+                        float r = 0.f;
+                        G::tick(st, p, a, seed_e, r, ended, score);
+                        raw += r;
+                    }
+                    if (ticks == 1) q = p;
+                    bool life_lost = false;
+                    if constexpr (G::kLives) life_lost = loaded && pre.episodic_life && G::lives(p) < lives0 && G::lives(p) > 0;
+                    terminal = ended || life_lost;
+                    if (loaded) reward = pre.clip_rewards ? (float)((raw > 0.f) - (raw < 0.f)) : raw;
+                    word = (w & ~FS_SOFT) | (life_lost && !ended ? FS_SOFT : 0u);
                 }
-                if (ticks == 1) q = p;
-                bool life_lost = false;
-                if constexpr (G::kLives) life_lost = loaded && pre.episodic_life && G::lives(p) < lives0 && G::lives(p) > 0;
-                terminal = ended || life_lost;
-                if (loaded) reward = pre.clip_rewards ? (float)((raw > 0.f) - (raw < 0.f)) : raw;
-                word = (w & ~FS_SOFT) | (life_lost && !ended ? FS_SOFT : 0u);
+                G::render2(q, p, frame, tid);
             }
-            G::render2(q, p, frame, tid);
-        }
-        fence_proxy_async_smem();
-        __syncthreads();
-        // ---- thread 0: bookkeeping + the bulk stores
-        if (tid == 0) {
-            G::store(st, e, p);
-            done[e] = terminal ? 1 : 0;
-            out.rewards[e] = reward;
-            out.terminals[e] = terminal ? 1 : 0;
-            if (out.write_const) out.truncations[e] = 0;
-            if (out.write_const) out.masks[e] = 1;
-            if (out.dones_f32) out.dones_f32[e] = terminal ? 1.f : 0.f;
-            if constexpr (PP) {
-                pre.word[e] = word;
-                if (pre.ended) pre.ended[e] = ended ? 1 : 0;
-            }
-            // EpisodeStats (postprocess.py:22-54), scalar form; PP: over every tick of the game, raw rewards, reported
-            // where the game ends
-            if (!PP && !loaded) { acc.ep_return[e] = 0.0; acc.ep_length[e] = 0; }
-            else {
-                const double ret = PP ? (fresh ? 0.0 : acc.ep_return[e]) + (double)raw : acc.ep_return[e] + (double)reward;
-                const int len = PP ? (fresh ? 0 : acc.ep_length[e]) + ticks : acc.ep_length[e] + 1;
-                acc.ep_return[e] = ret; acc.ep_length[e] = len;
-                if (PP ? ended : terminal) {
-                    acc.row_return[e] = ret; acc.row_length[e] = len; acc.row_score[e] = score;
-                    double* slot = acc.stats + 4 * (blockIdx.x & (PB_STAT_SLOTS - 1));
-                    atomicAdd(slot + 0, 1.0); atomicAdd(slot + 1, ret);
-                    atomicAdd(slot + 2, (double)len); atomicAdd(slot + 3, (double)score);
+            fence_proxy_async_smem();
+            __syncthreads();
+            // ---- thread 0: bookkeeping + the bulk stores
+            if (tid == 0) {
+                const int64_t orow = e * A + seat;   // the observation / output row
+                float reward_a = reward;
+                if constexpr (A > 1) reward_a = G::seat_reward(reward, seat);
+                if (seat == 0) {
+                    G::store(st, e, p);
+                    done[e] = terminal ? 1 : 0;
                 }
+                out.rewards[orow] = reward_a;
+                out.terminals[orow] = terminal ? 1 : 0;
+                if (out.write_const) out.truncations[orow] = 0;
+                if (out.write_const) out.masks[orow] = 1;
+                if (out.dones_f32) out.dones_f32[orow] = terminal ? 1.f : 0.f;
+                if constexpr (PP) {
+                    pre.word[e] = word;
+                    if (pre.ended) pre.ended[e] = ended ? 1 : 0;
+                }
+                // EpisodeStats (postprocess.py:22-54), scalar form; PP: over every tick of the game, raw rewards, reported
+                // where the game ends.  A > 1: per env, from agent 0's rewards, and the game's per-agent statistics
+                if (A > 1 && seat != 0) {
+                    // an env's statistics are kept at its item 0
+                } else if (!PP && !loaded) { acc.ep_return[e] = 0.0; acc.ep_length[e] = 0; }
+                else if constexpr (A > 1) {
+                    const double ret = acc.ep_return[e] + (double)reward;
+                    const int len = acc.ep_length[e] + 1;
+                    acc.ep_return[e] = ret; acc.ep_length[e] = len;
+                    if (terminal) {
+                        acc.row_return[e] = ret; acc.row_length[e] = len; acc.row_score[e] = score;
+                        G::game_over(st, len, score);
+                    }
+                } else {
+                    const double ret = PP ? (fresh ? 0.0 : acc.ep_return[e]) + (double)raw : acc.ep_return[e] + (double)reward;
+                    const int len = PP ? (fresh ? 0 : acc.ep_length[e]) + ticks : acc.ep_length[e] + 1;
+                    acc.ep_return[e] = ret; acc.ep_length[e] = len;
+                    if (PP ? ended : terminal) {
+                        acc.row_return[e] = ret; acc.row_length[e] = len; acc.row_score[e] = score;
+                        double* slot = acc.stats + 4 * (blockIdx.x & (PB_STAT_SLOTS - 1));
+                        atomicAdd(slot + 0, 1.0); atomicAdd(slot + 1, ret);
+                        atomicAdd(slot + 2, (double)len); atomicAdd(slot + 3, (double)score);
+                    }
+                }
+                unsigned char* row = out.obs + orow * out.stride;
+                if (S == 1) {
+                    tma_store_1d(row, frame, FS_FRAME);
+                } else if (loaded) {
+                    mbar_wait(&bars[s], phase[s]);     // the three old frames have landed
+                    tma_store_1d(row, buf, FS_ROW);
+                } else {
+                    for (int k = 0; k < 4; ++k) tma_store_1d(row + (size_t)k * FS_FRAME, frame, FS_FRAME);
+                }
+                tma_commit();
             }
-            unsigned char* row = out.obs + e * out.stride;
-            if (S == 1) {
-                tma_store_1d(row, frame, FS_FRAME);
-            } else if (loaded) {
-                mbar_wait(&bars[s], phase[s]);     // the three old frames have landed
-                tma_store_1d(row, buf, FS_ROW);
-            } else {
-                for (int k = 0; k < 4; ++k) tma_store_1d(row + (size_t)k * FS_FRAME, frame, FS_FRAME);
-            }
-            tma_commit();
+            if (S == 4 && loaded) phase[s] ^= 1;
+            // no trailing barrier: the next iteration uses another stage; this stage is refilled by thread 0 at the top of
+            // the next iteration (after wait_read) and rendered into FS_STAGES iterations later, behind block barriers
         }
-        if (S == 4 && loaded) phase[s] ^= 1;
-        // no trailing barrier: the next iteration uses another stage; this stage is refilled by thread 0 at the top of
-        // the next iteration (after wait_read) and rendered into FS_STAGES iterations later, behind block barriers
     }
     if (tid == 0) tma_wait_all<0>();
 }

@@ -6,7 +6,7 @@ device-resident multi-env (the PufferEnv seam, pufferlib/environment.py:1-21).  
 ``b200_kind`` attribute (ours) or by name for the reference's own ``make_squared``, ``make_memory``, ...
 (pufferlib/environments/ocean/environment.py:28-72), so the reference's creator can be passed unchanged.
 
-A kind may have several agents per env (multiagent: two); the backend reads that number from the library
+A kind may have several agents per env (multiagent, pong_versus: two); the backend reads that number from the library
 (pb_env_agents_per_env) and sizes every row buffer by agents, as the reference's vectorisers do (vector.py:85-92).
 """
 import math
@@ -18,7 +18,8 @@ from pufferlib_b200.exceptions import APIUsageError
 
 KNOWN_BY_NAME = {'make_squared': 'squared', 'make_breakout': 'breakout', 'make_snake': 'snake', 'make_pong': 'pong',
                  'make_memory': 'memory', 'make_password': 'password', 'make_stochastic': 'stochastic',
-                 'make_bandit': 'bandit', 'make_multiagent': 'multiagent', 'make_breakout_pixels': 'breakout_pixels'}
+                 'make_bandit': 'bandit', 'make_multiagent': 'multiagent', 'make_breakout_pixels': 'breakout_pixels',
+                 'make_pong_versus': 'pong_versus'}
 
 # Kinds whose reference env draws from a process-global RNG stream (CPython's `random` for squared, numpy's
 # `np.random` for memory and bandit): their results depend on which envs share a process, so the B200 backend gives
@@ -154,6 +155,18 @@ def resolve_config(creator, args, kwargs):
         iparam[1] = int(kwargs.pop('max_ticks', 0))
         _atari_options(kind, kwargs, iparam, iparam[1] if iparam[1] > 0 else 4096, iparam[0] if iparam[0] > 0 else 5)
         _framestack(kind, kwargs, iparam)
+    elif kind == 'pong_versus':
+        if args:
+            raise APIUsageError(f'pong_versus: takes keywords only, got args {list(args)}')
+        for name in ('frameskip', 'noop_max', 'episodic_life', 'clip_rewards'):
+            if name in kwargs:      # oracle/SPEC_PONG_VERSUS.md: the Atari preprocessing layer is single-agent
+                raise APIUsageError(f'pong_versus: {name} is not supported (the Atari preprocessing options are '
+                                    'single-agent)')
+        if 'max_score' in kwargs:   # scores and the tick counter are 4 and 16 bits of pong's packed state
+            iparam[0] = _int_in(kind, 'max_score', kwargs.pop('max_score'), 1, 15)
+        if 'max_ticks' in kwargs:
+            iparam[1] = _int_in(kind, 'max_ticks', kwargs.pop('max_ticks'), 1, 65535)
+        _framestack(kind, kwargs, iparam)
     elif kind == 'multiagent':
         if args or kwargs:      # make_multiagent() takes no arguments (ocean/environment.py:69-72)
             raise APIUsageError(f'multiagent: takes no arguments, got args {list(args or ())} kwargs {sorted(kwargs)}')
@@ -170,7 +183,8 @@ def resolve_config(creator, args, kwargs):
             iparam[0] = _int_in(kind, 'num_actions', v['num_actions'], 1, 1 << 15)
             dparam = [_finite(kind, 'reward_scale', v['reward_scale']), _finite(kind, 'reward_noise', v['reward_noise'])]
     if 'framestack' in kwargs:
-        raise APIUsageError(f'{kind}: framestack is an option of the pixel kinds (pong, breakout_pixels) only')
+        raise APIUsageError(f'{kind}: framestack is an option of the pixel kinds (pong, breakout_pixels, pong_versus) '
+                            'only')
     if kwargs:
         raise APIUsageError(f'{kind}: unexpected env kwargs {sorted(kwargs)}')
     return kind, iparam, dparam

@@ -536,14 +536,38 @@ class B200:
             rewards, term = host[:4 * n].view(np.float32), host[4 * n:].view(np.bool_)
             self.d2h_bytes += 5 * n
         ended = np.asarray(term).reshape(-1, a_per).all(axis=1)
+        if self.kind == 'pong_versus':
+            return self._versus_infos(np.nonzero(ended)[0])
         r = np.asarray(rewards).reshape(-1, a_per)
         return [{a + 1: {'score': int(r[e, a])} for a in range(a_per)} for e in np.nonzero(ended)[0]]
+
+    def _versus_infos(self, idx):
+        """pong_versus, for the envs `idx` whose game just ended, in env order: {1: {'score': s, 'episode_length': L},
+        2: {'score': -s, 'episode_length': L}}, python ints (oracle/SPEC_PONG_VERSUS.md): s = the right paddle's points
+        minus the left's, L = the game's ticks.  The device's per-env rows come to the host in one copy."""
+        if len(idx) == 0:
+            return []
+        lib, n = _native.lib(), self._envs
+        stage = torch.empty(8 * n, dtype=torch.uint8, device=self.buf.terminals.device)
+        base = stage.data_ptr()
+        for handle, lo, cnt in self._shards:
+            p_len, p_score = C.c_void_p(), C.c_void_p()
+            _native.check(lib.pb_env_episode_rows(handle, None, C.byref(p_len), C.byref(p_score)))
+            for src, off in ((p_len.value, 4 * lo), (p_score.value, 4 * n + 4 * lo)):
+                _native.check(lib.pb_copy_rows(C.c_void_p(src), 4 * cnt, C.c_void_p(base + off), 4 * cnt, 4 * cnt, 1,
+                                               _native.stream_ptr()))
+        host = stage.cpu().numpy()
+        self.d2h_bytes += 8 * n
+        length, score = host[:4 * n].view(np.int32), host[4 * n:].view(np.float32)
+        return [{1: {'score': int(score[e]), 'episode_length': int(length[e])},
+                 2: {'score': -int(score[e]), 'episode_length': int(length[e])}} for e in idx]
 
     def episode_stats(self, clear=True):
         """Device-side EpisodeStats reduction: {episode_return, episode_length, score} means over the episodes
         finished since the last call, plus their count (one 32-byte D2H).  Multi-agent kinds: {'1/score', '2/score'}
         means over the env steps since the last call (the keys the reference's evaluate builds from the per-agent infos
-        with unroll_nested_dict, clean_pufferl.py:119-121), plus that count."""
+        with unroll_nested_dict, clean_pufferl.py:119-121), plus that count; pong_versus: over the games ended, with
+        '1/episode_length' and '2/episode_length' (the game's ticks) beside the scores."""
         out = [0.0] * 4
         if self.agents_per_env > 1:
             with torch.cuda.device(self.device):
@@ -555,7 +579,10 @@ class B200:
             cnt = out[0]
             if cnt <= 0:
                 return {}, 0
-            return {f'{a + 1}/score': out[1 + a] / cnt for a in range(self.agents_per_env)}, int(cnt)
+            means = {f'{a + 1}/score': out[1 + a] / cnt for a in range(self.agents_per_env)}
+            if self.kind == 'pong_versus':
+                means.update({f'{a + 1}/episode_length': out[3] / cnt for a in range(self.agents_per_env)})
+            return means, int(cnt)
         with torch.cuda.device(self.device):
             for handle, _, _ in self._shards:
                 part = (C.c_double * 4)()
